@@ -60,7 +60,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def model_weights(seed, L, R, S, A):
@@ -291,7 +291,7 @@ def conditioning_producer_timing(eng, torch, args, T):
 
 
 def reference_gpu_kernels(args, our_khz, n_samples=600):
-    """The reference's OWN CUDA kernels (oracle/_ref/ref_gpu_harness: unmodified nv_wavenet.cuh rebuilt for sm_100a), same model,
+    """The reference's OWN CUDA kernels (oracle/_ref/ref_gpu_harness: unmodified nv_wavenet.cuh rebuilt for sm_90a), same model,
     same batch, same box, timed like nv_wavenet_perf.cu:67-87 -- the GPU baseline next to the headline.  Test infrastructure:
     a separate process; nothing of it is on our path."""
     try:
@@ -421,6 +421,12 @@ def run_ours(args, rank, world, local_rank):
     ev1.record(stream)
     barrier()
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        # what the timed path leaves for its caller: the sampled indices of the last step (exact in float32)
+        y_last = np.zeros((B, N), np.int32)
+        eng.get_yout(y_last, 0, N, stream); torch.cuda.synchronize()
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "samples.npy"), y_last.astype(np.float32))
     elapsed_ms = ev0.elapsed_time(ev1)
     kernel_ms = statistics.mean(a.elapsed_time(b) for a, b in kev)
     info = eng.launch_info()
@@ -482,23 +488,9 @@ def run_ours(args, rank, world, local_rank):
     peak, peak_src = measured_peaks()
     alg = algorithmic_bytes(L, R, S, A, T)
     achieved = B * N * alg / (kernel_ms * 1e-3) / 1e9                # one launch = one step of one GPU
-    # DRAM traffic cannot be measured on this run (no profiler in a timed run): `traffic` is dram read + written of the committed
-    # `ncu --set full` capture (profiles/ncu_summary.json) when that capture is of exactly this launch (same config, kernel, batch and
-    # sample count), else null; `traffic_extrapolated` scales the capture's bytes per unit to this launch in any case
     kname = {16: "wn_stream_kernel", 17: "wn_tc_kernel", 18: "wn_lat2_kernel" if info["cluster"] > 1 else "wn_lat_kernel"}.get(info["kernel"], str(info["kernel"]))
-    traffic = None                                  # DRAM bytes of one launch of this very shape, if the committed ncu capture is of it
+    traffic = None                                  # DRAM bytes: not measurable without a profiler in the timed run
     traffic_x = None
-    prof = os.path.join(ROOT, "profiles", "ncu_summary.json")
-    if os.path.exists(prof):
-        try:
-            pj = json.load(open(prof))
-            if pj.get("config") == args.config and pj.get("kernel_id") == info["kernel"] and kname in pj.get("kernel", ""):
-                if pj.get("capture_samples") == N and pj.get("capture_batch") == B:
-                    traffic = pj["dram_bytes_read"] + pj["dram_bytes_write"]
-                traffic_x = {"value": pj["dram_bytes_per_unit"] * B * N, "dram_bytes_per_unit": pj["dram_bytes_per_unit"],
-                             "capture_samples": pj.get("capture_samples"), "capture_batch": pj.get("capture_batch"), "source": "profiles/ncu_summary.json"}
-        except Exception:
-            traffic_x = None
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
                 "traffic_extrapolated": traffic_x, "peak_source": peak_src, "kernel": kname,
                 "kernel_ms_per_launch": kernel_ms, "algorithmic_bytes_per_unit": alg, "units_per_launch": B * N,
@@ -546,6 +538,8 @@ def main():
     ap.add_argument("--e2e-chunk", type=int, default=1000)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's outputs (sampled indices [batch][samples]) as DIR/samples.npy")
     args = ap.parse_args()
     MODEL.clear(); MODEL.update(CONFIGS[args.config])
     if args.batch is None:

@@ -4,7 +4,7 @@
  * (nv_wavenet.cuh:220-640) forwarding to the C-ABI of libwavenet_infer.so (include/nvwn_b200.h).
  *
  * The reference class is header-only and instantiates its kernels in the caller's translation unit;
- * this facade is plain host C++ (no nvcc needed): the sm_100a kernels are compiled once inside the
+ * this facade is plain host C++ (no nvcc needed): the sm_90a kernels are compiled once inside the
  * library for every supported (precision, R, S) and selected at run time.
  *
  *   T_weight / T_data : float / float  -> bit-exact fp32 path

@@ -1,5 +1,5 @@
 /*
- * nvwn_b200.h -- handle-based C-ABI of the B200 WaveNet inference engine.
+ * nvwn_b200.h -- handle-based C-ABI of the WaveNet inference engine.
  *
  * One entry point per public member of the reference's host class
  * nvWavenetInfer<T_weight,T_data,R,S,A> (nv_wavenet.cuh:220-640), so that the C++ facade

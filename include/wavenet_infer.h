@@ -18,7 +18,7 @@
  *   - synchronous; CUDA failures print "GPUassert: ..." to stderr and exit(code)
  *     (nv_wavenet_util.cuh:34-40);
  *   - `implementation` 0..4 (AUTO, SINGLE_BLOCK, DUAL_BLOCK, PERSISTENT, MANYBLOCK) is accepted
- *     and ignored: one sm_100a kernel family replaces all four.
+ *     and ignored: one sm_90a kernel family replaces all four.
  *
  * The arithmetic of this entry point is bit-exact fp32 (DESIGN.md §4).  wavenet_infer_fp16 (below) takes the same arguments
  * and runs the fp16 kernels (the reference builds a second library with T_data = half for that, README.md:24-25).

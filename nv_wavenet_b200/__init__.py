@@ -1,4 +1,4 @@
-"""nv_wavenet_b200 -- B200-native (sm_100a) autoregressive WaveNet inference behind nv-wavenet's interfaces.
+"""nv_wavenet_b200 -- H100-native (sm_90a) autoregressive WaveNet inference behind nv-wavenet's interfaces.
 
 The package is only the host-side mirror of the reference's operator interface; every computation
 runs in nv_wavenet_b200/lib/libwavenet_infer.so (hand-written CUDA, C-ABI in include/*.h).

@@ -72,7 +72,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -m nv_wavenet_b200.build` "
-                "(nvcc, sm_100a).  nv_wavenet_b200 has no CPU or PyTorch fallback.")
+                "(nvcc, sm_90a).  nv_wavenet_b200 has no CPU or PyTorch fallback.")
         l = C.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(l, name)          # AttributeError if the library does not export it

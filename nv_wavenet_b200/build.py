@@ -1,4 +1,4 @@
-"""Builds the in-tree CUDA library nv_wavenet_b200/lib/libwavenet_infer.so for sm_100a (nvcc, no GPU needed)."""
+"""Builds the in-tree CUDA library nv_wavenet_b200/lib/libwavenet_infer.so for sm_90a (nvcc, no GPU needed)."""
 import os
 import subprocess
 

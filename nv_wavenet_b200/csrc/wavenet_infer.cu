@@ -1,4 +1,4 @@
-// wavenet_infer.cu -- the reference's C-ABI (include/wavenet_infer.h) on top of the B200 engine.
+// wavenet_infer.cu -- the reference's C-ABI (include/wavenet_infer.h) on top of the engine.
 // Replaces pytorch/wavenet_infer.cu:40-149 of the reference; semantics documented in the header.
 #include "../../include/wavenet_infer.h"
 #include "../../include/nvwn_b200.h"

@@ -1,4 +1,4 @@
-// wn_common.h -- shared declarations of the B200 WaveNet inference engine (host + device).
+// wn_common.h -- shared declarations of the WaveNet inference engine (host + device).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

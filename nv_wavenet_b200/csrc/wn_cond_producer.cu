@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(256) project_tiled_kernel(float* __restrict__ 
 unsigned grid_for(size_t total)
 {
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     return (unsigned)(blocks ? blocks : 1);
 }
 

@@ -42,7 +42,7 @@ cudaError_t wn_f32_to_f16(__half* dst, const float* src_dev, size_t n, cudaStrea
     const int threads = 256;
     size_t blocks = (n / 4 + threads - 1) / threads;
     if (blocks < 1) blocks = 1;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     f32_to_f16_kernel<<<(unsigned)blocks, threads, 0, stream>>>(dst, src_dev, n);
     return cudaGetLastError();
 }
@@ -55,7 +55,7 @@ cudaError_t wn_f16_to_f32(float* dst, const __half* src_dev, size_t n, cudaStrea
 {
     if (n == 0) return cudaSuccess;
     size_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     f16_to_f32_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, src_dev, n);
     return cudaGetLastError();
 }
@@ -84,7 +84,7 @@ cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, cud
 {
     if (n == 0) return cudaSuccess;
     size_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     selectors_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, n, seed);
     return cudaGetLastError();
 }
@@ -104,7 +104,7 @@ cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B,
     const size_t total = (size_t)B * size;
     if (total == 0) return cudaSuccess;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     mulaw_decode_kernel<<<(unsigned)blocks, 256, 0, stream>>>(yOut, N, offset, size, total, A, lut_f, lut_s, out_f, out_s);
     return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-// wn_engine.cu -- host side of the B200 WaveNet inference engine + the handle C-ABI (include/nvwn_b200.h).
+// wn_engine.cu -- host side of the WaveNet inference engine + the handle C-ABI (include/nvwn_b200.h).
 //
 // Owns every device buffer, uploads / converts weights and inputs, picks the kernel and launches it.
 // Re-design of the reference host class nvWavenetInfer<T_weight,T_data,R,S,A> (nv_wavenet.cuh:220-640):
@@ -10,6 +10,7 @@
 #include "../../include/nvwn_b200.h"
 #include "wn_common.h"
 
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -148,7 +149,7 @@ int download(float* dst, const float* src, size_t n)
 }
 
 // fp16 kernel choice, made ONCE per engine (the layouts of the conditioning store and of the history ring depend on it):
-// 0 = stream, 1 = tensor-core (tcgen05, throughput mode), 2 = latency mode (mma.sync, register-resident chain).
+// 0 = stream, 1 = tensor-core (wgmma, throughput mode), 2 = latency mode (mma.sync, register-resident chain).
 // `impl` NVWN_KERNEL_* forces a kernel; the environment variable NVWN_FP16_KERNEL = stream | tc | lat overrides AUTO (tests).
 int decide_fp16_kernel(int dtype, int impl, int R, int S, int A, int L, int B)
 {
@@ -162,8 +163,9 @@ int decide_fp16_kernel(int dtype, int impl, int R, int S, int A, int L, int B)
         if (!strcmp(env, "tc")) return tc_ok ? 1 : 0;
         if (!strcmp(env, "lat")) return lat_ok ? 2 : 0;
     }
-    // one 16-utterance tile per SM: up to 148 x 16 utterances run as one wave of latency-mode CTAs
-    int lat_max = 148 * 16;
+    // the latency kernels beat the tensor-core kernel even when their 16-utterance tiles need several waves (H100 80GB HBM3,
+    // 400 W power limit, 2 560 utterances: 41.6 M against 14.1 M samples/s); NVWN_LAT_MAX_B caps the batch they take
+    int lat_max = INT_MAX;
     if (const char* env = getenv("NVWN_LAT_MAX_B")) lat_max = atoi(env);
     if (lat_ok && B <= lat_max) return 2;
     return tc_ok ? 1 : 0;
@@ -470,7 +472,7 @@ int nvwn_set_conditioning(nvwn_engine* e, const float* Lh, int first_sample, int
     const size_t per = (size_t)e->L * e->B * 2 * e->R;
     if (!e->tc_mode && !e->lat_mode)
         return upload(e, static_cast<char*>(e->Lh) + (size_t)first_sample * per * e->td, Lh, per * num_samples, (cudaStream_t)stream);
-    // tensor-core layout: fp16, tiled per 128 utterances, 128-byte rows pre-swizzled so that TMA drops them straight into
+    // tensor-core layout: fp16, tiled per 32 / 64 / 128 utterances, 128-byte rows pre-swizzled so that TMA drops them straight into
     // an MMA operand tile (wn_tc_kernel.cu).  Host sources bounce through the staging buffer in whole samples.
     cudaStream_t st = (cudaStream_t)stream;
     auto convert = [&](const float* src_dev, int first, int n) {

@@ -1,8 +1,8 @@
-// wn_lat_kernel.cu -- latency-mode fp16 kernel of the WaveNet inference loop (sm_100a).
+// wn_lat_kernel.cu -- latency-mode fp16 kernel of the WaveNet inference loop (sm_90a).
 //
 // The autoregressive loop is a chain of ~45 tiny dependent GEMMs per sample (M = utterances, N <= 256, K <= 256).  On such a
-// chain the tcgen05 round trip (MMA -> commit -> mbarrier -> tcgen05.ld, ~500 cycles) is the cost, not the tensor pipe
-// (wn_tc_kernel.cu: 2.4 k cycles per layer).  This kernel keeps the whole chain in REGISTERS: warp-level mma.sync
+// chain the round trip between the tensor cores and the epilogue of every link is the cost, not the tensor pipe.  This kernel
+// keeps the whole chain in REGISTERS: warp-level mma.sync
 // (m16n8k16, fp16 x fp16 -> fp32) with the utterances as the M dimension, so that the accumulator fragment of one GEMM is
 // -- after the row-local epilogue -- exactly the A fragment of the next one; the only exchange between the eight compute
 // warps is one 2 KB shared-memory tile + one named barrier per GEMM stage.
@@ -29,13 +29,13 @@
 // tanh.approx.f16x2; no weight folding.
 #include "wn_common.h"
 #include "wn_math.cuh"
-#include "wn_sm100.cuh"
+#include "wn_sm90.cuh"
 
 #include <stdlib.h>
 
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
 constexpr int R = 64, A = 256;
 constexpr int NCW = 8;                      // compute warps
@@ -1436,7 +1436,7 @@ cudaError_t wn_lat_cond_convert(void* dst, const float* src_dev, int first_sampl
     const int ntiles = wn_lat_tiles(B);
     const size_t total = (size_t)nsamples * L * ntiles * 256;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     lat_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, L, B, ntiles);
     return cudaGetLastError();
 }
@@ -1446,7 +1446,7 @@ cudaError_t wn_lat_cond_readback(float* dst_dev, const void* store, int first_sa
     if (nsamples <= 0) return cudaSuccess;
     const size_t total = (size_t)nsamples * L * B * 64;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     lat_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, L, B, wn_lat_tiles(B));
     return cudaGetLastError();
 }
@@ -1507,7 +1507,7 @@ static cudaError_t lat2_go(const WnParams& pp, const unsigned char* im8, int til
     e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, DUMP, TRC>, pp, im8, ntiles_alloc);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
-// how many clusters the device runs at once (a cluster needs NCL SMs of one GPC: fewer than 148 / NCL fit); 0 if the query fails
+// how many clusters the device runs at once (a cluster needs NCL SMs of one GPC: fewer than 132 / NCL fit on an H100); 0 if the query fails
 template <int S>
 static int lat2_max_clusters()
 {

@@ -23,7 +23,7 @@
 // of the slab with conflict-free 4-byte shared loads.  The arithmetic and its order are untouched (same bits).
 #include "wn_common.h"
 #include "wn_math.cuh"
-#include "wn_sm100.cuh"
+#include "wn_sm90.cuh"
 
 #include <type_traits>
 
@@ -127,7 +127,7 @@ __device__ __forceinline__ void dot_slab(const float* __restrict__ ws, int Mrt, 
                                          float (&acc)[BT], float (&odd)[BT])
 {
     const int M = MC ? MC : Mrt;
-    const uint32_t wp = sm100::smem_u32(ws + row);
+    const uint32_t wp = sm90::smem_u32(ws + row);
 #pragma unroll
     for (int j = 0; j < KS; j += 4) {
         const float w0 = lds_f32(wp + (j + 0) * M * 4), w1 = lds_f32(wp + (j + 1) * M * 4), w2 = lds_f32(wp + (j + 2) * M * 4), w3 = lds_f32(wp + (j + 3) * M * 4);
@@ -233,8 +233,8 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
     }
     if (tid < BT) { ysm[tid * 2] = p.yPrev[b0 + tid]; ysm[tid * 2 + 1] = p.yCur[b0 + tid]; }
     if (RING && tid == 0) {
-        for (int i = 0; i < RC::SLOTS; i++) { sm100::mbar_init(bar_full + i, 1); sm100::mbar_init(bar_empty + i, NT / 32); }
-        sm100::fence_mbar_init();
+        for (int i = 0; i < RC::SLOTS; i++) { sm90::mbar_init(bar_full + i, 1); sm90::mbar_init(bar_empty + i, NT / 32); }
+        sm90::fence_mbar_init();
     }
     __syncthreads();
 
@@ -248,11 +248,11 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
             uint32_t n = 0;
             auto put = [&](const float* s0, uint32_t f0, const float* s1, uint32_t f1) {       // floats of the one or two parts of a piece
                 const uint32_t sl = n % RC::SLOTS;
-                sm100::mbar_wait(bar_empty + sl, ((n / RC::SLOTS) & 1) ^ 1);
-                sm100::mbar_arrive_expect_tx(bar_full + sl, (f0 + f1) * 4);
+                sm90::mbar_wait(bar_empty + sl, ((n / RC::SLOTS) & 1) ^ 1);
+                sm90::mbar_arrive_expect_tx(bar_full + sl, (f0 + f1) * 4);
                 float* dst = ring_w + sl * (RC::PIECE / 4);
-                sm100::tma_load_1d(dst, s0, f0 * 4, bar_full + sl);
-                if (f1) sm100::tma_load_1d(dst + f0, s1, f1 * 4, bar_full + sl);
+                sm90::tma_load_1d(dst, s0, f0 * 4, bar_full + sl);
+                if (f1) sm90::tma_load_1d(dst + f0, s1, f1 * 4, bar_full + sl);
                 n++;
             };
             for (int t = p.init_sample; t < p.init_sample + p.count; t++) {
@@ -272,12 +272,12 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
     uint32_t pcn = 0;
     auto piece_wait = [&]() -> const float* {
         const uint32_t sl = pcn % RC::SLOTS;
-        sm100::mbar_wait(bar_full + sl, (pcn / RC::SLOTS) & 1);
+        sm90::mbar_wait(bar_full + sl, (pcn / RC::SLOTS) & 1);
         return ring_w + sl * (RC::PIECE / 4);
     };
     auto piece_done = [&]() {
         __syncwarp();
-        if ((tid & 31) == 0) sm100::mbar_arrive(bar_empty + pcn % RC::SLOTS);
+        if ((tid & 31) == 0) sm90::mbar_arrive(bar_empty + pcn % RC::SLOTS);
         pcn++;
     };
 

@@ -1,37 +1,43 @@
-// wn_tc_kernel.cu -- fp16 tensor-core kernel of the WaveNet inference loop (sm_100a: tcgen05 + TMEM + bulk TMA).
+// wn_tc_kernel.cu -- fp16 tensor-core kernel of the WaveNet inference loop (sm_90a: wgmma + bulk TMA + mbarrier).
 //
-// ONE persistent CTA (12 warps) per tile of 32 / 64 / 128 utterances runs the whole autoregressive loop for `count` samples:
+// ONE persistent CTA per 64 utterances runs the whole autoregressive loop for `count` samples.  Every GEMM of a
+// layer is  D[64 utterances x N channels] (fp32, registers) (+)= X[64 x 64] . W[N x 64]^T  on the warpgroup MMA, activations
+// as the A operand and weights as the B operand, both K-major SWIZZLE_128B tiles in shared memory.
 //
-//   warps 0-7  "epilogue": 2, 4 or 8 threads per utterance (an utterance occupies 1, 2 or 4 rows = TMEM lanes of every tile).
-//              embed -> per layer: [Dx + Bres + x -> x tile] [D1 + Lh + Bh -> tanh * sigmoid -> h tile]
-//              -> relu(skip) tile -> relu(Zs) tile -> softmax + categorical sample, all row-local
-//              (the reference spreads these over CTAs/threads: nv_wavenet_persistent.cuh:223-462, softmax.cuh:36-191).
-//   warp 8     TMA producer.  Streams the pre-tiled fp16 weight image (and the x[t-d] history tiles) from L2 through an
-//              NSTAGE x 16 KB shared-memory ring, and the conditioning tiles, with cp.async.bulk + mbarrier complete_tx.
-//   warp 9     MMA issuer A (and the only issuer of the unfused schedule): D[128 rows x N channels] (fp32, TMEM) +=
-//              X[128 x 64] . W[N x 64]^T with tcgen05.mma (activations = A operand, weights = B operand, both K-major
-//              SWIZZLE_128B); tcgen05.commit signals the epilogue and frees ring stages.
-//   warp 10    MMA issuer B of the fused schedule (skip and dilated-history GEMMs, half of the output GEMMs).
-//   warp 11    history copy of the fused schedule (x tile: shared -> global ring, one bulk copy).
+//   warpgroups 0, 1  consumers.  Warpgroup w owns residual / gate channels [32 w, 32 w + 32) and the w-th half of the skip,
+//                    Zs and Za columns of all 64 utterances, so that the gate (tanh(a_c) * sigmoid(g_c) needs accumulator
+//                    columns c and 64 + c) and the residual update stay local to a thread of the accumulator fragment.
+//                    They issue the MMAs and evaluate embedding -> per layer [gate -> h tile] [x += Wres.h + Bres -> x tile,
+//                    history ring] -> relu(skip) tile -> relu(Zs) tile -> softmax + categorical sample.
+//   warp 8           TMA producer.  Streams the pre-tiled fp16 weight image, the conditioning tiles and the x[t-d]
+//                    history tiles from L2 through an NSTAGE x 16 KB shared-memory ring with cp.async.bulk + mbarrier
+//                    complete_tx, in exactly the order the consumers take them.
+//
+// Tiles: the conditioning store and the history ring are laid out per tile of 64 utterances (default), 32 (the MMA rows of
+// the other 32 stay empty: twice the CTAs for a small batch) or 128 (two CTAs per tile, 64 rows each).
+// Schedules: unfused (the reference's order: cur GEMM -> gate -> res / skip GEMMs -> residual -> next layer) and FUSED (one
+// MMA round trip per layer: a_l = (Lh + Bh'_l) + Wprev_l.x_l[t-d] + Wcur_l.x_{l-1} + Wf_l.h_{l-1} with Wf_l = Wcur_l.Wres_{l-1}
+// and Bh'_l = Bh_l + Wcur_l.Bres_{l-1} folded at pack time, issued together with Wres_{l-1}.h_{l-1} and Wskip_{l-1}.h_{l-1}).
 //
 // Replaces nv_wavenet_persistent.cuh + matrix_math.cuh + softmax.cuh of the reference for T_data = half.
-// Numerical contract (oracle/wavenet_oracle.c, WNO_PREC_FP16): weights, biases, embeddings, Lh and every GEMM
-// input rounded to fp16; fp32 accumulation; residual stream, skip sum, softmax in fp32 (logits parked as fp16 offsets from the row max).  The fused schedule folds
-// Wcur_l . Wres_{l-1} into one fp16 matrix (see the kernel) -- same tolerance, checked by the same tests.
+// Numerical contract (oracle/wavenet_oracle.c, WNO_PREC_FP16): weights, biases, embeddings, Lh and every GEMM input
+// rounded to fp16; fp32 accumulation; residual stream, skip sum and softmax in fp32.
 #include "wn_common.h"
 #include "wn_math.cuh"
-#include "wn_sm100.cuh"
+#include "wn_sm90.cuh"
 
 #include <stdlib.h>
 
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
 constexpr int R = 64, A = 256;
-constexpr int TILE = 16384;                 // [128 rows x 64 fp16] K-major SW128
-constexpr int NT = 384;                     // 8 epilogue warps + TMA producer warp + 2 MMA issuer warps + history-copy warp
-constexpr int NEPI = 256;
+constexpr int TILE = 16384;                 // [128 rows x 64 fp16] K-major SW128: one weight chunk / ring stage
+constexpr int TU = 64;                      // utterances per CTA tile = rows of every activation tile = M of the MMA
+constexpr int ATILE = TU * 128;             // [64 rows x 64 fp16] activation tile
+constexpr int NCONS = 256;                  // two consumer warpgroups
+constexpr int NT = NCONS + 32;              // + the TMA producer warp
 
 struct TcImage {                            // byte offsets inside the packed image
     size_t layer_bytes, off_out, off_bias, total;
@@ -41,7 +47,7 @@ struct TcImage {                            // byte offsets inside the packed im
 __host__ __device__ inline TcImage tc_image(int S, int L)
 {
     TcImage im;
-    im.l_wf = (size_t)TILE * 2 + TILE / 2 + (size_t)(S / 128) * TILE;
+    im.l_wf = (size_t)TILE * 2 + TILE / 2 + (size_t)(S / 128) * TILE;           // Wprev | Wcur | Wres | Wskip chunks | Wf
     im.layer_bytes = im.l_wf + TILE;
     im.off_out = (size_t)L * im.layer_bytes;
     im.off_bias = im.off_out + (size_t)(S / 64) * 2 * TILE + (size_t)(A / 64) * 2 * TILE;
@@ -55,18 +61,15 @@ __host__ __device__ inline TcImage tc_image(int S, int L)
     return im;
 }
 
-__host__ __device__ inline size_t tc_smem_bytes(int S, int L, int nstage)
+__host__ __device__ inline size_t tc_smem_bytes(int nstage)
 {
-    // 4 activation tiles + weight ring + conditioning buffers (2 tiles) + biases (Bh, Bres, Bskip-sum, Bzs, Bza) + dilations + barriers
-    return 1024 + 4 * (size_t)TILE + (size_t)nstage * TILE + 2 * TILE + ((size_t)L * 192 + S + 2 * A) * sizeof(float) + (size_t)L * 4 +
-           128 * 5 * sizeof(float) + (2 * nstage + 20) * 8 + 16;
+    // alignment slack + weight ring + x and h tiles (two each) + 4 k-tiles of relu(skip) / relu(Zs) + fp32 logits + sampled indices + barriers
+    return 1024 + (size_t)nstage * TILE + 4 * ATILE + 4 * ATILE + (size_t)TU * A * sizeof(float) + TU * sizeof(int) + 2 * (size_t)nstage * 8;
 }
 
 // Conditioning in the tensor-core layout: fp16 [N][L][Bpad rows][2 halves of 64 channels], tiled per 128 utterances;
 // inside a tile: [half][row][128 B], 16-byte chunks XOR-swizzled with (row & 7) -- i.e. exactly the K-major
 // SWIZZLE_128B image of an MMA A-operand tile, so a 1-D bulk TMA copy of rows*128 bytes needs no further shuffling.
-// TU = utterances per tile: 64 (four threads per utterance, the lower-latency variant) while the batch fits the SMs
-// that way, 128 otherwise.
 __host__ __device__ inline int cond_rows(int B, int tile, int TU) { const int r = B - tile * TU; return r >= TU ? TU : ((r + 7) & ~7); }
 __host__ __device__ inline size_t cond_bpad(int B, int TU) { const int nt = (B + TU - 1) / TU; return (size_t)(nt - 1) * TU + cond_rows(B, nt - 1, TU); }
 
@@ -158,7 +161,7 @@ __global__ void tc_pack_kernel(WnParams p, unsigned char* __restrict__ img, TcIm
         const int a = (int)(i / A), z = (int)(i % A);
         put(off_wza + (size_t)((z / 64) * 2 + a / 128) * TILE, a % 128, z % 64, Wza[a + (size_t)z * A]);
     }
-    // biases -> fp32; running prefix of the skip biases (the skip sum is kept in TMEM without biases)
+    // biases -> fp32; running prefix of the skip biases (the skip sum is accumulated without biases)
     float* bias = reinterpret_cast<float*>(img + im.off_bias);
     const __half* Bh = static_cast<const __half*>(p.Bh);
     const __half* Bres = static_cast<const __half*>(p.Bres);
@@ -194,24 +197,21 @@ __device__ __forceinline__ float2 unpack_h2(uint32_t v)
 {
     return __half22float2(*reinterpret_cast<__half2*>(&v));
 }
-// chunk q (16 bytes = 8 fp16) of row `row` inside a SW128 tile
-__device__ __forceinline__ uint32_t chunk_off(int row, int q) { return (uint32_t)row * 128u + (uint32_t)((q ^ (row & 7)) << 4); }
-
-// DUP (tiles with <= 64 live utterances, e.g. the 64-per-GPU headline case): every utterance occupies TWO rows (u and u+64)
-// of each activation tile / TMEM accumulator, so that all four TMEM lane quadrants -- and with them all four warp
-// schedulers and their MUFU pipes -- work for it: 4 threads per utterance instead of 2, each on 16 of the 64 channels.
-//
-// FUSED (default schedule): ONE MMA <-> epilogue round trip per layer instead of two.  The pre-activation of layer l is
-// accumulated as  (Lh + Bh') [tcgen05.st] + Wprev_l.x_l[t-d] + Wcur_l.x_{l-1} [both in the background, one layer early]
-// + Wf_l.h_{l-1} [the only GEMM on the critical path], Wf_l = Wcur_l.Wres_{l-1} folded at pack time.  The residual GEMM
-// Wres_{l-1}.h_{l-1} still produces x_l (history ring, next layer's background GEMM, dump) but nothing waits on it
-// before the next gate.
-template <int S, int CP, bool FUSED>
-__global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const unsigned char* __restrict__ img, const int nstage)
+// two consecutive fp16 (k even) of row `row` of a SW128 tile, in shared or global memory
+__device__ __forceinline__ void st_pair(unsigned char* tile, int row, int k, float v0, float v1)
 {
-    // CP = row copies per utterance (1, 2, 4): tiles of 128 / CP utterances, 2 CP threads per utterance.  CP = 4 spreads a
-    // small batch over twice the SMs of CP = 2 and halves the per-thread gate / residual / softmax work once more.
-    constexpr bool DUP = CP > 1;
+    *reinterpret_cast<uint32_t*>(tile + sw128_offset(row, k)) = pack_h2(v0, v1);
+}
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Accumulator fragment of a warpgroup (wn_sm90.cuh): thread i holds rows r0 = 16 (i / 32) + (i % 32) / 4 and r0 + 8, and in
+// every 8-column group j the columns 8 j + 2 (i % 4) + {0, 1}.  Index 4 j + 2 r + e of a fragment array = row r0 + 8 r,
+// column 8 j + 2 (i % 4) + e.  x, the gate inputs and Dx of one thread are the same 16 (row, channel) pairs.
+template <int S, bool FUSED>
+__global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const unsigned char* __restrict__ img, const int nstage, const int tu)
+{
+    constexpr int SKN = S / 2;                     // skip columns per warpgroup
+    constexpr int SKC = S / 128;                   // skip weight chunks per layer
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     // 1024-byte alignment by OFFSET (not by pointer round-trip through an integer): the compiler keeps knowing these
     // are shared-memory addresses and emits LDS/STS instead of generic LD/ST
@@ -219,1055 +219,492 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
     const int L = p.L, B = p.B;
     const TcImage im = tc_image(S, L);
 
-    unsigned char* t_xc = smem;                    // x tile of the current layer        (= BIG k-tile 0)
-    unsigned char* t_x1 = smem + 3 * TILE;         // FUSED: x tiles ping-pong by layer parity (t_xc, t_x1 = BIG k-tile 3)
-    unsigned char* t_h = smem + TILE;              // gated activation tiles, double buffered by layer parity (= BIG k-tiles 1, 2)
-    unsigned char* t_big = smem;                   // [128 x 256] as 4 k-tiles: relu(skip), relu(Zs), then fp16 logits scratch
-    unsigned char* ring = smem + 4 * TILE;
-    // conditioning buffers: one Lh[t][l] tile = [2 halves][rows][128 B]; DUP tiles (<= 64 rows, 16 KB) are double
-    // buffered, full tiles (32 KB) single buffered
-    unsigned char* t_cond = ring + (size_t)nstage * TILE;
-    constexpr int NC = DUP ? 2 : 1;
-    constexpr int CB = DUP ? TILE : 2 * TILE;
-    float* s_bh = reinterpret_cast<float*>(t_cond + 2 * TILE);
-    float* s_bres = s_bh + (size_t)L * 128;
-    float* s_bsk = s_bres + (size_t)L * 64;
-    float* s_bzs = s_bsk + S;
-    float* s_bza = s_bzs + A;
-    int* s_dil = reinterpret_cast<int*>(s_bza + A);
-    float* s_pair = reinterpret_cast<float*>(s_dil + L + (L & 1));      // [128 rows][2 halves][max, sum] softmax exchange
-    int* s_y = reinterpret_cast<int*>(s_pair + 128 * 4);                // [128] sampled index per utterance
-    uint64_t* w_full = reinterpret_cast<uint64_t*>(s_y + 128);
+    unsigned char* ring = smem;                                    // nstage x 16 KB
+    unsigned char* t_xb = ring + (size_t)nstage * TILE;            // x tiles [2]: A operand of Wcur (FUSED: by layer parity)
+    unsigned char* t_hb = t_xb + 2 * ATILE;                        // h tiles [2]: A operand of Wres, Wskip (and Wf)
+    unsigned char* t_big = t_hb + 2 * ATILE;                       // 4 k-tiles: relu(skip), then relu(Zs)
+    float* s_z = reinterpret_cast<float*>(t_big + 4 * ATILE);      // [TU][A] logits, then exp(z - max)
+    int* s_y = reinterpret_cast<int*>(s_z + TU * A);               // [TU] sampled index
+    uint64_t* w_full = reinterpret_cast<uint64_t*>(s_y + TU);
     uint64_t* w_empty = w_full + nstage;
-    uint64_t* epi_done = w_empty + nstage;      // [2] at +0, +17: tile-published phases alternate between the two barriers
-    uint64_t* d1_full = epi_done + 1;
-    uint64_t* dx_full = epi_done + 2;
-    uint64_t* skip_full = epi_done + 3;
-    uint64_t* out_full = epi_done + 4;
-    uint64_t* pre_done = epi_done + 5;          // accumulator of the coming layer initialised with Lh + bias
-    uint64_t* cond_full = epi_done + 6;         // [NC]
-    uint64_t* cond_empty = epi_done + 8;        // [NC]
-    uint64_t* cx_done = epi_done + 10;          // fused schedule, see the issuer roles
-    uint64_t* b_done = epi_done + 11;           // [2] at +11, +14: alternating by layer parity, so that the signalling role can
-    uint64_t* hx_full = epi_done + 12;          //     never complete a barrier twice before its waiter has looked once
-    uint64_t* hx_done = epi_done + 13;          // [2] at +13, +15
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(epi_done + 16);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int tile = blockIdx.x, ntiles = gridDim.x;
+    const int tid = threadIdx.x;
+    const int sub = tu > TU ? tu / TU : 1;                         // CTAs per tile
+    const int tile = blockIdx.x / sub, ntiles = gridDim.x / sub;
+    const int row0 = (blockIdx.x % sub) * TU;                      // first row of this CTA inside its tile
+    const int live = tu < TU ? tu : TU;                            // MMA rows that hold utterances
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     unsigned char* gring = static_cast<unsigned char*>(p.ring);
     auto ring_tile = [&](int t, int l) -> unsigned char* {
-        return gring + (((size_t)(t % slots) * L + l) * ntiles + tile) * (size_t)TILE;
+        return gring + (((size_t)(t % slots) * L + l) * ntiles + tile) * (size_t)TILE + (size_t)row0 * 128;
+    };
+    // conditioning tile geometry (see tc_cond_kernel): [2 halves][c_rows][128 B]; this CTA's rows of each half land in a ring
+    // stage at offsets 0 and ATILE
+    const int c_rows = cond_rows(B, tile, tu);
+    const uint32_t c_bytes = (uint32_t)c_rows * 128u;
+    const int c_here = min(max(c_rows - row0, 0), TU);
+    const uint32_t c_bytes_here = (uint32_t)c_here * 128u;
+    const size_t c_bpad = cond_bpad(B, tu);
+    const unsigned char* gcond = static_cast<const unsigned char*>(p.Lh);
+    auto cond_ptr = [&](int t, int l) -> const unsigned char* {
+        return gcond + (((size_t)t * L + l) * c_bpad + (size_t)tile * tu) * 256 + (size_t)row0 * 128;
     };
 
     if (tid == 0) {
-        for (int s = 0; s < nstage; s++) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 1); }
-        mbar_init(epi_done, NEPI); mbar_init(epi_done + 17, NEPI);
-        mbar_init(d1_full, 1); mbar_init(dx_full, 1); mbar_init(skip_full, FUSED ? 2 : 1); mbar_init(out_full, FUSED ? 2 : 1);
-        mbar_init(cx_done, 1); mbar_init(b_done, 1); mbar_init(b_done + 3, 1); mbar_init(hx_full, NEPI); mbar_init(hx_done, 1); mbar_init(hx_done + 2, 1);
-        mbar_init(pre_done, NEPI);
-        for (int i = 0; i < NC; i++) { mbar_init(&cond_full[i], 1); mbar_init(&cond_empty[i], NEPI); }
+        for (int s = 0; s < nstage; s++) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], NCONS); }
         fence_mbar_init();
-        // dilation of layer l (nv_wavenet.cuh:99-111): 1,2,4..maxDil,1,2,...
-        int d = 1;
-        for (int l = 0; l < L; l++) { s_dil[l] = d; d <<= 1; if (d > p.maxDil) d = 1; }
     }
-    if (warp == 8) tmem_alloc<512>(tmem_slot);
-    {   // biases and the identity tile -> shared memory
-        const float* gb = reinterpret_cast<const float*>(img + im.off_bias);
-        for (int i = tid; i < L * 128; i += NT) s_bh[i] = gb[(FUSED ? im.b_bhf : im.b_bh) + i];
-        for (int i = tid; i < L * 64; i += NT) s_bres[i] = gb[im.b_bres + i];
-        for (int i = tid; i < S; i += NT) s_bsk[i] = gb[im.b_bskp + (size_t)(L - 1) * S + i];
-        for (int i = tid; i < A; i += NT) { s_bzs[i] = gb[im.b_bzs + i]; s_bza[i] = gb[im.b_bza + i]; }
-    }
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    // TMEM columns: [0,128) and [128,256) = pre-activation accumulators, ping-pong by layer parity; the residual GEMM of
-    // layer l writes columns [0,64) of the buffer the gate of layer l has just drained; [256,512) = skip sum over layers
-    // (then Zs); Za reuses [0,256).
-    const uint32_t D1B = tmem_base, DSKIP = tmem_base + 256, DZS = tmem_base + 256, DZA = tmem_base;
 
-    // conditioning tile geometry (see tc_cond_kernel)
-    constexpr int TU = 128 / CP;                    // utterances per tile
-    const int c_rows = cond_rows(B, tile, TU);
-    const uint32_t c_bytes = (uint32_t)c_rows * 128u;
-    const size_t c_bpad = cond_bpad(B, TU);
-    const unsigned char* gcond = static_cast<const unsigned char*>(p.Lh);
-    auto cond_ptr = [&](int t, int l, int half) -> const unsigned char* {
-        return gcond + (((size_t)t * L + l) * c_bpad + (size_t)tile * TU) * 256 + (size_t)half * c_bytes;
-    };
-
-    // debug timeline: role r (0 epilogue thread 0, 1 MMA issuer, 2 producer) appends (tag << 48 | clock) words
-    unsigned long long* trc = (p.trace && blockIdx.x == 0) ? p.trace : nullptr;
-    int trn = 0;
-    const int tr_t = p.trace_t & 0xFFFF, tr_tid = p.trace_t >> 16;     // sample and epilogue thread to trace
-#define TRACE(role, tag) do { if (trc && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
-
-    if (warp == 8) {
-        // =============================================================== TMA producer (whole warp converged, one lane issues)
-        {
+    if (tid >= NCONS) {
+        // =============================================================== TMA producer (one lane)
+        // Chunk order = consumption order, per sample:
+        //   unfused, per layer l:  Lh[t][l] | x_l[t-d] Wprev_l (if t >= d) | Wcur_l | Wres_l | Wskip_l (S/128 chunks)
+        //   FUSED:   layer 0:      Lh[t][0] | x_0[t-1] Wprev_0 (if t >= 1) | Wcur_0
+        //            layer l > 0:  Lh[t][l] | x_l[t-d] Wprev_l (if t >= d) | Wcur_l | Wf_l | Wres_{l-1} | Wskip_{l-1}
+        //            then:         Wres_{L-1} | Wskip_{L-1}
+        //   then the output layers, chunk (kt, nh) in the image's order.
+        if (tid == NCONS) {
             int stage = 0;
             uint32_t ph = 1;
-            auto put = [&](const void* src, uint32_t bytes) {
+            auto put2 = [&](const void* src0, uint32_t bytes0, const void* src1, uint32_t bytes1) {
                 mbar_wait(&w_empty[stage], ph);
-                if (elect_one()) {
-                    mbar_arrive_expect_tx(&w_full[stage], bytes);
-                    tma_load_1d(ring + (size_t)stage * TILE, src, bytes, &w_full[stage]);
-                }
-                __syncwarp();
+                mbar_arrive_expect_tx(&w_full[stage], bytes0 + bytes1);
+                if (bytes0) tma_load_1d(ring + (size_t)stage * TILE, src0, bytes0, &w_full[stage]);
+                if (bytes1) tma_load_1d(ring + (size_t)stage * TILE + ATILE, src1, bytes1, &w_full[stage]);
                 if (++stage == nstage) { stage = 0; ph ^= 1; }
             };
-            // history tile: `bytes` of rows from row 0; with DUP the same rows again from row 64
-            auto put_act = [&](const void* src, uint32_t bytes) {
-                if (!DUP) { put(src, bytes); return; }
-                mbar_wait(&w_empty[stage], ph);
-                if (elect_one()) {
-                    mbar_arrive_expect_tx(&w_full[stage], CP * bytes);
-#pragma unroll
-                    for (int k = 0; k < CP; k++) tma_load_1d(ring + (size_t)stage * TILE + (size_t)k * (TILE / CP), src, bytes, &w_full[stage]);
-                }
-                __syncwarp();
-                if (++stage == nstage) { stage = 0; ph ^= 1; }
+            auto put = [&](const void* src, uint32_t bytes) { put2(src, bytes, nullptr, 0); };
+            auto res_skip = [&](int l) {
+                const unsigned char* lw = img + (size_t)l * im.layer_bytes;
+                put(lw + 2 * TILE, TILE / 2);
+                for (int c = 0; c < SKC; c++) put(lw + 2 * TILE + TILE / 2 + (size_t)c * TILE, TILE);
             };
-            // conditioning tile g (g counts layers since the start of the launch) -> buffer g % NC
-            int g_cond = 0;
-            auto put_cond = [&](int t, int l) {
-                const int cbuf = g_cond % NC;
-                mbar_wait(&cond_empty[cbuf], ((g_cond / NC) & 1) ^ 1);
-                if (elect_one()) {
-                    mbar_arrive_expect_tx(&cond_full[cbuf], 2 * c_bytes);
-                    tma_load_1d(t_cond + (size_t)cbuf * CB, cond_ptr(t, l, 0), 2 * c_bytes, &cond_full[cbuf]);   // both halves are contiguous
-                    // pull the tiles a few layers ahead from HBM into L2
-                    int tl = t * L + l + 4;
-                    if (tl < t_end * L) tma_prefetch_l2(cond_ptr(tl / L, tl % L, 0), 2 * c_bytes);
-                }
-                __syncwarp();
-                g_cond++;
-            };
-            // Weight-ring chunk order = consumption order of the MMA issuer (see there):
-            //   prev(0) | cur(0) res(0) prev(1) | cur(1) skip(0) res(1) prev(2) | ... | cur(L-1) skip(L-2) res(L-1) | skip(L-1) | Wzs | Wza
-            // where prev(l) = the x[t-d_l] history tile + Wprev_l, present only if t >= d_l.
-            auto put_prev = [&](int t, int l, int d) {
-                if (t >= d) { put_act(ring_tile(t - d, l), TILE / CP); put(img + (size_t)l * im.layer_bytes, TILE); }
-            };
-            auto put_skip = [&](int l) {
-                for (int c = 0; c < S / 128; c++) put(img + (size_t)l * im.layer_bytes + 2 * TILE + TILE / 2 + (size_t)c * TILE, TILE);
-            };
-            if (FUSED) {
-                // chunk order of the fused schedule (see the MMA issuer):
-                //   prev(0) cur(0) prev(1) cur(1) | res(0) Wf(1) skip(0) prev(2) cur(2) | ... | res(L-2) Wf(L-1) skip(L-2) | skip(L-1) | Wzs | Wza
-                // (on the dumping sample skip(l-1) precedes Wf(l), and res(L-1) is computed as well)
-                for (int t = t_begin; t < t_end; t++) {
-                    const bool dstep = p.dump && (t == t_end - 1);
-                    put_cond(t, 0);
-                    put_prev(t, 0, 1);
-                    put(img + TILE, TILE);                              // Wcur_0
-                    if (L > 1) {
-                        put_cond(t, 1);
-                        put_prev(t, 1, s_dil[1]);
-                        put(img + im.layer_bytes + TILE, TILE);         // Wcur_1
-                    }
-                    for (int l = 1; l < L; l++) {
-                        const unsigned char* lw = img + (size_t)l * im.layer_bytes;
-                        if (lane == 0) TRACE(2, 100 + l);
-                        if (NC == 2 && l + 1 < L) put_cond(t, l + 1);
-                        put(lw - im.layer_bytes + 2 * TILE, TILE / 2);  // Wres_{l-1}
-                        if (dstep) put_skip(l - 1);
-                        put(lw + im.l_wf, TILE);                        // Wf_l
-                        if (!dstep) put_skip(l - 1);
-                        if (l + 1 < L) {
-                            // single conditioning buffer: its consumer (gate l) first needs the residual of layer l-1 above
-                            if (NC == 1) put_cond(t, l + 1);
-                            put_prev(t, l + 1, s_dil[l + 1]);
-                            put(lw + im.layer_bytes + TILE, TILE);      // Wcur_{l+1}
-                        }
-                    }
-                    if (dstep) put(img + (size_t)(L - 1) * im.layer_bytes + 2 * TILE, TILE / 2);
-                    put_skip(L - 1);
-                    const unsigned char* ow = img + im.off_out;
-                    for (int c = 0; c < (S / 64) * 2 + (A / 64) * 2; c++) put(ow + (size_t)c * TILE, TILE);
-                }
-            } else
-            for (int t = t_begin; t < t_end; t++) {
-                int d = 1;
-                put_cond(t, 0);
-                put_prev(t, 0, 1);
-                for (int l = 0; l < L; l++) {
-                    const unsigned char* lw = img + (size_t)l * im.layer_bytes;
-                    int dn = d << 1; if (dn > p.maxDil) dn = 1;
-                    if (lane == 0) TRACE(2, 100 + l);
-                    if (l + 1 < L) put_cond(t, l + 1);
-                    put(lw + TILE, TILE);                               // Wcur_l
-                    if (l > 0) put_skip(l - 1);
-                    put(lw + 2 * TILE, TILE / 2);                       // Wres_l
-                    if (l + 1 < L) put_prev(t, l + 1, dn);
-                    d = dn;
-                }
-                put_skip(L - 1);
-                const unsigned char* ow = img + im.off_out;
-                for (int c = 0; c < (S / 64) * 2 + (A / 64) * 2; c++) put(ow + (size_t)c * TILE, TILE);
-            }
-        }
-    } else if (warp >= 9) {
-        // =============================================================== MMA issuer(s) (whole warp converged, one lane issues)
-        {
-            const uint32_t idesc128 = make_idesc_f16(128, 128), idesc64 = make_idesc_f16(128, 64);
-            int stage = 0;
-            uint32_t ph_full = 0, ph_epi = 0;
-            const uint64_t d_ring = make_desc_kmajor_sw128(smem_u32(ring)), d_xc = make_desc_kmajor_sw128(smem_u32(t_xc)),
-                           d_h = make_desc_kmajor_sw128(smem_u32(t_h)), d_big = make_desc_kmajor_sw128(smem_u32(t_big));
-            uint32_t ph_pre = 0;
-            constexpr uint64_t TILE_D = TILE >> 4;                      // one tile further, in descriptor address units
-            auto wait_stage = [&]() -> uint64_t {                       // descriptor of the next ring stage once its data landed
-                mbar_wait(&w_full[stage], ph_full);
-                return d_ring + (uint64_t)stage * TILE_D;
-            };
-            auto advance = [&]() { if (++stage == nstage) { stage = 0; ph_full ^= 1; } };
-            // 4 K-slices of one 64-deep chunk, then (optionally) up to two commits; single elected lane
-            auto mma4 = [&](uint64_t da, uint64_t db, uint32_t d, uint32_t idesc, bool acc0, uint64_t* bar0, uint64_t* bar1) {
-                if (elect_one()) {
-#pragma unroll
-                    for (int k = 0; k < 4; k++) umma_f16(d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (acc0 || k) ? 1u : 0u);
-                    if (bar0) umma_commit(bar0);
-                    if (bar1) umma_commit(bar1);
-                }
-                __syncwarp();
-            };
-            // the epilogue's "tile published" phases alternate between two barriers (role B may be a whole gate behind role A:
-            // on a single barrier it could find TWO completions past the one it waits for, which a parity wait cannot see)
-            int n_epi = 0;
-            auto wait_epi = [&]() {
-                const int k = n_epi & 1;
-                mbar_wait(epi_done + k * 17, (ph_epi >> k) & 1u);
-                ph_epi ^= 1u << k;
-                n_epi++;
-                tc_fence_after_sync();
-            };
-            // open(l): the epilogue has initialised D1[l&1] with Lh[t][l] + Bh (tcgen05.st); add Wprev_l . x[t-d]
-            auto open_layer = [&](int l, bool has_prev) {
-                const uint32_t d1 = D1B + (uint32_t)(l & 1) * 128;
-                mbar_wait(pre_done, ph_pre); ph_pre ^= 1;
-                tc_fence_after_sync();
-                if (has_prev) {
-                    const uint64_t da = wait_stage();
-                    const int sa = stage;
-                    advance();
-                    const uint64_t db = wait_stage();
-                    tc_fence_after_sync();
-                    mma4(da, db, d1, idesc128, true, &w_empty[sa], &w_empty[stage]);
-                    advance();
-                }
-            };
-            // fused schedule: the conditioning and the bias are added by the gate itself, so the FIRST GEMM into an
-            // accumulator overwrites it: Wprev_l . x[t-d] if the history reaches back that far, else the Wcur GEMM
-            auto open_f = [&](int l, bool has_prev, bool wait_x) {
-                if (wait_x) { mbar_wait(pre_done, ph_pre); ph_pre ^= 1; tc_fence_after_sync(); }
-                if (has_prev) {
-                    const uint64_t da = wait_stage();
-                    const int sa = stage;
-                    advance();
-                    const uint64_t db = wait_stage();
-                    tc_fence_after_sync();
-                    mma4(da, db, D1B + (uint32_t)(l & 1) * 128, idesc128, false, &w_empty[sa], &w_empty[stage]);
-                    advance();
-                }
-            };
-            // skip(l): Dskip (+)= Wskip_l . h_l, h_l in the H buffer of parity l
-            auto skip_layer = [&](int l, uint64_t* done_bar) {
-                const uint64_t dh = d_h + (uint64_t)(l & 1) * TILE_D;
-                // all S/128 chunks as ONE issue block: a single election, the commits at the end
-                uint64_t dws[S / 128];
-                int sts[S / 128];
-#pragma unroll
-                for (int c = 0; c < S / 128; c++) { dws[c] = wait_stage(); sts[c] = stage; advance(); }
-                tc_fence_after_sync();
-                if (elect_one()) {
-#pragma unroll
-                    for (int c = 0; c < S / 128; c++)
-#pragma unroll
-                        for (int k = 0; k < 4; k++) umma_f16(DSKIP + c * 128, dh + (uint64_t)(2 * k), dws[c] + (uint64_t)(2 * k), idesc128, (l > 0 || k) ? 1u : 0u);
-#pragma unroll
-                    for (int c = 0; c < S / 128; c++) umma_commit(&w_empty[sts[c]]);
-                    if (done_bar) umma_commit(done_bar);
-                }
-                __syncwarp();
-            };
-            // Issue order per layer: cur(l) | skip(l-1) in the shadow of the gate epilogue | res(l) | prev(l+1) in the shadow
-            // of the residual epilogue.  Nothing but cur / res sits between an epilogue arrival and the accumulator it
-            // waits for.
-            auto out_gemms = [&]() {
-                wait_epi();                                             // relu(skip) tile ready
-                for (int kt = 0; kt < S / 64; kt++)
-                    for (int nh = 0; nh < 2; nh++) {
-                        const uint64_t dw = wait_stage();
-                        tc_fence_after_sync();
-                        const bool last = (kt == S / 64 - 1) && nh == 1;
-                        mma4(d_big + (uint64_t)kt * TILE_D, dw, DZS + nh * 128, idesc128, kt > 0, &w_empty[stage], last ? out_full : nullptr);
-                        advance();
-                    }
-                wait_epi();                                             // relu(Zs) tile ready
-                for (int kt = 0; kt < A / 64; kt++)
-                    for (int nh = 0; nh < 2; nh++) {
-                        const uint64_t dw = wait_stage();
-                        tc_fence_after_sync();
-                        const bool last = (kt == A / 64 - 1) && nh == 1;
-                        mma4(d_big + (uint64_t)kt * TILE_D, dw, DZA + nh * 128, idesc128, kt > 0, &w_empty[stage], last ? out_full : nullptr);
-                        advance();
-                    }
-            };
-            if (FUSED) {
-                // Three single-lane roles share the issue work, which -- not the tensor pipe -- bounds a one-CTA layer
-                // (every group of 4 MMAs + commits costs its issuing thread ~350 cycles, every mbarrier wait ~100):
-                //   A (warp 9)  critical path: per gate h_{l-1}: res(l-1) -> dx_full | Wf(l) -> d1_full | Wcur_{l+1}.x_l
-                //   B (warp 10) background:    skip(l-1) | Wprev_{l+1}.x_{l+1}[t-d]      (+ the nh = 1 half of Zs / Za)
-                //   C (warp 11) history ring:  published x_l tile -> global, one bulk copy (async proxy on both ends)
-                // All walk the same chunk sequence of the weight ring and wait only for their own chunks.
-                //   cx_done  A -> B: Wcur_{l+1}.x_l (which OVERWRITES D1) has completed, Wprev may accumulate
-                //   b_done   B -> gate threads: skip(l-1) [h tile of that parity reusable] and prev(l+1) completed; awaited next to
-                //                    d1_full(l+1), which also bounds how far B can fall behind
-                //   hx_full  epilogue -> C, hx_done C -> A: the copy of x_{l-1} has fully completed before A commits dx_full(l-1)
-                //                    (whose consumer overwrites an x tile) and before the commits that let the producer run on
-                const uint64_t d_x[2] = {d_xc, d_big + 3 * TILE_D};
-                const int role = warp - 9;
-                uint32_t ph_cx = 0, ph_hx = 0;                     // ph_hx: bit k = phase of barrier k of the pair
-                auto wait2 = [&](uint64_t* pair, int stride, uint32_t& ph, int k) {
-                    mbar_wait(pair + (k & 1) * stride, (ph >> (k & 1)) & 1u);
-                    ph ^= 1u << (k & 1);
-                };
-                auto skipc = [&](int n) { for (int i = 0; i < n; i++) advance(); };
-                constexpr int SKC = S / 128;
-                if (role == 2) {
-                    const uint32_t hist_bytes = (uint32_t)(TILE / CP);
-                    for (int t = t_begin; t < t_end; t++)
-                        for (int l = 0; l < L; l++) {
-                            mbar_wait(hx_full, ph_hx); ph_hx ^= 1;
-                            if (lane == 0) {
-                                tma_store_1d(ring_tile(t, l), (l & 1) ? t_x1 : t_xc, hist_bytes);
-                                tma_store_wait_all();
-                                mbar_arrive(hx_done + (l & 1) * 2);
-                            }
-                            __syncwarp();
-                        }
-                } else if (role == 0) {
-                    for (int t = t_begin; t < t_end; t++) {
-                        const bool dstep = p.dump && (t == t_end - 1);
-                        uint64_t dw;
-                        wait_epi();                                     // x_0 tile ready (and Dza of the previous sample consumed)
-                        if (lane == 0) TRACE(1, 20);
-                        open_f(0, t >= 1, false);                       // Wprev_0 . x_0[t-1] stays with A (start of the chain)
-                        dw = wait_stage();
-                        tc_fence_after_sync();
-                        mma4(d_x[0], dw, D1B, idesc128, t >= 1, d1_full, &w_empty[stage]);          // D1[0] (+)= Wcur_0 . x_0
-                        advance();
-                        if (L > 1) {
-                            const bool hp = t >= s_dil[1];
-                            if (hp) skipc(2);                           // B: Wprev_1
-                            dw = wait_stage();
-                            tc_fence_after_sync();
-                            mma4(d_x[0], dw, D1B + 128, idesc128, false, hp ? cx_done : nullptr, &w_empty[stage]);   // D1[1] = Wcur_1 . x_0
-                            advance();
-                        }
-                        for (int l = 1; l < L; l++) {
-                            const uint64_t dh = d_h + (uint64_t)((l - 1) & 1) * TILE_D;
-                            const bool hpn = (l + 1 < L) && t >= s_dil[l + 1];
-                            dw = wait_stage();                          // Wres_{l-1} already landed when h arrives
-                            if (!dstep) {                               // ... and so has Wf_l, the next chunk of the sequence
-                                const int s1 = (stage + 1 == nstage) ? 0 : stage + 1;
-                                mbar_wait(&w_full[s1], s1 ? ph_full : (ph_full ^ 1u));
-                            }
-                            wait_epi();                                 // h_{l-1} ready, D1[(l-1)&1] drained
-                            if (lane == 0) TRACE(1, 22);
-                            // (every tcgen05.commit sits in the election block of the MMAs it tracks: issued with nothing of its
-                            // thread outstanding it never arrives)
-                            mma4(dh, dw, D1B + (uint32_t)((l - 1) & 1) * 128, idesc64, false, dx_full, &w_empty[stage]);      // Dx = Wres . h
-                            advance();
-                            if (lane == 0) TRACE(1, 25);
-                            if (dstep) skip_layer(l - 1, nullptr);      // dumping sample: the skip sum through l-1 must be complete at gate l
-                            dw = wait_stage();
-                            tc_fence_after_sync();
-                            // D1[l] += Wf_l . h; B's share of D1[l] / the free h tile are awaited by the gate threads, not here
-                            mma4(dh, dw, D1B + (uint32_t)(l & 1) * 128, idesc128, true, d1_full, &w_empty[stage]);
-                            advance();
-                            if (lane == 0) TRACE(1, 21);
-                            if (!dstep) skipc(SKC);                     // B: skip(l-1)
-                            // history copy of x_{l-1} complete: before dx_full(l), whose consumer overwrites that x tile, and
-                            // before any further commit lets the producer run on
-                            wait2(hx_done, 2, ph_hx, l - 1);
-                            mbar_wait(pre_done, ph_pre); ph_pre ^= 1;   // x_l tile published, Dx of layer l-1 consumed
-                            tc_fence_after_sync();
-                            if (l + 1 < L) {
-                                if (hpn) skipc(2);                      // B: Wprev_{l+1}
-                                dw = wait_stage();
-                                tc_fence_after_sync();
-                                mma4(d_x[l & 1], dw, D1B + (uint32_t)((l + 1) & 1) * 128, idesc128, false, hpn ? cx_done : nullptr, &w_empty[stage]);   // = Wcur_{l+1} . x_l
-                                advance();
-                            }
-                            if (lane == 0) TRACE(1, 24);
-                        }
-                        wait_epi();                                     // h_{L-1}
-                        wait2(hx_done, 2, ph_hx, L - 1);                // x_{L-1} copied: the activation tiles may be reused
-                        if (dstep) {
-                            dw = wait_stage();
-                            tc_fence_after_sync();
-                            mma4(d_h + (uint64_t)((L - 1) & 1) * TILE_D, dw, D1B + (uint32_t)((L - 1) & 1) * 128, idesc64, false, dx_full, &w_empty[stage]);
-                            advance();
-                            skip_layer(L - 1, skip_full);
-                        } else {
-                            skipc(SKC);
-                        }
-                        if (lane == 0) mbar_arrive(skip_full);          // second arrival: this role's conditions for the output phase
-                        __syncwarp();
-                        // output GEMMs: A takes the nh = 0 half of the columns, B the other
-                        for (int g = 0; g < 2; g++) {
-                            wait_epi();                                 // relu(skip) / relu(Zs) tile ready
-                            const int KT = g ? A / 64 : S / 64;
-                            for (int kt = 0; kt < KT; kt++) {
-                                dw = wait_stage();
-                                tc_fence_after_sync();
-                                mma4(d_big + (uint64_t)kt * TILE_D, dw, (g ? DZA : DZS), idesc128, kt > 0, &w_empty[stage], kt == KT - 1 ? out_full : nullptr);
-                                advance();
-                                skipc(1);
-                            }
-                        }
-                    }
-                } else {
-                    for (int t = t_begin; t < t_end; t++) {
-                        const bool dstep = p.dump && (t == t_end - 1);
-                        // b_done of iteration j (0 at the start of the sample, l in the loop) is committed inside the LAST issue
-                        // block of the iteration, or -- if this role issued nothing -- signalled by a plain arrival
-                        auto bsig = [&](int j) { return b_done + (j & 1) * 3; };
-                        auto prev_b = [&](int l, uint64_t* done_bar) {  // D1[l&1] += Wprev_l . x_l[t-d], after A's overwrite has completed
-                            mbar_wait(cx_done, ph_cx); ph_cx ^= 1;
-                            const uint64_t da = wait_stage();
-                            const int sa = stage;
-                            advance();
-                            const uint64_t db = wait_stage();
-                            tc_fence_after_sync();
-                            if (elect_one()) {
-#pragma unroll
-                                for (int k = 0; k < 4; k++) umma_f16(D1B + (uint32_t)(l & 1) * 128, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc128, 1u);
-                                umma_commit(&w_empty[sa]);
-                                umma_commit(&w_empty[stage]);
-                                if (done_bar) umma_commit(done_bar);
-                            }
-                            __syncwarp();
-                            advance();
-                        };
-                        auto arrive_b = [&](int j) { if (elect_one()) mbar_arrive(bsig(j)); __syncwarp(); };
-                        wait_epi();                                     // x_0
-                        if (t >= 1) skipc(2);                           // A: Wprev_0
-                        skipc(1);                                       // A: Wcur_0
-                        if (L > 1) {
-                            if (t >= s_dil[1]) prev_b(1, bsig(0)); else arrive_b(0);
-                            skipc(1);                                   // A: Wcur_1
-                        }
-                        for (int l = 1; l < L; l++) {
-                            skipc(1);                                   // A: Wres_{l-1}
-                            wait_epi();                                 // h_{l-1}
-                            const bool hpn = (l + 1 < L) && t >= s_dil[l + 1];
-                            if (dstep) skipc(SKC + 1);                  // A: skip(l-1), Wf_l
-                            else { skipc(1); skip_layer(l - 1, hpn ? nullptr : bsig(l)); }
-                            if (l + 1 < L) {
-                                if (hpn) prev_b(l + 1, bsig(l));
-                                skipc(1);                               // A: Wcur_{l+1}
-                            }
-                            if (dstep && !hpn) arrive_b(l);             // nothing issued in this iteration
-                        }
-                        wait_epi();                                     // h_{L-1}
-                        if (dstep) skipc(1 + SKC);
-                        else skip_layer(L - 1, skip_full);
-                        for (int g = 0; g < 2; g++) {
-                            wait_epi();
-                            const int KT = g ? A / 64 : S / 64;
-                            for (int kt = 0; kt < KT; kt++) {
-                                skipc(1);
-                                const uint64_t dw = wait_stage();
-                                tc_fence_after_sync();
-                                mma4(d_big + (uint64_t)kt * TILE_D, dw, (g ? DZA : DZS) + 128, idesc128, kt > 0, &w_empty[stage], kt == KT - 1 ? out_full : nullptr);
-                                advance();
-                            }
-                        }
-                    }
-                }
-            } else if (warp == 9)
             for (int t = t_begin; t < t_end; t++) {
                 int d = 1;                                              // dilation of layer l (nv_wavenet.cuh:99-111)
                 for (int l = 0; l < L; l++) {
-                    int dn = d << 1; if (dn > p.maxDil) dn = 1;         // dilation of layer l + 1
-                    const uint32_t d1 = D1B + (uint32_t)(l & 1) * 128;
-                    uint64_t dw = 0;
-                    if (l > 0) dw = wait_stage();                       // Wcur_l is already in flight: wait for it before x_l
-                    wait_epi();                                         // x_l tile ready (and, for l = 0, Dza consumed)
-                    if (lane == 0) TRACE(1, 20);
-                    if (l == 0) { open_layer(0, t >= 1); dw = wait_stage(); }
-                    tc_fence_after_sync();
-                    mma4(d_xc, dw, d1, idesc128, true, d1_full, &w_empty[stage]);       // D1 += Wcur . x[t]
-                    advance();
-                    if (lane == 0) TRACE(1, 21);
-                    if (l > 0) skip_layer(l - 1, nullptr);              // in the shadow of the gate epilogue
-                    dw = wait_stage();                                  // Wres_l
-                    wait_epi();                                         // h tile ready, D1 consumed
-                    if (lane == 0) TRACE(1, 22);
-                    mma4(d_h + (uint64_t)(l & 1) * TILE_D, dw, d1, idesc64, false, dx_full, &w_empty[stage]);   // Dx = Wres . h
-                    advance();
-                    if (lane == 0) TRACE(1, 23);
-                    if (l + 1 < L) open_layer(l + 1, t >= dn);          // in the shadow of the residual epilogue
-                    if (lane == 0) TRACE(1, 24);
-                    d = dn;
+                    const unsigned char* lw = img + (size_t)l * im.layer_bytes;
+                    put2(cond_ptr(t, l), c_bytes_here, cond_ptr(t, l) + c_bytes, c_bytes_here);
+                    if (t + 1 < t_end && c_bytes_here) tma_prefetch_l2(cond_ptr(t + 1, l), c_bytes_here);
+                    if (t >= d) { put(ring_tile(t - d, l), ATILE); put(lw, TILE); }
+                    put(lw + TILE, TILE);
+                    if (FUSED) {
+                        if (l > 0) { put(lw + im.l_wf, TILE); res_skip(l - 1); }
+                    } else {
+                        res_skip(l);
+                    }
+                    d <<= 1; if (d > p.maxDil) d = 1;
                 }
-                skip_layer(L - 1, skip_full);
-                out_gemms();
+                if (FUSED) res_skip(L - 1);
+                for (int c = 0; c < (S / 64) * 2 + (A / 64) * 2; c++) put(img + im.off_out + (size_t)c * TILE, TILE);
             }
         }
-    } else {
-        // =============================================================== epilogue: 8 warps, TWO threads per utterance
-        // Warp w works on TMEM lane quadrant w % 4 (hardware rule) and on channel half w / 4: thread (quad, lane, ch)
-        // owns row 32*quad + lane and channels [32 ch, 32 ch + 32) of the 64-wide residual / gate, i.e. 16-byte chunks
-        // 4 ch .. 4 ch + 3 of its row in every 128-byte tile row.  Two warps per scheduler hide each other's latencies.
-        constexpr int NS = 2 * CP;                      // threads per utterance
-        constexpr int CW = 64 / NS;                     // residual / gate channels per thread
-        constexpr int CQ = CW / 8;                      // 16-byte chunks per thread in a 128-byte tile row
-        const int quad = warp & 3, ch = warp >> 2;
-        const int row = quad * 32 + lane;               // TMEM lane / tile row this thread reads
-        const int u = row & (TU - 1);                   // utterance of the tile
-        const int sub = ch * CP + row / TU;             // which CW-wide slice of the channels is mine
-        const int b = tile * TU + u;
-        const bool valid = b < B;
-        const bool wv = tile * TU + ((quad * 32) & (TU - 1)) < B;   // warp has a live utterance: dead warps only keep
-                                                        // the barrier protocol going (their rows are never read back)
-        const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-        const int c32 = CW * sub, q4 = CQ * sub;        // first channel / first chunk of this thread
-        // rows of the activation tiles this thread writes: its own row, and with DUP the twin row of the utterance
-        auto st_tile = [&](unsigned char* tile_base, int q, uint4 v) {
+        return;
+    }
+
+    // =============================================================== consumers: two warpgroups
+    const int wg = tid >> 7, i = tid & 127;
+    const int r0 = 16 * (i >> 5) + ((i & 31) >> 2), cq = 2 * (i & 3);
+    const int ch0 = 32 * wg + cq;                  // residual / gate channel of fragment column 0
+    int bb[2];
+    bool valid[2];
+    int yp[2], yc[2];
 #pragma unroll
-            for (int k = 0; k < CP; k++) *reinterpret_cast<uint4*>(tile_base + chunk_off(u + k * TU, q)) = v;   // same (row & 7): same swizzle
-        };
-        auto tmem_ldc = [&](uint32_t addr, uint32_t (&r)[32]) {       // CW columns into r[0..CW)
-            if constexpr (CW == 32) { tmem_ld32(addr, r); }
-            else if constexpr (CW == 16) {
-                uint32_t t16[16];
-                tmem_ld16(addr, t16);
+    for (int r = 0; r < 2; r++) {
+        bb[r] = tile * tu + row0 + r0 + 8 * r;
+        valid[r] = r0 + 8 * r < live && bb[r] < B;
+        yp[r] = valid[r] ? p.yPrev[bb[r]] : 0;
+        yc[r] = valid[r] ? p.yCur[bb[r]] : 0;
+    }
+    const __half* embPrev = static_cast<const __half*>(p.embPrev);
+    const __half* embCur = static_cast<const __half*>(p.embCur);
+    const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
+
+    int stage = 0;
+    uint32_t ph = 0;
+    auto take = [&](int& s) -> const unsigned char* {              // next ring stage, once its data has landed
+        s = stage;
+        mbar_wait(&w_full[stage], ph);
+        if (++stage == nstage) { stage = 0; ph ^= 1; }
+        return ring + (size_t)s * TILE;
+    };
+    auto release = [&](int s) { mbar_arrive(&w_empty[s]); };
+    auto desc = [](const void* p_) { return make_desc_sw128(smem_u32(p_)); };
+
+    float x[16];                                   // residual stream (fp32) of this thread's 16 (row, channel) pairs
+    float acc_s[SKN / 2];                          // skip sum over the layers, without biases
+    float acc_x[16];                               // Dx = Wres.h of the latest residual GEMM
+
+    for (int t = t_begin; t < t_end; t++) {
+        const bool dump = p.dump && (t == t_end - 1);
+        // ---------------- embedding: x0 = tanh(embPrev[yPrev] + embCur[yCur])   (reference.cpp:42-57)
 #pragma unroll
-                for (int i = 0; i < 16; i++) r[i] = t16[i];
-            } else {
-                uint32_t t8[8];
-                tmem_ld8(addr, t8);
+        for (int r = 0; r < 2; r++)
 #pragma unroll
-                for (int i = 0; i < 8; i++) r[i] = t8[i];
+            for (int j = 0; j < 4; j++) {
+                const int c = ch0 + 8 * j;
+                const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(embPrev + (size_t)yp[r] * R + c));
+                const float2 fc = __half22float2(*reinterpret_cast<const __half2*>(embCur + (size_t)yc[r] * R + c));
+                float e0 = fa.x + fc.x, e1 = fa.y + fc.y;
+                if (p.tanhEmbed) { e0 = wn::tanhf_fast(e0); e1 = wn::tanhf_fast(e1); }
+                if (!valid[r]) { e0 = 0.f; e1 = 0.f; }
+                x[4 * j + 2 * r] = e0; x[4 * j + 2 * r + 1] = e1;
             }
-        };
-        uint32_t ph_d1 = 0, ph_dx = 0, ph_skip = 0, ph_out = 0, ph_bd = 0;
-        const __half* embPrev = static_cast<const __half*>(p.embPrev);
-        const __half* embCur = static_cast<const __half*>(p.embCur);
-        const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
-        int yp = valid ? p.yPrev[b] : 0, yc = valid ? p.yCur[b] : 0;
-        float x[CW];                                  // this thread's slice of the residual stream (fp32)
+        // x tile and history ring: both hold x_l as the SW128 image of 64 rows (the ring is read back by TMA d samples later)
+        auto publish_x = [&](unsigned char* xt, unsigned char* gdst) {
 #pragma unroll
-        for (int i = 0; i < CW; i++) x[i] = 0.f;
-        // History ring (global, read back d samples later by TMA): written AFTER the barrier arrival that publishes the
-        // shared-memory tile, then fenced towards the async proxy while this thread would be waiting for the MMA anyway.
-        auto store_history = [&](unsigned char* grow) {
+            for (int r = 0; r < 2; r++)
 #pragma unroll
-            for (int q = 0; q < CQ; q++) {
-                uint32_t o[4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) o[j] = pack_h2(x[8 * q + 2 * j], x[8 * q + 2 * j + 1]);
-                *reinterpret_cast<uint4*>(grow + chunk_off(u, q4 + q)) = make_uint4(o[0], o[1], o[2], o[3]);   // one copy: row u
-            }
+                for (int j = 0; j < 4; j++) {
+                    st_pair(xt, r0 + 8 * r, ch0 + 8 * j, x[4 * j + 2 * r], x[4 * j + 2 * r + 1]);
+                    st_pair(gdst, r0 + 8 * r, ch0 + 8 * j, x[4 * j + 2 * r], x[4 * j + 2 * r + 1]);
+                }
             fence_proxy_async_global();
         };
-        int n_pub = 0;                                 // tiles published so far: selects the barrier of the pair
-        auto publish = [&]() {                         // smem tile written -> visible to the MMA (async proxy), then signal
-            tc_fence_before_sync();
-            fence_proxy_async_smem();
-            mbar_arrive(epi_done + (n_pub & 1) * 17);
-            n_pub++;
-        };
-        auto epi_bar = [&]() { asm volatile("bar.sync 1, 256;" ::: "memory"); };
-        // Initialise the pre-activation accumulator of layer `ln` with Lh[tn][ln] + Bh (fp32) straight from the TMA-fed
-        // conditioning buffer: tcgen05.st, done while this thread would otherwise wait for the residual GEMM.  Each row
-        // needs all 128 columns from the two threads that may touch its TMEM lane: channel half `ch`, both gate halves.
-        int g_pre = 0;
-        bool tr_on = false;
-        auto prestore = [&](int ln) {
-            const int cbuf = g_pre % NC;
-            mbar_wait(&cond_full[cbuf], (g_pre / NC) & 1);
-            if (tid == tr_tid && trc && tr_on && trn < 1023) trc[trn++] = (14ull << 48) | (clock64() & 0xFFFFFFFFFFFFull);
-            if (wv) {
-                const unsigned char* cb = t_cond + (size_t)cbuf * CB;
-                const uint32_t d1n = D1B + (uint32_t)(ln & 1) * 128 + lane_off;
-                // only the columns the gate thread of THIS row reads: [c32, c32 + CW) of both gate halves (with DUP the other
-                // columns of the row belong to the twin row's thread and are never read from this one)
+        publish_x(t_xb, ring_tile(t, 0));
+        fence_proxy_async_smem();
+        consumer_sync();                                                // x_0 tile complete
+
+        // Wres_l.h -> acc_x and Wskip_l.h -> acc_s (issued into the current wgmma batch; the caller commits and waits)
+        auto issue_res_skip = [&](int l, const unsigned char* th, int& sr, int (&sk)[SKC]) {
+            const unsigned char* wr = take(sr);
+            const unsigned char* wk[SKC];
 #pragma unroll
-                for (int half = 0; half < 2; half++) {
-                    const float* bh = s_bh + (size_t)ln * 128 + 64 * half + c32;
-                    uint32_t v[CW];
+            for (int c = 0; c < SKC; c++) wk[c] = take(sk[c]);
+            const uint64_t dh = desc(th), dr = desc(wr + 32 * wg * 128);
+            const uint64_t ds = (S == 256) ? desc(wk[wg]) : desc(wk[0] + SKN * wg * 128);
 #pragma unroll
-                    for (int q = 0; q < CQ; q++) {
-                        const uint4 w = *reinterpret_cast<const uint4*>(cb + (size_t)half * c_bytes + chunk_off(u, q4 + q));
-                        const uint32_t wv4[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-                        for (int j = 0; j < 4; j++) {
-                            const float2 f = unpack_h2(wv4[j]);
-                            v[8 * q + 2 * j] = __float_as_uint(f.x + bh[8 * q + 2 * j]);
-                            v[8 * q + 2 * j + 1] = __float_as_uint(f.y + bh[8 * q + 2 * j + 1]);
-                        }
-                    }
-                    if constexpr (CW == 32) tmem_st32(d1n + 64 * half + c32, v);
-                    else if constexpr (CW == 16) tmem_st16(d1n + 64 * half + c32, v);
-                    else tmem_st8(d1n + 64 * half + c32, v);
-                }
-                tmem_st_wait();
+            for (int k = 0; k < 4; k++) {
+                wgmma_f16<32>(acc_x, dh + 2 * k, dr + 2 * k, k > 0);
+                wgmma_f16<SKN>(acc_s, dh + 2 * k, ds + 2 * k, l > 0 || k > 0);
             }
-            if (tid == tr_tid && trc && tr_on && trn < 1023) trc[trn++] = (15ull << 48) | (clock64() & 0xFFFFFFFFFFFFull);
-            tc_fence_before_sync();
-            mbar_arrive(&cond_empty[cbuf]);
-            mbar_arrive(pre_done);
-            g_pre++;
         };
-        // relu(acc + bias) of this thread's half of a 256(or S)-wide accumulator -> fp16 rows of the 4-k-tile activation tile
-        auto relu_to_tile = [&](uint32_t dacc, const float* bias, int width, float* dump_dst) {
-            const int c_lo = sub * (width / NS);
-#pragma unroll 1
-            for (int c0 = c_lo; c0 < c_lo + width / NS; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld32(dacc + lane_off + c0, v);
-                tmem_ld_wait();
-                uint32_t o[16];
+        auto release_res_skip = [&](int sr, const int (&sk)[SKC]) {
+            release(sr);
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 bb = *reinterpret_cast<const float4*>(bias + c0 + j);
-                    float v0 = fmaxf(__uint_as_float(v[j]) + bb.x, 0.f), v1 = fmaxf(__uint_as_float(v[j + 1]) + bb.y, 0.f);
-                    float v2 = fmaxf(__uint_as_float(v[j + 2]) + bb.z, 0.f), v3 = fmaxf(__uint_as_float(v[j + 3]) + bb.w, 0.f);
-                    if (!valid) { v0 = 0.f; v1 = 0.f; v2 = 0.f; v3 = 0.f; }
-                    o[j >> 1] = pack_h2(v0, v1);
-                    o[(j >> 1) + 1] = pack_h2(v2, v3);
-                }
-                if (dump_dst && valid) {                                // last sample of a dumping launch only
+            for (int c = 0; c < SKC; c++) release(sk[c]);
+        };
+        // residual: x += Dx + Bres_l   (reference.cpp:82-84), then the dumps of layer l
+        auto residual = [&](int l) {
 #pragma unroll
-                    for (int j = 0; j < 32; j++) dump_dst[c0 + j] = fmaxf(__uint_as_float(v[j]) + bias[c0 + j], 0.f);
-                }
-                unsigned char* kt = t_big + (size_t)(c0 >> 6) * TILE;
-                const int q = (c0 & 63) >> 3;
+            for (int r = 0; r < 2; r++)
 #pragma unroll
-                for (int i = 0; i < 4; i++) st_tile(kt, q + i, make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]));
+                for (int j = 0; j < 4; j++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int q = 4 * j + 2 * r + e, c = ch0 + 8 * j + e;
+                        x[q] = valid[r] ? x[q] + (acc_x[q] + gbias[im.b_bres + (size_t)l * 64 + c]) : 0.f;
+                        if (dump && valid[r]) p.xtOut[((size_t)l * B + bb[r]) * R + c] = x[q];
+                    }
+            if (dump && l + 1 < L) {                                    // skip sum through layer l (the last one is dumped after relu)
+#pragma unroll
+                for (int j = 0; j < SKN / 8; j++)
+#pragma unroll
+                    for (int e = 0; e < 4; e++) {
+                        const int r = e >> 1, s = SKN * wg + 8 * j + cq + (e & 1);
+                        if (valid[r]) p.skipOut[((size_t)l * B + bb[r]) * S + s] = acc_s[4 * j + e] + gbias[im.b_bskp + (size_t)l * S + s];
+                    }
             }
         };
 
-        for (int t = t_begin; t < t_end; t++) {
-            const bool dump = p.dump && (t == t_end - 1);
-            tr_on = (t == tr_t);
-            const float sel = valid ? __ldg(p.sel + (size_t)t * B + b) : 0.5f;
-            if (!FUSED) prestore(0);                                    // D1[0] <- Lh[t][0] + Bh (Dza of the previous sample is consumed)
-            // ---------------- embedding: x0 = tanh(embPrev[yPrev] + embCur[yCur])   (reference.cpp:42-57)
-            if (wv) {
-                const uint4* ep = reinterpret_cast<const uint4*>(embPrev + (size_t)yp * R + c32);
-                const uint4* ec = reinterpret_cast<const uint4*>(embCur + (size_t)yc * R + c32);
+        int d = 1;
+        for (int l = 0; l < L; l++) {
+            // ---------------- Lh[t][l] + Bh (FUSED, l > 0: Bh') of this thread's gate inputs, from the TMA-fed conditioning chunk
+            float cnd_a[16], cnd_g[16];
+            {
+                int sc;
+                const unsigned char* cb = take(sc);
+                const float* bh = gbias + ((FUSED && l > 0) ? im.b_bhf : im.b_bh) + (size_t)l * 128;
 #pragma unroll
-                for (int q = 0; q < CQ; q++) {
-                    const uint4 a = __ldg(ep + q), c = __ldg(ec + q);
-                    const uint32_t av[4] = {a.x, a.y, a.z, a.w}, cv[4] = {c.x, c.y, c.z, c.w};
-                    uint32_t o[4];
+                for (int r = 0; r < 2; r++)
 #pragma unroll
                     for (int j = 0; j < 4; j++) {
-                        const float2 fa = unpack_h2(av[j]), fc = unpack_h2(cv[j]);
-                        float e0 = fa.x + fc.x, e1 = fa.y + fc.y;
-                        if (p.tanhEmbed) { e0 = wn::tanhf_fast(e0); e1 = wn::tanhf_fast(e1); }
-                        if (!valid) { e0 = 0.f; e1 = 0.f; }
-                        x[8 * q + 2 * j] = e0; x[8 * q + 2 * j + 1] = e1;
-                        o[j] = pack_h2(e0, e1);
+                        const int c = ch0 + 8 * j, row = r0 + 8 * r;
+                        const float2 la = unpack_h2(*reinterpret_cast<const uint32_t*>(cb + sw128_offset(row, c)));
+                        const float2 lg = unpack_h2(*reinterpret_cast<const uint32_t*>(cb + ATILE + sw128_offset(row, c)));
+                        const float2 ba = *reinterpret_cast<const float2*>(bh + c);
+                        const float2 bg = *reinterpret_cast<const float2*>(bh + 64 + c);
+                        cnd_a[4 * j + 2 * r] = la.x + ba.x; cnd_a[4 * j + 2 * r + 1] = la.y + ba.y;
+                        cnd_g[4 * j + 2 * r] = lg.x + bg.x; cnd_g[4 * j + 2 * r + 1] = lg.y + bg.y;
                     }
-                    st_tile(t_xc, q4 + q, make_uint4(o[0], o[1], o[2], o[3]));
-                }
+                release(sc);
             }
-            publish();                                                  // x_0 ready
-            if (FUSED) mbar_arrive(hx_full);
-            if (tid == tr_tid) TRACE(0, 1);
-            if (!FUSED && wv) store_history(ring_tile(t, 0));
-
-            // fused schedule: Lh[t][l] + Bh' of this thread's channels from the TMA-fed conditioning buffer -> registers
-            // (done BEFORE waiting for the accumulator)
-            float cnd[2 * CW];
-            auto load_cond = [&](int ln) {
-                const int cbuf = g_pre % NC;
-                mbar_wait(&cond_full[cbuf], (g_pre / NC) & 1);
-                if (tid == tr_tid) TRACE(0, 14);
-                if (wv) {
-                    const unsigned char* cb = t_cond + (size_t)cbuf * CB;
+            // ---------------- pre-activation: Wprev.x[t-d] + Wcur.x   (reference.cpp:67-80); FUSED: x = x_{l-1}, + Wf.h_{l-1}
+            const unsigned char* t_x = t_xb + (FUSED ? (size_t)((l + 1) & 1) * ATILE : 0);     // FUSED, l > 0: x_{l-1}
+            const unsigned char* t_hp = t_hb + (size_t)((l + 1) & 1) * ATILE;                  // FUSED: h_{l-1}
+            float acc_a[16], acc_g[16];
+            {
+                const bool hp = t >= d;
+                int sh = 0, sp = 0, sw, sf = 0, sr = 0, sk[SKC];
+                wgmma_fence();
+                if (hp) {
+                    const uint64_t dhx = desc(take(sh));
+                    const unsigned char* wp = take(sp);
+                    const uint64_t dpa = desc(wp + 32 * wg * 128), dpg = desc(wp + (64 + 32 * wg) * 128);
 #pragma unroll
-                    for (int half = 0; half < 2; half++) {
-                        const float* bh = s_bh + (size_t)ln * 128 + 64 * half + c32;
-#pragma unroll
-                        for (int q = 0; q < CQ; q++) {
-                            const uint4 w = *reinterpret_cast<const uint4*>(cb + (size_t)half * c_bytes + chunk_off(u, q4 + q));
-                            const uint32_t wv4[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-                            for (int j = 0; j < 4; j++) {
-                                const float2 f = unpack_h2(wv4[j]);
-                                cnd[half * CW + 8 * q + 2 * j] = f.x + bh[8 * q + 2 * j];
-                                cnd[half * CW + 8 * q + 2 * j + 1] = f.y + bh[8 * q + 2 * j + 1];
-                            }
-                        }
+                    for (int k = 0; k < 4; k++) {
+                        wgmma_f16<32>(acc_a, dhx + 2 * k, dpa + 2 * k, k > 0);
+                        wgmma_f16<32>(acc_g, dhx + 2 * k, dpg + 2 * k, k > 0);
                     }
+                    wgmma_commit();
                 }
-                mbar_arrive(&cond_empty[cbuf]);
-                g_pre++;
-            };
-            // gate of layer l: D1[l&1] -> h tile of parity l
-            auto gate = [&](int l) {
-                const uint32_t d1 = D1B + (uint32_t)(l & 1) * 128 + lane_off;
-                unsigned char* th = t_h + (size_t)(l & 1) * TILE;
-                uint32_t ta[32], sa[32];
-                tmem_ldc(d1 + c32, ta);
-                tmem_ldc(d1 + 64 + c32, sa);
-                tmem_ld_wait();
-                if (tid == tr_tid) TRACE(0, 16);
-                uint32_t hp[CW / 2];
+                const unsigned char* wc = take(sw);
+                const uint64_t dx = desc(l == 0 ? t_xb : t_x), dca = desc(wc + 32 * wg * 128), dcg = desc(wc + (64 + 32 * wg) * 128);
 #pragma unroll
-                for (int j = 0; j < CW; j += 2) {
-                    float a0 = __uint_as_float(ta[j]), a1 = __uint_as_float(ta[j + 1]);
-                    float g0 = __uint_as_float(sa[j]), g1 = __uint_as_float(sa[j + 1]);
-                    if (FUSED) {
-                        // the gate is MUFU-bound (2 transcendental per channel): evaluate both as packed fp16 pairs, one
-                        // MUFU.TANH per TWO values; h is rounded to fp16 for the next GEMM anyway
-                        a0 += cnd[j]; a1 += cnd[j + 1]; g0 += cnd[CW + j]; g1 += cnd[CW + j + 1];
-                        const __half2 th = wn::tanh_h2(__floats2half2_rn(a0, a1));
-                        const __half2 tg = wn::tanh_h2(__floats2half2_rn(0.5f * g0, 0.5f * g1));
-                        const __half2 hh = __hmul2(th, __hfma2(tg, __float2half2_rn(0.5f), __float2half2_rn(0.5f)));
-                        hp[j >> 1] = *reinterpret_cast<const uint32_t*>(&hh);
-                    } else {
-                        const float h0 = wn::tanhf_fast(a0) * wn::sigmoidf_fast(g0);
-                        const float h1 = wn::tanhf_fast(a1) * wn::sigmoidf_fast(g1);
-                        hp[j >> 1] = pack_h2(h0, h1);
+                for (int k = 0; k < 4; k++) {
+                    wgmma_f16<32>(acc_a, dx + 2 * k, dca + 2 * k, hp || k > 0);
+                    wgmma_f16<32>(acc_g, dx + 2 * k, dcg + 2 * k, hp || k > 0);
+                }
+                if (FUSED && l > 0) {
+                    wgmma_commit();
+                    const unsigned char* wf = take(sf);
+                    const uint64_t dh = desc(t_hp), dfa = desc(wf + 32 * wg * 128), dfg = desc(wf + (64 + 32 * wg) * 128);
+#pragma unroll
+                    for (int k = 0; k < 4; k++) {
+                        wgmma_f16<32>(acc_a, dh + 2 * k, dfa + 2 * k, 1u);
+                        wgmma_f16<32>(acc_g, dh + 2 * k, dfg + 2 * k, 1u);
                     }
+                    wgmma_commit();
+                    // the history / Wprev stages go back to the producer before the residual and skip chunks are taken: a
+                    // warpgroup never holds more than five ring stages at once
+                    if (hp) { wgmma_wait<2>(); release(sh); release(sp); }
+                    issue_res_skip(l - 1, t_hp, sr, sk);
                 }
-#pragma unroll
-                for (int q = 0; q < CQ; q++) st_tile(th, q4 + q, make_uint4(hp[4 * q], hp[4 * q + 1], hp[4 * q + 2], hp[4 * q + 3]));
-                if (tid == tr_tid) TRACE(0, 12);
-            };
-            // residual of layer l: x += Dx + Bres (Dx in columns [0,64) of D1[l&1]); optionally -> x tile `xt`
-            auto residual = [&](int l, unsigned char* xt) {
-                const uint32_t d1 = D1B + (uint32_t)(l & 1) * 128 + lane_off;
-                const float* br = s_bres + (size_t)l * 64 + c32;
-                uint32_t v[32];
-                tmem_ldc(d1 + c32, v);
-                tmem_ld_wait();
-                uint32_t o[CW / 2];
-#pragma unroll
-                for (int j = 0; j < CW; j += 2) {
-                    const float2 bb = *reinterpret_cast<const float2*>(br + j);
-                    float v0 = x[j] + (__uint_as_float(v[j]) + bb.x), v1 = x[j + 1] + (__uint_as_float(v[j + 1]) + bb.y);
-                    if (!valid) { v0 = 0.f; v1 = 0.f; }
-                    x[j] = v0; x[j + 1] = v1;
-                    o[j >> 1] = pack_h2(v0, v1);
-                }
-                if (xt) {
-#pragma unroll
-                    for (int q = 0; q < CQ; q++) st_tile(xt, q4 + q, make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]));
-                }
-                if (dump && valid) {                                    // last sample of a dumping launch only
-#pragma unroll
-                    for (int j = 0; j < CW; j++) p.xtOut[((size_t)l * B + b) * R + c32 + j] = x[j];
-                }
-            };
-            // dump only: skip sum through layer l (complete, and the next contribution not yet issued, at the call sites)
-            auto dump_skip = [&](int l) {
-                const int c_lo = sub * (S / NS);
-                for (int c0 = c_lo; c0 < c_lo + S / NS; c0 += 16) {
-                    uint32_t w[16];
-                    tmem_ld16(DSKIP + lane_off + c0, w);
-                    tmem_ld_wait();
-                    if (valid)
-                        for (int j = 0; j < 16; j++)
-                            p.skipOut[((size_t)l * B + b) * S + c0 + j] = __uint_as_float(w[j]) + gbias[im.b_bskp + (size_t)l * S + c0 + j];
-                }
-            };
-
+                wgmma_commit();
+                wgmma_wait<0>();
+                if (hp && !(FUSED && l > 0)) { release(sh); release(sp); }
+                release(sw);
+                if (FUSED && l > 0) { release(sf); release_res_skip(sr, sk); }
+            }
             if (FUSED) {
-                for (int l = 0; l < L; l++) {
-                    load_cond(l);                                       // in the shadow of the residual GEMM
-                    if (tid == tr_tid) TRACE(0, 5);
-                    if (l > 0) {
-                        // x_l = x_{l-1} + Wres_{l-1}.h_{l-1} + Bres_{l-1}: needed by the NEXT layer's background GEMM and the history
-                        mbar_wait(dx_full, ph_dx); ph_dx ^= 1;
-                        tc_fence_after_sync();
-                        if (tid == tr_tid) TRACE(0, 4);
-                        if (wv) residual(l - 1, (l & 1) ? t_x1 : t_xc);
-                        tc_fence_before_sync();                         // x_l tile published, Dx consumed
-                        fence_proxy_async_smem();
-                        mbar_arrive(pre_done);
-                        mbar_arrive(hx_full);
-                        if (tid == tr_tid) TRACE(0, 13);
-                        // B's share of this layer's accumulator (Wprev . x[t-d]) is complete and skip(l-2) has released the h tile
-                        mbar_wait(b_done + ((l - 1) & 1) * 3, (ph_bd >> ((l - 1) & 1)) & 1u); ph_bd ^= 1u << ((l - 1) & 1);
-                    }
-                    mbar_wait(d1_full, ph_d1); ph_d1 ^= 1;
-                    tc_fence_after_sync();
-                    if (tid == tr_tid) TRACE(0, 2);
-                    if (wv) gate(l);
-                    if (dump && l > 0 && wv) dump_skip(l - 1);
-                    publish();                                          // h_l ready, D1[l&1] drained
-                    if (tid == tr_tid) TRACE(0, 3);
+                // x_l = x_{l-1} + Wres_{l-1}.h_{l-1} + Bres_{l-1} -> x tile of parity l (next layer's Wcur operand) + history ring;
+                // the other warpgroup may still read the tiles of parity l-1, never those of parity l (one barrier per layer)
+                if (l > 0) {
+                    residual(l - 1);
+                    publish_x(t_xb + (size_t)(l & 1) * ATILE, ring_tile(t, l));
                 }
-                if (L > 1) { mbar_wait(b_done + ((L - 1) & 1) * 3, (ph_bd >> ((L - 1) & 1)) & 1u); ph_bd ^= 1u << ((L - 1) & 1); }
-                if (dump) {
-                    mbar_wait(dx_full, ph_dx); ph_dx ^= 1;
-                    tc_fence_after_sync();
-                    if (wv) residual(L - 1, nullptr);
+            }
+            // ---------------- gate: h = tanh(a) * sigmoid(g) -> h tile
+            unsigned char* t_h = t_hb + (FUSED ? (size_t)(l & 1) * ATILE : 0);
+#pragma unroll
+            for (int r = 0; r < 2; r++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const int q = 4 * j + 2 * r;
+                    float h0 = wn::tanhf_fast(acc_a[q] + cnd_a[q]) * wn::sigmoidf_fast(acc_g[q] + cnd_g[q]);
+                    float h1 = wn::tanhf_fast(acc_a[q + 1] + cnd_a[q + 1]) * wn::sigmoidf_fast(acc_g[q + 1] + cnd_g[q + 1]);
+                    if (!valid[r]) { h0 = 0.f; h1 = 0.f; }
+                    st_pair(t_h, r0 + 8 * r, ch0 + 8 * j, h0, h1);
                 }
-            } else
-            for (int l = 0; l < L; l++) {
-                // ---------------- gate: h = tanh(a[0:R]) * sigmoid(a[R:2R]); D1 already holds the complete pre-activation
-                // a = (Lh[t][l] + Bh) + Wprev.x[t-d] + Wcur.x[t]   (reference.cpp:67-80)
-                mbar_wait(d1_full, ph_d1); ph_d1 ^= 1;
-                tc_fence_after_sync();
-                if (tid == tr_tid) TRACE(0, 2);
-                if (wv) gate(l);
-                publish();                                              // h ready, D1 drained
-                if (tid == tr_tid) TRACE(0, 3);
-                if (l + 1 < L) prestore(l + 1);                         // while the residual GEMM runs
-                // ---------------- residual: x += Dx + Bres   (reference.cpp:82-84)
-                mbar_wait(dx_full, ph_dx); ph_dx ^= 1;
-                tc_fence_after_sync();
-                if (tid == tr_tid) TRACE(0, 4);
-                if (wv) {
-                    residual(l, (l + 1 < L) ? t_xc : nullptr);
-                    // skip sum through layer l-1 is complete here (its MMAs precede this layer's residual GEMM) and the
-                    // next contribution is only issued after the arrival below: no extra barrier needed
-                    if (dump && l > 0) dump_skip(l - 1);
-                }
+            fence_proxy_async_smem();
+            consumer_sync();                                            // h_l (FUSED: and x_l) tiles complete
+            if (!FUSED) {
+                // ---------------- Dx = Wres.h (this warpgroup's 32 channels), skip += Wskip.h (its S/2 columns)
+                int sr, sk[SKC];
+                wgmma_fence();
+                issue_res_skip(l, t_h, sr, sk);
+                wgmma_commit();
+                wgmma_wait<0>();
+                release_res_skip(sr, sk);
+                residual(l);
                 if (l + 1 < L) {
-                    publish();                                          // x_{l+1} ready
-                    if (tid == tr_tid) TRACE(0, 5);
-                    if (wv) store_history(ring_tile(t, l + 1));
+                    publish_x(t_xb, ring_tile(t, l + 1));
+                    fence_proxy_async_smem();
+                    consumer_sync();                                    // x_{l+1} tile complete
                 }
             }
-
-            // ---------------- relu(skip) -> GEMM input of the first output layer   (reference.cpp:88-90)
-            mbar_wait(skip_full, ph_skip); ph_skip ^= 1;
-            tc_fence_after_sync();
-            if (tid == tr_tid) TRACE(0, 6);
-            if (wv) relu_to_tile(DSKIP, s_bsk, S, dump ? p.skipOut + ((size_t)(L - 1) * B + b) * S : nullptr);
-            publish();                                                  // relu(skip) tile ready
-            if (tid == tr_tid) TRACE(0, 7);
-
-            // ---------------- Zs = relu(Wzs . skip + Bzs)   (reference.cpp:96-98)
-            mbar_wait(out_full, ph_out); ph_out ^= 1;
-            tc_fence_after_sync();
-            if (wv) relu_to_tile(DZS, s_bzs, A, dump ? p.Zs + (size_t)b * A : nullptr);
-            publish();                                                  // relu(Zs) tile ready
-            if (tid == tr_tid) TRACE(0, 9);
-
-            // ---------------- Za, softmax, categorical sample   (reference.cpp:100-121)
-            // The two threads of an utterance each take 128 logits: a first TMEM pass finds the local max in fp32, a second one parks
-            // (z - max) as fp16 in the thread's own row of the (now dead) activation tiles -- the rounding error is proportional to the
-            // distance from the max, i.e. negligible where the probability mass is; exp / sums / scan run from shared memory; the
-            // halves meet through s_pair (local max, local sum) and s_y.
-            mbar_wait(out_full, ph_out); ph_out ^= 1;
-            tc_fence_after_sync();
-            if (tid == tr_tid) TRACE(0, 10);
-            constexpr int PART = A / NS, NCH = PART / 16;               // logits per thread, 16-logit chunks per thread
-            const int a_lo = sub * PART;
-            float mx = 0.f;                                             // matrix.cpp:171 starts the max at 0
-            float csum[NCH];
-            float lsum = 0.f;
-            auto expz = [&](uint32_t packed, float& e0, float& e1) {       // packed = (z - local max) in fp16
-                const float2 z = unpack_h2(packed);
-                e0 = wn::exp2f_fast(z.x * 1.4426950408889634f);
-                e1 = wn::exp2f_fast(z.y * 1.4426950408889634f);
-            };
-            if (wv) {
-#pragma unroll 1
-                for (int c0 = a_lo; c0 < a_lo + PART; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(DZA + lane_off + c0, v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) {
-                        const float z0 = __uint_as_float(v[j]) + s_bza[c0 + j], z1 = __uint_as_float(v[j + 1]) + s_bza[c0 + j + 1];
-                        mx = fmaxf(mx, fmaxf(z0, z1));
-                        if (dump && valid) { p.Za[(size_t)b * A + c0 + j] = z0; p.Za[(size_t)b * A + c0 + j + 1] = z1; }
-                    }
-                }
-#pragma unroll 1
-                for (int c0 = a_lo; c0 < a_lo + PART; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(DZA + lane_off + c0, v);
-                    tmem_ld_wait();
-                    uint32_t o[16];
-#pragma unroll
-                    for (int j = 0; j < 32; j += 2) {
-                        const float z0 = __uint_as_float(v[j]) + s_bza[c0 + j], z1 = __uint_as_float(v[j + 1]) + s_bza[c0 + j + 1];
-                        o[j >> 1] = pack_h2(z0 - mx, z1 - mx);
-                    }
-                    unsigned char* kt = t_big + (size_t)(c0 >> 6) * TILE;      // scratch: own row only
-                    const int q = (c0 & 63) >> 3;
-#pragma unroll
-                    for (int i = 0; i < 4; i++)
-                        *reinterpret_cast<uint4*>(kt + chunk_off(row, q + i)) = make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-                }
-#pragma unroll
-                for (int c = 0; c < NCH; c++) {
-                    const int c0 = a_lo + 16 * c;
-                    const unsigned char* kt = t_big + (size_t)(c0 >> 6) * TILE;
-                    const int q = (c0 & 63) >> 3;
-                    const uint4 u0 = *reinterpret_cast<const uint4*>(kt + chunk_off(row, q)), u1 = *reinterpret_cast<const uint4*>(kt + chunk_off(row, q + 1));
-                    const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
-                    float sacc = 0.f;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) { float e0, e1; expz(w[j], e0, e1); sacc += e0; sacc += e1; }
-                    csum[c] = sacc;
-                    lsum += sacc;
-                }
-                s_pair[(u * NS + sub) * 2] = mx;
-                s_pair[(u * NS + sub) * 2 + 1] = lsum;
-            }
-            epi_bar();
-            int y = A - 1;
-            if (wv) {
-                float pm[NS], ps[NS];
-                float M = 0.f;
-#pragma unroll
-                for (int i = 0; i < NS; i++) { pm[i] = s_pair[(u * NS + i) * 2]; ps[i] = s_pair[(u * NS + i) * 2 + 1]; M = fmaxf(M, pm[i]); }
-                float total = 0.f, off = 0.f, fme = 1.f, mine_hi = 0.f;
-#pragma unroll
-                for (int i = 0; i < NS; i++) {
-                    const float f = wn::exp2f_fast((pm[i] - M) * 1.4426950408889634f);
-                    if (i == sub) { off = total; fme = f; }
-                    total += ps[i] * f;
-                    if (i == sub) mine_hi = total;
-                }
-                const float target = sel * total;
-                // owner = first part whose scaled running sum exceeds the target; the last part takes what is left
-                const bool mine = (sub == 0 || !(target < off)) && (target < mine_hi || sub == NS - 1);
-                if (mine) {
-                    int cb = NCH - 1;
-                    float base = off;
-                    {
-                        float run = off;
-                        bool found = false;
-#pragma unroll
-                        for (int c = 0; c < NCH; c++) {
-                            const float nxt = run + csum[c] * fme;
-                            if (!found && target < nxt) { cb = c; base = run; found = true; }
-                            run = nxt;
-                        }
-                        if (!found) base = run - csum[NCH - 1] * fme;
-                    }
-                    const int c0 = a_lo + 16 * cb;
-                    const unsigned char* kt = t_big + (size_t)(c0 >> 6) * TILE;
-                    const int q = (c0 & 63) >> 3;
-                    const uint4 u0 = *reinterpret_cast<const uint4*>(kt + chunk_off(row, q)), u1 = *reinterpret_cast<const uint4*>(kt + chunk_off(row, q + 1));
-                    const uint32_t w[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
-                    float run = base;
-                    bool found = false;
-                    int yy = (cb == NCH - 1 && sub == NS - 1) ? A - 1 : c0 + 15;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        float e0, e1;
-                        expz(w[j], e0, e1);
-                        run += e0 * fme;
-                        if (!found && target < run) { yy = c0 + 2 * j; found = true; }
-                        run += e1 * fme;
-                        if (!found && target < run) { yy = c0 + 2 * j + 1; found = true; }
-                    }
-                    s_y[u] = yy;
-                    if (valid) p.yOut[(size_t)b * p.N + t] = yy;
-                }
-                if (dump && valid) {
-                    const float inv = fme / total;
-                    for (int a = a_lo; a < a_lo + PART; a++) {
-                        const unsigned char* kt = t_big + (size_t)(a >> 6) * TILE;
-                        const float z = __half2float(*reinterpret_cast<const __half*>(kt + chunk_off(row, (a & 63) >> 3) + (a & 7) * 2));
-                        p.P[(size_t)b * A + a] = wn::exp2f_fast(z * 1.4426950408889634f) * inv;
-                    }
-                }
-            }
-            epi_bar();
-            if (wv) y = s_y[u];
-            if (valid) {
-                const int fb = p.forced ? p.forced[(size_t)b * p.N + t] : y;
-                yp = yc;
-                yc = fb;
-            }
-            if (tid == tr_tid) TRACE(0, 11);
-            // Dza is consumed: the x_0-ready arrival of the next sample (or kernel end) releases it
+            d <<= 1; if (d > p.maxDil) d = 1;
         }
-        if (valid && sub == 0) { p.yPrev[b] = yp; p.yCur[b] = yc; }
-        tc_fence_before_sync();
-    }
-#undef TRACE
+        if (FUSED) {                                                    // Wres_{L-1}, Wskip_{L-1} on h_{L-1}
+            int sr, sk[SKC];
+            wgmma_fence();
+            issue_res_skip(L - 1, t_hb + (size_t)((L - 1) & 1) * ATILE, sr, sk);
+            wgmma_commit();
+            wgmma_wait<0>();
+            release_res_skip(sr, sk);
+            residual(L - 1);
+        }
 
-    __syncthreads();
-    if (warp == 8) tmem_dealloc<512>(tmem_base);
+        // ---------------- relu(skip) -> A operand of the first output layer   (reference.cpp:88-90)
+#pragma unroll
+        for (int j = 0; j < SKN / 8; j++)
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                float v[2];
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int s = SKN * wg + 8 * j + cq + e;
+                    v[e] = valid[r] ? fmaxf(acc_s[4 * j + 2 * r + e] + gbias[im.b_bskp + (size_t)(L - 1) * S + s], 0.f) : 0.f;
+                    if (dump && valid[r]) p.skipOut[((size_t)(L - 1) * B + bb[r]) * S + s] = v[e];
+                }
+                const int s = SKN * wg + 8 * j + cq;
+                st_pair(t_big + (size_t)(s >> 6) * ATILE, r0 + 8 * r, s & 63, v[0], v[1]);
+            }
+        fence_proxy_async_smem();
+        consumer_sync();
+
+        // ---------------- output layers: warpgroup w computes columns [128 w, 128 w + 128) of Zs, then of Za
+        float acc_z[64];
+        auto out_gemm = [&](int KT) {
+            for (int kt = 0; kt < KT; kt++) {
+                int s0, s1;
+                const unsigned char* w0 = take(s0);
+                const unsigned char* w1 = take(s1);
+                const uint64_t da = desc(t_big + (size_t)kt * ATILE), dw = desc(wg ? w1 : w0);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; k++) wgmma_f16<128>(acc_z, da + 2 * k, dw + 2 * k, kt > 0 || k > 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                release(s0); release(s1);
+            }
+        };
+        out_gemm(S / 64);
+        consumer_sync();                                                // both warpgroups are done reading relu(skip)
+        // Zs = relu(Wzs . skip + Bzs)   (reference.cpp:96-98)
+#pragma unroll
+        for (int j = 0; j < 16; j++)
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                float v[2];
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int a = 128 * wg + 8 * j + cq + e;
+                    v[e] = valid[r] ? fmaxf(acc_z[4 * j + 2 * r + e] + gbias[im.b_bzs + a], 0.f) : 0.f;
+                    if (dump && valid[r]) p.Zs[(size_t)bb[r] * A + a] = v[e];
+                }
+                const int a = 128 * wg + 8 * j + cq;
+                st_pair(t_big + (size_t)(a >> 6) * ATILE, r0 + 8 * r, a & 63, v[0], v[1]);
+            }
+        fence_proxy_async_smem();
+        consumer_sync();
+        out_gemm(A / 64);
+        // Za = Wza . Zs + Bza   (reference.cpp:100-104) -> shared memory, one fp32 row per utterance
+#pragma unroll
+        for (int j = 0; j < 16; j++)
+#pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int r = e >> 1, a = 128 * wg + 8 * j + cq + (e & 1);
+                const float z = acc_z[4 * j + e] + gbias[im.b_bza + a];
+                s_z[(r0 + 8 * r) * A + a] = z;
+                if (dump && valid[r]) p.Za[(size_t)bb[r] * A + a] = z;
+            }
+        consumer_sync();
+
+        // ---------------- softmax + categorical sample   (reference.cpp:106-121)
+        // Four consecutive threads per utterance, 64 logits each; the parts meet through warp shuffles.
+        {
+            const int row = tid >> 2, part = tid & 3, lane = tid & 31;
+            const int b = tile * tu + row0 + row;
+            const bool v = row < live && b < B;
+            float* zr = s_z + row * A + 64 * part;
+            float mx = zr[0];
+            for (int a = 1; a < 64; a++) mx = fmaxf(mx, zr[a]);
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            float ps = 0.f;
+            for (int a = 0; a < 64; a++) {
+                const float ev = wn::exp2f_fast((zr[a] - mx) * 1.4426950408889634f);
+                zr[a] = ev;
+                ps += ev;
+            }
+            float pp[4];
+#pragma unroll
+            for (int k = 0; k < 4; k++) pp[k] = __shfl_sync(0xffffffffu, ps, (lane & ~3) + k);
+            float off = 0.f, total = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; k++) { if (k == part) off = total; total += pp[k]; }
+            const float target = (v ? __ldg(p.sel + (size_t)t * B + b) : 0.5f) * total;
+            // owner = the part whose running-sum interval holds the target; the first and last parts take what is outside
+            const bool mine = (part == 0 || !(target < off)) && (target < off + ps || part == 3);
+            if (mine) {
+                int yy = part == 3 ? A - 1 : 64 * part + 63;
+                float run = off;
+                for (int a = 0; a < 64; a++) {
+                    run += zr[a];
+                    if (target < run) { yy = 64 * part + a; break; }
+                }
+                s_y[row] = yy;
+                if (v) p.yOut[(size_t)b * p.N + t] = yy;
+            }
+            if (dump && v) {
+                const float inv = 1.f / total;
+                for (int a = 0; a < 64; a++) p.P[(size_t)b * A + 64 * part + a] = zr[a] * inv;
+            }
+        }
+        consumer_sync();
+#pragma unroll
+        for (int r = 0; r < 2; r++)
+            if (valid[r]) {
+                const int y = s_y[r0 + 8 * r];
+                yp[r] = yc[r];
+                yc[r] = p.forced ? p.forced[(size_t)bb[r] * p.N + t] : y;
+            }
+    }
+    if (wg == 0 && (i & 3) == 0) {
+#pragma unroll
+        for (int r = 0; r < 2; r++)
+            if (valid[r]) { p.yPrev[bb[r]] = yp[r]; p.yCur[bb[r]] = yc[r]; }
+    }
 }
 
-int pick_nstage(int S, int L)
+int pick_nstage()
 {
-    for (int n = 8; n >= 3; n--)
-        if (tc_smem_bytes(S, L, n) <= 227 * 1024) return n;
+    for (int n = 8; n >= 5; n--)                                // the fused schedule holds up to five stages at once
+        if (tc_smem_bytes(n) <= 227 * 1024) return n;
     return 0;
 }
 
 }  // namespace
 
-bool wn_tc_supported(int R_, int S, int A_, int L, int)
+bool wn_tc_supported(int R_, int S, int A_, int, int)
 {
-    return R_ == R && A_ == A && (S == 128 || S == 256) && pick_nstage(S, L) >= 3;
+    return R_ == R && A_ == A && (S == 128 || S == 256);
 }
 
 size_t wn_tc_image_bytes(int, int S, int, int L) { return tc_image(S, L).total; }
 
-// 64-utterance tiles (the lower-latency four-threads-per-utterance variant) as long as one wave of CTAs covers the batch
-// Utterances per CTA tile: 32 (eight threads per utterance) while that keeps the launch small enough to stay latency-bound,
-// 64 as long as one wave of CTAs covers the batch, else full 128-row tiles.  NVWN_TC_TILE / NVWN_TC_NODUP force a shape.
-int wn_tc_tile_utt(int B, int S)
+// Utterances per tile (the conditioning store and the history ring are laid out per tile, so an engine resolves it once):
+// 64 unless NVWN_TC_TILE (32 | 64 | 128) or NVWN_TC_NODUP (128) asks for another shape.
+int wn_tc_tile_utt(int, int)
 {
     if (getenv("NVWN_TC_NODUP")) return 128;
-    if (const char* v = getenv("NVWN_TC_TILE")) { const int t = atoi(v); if (t == 128 || t == 64 || (t == 32 && S == 256)) return t; }
-    // Round 2: the soak test (tests/test_gpu_parity.py::test_fp16_soak_determinism_and_chunking, tools/diag_determinism.py) shows
-    // rare run-to-run flips of a sampled index (about one per 1e5 utterance-samples) with the FUSED schedule (32- / 64-utterance
-    // tiles) and with the 128-row tiles; the unfused schedule on 64-utterance tiles is clean over the same soak.  Those variants
-    // stay reachable through NVWN_TC_TILE / NVWN_TC_NODUP / NVWN_TC_FUSED for investigation but are never selected automatically
-    // (the latency-mode kernel, wn_lat_kernel.cu, serves the batches they were meant for).
-    return 64;
+    if (const char* v = getenv("NVWN_TC_TILE")) { const int t = atoi(v); if (t == 128 || t == 64 || t == 32) return t; }
+    return TU;
 }
 
-// schedule of an engine, resolved once at creation: "0" / "1" in NVWN_TC_FUSED force one (tests); see wn_tc_tile_utt() for the default
+// schedule of an engine, resolved once at creation: "0" / "1" in NVWN_TC_FUSED force one; unfused by default
 bool wn_tc_fused_default()
 {
     const char* fv = getenv("NVWN_TC_FUSED");
     return fv ? fv[0] != '0' : false;
 }
 
-size_t wn_tc_ring_bytes(int TU, int L, int maxDil, int B)
+size_t wn_tc_ring_bytes(int TU_, int L, int maxDil, int B)
 {
-    return (size_t)(maxDil + 1) * L * ((B + TU - 1) / TU) * TILE;
+    return (size_t)(maxDil + 1) * L * ((B + TU_ - 1) / TU_) * TILE;
 }
 
-size_t wn_tc_cond_bytes(int TU, int L, int B, int N) { return (size_t)N * L * cond_bpad(B, TU) * 256; }
+size_t wn_tc_cond_bytes(int TU_, int L, int B, int N) { return (size_t)N * L * cond_bpad(B, TU_) * 256; }
 
-cudaError_t wn_tc_cond_convert(void* dst, const float* src_dev, int first_sample, int nsamples, int TU, int L, int B, cudaStream_t stream)
+cudaError_t wn_tc_cond_convert(void* dst, const float* src_dev, int first_sample, int nsamples, int TU_, int L, int B, cudaStream_t stream)
 {
     if (nsamples <= 0) return cudaSuccess;
     const size_t total = (size_t)nsamples * L * B * 16;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
-    tc_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, L, B, TU);
+    if (blocks > 4096) blocks = 4096;
+    tc_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, L, B, TU_);
     return cudaGetLastError();
 }
 
-cudaError_t wn_tc_cond_readback(float* dst_dev, const void* store, int first_sample, int nsamples, int TU, int L, int B, cudaStream_t stream)
+cudaError_t wn_tc_cond_readback(float* dst_dev, const void* store, int first_sample, int nsamples, int TU_, int L, int B, cudaStream_t stream)
 {
     if (nsamples <= 0) return cudaSuccess;
     const size_t total = (size_t)nsamples * L * B * 16;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
-    tc_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, L, B, TU);
+    if (blocks > 4096) blocks = 4096;
+    tc_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, L, B, TU_);
     return cudaGetLastError();
 }
 
@@ -1276,38 +713,27 @@ cudaError_t wn_tc_pack(void* image, const WnParams& p, cudaStream_t stream)
     const TcImage im = tc_image(p.S, p.L);
     cudaError_t e = cudaMemsetAsync(image, 0, im.total, stream);
     if (e != cudaSuccess) return e;
-    tc_pack_kernel<<<296, 256, 0, stream>>>(p, static_cast<unsigned char*>(image), im);
+    tc_pack_kernel<<<264, 256, 0, stream>>>(p, static_cast<unsigned char*>(image), im);
     return cudaGetLastError();
 }
 
-cudaError_t wn_launch_tc(const WnParams& p, const void* tc_image_, int TU, bool fused, cudaStream_t stream, WnLaunchInfo* info)
+cudaError_t wn_launch_tc(const WnParams& p, const void* tc_image_, int tu, bool fused, cudaStream_t stream, WnLaunchInfo* info)
 {
-    const int nstage = pick_nstage(p.S, p.L);
-    if (nstage < 3) return cudaErrorInvalidValue;
-    const size_t smem = tc_smem_bytes(p.S, p.L, nstage);
-    const int grid = (p.B + TU - 1) / TU;
-    cudaError_t e = cudaErrorInvalidValue;
-    const int cp = 128 / TU;                                    // row copies per utterance: 2 cp threads work for each
+    const int nstage = pick_nstage();
+    if (nstage < 5 || (tu != 32 && tu != 64 && tu != 128)) return cudaErrorInvalidValue;
+    const size_t smem = tc_smem_bytes(nstage);
+    const int grid = (p.B + tu - 1) / tu * (tu > TU ? tu / TU : 1);
     const unsigned char* im8 = static_cast<const unsigned char*>(tc_image_);
-    // Fused schedule (one MMA<->epilogue round trip per layer, +1 weight chunk per layer) while the launch is latency-bound;
-    // with (nearly) every SM streaming the weights from L2 the extra chunk costs more than the round trip saves
-    // (measured, 64-utterance tiles: 2048 utt. 50.9M vs 44.5M samples/s fused; 9472 utt. 175.6M fused vs 196.4M unfused).
-#define WN_TC_LAUNCH(SV, DV, FV)                                                                                     \
-    do {                                                                                                             \
-        e = cudaFuncSetAttribute(wn_tc_kernel<SV, DV, FV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
-        if (e != cudaSuccess) return e;                                                                              \
-        wn_tc_kernel<SV, DV, FV><<<grid, NT, smem, stream>>>(p, im8, nstage);                                       \
+    cudaError_t e = cudaErrorInvalidValue;
+#define WN_TC_LAUNCH(SV, FV)                                                                                     \
+    do {                                                                                                         \
+        e = cudaFuncSetAttribute(wn_tc_kernel<SV, FV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
+        if (e != cudaSuccess) return e;                                                                          \
+        wn_tc_kernel<SV, FV><<<grid, NT, smem, stream>>>(p, im8, nstage, tu);                                   \
     } while (0)
-#define WN_TC_LAUNCH2(SV, DV) do { if (fused) WN_TC_LAUNCH(SV, DV, true); else WN_TC_LAUNCH(SV, DV, false); } while (0)
-    if (p.S == 256) {
-        if (cp == 4) WN_TC_LAUNCH(256, 4, true);                // 32-utterance tiles exist for the fused schedule only (NVWN_TC_TILE=32)
-        else if (cp == 2) WN_TC_LAUNCH2(256, 2);
-        else WN_TC_LAUNCH2(256, 1);
-    } else {
-        if (cp == 2) WN_TC_LAUNCH2(128, 2); else WN_TC_LAUNCH2(128, 1);
-    }
-#undef WN_TC_LAUNCH2
+    if (p.S == 256) { if (fused) WN_TC_LAUNCH(256, true); else WN_TC_LAUNCH(256, false); }
+    else { if (fused) WN_TC_LAUNCH(128, true); else WN_TC_LAUNCH(128, false); }
 #undef WN_TC_LAUNCH
-    if (info) { info->kernel = 17; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = 1; }
+    if (info) { info->kernel = 17; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = tu < TU ? tu : TU; info->cluster = 1; }
     return cudaGetLastError();
 }

@@ -1,14 +1,14 @@
-// wn_tc_selftest.cu -- minimal tcgen05 GEMM used by tests/test_gpu_tc_primitives.py to pin the operand layouts,
+// wn_tc_selftest.cu -- minimal wgmma GEMM used by tests/test_gpu_tc_primitives.py to pin the operand layouts,
 // descriptors and synchronisation idioms the tensor-core WaveNet kernel is built from:
-//     D[128 x N] (fp32, TMEM) = A[128 x K] (fp16, written row-per-thread into K-major SWIZZLE_128B tiles)
-//                             x B[N x K]^T (fp16, pre-tiled image brought in by 1-D bulk TMA)
-// Same warp roles as the real kernel: warps 0-3 write A / read D, warp 4 lane 0 = TMA producer, warp 5 lane 0 = MMA issuer.
+//     D[128 x N] (fp32, registers) = A[128 x K] (fp16, written row-per-thread into K-major SWIZZLE_128B tiles)
+//                                  x B[N x K]^T (fp16, pre-tiled image brought in by 1-D bulk TMA)
+// Two warpgroups, one per 64-row half of A, as in the real kernel; thread 0 issues the TMA.
 #include "wn_common.h"
-#include "wn_sm100.cuh"
+#include "wn_sm90.cuh"
 
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
 constexpr int TILE_BYTES = 128 * 128;      // [128 rows x 64 fp16] K-major SW128
 
@@ -26,38 +26,54 @@ __global__ void pack_b_kernel(const __half* __restrict__ B, int N, int K, unsign
     }
 }
 
-__global__ void __launch_bounds__(192, 1) umma_selftest_kernel(const __half* __restrict__ A, const unsigned char* __restrict__ Bimg,
-                                                               int N, int K, float* __restrict__ D, int mode)
+// D columns [col0, col0 + NW) of this warpgroup's 64 rows = A . (NW rows of B starting at chunk c0 of every K tile)^T
+template <int NW>
+__device__ __forceinline__ void gemm_rows(const unsigned char* a_tiles, const unsigned char* b_tiles, int KT, int chunks_n, int c0,
+                                          int wg, float* __restrict__ D, int N, int col0)
+{
+    float acc[NW / 2];
+    wgmma_fence();
+    for (int kt = 0; kt < KT; kt++) {
+        const uint64_t da = make_desc_sw128(smem_u32(a_tiles + (size_t)kt * TILE_BYTES + (size_t)wg * 64 * 128));
+        const uint64_t db = make_desc_sw128(smem_u32(b_tiles + (size_t)(kt * chunks_n + c0) * TILE_BYTES));
+#pragma unroll
+        for (int k = 0; k < 4; k++) wgmma_f16<NW>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kt | k) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    const int i = threadIdx.x & 127;
+    const int r0 = wg * 64 + 16 * (i >> 5) + ((i & 31) >> 2), cq = 2 * (i & 3);
+#pragma unroll
+    for (int j = 0; j < NW / 8; j++)
+#pragma unroll
+        for (int e = 0; e < 4; e++) D[(size_t)(r0 + 8 * (e >> 1)) * N + col0 + 8 * j + cq + (e & 1)] = acc[4 * j + e];
+}
+
+__global__ void __launch_bounds__(256, 1) wgmma_selftest_kernel(const __half* __restrict__ A, const unsigned char* __restrict__ Bimg,
+                                                                int N, int K, float* __restrict__ D, int mode)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // 1024-byte alignment by OFFSET (not by pointer round-trip through an integer): the compiler keeps knowing these
-    // are shared-memory addresses and emits LDS/STS instead of generic LD/ST
     unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int KT = K / 64;
     const int rows_per_chunk = N < 128 ? N : 128;
     const int chunks_n = N / rows_per_chunk;
     unsigned char* a_tiles = smem;                               // KT tiles
     unsigned char* b_tiles = smem + (size_t)KT * TILE_BYTES;     // KT * chunks_n tiles
-    uint64_t* bars = reinterpret_cast<uint64_t*>(b_tiles + (size_t)KT * chunks_n * TILE_BYTES);
-    uint64_t* b_full = bars;          // TMA landed
-    uint64_t* a_ready = bars + 1;     // 128 epilogue threads wrote A
-    uint64_t* mma_done = bars + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(b_tiles + (size_t)KT * chunks_n * TILE_BYTES);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wg = tid >> 7;
     if (tid == 0) {
         mbar_init(b_full, 1);
-        mbar_init(a_ready, 128);
-        mbar_init(mma_done, 1);
         fence_mbar_init();
     }
-    if (warp == 4) tmem_alloc<512>(tmem_slot);
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp < 4) {
+    if (tid == 0) {
+        const uint32_t bytes = (uint32_t)(KT * chunks_n) * (uint32_t)(rows_per_chunk * 128);
+        mbar_arrive_expect_tx(b_full, bytes);
+        for (int c = 0; c < KT * chunks_n; c++)
+            tma_load_1d(b_tiles + (size_t)c * TILE_BYTES, Bimg + (size_t)c * TILE_BYTES, rows_per_chunk * 128, b_full);
+    }
+    if (tid < 128) {
         // each thread writes its own row of A into every K tile (8 x 16-byte chunks per tile), as the kernel's epilogue does
         const int row = tid;
         for (int kt = 0; kt < KT; kt++) {
@@ -67,50 +83,21 @@ __global__ void __launch_bounds__(192, 1) umma_selftest_kernel(const __half* __r
                 *reinterpret_cast<uint4*>(a_tiles + (size_t)kt * TILE_BYTES + row * 128 + ((j ^ (row & 7)) << 4)) = v;
             }
         }
-        fence_proxy_async();
-        mbar_arrive(a_ready);
-        // wait for the accumulator, read it back
-        mbar_wait(mma_done, 0);
-        tc_fence_after_sync();
-        for (int c0 = 0; c0 < N; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + c0, r);
-            tmem_ld_wait();
-            for (int j = 0; j < 32; j++) D[(size_t)row * N + c0 + j] = __uint_as_float(r[j]);
-        }
-        tc_fence_before_sync();
-    } else if (warp == 4 && lane == 0) {
-        const uint32_t bytes = (uint32_t)(KT * chunks_n) * (uint32_t)(rows_per_chunk * 128);
-        mbar_arrive_expect_tx(b_full, bytes);
-        for (int c = 0; c < KT * chunks_n; c++)
-            tma_load_1d(b_tiles + (size_t)c * TILE_BYTES, Bimg + (size_t)c * TILE_BYTES, rows_per_chunk * 128, b_full);
-    } else if (warp == 5 && lane == 0) {
-        mbar_wait(b_full, 0);
-        mbar_wait(a_ready, 0);
-        tc_fence_after_sync();
-        if (mode == 0) {
-            // one MMA per (K=16 slice, 128-row chunk of B): D columns [nc*128, ...)
-            const uint32_t idesc = make_idesc_f16(128, rows_per_chunk);
-            for (int kt = 0; kt < KT; kt++)
-                for (int nc = 0; nc < chunks_n; nc++) {
-                    const uint64_t da = make_desc_kmajor_sw128(smem_u32(a_tiles + (size_t)kt * TILE_BYTES));
-                    const uint64_t db = make_desc_kmajor_sw128(smem_u32(b_tiles + (size_t)(kt * chunks_n + nc) * TILE_BYTES));
-                    for (int k = 0; k < 4; k++)
-                        umma_f16(tmem_base + nc * 128, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kt | k) ? 1u : 0u);
-                }
-        } else {
-            // N = 256 as ONE instruction per K slice: the two 128-row chunks of a K tile are contiguous (SBO walks across)
-            const uint32_t idesc = make_idesc_f16(128, N);
-            for (int kt = 0; kt < KT; kt++) {
-                const uint64_t da = make_desc_kmajor_sw128(smem_u32(a_tiles + (size_t)kt * TILE_BYTES));
-                const uint64_t db = make_desc_kmajor_sw128(smem_u32(b_tiles + (size_t)(kt * chunks_n) * TILE_BYTES));
-                for (int k = 0; k < 4; k++) umma_f16(tmem_base, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kt | k) ? 1u : 0u);
-            }
-        }
-        umma_commit(mma_done);
     }
+    fence_proxy_async_smem();
     __syncthreads();
-    if (warp == 4) tmem_dealloc<512>(tmem_base);
+    mbar_wait(b_full, 0);
+    if (mode == 0) {
+        // one instruction per 128-row chunk of B (or the whole of a smaller B): D columns [nc * 128, ...)
+        for (int nc = 0; nc < chunks_n; nc++) {
+            if (rows_per_chunk == 64) gemm_rows<64>(a_tiles, b_tiles, KT, chunks_n, nc, wg, D, N, nc * 128);
+            else gemm_rows<128>(a_tiles, b_tiles, KT, chunks_n, nc, wg, D, N, nc * 128);
+        }
+    } else {
+        // N = 256 as ONE instruction per K slice: the two 128-row chunks of a K tile are contiguous (SBO walks across)
+        if (N == 256) gemm_rows<256>(a_tiles, b_tiles, KT, chunks_n, 0, wg, D, N, 0);
+        else gemm_rows<128>(a_tiles, b_tiles, KT, chunks_n, 0, wg, D, N, 0);
+    }
 }
 
 }  // namespace
@@ -119,7 +106,7 @@ __global__ void __launch_bounds__(192, 1) umma_selftest_kernel(const __half* __r
 // N in {64, 128, 256}.  mode 0: N<=128-wide instructions per 128-row chunk; mode 1: one N-wide instruction.
 extern "C" int nvwn_selftest_umma(const void* A, const void* B, int N, int K, float* D, int mode)
 {
-    if (K % 64 || (N != 64 && N != 128 && N != 256) || K > 256) return -1;
+    if (K % 64 || (N != 64 && N != 128 && N != 256) || K > 256 || (mode != 0 && N == 64)) return -1;
     __half *dA = nullptr, *dB = nullptr;
     unsigned char* img = nullptr;
     float* dD = nullptr;
@@ -133,8 +120,8 @@ extern "C" int nvwn_selftest_umma(const void* A, const void* B, int N, int K, fl
     ST(cudaMemcpy(dB, B, (size_t)N * K * 2, cudaMemcpyHostToDevice));
     pack_b_kernel<<<64, 256>>>(dB, N, K, img);
     const size_t smem = 1024 + (size_t)(K / 64) * TILE_BYTES + (size_t)chunks * TILE_BYTES + 64;
-    ST(cudaFuncSetAttribute(umma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    umma_selftest_kernel<<<1, 192, smem>>>(dA, img, N, K, dD, mode);
+    ST(cudaFuncSetAttribute(wgmma_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    wgmma_selftest_kernel<<<1, 256, smem>>>(dA, img, N, K, dD, mode);
     ST(cudaGetLastError());
     ST(cudaDeviceSynchronize());
     ST(cudaMemcpy(D, dD, 128 * N * 4, cudaMemcpyDeviceToHost));

@@ -12,7 +12,7 @@ import numpy as np
 from . import _lib
 from ._lib import FP16, FP32, FP32_FAST, KERNEL_AUTO, KERNEL_STREAM, KERNEL_TENSORCORE, check  # noqa: F401
 
-# Implementation enum of the reference (nv_wavenet.cuh:223-229); accepted, all map to the sm_100a kernels
+# Implementation enum of the reference (nv_wavenet.cuh:223-229); accepted, all map to the sm_90a kernels
 AUTO, SINGLE_BLOCK, DUAL_BLOCK, PERSISTENT, MANYBLOCK_NONPERSISTENT = 0, 1, 2, 3, 4
 
 

@@ -1,13 +1,13 @@
-"""Numerical contract of the fused tensor-core schedule, explored on the CPU.
+"""Numerical contract of a fused tensor-core layer schedule, explored on the CPU.
 
-The fused schedule (csrc/wn_tc_kernel.cu) does not evaluate the layer the way the reference writes it
+A fused schedule (one MMA <-> epilogue round trip per layer) does not evaluate the layer the way the reference writes it
 (nv_wavenet_reference.cpp:59-86): it folds Wf_l = Wcur_l . Wres_{l-1} (one fp16 matrix) and
 Bh'_l = Bh_l + Wcur_l . Bres_{l-1}, accumulates a_l = (Lh + Bh') + Wprev.x_l[t-d] + Wcur.x_{l-1} + Wf.h_{l-1}, and
 evaluates tanh / sigmoid on fp16 values.  This test restates that arithmetic in numpy (fp16 roundings where the kernel
 has them, fp32 accumulation), teacher-forced on the fp32 oracle's trajectory, and checks over several seeds and shapes
 that its logits stay within the north-star tolerance (1e-2 relative, same criterion as tests/test_gpu_parity.py) of the
 fp32 oracle -- i.e. that the algebraic fold costs no accuracy class.  The unfused fp16 contract is run alongside as
-a yardstick.  (The kernel itself is compared with the oracle on the GPU; this covers more seeds than the GPU budget.)"""
+a yardstick."""
 import numpy as np
 import pytest
 

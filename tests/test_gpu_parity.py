@@ -211,17 +211,17 @@ def _select_fp16_kernel(kernel, monkeypatch):
         monkeypatch.delenv(k, raising=False)
     if kernel == "stream":
         monkeypatch.setenv("NVWN_FP16_KERNEL", "stream")
-    elif kernel == "lat":                          # latency-mode kernel (mma.sync, 16-utterance tiles, a three-CTA cluster per tile while all clusters are resident, 720 utterances): AUTO up to 2368 utterances
+    elif kernel == "lat":                          # latency-mode kernel (mma.sync, 16-utterance tiles, a three-CTA cluster per tile while all clusters are resident): AUTO
         monkeypatch.setenv("NVWN_FP16_KERNEL", "lat")
-    elif kernel == "lat_single":                   # ... one CTA per tile: what AUTO uses from 1185 to 2368 utterances
+    elif kernel == "lat_single":                   # ... one CTA per tile: what AUTO uses once the clusters no longer fit one wave
         monkeypatch.setenv("NVWN_FP16_KERNEL", "lat"); monkeypatch.setenv("NVWN_LAT_CLUSTER", "0")
-    else:                                          # tensor-core (tcgen05) kernel; "tc" = the auto-selected 64-utterance tiles, unfused schedule
+    else:                                          # tensor-core (wgmma) kernel; "tc" = the default 64-utterance tiles, unfused schedule
         monkeypatch.setenv("NVWN_FP16_KERNEL", "tc")
-        if kernel == "tc_nodup":                   # 128-utterance tiles, two threads per utterance (debug variant, see wn_tc_tile_utt)
+        if kernel == "tc_nodup":                   # 128-utterance tiles, two CTAs per tile (see wn_tc_tile_utt)
             monkeypatch.setenv("NVWN_TC_NODUP", "1")
-        if kernel == "tc_tile32_fused":            # 32-utterance tiles exist for the fused schedule only (debug variant)
+        if kernel == "tc_tile32_fused":            # 32-utterance tiles run the fused schedule
             monkeypatch.setenv("NVWN_TC_TILE", "32")
-        if kernel == "tc_tile64_fused":            # fused schedule on 64-utterance tiles (debug variant)
+        if kernel == "tc_tile64_fused":            # fused schedule on 64-utterance tiles
             monkeypatch.setenv("NVWN_TC_TILE", "64"); monkeypatch.setenv("NVWN_TC_FUSED", "1")
 
 
@@ -247,8 +247,6 @@ def _check_sampled_index(p, sel, y):
 ])
 def test_fp16_logits_teacher_forced(shape, kernel, monkeypatch):
     R, S, A, L, B, N, md = shape
-    if kernel in ("stream", "tc_tile64_fused") and B > 64:
-        pytest.skip("covered by the smaller shapes")
     _select_fp16_kernel(kernel, monkeypatch)
     w = refgen.lively_inputs(21 + B, R, S, A, L, B, N)
     o32 = cpu_oracle(w, L, B, N, R, S, A, md)
@@ -314,7 +312,7 @@ def _run_range(e, init, count, N, B, y=None):
     e._samples_per_chunk = 0
 
 
-@pytest.mark.parametrize("kernel", ["lat", "lat_single", "tc"])      # "tc" = what AUTO selects above the latency kernels' range: 64-utterance tiles, unfused schedule
+@pytest.mark.parametrize("kernel", ["lat", "lat_single", "tc"])      # "tc" = the tensor-core kernel's default: 64-utterance tiles, unfused schedule
 def test_fp16_soak_determinism_and_chunking(kernel, monkeypatch):
     """The fp16 kernels at the C3 shape (L20 R64 S256 A256, maxDil 512, 64 utterances) over 2000 samples -- several turns of the
     513-slot history ring and of the dilation cycle: run twice -> identical yOut; run_chunks(97) and three unequal

@@ -1,6 +1,6 @@
-"""Pins the tcgen05 building blocks of the tensor-core kernel on real hardware: K-major SWIZZLE_128B operand
-tiles written row-per-thread, pre-tiled weight images moved by 1-D bulk TMA, shared-memory / instruction
-descriptors, K-slice advance, accumulate flag, commit->mbarrier, TMEM load.  Checked against numpy."""
+"""Pins the wgmma building blocks of the tensor-core kernel on real hardware: K-major SWIZZLE_128B operand
+tiles written row-per-thread, pre-tiled weight images moved by 1-D bulk TMA, shared-memory descriptors,
+K-slice and row-block advance, accumulate flag, the accumulator fragment layout.  Checked against numpy."""
 import ctypes as C
 
 import numpy as np

@@ -1,6 +1,7 @@
-"""The synchronisation protocol of the fused tensor-core kernel, checked on the CPU by a discrete-event model
-(tools/tc_protocol_model.py): random latencies, stressed roles, every layer / dilation / dump / buffering variant.
-The three defects that the hardware runs of round 1 actually hit are re-introduced to show the model sees them."""
+"""The synchronisation protocol of a warp-specialised fused tensor-core schedule, checked on the CPU by a discrete-event
+model (tools/tc_protocol_model.py): random latencies, stressed roles, every layer / dilation / dump / buffering variant.
+Three protocol defects (a single conditioning buffer, a commit with nothing outstanding, phase aliasing) are
+re-introduced to show the model sees them."""
 import random
 
 import pytest

@@ -1,5 +1,5 @@
 """GPU baseline: the reference's own kernels (oracle/_ref/ref_gpu_harness, unmodified nv_wavenet.cuh rebuilt for
-sm_100a) timed exactly like nv_wavenet_perf.cu:67-87 (run_chunks incl. chunked D2H), next to our kernels, same inputs."""
+sm_90a) timed exactly like nv_wavenet_perf.cu:67-87 (run_chunks incl. chunked D2H), next to our kernels, same inputs."""
 import json
 import sys
 

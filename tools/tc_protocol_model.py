@@ -1,17 +1,17 @@
-"""Discrete-event model of the synchronisation protocol of the fused tensor-core kernel (csrc/wn_tc_kernel.cu,
-`FUSED` schedule): producer warp, issuer roles A / B, history-copy role C and the eight epilogue warps exchange
-mbarrier phases, weight-ring stages and tcgen05 commits exactly in the order the kernel does, with randomised
-latencies.  It checks what cannot be seen in a passing GPU run:
+"""Discrete-event model of a warp-specialised fused tensor-core layer schedule for single-thread-issued MMAs whose
+completion is committed to mbarriers (the tcgen05 model of issue; csrc/wn_tc_kernel.cu issues wgmma from its consumer
+warpgroups instead and does not use this schedule): producer warp, issuer roles A / B, history-copy role C and the
+eight epilogue warps exchange mbarrier phases, weight-ring stages and MMA commits, with randomised latencies.  It checks what cannot be seen in a passing GPU run:
 
   * deadlock: every role must finish every sample;
   * phase aliasing: an mbarrier waiter may never be two completed phases behind (parity waits would then block
     for ever or pass early) -- the model tracks, per waiter, WHICH completion it is waiting for;
-  * late commits: a tcgen05.commit issued when its thread has no MMA in flight never arrives on sm_100a (measured);
+  * late commits: a commit issued when its thread has no MMA in flight never arrives;
   * ring order: every role consumes the chunk the producer put into that stage;
   * the data hazards the handshakes exist for (h / x tiles, accumulators, conditioning buffers).
 
 Pure Python, no GPU.  `python tools/tc_protocol_model.py [runs]` runs random trials; tests/test_tc_protocol_model.py
-runs a bounded number of them.  The model follows the kernel source; keep them in step when the kernel changes.
+runs a bounded number of them.
 """
 import heapq
 import random
@@ -168,7 +168,7 @@ def _once(fn):
     yield
 
 
-# ---------------------------------------------------------------------- the roles, transcribed from the kernel
+# ---------------------------------------------------------------------- the roles
 def build(sim):
     L, SKC, nstage, NC = sim.L, sim.SKC, sim.nstage, sim.NC
     dil = sim.dil
