@@ -1068,6 +1068,9 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
 #pragma unroll
                         for (int i = 0; i < 4; i++) { accp[0][i] += u0[i]; accp[1][i] += u1[i]; }
                     }
+                    // the res GEMM's B fragments (same ring piece), read while the shared-memory pipe is idle under the HMMAs and the
+                    // gate, so that only the h tile is read between the barrier below and the res HMMAs
+                    const uint4 bw0 = lds128(p1 + o_res), bw1 = lds128(p1 + o_res + 512);
                     {
                         const __half2 half = __floats2half2_rn(0.5f, 0.5f);
                         const __half2 tg0 = wn::tanh_h2(h2(pack_h2(accp[0][0], accp[0][1]))), tg1 = wn::tanh_h2(h2(pack_h2(accp[0][2], accp[0][3])));
@@ -1088,11 +1091,8 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     for (int j = 0; j < 4; j++) load_a(ha[j], sm + M::C_HBUF + j * 512 + lane16);
                     TRACE2(0, 10);
                     float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
-                    {
-                        const uint4 bw0 = lds128(p1 + o_res), bw1 = lds128(p1 + o_res + 512);
-                        hmma(ra, ha[0], bw0.x, bw0.y); hmma(rb, ha[2], bw1.x, bw1.y);
-                        hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
-                    }
+                    hmma(ra, ha[0], bw0.x, bw0.y); hmma(rb, ha[2], bw1.x, bw1.y);
+                    hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
                     release(s_empty + 8 * sl);
                     xres[0] = ((ra[0] + rb[0]) + br.x) + xres[0]; xres[1] = ((ra[1] + rb[1]) + br.y) + xres[1];
                     xres[2] = ((ra[2] + rb[2]) + br.x) + xres[2]; xres[3] = ((ra[3] + rb[3]) + br.y) + xres[3];
