@@ -821,21 +821,26 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
 // B fragments and 48 KB of A fragments read back; ncu: 0.57 LSU wavefronts per cycle + the TMA writes).  Here one 16-utterance tile
 // is served by a CLUSTER OF THREE CTAs on three SMs, and only what depends on the previous sample stays on the first one:
 //   rank 0 "chain": embedding, cur / res GEMMs, gate, history ring writes             ring pieces [Wcur_l | Wres_l] (24 KB)
-//   rank 1 "tail":  skip GEMM of every step (off the chain), Zs, Za, softmax, sampling ring pieces Wskip_l and the output pieces
-//   rank 2 "prep":  (Bh + Lh) + Wprev . x[t-d] of the steps to come, up to NAP ahead   ring pieces Wprev_l (16 KB)
-// Distributed shared memory carries three flows, all as st.async with complete_tx on a transaction barrier that the receiver arms
+//   rank 1 "tail":  skip GEMM of every step (off the chain), output columns 0-127 of   ring pieces Wskip_l
+//                   Zs and Za, softmax, sampling
+//   rank 2 "prep":  (Bh + Lh) + Wprev . x[t-d] of the steps to come, up to NAP ahead;  ring pieces Wprev_l (16 KB)
+//                   output columns 128-255 of Zs and Za, between two of its steps
+// The output weights stay resident: every compute thread of the tail and prep CTAs loads the B fragments of its two n-tiles once, at
+// kernel start, Wzs into registers (S / 4) and Wza into its CTA's shared memory (64 KB per CTA).
+// Distributed shared memory carries six flows, all as st.async with complete_tx on a transaction barrier that the receiver arms
 // one phase ahead (data and signal travel together, no release fence on the sender), buffers handed back with relaxed remote arrives:
 // h (2 KB per step, chain -> tail), the pre-activation before the current-sample GEMM (8 KB per step, prep -> chain), the 16 sampled
-// indices (once per sample, tail -> chain).  Each CTA moves less than ~100 KB per step through its shared memory; a single CTA
-// doing all of it moves ~190 KB per step and is bound by that.
+// indices (once per sample, tail -> chain); once per sample for the output layers: relu(skip + Bskip) (S x 32 B, tail -> prep),
+// the relu(Zs) halves (4 KB each way, tail <-> prep) and the prep's logits half (8 KB fp32, prep -> tail).  Each CTA moves less than
+// ~100 KB per step through its shared memory; a single CTA doing all of it moves ~190 KB per step and is bound by that.
 constexpr int NTC = NCT + 32;
 
 template <int S>
 struct CfgC {
     using C = Cfg<S>;
     static constexpr uint32_t PIECE0 = 24576;                              // chain: [Wcur | Wres]
-    static constexpr uint32_t SLOT1 = 32768;                               // tail: Wskip_l (S x 128 B) or an output piece
-    static constexpr int NSLOT1 = 4;
+    static constexpr uint32_t SLOT1 = S * 128;                             // tail: Wskip_l
+    static constexpr int NSLOT1 = 3;
     static constexpr int NAP = 4;                                          // pre-activation tiles in flight from the prep CTA to the chain CTA
     static constexpr int NPS = 8;                                          // staged history / conditioning tiles of the prep CTA
     // chain CTA
@@ -848,24 +853,33 @@ struct CfgC {
     static constexpr uint32_t C_BIAS = C_AP + NAP * 8192;                  // [L][8 warps][4][8] fp32: Bh / Bres pairs per thread (Bres is read here)
     static constexpr uint32_t C_END = C_BIAS + MAXL * 1024;
     // tail CTA
+    // Output layers, tail and prep CTAs: OB0 = relu(skip + Bskip) and OB1 = relu(Zs) in A-fragment order (OB1 k-steps 0-7 come from
+    // the tail, 8-15 from the prep; each CTA writes into the other's), ZA = this CTA's half of Wza in B-fragment order, resident.
+    static constexpr uint32_t OB0_BYTES = (S / 16) * 512, OB1_BYTES = (A / 16) * 512, ZA_BYTES = 16 * (A / 32) * 512;
     static constexpr uint32_t T_RING = 0;                                  // NSLOT1 x SLOT1
-    static constexpr uint32_t T_BOUT = NSLOT1 * SLOT1;
-    static constexpr uint32_t T_HBUF = T_BOUT + (S + 2 * A) * 4;           // 2 x 2 KB, written by the chain CTA
-    static constexpr uint32_t T_OB0 = T_HBUF + 2 * 2048;
-    static constexpr uint32_t T_OB1 = T_OB0 + (S / 16) * 512;
-    static constexpr uint32_t T_LBUF = T_OB1 + (A / 16) * 512;
-    static constexpr uint32_t T_END = T_LBUF + TU * LROW * 4;
+    static constexpr uint32_t T_HBUF = NSLOT1 * SLOT1;                     // 2 x 2 KB, written by the chain CTA
+    static constexpr uint32_t T_LBUF = T_HBUF + 2 * 2048;                  // transposed logits; columns 128-255 written by the prep CTA
+    static constexpr uint32_t T_BOUT = T_LBUF + TU * LROW * 4;             // fp32: Bskip total [S], Bzs [A], Bza [A]
+    static constexpr uint32_t T_OB0 = T_BOUT + (S + 2 * A) * 4;
+    static constexpr uint32_t T_OB1 = T_OB0 + OB0_BYTES;
+    static constexpr uint32_t T_ZA = T_OB1 + OB1_BYTES;
+    static constexpr uint32_t T_END = T_ZA + ZA_BYTES;
     // prep CTA
     static constexpr uint32_t P_RING = 0;                                  // 4 x 16 KB: Wprev_l
     static constexpr uint32_t P_PST = 4 * 16384;                           // NPS x 2 KB: staged history tiles x[t-d] (A-fragment order)
     static constexpr uint32_t P_COND = P_PST + NPS * 2048;                 // NPS x 4 KB: conditioning tiles, staged with the history tiles (cp.async)
     static constexpr uint32_t P_BIAS = P_COND + NPS * 4096;                // [L][8 warps][4][4] fp32: this thread's Bh
     static constexpr uint32_t P_DIL = P_BIAS + MAXL * 512;
-    static constexpr uint32_t P_END = P_DIL + MAXL * 4;
+    static constexpr uint32_t P_BOUT = P_DIL + MAXL * 4;                   // fp32: Bzs [A], Bza [A]
+    static constexpr uint32_t P_OB0 = P_BOUT + 2 * A * 4;
+    static constexpr uint32_t P_OB1 = P_OB0 + OB0_BYTES;
+    static constexpr uint32_t P_ZA = P_OB1 + OB1_BYTES;
+    static constexpr uint32_t P_END = P_ZA + ZA_BYTES;
     // common tail of the maps (same offsets in every CTA, so that remote addresses are computed with mapa on local ones)
     static constexpr uint32_t O_YS = (C_END > T_END ? (C_END > P_END ? C_END : P_END) : (T_END > P_END ? T_END : P_END));
     static constexpr uint32_t O_BAR = O_YS + 2 * TU * 4;
-    static constexpr uint32_t SMEM = O_BAR + 32 * 8;
+    static constexpr uint32_t SMEM = O_BAR + 40 * 8;
+    static_assert(SMEM <= 227 * 1024, "the cluster kernel's shared-memory map exceeds the 227 KB an H100 CTA may use");
 };
 constexpr int NCL = 3;                       // CTAs per cluster
 
@@ -880,10 +894,14 @@ __device__ __forceinline__ void st_async_v2(uint32_t raddr, uint32_t a, uint32_t
 {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.b32 [%0], {%1,%2}, [%3];" ::"r"(raddr), "r"(a), "r"(b), "r"(rbar) : "memory");
 }
-__device__ __forceinline__ void st_async_v4(uint32_t raddr, float a, float b, float c, float d, uint32_t rbar)
+__device__ __forceinline__ void st_async_v4(uint32_t raddr, uint4 v, uint32_t rbar)
 {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1,%2,%3,%4}, [%5];"
-                 ::"r"(raddr), "r"(__float_as_uint(a)), "r"(__float_as_uint(b)), "r"(__float_as_uint(c)), "r"(__float_as_uint(d)), "r"(rbar) : "memory");
+                 ::"r"(raddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(rbar) : "memory");
+}
+__device__ __forceinline__ void st_async_v4(uint32_t raddr, float a, float b, float c, float d, uint32_t rbar)
+{
+    st_async_v4(raddr, make_uint4(__float_as_uint(a), __float_as_uint(b), __float_as_uint(c), __float_as_uint(d)), rbar);
 }
 __device__ __forceinline__ void st_async_u32(uint32_t raddr, uint32_t a, uint32_t rbar)
 {
@@ -899,8 +917,8 @@ __device__ __forceinline__ void cluster_sync_all()
 template <int S, bool DUMP, bool TRC>
 __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
 {
-    // debug timeline (tools/lat_trace.py): role 0 = chain CTA thread 0, role 1 = tail CTA thread 0, of the first cluster
-    unsigned long long* trc = (TRC && p.trace && blockIdx.x < 2) ? p.trace : nullptr;
+    // debug timeline (tools/lat_trace.py): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
+    unsigned long long* trc = (TRC && p.trace && blockIdx.x < NCL) ? p.trace : nullptr;
     int trn = 0;
     const int tr_t = p.trace_t & 0xFFFF;
 #define TRACE2(role, tag) do { if (TRC && trc && threadIdx.x == 0 && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
@@ -918,13 +936,17 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
-    constexpr int NQ = C::NQ_ZS + C::NQ_ZA;
 
-    // barriers (same offsets in every CTA): ring full[4] / empty[4] (the chain uses two of each); pfull[NPS] (prep: staged history
+    // barriers (same offsets in every CTA): ring full[4] / empty[4] (the chain uses two of each, the tail three); pfull[NPS] (prep: staged history
     // tiles); hfull[2] (tail: h tiles, bytes from the chain); hfree[2], yfull, apfull[NAP] (chain: bytes from the tail / the prep CTA);
-    // apfree[NAP] (prep: arrived by the chain's warps)
+    // apfree[NAP] (prep: arrived by the chain's warps).  Output layers, once per sample: ob0full (prep: relu(skip) bytes from the
+    // tail); ob0free (tail: arrived by the prep's warps); ob1full (tail and prep: the peer's relu(Zs) half); ob1free (tail and prep:
+    // arrived by the warps of both CTAs once they have read OB1); lfull (tail: the prep's logits bytes); lfree (prep: arrived by the
+    // tail's warps once the softmax has read the logits)
     const uint32_t s_full = sm + M::O_BAR, s_empty = s_full + 32, s_pfull = s_full + 64, s_hfull = s_full + 128, s_hfree = s_full + 144, s_yfull = s_full + 160;
     const uint32_t s_apfull = s_full + 168, s_apfree = s_full + 200;
+    const uint32_t s_ob0full = s_full + 232, s_ob0free = s_full + 240, s_ob1full = s_full + 248, s_ob1free = s_full + 256;
+    const uint32_t s_lfull = s_full + 264, s_lfree = s_full + 272;
     int* ys = reinterpret_cast<int*>(smem_raw + M::O_YS);
 
     if (tid == 0) {
@@ -933,11 +955,15 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
         for (int i = 0; i < 2; i++) { mbar_init_a(s_hfull + 8 * i, 1); mbar_init_a(s_hfree + 8 * i, NCW); }
         for (int i = 0; i < M::NAP; i++) { mbar_init_a(s_apfull + 8 * i, 1); mbar_init_a(s_apfree + 8 * i, NCW); }
         mbar_init_a(s_yfull, 1);
+        mbar_init_a(s_ob0full, 1); mbar_init_a(s_ob0free, NCW); mbar_init_a(s_ob1full, 1); mbar_init_a(s_ob1free, 2 * NCW);
+        mbar_init_a(s_lfull, 1); mbar_init_a(s_lfree, NCW);
         fence_mbar_init();
         // transaction barriers are armed by their owner one phase ahead: the tail expects 2 KB per h tile, the chain 128 B of indices
-        // and 8 KB per pre-activation tile
+        // and 8 KB per pre-activation tile; once per sample the prep expects relu(skip) and a relu(Zs) half, the tail a relu(Zs) half
+        // and the logits half
         if (is_chain) { mbar_expect_a(s_yfull, 2 * TU * 4); for (int i = 0; i < M::NAP; i++) mbar_expect_a(s_apfull + 8 * i, 8192); }
-        else if (is_tail) { mbar_expect_a(s_hfull, 2048); mbar_expect_a(s_hfull + 8, 2048); }
+        else if (is_tail) { mbar_expect_a(s_hfull, 2048); mbar_expect_a(s_hfull + 8, 2048); mbar_expect_a(s_ob1full, TU * 128 * 2); mbar_expect_a(s_lfull, TU * 128 * 4); }
+        else { mbar_expect_a(s_ob0full, TU * S * 2); mbar_expect_a(s_ob1full, TU * 128 * 2); }
     }
     if (tid < TU) {
         const int b = tile * TU + tid;
@@ -956,6 +982,8 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
         int* dil = reinterpret_cast<int*>(smem_raw + M::P_DIL);
         if (tid == 0) { int d = 1; for (int l = 0; l < L; l++) { dil[l] = d; d <<= 1; if (d > p.maxDil) d = 1; } }   // nv_wavenet.cuh:99-111
         for (int i = tid; i < L * 128; i += NTC) sts32(sm + M::P_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + (i >> 2) * 8 + (i & 3)]));
+        float* s_bout = reinterpret_cast<float*>(smem_raw + M::P_BOUT);
+        for (int i = tid; i < A; i += NTC) { s_bout[i] = gbias[im.b_bzs + i]; s_bout[A + i] = gbias[im.b_bza + i]; }
     }
     __syncthreads();
     cluster_sync_all();                                    // every CTA's barriers are initialised before anybody signals a peer
@@ -968,6 +996,115 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     const uint32_t xchg = (uint32_t)(jw * 512 + hw * 8) + lane16;
     auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive_a(bar); };
     auto release_remote = [&](uint32_t local_bar, uint32_t rank) { __syncwarp(); if (lane == 0) mbar_arrive_remote(mapa_u32(local_bar, rank)); };
+
+    // ---------------- output layers, tail (half 0) and prep (half 1) CTAs: n-tiles 16 half + 2w and 16 half + 2w + 1 of Zs and Za.
+    // Their B fragments (lat_pack_kernel: piece q of a matrix = k-step pairs [q OJP, (q+1) OJP) of all 32 n-tiles, fragment
+    // (n-tile OJP + jp) x 512 + lane x 16) are loaded once, at kernel start: Wzs into registers (S / 4 per thread), Wza into this
+    // CTA's ZA region, where every thread reads back only the 16 B it stored itself (fragment (2w + i) x A/32 + jp).  Wza resident
+    // in registers as well would not fit: nine warps leave 168 registers per thread (three warps share a sub-partition's 64 KB),
+    // and the tail's skip loop and the prep's step loop would spill ~300 B at S = 256.
+    auto load_out_w = [&](uint4 (&zsw)[2][S / 32], const uint32_t half) {
+        const uint32_t za = sm + (half ? M::P_ZA : M::T_ZA) + lane16;
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int nt = 16 * half + 2 * w + i;
+#pragma unroll
+            for (int jp = 0; jp < S / 32; jp++)
+                zsw[i][jp] = ldg_nc_v4(img + im.off_zs + (size_t)(jp / C::OJP_ZS) * C::ZS_PIECE + (size_t)(nt * C::OJP_ZS + jp % C::OJP_ZS) * 512 + lane16);
+            for (int jp = 0; jp < A / 32; jp++)
+                sts128(za + ((2 * w + i) * (A / 32) + jp) * 512,
+                       ldg_nc_v4(img + im.off_za + (size_t)(jp / C::OJP_ZA) * C::ZA_PIECE + (size_t)(nt * C::OJP_ZA + jp % C::OJP_ZA) * 512 + lane16));
+        }
+    };
+    // relu(skip + Bskip) is in this CTA's OB0 (the prep waits for it here).  Per n-tile the HMMAs run from the bias through the
+    // k-steps in order on one accumulator, as in the single-CTA kernel.  relu(Zs) of the two n-tiles is k-step 8 half + w of the
+    // Za GEMM's A operand: 16 B per thread into this CTA's OB1 and the peer's.  Leaves the logits of the two n-tiles in zz.
+    auto out_half = [&](const int t, const uint4 (&zsw)[2][S / 32], const uint32_t half, float (&zz)[2][4]) {
+        const uint32_t peer = half ? 1 : 2, par = (uint32_t)(t - t_begin) & 1;
+        const float* bz = reinterpret_cast<const float*>(smem_raw + (half ? M::P_BOUT : M::T_BOUT + S * 4));   // Bzs [A], Bza [A]
+        const uint32_t ob0 = sm + (half ? M::P_OB0 : M::T_OB0), ob1 = sm + (half ? M::P_OB1 : M::T_OB1), za = sm + (half ? M::P_ZA : M::T_ZA);
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
+            zz[i][0] = zz[i][2] = bz[c]; zz[i][1] = zz[i][3] = bz[c + 1];
+        }
+        // the Wza fragments of the first half of K (32 registers) are read while the CTA would wait anyway: the prep before relu(skip)
+        // arrives, the tail after its Zs HMMAs, while the prep's relu(Zs) half is still on its way; those of the second half inside
+        // the Za GEMM (three quarters or more up front spill at S = 256)
+        constexpr int ZPRE = A / 64;
+        uint4 zab[2][A / 32];
+        auto load_za = [&]() {
+#pragma unroll
+            for (int jp = 0; jp < ZPRE; jp++)
+#pragma unroll
+                for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
+        };
+        if (half) { load_za(); mbar_wait_a(s_ob0full, par); }
+#pragma unroll
+        for (int jp = 0; jp < S / 32; jp++) {
+            uint32_t a0[4], a1[4];
+            load_a(a0, ob0 + (2 * jp) * 512 + lane16);
+            load_a(a1, ob0 + (2 * jp + 1) * 512 + lane16);
+#pragma unroll
+            for (int i = 0; i < 2; i++) hmma(zz[i], a0, zsw[i][jp].x, zsw[i][jp].y);
+#pragma unroll
+            for (int i = 0; i < 2; i++) hmma(zz[i], a1, zsw[i][jp].z, zsw[i][jp].w);
+        }
+        if (!half) load_za();
+        if (half) {                                    // OB0 has been read: arm its barrier for the next sample, then free it
+            if (tid == 0) mbar_expect_a(s_ob0full, TU * S * 2);
+            release_remote(s_ob0free, 1);
+        }
+        TRACE2(crank, 24);
+        uint32_t zp[4];
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
+            const float z0 = fmaxf(zz[i][0], 0.f), z1 = fmaxf(zz[i][1], 0.f), z2 = fmaxf(zz[i][2], 0.f), z3 = fmaxf(zz[i][3], 0.f);
+            zp[2 * i] = pack_h2(z0, z1); zp[2 * i + 1] = pack_h2(z2, z3);
+            if (DUMP) {
+                if (v0) { p.Zs[(size_t)b0 * A + c] = z0; p.Zs[(size_t)b0 * A + c + 1] = z1; }
+                if (v1) { p.Zs[(size_t)b1 * A + c] = z2; p.Zs[(size_t)b1 * A + c + 1] = z3; }
+            }
+            zz[i][0] = zz[i][2] = bz[A + c]; zz[i][1] = zz[i][3] = bz[A + c + 1];
+        }
+        {   // both CTAs' warps have read the previous sample's OB1
+            const uint32_t o = (8 * half + w) * 512 + lane16;
+            const uint4 v = make_uint4(zp[0], zp[1], zp[2], zp[3]);
+            mbar_wait_a(s_ob1free, par ^ 1);
+            sts128(ob1 + o, v);
+            st_async_v4(mapa_u32(sm + (half ? M::T_OB1 : M::P_OB1) + o, peer), v, mapa_u32(s_ob1full, peer));
+        }
+        bar_compute();
+        mbar_wait_a(s_ob1full, par);
+        TRACE2(crank, 21);
+#pragma unroll
+        for (int jp = 0; jp < A / 32; jp++) {
+            uint32_t a0[4], a1[4];
+            load_a(a0, ob1 + (2 * jp) * 512 + lane16);
+            load_a(a1, ob1 + (2 * jp + 1) * 512 + lane16);
+            if (jp >= ZPRE) {
+#pragma unroll
+                for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
+            }
+#pragma unroll
+            for (int i = 0; i < 2; i++) hmma(zz[i], a0, zab[i][jp].x, zab[i][jp].y);
+#pragma unroll
+            for (int i = 0; i < 2; i++) hmma(zz[i], a1, zab[i][jp].z, zab[i][jp].w);
+        }
+        // OB1 has been read: arm its barrier for the peer's next half, then free it for both CTAs
+        if (tid == 0) mbar_expect_a(s_ob1full, TU * 128 * 2);
+        release(s_ob1free);
+        release_remote(s_ob1free, peer);
+        if (DUMP) {
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
+                if (v0) { p.Za[(size_t)b0 * A + c] = zz[i][0]; p.Za[(size_t)b0 * A + c + 1] = zz[i][1]; }
+                if (v1) { p.Za[(size_t)b1 * A + c] = zz[i][2]; p.Za[(size_t)b1 * A + c + 1] = zz[i][3]; }
+            }
+        }
+    };
 
     if (is_chain) {
         // ===================================================================================== chain CTA
@@ -1132,22 +1269,20 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
             if (lane == 0) {
                 uint32_t pc = 0;
                 auto put = [&](const unsigned char* src, uint32_t bytes) {
-                    const uint32_t sl = pc & 3;
-                    mbar_wait_a(s_empty + 8 * sl, ((pc >> 2) & 1) ^ 1);
+                    const uint32_t sl = pc % M::NSLOT1;
+                    mbar_wait_a(s_empty + 8 * sl, ((pc / M::NSLOT1) & 1) ^ 1);
                     mbar_expect_a(s_full + 8 * sl, bytes);
                     tma_load_a(sm + M::T_RING + sl * M::SLOT1, src, bytes, s_full + 8 * sl);
                     pc++;
                 };
-                for (int t = t_begin; t < t_end; t++) {
+                for (int t = t_begin; t < t_end; t++)
                     for (int l = 0; l < L; l++) put(img + (size_t)l * im.layer_bytes + C::W_SKIP, S * 128);
-                    for (int q = 0; q < NQ; q++)
-                        put(q < C::NQ_ZS ? img + im.off_zs + (size_t)q * C::ZS_PIECE : img + im.off_za + (size_t)(q - C::NQ_ZS) * C::ZA_PIECE,
-                            q < C::NQ_ZS ? C::ZS_PIECE : C::ZA_PIECE);
-                }
             }
         } else {
-            float* s_bout = reinterpret_cast<float*>(smem_raw + M::T_BOUT);
-            const uint32_t o_skip = (uint32_t)(w * C::NSK * 2) * 512 + lane16, o_out = (uint32_t)(4 * w) * 512;
+            const float* s_bout = reinterpret_cast<const float*>(smem_raw + M::T_BOUT);
+            const uint32_t o_skip = (uint32_t)(w * C::NSK * 2) * 512 + lane16;
+            uint4 zsw[2][S / 32];
+            load_out_w(zsw, 0);
             float sk[C::NSK][4];
 #pragma unroll
             for (int i = 0; i < C::NSK; i++) sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
@@ -1162,8 +1297,8 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     uint32_t ha[4][4];
 #pragma unroll
                     for (int j = 0; j < 4; j++) load_a(ha[j], hb + j * 512 + lane16);
-                    const uint32_t sl = pc & 3, p2 = sm + M::T_RING + sl * M::SLOT1;
-                    mbar_wait_a(s_full + 8 * sl, (pc >> 2) & 1);
+                    const uint32_t sl = pc % M::NSLOT1, p2 = sm + M::T_RING + sl * M::SLOT1;
+                    mbar_wait_a(s_full + 8 * sl, (pc / M::NSLOT1) & 1);
 #pragma unroll
                     for (int jp = 0; jp < 2; jp++) {
                         uint4 bw[C::NSK];
@@ -1193,68 +1328,38 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     }
                 }
                 // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
+                {   // relu(skip + Bskip): 16 B per pair of skip n-tiles, into this CTA's OB0 and the prep CTA's (free once the prep's
+                    // warps have read the previous sample's)
+                    uint4 v[C::NSK / 2];
 #pragma unroll
-                for (int i = 0; i < C::NSK; i++) {
-                    const int nt = w * C::NSK + i, c = 8 * nt + 2 * t4;
-                    const float b0f = s_bout[c], b1f = s_bout[c + 1];
-                    sts64(sm + M::T_OB0 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8,
-                          pack_h2(fmaxf(sk[i][0] + b0f, 0.f), fmaxf(sk[i][1] + b1f, 0.f)), pack_h2(fmaxf(sk[i][2] + b0f, 0.f), fmaxf(sk[i][3] + b1f, 0.f)));
-                    sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
+                    for (int i = 0; i < C::NSK; i++) {
+                        const int c = 8 * (w * C::NSK + i) + 2 * t4;
+                        const float b0f = s_bout[c], b1f = s_bout[c + 1];
+                        const uint32_t lo = pack_h2(fmaxf(sk[i][0] + b0f, 0.f), fmaxf(sk[i][1] + b1f, 0.f)), hi = pack_h2(fmaxf(sk[i][2] + b0f, 0.f), fmaxf(sk[i][3] + b1f, 0.f));
+                        if (i & 1) { v[i >> 1].z = lo; v[i >> 1].w = hi; } else { v[i >> 1].x = lo; v[i >> 1].y = hi; }
+                        sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
+                    }
+                    mbar_wait_a(s_ob0free, ((uint32_t)(t - t_begin) & 1) ^ 1);
+                    const uint32_t r_ob0full = mapa_u32(s_ob0full, 2);
+#pragma unroll
+                    for (int j = 0; j < C::NSK / 2; j++) {
+                        const uint32_t o = (w * C::NSK / 2 + j) * 512 + lane16;
+                        sts128(sm + M::T_OB0 + o, v[j]);
+                        st_async_v4(mapa_u32(sm + M::P_OB0 + o, 2), v[j], r_ob0full);
+                    }
                 }
                 bar_compute();
                 TRACE2(1, 20);
-                float zz[4][4];
+                float zz[2][4];
+                out_half(t, zsw, 0, zz);
 #pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const int c = 32 * w + 8 * i + 2 * t4;
-                    zz[i][0] = zz[i][2] = s_bout[S + c]; zz[i][1] = zz[i][3] = s_bout[S + c + 1];
-                }
-                auto out_gemm = [&](const int ojp, const uint32_t abuf, const int kp0) {
-                    const uint32_t sl = pc & 3, st = sm + M::T_RING + sl * M::SLOT1 + o_out * ojp + lane16;
-                    mbar_wait_a(s_full + 8 * sl, (pc >> 2) & 1);
-                    for (int jp = 0; jp < ojp; jp++) {
-                        uint32_t a0[4], a1[4];
-                        load_a(a0, abuf + ((kp0 + jp) * 2) * 512 + lane16);
-                        load_a(a1, abuf + ((kp0 + jp) * 2 + 1) * 512 + lane16);
-                        uint4 bw[4];
-#pragma unroll
-                        for (int i = 0; i < 4; i++) bw[i] = lds128(st + (i * ojp + jp) * 512);
-#pragma unroll
-                        for (int i = 0; i < 4; i++) hmma(zz[i], a0, bw[i].x, bw[i].y);
-#pragma unroll
-                        for (int i = 0; i < 4; i++) hmma(zz[i], a1, bw[i].z, bw[i].w);
-                    }
-                    release(s_empty + 8 * sl);
-                    pc++;
-                };
-#pragma unroll
-                for (int q = 0; q < C::NQ_ZS; q++) out_gemm(C::OJP_ZS, sm + M::T_OB0, q * C::OJP_ZS);
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const int nt = 4 * w + i, c = 8 * nt + 2 * t4;
-                    const float z0 = fmaxf(zz[i][0], 0.f), z1 = fmaxf(zz[i][1], 0.f), z2 = fmaxf(zz[i][2], 0.f), z3 = fmaxf(zz[i][3], 0.f);
-                    sts64(sm + M::T_OB1 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8, pack_h2(z0, z1), pack_h2(z2, z3));
-                    if (DUMP) {
-                        if (v0) { p.Zs[(size_t)b0 * A + c] = z0; p.Zs[(size_t)b0 * A + c + 1] = z1; }
-                        if (v1) { p.Zs[(size_t)b1 * A + c] = z2; p.Zs[(size_t)b1 * A + c + 1] = z3; }
-                    }
-                    zz[i][0] = zz[i][2] = s_bout[S + A + c]; zz[i][1] = zz[i][3] = s_bout[S + A + c + 1];
-                }
-                bar_compute();
-                TRACE2(1, 21);
-#pragma unroll
-                for (int q = 0; q < C::NQ_ZA; q++) out_gemm(C::OJP_ZA, sm + M::T_OB1, q * C::OJP_ZA);
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const int c = 32 * w + 8 * i + 2 * t4;
+                for (int i = 0; i < 2; i++) {
+                    const int c = 8 * (2 * w + i) + 2 * t4;
                     sts64(sm + M::T_LBUF + (g * LROW + c) * 4, __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]));
                     sts64(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
-                    if (DUMP) {
-                        if (v0) { p.Za[(size_t)b0 * A + c] = zz[i][0]; p.Za[(size_t)b0 * A + c + 1] = zz[i][1]; }
-                        if (v1) { p.Za[(size_t)b1 * A + c] = zz[i][2]; p.Za[(size_t)b1 * A + c + 1] = zz[i][3]; }
-                    }
                 }
                 bar_compute();
+                mbar_wait_a(s_lfull, (uint32_t)(t - t_begin) & 1);  // columns 128-255 from the prep CTA
                 TRACE2(1, 22);
                 {   // softmax + categorical sample: warp w serves utterances 2w and 2w+1; lane holds 8 consecutive classes of each
                     float e[2][8], m[2] = {0.f, 0.f};
@@ -1271,6 +1376,9 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                         m[0] = fmaxf(m[0], __shfl_xor_sync(0xffffffffu, m[0], o));
                         m[1] = fmaxf(m[1], __shfl_xor_sync(0xffffffffu, m[1], o));
                     }
+                    // the logits have been read: arm lfull for the prep's next half, then hand the buffer back to it
+                    if (tid == 0) mbar_expect_a(s_lfull, TU * 128 * 4);
+                    release_remote(s_lfree, 2);
                     float incl[2];
 #pragma unroll
                     for (int r = 0; r < 2; r++) {
@@ -1383,8 +1491,25 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 pcnt++;
                 if (++itp.l == L) { itp.l = 0; itp.t++; if (++itp.slot == slots) itp.slot = 0; }
             };
+            uint4 zsw[2][S / 32];
+            load_out_w(zsw, 1);
+            // output columns 128-255 of sample t; the logits go to the tail CTA (free once its softmax has read the previous ones)
+            auto out_prep = [&](const int t) {
+                float zz[2][4];
+                TRACE2(2, 30);
+                out_half(t, zsw, 1, zz);
+                const uint32_t r_lfull = mapa_u32(s_lfull, 1);
+                mbar_wait_a(s_lfree, ((uint32_t)(t - t_begin) & 1) ^ 1);
+#pragma unroll
+                for (int i = 0; i < 2; i++) {
+                    const int c = 8 * (16 + 2 * w + i) + 2 * t4;
+                    st_async_v2(mapa_u32(sm + M::T_LBUF + (g * LROW + c) * 4, 1), __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]), r_lfull);
+                    st_async_v2(mapa_u32(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, 1), __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]), r_lfull);
+                }
+                TRACE2(2, 33);
+            };
             stage(); stage(); stage();
-            int l1 = 0;
+            int l1 = 0, tout = t_begin;                        // tout: the next sample whose output half is due
             for (int n = 0; n < nsteps; n++) {
                 const uint32_t sl = n & 3, pa = sm + M::P_RING + sl * 16384, slot = n & (M::NPS - 1), buf = n & (M::NAP - 1);
                 cp_async_wait_pending<2>();                    // this thread's conditioning of step n has landed (two later groups may be in flight)
@@ -1409,7 +1534,12 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 st_async_v4(r_ap + buf * 8192 + 16, a1[0] + u1[0], a1[1] + u1[1], a1[2] + u1[2], a1[3] + u1[3], r_apfull + 8 * buf);
                 stage();
                 if (++l1 == L) l1 = 0;
+                // the output half of sample tout: after step (tout + 1, 1) has been shipped, so that the chain CTA starts sample
+                // tout + 1 with its first two pre-activation tiles at hand, and before the wait for the buffer of step
+                // (tout + 1, NAP + 1), which the chain CTA frees only inside sample tout + 1
+                if (n == (tout - t_begin + 1) * L + 1) out_prep(tout++);
             }
+            while (tout < t_end) out_prep(tout++);             // the last sample: no steps follow it
             cp_async_wait_all();
         }
     }

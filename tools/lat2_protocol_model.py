@@ -6,8 +6,9 @@ what a passing GPU run cannot show:
   * deadlock: every warp must finish every sample;
   * phase aliasing: a parity wait passes iff (completions - awaited) is odd -- a waiter two completions behind blocks for ever,
     three behind passes early; the model flags any wait that is ever two or more behind;
-  * buffer hazards: a ring slot, an h tile, a pre-activation tile, a staged history / conditioning slot must not be rewritten before
-    every warp that reads its previous occupant has read it, and every reader must find the occupant it expects;
+  * buffer hazards: a ring slot, an h tile, a pre-activation tile, a staged history / conditioning slot, the output layers' OB0 /
+    OB1 tiles and the logits buffer must not be rewritten before every warp that reads its previous occupant has read it, and
+    every reader must find the occupant it expects;
   * history visibility: the prep CTA stages x_l[t-d] from global memory with plain loads -- the chain CTA must have finished the step
     that wrote it; the model reports the smallest distance (in chain steps) it saw, which is what `L >= 12` in wn_launch_lat buys.
 
@@ -20,6 +21,7 @@ import sys
 
 NCW = 8          # compute warps per CTA
 NAP = 4          # pre-activation tile buffers (chain CTA)
+TSLOTS = 3       # tail ring slots (Wskip_l)
 NPS = 8          # staged history / conditioning slots (prep CTA)
 STAGE_AHEAD = 3  # the prep CTA stages tile n + 3 while it works on tile n
 
@@ -91,9 +93,16 @@ class Sim:
         self.yfull = B("chain.yfull", 1)
         self.apfull = [B(f"chain.apfull{i}", 1) for i in range(NAP)]
         # tail CTA
-        self.t_full = [B(f"tail.full{i}", 1) for i in range(4)]
-        self.t_empty = [B(f"tail.empty{i}", NCW) for i in range(4)]
+        self.t_full = [B(f"tail.full{i}", 1) for i in range(TSLOTS)]
+        self.t_empty = [B(f"tail.empty{i}", NCW) for i in range(TSLOTS)]
         self.hfull = [B(f"tail.hfull{i}", 1) for i in range(2)]
+        # output layers (tail = columns 0-127, prep = 128-255): relu(skip) tail -> prep, relu(Zs) halves both ways, logits prep -> tail
+        self.ob0full = B("prep.ob0full", 1)
+        self.ob0free = B("tail.ob0free", NCW)
+        self.ob1full = {c: B(f"{c}.ob1full", 1) for c in ("tail", "prep")}
+        self.ob1free = {c: B(f"{c}.ob1free", 2 * NCW) for c in ("tail", "prep")}   # arrived by the warps of both CTAs
+        self.lfull = B("tail.lfull", 1)
+        self.lfree = B("prep.lfree", NCW)
         # prep CTA
         self.p_full = [B(f"prep.full{i}", 1) for i in range(4)]
         self.p_empty = [B(f"prep.empty{i}", NCW) for i in range(4)]
@@ -105,6 +114,10 @@ class Sim:
             b.expect_tx(8192)
         for b in self.hfull:
             b.expect_tx(2048)
+        self.ob0full.expect_tx(8192)
+        for b in self.ob1full.values():
+            b.expect_tx(4096)
+        self.lfull.expect_tx(8192)
         # buffers: occupant tag + how many warps have read it
         self.slot = {}                                       # name -> [tag, reads]
         self.chain_steps_done = 0                            # steps whose x output (history ring write) is complete, all warps
@@ -262,33 +275,78 @@ class Sim:
             for l in range(L):
                 yield ("wait", self.hfull[hc & 1], hc >> 1)
                 self.read(who, f"h{hc & 1}", hc)
-                yield ("wait", self.t_full[pc & 3], pc >> 2)
-                self.read(who, f"tring{pc & 3}", pc)
+                yield ("wait", self.t_full[pc % TSLOTS], pc // TSLOTS)
+                self.read(who, f"tring{pc % TSLOTS}", pc)
                 yield ("delay", self.lat(250, 500, who))     # skip GEMM
                 if w == 0:
                     self.hfull[hc & 1].expect_tx(2048)       # armed for the tile after next, before this warp's "free" signal
                 self.after(self.lat(150, 400), self.hfree[hc & 1].arrive)
-                self.t_empty[pc & 3].arrive()
+                self.t_empty[pc % TSLOTS].arrive()
                 pc += 1
                 hc += 1
-            for stage in range(2):                           # Zs, Za: four pieces each
-                yield from self.cta_bar("tail", who)
-                for q in range(4):
-                    yield ("wait", self.t_full[pc & 3], pc >> 2)
-                    self.read(who, f"tring{pc & 3}", pc)
-                    yield ("delay", self.lat(300, 500, who))
-                    self.t_empty[pc & 3].arrive()
-                    pc += 1
+            # relu(skip + Bskip): this warp's 1 KB into the prep CTA's OB0 (and its own, ordered by the CTA barrier)
+            yield ("wait", self.ob0free, t - 1)
+
+            def land_ob0(t=t):
+                self.touch("prep.ob0", t, NCW)
+                self.ob0full.complete_tx(1024)
+            self.after(self.lat(200, 700), land_ob0)
             yield from self.cta_bar("tail", who)
+            yield from self.out_half("tail", w, t)
+            self.touch("tail.lbuf", t, NCW)                  # this warp's logits of columns 0-127
+            yield from self.cta_bar("tail", who)
+            yield ("wait", self.lfull, t)                    # columns 128-255 from the prep CTA
+            self.read(who, "tail.lbuf", t)
             yield ("delay", self.lat(800, 1500, who))        # softmax + sampling of this warp's two utterances
+            if w == 0:
+                self.lfull.expect_tx(8192)                   # armed for the next sample, before this warp's "free" signal
+            self.after(self.lat(150, 400), self.lfree.arrive)
             if t + 1 < T:
                 self.after(self.lat(200, 700), lambda: self.yfull.complete_tx(16))
             yield from self.cta_bar("tail", who)
+
+    def out_half(self, cta, w, t):
+        """Zs -> relu(Zs) exchange -> Za of one CTA's 128 output columns (wn_lat2_kernel's out_half)."""
+        who, peer = f"{cta}.w{w}", "prep" if cta == "tail" else "tail"
+        if cta == "prep":
+            yield ("wait", self.ob0full, t)
+            self.read(who, "prep.ob0", t)
+        yield ("delay", self.lat(300, 700, who))             # Zs GEMM, weights resident
+        if cta == "prep":
+            if w == 0:
+                self.ob0full.expect_tx(8192)
+            self.after(self.lat(150, 400), self.ob0free.arrive)
+        yield ("wait", self.ob1free[cta], t - 1)
+        self.touch(f"{cta}.ob1", t, NCW)                     # this warp's 16 B per thread, locally ...
+
+        def land_ob1(t=t):                                   # ... and into the peer's OB1
+            self.touch(f"{peer}.ob1", t, NCW)
+            self.ob1full[peer].complete_tx(512)
+        self.after(self.lat(200, 700), land_ob1)
+        yield from self.cta_bar(cta, who)
+        if self.bug != "no_ob1full_wait":
+            yield ("wait", self.ob1full[cta], t)
+        self.read(who, f"{cta}.ob1", t)
+        yield ("delay", self.lat(300, 900, who))             # Za GEMM
+        if w == 0:
+            self.ob1full[cta].expect_tx(4096)
+        self.ob1free[cta].arrive()
+        self.after(self.lat(150, 400), self.ob1free[peer].arrive)
+
+    def out_prep(self, w, t):
+        yield from self.out_half("prep", w, t)
+        yield ("wait", self.lfree, t - 1)
+
+        def land_l(t=t):                                     # this warp's 1 KB of logits into the tail CTA's buffer
+            self.touch("tail.lbuf", t, NCW)
+            self.lfull.complete_tx(1024)
+        self.after(self.lat(200, 700), land_l)
 
     def prep_warp(self, w):
         who = f"prep.w{w}"
         L = self.L
         pcnt = 0
+        tout = 0                                             # the next sample whose output half is due
 
         def stage():
             nonlocal pcnt
@@ -337,11 +395,20 @@ class Sim:
             self.after(self.lat(300, 900), land_ap)
             yield ("delay", self.lat(100, 400, who))         # the remote stores occupy this CTA's load/store pipe
             stage()
+            # the output half of sample tout: after step (tout + 1, 1) has been shipped, before the wait for the buffer of step
+            # (tout + 1, NAP + 1) -- the chain CTA frees it only inside sample tout + 1 ("prep_out_late" waits past it: deadlock)
+            due = (tout + 1) * L + 1 + (NAP if self.bug == "prep_out_late" else 0)
+            if n == due:
+                yield from self.out_prep(w, tout)
+                tout += 1
+        while tout < self.T:                                 # the last sample: no steps follow it
+            yield from self.out_prep(w, tout)
+            tout += 1
 
     def build(self):
         L, T = self.L, self.T
         self.spawn("chain.producer", self.producer("chain.producer", self.c_full, self.c_empty, 2, [24576] * (T * L), "cring"))
-        self.spawn("tail.producer", self.producer("tail.producer", self.t_full, self.t_empty, 4, ([32768] * L + [32768] * 8) * T, "tring"))
+        self.spawn("tail.producer", self.producer("tail.producer", self.t_full, self.t_empty, TSLOTS, [32768] * (T * L), "tring"))
         self.spawn("prep.producer", self.producer("prep.producer", self.p_full, self.p_empty, 4, [16384] * (T * L), "pring"))
         for w in range(NCW):
             self.spawn(f"chain.w{w}", self.chain_warp(w))

@@ -9,7 +9,8 @@ import torch
 sys.path.insert(0, ".")
 import os
 os.environ.setdefault("NVWN_FP16_KERNEL", "lat")
-# NVWN_LAT_CLUSTER=0 traces the single-CTA kernel; default: the cluster kernel (role 0 = chain CTA, role 1 = tail CTA; the prep CTA is not traced)
+# NVWN_LAT_CLUSTER=0 traces the single-CTA kernel; default: the cluster kernel (role 0 = chain CTA, role 1 = tail CTA, role 2 = prep CTA:
+# thread 0 of each, the prep only around its half of the output layers)
 import nv_wavenet_b200 as nw
 from nv_wavenet_b200 import _lib
 from tests import refgen
@@ -28,7 +29,8 @@ e.run(N, B, None); torch.cuda.synchronize()
 buf = np.zeros(3 * 1024, np.uint64)
 assert lib.nvwn_debug_trace(e._h, T, buf.ctypes.data, 1) == 0
 names = {1: "sample start (ys read)", 2: "x0 built", 10: "h exchanged", 11: "layer done (x exchanged)", 12: "cur+prev GEMM issued", 13: "probes issued",
-         14: "res done", 15: "skip issued", 16: "tail: h seen", 17: "tail: prev part starts", 18: "tail: pre-activation shipped", 20: "relu(skip) exchanged", 21: "relu(Zs) exchanged", 22: "logits exchanged", 23: "sample done"}
+         14: "res done", 15: "skip issued", 16: "tail: h seen", 17: "tail: prev part starts", 18: "tail: pre-activation shipped", 20: "relu(skip) sent", 21: "relu(Zs) exchanged",
+         22: "logits half received", 23: "sample done", 24: "Zs done", 30: "prep: output half starts", 33: "prep: logits half sent"}
 ev = []
 for role in range(3):
     for v in buf[role * 1024:(role + 1) * 1024]:
