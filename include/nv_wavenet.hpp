@@ -126,6 +126,15 @@ public:
         return rc == 0;
     }
 
+    /* Not in the reference class: teacher-forced scoring, logp[b * num_samples + t] = log p(audio[b][t] | audio[b][0..t),
+     * conditioning) for every step at once, and optionally the fp32 logits; see nvwn_score.  fp16 engines only. */
+    bool score(const int* audio, int num_samples, int batch_size, float* logp, float* logits = NULL, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_score(m_engine, audio, num_samples, batch_size, logp, logits, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)
     {

@@ -108,6 +108,19 @@ int nvwn_get_audio(nvwn_engine* e, float* audio_f32, short* audio_i16, int offse
  * the three outputs (A entries each) may be NULL. */
 int nvwn_mulaw_table(int A, float* f32, short* i16_wrap, short* i16_saturate);
 
+/* Teacher-forced scoring.  logp[b*num_samples + t] = log softmax(Za_t)[audio[b*num_samples + t]], where Za_t are the logits
+ * generation would compute at step t from silence with audio[b][0..t) fed back (teacher forcing): the embedding input of step t
+ * is (audio[t-2], audio[t-1]) with audio[-1] = audio[-2] = 128, x_l[t-d] = 0 for t < d, and step t uses the conditioning Lh[t]
+ * in the engine's store (set_inputs, set_conditioning or the conditioning producer).  All steps are computed at once, over
+ * the first batch_size utterances of the store (batch_size <= B, num_samples <= N).  logits (NULL, or [batch_size][num_samples][A])
+ * receives the fp32 logits.  audio, logp and logits may each be host or device memory; the call returns after completion if
+ * any destination is on the host, device destinations are filled asynchronously on `stream`.  The generation state (history,
+ * yOut, selectors, forced indices, dumps, launch info) is left untouched.  Each output (b, t) depends only on audio[b][0..t],
+ * the conditioning and the weights, bit for bit.  NVWN_FP16 engines with A = 256 only (else NVWN_EUNSUPPORTED); an audio value
+ * outside [0, A) is NVWN_EINVAL and the message names the first offending (b, t). */
+int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size,
+               float* logp, float* logits, void* stream);
+
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);
 int nvwn_get_skip_out(nvwn_engine* e, int layer, float* out);

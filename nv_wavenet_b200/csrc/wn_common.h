@@ -41,6 +41,30 @@ struct WnLaunchInfo {
 cudaError_t wn_launch_stream(const WnParams& p, int contract, cudaStream_t stream, WnLaunchInfo* info);   // 0 fp32 exact, 1 fp16, 2 fp32 fast
 bool wn_stream_supported(int R, int S, int A, bool fp16);
 
+// teacher-forced scoring (wn_score_kernel.cu, DESIGN.md §5.4): one time chunk of T steps x Bs utterances, rows m = (t - t0) * Bs + b
+struct WnScoreChunk {
+    int L, R, S, A, maxDil, tanhEmbed;
+    int Bs, Be;                     // utterances scored / of the engine (stride of the conditioning chunk)
+    int N, t0, T, Tcap;             // num_samples of the call (row stride of audio and logp), first step, steps, chunk capacity
+    const void* image;              // scorer weight image (wn_score_pack)
+    const void *embPrev, *embCur;   // fp16 [A][R] (engine blob)
+    const int* audio;               // device [Bs][N]
+    const float* lh;                // conditioning of the chunk, fp32 [T][L][Be][2R]
+    __half* xh;                     // fp16 layer inputs; layer l at wn_score_xh_offset(l): [d_l * Bs history rows | T * Bs rows][R]
+    float* xf;                      // fp32 residual stream [T * Bs][R]
+    __half* H;                      // gate outputs [T * Bs][L * R]
+    float* logp;                    // device [Bs][N]
+    float* logits;                  // row (t, b) -> logits + b * logits_ld + (t - logits_t0) * A, or NULL
+    long long logits_ld;
+    int logits_t0;
+};
+int wn_score_dilation(int layer, int maxDil);
+size_t wn_score_xh_offset(int layer, int L, int maxDil, int Tcap, int Be, int R);   // in elements; layer = L gives the total
+size_t wn_score_image_bytes(int R, int S, int A, int L);
+cudaError_t wn_score_pack(void* image, const WnParams& p, cudaStream_t stream);
+cudaError_t wn_score_check_audio(const int* audio, size_t n, int A, unsigned long long* first_bad, cudaStream_t stream);
+cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t stream);
+
 // conversions (wn_convert.cu)
 cudaError_t wn_f32_to_f16(__half* dst, const float* src_dev, size_t n, cudaStream_t stream);
 cudaError_t wn_f16_to_f32(float* dst, const __half* src_dev, size_t n, cudaStream_t stream);

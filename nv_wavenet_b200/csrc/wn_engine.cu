@@ -106,6 +106,12 @@ struct nvwn_engine {
     size_t cp_floats = 0;
     int cp_C = 0, cp_T = 0, cp_K = 0, cp_stride = 0, cp_chunk = 0;
 
+    // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
+    void* score_image = nullptr;
+    bool score_dirty = true;                 // set wherever tc_dirty is: the image is repacked on the next nvwn_score
+    char* score_scratch = nullptr;
+    int score_T = 0;                         // time steps per chunk: SCORE_ROWS / B
+
     float* lut_f = nullptr;                  // mu-law decode tables (nvwn_get_audio): A floats, then 2 x A int16 (wrap / saturate)
     unsigned long long* trace = nullptr;     // debug timeline (nvwn_debug_trace)
     int trace_t = -1;
@@ -185,6 +191,42 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, int count, 
     p.yPrev = e->yPrev; p.yCur = e->yCur; p.ring = e->ring; p.yOut = e->yOut;
     p.xtOut = e->xtOut; p.skipOut = e->skipOut; p.Zs = e->Zs; p.Za = e->Za; p.P = e->P;
     p.trace = e->trace; p.trace_t = e->trace_t;
+}
+
+// the engine's conditioning store for samples [first_sample, first_sample + num_samples) as fp32 [num_samples][L][B][2R] in
+// device memory, whatever the kernel-native layout (plain / tiled fp16 / fragment order) is
+cudaError_t cond_readback(const nvwn_engine* e, float* dst_dev, int first_sample, int num_samples, cudaStream_t st)
+{
+    const size_t per = (size_t)e->L * e->B * 2 * e->R, n = per * num_samples;
+    if (e->lat_mode) return wn_lat_cond_readback(dst_dev, e->Lh, first_sample, num_samples, e->L, e->B, st);
+    if (e->tc_mode) return wn_tc_cond_readback(dst_dev, e->Lh, first_sample, num_samples, e->tc_tile, e->L, e->B, st);
+    if (e->dtype == NVWN_FP16) return wn_f16_to_f32(dst_dev, static_cast<const __half*>(e->Lh) + (size_t)first_sample * per, n, st);
+    return cudaMemcpyAsync(dst_dev, static_cast<const float*>(e->Lh) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+}
+
+// rows (t, b) of one scoring chunk; bounds the chunk scratch: DESIGN.md §5.4
+constexpr int SCORE_ROWS = 16384;
+
+// byte offsets of the scoring scratch, for the engine's B and N and a chunk of T steps
+struct ScoreScratch {
+    size_t audio, logp, bad, lh, xh, xf, H, lgt, bytes;
+};
+ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
+{
+    ScoreScratch o;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t r = off; off = align_up(off + bytes, 256); return r; };
+    const size_t B = e->B, N = e->N, L = e->L, R = e->R, Tz = T;
+    o.audio = take(B * N * sizeof(int));
+    o.logp = take(B * N * sizeof(float));
+    o.bad = take(sizeof(unsigned long long));
+    o.lh = take(Tz * L * B * 2 * R * sizeof(float));
+    o.xh = take(wn_score_xh_offset(e->L, e->L, e->maxDil, T, e->B, e->R) * sizeof(__half));
+    o.xf = take(Tz * B * R * sizeof(float));
+    o.H = take(Tz * B * L * R * sizeof(__half));
+    o.lgt = take(Tz * B * e->A * sizeof(float));
+    o.bytes = off;
+    return o;
 }
 
 }  // namespace
@@ -293,7 +335,7 @@ int nvwn_destroy(nvwn_engine* e)
 {
     if (!e) return 0;
     void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
-                    e->Zs, e->Za, e->P, e->stage_dev, e->tc_image, e->trace, e->lut_f, e->cp_scratch};
+                    e->Zs, e->Za, e->P, e->stage_dev, e->tc_image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
@@ -305,7 +347,7 @@ int nvwn_set_embeddings(nvwn_engine* e, const float* embedPrev, const float* emb
     int rc;
     if ((rc = upload(e, e->blob + e->o_embPrev, embedPrev, (size_t)e->A * e->R))) return rc;
     if ((rc = upload(e, e->blob + e->o_embCur, embedCur, (size_t)e->A * e->R))) return rc;
-    e->tc_dirty = true;
+    e->tc_dirty = e->score_dirty = true;
     CK(cudaStreamSynchronize(0));
     return 0;
 }
@@ -324,7 +366,7 @@ int nvwn_set_layer_weights(nvwn_engine* e, int layer, const float* Wprev, const 
     if ((rc = upload(e, e->blob + e->o_Bres + l * R * td, Bres, R))) return rc;
     if ((rc = upload(e, e->blob + e->o_Wskip + l * S * R * td, Wskip, S * R))) return rc;
     if ((rc = upload(e, e->blob + e->o_Bskip + l * S * td, Bskip, S))) return rc;
-    e->tc_dirty = true;
+    e->tc_dirty = e->score_dirty = true;
     CK(cudaStreamSynchronize(0));       // sources may be freed by the caller right after return
     return 0;
 }
@@ -338,7 +380,7 @@ int nvwn_set_out_weights(nvwn_engine* e, const float* Wzs, const float* Bzs, con
     if ((rc = upload(e, e->blob + e->o_Bzs, Bzs, A))) return rc;
     if ((rc = upload(e, e->blob + e->o_Wza, Wza, A * A))) return rc;
     if ((rc = upload(e, e->blob + e->o_Bza, Bza, A))) return rc;
-    e->tc_dirty = true;
+    e->tc_dirty = e->score_dirty = true;
     CK(cudaStreamSynchronize(0));
     return 0;
 }
@@ -525,7 +567,7 @@ int nvwn_weight_blob(nvwn_engine* e, void** dev_ptr, unsigned long long* bytes)
 int nvwn_weights_updated(nvwn_engine* e)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_weights_updated: NULL engine");
-    e->tc_dirty = true;
+    e->tc_dirty = e->score_dirty = true;
     return 0;
 }
 
@@ -656,6 +698,97 @@ int nvwn_get_audio(nvwn_engine* e, float* audio_f32, short* audio_i16, int offse
     return 0;
 }
 
+int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size, float* logp, float* logits, void* stream_)
+{
+    if (!e || !audio || !logp) return fail(NVWN_EINVAL, "nvwn_score: NULL engine, audio or logp");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, "nvwn_score: only NVWN_FP16 engines can score");
+    if (e->A != 256) return fail(NVWN_EUNSUPPORTED, "nvwn_score: scoring needs A = 256");
+    if (batch_size < 1 || batch_size > e->B) return fail(NVWN_EINVAL, "nvwn_score: batch_size outside [1, B]");
+    if (num_samples < 1 || num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_score: num_samples outside [1, N]");
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int Bs = batch_size, N = num_samples, L = e->L, R = e->R, A = e->A;
+    if (!e->score_scratch) {
+        int T = SCORE_ROWS / e->B;
+        if (T < 1) T = 1;
+        if (T > e->N) T = e->N;
+        const ScoreScratch o = score_scratch_layout(e, T);
+        CK(cudaMalloc((void**)&e->score_scratch, o.bytes));
+        cudaError_t ce = cudaMalloc(&e->score_image, wn_score_image_bytes(R, e->S, A, L));
+        if (ce != cudaSuccess) { cudaFree(e->score_scratch); e->score_scratch = nullptr; CK(ce); }
+        e->score_T = T;
+        e->score_dirty = true;
+    }
+    const int T = e->score_T;
+    const ScoreScratch o = score_scratch_layout(e, T);
+    char* sc = e->score_scratch;
+    int* d_audio = reinterpret_cast<int*>(sc + o.audio);
+    unsigned long long* d_bad = reinterpret_cast<unsigned long long*>(sc + o.bad);
+    __half* xh = reinterpret_cast<__half*>(sc + o.xh);
+
+    // the audio is outside input: range-check it on the device whatever memory it is in, and name the first offender
+    const size_t n_audio = (size_t)Bs * N;
+    CK(cudaMemcpyAsync(d_audio, audio, n_audio * sizeof(int), cudaMemcpyDefault, st));
+    CK(cudaMemsetAsync(d_bad, 0xff, sizeof(unsigned long long), st));
+    CK(wn_score_check_audio(d_audio, n_audio, A, d_bad, st));
+    unsigned long long bad = 0;
+    CK(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (bad != ~0ull) {
+        int v = 0;
+        CK(cudaMemcpy(&v, d_audio + bad, sizeof v, cudaMemcpyDeviceToHost));
+        return fail(NVWN_EINVAL, "nvwn_score: audio[" + std::to_string(bad / N) + "][" + std::to_string(bad % N) + "] = " + std::to_string(v) +
+                                     " is outside [0, " + std::to_string(A) + ")");
+    }
+    if (e->score_dirty) {
+        WnParams p;
+        fill_params(e, p, 0, 0, N, Bs, 0);
+        CK(wn_score_pack(e->score_image, p, st));
+        e->score_dirty = false;
+    }
+    const bool logp_dev = is_device_ptr(logp), logits_dev = logits && is_device_ptr(logits);
+    for (int l = 0; l < L; l++)              // x_l[t - d] = 0 for t < d
+        CK(cudaMemsetAsync(xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R), 0,
+                           (size_t)wn_score_dilation(l, e->maxDil) * Bs * R * sizeof(__half), st));
+    WnScoreChunk c;
+    c.L = L; c.R = R; c.S = e->S; c.A = A; c.maxDil = e->maxDil; c.tanhEmbed = e->tanhEmbed;
+    c.Bs = Bs; c.Be = e->B; c.N = N; c.Tcap = T;
+    c.image = e->score_image; c.embPrev = e->blob + e->o_embPrev; c.embCur = e->blob + e->o_embCur;
+    c.audio = d_audio;
+    c.lh = reinterpret_cast<const float*>(sc + o.lh);
+    c.xh = xh;
+    c.xf = reinterpret_cast<float*>(sc + o.xf);
+    c.H = reinterpret_cast<__half*>(sc + o.H);
+    c.logp = logp_dev ? logp : reinterpret_cast<float*>(sc + o.logp);
+    float* lgt = reinterpret_cast<float*>(sc + o.lgt);
+    for (int t0 = 0; t0 < N; t0 += T) {
+        const int Tc = N - t0 < T ? N - t0 : T;
+        CK(cond_readback(e, reinterpret_cast<float*>(sc + o.lh), t0, Tc, st));
+        c.t0 = t0; c.T = Tc;
+        c.logits = logits ? (logits_dev ? logits : lgt) : nullptr;
+        c.logits_ld = logits_dev ? (long long)N * A : (long long)Tc * A;
+        c.logits_t0 = logits_dev ? 0 : t0;
+        CK(wn_score_chunk(c, st));
+        if (logits && !logits_dev)
+            CK(cudaMemcpy2DAsync(logits + (size_t)t0 * A, (size_t)N * A * sizeof(float), lgt, (size_t)Tc * A * sizeof(float),
+                                 (size_t)Tc * A * sizeof(float), Bs, cudaMemcpyDeviceToHost, st));
+        if (t0 + Tc < N) {
+            // carry the last d_l steps of every layer's input to the front of its buffer, in pieces that do not overlap
+            const size_t piece = (size_t)Tc * Bs;
+            for (int l = 0; l < L; l++) {
+                __half* buf = xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R);
+                const size_t hist = (size_t)wn_score_dilation(l, e->maxDil) * Bs;
+                for (size_t done = 0; done < hist; done += piece) {
+                    const size_t m = hist - done < piece ? hist - done : piece;
+                    CK(cudaMemcpyAsync(buf + done * R, buf + (piece + done) * R, m * R * sizeof(__half), cudaMemcpyDeviceToDevice, st));
+                }
+            }
+        }
+    }
+    if (!logp_dev) CK(cudaMemcpyAsync(logp, c.logp, n_audio * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (!logp_dev || (logits && !logits_dev)) CK(cudaStreamSynchronize(st));
+    return 0;
+}
+
 // debug only (not part of the public ABI): the engine's conditioning store for samples [first_sample, first_sample + num_samples),
 // converted back to fp32 [num_samples][L][B][2R] whatever the kernel-native layout (plain / tiled fp16 / fragment order) is
 int nvwn_debug_get_conditioning(nvwn_engine* e, float* out, int first_sample, int num_samples)
@@ -666,11 +799,7 @@ int nvwn_debug_get_conditioning(nvwn_engine* e, float* out, int first_sample, in
     if (n == 0) return 0;
     float* tmp = nullptr;
     CK(cudaMalloc((void**)&tmp, n * sizeof(float)));
-    cudaError_t ce;
-    if (e->lat_mode) ce = wn_lat_cond_readback(tmp, e->Lh, first_sample, num_samples, e->L, e->B, 0);
-    else if (e->tc_mode) ce = wn_tc_cond_readback(tmp, e->Lh, first_sample, num_samples, e->tc_tile, e->L, e->B, 0);
-    else if (e->dtype == NVWN_FP16) ce = wn_f16_to_f32(tmp, static_cast<const __half*>(e->Lh) + (size_t)first_sample * per, n, 0);
-    else ce = cudaMemcpyAsync(tmp, static_cast<const float*>(e->Lh) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, 0);
+    cudaError_t ce = cond_readback(e, tmp, first_sample, num_samples, 0);
     if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
     cudaFree(tmp);
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_conditioning: ") + cudaGetErrorString(ce));

@@ -183,6 +183,29 @@ class NVWavenetInfer:
                                      _stream(stream)), "getAudio")
         return out
 
+    # ---- teacher-forced scoring (nvwn_score) ----
+    def score(self, audio, num_samples=None, batch_size=None, logits=False, stream=None):
+        """Log-likelihood of given audio under the engine's fp16 model: logp[b][t] = log softmax(Za_t)[audio[b][t]], with
+        audio[b][0..t) fed back and the conditioning already in the engine.  `audio`: int [batch][samples] numpy array
+        (numpy results) or CUDA tensor (CUDA tensors, filled asynchronously on `stream`).  Returns logp [batch_size][num_samples],
+        or (logp, logits [batch_size][num_samples][A]) with logits=True.  The generation state is left untouched."""
+        n = audio.shape[1] if num_samples is None else num_samples
+        bs = audio.shape[0] if batch_size is None else batch_size
+        if hasattr(audio, "is_cuda") and audio.is_cuda:
+            import torch
+            a = audio[:bs, :n].to(torch.int32).contiguous()
+            lp = torch.empty((bs, n), dtype=torch.float32, device=audio.device)
+            lg = torch.empty((bs, n, self.A), dtype=torch.float32, device=audio.device) if logits else None
+            ptrs = (a.data_ptr(), lp.data_ptr(), lg.data_ptr() if logits else None)
+        else:
+            a = np.ascontiguousarray(np.asarray(audio)[:bs, :n], dtype=np.int32)
+            lp = np.empty((bs, n), np.float32)
+            lg = np.empty((bs, n, self.A), np.float32) if logits else None
+            ptrs = (a.ctypes.data, lp.ctypes.data, lg.ctypes.data if logits else None)
+        check(self._l.nvwn_score(self._h, C.c_void_p(ptrs[0]), n, bs, C.c_void_p(ptrs[1]),
+                                 None if ptrs[2] is None else C.c_void_p(ptrs[2]), _stream(stream)), "score")
+        return (lp, lg) if logits else lp
+
     # ---- run (nv_wavenet.cuh:445-639) ----
     def run_partial(self, init_sample, num_samples, batch_size, y_out=None, batch_size_per_block=1,
                     dump_activations=False, stream=None):

@@ -136,3 +136,18 @@ class NVWaveNet:
         eng.run(sample_count, batch_size, samples, dump_activations=False)
         torch.cuda.synchronize()
         return samples
+
+    def log_likelihood(self, cond_input, audio):
+        """Per-sample log-likelihood of `audio` (int mu-law codes [batch][samples]) given `cond_input` (channels x batch x
+        num_layers x samples, as for infer()): log p(audio[b][t] | audio[b][0..t), conditioning) under the fp16 engine of that
+        size, all steps at once.  Returns a float32 CUDA tensor [batch][samples]."""
+        if (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
+            raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
+        batch_size, sample_count = cond_input.size(1), cond_input.size(3)
+        if tuple(audio.size()) != (batch_size, sample_count):
+            raise AssertionError(f"audio must be [batch][samples] = {(batch_size, sample_count)}; got {tuple(audio.size())}")
+        eng = self._engine(batch_size, sample_count, True)
+        eng.set_conditioning(column_major(cond_input).float(), 0, sample_count)
+        logp = eng.score(audio.to(device="cuda", dtype=torch.int32))
+        torch.cuda.synchronize()
+        return logp
