@@ -21,7 +21,10 @@
 //   Lh (the only HBM stream), biases and the dilated history x[t-d] are prefetched into registers one / two layers ahead.
 //
 // wn_lat2_kernel (second half of this file, the default up to ~720 utterances) spreads the same data flow over a cluster of three
-// CTAs per tile -- chain / tail / prep -- that hand tiles over through distributed shared memory; see the comment there.
+// CTAs per tile -- chain / tail / prep -- that hand tiles over through distributed shared memory; see the comment there.  The
+// K = 64 gate GEMM (except the chain CTA's Wcur.x), the gate, the residual GEMM and update with the x-tile / history-ring store, the xtOut dump, the relu(skip + Bskip)
+// packing and the final index store are defined once ("stages of both latency kernels") and called by both, with the trace
+// points between the calls; the mbarrier / bulk-TMA wrappers come from wn_sm90.cuh.
 //
 // Replaces nv_wavenet_{singleblock,dualblock,persistent}.cuh + matrix_math.cuh + softmax.cuh of the reference for
 // T_data = half while the batch is small enough to be latency-bound.  Numerical contract: oracle/wavenet_oracle.c
@@ -143,12 +146,8 @@ __device__ __forceinline__ void ldg_nc_v4_if(uint4& d, const void* p, bool pred)
 }
 __device__ __forceinline__ void stg_v2(void* p, uint32_t a, uint32_t b) { asm volatile("st.global.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(a), "r"(b) : "memory"); }
 __device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, %0;" ::"n"(NCT) : "memory"); }
-__device__ __forceinline__ uint32_t pack_h2(float a, float b)
-{
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_h2(uint32_t v) { return __half22float2(*reinterpret_cast<__half2*>(&v)); }
+using wn::pack_h2;
+using wn::unpack_h2;
 __device__ __forceinline__ uint32_t u32(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 __device__ __forceinline__ __half2 h2(uint32_t v) { return *reinterpret_cast<__half2*>(&v); }
 
@@ -159,51 +158,6 @@ __device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) { asm volati
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait_pending() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-// mbarrier by shared-memory address
-__device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_arrive_a(uint32_t bar) { asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void mbar_expect_a(uint32_t bar, uint32_t bytes) { asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory"); }
-__device__ __forceinline__ bool mbar_try_a(uint32_t bar, uint32_t parity)
-{
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    return ok != 0;
-}
-// a look that never suspends the thread (try_wait parks it until a time limit when the phase is still running)
-__device__ __forceinline__ bool mbar_probe_a(uint32_t bar, uint32_t parity)
-{
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    return ok != 0;
-}
-// three looks issued back to back: their ~90-cycle latencies overlap
-__device__ __forceinline__ void mbar_try3_a(uint32_t b1, uint32_t p1, uint32_t b2, uint32_t p2, uint32_t b3, uint32_t p3, bool& o1, bool& o2, bool& o3)
-{
-    uint32_t r1, r2, r3;
-    asm volatile("{\n\t.reg .pred q1, q2, q3;\n\t"
-                 "mbarrier.try_wait.parity.shared::cta.b64 q1, [%3], %4;\n\t"
-                 "mbarrier.try_wait.parity.shared::cta.b64 q2, [%5], %6;\n\t"
-                 "mbarrier.try_wait.parity.shared::cta.b64 q3, [%7], %8;\n\t"
-                 "selp.u32 %0, 1, 0, q1;\n\tselp.u32 %1, 1, 0, q2;\n\tselp.u32 %2, 1, 0, q3;\n\t}"
-                 : "=r"(r1), "=r"(r2), "=r"(r3) : "r"(b1), "r"(p1), "r"(b2), "r"(p2), "r"(b3), "r"(p3) : "memory");
-    o1 = r1 != 0; o2 = r2 != 0; o3 = r3 != 0;
-}
-static __device__ __noinline__ void lat_timeout(uint32_t bar, uint32_t parity)
-{
-    printf("wn_lat: mbarrier wait timed out: block %d thread %d barrier@0x%x parity %u\n", blockIdx.x, threadIdx.x, bar, parity);
-    __trap();
-}
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity)
-{
-    uint32_t spins = 0;
-    while (!mbar_try_a(bar, parity))
-        if (++spins > (1u << 24)) lat_timeout(bar, parity);
-}
-__device__ __forceinline__ void tma_load_a(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
 
 // ------------------------------------------------------------------------------------------------ conditioning layout
 // fp16, [N][L][tiles][8 warps][32 lanes][16 B]: the uint4 of thread (w, lane = 4 g + t) holds, as half2 pairs of channels
@@ -332,8 +286,86 @@ __global__ void lat_pack_kernel(WnParams p, unsigned char* __restrict__ img, Lat
     }
 }
 
-// ------------------------------------------------------------------------------------------------ the kernel
+// ------------------------------------------------------------------------------------------------ stages of both latency kernels
+// Each stage is called by both wn_lat_kernel and wn_lat2_kernel.  Per thread of the eight compute warps: warp w, lane = 4 g + t4;
+// the thread holds rows g and g + 8 of the 16 utterances and channels 8 w + 2 t4 + {0, 1} of an activation tile (k-step w >> 1,
+// half w & 1 of its A fragments).
 struct StepIt { int t, l, slot; };       // coordinates of a layer step: sample, layer, history-ring slot of that sample
+
+// feedback state of the tile ([TU] current index, [TU] previous index) -> yCur / yPrev
+__device__ __forceinline__ void store_ys(const WnParams& p, int B, const int* ys, int tile, int tid)
+{
+    if (tid < TU && tile * TU + tid < B) { p.yCur[tile * TU + tid] = ys[tid]; p.yPrev[tile * TU + tid] = ys[TU + tid]; }
+}
+// this thread's four values of x (fp16) -> the x exchange tile and row `row` (= history slot x L + layer) of the history ring
+__device__ __forceinline__ void store_x(const float (&x)[4], uint32_t xtile, unsigned char* gring, uint32_t row, uint32_t rstride, int w)
+{
+    const uint32_t x01 = pack_h2(x[0], x[1]), x23 = pack_h2(x[2], x[3]);
+    sts64(xtile, x01, x23);
+    stg_v2(gring + (size_t)(row * rstride) + (w >> 1) * 512 + (w & 1) * 8, x01, x23);
+}
+// B fragments of warp w's gate columns for a K = 64 GEMM: tanh and sigmoid n-tiles, k-step pairs 0 and 1
+struct GateW { uint4 t0, g0, t1, g1; };
+__device__ __forceinline__ GateW lds_gate_w(uint32_t piece, uint32_t o_t0, uint32_t o_g0)
+{
+    return {lds128(piece + o_t0), lds128(piece + o_g0), lds128(piece + o_t0 + 512), lds128(piece + o_g0 + 512)};
+}
+// K = 64 gate GEMM (Wcur.x or Wprev.x[t-d]) as two independent chains: k-steps 0-1 into d, 2-3 into u ([0] tanh, [1] sigmoid)
+__device__ __forceinline__ void hmma_k64(float (&d)[2][4], float (&u)[2][4], const uint32_t (&a)[4][4], const GateW& b)
+{
+    hmma(d[0], a[0], b.t0.x, b.t0.y); hmma(d[1], a[0], b.g0.x, b.g0.y); hmma(u[0], a[2], b.t1.x, b.t1.y); hmma(u[1], a[2], b.g1.x, b.g1.y);
+    hmma(d[0], a[1], b.t0.z, b.t0.w); hmma(d[1], a[1], b.g0.z, b.g0.w); hmma(u[0], a[3], b.t1.z, b.t1.w); hmma(u[1], a[3], b.g1.z, b.g1.w);
+}
+__device__ __forceinline__ void gemm_k64(float (&d)[2][4], const uint32_t (&a)[4][4], const GateW& b)
+{
+    float u[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    hmma_k64(d, u, a, b);
+#pragma unroll
+    for (int i = 0; i < 4; i++) { d[0][i] += u[0][i]; d[1][i] += u[1][i]; }
+}
+// h = tanh(a[:R]) * sigmoid(a[R:]) in packed fp16 (MUFU; sigmoid(x) = 0.5 tanh(x/2) + 0.5) -> the h tile; returns the two words
+__device__ __forceinline__ void gate(const float (&a)[2][4], uint32_t htile, uint32_t& h01, uint32_t& h23)
+{
+    const __half2 half = __floats2half2_rn(0.5f, 0.5f);
+    const __half2 tg0 = wn::tanh_h2(h2(pack_h2(a[0][0], a[0][1]))), tg1 = wn::tanh_h2(h2(pack_h2(a[0][2], a[0][3])));
+    const __half2 sg0 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * a[1][0], 0.5f * a[1][1]))), half, half);
+    const __half2 sg1 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * a[1][2], 0.5f * a[1][3]))), half, half);
+    h01 = u32(__hmul2(tg0, sg0)); h23 = u32(__hmul2(tg1, sg1));
+    sts64(htile, h01, h23);
+}
+// Wres.h as two half-K chains (B fragments bw0, bw1 of k-step pairs 0 and 1)
+__device__ __forceinline__ void hmma_res(float (&ra)[4], float (&rb)[4], const uint32_t (&ha)[4][4], uint4 bw0, uint4 bw1)
+{
+    hmma(ra, ha[0], bw0.x, bw0.y); hmma(rb, ha[2], bw1.x, bw1.y);
+    hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
+}
+// x' = ((ra + rb) + Bres) + x; below the last layer x' goes to the x tile and history ring row `row`
+__device__ __forceinline__ void residual(float (&x)[4], const float (&ra)[4], const float (&rb)[4], float2 br, bool store, uint32_t xtile,
+                                         unsigned char* gring, uint32_t row, uint32_t rstride, int w)
+{
+    x[0] = ((ra[0] + rb[0]) + br.x) + x[0]; x[1] = ((ra[1] + rb[1]) + br.y) + x[1];
+    x[2] = ((ra[2] + rb[2]) + br.x) + x[2]; x[3] = ((ra[3] + rb[3]) + br.y) + x[3];
+    if (store) store_x(x, xtile, gring, row, rstride, w);
+}
+template <bool DUMP>
+__device__ __forceinline__ void dump_xt(const WnParams& p, int B, int l, int b0, int b1, int cw, const float (&x)[4])
+{
+    if (DUMP) {
+        if (b0 < B) { p.xtOut[((size_t)l * B + b0) * R + cw] = x[0]; p.xtOut[((size_t)l * B + b0) * R + cw + 1] = x[1]; }
+        if (b1 < B) { p.xtOut[((size_t)l * B + b1) * R + cw] = x[2]; p.xtOut[((size_t)l * B + b1) * R + cw + 1] = x[3]; }
+    }
+}
+// relu(skip + Bskip) of one skip n-tile (columns c, c + 1), packed as A-fragment words of rows g and g + 8; the sum restarts at 0
+__device__ __forceinline__ void relu_skip(float (&sk)[4], const float* bskip, int c, uint32_t& lo, uint32_t& hi)
+{
+    const float b0f = bskip[c], b1f = bskip[c + 1];
+    lo = pack_h2(fmaxf(sk[0] + b0f, 0.f), fmaxf(sk[1] + b1f, 0.f));
+    hi = pack_h2(fmaxf(sk[2] + b0f, 0.f), fmaxf(sk[3] + b1f, 0.f));
+    sk[0] = sk[1] = sk[2] = sk[3] = 0.f;
+}
+
+
+// ------------------------------------------------------------------------------------------------ the kernel
 
 // DUMP: write the last-sample activations (the host runs the final sample of a dumping launch with this variant).
 // TRC:  record the clock64 timeline (debug; tools/lat_trace.py).
@@ -366,8 +398,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
 #define TRACE(role, tag) do { if (TRC && trc && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
 
     if (tid == 0) {
-        for (int i = 0; i < 4; i++) { mbar_init_a(s_full + 8 * i, 1); mbar_init_a(s_empty + 8 * i, NCW); }
-        for (int i = 0; i < 3; i++) mbar_init_a(s_pfull + 8 * i, 128);
+        for (int i = 0; i < 4; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
+        for (int i = 0; i < 3; i++) mbar_init(s_pfull + 8 * i, 128);
         fence_mbar_init();
         int d = 1;                                     // dilation of layer l (nv_wavenet.cuh:99-111): 1,2,4..maxDil,1,2,...
         for (int l = 0; l < L; l++) { dil[l] = d; d <<= 1; if (d > p.maxDil) d = 1; }
@@ -394,9 +426,9 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             auto put = [&](const unsigned char* src, uint32_t bytes) {
                 const uint32_t idx = (pc >> 1) & 1, bo = ((pc & 1) * 2 + idx) * 8;
                 const uint32_t dst = (pc & 1) ? sm + C::O_RING2 + idx * C::SLOT2 : sm + C::O_RING1 + idx * C::SLOT1;
-                mbar_wait_a(s_empty + bo, ((pc >> 2) & 1) ^ 1);
-                mbar_expect_a(s_full + bo, bytes);
-                tma_load_a(dst, src, bytes, s_full + bo);
+                mbar_wait(s_empty + bo, ((pc >> 2) & 1) ^ 1);
+                mbar_arrive_expect_tx(s_full + bo, bytes);
+                tma_load_1d(dst, src, bytes, s_full + bo);
                 pc++;
             };
             for (int t = t_begin; t < t_end; t++) {
@@ -432,12 +464,12 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
         const uint32_t o_out = (uint32_t)(4 * w) * 512;                                                         // output pieces: x OJP, + lane16
 
         auto advance = [&](StepIt& it) { if (++it.l == L) { it.l = 0; it.t++; if (++it.slot == slots) it.slot = 0; } };
-        auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive_a(bar); };
+        auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
         // Every mbarrier wait costs ~90 cycles even when the phase completed long ago (TRYWAIT latency).  The barriers of the coming
         // step are therefore looked at once, at the end of the running step (measured: 40.1 kHz at C3 B=64 against 38.4 kHz with
         // plain waits at the point of use, and 35.9 kHz with blocking waits moved behind the preceding HMMA batches).
-        auto probe = [&](uint32_t bar, uint32_t parity) -> bool { return mbar_try_a(bar, parity); };
-        auto ensure = [&](bool ok, uint32_t bar, uint32_t parity) { if (!ok) mbar_wait_a(bar, parity); };
+        auto probe = [&](uint32_t bar, uint32_t parity) -> bool { return mbar_try_wait(bar, parity); };
+        auto ensure = [&](bool ok, uint32_t bar, uint32_t parity) { if (!ok) mbar_wait(bar, parity); };
 
         // dilated history x_l[t - d] (zero before the start of the utterance, nv_wavenet.cuh:106) of the step `itp`: staged three
         // steps ahead into a 3-slot shared-memory ring by warps 0-3 (128 threads x 16 B, cp.async; completion on an mbarrier)
@@ -450,7 +482,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
                 const uint32_t dst = sm + C::O_PST + slot3 * 2048 + (uint32_t)(w * 32 + lane) * 16;
                 if (itp.t >= t_end || itp.t < d) {
                     sts128(dst, make_uint4(0, 0, 0, 0));
-                    mbar_arrive_a(s_pfull + 8 * slot3);
+                    mbar_arrive(s_pfull + 8 * slot3);
                 } else {
                     int sl = itp.slot - d; if (sl < 0) sl += slots;
                     cp_async16(dst, gring - lane16 + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
@@ -487,23 +519,18 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             }
             const uint32_t slot3 = pn % 3;
             if (it1.t < t_end) {
-                uint4 bt0, bg0, bt1, bg1;
+                GateW bw;
                 if (from_global) {
                     const unsigned char* gp = img + (size_t)(L - 1) * im.layer_bytes + C::W_PREV;
-                    bt0 = ldg_nc_v4(gp + o_t0); bg0 = ldg_nc_v4(gp + o_g0); bt1 = ldg_nc_v4(gp + o_t0 + 512); bg1 = ldg_nc_v4(gp + o_g0 + 512);
+                    bw = {ldg_nc_v4(gp + o_t0), ldg_nc_v4(gp + o_g0), ldg_nc_v4(gp + o_t0 + 512), ldg_nc_v4(gp + o_g0 + 512)};
                 } else {
-                    bt0 = lds128(p1 + C::W_PREV + o_t0); bg0 = lds128(p1 + C::W_PREV + o_g0);
-                    bt1 = lds128(p1 + C::W_PREV + o_t0 + 512); bg1 = lds128(p1 + C::W_PREV + o_g0 + 512);
+                    bw = lds_gate_w(p1 + C::W_PREV, o_t0, o_g0);
                 }
                 ensure(pf_ok, s_pfull + 8 * slot3, (pn / 3) & 1);
                 uint32_t pb[4][4];
 #pragma unroll
                 for (int j = 0; j < 4; j++) load_a(pb[j], sm + C::O_PST + slot3 * 2048 + j * 512 + lane16);
-                float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};         // second half of K: independent chains
-                hmma(accp[0], pb[0], bt0.x, bt0.y); hmma(accp[1], pb[0], bg0.x, bg0.y); hmma(u0, pb[2], bt1.x, bt1.y); hmma(u1, pb[2], bg1.x, bg1.y);
-                hmma(accp[0], pb[1], bt0.z, bt0.w); hmma(accp[1], pb[1], bg0.z, bg0.w); hmma(u0, pb[3], bt1.z, bt1.w); hmma(u1, pb[3], bg1.z, bg1.w);
-#pragma unroll
-                for (int i = 0; i < 4; i++) { accp[0][i] += u0[i]; accp[1][i] += u1[i]; }
+                gemm_k64(accp, pb, bw);
             }
             pn++;
             {   // ... and refills it with the conditioning of step k + 3
@@ -549,21 +576,11 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             const float2 br = brn;
             // ---- a = Wcur.x + [Wprev.x[t-d] + Bh + Lh]   (nv_wavenet.cuh:131-157); the two halves of K as independent chains
             ensure(ok_f1, f1, fph);
+            gemm_k64(accp, xa, lds_gate_w(p1, o_t0, o_g0));
+            // ---- h = tanh(a[:R]) * sigmoid(a[R:])
             {
-                const uint4 bt0 = lds128(p1 + o_t0), bg0 = lds128(p1 + o_g0), bt1 = lds128(p1 + o_t0 + 512), bg1 = lds128(p1 + o_g0 + 512);
-                float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
-                hmma(accp[0], xa[0], bt0.x, bt0.y); hmma(accp[1], xa[0], bg0.x, bg0.y); hmma(u0, xa[2], bt1.x, bt1.y); hmma(u1, xa[2], bg1.x, bg1.y);
-                hmma(accp[0], xa[1], bt0.z, bt0.w); hmma(accp[1], xa[1], bg0.z, bg0.w); hmma(u0, xa[3], bt1.z, bt1.w); hmma(u1, xa[3], bg1.z, bg1.w);
-#pragma unroll
-                for (int i = 0; i < 4; i++) { accp[0][i] += u0[i]; accp[1][i] += u1[i]; }
-            }
-            // ---- h = tanh(a[:R]) * sigmoid(a[R:])   (packed fp16 MUFU; sigmoid(x) = 0.5 tanh(x/2) + 0.5)
-            {
-                const __half2 half = __floats2half2_rn(0.5f, 0.5f);
-                const __half2 tg0 = wn::tanh_h2(h2(pack_h2(accp[0][0], accp[0][1]))), tg1 = wn::tanh_h2(h2(pack_h2(accp[0][2], accp[0][3])));
-                const __half2 sg0 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * accp[1][0], 0.5f * accp[1][1]))), half, half);
-                const __half2 sg1 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * accp[1][2], 0.5f * accp[1][3]))), half, half);
-                sts64(sm + C::O_HBUF + xchg, u32(__hmul2(tg0, sg0)), u32(__hmul2(tg1, sg1)));
+                uint32_t h01, h23;
+                gate(accp, sm + C::O_HBUF + xchg, h01, h23);
             }
             if (tid == 0) TRACE(0, 12);
             // ---- while the other warps finish their part of h: the dilated-history half of the next step's pre-activation
@@ -580,21 +597,11 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             ensure(ok_f2, f2, fph);
             {
                 const uint4 bw0 = lds128(p2 + o_res), bw1 = lds128(p2 + o_res + 512);
-                hmma(ra, ha[0], bw0.x, bw0.y); hmma(rb, ha[2], bw1.x, bw1.y);
-                hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
+                hmma_res(ra, rb, ha, bw0, bw1);
             }
-            xres[0] = ((ra[0] + rb[0]) + br.x) + xres[0]; xres[1] = ((ra[1] + rb[1]) + br.y) + xres[1];
-            xres[2] = ((ra[2] + rb[2]) + br.x) + xres[2]; xres[3] = ((ra[3] + rb[3]) + br.y) + xres[3];
-            if (l + 1 < L) {
-                const uint32_t x01 = pack_h2(xres[0], xres[1]), x23 = pack_h2(xres[2], xres[3]);
-                sts64(sm + C::O_XBUF + xchg, x01, x23);
-                stg_v2(gring + (size_t)((uint32_t)(it0.slot * L + l + 1) * rstride) + jw * 512 + hw * 8, x01, x23);
-            }
+            residual(xres, ra, rb, br, l + 1 < L, sm + C::O_XBUF + xchg, gring, (uint32_t)(it0.slot * L + l + 1), rstride, w);
             if (tid == 0) TRACE(0, 14);
-            if (DUMP) {
-                if (v0) { p.xtOut[((size_t)l * B + b0) * R + cw] = xres[0]; p.xtOut[((size_t)l * B + b0) * R + cw + 1] = xres[1]; }
-                if (v1) { p.xtOut[((size_t)l * B + b1) * R + cw] = xres[2]; p.xtOut[((size_t)l * B + b1) * R + cw + 1] = xres[3]; }
-            }
+            dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
             // ---- while the other warps finish their part of x': skip += Wskip.h   (biases are added once, after the last layer)
 #pragma unroll
             for (int jp = 0; jp < 2; jp++) {
@@ -610,7 +617,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             stage_history();                           // the history tile of three steps ahead
             {   // look at the coming step's barriers now; the answers are consumed a barrier later
                 const uint32_t nsb = sb ^ 1, nph = fph ^ sb;
-                mbar_try3_a(s_full + nsb * 8, nph, s_full + 16 + nsb * 8, nph, s_pfull + 8 * (pn % 3), (pn / 3) & 1, ok_f1, ok_f2, ok_pf);
+                mbar_try_wait3(s_full + nsb * 8, nph, s_full + 16 + nsb * 8, nph, s_pfull + 8 * (pn % 3), (pn / 3) & 1, ok_f1, ok_f2, ok_pf);
             }
             if (tid == 0) TRACE(0, 15);
             if (DUMP) {
@@ -670,11 +677,10 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
 #pragma unroll
             for (int i = 0; i < C::NSK; i++) {
-                const int nt = w * C::NSK + i, c = 8 * nt + 2 * t4;
-                const float b0f = s_bout[c], b1f = s_bout[c + 1];
-                sts64(sm + C::O_OB0 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8,
-                      pack_h2(fmaxf(sk[i][0] + b0f, 0.f), fmaxf(sk[i][1] + b1f, 0.f)), pack_h2(fmaxf(sk[i][2] + b0f, 0.f), fmaxf(sk[i][3] + b1f, 0.f)));
-                sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
+                const int nt = w * C::NSK + i;
+                uint32_t lo, hi;
+                relu_skip(sk[i], s_bout, 8 * nt + 2 * t4, lo, hi);
+                sts64(sm + C::O_OB0 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8, lo, hi);
             }
             bar_compute();
             if (tid == 0) TRACE(0, 20);
@@ -688,7 +694,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             auto out_gemm = [&](const int q, const int ojp, const uint32_t abuf, const int kp0) {
                 const uint32_t idx = sb ^ ((q >> 1) & 1), bo = ((q & 1) * 2 + idx) * 8;
                 const uint32_t st = ((q & 1) ? sm + C::O_RING2 + idx * C::SLOT2 : sm + C::O_RING1 + idx * C::SLOT1) + o_out * ojp + lane16;
-                mbar_wait_a(s_full + bo, fph ^ (((sb + (q >> 1)) >> 1) & 1));
+                mbar_wait(s_full + bo, fph ^ (((sb + (q >> 1)) >> 1) & 1));
                 for (int jp = 0; jp < ojp; jp++) {
                     uint32_t a0[4], a1[4];
                     load_a(a0, abuf + ((kp0 + jp) * 2) * 512 + lane16);
@@ -811,7 +817,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             if (++it0.slot == slots) it0.slot = 0;
             it0.t++;
         }
-        if (tid < TU && tile * TU + tid < B) { p.yCur[tile * TU + tid] = ys[tid]; p.yPrev[tile * TU + tid] = ys[TU + tid]; }
+        store_ys(p, B, ys, tile, tid);
     }
 #undef TRACE
 }
@@ -833,8 +839,6 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
 // indices (once per sample, tail -> chain); once per sample for the output layers: relu(skip + Bskip) (S x 32 B, tail -> prep),
 // the relu(Zs) halves (4 KB each way, tail <-> prep) and the prep's logits half (8 KB fp32, prep -> tail).  Each CTA moves less than
 // ~100 KB per step through its shared memory; a single CTA doing all of it moves ~190 KB per step and is bound by that.
-constexpr int NTC = NCT + 32;
-
 template <int S>
 struct CfgC {
     using C = Cfg<S>;
@@ -915,7 +919,7 @@ __device__ __forceinline__ void cluster_sync_all()
 }
 
 template <int S, bool DUMP, bool TRC>
-__global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
+__global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
 {
     // debug timeline (tools/lat_trace.py): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
     unsigned long long* trc = (TRC && p.trace && blockIdx.x < NCL) ? p.trace : nullptr;
@@ -950,20 +954,20 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     int* ys = reinterpret_cast<int*>(smem_raw + M::O_YS);
 
     if (tid == 0) {
-        for (int i = 0; i < 4; i++) { mbar_init_a(s_full + 8 * i, 1); mbar_init_a(s_empty + 8 * i, NCW); }
-        for (int i = 0; i < M::NPS; i++) mbar_init_a(s_pfull + 8 * i, 128);
-        for (int i = 0; i < 2; i++) { mbar_init_a(s_hfull + 8 * i, 1); mbar_init_a(s_hfree + 8 * i, NCW); }
-        for (int i = 0; i < M::NAP; i++) { mbar_init_a(s_apfull + 8 * i, 1); mbar_init_a(s_apfree + 8 * i, NCW); }
-        mbar_init_a(s_yfull, 1);
-        mbar_init_a(s_ob0full, 1); mbar_init_a(s_ob0free, NCW); mbar_init_a(s_ob1full, 1); mbar_init_a(s_ob1free, 2 * NCW);
-        mbar_init_a(s_lfull, 1); mbar_init_a(s_lfree, NCW);
+        for (int i = 0; i < 4; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
+        for (int i = 0; i < M::NPS; i++) mbar_init(s_pfull + 8 * i, 128);
+        for (int i = 0; i < 2; i++) { mbar_init(s_hfull + 8 * i, 1); mbar_init(s_hfree + 8 * i, NCW); }
+        for (int i = 0; i < M::NAP; i++) { mbar_init(s_apfull + 8 * i, 1); mbar_init(s_apfree + 8 * i, NCW); }
+        mbar_init(s_yfull, 1);
+        mbar_init(s_ob0full, 1); mbar_init(s_ob0free, NCW); mbar_init(s_ob1full, 1); mbar_init(s_ob1free, 2 * NCW);
+        mbar_init(s_lfull, 1); mbar_init(s_lfree, NCW);
         fence_mbar_init();
         // transaction barriers are armed by their owner one phase ahead: the tail expects 2 KB per h tile, the chain 128 B of indices
         // and 8 KB per pre-activation tile; once per sample the prep expects relu(skip) and a relu(Zs) half, the tail a relu(Zs) half
         // and the logits half
-        if (is_chain) { mbar_expect_a(s_yfull, 2 * TU * 4); for (int i = 0; i < M::NAP; i++) mbar_expect_a(s_apfull + 8 * i, 8192); }
-        else if (is_tail) { mbar_expect_a(s_hfull, 2048); mbar_expect_a(s_hfull + 8, 2048); mbar_expect_a(s_ob1full, TU * 128 * 2); mbar_expect_a(s_lfull, TU * 128 * 4); }
-        else { mbar_expect_a(s_ob0full, TU * S * 2); mbar_expect_a(s_ob1full, TU * 128 * 2); }
+        if (is_chain) { mbar_arrive_expect_tx(s_yfull, 2 * TU * 4); for (int i = 0; i < M::NAP; i++) mbar_arrive_expect_tx(s_apfull + 8 * i, 8192); }
+        else if (is_tail) { mbar_arrive_expect_tx(s_hfull, 2048); mbar_arrive_expect_tx(s_hfull + 8, 2048); mbar_arrive_expect_tx(s_ob1full, TU * 128 * 2); mbar_arrive_expect_tx(s_lfull, TU * 128 * 4); }
+        else { mbar_arrive_expect_tx(s_ob0full, TU * S * 2); mbar_arrive_expect_tx(s_ob1full, TU * 128 * 2); }
     }
     if (tid < TU) {
         const int b = tile * TU + tid;
@@ -972,18 +976,18 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     }
     if (is_chain) {
         const uint32_t* ec = static_cast<const uint32_t*>(p.embCur);
-        for (int i = tid; i < A * 32; i += NTC) sts32(sm + M::C_EMB + ((i >> 5) * EROW + (i & 31)) * 4, ec[i]);
-        for (int i = tid; i < L * 256; i += NTC) sts32(sm + M::C_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + i]));
+        for (int i = tid; i < A * 32; i += NT) sts32(sm + M::C_EMB + ((i >> 5) * EROW + (i & 31)) * 4, ec[i]);
+        for (int i = tid; i < L * 256; i += NT) sts32(sm + M::C_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + i]));
     } else if (is_tail) {
         float* s_bout = reinterpret_cast<float*>(smem_raw + M::T_BOUT);
-        for (int i = tid; i < S; i += NTC) s_bout[i] = gbias[im.b_skpre + (size_t)(L - 1) * S + i];
-        for (int i = tid; i < A; i += NTC) { s_bout[S + i] = gbias[im.b_bzs + i]; s_bout[S + A + i] = gbias[im.b_bza + i]; }
+        for (int i = tid; i < S; i += NT) s_bout[i] = gbias[im.b_skpre + (size_t)(L - 1) * S + i];
+        for (int i = tid; i < A; i += NT) { s_bout[S + i] = gbias[im.b_bzs + i]; s_bout[S + A + i] = gbias[im.b_bza + i]; }
     } else {
         int* dil = reinterpret_cast<int*>(smem_raw + M::P_DIL);
         if (tid == 0) { int d = 1; for (int l = 0; l < L; l++) { dil[l] = d; d <<= 1; if (d > p.maxDil) d = 1; } }   // nv_wavenet.cuh:99-111
-        for (int i = tid; i < L * 128; i += NTC) sts32(sm + M::P_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + (i >> 2) * 8 + (i & 3)]));
+        for (int i = tid; i < L * 128; i += NT) sts32(sm + M::P_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + (i >> 2) * 8 + (i & 3)]));
         float* s_bout = reinterpret_cast<float*>(smem_raw + M::P_BOUT);
-        for (int i = tid; i < A; i += NTC) { s_bout[i] = gbias[im.b_bzs + i]; s_bout[A + i] = gbias[im.b_bza + i]; }
+        for (int i = tid; i < A; i += NT) { s_bout[i] = gbias[im.b_bzs + i]; s_bout[A + i] = gbias[im.b_bza + i]; }
     }
     __syncthreads();
     cluster_sync_all();                                    // every CTA's barriers are initialised before anybody signals a peer
@@ -994,7 +998,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     const uint32_t lane16 = (uint32_t)lane * 16;
     const int jw = w >> 1, hw = w & 1;
     const uint32_t xchg = (uint32_t)(jw * 512 + hw * 8) + lane16;
-    auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive_a(bar); };
+    auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
     auto release_remote = [&](uint32_t local_bar, uint32_t rank) { __syncwarp(); if (lane == 0) mbar_arrive_remote(mapa_u32(local_bar, rank)); };
 
     // ---------------- output layers, tail (half 0) and prep (half 1) CTAs: n-tiles 16 half + 2w and 16 half + 2w + 1 of Zs and Za.
@@ -1039,7 +1043,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
 #pragma unroll
                 for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
         };
-        if (half) { load_za(); mbar_wait_a(s_ob0full, par); }
+        if (half) { load_za(); mbar_wait(s_ob0full, par); }
 #pragma unroll
         for (int jp = 0; jp < S / 32; jp++) {
             uint32_t a0[4], a1[4];
@@ -1052,7 +1056,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
         }
         if (!half) load_za();
         if (half) {                                    // OB0 has been read: arm its barrier for the next sample, then free it
-            if (tid == 0) mbar_expect_a(s_ob0full, TU * S * 2);
+            if (tid == 0) mbar_arrive_expect_tx(s_ob0full, TU * S * 2);
             release_remote(s_ob0free, 1);
         }
         TRACE2(crank, 24);
@@ -1071,12 +1075,12 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
         {   // both CTAs' warps have read the previous sample's OB1
             const uint32_t o = (8 * half + w) * 512 + lane16;
             const uint4 v = make_uint4(zp[0], zp[1], zp[2], zp[3]);
-            mbar_wait_a(s_ob1free, par ^ 1);
+            mbar_wait(s_ob1free, par ^ 1);
             sts128(ob1 + o, v);
             st_async_v4(mapa_u32(sm + (half ? M::T_OB1 : M::P_OB1) + o, peer), v, mapa_u32(s_ob1full, peer));
         }
         bar_compute();
-        mbar_wait_a(s_ob1full, par);
+        mbar_wait(s_ob1full, par);
         TRACE2(crank, 21);
 #pragma unroll
         for (int jp = 0; jp < A / 32; jp++) {
@@ -1093,7 +1097,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
             for (int i = 0; i < 2; i++) hmma(zz[i], a1, zab[i][jp].z, zab[i][jp].w);
         }
         // OB1 has been read: arm its barrier for the peer's next half, then free it for both CTAs
-        if (tid == 0) mbar_expect_a(s_ob1full, TU * 128 * 2);
+        if (tid == 0) mbar_arrive_expect_tx(s_ob1full, TU * 128 * 2);
         release(s_ob1free);
         release_remote(s_ob1free, peer);
         if (DUMP) {
@@ -1114,10 +1118,10 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 for (int t = t_begin; t < t_end; t++)
                     for (int l = 0; l < L; l++, pc++) {
                         const uint32_t sl = pc & 1;
-                        mbar_wait_a(s_empty + 8 * sl, ((pc >> 1) & 1) ^ 1);
-                        mbar_expect_a(s_full + 8 * sl, M::PIECE0);
-                        tma_load_a(sm + M::C_RING + sl * M::PIECE0, img + (size_t)l * im.layer_bytes + C::W_CUR, 16384, s_full + 8 * sl);
-                        tma_load_a(sm + M::C_RING + sl * M::PIECE0 + 16384, img + (size_t)l * im.layer_bytes + C::W_RES, 8192, s_full + 8 * sl);
+                        mbar_wait(s_empty + 8 * sl, ((pc >> 1) & 1) ^ 1);
+                        mbar_arrive_expect_tx(s_full + 8 * sl, M::PIECE0);
+                        tma_load_1d(sm + M::C_RING + sl * M::PIECE0, img + (size_t)l * im.layer_bytes + C::W_CUR, 16384, s_full + 8 * sl);
+                        tma_load_1d(sm + M::C_RING + sl * M::PIECE0 + 16384, img + (size_t)l * im.layer_bytes + C::W_RES, 8192, s_full + 8 * sl);
                     }
             }
         } else {
@@ -1139,14 +1143,14 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
             auto prep = [&](const bool ap_ok) {
                 if (t1 < t_end) {
                     const uint2 b2 = lds64(s_bias + l1 * 1024 + 16);
-                    if (!ap_ok) mbar_wait_a(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
+                    if (!ap_ok) mbar_wait(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
                     const uint4 a0 = lds128(s_ap + (pn & 3) * 8192), a1 = lds128(s_ap + (pn & 3) * 8192 + 16);
                     brn = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
                     accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
                     accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
                     // the tile has been read: arm its barrier for the tile NAP steps on (one thread, ordered before this warp's "free"
                     // signal), then hand the buffer back to the prep CTA
-                    if (tid == 0) mbar_expect_a(s_apfull + 8 * (pn & 3), 8192);
+                    if (tid == 0) mbar_arrive_expect_tx(s_apfull + 8 * (pn & 3), 8192);
                     release_remote(s_apfree + 8 * (pn & 3), 2);
                 }
                 pn++;
@@ -1166,8 +1170,8 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
             for (int t = t_begin; t < t_end; t++) {
                 TRACE2(0, 1);
                 if (t > t_begin) {                             // the tail CTA has written this sample's indices into ys
-                    mbar_wait_a(s_yfull, (uint32_t)(t - t_begin - 1) & 1);
-                    if (tid == 0 && t + 1 < t_end) mbar_expect_a(s_yfull, 2 * TU * 4);          // arm the next hand-back
+                    mbar_wait(s_yfull, (uint32_t)(t - t_begin - 1) & 1);
+                    if (tid == 0 && t + 1 < t_end) mbar_arrive_expect_tx(s_yfull, 2 * TU * 4);          // arm the next hand-back
                 }
                 {   // embedding (reference.cpp:42-57), this warp's 8 channels
                     const int yc0 = ys[g], yc1 = ys[g + 8];
@@ -1196,7 +1200,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 for (int l = 0; l < L; l++, pc++) {
                     const uint32_t sl = pc & 1, p1 = sm + M::C_RING + sl * M::PIECE0, fph = (pc >> 1) & 1;
                     const float2 br = brn;
-                    if (!ok_f) mbar_wait_a(s_full + 8 * sl, fph);
+                    if (!ok_f) mbar_wait(s_full + 8 * sl, fph);
                     {
                         const uint4 bt0 = lds128(p1 + o_t0), bg0 = lds128(p1 + o_g0), bt1 = lds128(p1 + o_t0 + 512), bg1 = lds128(p1 + o_g0 + 512);
                         float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
@@ -1209,14 +1213,10 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     // gate, so that only the h tile is read between the barrier below and the res HMMAs
                     const uint4 bw0 = lds128(p1 + o_res), bw1 = lds128(p1 + o_res + 512);
                     {
-                        const __half2 half = __floats2half2_rn(0.5f, 0.5f);
-                        const __half2 tg0 = wn::tanh_h2(h2(pack_h2(accp[0][0], accp[0][1]))), tg1 = wn::tanh_h2(h2(pack_h2(accp[0][2], accp[0][3])));
-                        const __half2 sg0 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * accp[1][0], 0.5f * accp[1][1]))), half, half);
-                        const __half2 sg1 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * accp[1][2], 0.5f * accp[1][3]))), half, half);
-                        const uint32_t h01 = u32(__hmul2(tg0, sg0)), h23 = u32(__hmul2(tg1, sg1));
-                        sts64(sm + M::C_HBUF + xchg, h01, h23);
+                        uint32_t h01, h23;
+                        gate(accp, sm + M::C_HBUF + xchg, h01, h23);
                         // the tail CTA's copy: buffer hcnt & 1, free once the tail has read the tile of two steps ago
-                        if (!ok_hf) mbar_wait_a(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
+                        if (!ok_hf) mbar_wait(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
                         st_async_v2(r_hbuf + (hcnt & 1) * 2048, h01, h23, r_hfull + 8 * (hcnt & 1));
                         hcnt++;
                     }
@@ -1228,26 +1228,16 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     for (int j = 0; j < 4; j++) load_a(ha[j], sm + M::C_HBUF + j * 512 + lane16);
                     TRACE2(0, 10);
                     float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
-                    hmma(ra, ha[0], bw0.x, bw0.y); hmma(rb, ha[2], bw1.x, bw1.y);
-                    hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
+                    hmma_res(ra, rb, ha, bw0, bw1);
                     release(s_empty + 8 * sl);
-                    xres[0] = ((ra[0] + rb[0]) + br.x) + xres[0]; xres[1] = ((ra[1] + rb[1]) + br.y) + xres[1];
-                    xres[2] = ((ra[2] + rb[2]) + br.x) + xres[2]; xres[3] = ((ra[3] + rb[3]) + br.y) + xres[3];
-                    if (l + 1 < L) {
-                        const uint32_t x01 = pack_h2(xres[0], xres[1]), x23 = pack_h2(xres[2], xres[3]);
-                        sts64(sm + M::C_XBUF + xchg, x01, x23);
-                        stg_v2(gring + lane16 + (size_t)((uint32_t)(it0.slot * L + l + 1) * rstride) + jw * 512 + hw * 8, x01, x23);
-                    }
+                    residual(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
                     TRACE2(0, 14);
-                    if (DUMP) {
-                        if (v0) { p.xtOut[((size_t)l * B + b0) * R + cw] = xres[0]; p.xtOut[((size_t)l * B + b0) * R + cw + 1] = xres[1]; }
-                        if (v1) { p.xtOut[((size_t)l * B + b1) * R + cw] = xres[2]; p.xtOut[((size_t)l * B + b1) * R + cw + 1] = xres[3]; }
-                    }
+                    dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
                     {   // look at the coming step's barriers
                         const uint32_t npc = pc + 1;
-                        ok_f = mbar_probe_a(s_full + 8 * (npc & 1), (npc >> 1) & 1);
-                        ok_ap = mbar_probe_a(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
-                        ok_hf = mbar_probe_a(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
+                        ok_f = mbar_test_wait(s_full + 8 * (npc & 1), (npc >> 1) & 1);
+                        ok_ap = mbar_test_wait(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
+                        ok_hf = mbar_test_wait(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
                     }
                     TRACE2(0, 13);
                     if (l + 1 < L) {
@@ -1270,9 +1260,9 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 uint32_t pc = 0;
                 auto put = [&](const unsigned char* src, uint32_t bytes) {
                     const uint32_t sl = pc % M::NSLOT1;
-                    mbar_wait_a(s_empty + 8 * sl, ((pc / M::NSLOT1) & 1) ^ 1);
-                    mbar_expect_a(s_full + 8 * sl, bytes);
-                    tma_load_a(sm + M::T_RING + sl * M::SLOT1, src, bytes, s_full + 8 * sl);
+                    mbar_wait(s_empty + 8 * sl, ((pc / M::NSLOT1) & 1) ^ 1);
+                    mbar_arrive_expect_tx(s_full + 8 * sl, bytes);
+                    tma_load_1d(sm + M::T_RING + sl * M::SLOT1, src, bytes, s_full + 8 * sl);
                     pc++;
                 };
                 for (int t = t_begin; t < t_end; t++)
@@ -1292,13 +1282,13 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 const float sel1 = (2 * w + 1 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w + 1] : 0.5f;
                 for (int l = 0; l < L; l++, pc++, hcnt++) {
                     const uint32_t hb = sm + M::T_HBUF + (hcnt & 1) * 2048;
-                    mbar_wait_a(s_hfull + 8 * (hcnt & 1), (hcnt >> 1) & 1);
+                    mbar_wait(s_hfull + 8 * (hcnt & 1), (hcnt >> 1) & 1);
                     TRACE2(1, 16);
                     uint32_t ha[4][4];
 #pragma unroll
                     for (int j = 0; j < 4; j++) load_a(ha[j], hb + j * 512 + lane16);
                     const uint32_t sl = pc % M::NSLOT1, p2 = sm + M::T_RING + sl * M::SLOT1;
-                    mbar_wait_a(s_full + 8 * sl, (pc / M::NSLOT1) & 1);
+                    mbar_wait(s_full + 8 * sl, (pc / M::NSLOT1) & 1);
 #pragma unroll
                     for (int jp = 0; jp < 2; jp++) {
                         uint4 bw[C::NSK];
@@ -1311,7 +1301,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     }
                     // the h tile has been read (the HMMAs above hold its values): arm its barrier for the tile after next (one thread,
                     // ordered before this warp's "free" signal), then hand the buffer back to the chain CTA
-                    if (tid == 0) mbar_expect_a(s_hfull + 8 * (hcnt & 1), 2048);
+                    if (tid == 0) mbar_arrive_expect_tx(s_hfull + 8 * (hcnt & 1), 2048);
                     release_remote(s_hfree + 8 * (hcnt & 1), 0);
                     release(s_empty + 8 * sl);
                     TRACE2(1, 15);
@@ -1333,13 +1323,11 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     uint4 v[C::NSK / 2];
 #pragma unroll
                     for (int i = 0; i < C::NSK; i++) {
-                        const int c = 8 * (w * C::NSK + i) + 2 * t4;
-                        const float b0f = s_bout[c], b1f = s_bout[c + 1];
-                        const uint32_t lo = pack_h2(fmaxf(sk[i][0] + b0f, 0.f), fmaxf(sk[i][1] + b1f, 0.f)), hi = pack_h2(fmaxf(sk[i][2] + b0f, 0.f), fmaxf(sk[i][3] + b1f, 0.f));
+                        uint32_t lo, hi;
+                        relu_skip(sk[i], s_bout, 8 * (w * C::NSK + i) + 2 * t4, lo, hi);
                         if (i & 1) { v[i >> 1].z = lo; v[i >> 1].w = hi; } else { v[i >> 1].x = lo; v[i >> 1].y = hi; }
-                        sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
                     }
-                    mbar_wait_a(s_ob0free, ((uint32_t)(t - t_begin) & 1) ^ 1);
+                    mbar_wait(s_ob0free, ((uint32_t)(t - t_begin) & 1) ^ 1);
                     const uint32_t r_ob0full = mapa_u32(s_ob0full, 2);
 #pragma unroll
                     for (int j = 0; j < C::NSK / 2; j++) {
@@ -1359,7 +1347,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     sts64(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
                 }
                 bar_compute();
-                mbar_wait_a(s_lfull, (uint32_t)(t - t_begin) & 1);  // columns 128-255 from the prep CTA
+                mbar_wait(s_lfull, (uint32_t)(t - t_begin) & 1);  // columns 128-255 from the prep CTA
                 TRACE2(1, 22);
                 {   // softmax + categorical sample: warp w serves utterances 2w and 2w+1; lane holds 8 consecutive classes of each
                     float e[2][8], m[2] = {0.f, 0.f};
@@ -1377,7 +1365,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                         m[1] = fmaxf(m[1], __shfl_xor_sync(0xffffffffu, m[1], o));
                     }
                     // the logits have been read: arm lfull for the prep's next half, then hand the buffer back to it
-                    if (tid == 0) mbar_expect_a(s_lfull, TU * 128 * 4);
+                    if (tid == 0) mbar_arrive_expect_tx(s_lfull, TU * 128 * 4);
                     release_remote(s_lfree, 2);
                     float incl[2];
 #pragma unroll
@@ -1434,7 +1422,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 TRACE2(1, 23);
                 bar_compute();
             }
-            if (tid < TU && tile * TU + tid < B) { p.yCur[tile * TU + tid] = ys[tid]; p.yPrev[tile * TU + tid] = ys[TU + tid]; }
+            store_ys(p, B, ys, tile, tid);
         }
     } else {
         // ===================================================================================== prep CTA
@@ -1446,10 +1434,10 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 int l = 0;
                 for (int n = 0; n < nsteps; n++) {
                     const uint32_t sl = n & 3;
-                    mbar_wait_a(s_empty + 8 * sl, ((n >> 2) & 1) ^ 1);
-                    mbar_expect_a(s_full + 8 * sl, 16384);
+                    mbar_wait(s_empty + 8 * sl, ((n >> 2) & 1) ^ 1);
+                    mbar_arrive_expect_tx(s_full + 8 * sl, 16384);
                     // Wprev of layer l lives in the block of the layer before it (lat_pack_kernel)
-                    tma_load_a(sm + M::P_RING + sl * 16384, img + (size_t)((l + L - 1) % L) * im.layer_bytes + C::W_PREV, 16384, s_full + 8 * sl);
+                    tma_load_1d(sm + M::P_RING + sl * 16384, img + (size_t)((l + L - 1) % L) * im.layer_bytes + C::W_PREV, 16384, s_full + 8 * sl);
                     if (++l == L) l = 0;
                 }
             }
@@ -1480,7 +1468,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                     const uint32_t dst = sm + M::P_PST + slot * 2048 + (uint32_t)(w * 32 + lane) * 16;
                     if (itp.t >= t_end || itp.t < d) {
                         sts128(dst, make_uint4(0, 0, 0, 0));
-                        mbar_arrive_a(s_pfull + 8 * slot);
+                        mbar_arrive(s_pfull + 8 * slot);
                     } else {
                         int sl = itp.slot - d; if (sl < 0) sl += slots;
                         cp_async16(dst, gring + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
@@ -1499,7 +1487,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 TRACE2(2, 30);
                 out_half(t, zsw, 1, zz);
                 const uint32_t r_lfull = mapa_u32(s_lfull, 1);
-                mbar_wait_a(s_lfree, ((uint32_t)(t - t_begin) & 1) ^ 1);
+                mbar_wait(s_lfree, ((uint32_t)(t - t_begin) & 1) ^ 1);
 #pragma unroll
                 for (int i = 0; i < 2; i++) {
                     const int c = 8 * (16 + 2 * w + i) + 2 * t4;
@@ -1515,23 +1503,22 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
                 cp_async_wait_pending<2>();                    // this thread's conditioning of step n has landed (two later groups may be in flight)
                 const uint4 cb = lds128(s_cond + slot * 4096);
                 const uint4 bq = lds128(s_bias + l1 * 512);
-                mbar_wait_a(s_full + 8 * sl, (n >> 2) & 1);
-                const uint4 bt0 = lds128(pa + o_t0), bg0 = lds128(pa + o_g0), bt1 = lds128(pa + o_t0 + 512), bg1 = lds128(pa + o_g0 + 512);
-                mbar_wait_a(s_pfull + 8 * slot, (n >> 3) & 1);
+                mbar_wait(s_full + 8 * sl, (n >> 2) & 1);
+                const GateW bw = lds_gate_w(pa, o_t0, o_g0);
+                mbar_wait(s_pfull + 8 * slot, (n >> 3) & 1);
                 uint32_t pb[4][4];
 #pragma unroll
                 for (int j = 0; j < 4; j++) load_a(pb[j], sm + M::P_PST + slot * 2048 + j * 512 + lane16);
                 const float4 bh = make_float4(__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w));
                 const float2 c0 = unpack_h2(cb.x), c1 = unpack_h2(cb.y), c2 = unpack_h2(cb.z), c3 = unpack_h2(cb.w);
-                float a0[4] = {bh.x + c0.x, bh.y + c0.y, bh.x + c1.x, bh.y + c1.y}, a1[4] = {bh.z + c2.x, bh.w + c2.y, bh.z + c3.x, bh.w + c3.y};
-                float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
-                hmma(a0, pb[0], bt0.x, bt0.y); hmma(a1, pb[0], bg0.x, bg0.y); hmma(u0, pb[2], bt1.x, bt1.y); hmma(u1, pb[2], bg1.x, bg1.y);
-                hmma(a0, pb[1], bt0.z, bt0.w); hmma(a1, pb[1], bg0.z, bg0.w); hmma(u0, pb[3], bt1.z, bt1.w); hmma(u1, pb[3], bg1.z, bg1.w);
+                float a[2][4] = {{bh.x + c0.x, bh.y + c0.y, bh.x + c1.x, bh.y + c1.y}, {bh.z + c2.x, bh.w + c2.y, bh.z + c3.x, bh.w + c3.y}};
+                float u[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+                hmma_k64(a, u, pb, bw);
                 release(s_empty + 8 * sl);
                 // the chain CTA's tile buffer n % NAP is free once it has read tile n - NAP
-                mbar_wait_a(s_apfree + 8 * buf, ((n / M::NAP) & 1) ^ 1);
-                st_async_v4(r_ap + buf * 8192, a0[0] + u0[0], a0[1] + u0[1], a0[2] + u0[2], a0[3] + u0[3], r_apfull + 8 * buf);
-                st_async_v4(r_ap + buf * 8192 + 16, a1[0] + u1[0], a1[1] + u1[1], a1[2] + u1[2], a1[3] + u1[3], r_apfull + 8 * buf);
+                mbar_wait(s_apfree + 8 * buf, ((n / M::NAP) & 1) ^ 1);
+                st_async_v4(r_ap + buf * 8192, a[0][0] + u[0][0], a[0][1] + u[0][1], a[0][2] + u[0][2], a[0][3] + u[0][3], r_apfull + 8 * buf);
+                st_async_v4(r_ap + buf * 8192 + 16, a[1][0] + u[1][0], a[1][1] + u[1][1], a[1][2] + u[1][2], a[1][3] + u[1][3], r_apfull + 8 * buf);
                 stage();
                 if (++l1 == L) l1 = 0;
                 // the output half of sample tout: after step (tout + 1, 1) has been shipped, so that the chain CTA starts sample
@@ -1590,51 +1577,43 @@ cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-// p.B = utterances of this run; engine_B = batch size the conditioning store / history ring were laid out for
-template <int S>
-static cudaError_t lat_launch_S(const WnParams& p, const unsigned char* im8, int grid, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
+// one launch of a latency kernel variant; p.B = utterances of this run, ntiles_alloc = tiles of the batch size the conditioning
+// store / history ring were laid out for
+using LatGo = cudaError_t (*)(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream);
+
+template <int S, bool DUMP, bool TRC>
+static cudaError_t lat_go(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
 {
     const size_t smem = Cfg<S>::SMEM;
-    *smem_out = smem;
-    cudaError_t e;
-#define LAT_GO(DUMPV, TRCV, PP)                                                                                                    \
-    do {                                                                                                                           \
-        e = cudaFuncSetAttribute(wn_lat_kernel<S, DUMPV, TRCV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);          \
-        if (e != cudaSuccess) return e;                                                                                            \
-        wn_lat_kernel<S, DUMPV, TRCV><<<grid, NT, smem, stream>>>(PP, im8, ntiles_alloc);                                          \
-        e = cudaGetLastError();                                                                                                    \
-        if (e != cudaSuccess) return e;                                                                                            \
-    } while (0)
-    // a dumping launch = every sample but the last with the plain kernel, then the last one with the dumping variant
-    // (a continuation is bit-identical to one launch: the whole state lives in global memory between launches)
-    WnParams head = p, tail = p;
-    if (p.dump) { head.count = p.count - 1; head.dump = 0; tail.init_sample = p.init_sample + p.count - 1; tail.count = 1; }
-    if (head.count > 0) {
-        if (p.trace) LAT_GO(false, true, head); else LAT_GO(false, false, head);
-    }
-    if (p.dump) LAT_GO(true, false, tail);
-#undef LAT_GO
-    return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(wn_lat_kernel<S, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    wn_lat_kernel<S, DUMP, TRC><<<tiles, NT, smem, stream>>>(p, im8, ntiles_alloc);
+    return cudaGetLastError();
 }
 
-// the cluster variant: grid = NCL x tiles, cluster (NCL, 1, 1)
-template <int S, bool DUMP, bool TRC>
-static cudaError_t lat2_go(const WnParams& pp, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
+// the cluster variant: grid = NCL x `clusters` CTAs, cluster (NCL, 1, 1); `at` receives the cluster attribute the config points to
+template <int S>
+static cudaLaunchConfig_t lat2_config(int clusters, cudaStream_t stream, cudaLaunchAttribute& at)
 {
-    const size_t smem = CfgC<S>::SMEM;
-    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(NCL * tiles, 1, 1);
-    cfg.blockDim = dim3(NTC, 1, 1);
-    cfg.dynamicSmemBytes = smem;
+    cfg.gridDim = dim3(NCL * clusters, 1, 1);
+    cfg.blockDim = dim3(NT, 1, 1);
+    cfg.dynamicSmemBytes = CfgC<S>::SMEM;
     cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = NCL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
+    at.id = cudaLaunchAttributeClusterDimension;
+    at.val.clusterDim.x = NCL; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+    cfg.attrs = &at;
     cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, DUMP, TRC>, pp, im8, ntiles_alloc);
+    return cfg;
+}
+template <int S, bool DUMP, bool TRC>
+static cudaError_t lat2_go(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
+{
+    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S>::SMEM);
+    if (e != cudaSuccess) return e;
+    cudaLaunchAttribute at;
+    const cudaLaunchConfig_t cfg = lat2_config<S>(tiles, stream, at);
+    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, DUMP, TRC>, p, im8, ntiles_alloc);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 // how many clusters the device runs at once (a cluster needs NCL SMs of one GPC: fewer than 132 / NCL fit on an H100); 0 if the query fails
@@ -1643,31 +1622,37 @@ static int lat2_max_clusters()
 {
     static int cached = -1;
     if (cached >= 0) return cached;
-    const size_t smem = CfgC<S>::SMEM;
-    if (cudaFuncSetAttribute(wn_lat2_kernel<S, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(NCL * 48, 1, 1);
-    cfg.blockDim = dim3(NTC, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = NCL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
+    if (cudaFuncSetAttribute(wn_lat2_kernel<S, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
+    cudaLaunchAttribute at;
+    const cudaLaunchConfig_t cfg = lat2_config<S>(48, 0, at);
     int n = 0;
     if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
     return cached = n;
+}
+
+// a dumping launch = every sample but the last with the plain (or tracing) variant, then the last one with the dumping variant
+// (a continuation is bit-identical to one launch: the whole state lives in global memory between launches)
+static cudaError_t lat_launch_split(const WnParams& p, LatGo plain, LatGo trace, LatGo dump, const unsigned char* im8, int tiles, int ntiles_alloc,
+                                    cudaStream_t stream)
+{
+    WnParams head = p, tail = p;
+    if (p.dump) { head.count = p.count - 1; head.dump = 0; tail.init_sample = p.init_sample + p.count - 1; tail.count = 1; }
+    cudaError_t e = cudaSuccess;
+    if (head.count > 0) e = (p.trace ? trace : plain)(head, im8, tiles, ntiles_alloc, stream);
+    if (e == cudaSuccess && p.dump) e = dump(tail, im8, tiles, ntiles_alloc, stream);
+    return e;
+}
+template <int S>
+static cudaError_t lat_launch_S(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
+{
+    *smem_out = Cfg<S>::SMEM;
+    return lat_launch_split(p, lat_go<S, false, false>, lat_go<S, false, true>, lat_go<S, true, false>, im8, tiles, ntiles_alloc, stream);
 }
 template <int S>
 static cudaError_t lat2_launch_S(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
 {
     *smem_out = CfgC<S>::SMEM;
-    WnParams head = p, tail = p;
-    if (p.dump) { head.count = p.count - 1; head.dump = 0; tail.init_sample = p.init_sample + p.count - 1; tail.count = 1; }
-    cudaError_t e = cudaSuccess;
-    if (head.count > 0) e = p.trace ? lat2_go<S, false, true>(head, im8, tiles, ntiles_alloc, stream) : lat2_go<S, false, false>(head, im8, tiles, ntiles_alloc, stream);
-    if (e == cudaSuccess && p.dump) e = lat2_go<S, true, false>(tail, im8, tiles, ntiles_alloc, stream);
-    return e;
+    return lat_launch_split(p, lat2_go<S, false, false>, lat2_go<S, false, true>, lat2_go<S, true, false>, im8, tiles, ntiles_alloc, stream);
 }
 
 int wn_lat_max_clusters(int S) { return S == 256 ? lat2_max_clusters<256>() : S == 128 ? lat2_max_clusters<128>() : 0; }
@@ -1686,7 +1671,7 @@ cudaError_t wn_launch_lat(const WnParams& p, const void* image, int engine_B, bo
         else if (p.S == 128) e = lat2_launch_S<128>(p, im8, grid, ntiles_alloc, stream, &smem);
         else return cudaErrorInvalidValue;
         if (e != cudaSuccess) return e;
-        if (info) { info->kernel = 18; info->grid = NCL * grid; info->block = NTC; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = NCL; }
+        if (info) { info->kernel = 18; info->grid = NCL * grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = NCL; }
         return cudaGetLastError();
     }
     if (p.S == 256) e = lat_launch_S<256>(p, im8, grid, ntiles_alloc, stream, &smem);

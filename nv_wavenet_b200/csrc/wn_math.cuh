@@ -9,6 +9,8 @@
 // --use_fast_math expf/tanhf of nv_wavenet_util.cuh:78-86).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
+#include <stdint.h>
 
 namespace wn {
 
@@ -102,5 +104,13 @@ __device__ __forceinline__ float exp2f_fast(float x)
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
+
+// two floats <-> one 32-bit word of two fp16 (round to nearest even)
+__device__ __forceinline__ uint32_t pack_h2(float a, float b)
+{
+    __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ float2 unpack_h2(uint32_t v) { return __half22float2(*reinterpret_cast<__half2*>(&v)); }
 
 }  // namespace wn

@@ -10,24 +10,24 @@ namespace sm90 {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-// ------------------------------------------------------------------ mbarrier
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count)
+// ------------------------------------------------------------------ mbarrier, by shared-memory address (uint64_t* forms below)
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
 {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 __device__ __forceinline__ void fence_mbar_init()
 {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
+    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes)
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes)
 {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity)
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity)
 {
     uint32_t ok;
     asm volatile(
@@ -35,23 +35,46 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity)
         "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
         "selp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
+        : "r"(bar), "r"(parity)
         : "memory");
     return ok != 0;
 }
-// Bounded spin: a protocol slip must surface as a launch failure with a message, never as a hung GPU.
-static __device__ __noinline__ void mbar_timeout(uint32_t bar_addr, uint32_t parity)
+// a look that never suspends the thread (try_wait parks it until a time limit when the phase is still running)
+__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity)
 {
-    printf("wn_tc: mbarrier wait timed out: block %d thread %d barrier@0x%x parity %u\n", blockIdx.x, threadIdx.x, bar_addr, parity);
+    uint32_t ok;
+    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+    return ok != 0;
+}
+// three looks issued back to back: their ~90-cycle latencies overlap
+__device__ __forceinline__ void mbar_try_wait3(uint32_t b1, uint32_t p1, uint32_t b2, uint32_t p2, uint32_t b3, uint32_t p3, bool& o1, bool& o2, bool& o3)
+{
+    uint32_t r1, r2, r3;
+    asm volatile("{\n\t.reg .pred q1, q2, q3;\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 q1, [%3], %4;\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 q2, [%5], %6;\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 q3, [%7], %8;\n\t"
+                 "selp.u32 %0, 1, 0, q1;\n\tselp.u32 %1, 1, 0, q2;\n\tselp.u32 %2, 1, 0, q3;\n\t}"
+                 : "=r"(r1), "=r"(r2), "=r"(r3) : "r"(b1), "r"(p1), "r"(b2), "r"(p2), "r"(b3), "r"(p3) : "memory");
+    o1 = r1 != 0; o2 = r2 != 0; o3 = r3 != 0;
+}
+// Bounded spin: a protocol slip must surface as a launch failure with a message, never as a hung GPU.
+static __device__ __noinline__ void mbar_timeout(uint32_t bar, uint32_t parity)
+{
+    printf("nv_wavenet: mbarrier wait timed out: block %d thread %d barrier@0x%x parity %u\n", blockIdx.x, threadIdx.x, bar, parity);
     __trap();
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 {
     uint32_t spins = 0;
-    while (!mbar_try_wait(bar, parity)) {
-        if (++spins > (1u << 24)) mbar_timeout(smem_u32(bar), parity);
-    }
+    while (!mbar_try_wait(bar, parity))
+        if (++spins > (1u << 24)) mbar_timeout(bar, parity);
 }
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { mbar_init(smem_u32(bar), count); }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { mbar_arrive(smem_u32(bar)); }
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) { mbar_arrive_expect_tx(smem_u32(bar), bytes); }
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) { return mbar_try_wait(smem_u32(bar), parity); }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 
 // ------------------------------------------------------------------ fences
 // generic-proxy writes (st.shared / st.global) -> visible to the async proxy (TMA, wgmma operand reads)
@@ -60,11 +83,15 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 // ------------------------------------------------------------------ 1-D bulk TMA: global -> shared, completes on an mbarrier
-__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar)
+__device__ __forceinline__ void tma_load_1d(uint32_t smem_dst, const void* gmem_src, uint32_t bytes, uint32_t bar)
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+                 ::"r"(smem_dst), "l"(gmem_src), "r"(bytes), "r"(bar)
                  : "memory");
+}
+__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar)
+{
+    tma_load_1d(smem_u32(smem_dst), gmem_src, bytes, smem_u32(bar));
 }
 // pull a global range towards L2 ahead of the TMA that will read it
 __device__ __forceinline__ void tma_prefetch_l2(const void* gmem_src, uint32_t bytes)

@@ -188,15 +188,8 @@ __global__ void tc_pack_kernel(WnParams p, unsigned char* __restrict__ img, TcIm
 }
 
 // ------------------------------------------------------------------------------------------------ helpers
-__device__ __forceinline__ uint32_t pack_h2(float a, float b)
-{
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_h2(uint32_t v)
-{
-    return __half22float2(*reinterpret_cast<__half2*>(&v));
-}
+using wn::pack_h2;
+using wn::unpack_h2;
 // two consecutive fp16 (k even) of row `row` of a SW128 tile, in shared or global memory
 __device__ __forceinline__ void st_pair(unsigned char* tile, int row, int k, float v0, float v1)
 {
