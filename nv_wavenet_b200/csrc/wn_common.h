@@ -1,9 +1,23 @@
 // wn_common.h -- shared declarations of the WaveNet inference engine (host + device).
 #pragma once
+#include "../../include/nvwn_b200.h"
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
+
+// An engine's sizes and its kernel choice, both fixed by nvwn_create (wn_engine.cu, resolve_config) from its arguments and the
+// environment switches of INTEGRATION.md §1.  Together they fix the layouts of the conditioning store, the history ring and the
+// weight image.
+struct WnConfig {
+    int dtype, R, S, A, L, maxDil, B, N;    // B, N: what the engine holds; a run may take fewer
+    int kernel;                             // NVWN_KERNEL_STREAM | NVWN_KERNEL_TENSORCORE | NVWN_KERNEL_LATENCY
+    int tc_tile;                            // tensor-core: utterances per tile, 32 | 64 | 128
+    bool tc_fused;                          // tensor-core: the fused schedule
+    bool lat_cluster;                       // latency: the three-CTA cluster kernel may run
+    int stream_bt;                          // stream: utterances per CTA, 1 | 2 | 4; 0 = chosen from the run's batch
+    bool stream_ring;                       // stream, fp32: the weights may go through the shared-memory ring
+};
 
 // Everything a kernel launch needs.  Device pointers only.
 // Replaces nv_wavenet_params<T_weight,T_data> (nv_wavenet.cuh:40-85) of the reference.
@@ -37,9 +51,31 @@ struct WnLaunchInfo {
     int kernel, grid, block, smem_bytes, batch_per_cta, cluster;
 };
 
-// stream kernel (wn_stream_kernel.cu): CUDA-core, one CTA per batch tile, weights streamed from L2.
-cudaError_t wn_launch_stream(const WnParams& p, int contract, cudaStream_t stream, WnLaunchInfo* info);   // 0 fp32 exact, 1 fp16, 2 fp32 fast
+// One kernel family as the engine sees it: the sizes of its conditioning store, history ring and weight image, the conversions of
+// the store, and the launch.  The engine picks one at creation.  Conditioning enters and leaves the store as fp32 [n][L][B][2R]
+// in device memory; the plain fp32 store also copies from host memory.
+struct WnFamily {
+    size_t (*store_bytes)(const WnConfig& c);       // c.N samples of conditioning
+    size_t (*ring_bytes)(const WnConfig& c);
+    size_t (*image_bytes)(const WnConfig& c);       // NULL when pack is
+    cudaError_t (*convert)(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
+    cudaError_t (*readback)(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
+    cudaError_t (*pack)(void* image, const WnParams& p, cudaStream_t stream);      // weight blob -> image; NULL: the kernels read the blob
+    cudaError_t (*launch)(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info);
+    bool whole_batch;                               // a run must take all c.B utterances
+};
+extern const WnFamily wn_stream_family;             // wn_stream_kernel.cu: CUDA-core, one CTA per batch tile, weights streamed from L2
+extern const WnFamily wn_tc_family;                 // wn_tc_kernel.cu: fp16 tensor-core (wgmma) kernel
+extern const WnFamily wn_lat_family;                // wn_lat_kernel.cu: fp16 latency-mode kernels
 bool wn_stream_supported(int R, int S, int A, bool fp16);
+bool wn_tc_supported(int R, int S, int A, int L, int B);
+bool wn_lat_supported(int R, int S, int A, int L);
+int wn_lat_max_clusters(int S);                     // three-CTA clusters of the latency kernel the device runs at once
+
+// the plain conditioning store of the stream kernel (wn_convert.cu): [N][L][B][2R], fp16 on NVWN_FP16 engines, else fp32
+size_t wn_plain_store_bytes(const WnConfig& c);
+cudaError_t wn_plain_convert(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
+cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
 
 // teacher-forced scoring (wn_score_kernel.cu, DESIGN.md §5.4): one time chunk of T steps x Bs utterances, rows m = (t - t0) * Bs + b
 struct WnScoreChunk {
@@ -70,3 +106,12 @@ cudaError_t wn_f32_to_f16(__half* dst, const float* src_dev, size_t n, cudaStrea
 cudaError_t wn_f16_to_f32(float* dst, const __half* src_dev, size_t n, cudaStream_t stream);
 cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, cudaStream_t stream);
 cudaError_t wn_fill_int(int* dst, int value, size_t n, cudaStream_t stream);
+cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
+                            short* out_s, cudaStream_t stream);
+
+// conditioning producer (wn_cond_producer.cu)
+cudaError_t wn_cond_transpose_wu(float* WuT, const float* Wu, int C, int K, cudaStream_t stream);
+cudaError_t wn_cond_produce(float* out, float* U, const float* feat, const float* WuT, const float* bu, const float* Wc, const float* bc,
+                            int B, int C, int T, int K, int stride, int L, int R, int n0, int m, cudaStream_t stream);
+void wn_cond_host(float* Lh, const float* feat, const float* Wu, const float* bu, const float* Wc, const float* bc,
+                  int B, int C, int T, int K, int stride, int L, int R);

@@ -98,6 +98,25 @@ cudaError_t wn_fill_int(int* dst, int value, size_t n, cudaStream_t stream)
     return cudaGetLastError();
 }
 
+size_t wn_plain_store_bytes(const WnConfig& c)
+{
+    return (size_t)c.N * c.L * c.B * 2 * c.R * (c.dtype == NVWN_FP16 ? sizeof(__half) : sizeof(float));
+}
+
+cudaError_t wn_plain_convert(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream)
+{
+    const size_t per = (size_t)c.L * c.B * 2 * c.R, n = per * num_samples;
+    if (c.dtype == NVWN_FP16) return wn_f32_to_f16(static_cast<__half*>(store) + (size_t)first_sample * per, src, n, stream);
+    return cudaMemcpyAsync(static_cast<float*>(store) + (size_t)first_sample * per, src, n * sizeof(float), cudaMemcpyDefault, stream);
+}
+
+cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream)
+{
+    const size_t per = (size_t)c.L * c.B * 2 * c.R, n = per * num_samples;
+    if (c.dtype == NVWN_FP16) return wn_f16_to_f32(dst_dev, static_cast<const __half*>(store) + (size_t)first_sample * per, n, stream);
+    return cudaMemcpyAsync(dst_dev, static_cast<const float*>(store) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
+}
+
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream)
 {

@@ -17,34 +17,6 @@
 #include <string>
 #include <vector>
 
-cudaError_t wn_launch_tc(const WnParams& p, const void* tc_image, int TU, bool fused, cudaStream_t stream, WnLaunchInfo* info);   // wn_tc_kernel.cu
-int wn_tc_tile_utt(int B, int S);
-bool wn_tc_fused_default();
-bool wn_tc_supported(int R, int S, int A, int L, int B);
-cudaError_t wn_cond_transpose_wu(float* WuT, const float* Wu, int C, int K, cudaStream_t stream);              // wn_cond_producer.cu
-cudaError_t wn_cond_produce(float* out, float* U, const float* feat, const float* WuT, const float* bu, const float* Wc, const float* bc,
-                            int B, int C, int T, int K, int stride, int L, int R, int n0, int m, cudaStream_t stream);
-void wn_cond_host(float* Lh, const float* feat, const float* Wu, const float* bu, const float* Wc, const float* bc,
-                  int B, int C, int T, int K, int stride, int L, int R);
-cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
-                            short* out_s, cudaStream_t stream);                                                  // wn_convert.cu
-size_t wn_tc_image_bytes(int R, int S, int A, int L);
-cudaError_t wn_tc_pack(void* image, const WnParams& p, cudaStream_t stream);
-size_t wn_tc_ring_bytes(int TU, int L, int maxDil, int B);
-size_t wn_tc_cond_bytes(int TU, int L, int B, int N);
-cudaError_t wn_tc_cond_convert(void* dst, const float* src_dev, int first_sample, int nsamples, int TU, int L, int B, cudaStream_t stream);
-// latency-mode fp16 kernel (wn_lat_kernel.cu)
-bool wn_lat_supported(int R, int S, int A, int L);
-size_t wn_lat_image_bytes(int S, int L);
-size_t wn_lat_ring_bytes(int L, int maxDil, int B);
-size_t wn_lat_cond_bytes(int L, int B, int N);
-cudaError_t wn_lat_cond_convert(void* dst, const float* src_dev, int first_sample, int nsamples, int L, int B, cudaStream_t stream);
-cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream);
-cudaError_t wn_lat_cond_readback(float* dst_dev, const void* store, int first_sample, int nsamples, int L, int B, cudaStream_t stream);
-cudaError_t wn_tc_cond_readback(float* dst_dev, const void* store, int first_sample, int nsamples, int TU, int L, int B, cudaStream_t stream);
-cudaError_t wn_launch_lat(const WnParams& p, const void* image, int engine_B, bool cluster, cudaStream_t stream, WnLaunchInfo* info);
-int wn_lat_max_clusters(int S);
-
 namespace {
 
 thread_local std::string g_err;
@@ -73,9 +45,10 @@ bool is_device_ptr(const void* p)
 
 }  // namespace
 
-struct nvwn_engine {
-    int dtype, R, S, A, L, maxDil, B, N, impl, tanhEmbed, device;
+struct nvwn_engine : WnConfig {
+    int impl, tanhEmbed, device;
     size_t td;                               // sizeof(TD)
+    const WnFamily* family;                  // the kernel family of `kernel`: the layouts of Lh, ring and image, and the launch
 
     // packed weight blob (TD elements), offsets in bytes
     char* blob = nullptr;
@@ -90,16 +63,11 @@ struct nvwn_engine {
     void* ring = nullptr;
     float *xtOut = nullptr, *skipOut = nullptr, *Zs = nullptr, *Za = nullptr, *P = nullptr;
 
-    float* stage_dev = nullptr;              // device fp32 staging for host->fp16 uploads
+    float* stage_dev = nullptr;              // device fp32 staging for host->fp16 uploads (fp16 engines only)
     size_t stage_elems = 0;
 
-    void* tc_image = nullptr;                // tensor-core kernel's pre-tiled weight image
-    bool tc_dirty = true;
-    bool tc_mode = false;                    // decided once at creation: conditioning + history use the tiled layouts
-    int tc_tile = 64;                        // utterances per tensor-core tile and its schedule: resolved ONCE at creation (the
-    bool tc_fused = false;                   // conditioning store, the history ring and every launch depend on them)
-    bool lat_cluster = true;                 // latency mode: a three-CTA cluster per tile while 3 x tiles fit one wave (NVWN_LAT_CLUSTER=0 disables; read once)
-    bool lat_mode = false;                   // decided once at creation: latency-mode kernel (fragment-ordered layouts); tc_image holds its weight image
+    void* image = nullptr;                   // the family's weight image, packed from the blob before the first launch after a change
+    bool image_dirty = true;
 
     // conditioning producer (nvwn_cond_producer_load / _run): features | Wu | WuT | bu | Wc | bc | U chunk | Lh chunk in one allocation
     float* cp_scratch = nullptr;
@@ -108,7 +76,7 @@ struct nvwn_engine {
 
     // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
     void* score_image = nullptr;
-    bool score_dirty = true;                 // set wherever tc_dirty is: the image is repacked on the next nvwn_score
+    bool score_dirty = true;                 // set wherever image_dirty is: the image is repacked on the next nvwn_score
     char* score_scratch = nullptr;
     int score_T = 0;                         // time steps per chunk: SCORE_ROWS / B
 
@@ -124,27 +92,34 @@ struct nvwn_engine {
 
 namespace {
 
-// dst (TD, device) <- src (fp32, host or device), n elements
-int upload(nvwn_engine* e, void* dst, const float* src, size_t n, cudaStream_t stream = 0)
+// Hands n units of `unit` fp32 values at `src` (host or device) to convert(src_dev, first_unit, num_units).  fp16 engines bounce a
+// host source through the device staging buffer, whole units at a time, and wait for those copies: the buffer and the source are
+// free again on return.  fp32 engines have no staging buffer: their conversions are copies that also read host memory.
+template <typename Convert>
+int feed(nvwn_engine* e, const float* src, size_t n, size_t unit, cudaStream_t stream, Convert convert)
 {
     if (n == 0) return 0;
-    if (e->dtype != NVWN_FP16) {
-        CK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDefault, stream));
+    if (!e->stage_dev || is_device_ptr(src)) {
+        CK(convert(src, 0, n));
         return 0;
     }
-    if (is_device_ptr(src)) {
-        CK(wn_f32_to_f16(static_cast<__half*>(dst), src, n, stream));
-        return 0;
+    const size_t chunk = e->stage_elems / unit;                              // >= 1: nvwn_create sizes the buffer for it
+    for (size_t done = 0; done < n; done += chunk) {
+        const size_t m = n - done < chunk ? n - done : chunk;
+        CK(cudaMemcpyAsync(e->stage_dev, src + done * unit, m * unit * sizeof(float), cudaMemcpyHostToDevice, stream));
+        CK(convert(e->stage_dev, done, m));
     }
-    // host source: bounce through the device staging buffer in chunks
-    size_t done = 0;
-    while (done < n) {
-        const size_t m = (n - done < e->stage_elems) ? n - done : e->stage_elems;
-        CK(cudaMemcpyAsync(e->stage_dev, src + done, m * sizeof(float), cudaMemcpyHostToDevice, stream));
-        CK(wn_f32_to_f16(static_cast<__half*>(dst) + done, e->stage_dev, m, stream));
-        done += m;
-    }
+    CK(cudaStreamSynchronize(stream));
     return 0;
+}
+
+// dst (TD, device) <- src (fp32, host or device), n elements
+int upload(nvwn_engine* e, void* dst, const float* src, size_t n)
+{
+    return feed(e, src, n, 1, 0, [&](const float* s, size_t first, size_t m) {
+        return e->dtype == NVWN_FP16 ? wn_f32_to_f16(static_cast<__half*>(dst) + first, s, m, 0)
+                                     : cudaMemcpyAsync(static_cast<float*>(dst) + first, s, m * sizeof(float), cudaMemcpyDefault, 0);
+    });
 }
 
 // dst (fp32, host or device) <- src (fp32 device)
@@ -154,27 +129,40 @@ int download(float* dst, const float* src, size_t n)
     return 0;
 }
 
-// fp16 kernel choice, made ONCE per engine (the layouts of the conditioning store and of the history ring depend on it):
-// 0 = stream, 1 = tensor-core (wgmma, throughput mode), 2 = latency mode (mma.sync, register-resident chain).
-// `impl` NVWN_KERNEL_* forces a kernel; the environment variable NVWN_FP16_KERNEL = stream | tc | lat overrides AUTO (tests).
-int decide_fp16_kernel(int dtype, int impl, int R, int S, int A, int L, int B)
+// The engine's kernel family and its variant, from its sizes, `impl` (an NVWN_KERNEL_* id forces a family) and the environment
+// switches of INTEGRATION.md §1.  The only place the library reads the environment, once per engine: the conditioning store, the
+// history ring and the weight image are laid out for what it decides.
+void resolve_config(WnConfig& c, int impl)
 {
-    if (dtype != NVWN_FP16) return 0;
-    if (impl == NVWN_KERNEL_STREAM) return 0;
-    const bool tc_ok = wn_tc_supported(R, S, A, L, B), lat_ok = wn_lat_supported(R, S, A, L);
-    if (impl == NVWN_KERNEL_TENSORCORE) return tc_ok ? 1 : 0;
-    if (impl == NVWN_KERNEL_LATENCY) return lat_ok ? 2 : 0;
-    if (const char* env = getenv("NVWN_FP16_KERNEL")) {
-        if (!strcmp(env, "stream")) return 0;
-        if (!strcmp(env, "tc")) return tc_ok ? 1 : 0;
-        if (!strcmp(env, "lat")) return lat_ok ? 2 : 0;
-    }
+    auto num = [](const char* name, int unset) { const char* v = getenv(name); return v ? atoi(v) : unset; };
+    const int tc = wn_tc_supported(c.R, c.S, c.A, c.L, c.B) ? NVWN_KERNEL_TENSORCORE : NVWN_KERNEL_STREAM;
+    const int lat = wn_lat_supported(c.R, c.S, c.A, c.L) ? NVWN_KERNEL_LATENCY : NVWN_KERNEL_STREAM;
+    const char* fp16 = getenv("NVWN_FP16_KERNEL");
+    if (c.dtype != NVWN_FP16 || impl == NVWN_KERNEL_STREAM) c.kernel = NVWN_KERNEL_STREAM;
+    else if (impl == NVWN_KERNEL_TENSORCORE) c.kernel = tc;
+    else if (impl == NVWN_KERNEL_LATENCY) c.kernel = lat;
+    else if (fp16 && !strcmp(fp16, "stream")) c.kernel = NVWN_KERNEL_STREAM;
+    else if (fp16 && !strcmp(fp16, "tc")) c.kernel = tc;
+    else if (fp16 && !strcmp(fp16, "lat")) c.kernel = lat;
     // the latency kernels beat the tensor-core kernel even when their 16-utterance tiles need several waves (H100 80GB HBM3,
     // 400 W power limit, 2 560 utterances: 41.6 M against 14.1 M samples/s); NVWN_LAT_MAX_B caps the batch they take
-    int lat_max = INT_MAX;
-    if (const char* env = getenv("NVWN_LAT_MAX_B")) lat_max = atoi(env);
-    if (lat_ok && B <= lat_max) return 2;
-    return tc_ok ? 1 : 0;
+    else c.kernel = lat == NVWN_KERNEL_LATENCY && c.B <= num("NVWN_LAT_MAX_B", INT_MAX) ? lat : tc;
+
+    // tensor-core: 64-utterance tiles unless NVWN_TC_TILE (32 | 64 | 128) or NVWN_TC_NODUP (128) asks for another shape; the
+    // unfused schedule unless NVWN_TC_FUSED is set and not "0", or the tiles are 32 utterances
+    c.tc_tile = 64;
+    c.tc_fused = false;
+    if (c.kernel == NVWN_KERNEL_TENSORCORE) {
+        const int t = num("NVWN_TC_TILE", 64);
+        if (t == 32 || t == 128) c.tc_tile = t;
+        if (getenv("NVWN_TC_NODUP")) c.tc_tile = 128;
+        const char* fused = getenv("NVWN_TC_FUSED");
+        c.tc_fused = (fused && fused[0] != '0') || c.tc_tile == 32;
+    }
+    c.lat_cluster = num("NVWN_LAT_CLUSTER", 1) != 0;
+    const int bt = num("NVWN_STREAM_BT", 0);
+    c.stream_bt = bt == 1 || bt == 2 || bt == 4 ? bt : 0;
+    c.stream_ring = num("NVWN_STREAM_RING", 1) != 0;
 }
 
 void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, int count, int num_samples, int batch, int dump)
@@ -191,17 +179,6 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, int count, 
     p.yPrev = e->yPrev; p.yCur = e->yCur; p.ring = e->ring; p.yOut = e->yOut;
     p.xtOut = e->xtOut; p.skipOut = e->skipOut; p.Zs = e->Zs; p.Za = e->Za; p.P = e->P;
     p.trace = e->trace; p.trace_t = e->trace_t;
-}
-
-// the engine's conditioning store for samples [first_sample, first_sample + num_samples) as fp32 [num_samples][L][B][2R] in
-// device memory, whatever the kernel-native layout (plain / tiled fp16 / fragment order) is
-cudaError_t cond_readback(const nvwn_engine* e, float* dst_dev, int first_sample, int num_samples, cudaStream_t st)
-{
-    const size_t per = (size_t)e->L * e->B * 2 * e->R, n = per * num_samples;
-    if (e->lat_mode) return wn_lat_cond_readback(dst_dev, e->Lh, first_sample, num_samples, e->L, e->B, st);
-    if (e->tc_mode) return wn_tc_cond_readback(dst_dev, e->Lh, first_sample, num_samples, e->tc_tile, e->L, e->B, st);
-    if (e->dtype == NVWN_FP16) return wn_f16_to_f32(dst_dev, static_cast<const __half*>(e->Lh) + (size_t)first_sample * per, n, st);
-    return cudaMemcpyAsync(dst_dev, static_cast<const float*>(e->Lh) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
 }
 
 // rows (t, b) of one scoring chunk; bounds the chunk scratch: DESIGN.md §5.4
@@ -267,6 +244,8 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     e->B = batch_size; e->N = num_samples; e->impl = impl; e->tanhEmbed = tanh_embed ? 1 : 0;
     e->td = dtype == NVWN_FP16 ? 2 : 4;
     cudaGetDevice(&e->device);
+    resolve_config(*e, impl);
+    e->family = e->kernel == NVWN_KERNEL_TENSORCORE ? &wn_tc_family : e->kernel == NVWN_KERNEL_LATENCY ? &wn_lat_family : &wn_stream_family;
 
     const size_t L = num_layers, td = e->td;
     size_t off = 0;
@@ -280,7 +259,10 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     e->blob_bytes = off;
 
     const size_t Bz = batch_size, Nz = num_samples;
-    e->stage_elems = dtype == NVWN_FP16 ? ((size_t)16 << 20) : 0;      // 64 MB of fp32 staging
+    if (dtype == NVWN_FP16) {                                          // 64 MB of fp32 staging, or one sample of conditioning if larger
+        const size_t per = L * Bz * 2 * R;
+        e->stage_elems = per > ((size_t)16 << 20) ? per : ((size_t)16 << 20);
+    }
 #define ALLOC(ptr, bytes)                                                                     \
     do {                                                                                      \
         cudaError_t _e = cudaMalloc((void**)&(ptr), (bytes));                                 \
@@ -291,25 +273,13 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
         }                                                                                     \
     } while (0)
     ALLOC(e->blob, e->blob_bytes);
-    {
-        const int k = decide_fp16_kernel(dtype, impl, R, S, A, num_layers, batch_size);
-        e->tc_mode = k == 1; e->lat_mode = k == 2;
-        if (const char* v = getenv("NVWN_LAT_CLUSTER")) e->lat_cluster = atoi(v) != 0;
-        if (e->tc_mode) { e->tc_tile = wn_tc_tile_utt(batch_size, S); e->tc_fused = wn_tc_fused_default() || e->tc_tile == 32; }
-    }
-    ALLOC(e->Lh, e->tc_mode ? wn_tc_cond_bytes(e->tc_tile, num_layers, batch_size, num_samples)
-                 : e->lat_mode ? wn_lat_cond_bytes(num_layers, batch_size, num_samples) : Nz * L * Bz * 2 * R * td);
+    ALLOC(e->Lh, e->family->store_bytes(*e));
     ALLOC(e->sel, Nz * Bz * sizeof(float));
     ALLOC(e->forced, Nz * Bz * sizeof(int));
     ALLOC(e->yPrev, Bz * sizeof(int));
     ALLOC(e->yCur, Bz * sizeof(int));
     ALLOC(e->yOut, Nz * Bz * sizeof(int));
-    size_t ring_bytes = (size_t)(max_dilation + 1) * L * Bz * R * td;
-    if (e->tc_mode) {
-        const size_t tcb = wn_tc_ring_bytes(e->tc_tile, num_layers, max_dilation, batch_size);     // tiled history layout of the tensor-core kernel
-        if (tcb > ring_bytes) ring_bytes = tcb;
-    }
-    if (e->lat_mode) ring_bytes = wn_lat_ring_bytes(num_layers, max_dilation, batch_size);
+    const size_t ring_bytes = e->family->ring_bytes(*e);
     ALLOC(e->ring, ring_bytes);
     ALLOC(e->xtOut, L * Bz * R * sizeof(float));
     ALLOC(e->skipOut, L * Bz * S * sizeof(float));
@@ -317,8 +287,7 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     ALLOC(e->Za, Bz * A * sizeof(float));
     ALLOC(e->P, Bz * A * sizeof(float));
     if (e->stage_elems) ALLOC(e->stage_dev, e->stage_elems * sizeof(float));
-    if (e->tc_mode) ALLOC(e->tc_image, wn_tc_image_bytes(R, S, A, num_layers));
-    if (e->lat_mode) ALLOC(e->tc_image, wn_lat_image_bytes(S, num_layers));
+    if (e->family->pack) ALLOC(e->image, e->family->image_bytes(*e));
 #undef ALLOC
     cudaMemsetAsync(e->blob, 0, e->blob_bytes, 0);
     cudaMemsetAsync(e->yOut, 0, Nz * Bz * sizeof(int), 0);
@@ -335,7 +304,7 @@ int nvwn_destroy(nvwn_engine* e)
 {
     if (!e) return 0;
     void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
-                    e->Zs, e->Za, e->P, e->stage_dev, e->tc_image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch};
+                    e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
@@ -347,7 +316,7 @@ int nvwn_set_embeddings(nvwn_engine* e, const float* embedPrev, const float* emb
     int rc;
     if ((rc = upload(e, e->blob + e->o_embPrev, embedPrev, (size_t)e->A * e->R))) return rc;
     if ((rc = upload(e, e->blob + e->o_embCur, embedCur, (size_t)e->A * e->R))) return rc;
-    e->tc_dirty = e->score_dirty = true;
+    e->image_dirty = e->score_dirty = true;
     CK(cudaStreamSynchronize(0));
     return 0;
 }
@@ -366,7 +335,7 @@ int nvwn_set_layer_weights(nvwn_engine* e, int layer, const float* Wprev, const 
     if ((rc = upload(e, e->blob + e->o_Bres + l * R * td, Bres, R))) return rc;
     if ((rc = upload(e, e->blob + e->o_Wskip + l * S * R * td, Wskip, S * R))) return rc;
     if ((rc = upload(e, e->blob + e->o_Bskip + l * S * td, Bskip, S))) return rc;
-    e->tc_dirty = e->score_dirty = true;
+    e->image_dirty = e->score_dirty = true;
     CK(cudaStreamSynchronize(0));       // sources may be freed by the caller right after return
     return 0;
 }
@@ -380,7 +349,7 @@ int nvwn_set_out_weights(nvwn_engine* e, const float* Wzs, const float* Bzs, con
     if ((rc = upload(e, e->blob + e->o_Bzs, Bzs, A))) return rc;
     if ((rc = upload(e, e->blob + e->o_Wza, Wza, A * A))) return rc;
     if ((rc = upload(e, e->blob + e->o_Bza, Bza, A))) return rc;
-    e->tc_dirty = e->score_dirty = true;
+    e->image_dirty = e->score_dirty = true;
     CK(cudaStreamSynchronize(0));
     return 0;
 }
@@ -511,29 +480,10 @@ int nvwn_set_conditioning(nvwn_engine* e, const float* Lh, int first_sample, int
 {
     if (!e || !Lh) return fail(NVWN_EINVAL, "nvwn_set_conditioning: NULL argument");
     if (first_sample < 0 || num_samples < 0 || first_sample + num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_set_conditioning: sample range out of bounds");
-    const size_t per = (size_t)e->L * e->B * 2 * e->R;
-    if (!e->tc_mode && !e->lat_mode)
-        return upload(e, static_cast<char*>(e->Lh) + (size_t)first_sample * per * e->td, Lh, per * num_samples, (cudaStream_t)stream);
-    // tensor-core layout: fp16, tiled per 32 / 64 / 128 utterances, 128-byte rows pre-swizzled so that TMA drops them straight into
-    // an MMA operand tile (wn_tc_kernel.cu).  Host sources bounce through the staging buffer in whole samples.
     cudaStream_t st = (cudaStream_t)stream;
-    auto convert = [&](const float* src_dev, int first, int n) {
-        return e->lat_mode ? wn_lat_cond_convert(e->Lh, src_dev, first, n, e->L, e->B, st)
-                           : wn_tc_cond_convert(e->Lh, src_dev, first, n, e->tc_tile, e->L, e->B, st);
-    };
-    if (is_device_ptr(Lh)) {
-        CK(convert(Lh, first_sample, num_samples));
-        return 0;
-    }
-    const int chunk = (int)(e->stage_elems / per);
-    if (chunk < 1) return fail(NVWN_ENOMEM, "nvwn_set_conditioning: staging buffer smaller than one sample of conditioning");
-    for (int done = 0; done < num_samples; done += chunk) {
-        const int m = (num_samples - done < chunk) ? num_samples - done : chunk;
-        CK(cudaMemcpyAsync(e->stage_dev, Lh + (size_t)done * per, (size_t)m * per * sizeof(float), cudaMemcpyHostToDevice, st));
-        CK(convert(e->stage_dev, first_sample + done, m));
-    }
-    CK(cudaStreamSynchronize(st));      // host source: the header promises the data is copied before return
-    return 0;
+    return feed(e, Lh, num_samples, (size_t)e->L * e->B * 2 * e->R, st, [&](const float* src, size_t first, size_t m) {
+        return e->family->convert(*e, e->Lh, src, first_sample + (int)first, (int)m, st);
+    });
 }
 
 int nvwn_set_inputs(nvwn_engine* e, const float* Lh, const float* selectors)
@@ -567,7 +517,7 @@ int nvwn_weight_blob(nvwn_engine* e, void** dev_ptr, unsigned long long* bytes)
 int nvwn_weights_updated(nvwn_engine* e)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_weights_updated: NULL engine");
-    e->tc_dirty = e->score_dirty = true;
+    e->image_dirty = e->score_dirty = true;
     return 0;
 }
 
@@ -582,25 +532,13 @@ int nvwn_run_partial(nvwn_engine* e, int init_sample, int count, int num_samples
     WnParams p;
     fill_params(e, p, init_sample, count, num_samples, batch_size, dump_activations ? 1 : 0);
     if (count > 0) {
-        if (e->lat_mode) {
-            // a smaller batch_size runs the first batch_size utterances of the engine's batch (conditioning was laid out per
-            // 16-utterance tile for the engine's batch size at upload)
-            if (e->tc_dirty) {
-                CK(wn_lat_pack(e->tc_image, p, stream));
-                e->tc_dirty = false;
-            }
-            CK(wn_launch_lat(p, e->tc_image, e->B, e->lat_cluster, stream, &e->last));
-        } else if (e->tc_mode) {
-            if (batch_size != e->B)
-                return fail(NVWN_EINVAL, "nvwn_run_partial: the tensor-core path needs batch_size equal to the engine's batch size");
-            if (e->tc_dirty) {
-                CK(wn_tc_pack(e->tc_image, p, stream));
-                e->tc_dirty = false;
-            }
-            CK(wn_launch_tc(p, e->tc_image, e->tc_tile, e->tc_fused, stream, &e->last));
-        } else {
-            CK(wn_launch_stream(p, e->dtype == NVWN_FP16 ? 1 : (e->dtype == NVWN_FP32_FAST ? 2 : 0), stream, &e->last));
+        if (e->family->whole_batch && batch_size != e->B)
+            return fail(NVWN_EINVAL, "nvwn_run_partial: the tensor-core path needs batch_size equal to the engine's batch size");
+        if (e->family->pack && e->image_dirty) {
+            CK(e->family->pack(e->image, p, stream));
+            e->image_dirty = false;
         }
+        CK(e->family->launch(*e, p, e->image, stream, &e->last));
         e->launches++;
     }
     if (yOut) CK(cudaMemcpyAsync(yOut, e->yOut, (size_t)num_samples * batch_size * sizeof(int), cudaMemcpyDefault, stream));
@@ -762,7 +700,7 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
     float* lgt = reinterpret_cast<float*>(sc + o.lgt);
     for (int t0 = 0; t0 < N; t0 += T) {
         const int Tc = N - t0 < T ? N - t0 : T;
-        CK(cond_readback(e, reinterpret_cast<float*>(sc + o.lh), t0, Tc, st));
+        CK(e->family->readback(*e, reinterpret_cast<float*>(sc + o.lh), e->Lh, t0, Tc, st));
         c.t0 = t0; c.T = Tc;
         c.logits = logits ? (logits_dev ? logits : lgt) : nullptr;
         c.logits_ld = logits_dev ? (long long)N * A : (long long)Tc * A;
@@ -799,7 +737,7 @@ int nvwn_debug_get_conditioning(nvwn_engine* e, float* out, int first_sample, in
     if (n == 0) return 0;
     float* tmp = nullptr;
     CK(cudaMalloc((void**)&tmp, n * sizeof(float)));
-    cudaError_t ce = cond_readback(e, tmp, first_sample, num_samples, 0);
+    cudaError_t ce = e->family->readback(*e, tmp, e->Lh, first_sample, num_samples, 0);
     if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
     cudaFree(tmp);
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_conditioning: ") + cudaGetErrorString(ce));

@@ -1542,33 +1542,33 @@ bool wn_lat_supported(int R_, int S, int A_, int L)
 {
     return R_ == R && A_ == A && (S == 128 || S == 256) && L >= 4 && L <= MAXL;     // L >= 4: history prefetch runs 3 steps ahead (single-CTA kernel)
 }
-int wn_lat_tiles(int B) { return (B + TU - 1) / TU; }
-size_t wn_lat_image_bytes(int S, int L) { return lat_image(S, L).total; }
-size_t wn_lat_ring_bytes(int L, int maxDil, int B) { return (size_t)(maxDil + 1) * L * wn_lat_tiles(B) * 2048; }
-size_t wn_lat_cond_bytes(int L, int B, int N) { return (size_t)N * L * wn_lat_tiles(B) * 4096; }
+static int lat_tiles(int B) { return (B + TU - 1) / TU; }
+static size_t image_bytes(const WnConfig& c) { return lat_image(c.S, c.L).total; }
+static size_t ring_bytes(const WnConfig& c) { return (size_t)(c.maxDil + 1) * c.L * lat_tiles(c.B) * 2048; }
+static size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * lat_tiles(c.B) * 4096; }
 
-cudaError_t wn_lat_cond_convert(void* dst, const float* src_dev, int first_sample, int nsamples, int L, int B, cudaStream_t stream)
+static cudaError_t cond_convert(const WnConfig& c, void* dst, const float* src_dev, int first_sample, int nsamples, cudaStream_t stream)
 {
     if (nsamples <= 0) return cudaSuccess;
-    const int ntiles = wn_lat_tiles(B);
-    const size_t total = (size_t)nsamples * L * ntiles * 256;
+    const int ntiles = lat_tiles(c.B);
+    const size_t total = (size_t)nsamples * c.L * ntiles * 256;
     size_t blocks = (total + 255) / 256;
     if (blocks > 132 * 32) blocks = 132 * 32;
-    lat_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, L, B, ntiles);
+    lat_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, c.L, c.B, ntiles);
     return cudaGetLastError();
 }
 
-cudaError_t wn_lat_cond_readback(float* dst_dev, const void* store, int first_sample, int nsamples, int L, int B, cudaStream_t stream)
+static cudaError_t cond_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int nsamples, cudaStream_t stream)
 {
     if (nsamples <= 0) return cudaSuccess;
-    const size_t total = (size_t)nsamples * L * B * 64;
+    const size_t total = (size_t)nsamples * c.L * c.B * 64;
     size_t blocks = (total + 255) / 256;
     if (blocks > 132 * 32) blocks = 132 * 32;
-    lat_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, L, B, wn_lat_tiles(B));
+    lat_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, c.L, c.B, lat_tiles(c.B));
     return cudaGetLastError();
 }
 
-cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream)
+static cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream)
 {
     const LatImage im = lat_image(p.S, p.L);
     cudaError_t e = cudaMemsetAsync(image, 0, im.total, stream);
@@ -1657,10 +1657,13 @@ static cudaError_t lat2_launch_S(const WnParams& p, const unsigned char* im8, in
 
 int wn_lat_max_clusters(int S) { return S == 256 ? lat2_max_clusters<256>() : S == 128 ? lat2_max_clusters<128>() : 0; }
 
-// cluster: serve every 16-utterance tile with a cluster of three CTAs (chain / tail / prep) instead of one
-cudaError_t wn_launch_lat(const WnParams& p, const void* image, int engine_B, bool cluster, cudaStream_t stream, WnLaunchInfo* info)
+// c.lat_cluster: serve every 16-utterance tile with a cluster of three CTAs (chain / tail / prep) instead of one.  A run of fewer
+// utterances than the engine holds takes the first p.B of them: the conditioning store and the history ring stay laid out per
+// 16-utterance tile of the engine's batch.
+static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info)
 {
-    const int grid = wn_lat_tiles(p.B), ntiles_alloc = wn_lat_tiles(engine_B);
+    const bool cluster = c.lat_cluster;
+    const int grid = lat_tiles(p.B), ntiles_alloc = lat_tiles(c.B);
     const unsigned char* im8 = static_cast<const unsigned char*>(image);
     size_t smem = 0;
     cudaError_t e;
@@ -1671,13 +1674,15 @@ cudaError_t wn_launch_lat(const WnParams& p, const void* image, int engine_B, bo
         else if (p.S == 128) e = lat2_launch_S<128>(p, im8, grid, ntiles_alloc, stream, &smem);
         else return cudaErrorInvalidValue;
         if (e != cudaSuccess) return e;
-        if (info) { info->kernel = 18; info->grid = NCL * grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = NCL; }
+        if (info) { info->kernel = NVWN_KERNEL_LATENCY; info->grid = NCL * grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = NCL; }
         return cudaGetLastError();
     }
     if (p.S == 256) e = lat_launch_S<256>(p, im8, grid, ntiles_alloc, stream, &smem);
     else if (p.S == 128) e = lat_launch_S<128>(p, im8, grid, ntiles_alloc, stream, &smem);
     else return cudaErrorInvalidValue;
     if (e != cudaSuccess) return e;
-    if (info) { info->kernel = 18; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = 1; }
+    if (info) { info->kernel = NVWN_KERNEL_LATENCY; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = 1; }
     return cudaGetLastError();
 }
+
+const WnFamily wn_lat_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, wn_lat_pack, wn_launch_lat, false};

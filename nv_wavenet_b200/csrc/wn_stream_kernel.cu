@@ -618,15 +618,14 @@ cudaError_t launch_kernel(const WnParams& p, cudaStream_t stream, WnLaunchInfo* 
     return cudaGetLastError();
 }
 
-// fp32: weights through the shared-memory ring when the output layers fit one row per thread and every matrix starts on a
-// 16-byte boundary (bulk copies); NVWN_STREAM_RING=0 keeps the per-thread L2 loads
+// fp32: weights through the shared-memory ring when the engine allows it (WnConfig::stream_ring), the output layers fit one row
+// per thread and every matrix starts on a 16-byte boundary (bulk copies); otherwise per-thread L2 loads
 template <typename TD, int R, int S, int BT, bool FAST>
-cudaError_t launch_one(const WnParams& p, cudaStream_t stream, WnLaunchInfo* info)
+cudaError_t launch_one(const WnParams& p, bool ring, cudaStream_t stream, WnLaunchInfo* info)
 {
     if constexpr (std::is_same<TD, float>::value && R <= 64) {                 // (R = 128: measured slower than the per-thread loads)
-        static const bool want = [] { const char* v = getenv("NVWN_STREAM_RING"); return !v || atoi(v) != 0; }();
         const void* mats[] = {p.Wprev, p.Wcur, p.Wres, p.Wskip, p.Wzs, p.Wza};
-        bool ok = want && p.A <= Shape<R, S>::NT && p.A % 32 == 0;
+        bool ok = ring && p.A <= Shape<R, S>::NT && p.A % 32 == 0;
         for (const void* m : mats) ok = ok && (reinterpret_cast<uintptr_t>(m) & 15) == 0;
         const size_t smem = stream_smem_floats<R, S, BT>(p.A, p.L) * sizeof(float) + 128 + (size_t)RingCfg<R, S>::SLOTS * RingCfg<R, S>::PIECE + 64;
         if (ok && smem <= 232448) return launch_kernel<TD, R, S, BT, FAST, true>(p, stream, info);
@@ -635,23 +634,49 @@ cudaError_t launch_one(const WnParams& p, cudaStream_t stream, WnLaunchInfo* inf
 }
 
 template <typename TD, int R, int S, bool FAST>
-cudaError_t launch_bt(const WnParams& p, int bt, cudaStream_t stream, WnLaunchInfo* info)
+cudaError_t launch_bt(const WnParams& p, int bt, bool ring, cudaStream_t stream, WnLaunchInfo* info)
 {
     switch (bt) {
-        case 4: return launch_one<TD, R, S, 4, FAST>(p, stream, info);
-        case 2: return launch_one<TD, R, S, 2, FAST>(p, stream, info);
-        default: return launch_one<TD, R, S, 1, FAST>(p, stream, info);
+        case 4: return launch_one<TD, R, S, 4, FAST>(p, ring, stream, info);
+        case 2: return launch_one<TD, R, S, 2, FAST>(p, ring, stream, info);
+        default: return launch_one<TD, R, S, 1, FAST>(p, ring, stream, info);
     }
 }
 
 template <typename TD, bool FAST>
-cudaError_t launch_shape(const WnParams& p, int bt, cudaStream_t stream, WnLaunchInfo* info)
+cudaError_t launch_shape(const WnParams& p, int bt, bool ring, cudaStream_t stream, WnLaunchInfo* info)
 {
-    if (p.R == 32 && p.S == 128) return launch_bt<TD, 32, 128, FAST>(p, bt, stream, info);
-    if (p.R == 64 && p.S == 128) return launch_bt<TD, 64, 128, FAST>(p, bt, stream, info);
-    if (p.R == 64 && p.S == 256) return launch_bt<TD, 64, 256, FAST>(p, bt, stream, info);
-    if (p.R == 128 && p.S == 256) return launch_bt<TD, 128, 256, FAST>(p, bt, stream, info);
+    if (p.R == 32 && p.S == 128) return launch_bt<TD, 32, 128, FAST>(p, bt, ring, stream, info);
+    if (p.R == 64 && p.S == 128) return launch_bt<TD, 64, 128, FAST>(p, bt, ring, stream, info);
+    if (p.R == 64 && p.S == 256) return launch_bt<TD, 64, 256, FAST>(p, bt, ring, stream, info);
+    if (p.R == 128 && p.S == 256) return launch_bt<TD, 128, 256, FAST>(p, bt, ring, stream, info);
     return cudaErrorInvalidValue;
+}
+
+// Batch tile per CTA: the engine's forced one (WnConfig::stream_bt) if it divides the run's batch, else chosen here.  Every CTA
+// re-reads all weights from L2 each sample, so L2 traffic per step is (B / BT) * weight_bytes; keep that under ~128 MB/step while
+// using as many SMs as possible.
+int pick_bt(const WnParams& p, bool fp16, int forced)
+{
+    if (forced && p.B % forced == 0) return forced;
+    const double wbytes = (fp16 ? 2.0 : 4.0) * ((double)p.L * (5.0 * p.R * p.R + (double)p.S * p.R) + (double)p.A * p.S + (double)p.A * p.A);
+    int bt = 1;
+    while (bt < 4 && p.B % (bt * 2) == 0 && ((double)(p.B / bt) * wbytes > 128e6 || p.B / bt > 296)) bt *= 2;
+    return bt;
+}
+
+size_t ring_bytes(const WnConfig& c) { return (size_t)(c.maxDil + 1) * c.L * c.B * c.R * (c.dtype == NVWN_FP16 ? sizeof(__half) : sizeof(float)); }
+
+// NVWN_FP32: bit-exact (CPU model's operation order); NVWN_FP16: fp16 storage; NVWN_FP32_FAST: the reference GPU kernels' arithmetic
+cudaError_t wn_launch_stream(const WnConfig& c, const WnParams& p, const void*, cudaStream_t stream, WnLaunchInfo* info)
+{
+    const bool fp16 = c.dtype == NVWN_FP16;
+    if (!wn_stream_supported(p.R, p.S, p.A, fp16)) return cudaErrorInvalidValue;
+    const int bt = pick_bt(p, fp16, c.stream_bt);
+    if (info) info->kernel = NVWN_KERNEL_STREAM;
+    if (fp16) return launch_shape<__half, false>(p, bt, c.stream_ring, stream, info);
+    return c.dtype == NVWN_FP32_FAST ? launch_shape<float, true>(p, bt, c.stream_ring, stream, info)
+                                     : launch_shape<float, false>(p, bt, c.stream_ring, stream, info);
 }
 
 }  // namespace
@@ -662,27 +687,5 @@ bool wn_stream_supported(int R, int S, int A, bool)
     return shape && A % 32 == 0 && A >= 32 && A <= 4096;
 }
 
-// Batch tile per CTA: every CTA re-reads all weights from L2 each sample, so L2 traffic per step is
-// (B / BT) * weight_bytes; keep that under ~128 MB/step while using as many SMs as possible.
-static int pick_bt(const WnParams& p, bool fp16)
-{
-    if (const char* env = getenv("NVWN_STREAM_BT")) {
-        const int v = atoi(env);
-        if ((v == 1 || v == 2 || v == 4) && p.B % v == 0) return v;
-    }
-    const double wbytes = (fp16 ? 2.0 : 4.0) * ((double)p.L * (5.0 * p.R * p.R + (double)p.S * p.R) + (double)p.A * p.S + (double)p.A * p.A);
-    int bt = 1;
-    while (bt < 4 && p.B % (bt * 2) == 0 && ((double)(p.B / bt) * wbytes > 128e6 || p.B / bt > 296)) bt *= 2;
-    return bt;
-}
-
-// contract: 0 = fp32 bit-exact (CPU model's operation order), 1 = fp16 storage, 2 = fp32 in the reference GPU kernels' arithmetic
-cudaError_t wn_launch_stream(const WnParams& p, int contract, cudaStream_t stream, WnLaunchInfo* info)
-{
-    const bool fp16 = contract == 1;
-    if (!wn_stream_supported(p.R, p.S, p.A, fp16)) return cudaErrorInvalidValue;
-    const int bt = pick_bt(p, fp16);
-    if (info) info->kernel = 16;
-    if (fp16) return launch_shape<__half, false>(p, bt, stream, info);
-    return contract == 2 ? launch_shape<float, true>(p, bt, stream, info) : launch_shape<float, false>(p, bt, stream, info);
-}
+// the kernels read the weight blob and the plain conditioning store (wn_convert.cu); any batch up to the engine's
+const WnFamily wn_stream_family = {wn_plain_store_bytes, ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, nullptr, wn_launch_stream, false};

@@ -26,8 +26,6 @@
 #include "wn_math.cuh"
 #include "wn_sm90.cuh"
 
-#include <stdlib.h>
-
 namespace {
 
 using namespace sm90;
@@ -649,55 +647,35 @@ int pick_nstage()
     return 0;
 }
 
-}  // namespace
+// the conditioning store and the history ring are laid out per tile of c.tc_tile utterances
+size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * cond_bpad(c.B, c.tc_tile) * 256; }
 
-bool wn_tc_supported(int R_, int S, int A_, int, int)
+size_t ring_bytes(const WnConfig& c)
 {
-    return R_ == R && A_ == A && (S == 128 || S == 256);
+    const size_t tiled = (size_t)(c.maxDil + 1) * c.L * ((c.B + c.tc_tile - 1) / c.tc_tile) * TILE;
+    const size_t plain = wn_stream_family.ring_bytes(c);
+    return tiled > plain ? tiled : plain;
 }
 
-size_t wn_tc_image_bytes(int, int S, int, int L) { return tc_image(S, L).total; }
+size_t image_bytes(const WnConfig& c) { return tc_image(c.S, c.L).total; }
 
-// Utterances per tile (the conditioning store and the history ring are laid out per tile, so an engine resolves it once):
-// 64 unless NVWN_TC_TILE (32 | 64 | 128) or NVWN_TC_NODUP (128) asks for another shape.
-int wn_tc_tile_utt(int, int)
-{
-    if (getenv("NVWN_TC_NODUP")) return 128;
-    if (const char* v = getenv("NVWN_TC_TILE")) { const int t = atoi(v); if (t == 128 || t == 64 || t == 32) return t; }
-    return TU;
-}
-
-// schedule of an engine, resolved once at creation: "0" / "1" in NVWN_TC_FUSED force one; unfused by default
-bool wn_tc_fused_default()
-{
-    const char* fv = getenv("NVWN_TC_FUSED");
-    return fv ? fv[0] != '0' : false;
-}
-
-size_t wn_tc_ring_bytes(int TU_, int L, int maxDil, int B)
-{
-    return (size_t)(maxDil + 1) * L * ((B + TU_ - 1) / TU_) * TILE;
-}
-
-size_t wn_tc_cond_bytes(int TU_, int L, int B, int N) { return (size_t)N * L * cond_bpad(B, TU_) * 256; }
-
-cudaError_t wn_tc_cond_convert(void* dst, const float* src_dev, int first_sample, int nsamples, int TU_, int L, int B, cudaStream_t stream)
+cudaError_t cond_convert(const WnConfig& c, void* dst, const float* src_dev, int first_sample, int nsamples, cudaStream_t stream)
 {
     if (nsamples <= 0) return cudaSuccess;
-    const size_t total = (size_t)nsamples * L * B * 16;
+    const size_t total = (size_t)nsamples * c.L * c.B * 16;
     size_t blocks = (total + 255) / 256;
     if (blocks > 4096) blocks = 4096;
-    tc_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, L, B, TU_);
+    tc_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, c.L, c.B, c.tc_tile);
     return cudaGetLastError();
 }
 
-cudaError_t wn_tc_cond_readback(float* dst_dev, const void* store, int first_sample, int nsamples, int TU_, int L, int B, cudaStream_t stream)
+cudaError_t cond_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int nsamples, cudaStream_t stream)
 {
     if (nsamples <= 0) return cudaSuccess;
-    const size_t total = (size_t)nsamples * L * B * 16;
+    const size_t total = (size_t)nsamples * c.L * c.B * 16;
     size_t blocks = (total + 255) / 256;
     if (blocks > 4096) blocks = 4096;
-    tc_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, L, B, TU_);
+    tc_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, c.L, c.B, c.tc_tile);
     return cudaGetLastError();
 }
 
@@ -710,8 +688,10 @@ cudaError_t wn_tc_pack(void* image, const WnParams& p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-cudaError_t wn_launch_tc(const WnParams& p, const void* tc_image_, int tu, bool fused, cudaStream_t stream, WnLaunchInfo* info)
+cudaError_t wn_launch_tc(const WnConfig& c, const WnParams& p, const void* tc_image_, cudaStream_t stream, WnLaunchInfo* info)
 {
+    const int tu = c.tc_tile;
+    const bool fused = c.tc_fused;
     const int nstage = pick_nstage();
     if (nstage < 5 || (tu != 32 && tu != 64 && tu != 128)) return cudaErrorInvalidValue;
     const size_t smem = tc_smem_bytes(nstage);
@@ -727,6 +707,15 @@ cudaError_t wn_launch_tc(const WnParams& p, const void* tc_image_, int tu, bool 
     if (p.S == 256) { if (fused) WN_TC_LAUNCH(256, true); else WN_TC_LAUNCH(256, false); }
     else { if (fused) WN_TC_LAUNCH(128, true); else WN_TC_LAUNCH(128, false); }
 #undef WN_TC_LAUNCH
-    if (info) { info->kernel = 17; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = tu < TU ? tu : TU; info->cluster = 1; }
+    if (info) { info->kernel = NVWN_KERNEL_TENSORCORE; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = tu < TU ? tu : TU; info->cluster = 1; }
     return cudaGetLastError();
 }
+
+}  // namespace
+
+bool wn_tc_supported(int R_, int S, int A_, int, int)
+{
+    return R_ == R && A_ == A && (S == 128 || S == 256);
+}
+
+const WnFamily wn_tc_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, wn_tc_pack, wn_launch_tc, true};

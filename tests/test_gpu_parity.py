@@ -94,6 +94,34 @@ def test_fp32_bit_exact_fresh_shapes(shape, gen, monkeypatch):
         assert len(np.unique(y)) > 8          # a non-degenerate sampled distribution
 
 
+def test_stream_switches_are_read_at_engine_creation(monkeypatch):
+    """NVWN_STREAM_BT and NVWN_STREAM_RING hold for an engine from its creation on: changing them later does not reach its
+    launches, and every new engine reads them again."""
+    R, S, A, L, B, N, md = 64, 128, 256, 3, 4, 12, 4
+    w = refgen.lively_inputs(8, R, S, A, L, B, N)
+    monkeypatch.delenv("NVWN_STREAM_RING", raising=False)
+    monkeypatch.setenv("NVWN_STREAM_BT", "4")
+    e = gpu_engine(w, L, B, N, R, S, A, md)
+    monkeypatch.setenv("NVWN_STREAM_BT", "1")
+    assert e.run(N, B, np.zeros((B, N), np.int32)); e.synchronize()
+    assert e.launch_info()["batch_per_cta"] == 4
+    monkeypatch.delenv("NVWN_STREAM_BT")
+
+    NT = max(4 * R, R + S, 128)                     # threads of the stream kernel; the weight ring adds one warp
+    blocks, ys = [], []
+    for ring in ("0", None):
+        if ring is None:
+            monkeypatch.delenv("NVWN_STREAM_RING")
+        else:
+            monkeypatch.setenv("NVWN_STREAM_RING", ring)
+        e = gpu_engine(w, L, B, N, R, S, A, md)
+        y = np.zeros((B, N), np.int32)
+        assert e.run(N, B, y); e.synchronize()
+        blocks.append(e.launch_info()["block"]); ys.append(y)
+    assert blocks == [NT, NT + 32]
+    assert np.array_equal(ys[0], ys[1])
+
+
 def test_fp32_no_tanh_embed_and_forced_history():
     """tanhEmbed=false (the PyTorch export path, pytorch/wavenet.py:153-154) and teacher forcing."""
     R, S, A, L, B, N, md = 64, 256, 256, 4, 4, 20, 8
@@ -217,7 +245,7 @@ def _select_fp16_kernel(kernel, monkeypatch):
         monkeypatch.setenv("NVWN_FP16_KERNEL", "lat"); monkeypatch.setenv("NVWN_LAT_CLUSTER", "0")
     else:                                          # tensor-core (wgmma) kernel; "tc" = the default 64-utterance tiles, unfused schedule
         monkeypatch.setenv("NVWN_FP16_KERNEL", "tc")
-        if kernel == "tc_nodup":                   # 128-utterance tiles, two CTAs per tile (see wn_tc_tile_utt)
+        if kernel == "tc_nodup":                   # 128-utterance tiles, two CTAs per tile (see resolve_config in wn_engine.cu)
             monkeypatch.setenv("NVWN_TC_NODUP", "1")
         if kernel == "tc_tile32_fused":            # 32-utterance tiles run the fused schedule
             monkeypatch.setenv("NVWN_TC_TILE", "32")
