@@ -907,10 +907,6 @@ __device__ __forceinline__ void st_async_v4(uint32_t raddr, float a, float b, fl
 {
     st_async_v4(raddr, make_uint4(__float_as_uint(a), __float_as_uint(b), __float_as_uint(c), __float_as_uint(d)), rbar);
 }
-__device__ __forceinline__ void st_async_u32(uint32_t raddr, uint32_t a, uint32_t rbar)
-{
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(raddr), "r"(a), "r"(rbar) : "memory");
-}
 // "this buffer is free again": no data behind it, so no release ordering is paid for
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t raddr) { asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory"); }
 __device__ __forceinline__ void cluster_sync_all()
@@ -1382,6 +1378,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                         const float a0 = __shfl_up_sync(0xffffffffu, incl[0], o), a1 = __shfl_up_sync(0xffffffffu, incl[1], o);
                         if (lane >= o) { incl[0] += a0; incl[1] += a1; }
                     }
+                    int yv[2];                                    // the sampled index of each row
 #pragma unroll
                     for (int r = 0; r < 2; r++) {
                         const float total = __shfl_sync(0xffffffffu, incl[r], 31);
@@ -1393,7 +1390,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                         const unsigned ball = __ballot_sync(0xffffffffu, target < incl[r]);
                         const int lf = ball ? __ffs(ball) - 1 : 31;
                         const int ck = __shfl_sync(0xffffffffu, cntk, lf);
-                        const int y = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
+                        yv[r] = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
                         const int b = tile * TU + 2 * w + r;
                         if (DUMP && b < B) {
                             const float inv = 1.f / total;
@@ -1401,21 +1398,27 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
 #pragma unroll
                             for (int k = 0; k < 8; k++) { p.P[(size_t)b * A + 8 * lane + k] = (e[r][k] - prevv) * inv; prevv = e[r][k]; }
                         }
-                        if (lane == 0) {
-                            int fbk = y;
+                    }
+                    // both rows' indices are chosen before lane 0 stores anything: the shuffles of the second row cannot move past the
+                    // first row's stores, so selecting and storing row by row would run the two selections one after the other
+                    if (lane == 0) {
+                        int fbk[2], yold[2];
+#pragma unroll
+                        for (int r = 0; r < 2; r++) {
+                            const int b = tile * TU + 2 * w + r;
+                            fbk[r] = yv[r];
                             if (b < B) {
-                                p.yOut[(size_t)b * p.N + t] = y;
-                                if (p.forced) fbk = p.forced[(size_t)b * p.N + t];
-                            } else fbk = 128;
-                            const int yold = ys[2 * w + r];
-                            ys[TU + 2 * w + r] = yold;
-                            ys[2 * w + r] = fbk;
-                            // the chain CTA's copy (it reads it after waiting for yfull)
-                            if (t + 1 < t_end) {                  // the chain CTA's copy: data + completion on its yfull barrier
-                                const uint32_t rb = mapa_u32(s_yfull, 0);
-                                st_async_u32(mapa_u32(sm + M::O_YS + (TU + 2 * w + r) * 4, 0), (uint32_t)yold, rb);
-                                st_async_u32(mapa_u32(sm + M::O_YS + (2 * w + r) * 4, 0), (uint32_t)fbk, rb);
-                            }
+                                p.yOut[(size_t)b * p.N + t] = yv[r];
+                                if (p.forced) fbk[r] = p.forced[(size_t)b * p.N + t];
+                            } else fbk[r] = 128;
+                            yold[r] = ys[2 * w + r];
+                            ys[TU + 2 * w + r] = yold[r];
+                            ys[2 * w + r] = fbk[r];
+                        }
+                        if (t + 1 < t_end) {                      // the chain CTA's copy: data + completion on its yfull barrier
+                            const uint32_t rb = mapa_u32(s_yfull, 0);
+                            st_async_v2(mapa_u32(sm + M::O_YS + (TU + 2 * w) * 4, 0), (uint32_t)yold[0], (uint32_t)yold[1], rb);
+                            st_async_v2(mapa_u32(sm + M::O_YS + (2 * w) * 4, 0), (uint32_t)fbk[0], (uint32_t)fbk[1], rb);
                         }
                     }
                 }
