@@ -126,6 +126,15 @@ public:
         return rc == 0;
     }
 
+    /* Not in the reference class: streaming generation of absolute samples [first_sample, first_sample + count) through the
+     * engine's numSamples buffers used as rings, continuing from the last generation; see nvwn_run_stream. */
+    bool run_stream(long long first_sample, int count, int batch_size, bool dumpActivations = false, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_run_stream(m_engine, first_sample, count, batch_size, dumpActivations ? 1 : 0, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
     /* Not in the reference class: teacher-forced scoring, logp[b * num_samples + t] = log p(audio[b][t] | audio[b][0..t),
      * conditioning) for every step at once, and optionally the fp32 logits; see nvwn_score.  fp16 engines only. */
     bool score(const int* audio, int num_samples, int batch_size, float* logp, float* logits = NULL, cudaStream_t stream = 0)

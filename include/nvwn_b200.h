@@ -53,6 +53,10 @@ int nvwn_set_conditioning(nvwn_engine* e, const float* Lh, int first_sample, int
  * batch_size + b, is the first output of Philox-4x32-10 with counter (i, 0) and key `seed`, as (x >> 8) * 2^-24 in [0, 1)
  * (the reference draws them on the host with libc rand(), pytorch/wavenet_infer.cu:92-93).  Asynchronous on `stream`. */
 int nvwn_set_selectors_random(nvwn_engine* e, unsigned long long seed, void* stream);
+/* Streaming (see nvwn_run_stream): the selectors of absolute samples [first_sample, first_sample + num_samples), num_samples <=
+ * num_samples of the engine: selector (t, b) from counter t * batch_size + b, stored at position t mod num_samples.  For t < N
+ * these are the values nvwn_set_selectors_random writes; they do not depend on the engine's num_samples. */
+int nvwn_set_selectors_random_stream(nvwn_engine* e, unsigned long long seed, long long first_sample, int num_samples, void* stream);
 /* host helper (needs no GPU): the selectors exactly as the reference wrapper draws them -- Matrix(batch, samples).randomize(0.5, 1.0)
  * on the caller's libc rand() stream (pytorch/wavenet_infer.cu:92-93, matrix.cpp:38-56) -- into selectors[sample * batch_size + b]. */
 int nvwn_libc_selectors(float* selectors, int batch_size, int sample_count);
@@ -75,6 +79,9 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
                             const float* upsample_weight, const float* upsample_bias, int window, int stride,
                             const float* cond_weight, const float* cond_bias, void* stream);
 int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, int sample_count, void* stream);
+/* Streaming (see nvwn_run_stream): samples [sample_begin, sample_begin + sample_count) of the loaded sequence, sample s stored at
+ * position s mod num_samples; sample_count <= num_samples.  Asynchronous on `stream` like nvwn_cond_producer_run. */
+int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sample_count, void* stream);
 /* The same arithmetic on the host (needs no GPU; test / reference use): Lh [T*stride][L][B][2R], host pointers. */
 int nvwn_cond_from_features_host(float* Lh, const float* features, int batch_size, int n_cond_channels, int num_frames,
                                  const float* upsample_weight, const float* upsample_bias, int window, int stride,
@@ -94,6 +101,15 @@ int nvwn_weights_updated(nvwn_engine* e);
 int nvwn_run_partial(nvwn_engine* e, int init_sample, int count, int num_samples, int batch_size,
                      int* yOut, int dump_activations, void* stream);
 int nvwn_run(nvwn_engine* e, int num_samples, int batch_size, int* yOut, int dump_activations, void* stream);
+/* Streaming generation: utterances of any length through an engine of num_samples = N.  The N-sample buffers are rings: absolute
+ * sample t of the utterance batch uses position t mod N of the conditioning, the selectors, the forced indices and yOut (row stride
+ * N), while the history goes by t itself.  So the result is bit-identical to one engine that holds the whole length.  Generates
+ * absolute samples [first_sample, first_sample + count), count <= N, in at most two launches (split at the wrap; dumps come from the
+ * last).  first_sample must be the engine's next sample: 0 after nvwn_reset_history / nvwn_set_inputs, else the end of the last
+ * generation (nvwn_run_partial / nvwn_run included); any other value is NVWN_EINVAL.  batch_size as for nvwn_run_partial.
+ * Fill the positions of a range (conditioning, selectors, forced indices) before the call, and read them (nvwn_get_yout,
+ * nvwn_get_audio) before a later call overwrites them. */
+int nvwn_run_stream(nvwn_engine* e, long long first_sample, int count, int batch_size, int dump_activations, void* stream);
 /* nv_wavenet.cuh:439-444: 2-D copy of yOut[b][offset .. offset+size) for every b */
 int nvwn_get_yout(nvwn_engine* e, int* yOut, int offset, int size, void* stream);
 /* Output side (SURVEY.md 8f next-3): replaces the host post-processing of pytorch/nv_wavenet_inference.py:55-60 --

@@ -32,6 +32,7 @@ SYMBOLS = {
     "nvwn_set_selectors": (C.c_int, [_vp, _vp]),
     "nvwn_set_conditioning": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp]),
     "nvwn_set_selectors_random": (C.c_int, [_vp, C.c_ulonglong, _vp]),
+    "nvwn_set_selectors_random_stream": (C.c_int, [_vp, C.c_ulonglong, C.c_longlong, C.c_int, _vp]),
     "nvwn_libc_selectors": (C.c_int, [_vp, C.c_int, C.c_int]),
     "nvwn_reset_history": (C.c_int, [_vp]),
     "nvwn_set_forced": (C.c_int, [_vp, _vp]),
@@ -39,12 +40,14 @@ SYMBOLS = {
     "nvwn_weights_updated": (C.c_int, [_vp]),
     "nvwn_run_partial": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp]),
     "nvwn_run": (C.c_int, [_vp, C.c_int, C.c_int, _vp, C.c_int, _vp]),
+    "nvwn_run_stream": (C.c_int, [_vp, C.c_longlong, C.c_int, C.c_int, C.c_int, _vp]),
     "nvwn_get_yout": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp]),
     "nvwn_get_audio": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "nvwn_mulaw_table": (C.c_int, [C.c_int, _vp, _vp, _vp]),
     "nvwn_set_conditioning_from_features": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, _vp]),
     "nvwn_cond_producer_load": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_cond_producer_run": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp]),
+    "nvwn_cond_producer_run_stream": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp]),
     "nvwn_cond_from_features_host": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int]),
     "nvwn_score": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_get_xt_out": (C.c_int, [_vp, C.c_int, _vp]),

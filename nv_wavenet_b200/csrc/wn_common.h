@@ -25,7 +25,7 @@ struct WnParams {
     int L, R, S, A, maxDil;
     int B;              // batch size of this run (stride of Lh / selectors / ring, nv_wavenet.cuh:144)
     int N;              // num_samples of this run (row stride of yOut, singleblock.cuh:245)
-    int init_sample, count;
+    int init_sample, count;                             // buffer positions: Lh, sel, forced and yOut rows (see ring_slot)
     int tanhEmbed, dump;
     // model (TD = float in fp32 mode, __half in fp16 mode)
     const void *embPrev, *embCur;                       // TD [A][R]
@@ -45,7 +45,20 @@ struct WnParams {
     // optional timeline trace of one sample (debug): 3 x 1024 (tag << 48 | clock) words, or NULL
     unsigned long long* trace;
     int trace_t;
+    // Absolute time of step init_sample, for the history only (the buffers are rings in streaming use, DESIGN.md §6):
+    int ring_slot;      // its history-ring slot, t mod (maxDil+1)
+    int hist_t;         // t clamped to maxDil: x_l[t-d] exists iff hist_t + (step - init_sample) >= d, and d <= maxDil
 };
+
+// p with its first k steps dropped (a launch split into pieces)
+inline WnParams wn_params_skip(WnParams p, int k)
+{
+    p.init_sample += k;
+    p.count -= k;
+    p.ring_slot = (p.ring_slot + k) % (p.maxDil + 1);
+    p.hist_t = p.hist_t + k < p.maxDil ? p.hist_t + k : p.maxDil;
+    return p;
+}
 
 struct WnLaunchInfo {
     int kernel, grid, block, smem_bytes, batch_per_cta, cluster;
@@ -104,7 +117,7 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t stream);
 // conversions (wn_convert.cu)
 cudaError_t wn_f32_to_f16(__half* dst, const float* src_dev, size_t n, cudaStream_t stream);
 cudaError_t wn_f16_to_f32(float* dst, const __half* src_dev, size_t n, cudaStream_t stream);
-cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, cudaStream_t stream);
+cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, unsigned long long first, cudaStream_t stream);
 cudaError_t wn_fill_int(int* dst, int value, size_t n, cudaStream_t stream);
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream);

@@ -75,17 +75,18 @@ __host__ __device__ inline unsigned wn_philox_first(unsigned long long ctr, unsi
     }
     return c0;
 }
-__global__ void selectors_kernel(float* __restrict__ dst, size_t n, unsigned long long seed)
+__global__ void selectors_kernel(float* __restrict__ dst, size_t n, unsigned long long seed, unsigned long long first)
 {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        dst[i] = (float)(wn_philox_first(i, seed) >> 8) * (1.0f / 16777216.0f);
+        dst[i] = (float)(wn_philox_first(first + i, seed) >> 8) * (1.0f / 16777216.0f);
 }
-cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, cudaStream_t stream)
+// dst[i] = selector of counter first + i
+cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, unsigned long long first, cudaStream_t stream)
 {
     if (n == 0) return cudaSuccess;
     size_t blocks = (n + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    selectors_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, n, seed);
+    selectors_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, n, seed, first);
     return cudaGetLastError();
 }
 

@@ -61,6 +61,7 @@ struct nvwn_engine : WnConfig {
     bool use_forced = false;
     int *yPrev = nullptr, *yCur = nullptr, *yOut = nullptr;
     void* ring = nullptr;
+    long long next_t = 0;                    // absolute time of the next sample to generate: where nvwn_run_stream must continue
     float *xtOut = nullptr, *skipOut = nullptr, *Zs = nullptr, *Za = nullptr, *P = nullptr;
 
     float* stage_dev = nullptr;              // device fp32 staging for host->fp16 uploads (fp16 engines only)
@@ -165,11 +166,14 @@ void resolve_config(WnConfig& c, int impl)
     c.stream_ring = num("NVWN_STREAM_RING", 1) != 0;
 }
 
-void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, int count, int num_samples, int batch, int dump)
+// init_sample: buffer position of the first step; t_abs: its absolute time in the utterance batch (equal outside streaming use)
+void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, long long t_abs, int count, int num_samples, int batch, int dump)
 {
     memset(&p, 0, sizeof p);
     p.L = e->L; p.R = e->R; p.S = e->S; p.A = e->A; p.maxDil = e->maxDil;
     p.B = batch; p.N = num_samples; p.init_sample = init_sample; p.count = count;
+    p.ring_slot = (int)(t_abs % (e->maxDil + 1));
+    p.hist_t = (int)(t_abs < e->maxDil ? t_abs : e->maxDil);
     p.tanhEmbed = e->tanhEmbed; p.dump = dump;
     p.embPrev = e->blob + e->o_embPrev; p.embCur = e->blob + e->o_embCur;
     p.Wprev = e->blob + e->o_Wprev; p.Wcur = e->blob + e->o_Wcur; p.Wres = e->blob + e->o_Wres; p.Wskip = e->blob + e->o_Wskip;
@@ -179,6 +183,26 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, int count, 
     p.yPrev = e->yPrev; p.yCur = e->yCur; p.ring = e->ring; p.yOut = e->yOut;
     p.xtOut = e->xtOut; p.skipOut = e->skipOut; p.Zs = e->Zs; p.Za = e->Za; p.P = e->P;
     p.trace = e->trace; p.trace_t = e->trace_t;
+}
+
+// One generation launch: `count` steps from buffer position `pos` (pos + count <= num_samples, the yOut row stride), the first at
+// absolute time t_abs.  Moves the engine's next sample to the end of the range.
+int launch_steps(nvwn_engine* e, const char* who, int pos, long long t_abs, int count, int num_samples, int batch, int dump, cudaStream_t stream)
+{
+    WnParams p;
+    fill_params(e, p, pos, t_abs, count, num_samples, batch, dump);
+    if (count > 0) {
+        if (e->family->whole_batch && batch != e->B)
+            return fail(NVWN_EINVAL, std::string(who) + ": the tensor-core path needs batch_size equal to the engine's batch size");
+        if (e->family->pack && e->image_dirty) {
+            CK(e->family->pack(e->image, p, stream));
+            e->image_dirty = false;
+        }
+        CK(e->family->launch(*e, p, e->image, stream, &e->last));
+        e->launches++;
+    }
+    e->next_t = t_abs + count;
+    return 0;
 }
 
 // rows (t, b) of one scoring chunk; bounds the chunk scratch: DESIGN.md §5.4
@@ -395,16 +419,16 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
     return 0;
 }
 
-int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, int sample_count, void* stream)
+}  // extern "C"
+
+namespace {
+
+// conditioning of samples [sample_begin, sample_begin + sample_count) of the loaded sequence into store positions from `pos`; the
+// caller has checked both ranges
+int cond_produce(nvwn_engine* e, int pos, int sample_begin, int sample_count, void* stream)
 {
-    if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: NULL engine");
-    if (!e->cp_scratch || e->cp_T < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: nvwn_cond_producer_load has not been called");
     const int C = e->cp_C, T = e->cp_T, K = e->cp_K, stride = e->cp_stride, chunk = e->cp_chunk;
-    const long long Nn = (long long)T * stride;
-    if (sample_begin < 0 || sample_count < 0 || sample_begin + (long long)sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: sample range outside num_frames * stride");
-    if (first_sample < 0 || first_sample + (long long)sample_begin + sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: samples do not fit the engine");
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t per = (size_t)e->L * e->B * 2 * e->R;
     const size_t n_feat = (size_t)e->B * C * T, n_wu = (size_t)C * C * K, n_wc = (size_t)e->L * 2 * e->R * C, n_bc = (size_t)e->L * 2 * e->R;
     float* d_feat = e->cp_scratch; float* d_wut = d_feat + n_feat + n_wu; float* d_bu = d_wut + n_wu;
     float* d_wc = d_bu + C; float* d_bc = d_wc + n_wc; float* d_u = d_bc + n_bc;
@@ -416,9 +440,36 @@ int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, i
         const long long left = sample_begin + (long long)sample_count - done;
         const int m = (int)(left < chunk ? left : chunk);
         ce = wn_cond_produce(d_out, d_u, d_feat, d_wut, d_bu, d_wc, d_bc, e->B, C, T, K, stride, e->L, e->R, (int)done, m, st);
-        if (ce == cudaSuccess) rc = nvwn_set_conditioning(e, d_out, first_sample + (int)done, m, stream);      // device source: converted in place, stream-ordered
+        if (ce == cudaSuccess) rc = nvwn_set_conditioning(e, d_out, pos + (int)(done - sample_begin), m, stream);      // device source: converted in place, stream-ordered
     }
-    if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_cond_producer_run: ") + cudaGetErrorString(ce));
+    if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_cond_producer: ") + cudaGetErrorString(ce));
+    return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, int sample_count, void* stream)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: NULL engine");
+    if (!e->cp_scratch || e->cp_T < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: nvwn_cond_producer_load has not been called");
+    const long long Nn = (long long)e->cp_T * e->cp_stride;
+    if (sample_begin < 0 || sample_count < 0 || sample_begin + (long long)sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: sample range outside num_frames * stride");
+    if (first_sample < 0 || first_sample + (long long)sample_begin + sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: samples do not fit the engine");
+    return cond_produce(e, first_sample + sample_begin, sample_begin, sample_count, stream);
+}
+
+int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sample_count, void* stream)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: NULL engine");
+    if (!e->cp_scratch || e->cp_T < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: nvwn_cond_producer_load has not been called");
+    const long long Nn = (long long)e->cp_T * e->cp_stride;
+    if (sample_begin < 0 || sample_count < 0 || sample_begin + sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: sample range outside num_frames * stride");
+    if (sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: more samples than the engine's num_samples (" + std::to_string(e->N) + ")");
+    const int pos = (int)(sample_begin % e->N), head = sample_count < e->N - pos ? sample_count : e->N - pos;
+    int rc = cond_produce(e, pos, (int)sample_begin, head, stream);
+    if (rc == 0 && head < sample_count) rc = cond_produce(e, 0, (int)sample_begin + head, sample_count - head, stream);
     return rc;
 }
 
@@ -442,6 +493,7 @@ int nvwn_reset_history(nvwn_engine* e)
     if (!e) return fail(NVWN_EINVAL, "nvwn_reset_history: NULL engine");
     CK(wn_fill_int(e->yPrev, 128, e->B, 0));      // silenceInputs, nv_wavenet.cuh:213-218
     CK(wn_fill_int(e->yCur, 128, e->B, 0));
+    e->next_t = 0;
     return 0;
 }
 
@@ -472,7 +524,19 @@ int nvwn_libc_selectors(float* selectors, int batch_size, int sample_count)
 int nvwn_set_selectors_random(nvwn_engine* e, unsigned long long seed, void* stream)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_set_selectors_random: NULL engine");
-    CK(wn_fill_selectors(e->sel, (size_t)e->N * e->B, seed, (cudaStream_t)stream));
+    CK(wn_fill_selectors(e->sel, (size_t)e->N * e->B, seed, 0, (cudaStream_t)stream));
+    return 0;
+}
+
+int nvwn_set_selectors_random_stream(nvwn_engine* e, unsigned long long seed, long long first_sample, int num_samples, void* stream)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_set_selectors_random_stream: NULL engine");
+    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
+        return fail(NVWN_EINVAL, "nvwn_set_selectors_random_stream: need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) + ") of the engine");
+    const size_t B = e->B;
+    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
+    CK(wn_fill_selectors(e->sel + (size_t)pos * B, (size_t)head * B, seed, (unsigned long long)first_sample * B, (cudaStream_t)stream));
+    CK(wn_fill_selectors(e->sel, (size_t)(num_samples - head) * B, seed, (unsigned long long)(first_sample + head) * B, (cudaStream_t)stream));
     return 0;
 }
 
@@ -529,20 +593,27 @@ int nvwn_run_partial(nvwn_engine* e, int init_sample, int count, int num_samples
         return fail(NVWN_EINVAL, "nvwn_run_partial: batch_size / num_samples exceed what the engine was created for");
     if (init_sample < 0 || count < 0 || init_sample + count > num_samples) return fail(NVWN_EINVAL, "nvwn_run_partial: sample range out of bounds");
     cudaStream_t stream = (cudaStream_t)stream_;
-    WnParams p;
-    fill_params(e, p, init_sample, count, num_samples, batch_size, dump_activations ? 1 : 0);
-    if (count > 0) {
-        if (e->family->whole_batch && batch_size != e->B)
-            return fail(NVWN_EINVAL, "nvwn_run_partial: the tensor-core path needs batch_size equal to the engine's batch size");
-        if (e->family->pack && e->image_dirty) {
-            CK(e->family->pack(e->image, p, stream));
-            e->image_dirty = false;
-        }
-        CK(e->family->launch(*e, p, e->image, stream, &e->last));
-        e->launches++;
-    }
+    const int rc = launch_steps(e, "nvwn_run_partial", init_sample, init_sample, count, num_samples, batch_size, dump_activations ? 1 : 0, stream);
+    if (rc != 0) return rc;
     if (yOut) CK(cudaMemcpyAsync(yOut, e->yOut, (size_t)num_samples * batch_size * sizeof(int), cudaMemcpyDefault, stream));
     return 0;
+}
+
+int nvwn_run_stream(nvwn_engine* e, long long first_sample, int count, int batch_size, int dump_activations, void* stream_)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_run_stream: NULL engine");
+    if (batch_size < 1 || batch_size > e->B) return fail(NVWN_EINVAL, "nvwn_run_stream: batch_size outside [1, B] of the engine");
+    if (first_sample < 0 || count < 0 || count > e->N)
+        return fail(NVWN_EINVAL, "nvwn_run_stream: need first_sample >= 0 and 0 <= count <= num_samples (" + std::to_string(e->N) + ") of the engine");
+    if (first_sample != e->next_t)
+        return fail(NVWN_EINVAL, "nvwn_run_stream: first_sample " + std::to_string(first_sample) + " does not continue the utterance batch: the next sample is " +
+                                     std::to_string(e->next_t) + " (nvwn_reset_history starts over at 0)");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const int pos = (int)(first_sample % e->N), head = count < e->N - pos ? count : e->N - pos;
+    const int dump = dump_activations ? 1 : 0;
+    int rc = launch_steps(e, "nvwn_run_stream", pos, first_sample, head, e->N, batch_size, head == count ? dump : 0, stream);
+    if (rc == 0 && head < count) rc = launch_steps(e, "nvwn_run_stream", 0, first_sample + head, count - head, e->N, batch_size, dump, stream);
+    return rc;
 }
 
 int nvwn_run(nvwn_engine* e, int num_samples, int batch_size, int* yOut, int dump_activations, void* stream)
@@ -679,7 +750,7 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
     }
     if (e->score_dirty) {
         WnParams p;
-        fill_params(e, p, 0, 0, N, Bs, 0);
+        fill_params(e, p, 0, 0, 0, N, Bs, 0);
         CK(wn_score_pack(e->score_image, p, st));
         e->score_dirty = false;
     }

@@ -472,15 +472,17 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
         auto ensure = [&](bool ok, uint32_t bar, uint32_t parity) { if (!ok) mbar_wait(bar, parity); };
 
         // dilated history x_l[t - d] (zero before the start of the utterance, nv_wavenet.cuh:106) of the step `itp`: staged three
-        // steps ahead into a 3-slot shared-memory ring by warps 0-3 (128 threads x 16 B, cp.async; completion on an mbarrier)
-        StepIt itp{t_begin, 0, t_begin % slots};
+        // steps ahead into a 3-slot shared-memory ring by warps 0-3 (128 threads x 16 B, cp.async; completion on an mbarrier).
+        // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
+        StepIt itp{p.hist_t, 0, p.ring_slot};
+        const int h_end = p.hist_t + p.count;
         uint32_t pcnt = 0;                             // tiles staged so far (slot = pcnt % 3)
         auto stage_history = [&]() {
             if (w < 4) {
                 const uint32_t slot3 = pcnt % 3;
                 const int d = dil[itp.l];
                 const uint32_t dst = sm + C::O_PST + slot3 * 2048 + (uint32_t)(w * 32 + lane) * 16;
-                if (itp.t >= t_end || itp.t < d) {
+                if (itp.t >= h_end || itp.t < d) {
                     sts128(dst, make_uint4(0, 0, 0, 0));
                     mbar_arrive(s_pfull + 8 * slot3);
                 } else {
@@ -551,7 +553,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             sts32(sm + C::O_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TU + g] * 32 + 4 * w + t4]);
             sts32(sm + C::O_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
         }
-        StepIt it0{t_begin, 0, t_begin % slots};
+        StepIt it0{t_begin, 0, p.ring_slot};
         stage_history(); stage_history(); stage_history();              // history tiles of steps 0, 1, 2
         {
             it1 = it0; it3 = it0;
@@ -1157,7 +1159,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                 sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TU + g] * 32 + 4 * w + t4]);
                 sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
             }
-            StepIt it0{t_begin, 0, t_begin % slots};
+            StepIt it0{t_begin, 0, p.ring_slot};
             prep(false);                                       // step 0
             bar_compute();
 
@@ -1459,17 +1461,19 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             //  * its dilated history x_l[t-d] (zero before the start of the utterance, nv_wavenet.cuh:106): warps 0-3, 128 x 16 B,
             //    completion on an mbarrier (every warp reads the whole tile).
             // NPS = 8 slots: a slot is staged again five steps after its use, and the weight ring (4 pieces) keeps the warps within four.
-            StepIt itp{t_begin, 0, t_begin % slots};
+            // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
+            StepIt itp{p.hist_t, 0, p.ring_slot};
+            const int h_end = p.hist_t + p.count;
             uint32_t pcnt = 0;
             const unsigned char* cptr = static_cast<const unsigned char*>(p.Lh) + (size_t)tile * 4096 + (size_t)(w * 32 + lane) * 16 + (size_t)t_begin * L * cstride;
             auto stage = [&]() {
                 const uint32_t slot = pcnt & (M::NPS - 1);
-                if (itp.t < t_end) cp_async16(s_cond + slot * 4096, cptr);
+                if (itp.t < h_end) cp_async16(s_cond + slot * 4096, cptr);
                 cptr += cstride;
                 if (w < 4) {
                     const int d = dil[itp.l];
                     const uint32_t dst = sm + M::P_PST + slot * 2048 + (uint32_t)(w * 32 + lane) * 16;
-                    if (itp.t >= t_end || itp.t < d) {
+                    if (itp.t >= h_end || itp.t < d) {
                         sts128(dst, make_uint4(0, 0, 0, 0));
                         mbar_arrive(s_pfull + 8 * slot);
                     } else {
@@ -1639,7 +1643,7 @@ static cudaError_t lat_launch_split(const WnParams& p, LatGo plain, LatGo trace,
                                     cudaStream_t stream)
 {
     WnParams head = p, tail = p;
-    if (p.dump) { head.count = p.count - 1; head.dump = 0; tail.init_sample = p.init_sample + p.count - 1; tail.count = 1; }
+    if (p.dump) { head.count = p.count - 1; head.dump = 0; tail = wn_params_skip(p, p.count - 1); }
     cudaError_t e = cudaSuccess;
     if (head.count > 0) e = (p.trace ? trace : plain)(head, im8, tiles, ntiles_alloc, stream);
     if (e == cudaSuccess && p.dump) e = dump(tail, im8, tiles, ntiles_alloc, stream);

@@ -286,8 +286,12 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
     const int xb = has_x ? tid / R : 0, xr = has_x ? tid % R : 0;
 
     const int t_end = p.init_sample + p.count;
+    // t below is a buffer position; the history goes by the utterance's time (DESIGN.md §6): x_l[t-d] exists iff t + t_hist >= d,
+    // and position t has the ring slot (t + slot_shift) % slots (the sum is >= 0 for every t >= init_sample - maxDil)
+    const int t_hist = p.hist_t - p.init_sample;
+    const int slot_shift = p.ring_slot - p.init_sample % slots + slots;
     auto ring_at = [&](int t, int l, int b, int r) -> TD* {
-        return ring + (((size_t)(t % slots) * L + l) * B + (b0 + b)) * R + r;
+        return ring + (((size_t)((t + slot_shift) % slots) * L + l) * B + (b0 + b)) * R + r;
     };
     auto lh_at = [&](int t, int l, int idx) -> const TD* {
         const int b = idx / (2 * R), row = idx % (2 * R);
@@ -305,7 +309,7 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
             lh_nxt[j] = (idx < NACT && t < t_end) ? N::ldcg(lh_at(t, 0, idx)) : 0.f;
             bh_nxt[j] = (idx < NACT) ? N::ld(Bh + idx % (2 * R)) : 0.f;
         }
-        if (has_x) xp_nxt = (t >= 1) ? N::ldcg(ring_at(t - 1, 0, xb, xr)) : 0.f;
+        if (has_x) xp_nxt = (t + t_hist >= 1) ? N::ldcg(ring_at(t - 1, 0, xb, xr)) : 0.f;
     }
 
     for (int t = p.init_sample; t < t_end; t++) {
@@ -341,7 +345,7 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
                 // x[t-d] of the next layer.  For (t+1, layer 0) the source is this sample's embedding,
                 // written above by this CTA and ordered by the barriers in between.
                 const int dn = dil[ln];
-                xp_nxt = (live && has_x && tn >= dn) ? N::ldcg(ring_at(tn - dn, ln, xb, xr)) : 0.f;
+                xp_nxt = (live && has_x && tn + t_hist >= dn) ? N::ldcg(ring_at(tn - dn, ln, xb, xr)) : 0.f;
             }
 
             // ---- stage 1: a_prev = Wprev.x[t-d], a_cur = Wcur.x[t]  (reference.cpp:61-65) ----

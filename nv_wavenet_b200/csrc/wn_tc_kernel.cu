@@ -226,9 +226,13 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
     const int live = tu < TU ? tu : TU;                            // MMA rows that hold utterances
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
+    // t below is a buffer position; the history goes by the utterance's time (DESIGN.md §6): x_l[t-d] exists iff t + t_hist >= d,
+    // and position t has the ring slot (t + slot_shift) % slots (the sum is >= 0 for every t >= t_begin - maxDil)
+    const int t_hist = p.hist_t - t_begin;
+    const int slot_shift = p.ring_slot - t_begin % slots + slots;
     unsigned char* gring = static_cast<unsigned char*>(p.ring);
     auto ring_tile = [&](int t, int l) -> unsigned char* {
-        return gring + (((size_t)(t % slots) * L + l) * ntiles + tile) * (size_t)TILE + (size_t)row0 * 128;
+        return gring + (((size_t)((t + slot_shift) % slots) * L + l) * ntiles + tile) * (size_t)TILE + (size_t)row0 * 128;
     };
     // conditioning tile geometry (see tc_cond_kernel): [2 halves][c_rows][128 B]; this CTA's rows of each half land in a ring
     // stage at offsets 0 and ATILE
@@ -278,7 +282,7 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
                     const unsigned char* lw = img + (size_t)l * im.layer_bytes;
                     put2(cond_ptr(t, l), c_bytes_here, cond_ptr(t, l) + c_bytes, c_bytes_here);
                     if (t + 1 < t_end && c_bytes_here) tma_prefetch_l2(cond_ptr(t + 1, l), c_bytes_here);
-                    if (t >= d) { put(ring_tile(t - d, l), ATILE); put(lw, TILE); }
+                    if (t + t_hist >= d) { put(ring_tile(t - d, l), ATILE); put(lw, TILE); }
                     put(lw + TILE, TILE);
                     if (FUSED) {
                         if (l > 0) { put(lw + im.l_wf, TILE); res_skip(l - 1); }
@@ -426,7 +430,7 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
             const unsigned char* t_hp = t_hb + (size_t)((l + 1) & 1) * ATILE;                  // FUSED: h_{l-1}
             float acc_a[16], acc_g[16];
             {
-                const bool hp = t >= d;
+                const bool hp = t + t_hist >= d;
                 int sh = 0, sp = 0, sw, sf = 0, sr = 0, sk[SKC];
                 wgmma_fence();
                 if (hp) {

@@ -42,6 +42,19 @@ def _stream(stream):
     return C.c_void_p(int(stream))
 
 
+def split_at_wrap(first_sample, count, num_samples):
+    """Absolute samples [first_sample, first_sample + count) of buffers of `num_samples` used as rings, as at most two pieces
+    (position, offset, n): samples first_sample + offset .. + n - 1 sit at positions position .. position + n - 1."""
+    if first_sample < 0 or count < 0 or count > num_samples:
+        raise ValueError(f"need first_sample >= 0 and 0 <= count <= {num_samples}; got {first_sample}, {count}")
+    pos = first_sample % num_samples
+    head = min(count, num_samples - pos)
+    pieces = [(pos, 0, head)] if head else []
+    if head < count:
+        pieces.append((0, head, count - head))
+    return pieces
+
+
 class NVWavenetInfer:
     """nvWavenetInfer(numLayers, maxDilation, batchSize, numSamples, impl=0, tanhEmbed=True)
     with the template parameters (precision, R, S, A) as keyword arguments."""
@@ -134,6 +147,55 @@ class NVWavenetInfer:
         """Second half: conditioning of samples [sample_begin, sample_begin + sample_count) of the loaded sequence, asynchronously on
         `stream` (record an event after it and make the generating stream wait for it)."""
         check(self._l.nvwn_cond_producer_run(self._h, first_sample, sample_begin, sample_count, _stream(stream)), "condProducerRun")
+
+    # ---- streaming: the N-sample buffers used as rings (nvwn_run_stream); ranges are in absolute samples ----
+    def set_selectors_random_stream(self, seed, first_sample, num_samples, stream=None):
+        """Device selectors of absolute samples [first_sample, first_sample + num_samples), the values set_selectors_random gives
+        an engine that holds them all."""
+        check(self._l.nvwn_set_selectors_random_stream(self._h, C.c_ulonglong(int(seed) & (2 ** 64 - 1)), first_sample, num_samples,
+                                                       _stream(stream)), "setSelectorsRandomStream")
+
+    def cond_producer_run_stream(self, sample_begin, sample_count, stream=None):
+        """cond_producer_run for the ring: sample s of the loaded sequence goes to position s mod N."""
+        check(self._l.nvwn_cond_producer_run_stream(self._h, sample_begin, sample_count, _stream(stream)), "condProducerRunStream")
+
+    def set_conditioning_stream(self, Lh, first_sample, stream=None):
+        """Lh [n][L][B][2R]: the conditioning of absolute samples [first_sample, first_sample + n)."""
+        a, k = _ptr(Lh, np.float32)
+        per = self.L * self.B * 2 * self.R
+        n = (k.size if isinstance(k, np.ndarray) else k.numel()) // per
+        for pos, off, m in split_at_wrap(first_sample, n, self.N):
+            check(self._l.nvwn_set_conditioning(self._h, C.c_void_p(a.value + off * per * 4), pos, m, _stream(stream)), "setConditioning")
+        return k
+
+    def get_yout_stream(self, out, first_sample, count, stream=None):
+        """out [B][count] (numpy int32 array, or int32 torch tensor filled on `stream`) <- yOut of absolute samples
+        [first_sample, first_sample + count)."""
+        if isinstance(out, np.ndarray):
+            stage = np.empty((self.B, self.N), np.int32)
+            for pos, off, n in split_at_wrap(first_sample, count, self.N):
+                self.get_yout(stage, pos, n, stream)
+                out[:, off:off + n] = stage[:, pos:pos + n]
+            return out
+        import contextlib
+        import torch
+        with torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext():
+            stage = torch.empty((self.B, self.N), dtype=torch.int32, device=out.device)     # allocated on the stream that uses it
+            for pos, off, n in split_at_wrap(first_sample, count, self.N):
+                self.get_yout(stage, pos, n, stream if stream is not None else torch.cuda.current_stream())
+                out[:, off:off + n].copy_(stage[:, pos:pos + n])
+        return out
+
+    def get_audio_stream(self, first_sample, count, int16=False, saturate=False, stream=None):
+        """get_audio of absolute samples [first_sample, first_sample + count): numpy [B][count]."""
+        pieces = [self.get_audio(pos, n, int16, saturate, stream=stream) for pos, _, n in split_at_wrap(first_sample, count, self.N)]
+        return np.concatenate(pieces, axis=1) if pieces else np.empty((self.B, 0), np.int16 if int16 else np.float32)
+
+    def run_stream(self, first_sample, count, batch_size, dump_activations=False, stream=None):
+        """Generates absolute samples [first_sample, first_sample + count), count <= N, continuing from the last generation
+        (first_sample 0 after reset_history).  Asynchronous on `stream`."""
+        check(self._l.nvwn_run_stream(self._h, first_sample, count, batch_size, int(dump_activations), _stream(stream)), "run_stream")
+        return True
 
     def reset_history(self):
         check(self._l.nvwn_reset_history(self._h), "resetHistory")

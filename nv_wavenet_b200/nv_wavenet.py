@@ -15,6 +15,7 @@ kernel are those of pytorch/nv_wavenet.py:55-196; the code is organised around o
 """
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -115,25 +116,42 @@ class NVWaveNet:
             self.engines_created += 1
         return eng
 
-    def infer(self, cond_input, implementation, seed=None, fp16=False):
+    def infer(self, cond_input, implementation, seed=None, fp16=False, window=None):
         """cond_input: channels x batch x num_layers x samples (pytorch/nv_wavenet.py:172-196); returns int32 [batch][samples].
-        `implementation` (Impl.*) is accepted for compatibility: one kernel family serves all of them."""
+        `implementation` (Impl.*) is accepted for compatibility: one kernel family serves all of them.
+        window=W generates through one engine of W samples per (batch, W, precision), whatever the length, in windows of W
+        samples (nvwn_run_stream); the result is the same as without a window, bit for bit."""
         if (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
             raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
         batch_size, sample_count = cond_input.size(1), cond_input.size(3)
-        eng = self._engine(batch_size, sample_count, fp16)
+        eng = self._engine(batch_size, sample_count if window is None else window, fp16)
         lh = column_major(cond_input).float()                       # [samples][layers][batch][2R]
         eng.reset_history()
-        eng.set_conditioning(lh, 0, sample_count)
+        sel = None
         if seed is None:                                            # the reference's host draw, on the caller's rand() stream
-            import numpy as np
             sel = np.empty(sample_count * batch_size, np.float32)
             _lib.check(self._lib.nvwn_libc_selectors(C.c_void_p(sel.ctypes.data), batch_size, sample_count), "selectors")
-            eng.set_selectors(sel)
-        else:
-            eng.set_selectors_random(seed)
         samples = torch.empty((batch_size, sample_count), dtype=torch.int32, device="cuda")
-        eng.run(sample_count, batch_size, samples, dump_activations=False)
+        if window is None:
+            eng.set_conditioning(lh, 0, sample_count)
+            if sel is None:
+                eng.set_selectors_random(seed)
+            else:
+                eng.set_selectors(sel)
+            eng.run(sample_count, batch_size, samples, dump_activations=False)
+        else:
+            # windows start at multiples of W, so each one fills the buffers from position 0
+            for first in range(0, sample_count, window):
+                n = min(window, sample_count - first)
+                eng.set_conditioning(lh[first:first + n], 0, n)
+                if sel is None:
+                    eng.set_selectors_random_stream(seed, first, n)
+                else:
+                    chunk = np.zeros(window * batch_size, np.float32)
+                    chunk[:n * batch_size] = sel[first * batch_size:(first + n) * batch_size]
+                    eng.set_selectors(chunk)
+                eng.run_stream(first, n, batch_size)
+                eng.get_yout_stream(samples[:, first:first + n], first, n)
         torch.cuda.synchronize()
         return samples
 
