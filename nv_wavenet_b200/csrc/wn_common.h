@@ -83,7 +83,7 @@ extern const WnFamily wn_lat_family;                // wn_lat_kernel.cu: fp16 la
 bool wn_stream_supported(int R, int S, int A, bool fp16);
 bool wn_tc_supported(int R, int S, int A, int L, int B);
 bool wn_lat_supported(int R, int S, int A, int L);
-int wn_lat_max_clusters(int S);                     // three-CTA clusters of the latency kernel the device runs at once
+int wn_lat_max_clusters(int S, int rows);          // three-CTA clusters of `rows` (8 or 16) utterances the device runs at once
 
 // the plain conditioning store of the stream kernel (wn_convert.cu): [N][L][B][2R], fp16 on NVWN_FP16 engines, else fp32
 size_t wn_plain_store_bytes(const WnConfig& c);

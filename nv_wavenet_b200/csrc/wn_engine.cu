@@ -829,8 +829,9 @@ int nvwn_debug_trace(nvwn_engine* e, int t, unsigned long long* out_host, int fe
     return 0;
 }
 
-// debug only: how many three-CTA clusters of the latency kernel the device runs at once (batches up to 16 x this use it)
-int nvwn_debug_lat_max_clusters(int S) { return wn_lat_max_clusters(S); }
+// debug only: how many three-CTA clusters of `rows` (8 or 16) utterances the latency kernel runs at once (batches up to rows x this
+// can use that tile height)
+int nvwn_debug_lat_max_clusters(int S, int rows) { return wn_lat_max_clusters(S, rows); }
 
 int nvwn_get_launch_info(nvwn_engine* e, nvwn_launch_info* info)
 {

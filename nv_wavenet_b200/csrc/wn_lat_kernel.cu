@@ -145,6 +145,7 @@ __device__ __forceinline__ void ldg_nc_v4_if(uint4& d, const void* p, bool pred)
                  : "+r"(d.x), "+r"(d.y), "+r"(d.z), "+r"(d.w) : "l"(p), "r"((uint32_t)pred) : "memory");
 }
 __device__ __forceinline__ void stg_v2(void* p, uint32_t a, uint32_t b) { asm volatile("st.global.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(a), "r"(b) : "memory"); }
+__device__ __forceinline__ void stg_b32(void* p, uint32_t a) { asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(a) : "memory"); }
 __device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, %0;" ::"n"(NCT) : "memory"); }
 using wn::pack_h2;
 using wn::unpack_h2;
@@ -289,20 +290,54 @@ __global__ void lat_pack_kernel(WnParams p, unsigned char* __restrict__ img, Lat
 // ------------------------------------------------------------------------------------------------ stages of both latency kernels
 // Each stage is called by both wn_lat_kernel and wn_lat2_kernel.  Per thread of the eight compute warps: warp w, lane = 4 g + t4;
 // the thread holds rows g and g + 8 of the 16 utterances and channels 8 w + 2 t4 + {0, 1} of an activation tile (k-step w >> 1,
-// half w & 1 of its A fragments).
+// half w & 1 of its A fragments).  The cluster kernel also runs tiles of TR = 8 utterances: the MMA is still m16n8k16, rows 8-15
+// of every A fragment are the constant 0 and the epilogue of accumulator rows g + 8 is skipped.  Rows 0-7 go through the same
+// HMMAs in the same order, so every value they produce is the one a 16-row tile produces.
 struct StepIt { int t, l, slot; };       // coordinates of a layer step: sample, layer, history-ring slot of that sample
 
-// feedback state of the tile ([TU] current index, [TU] previous index) -> yCur / yPrev
-__device__ __forceinline__ void store_ys(const WnParams& p, int B, const int* ys, int tile, int tid)
+// An activation tile in shared memory (TR rows x 64 channels, fp16) is kept in A-fragment order, TR bytes per lane and k-step:
+// 16 rows = the whole fragment (a0 a1 a2 a3), 8 rows = only the words of rows g (a0 a2).  The thread's slot of channels
+// 8 w + 2 t4 + {0, 1}: k-step w >> 1, half w & 1.
+template <int TR> __device__ __forceinline__ uint32_t xslot(int w, int lane)
 {
-    if (tid < TU && tile * TU + tid < B) { p.yCur[tile * TU + tid] = ys[tid]; p.yPrev[tile * TU + tid] = ys[TU + tid]; }
+    return (uint32_t)((w >> 1) * 32 * TR + lane * TR + (w & 1) * (TR / 2));
 }
-// this thread's four values of x (fp16) -> the x exchange tile and row `row` (= history slot x L + layer) of the history ring
+// A fragment of k-step j of such a tile
+template <int TR> __device__ __forceinline__ void load_a_rows(uint32_t (&a)[4], uint32_t tile, int j, int lane)
+{
+    if (TR == TU) load_a(a, tile + (uint32_t)(j * 512 + lane * 16));
+    else { const uint2 v = lds64(tile + (uint32_t)(j * 256 + lane * 8)); a[0] = v.x; a[1] = 0u; a[2] = v.y; a[3] = 0u; }
+}
+
+// this tile's rows of a 16-byte group of a 16-row layout (words: row g, row g + 8, row g, row g + 8 of two k or channel halves):
+// the whole group for 16 rows; for 8 rows, half `hi` of the 16-row tile, as (row g word, 0, row g word, 0)
+template <int TR> __device__ __forceinline__ uint4 own_rows(uint4 v, bool hi)
+{
+    if (TR == TU) return v;
+    return make_uint4(hi ? v.y : v.x, 0u, hi ? v.w : v.z, 0u);
+}
+
+// feedback state of the tile ([TR] current index, [TR] previous index) of utterances ub .. ub + TR - 1 -> yCur / yPrev
+template <int TR = TU>
+__device__ __forceinline__ void store_ys(const WnParams& p, int B, const int* ys, int ub, int tid)
+{
+    if (tid < TR && ub + tid < B) { p.yCur[ub + tid] = ys[tid]; p.yPrev[ub + tid] = ys[TR + tid]; }
+}
+// this thread's values of x (fp16) -> the x exchange tile and row `row` (= history slot x L + layer) of the history ring.  The
+// ring keeps the 16-row A-fragment order; an 8-row tile writes only its rows' words (`gring` points at them).
+template <int TR = TU>
 __device__ __forceinline__ void store_x(const float (&x)[4], uint32_t xtile, unsigned char* gring, uint32_t row, uint32_t rstride, int w)
 {
-    const uint32_t x01 = pack_h2(x[0], x[1]), x23 = pack_h2(x[2], x[3]);
-    sts64(xtile, x01, x23);
-    stg_v2(gring + (size_t)(row * rstride) + (w >> 1) * 512 + (w & 1) * 8, x01, x23);
+    unsigned char* gp = gring + (size_t)(row * rstride) + (w >> 1) * 512 + (w & 1) * 8;
+    const uint32_t x01 = pack_h2(x[0], x[1]);
+    if (TR == TU) {
+        const uint32_t x23 = pack_h2(x[2], x[3]);
+        sts64(xtile, x01, x23);
+        stg_v2(gp, x01, x23);
+    } else {
+        sts32(xtile, x01);
+        stg_b32(gp, x01);
+    }
 }
 // B fragments of warp w's gate columns for a K = 64 GEMM: tanh and sigmoid n-tiles, k-step pairs 0 and 1
 struct GateW { uint4 t0, g0, t1, g1; };
@@ -324,14 +359,23 @@ __device__ __forceinline__ void gemm_k64(float (&d)[2][4], const uint32_t (&a)[4
     for (int i = 0; i < 4; i++) { d[0][i] += u[0][i]; d[1][i] += u[1][i]; }
 }
 // h = tanh(a[:R]) * sigmoid(a[R:]) in packed fp16 (MUFU; sigmoid(x) = 0.5 tanh(x/2) + 0.5) -> the h tile; returns the two words
+// (8-row tiles: row g only, h23 = 0)
+template <int TR = TU>
 __device__ __forceinline__ void gate(const float (&a)[2][4], uint32_t htile, uint32_t& h01, uint32_t& h23)
 {
     const __half2 half = __floats2half2_rn(0.5f, 0.5f);
-    const __half2 tg0 = wn::tanh_h2(h2(pack_h2(a[0][0], a[0][1]))), tg1 = wn::tanh_h2(h2(pack_h2(a[0][2], a[0][3])));
+    const __half2 tg0 = wn::tanh_h2(h2(pack_h2(a[0][0], a[0][1])));
     const __half2 sg0 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * a[1][0], 0.5f * a[1][1]))), half, half);
-    const __half2 sg1 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * a[1][2], 0.5f * a[1][3]))), half, half);
-    h01 = u32(__hmul2(tg0, sg0)); h23 = u32(__hmul2(tg1, sg1));
-    sts64(htile, h01, h23);
+    h01 = u32(__hmul2(tg0, sg0));
+    if (TR == TU) {
+        const __half2 tg1 = wn::tanh_h2(h2(pack_h2(a[0][2], a[0][3])));
+        const __half2 sg1 = __hfma2(wn::tanh_h2(h2(pack_h2(0.5f * a[1][2], 0.5f * a[1][3]))), half, half);
+        h23 = u32(__hmul2(tg1, sg1));
+        sts64(htile, h01, h23);
+    } else {
+        h23 = 0u;
+        sts32(htile, h01);
+    }
 }
 // Wres.h as two half-K chains (B fragments bw0, bw1 of k-step pairs 0 and 1)
 __device__ __forceinline__ void hmma_res(float (&ra)[4], float (&rb)[4], const uint32_t (&ha)[4][4], uint4 bw0, uint4 bw1)
@@ -339,13 +383,14 @@ __device__ __forceinline__ void hmma_res(float (&ra)[4], float (&rb)[4], const u
     hmma(ra, ha[0], bw0.x, bw0.y); hmma(rb, ha[2], bw1.x, bw1.y);
     hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
 }
-// x' = ((ra + rb) + Bres) + x; below the last layer x' goes to the x tile and history ring row `row`
+// x' = ((ra + rb) + Bres) + x; below the last layer x' goes to the x tile and history ring row `row` (8-row tiles: row g only)
+template <int TR = TU>
 __device__ __forceinline__ void residual(float (&x)[4], const float (&ra)[4], const float (&rb)[4], float2 br, bool store, uint32_t xtile,
                                          unsigned char* gring, uint32_t row, uint32_t rstride, int w)
 {
     x[0] = ((ra[0] + rb[0]) + br.x) + x[0]; x[1] = ((ra[1] + rb[1]) + br.y) + x[1];
-    x[2] = ((ra[2] + rb[2]) + br.x) + x[2]; x[3] = ((ra[3] + rb[3]) + br.y) + x[3];
-    if (store) store_x(x, xtile, gring, row, rstride, w);
+    if (TR == TU) { x[2] = ((ra[2] + rb[2]) + br.x) + x[2]; x[3] = ((ra[3] + rb[3]) + br.y) + x[3]; }
+    if (store) store_x<TR>(x, xtile, gring, row, rstride, w);
 }
 template <bool DUMP>
 __device__ __forceinline__ void dump_xt(const WnParams& p, int B, int l, int b0, int b1, int cw, const float (&x)[4])
@@ -819,7 +864,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
             if (++it0.slot == slots) it0.slot = 0;
             it0.t++;
         }
-        store_ys(p, B, ys, tile, tid);
+        store_ys(p, B, ys, tile * TU, tid);
     }
 #undef TRACE
 }
@@ -841,37 +886,45 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
 // indices (once per sample, tail -> chain); once per sample for the output layers: relu(skip + Bskip) (S x 32 B, tail -> prep),
 // the relu(Zs) halves (4 KB each way, tail <-> prep) and the prep's logits half (8 KB fp32, prep -> tail).  Each CTA moves less than
 // ~100 KB per step through its shared memory; a single CTA doing all of it moves ~190 KB per step and is bound by that.
-template <int S>
+// TR = utterances per cluster, 16 or 8.  An 8-row cluster c serves half c & 1 of 16-row tile c >> 1 of the conditioning store and the
+// history ring (their layouts do not change: it reads and writes only its rows' words), keeps its shared-memory tiles at 8 rows and
+// moves half the bytes of every flow above; the weights, and so the HMMAs and the B-fragment reads, are the same.
+template <int S, int TR>
 struct CfgC {
     using C = Cfg<S>;
+    static_assert(TR == 16 || TR == 8, "a cluster serves 16 or 8 utterances");
     static constexpr uint32_t PIECE0 = 24576;                              // chain: [Wcur | Wres]
     static constexpr uint32_t SLOT1 = S * 128;                             // tail: Wskip_l
     static constexpr int NSLOT1 = 3;
     static constexpr int NAP = 4;                                          // pre-activation tiles in flight from the prep CTA to the chain CTA
     static constexpr int NPS = 8;                                          // staged history / conditioning tiles of the prep CTA
+    static constexpr int RPW = TR / NCW;                                   // rows sampled per tail warp
+    static constexpr uint32_t XT = TR * 128;                               // activation tile (x, h, x[t-d]): TR rows x 64 channels fp16
+    static constexpr uint32_t AP = TR * 512;                               // pre-activation tile: TR rows x 128 channels fp32
     // chain CTA
     static constexpr uint32_t C_RING = 0;                                  // 2 x PIECE0
     static constexpr uint32_t C_EMB = 2 * PIECE0;
     static constexpr uint32_t C_EPBUF = C_EMB + A * EROW * 4;
-    static constexpr uint32_t C_XBUF = C_EPBUF + 2 * TU * EROW * 4;
-    static constexpr uint32_t C_HBUF = C_XBUF + 2048;
-    static constexpr uint32_t C_AP = C_HBUF + 2048;                        // NAP x 8 KB: (Bh + Lh) + Wprev . x[t-d] of the coming steps, written by the prep CTA
-    static constexpr uint32_t C_BIAS = C_AP + NAP * 8192;                  // [L][8 warps][4][8] fp32: Bh / Bres pairs per thread (Bres is read here)
+    static constexpr uint32_t C_XBUF = C_EPBUF + 2 * TR * EROW * 4;
+    static constexpr uint32_t C_HBUF = C_XBUF + XT;
+    static constexpr uint32_t C_AP = C_HBUF + XT;                          // NAP x AP: (Bh + Lh) + Wprev . x[t-d] of the coming steps, written by the prep CTA
+    static constexpr uint32_t C_BIAS = C_AP + NAP * AP;                    // [L][8 warps][4][8] fp32: Bh / Bres pairs per thread (Bres is read here)
     static constexpr uint32_t C_END = C_BIAS + MAXL * 1024;
     // tail CTA
     // Output layers, tail and prep CTAs: OB0 = relu(skip + Bskip) and OB1 = relu(Zs) in A-fragment order (OB1 k-steps 0-7 come from
     // the tail, 8-15 from the prep; each CTA writes into the other's), ZA = this CTA's half of Wza in B-fragment order, resident.
-    static constexpr uint32_t OB0_BYTES = (S / 16) * 512, OB1_BYTES = (A / 16) * 512, ZA_BYTES = 16 * (A / 32) * 512;
+    static constexpr uint32_t OB0_BYTES = (S / 16) * 32 * TR, OB1_BYTES = (A / 16) * 32 * TR, ZA_BYTES = 16 * (A / 32) * 512;
     static constexpr uint32_t T_RING = 0;                                  // NSLOT1 x SLOT1
-    static constexpr uint32_t T_HBUF = NSLOT1 * SLOT1;                     // 2 x 2 KB, written by the chain CTA
-    static constexpr uint32_t T_LBUF = T_HBUF + 2 * 2048;                  // transposed logits; columns 128-255 written by the prep CTA
-    static constexpr uint32_t T_BOUT = T_LBUF + TU * LROW * 4;             // fp32: Bskip total [S], Bzs [A], Bza [A]
+    static constexpr uint32_t T_HBUF = NSLOT1 * SLOT1;                     // 2 x XT, written by the chain CTA
+    static constexpr uint32_t T_LBUF = T_HBUF + 2 * XT;                    // transposed logits; columns 128-255 written by the prep CTA
+    static constexpr uint32_t T_BOUT = T_LBUF + TR * LROW * 4;             // fp32: Bskip total [S], Bzs [A], Bza [A]
     static constexpr uint32_t T_OB0 = T_BOUT + (S + 2 * A) * 4;
     static constexpr uint32_t T_OB1 = T_OB0 + OB0_BYTES;
     static constexpr uint32_t T_ZA = T_OB1 + OB1_BYTES;
     static constexpr uint32_t T_END = T_ZA + ZA_BYTES;
     // prep CTA
     static constexpr uint32_t P_RING = 0;                                  // 4 x 16 KB: Wprev_l
+    // (both staged as whole 16-row tiles at either height: see the prep CTA's staging)
     static constexpr uint32_t P_PST = 4 * 16384;                           // NPS x 2 KB: staged history tiles x[t-d] (A-fragment order)
     static constexpr uint32_t P_COND = P_PST + NPS * 2048;                 // NPS x 4 KB: conditioning tiles, staged with the history tiles (cp.async)
     static constexpr uint32_t P_BIAS = P_COND + NPS * 4096;                // [L][8 warps][4][4] fp32: this thread's Bh
@@ -883,7 +936,7 @@ struct CfgC {
     static constexpr uint32_t P_END = P_ZA + ZA_BYTES;
     // common tail of the maps (same offsets in every CTA, so that remote addresses are computed with mapa on local ones)
     static constexpr uint32_t O_YS = (C_END > T_END ? (C_END > P_END ? C_END : P_END) : (T_END > P_END ? T_END : P_END));
-    static constexpr uint32_t O_BAR = O_YS + 2 * TU * 4;
+    static constexpr uint32_t O_BAR = O_YS + 2 * TR * 4;
     static constexpr uint32_t SMEM = O_BAR + 40 * 8;
     static_assert(SMEM <= 227 * 1024, "the cluster kernel's shared-memory map exceeds the 227 KB an H100 CTA may use");
 };
@@ -896,6 +949,10 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank)
     return r;
 }
 // remote stores that complete bytes on a remote mbarrier (data and signal travel together: no release fence on the sender)
+__device__ __forceinline__ void st_async_b32(uint32_t raddr, uint32_t a, uint32_t rbar)
+{
+    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(raddr), "r"(a), "r"(rbar) : "memory");
+}
 __device__ __forceinline__ void st_async_v2(uint32_t raddr, uint32_t a, uint32_t b, uint32_t rbar)
 {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.b32 [%0], {%1,%2}, [%3];" ::"r"(raddr), "r"(a), "r"(b), "r"(rbar) : "memory");
@@ -916,7 +973,7 @@ __device__ __forceinline__ void cluster_sync_all()
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <int S, bool DUMP, bool TRC>
+template <int S, int TR, bool DUMP, bool TRC>
 __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
 {
     // debug timeline (tools/lat_trace.py): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
@@ -925,7 +982,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     const int tr_t = p.trace_t & 0xFFFF;
 #define TRACE2(role, tag) do { if (TRC && trc && threadIdx.x == 0 && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
     using C = Cfg<S>;
-    using M = CfgC<S>;
+    using M = CfgC<S, TR>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     const uint32_t sm = smem_u32(smem_raw);
     const int L = p.L, B = p.B;
@@ -934,7 +991,10 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     uint32_t crank;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
     const bool is_chain = crank == 0, is_tail = crank == 1;
-    const int tile = blockIdx.x / NCL;
+    // this cluster serves utterances ub .. ub + TR - 1: all of 16-row tile `tile` of the conditioning store and the history ring, or
+    // (TR = 8) its half ub & 8, whose words sit `hw4` bytes into every 16-byte group of the tile's accumulator / A-fragment order
+    const int ub = blockIdx.x / NCL * TR, tile = ub / TU;
+    const uint32_t hw4 = (uint32_t)(ub & 8) >> 1;
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
@@ -960,17 +1020,17 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
         mbar_init(s_ob0full, 1); mbar_init(s_ob0free, NCW); mbar_init(s_ob1full, 1); mbar_init(s_ob1free, 2 * NCW);
         mbar_init(s_lfull, 1); mbar_init(s_lfree, NCW);
         fence_mbar_init();
-        // transaction barriers are armed by their owner one phase ahead: the tail expects 2 KB per h tile, the chain 128 B of indices
-        // and 8 KB per pre-activation tile; once per sample the prep expects relu(skip) and a relu(Zs) half, the tail a relu(Zs) half
-        // and the logits half
-        if (is_chain) { mbar_arrive_expect_tx(s_yfull, 2 * TU * 4); for (int i = 0; i < M::NAP; i++) mbar_arrive_expect_tx(s_apfull + 8 * i, 8192); }
-        else if (is_tail) { mbar_arrive_expect_tx(s_hfull, 2048); mbar_arrive_expect_tx(s_hfull + 8, 2048); mbar_arrive_expect_tx(s_ob1full, TU * 128 * 2); mbar_arrive_expect_tx(s_lfull, TU * 128 * 4); }
-        else { mbar_arrive_expect_tx(s_ob0full, TU * S * 2); mbar_arrive_expect_tx(s_ob1full, TU * 128 * 2); }
+        // transaction barriers are armed by their owner one phase ahead: the tail expects an h tile per step (TR x 128 B), the chain
+        // the sampled indices (2 x TR x 4 B) and a pre-activation tile per step (TR x 512 B); once per sample the prep expects relu(skip)
+        // and a relu(Zs) half, the tail a relu(Zs) half and the logits half
+        if (is_chain) { mbar_arrive_expect_tx(s_yfull, 2 * TR * 4); for (int i = 0; i < M::NAP; i++) mbar_arrive_expect_tx(s_apfull + 8 * i, M::AP); }
+        else if (is_tail) { mbar_arrive_expect_tx(s_hfull, M::XT); mbar_arrive_expect_tx(s_hfull + 8, M::XT); mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2); mbar_arrive_expect_tx(s_lfull, TR * 128 * 4); }
+        else { mbar_arrive_expect_tx(s_ob0full, TR * S * 2); mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2); }
     }
-    if (tid < TU) {
-        const int b = tile * TU + tid;
+    if (tid < TR) {
+        const int b = ub + tid;
         ys[tid] = b < B ? p.yCur[b] : 128;
-        ys[TU + tid] = b < B ? p.yPrev[b] : 128;
+        ys[TR + tid] = b < B ? p.yPrev[b] : 128;
     }
     if (is_chain) {
         const uint32_t* ec = static_cast<const uint32_t*>(p.embCur);
@@ -991,11 +1051,10 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     cluster_sync_all();                                    // every CTA's barriers are initialised before anybody signals a peer
 
     const int w = warp, g = lane >> 2, t4 = lane & 3;
-    const int b0 = tile * TU + g, b1 = b0 + 8;
+    const int b0 = ub + g, b1 = TR == TU ? b0 + 8 : B;       // an 8-row tile has no row g + 8
     const bool v0 = b0 < B, v1 = b1 < B;
     const uint32_t lane16 = (uint32_t)lane * 16;
-    const int jw = w >> 1, hw = w & 1;
-    const uint32_t xchg = (uint32_t)(jw * 512 + hw * 8) + lane16;
+    const uint32_t xchg = xslot<TR>(w, lane);                // this thread's slot of an activation tile
     auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
     auto release_remote = [&](uint32_t local_bar, uint32_t rank) { __syncwarp(); if (lane == 0) mbar_arrive_remote(mapa_u32(local_bar, rank)); };
 
@@ -1045,8 +1104,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
 #pragma unroll
         for (int jp = 0; jp < S / 32; jp++) {
             uint32_t a0[4], a1[4];
-            load_a(a0, ob0 + (2 * jp) * 512 + lane16);
-            load_a(a1, ob0 + (2 * jp + 1) * 512 + lane16);
+            load_a_rows<TR>(a0, ob0, 2 * jp, lane);
+            load_a_rows<TR>(a1, ob0, 2 * jp + 1, lane);
 #pragma unroll
             for (int i = 0; i < 2; i++) hmma(zz[i], a0, zsw[i][jp].x, zsw[i][jp].y);
 #pragma unroll
@@ -1054,7 +1113,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
         }
         if (!half) load_za();
         if (half) {                                    // OB0 has been read: arm its barrier for the next sample, then free it
-            if (tid == 0) mbar_arrive_expect_tx(s_ob0full, TU * S * 2);
+            if (tid == 0) mbar_arrive_expect_tx(s_ob0full, TR * S * 2);
             release_remote(s_ob0free, 1);
         }
         TRACE2(crank, 24);
@@ -1071,11 +1130,17 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             zz[i][0] = zz[i][2] = bz[A + c]; zz[i][1] = zz[i][3] = bz[A + c + 1];
         }
         {   // both CTAs' warps have read the previous sample's OB1
-            const uint32_t o = (8 * half + w) * 512 + lane16;
-            const uint4 v = make_uint4(zp[0], zp[1], zp[2], zp[3]);
+            const uint32_t o = (uint32_t)((8 * half + w) * 32 * TR + lane * TR);      // k-step 8 half + w of OB1
+            const uint32_t ro = mapa_u32(sm + (half ? M::T_OB1 : M::P_OB1) + o, peer), rbar = mapa_u32(s_ob1full, peer);
             mbar_wait(s_ob1free, par ^ 1);
-            sts128(ob1 + o, v);
-            st_async_v4(mapa_u32(sm + (half ? M::T_OB1 : M::P_OB1) + o, peer), v, mapa_u32(s_ob1full, peer));
+            if (TR == TU) {
+                const uint4 v = make_uint4(zp[0], zp[1], zp[2], zp[3]);
+                sts128(ob1 + o, v);
+                st_async_v4(ro, v, rbar);
+            } else {
+                sts64(ob1 + o, zp[0], zp[2]);
+                st_async_v2(ro, zp[0], zp[2], rbar);
+            }
         }
         bar_compute();
         mbar_wait(s_ob1full, par);
@@ -1083,8 +1148,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
 #pragma unroll
         for (int jp = 0; jp < A / 32; jp++) {
             uint32_t a0[4], a1[4];
-            load_a(a0, ob1 + (2 * jp) * 512 + lane16);
-            load_a(a1, ob1 + (2 * jp + 1) * 512 + lane16);
+            load_a_rows<TR>(a0, ob1, 2 * jp, lane);
+            load_a_rows<TR>(a1, ob1, 2 * jp + 1, lane);
             if (jp >= ZPRE) {
 #pragma unroll
                 for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
@@ -1095,7 +1160,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             for (int i = 0; i < 2; i++) hmma(zz[i], a1, zab[i][jp].z, zab[i][jp].w);
         }
         // OB1 has been read: arm its barrier for the peer's next half, then free it for both CTAs
-        if (tid == 0) mbar_arrive_expect_tx(s_ob1full, TU * 128 * 2);
+        if (tid == 0) mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2);
         release(s_ob1free);
         release_remote(s_ob1free, peer);
         if (DUMP) {
@@ -1124,13 +1189,13 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             }
         } else {
             const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u;
-            unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048;
+            unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048 + hw4;
             const int cw = 8 * w + 2 * t4;
             const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16, o_res = 16384u + (uint32_t)(w * 2) * 512 + lane16;
             const uint32_t r_hbuf = mapa_u32(sm + M::T_HBUF + xchg, 1);            // this thread's slot of the tail CTA's h tiles
             const uint32_t r_hfull = mapa_u32(s_hfull, 1);
             const uint32_t s_bias = sm + M::C_BIAS + (uint32_t)(w * 4 + t4) * 32;   // this thread's Bh / Bres pairs of layer 0 (+ 1 KB per layer)
-            const uint32_t s_ap = sm + M::C_AP + (uint32_t)(w * 32 + lane) * 32;    // this thread's 8 floats of a pre-activation tile (+ 8 KB per buffer)
+            const uint32_t s_ap = sm + M::C_AP + (uint32_t)tid * (2 * TR);         // this thread's 2 TR / 4 floats of a pre-activation tile (+ AP per buffer)
             uint32_t xa[4][4];
             float accp[2][4];
             float2 brn = make_float2(0.f, 0.f);
@@ -1142,13 +1207,19 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                 if (t1 < t_end) {
                     const uint2 b2 = lds64(s_bias + l1 * 1024 + 16);
                     if (!ap_ok) mbar_wait(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
-                    const uint4 a0 = lds128(s_ap + (pn & 3) * 8192), a1 = lds128(s_ap + (pn & 3) * 8192 + 16);
+                    const uint4 a0 = lds128(s_ap + (pn & 3) * M::AP);
                     brn = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
-                    accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
-                    accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
+                    if (TR == TU) {
+                        const uint4 a1 = lds128(s_ap + (pn & 3) * M::AP + 16);
+                        accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
+                        accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
+                    } else {                                   // row g only: tanh pair, sigmoid pair
+                        accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[1][0] = __uint_as_float(a0.z); accp[1][1] = __uint_as_float(a0.w);
+                        accp[0][2] = accp[0][3] = accp[1][2] = accp[1][3] = 0.f;
+                    }
                     // the tile has been read: arm its barrier for the tile NAP steps on (one thread, ordered before this warp's "free"
                     // signal), then hand the buffer back to the prep CTA
-                    if (tid == 0) mbar_arrive_expect_tx(s_apfull + 8 * (pn & 3), 8192);
+                    if (tid == 0) mbar_arrive_expect_tx(s_apfull + 8 * (pn & 3), M::AP);
                     release_remote(s_apfree + 8 * (pn & 3), 2);
                 }
                 pn++;
@@ -1156,8 +1227,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             };
             {   // prologue: previous-index rows of the first sample; staging of steps 0, 1, 2; pre-activation of step 0
                 const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
-                sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TU + g] * 32 + 4 * w + t4]);
-                sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
+                sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TR + g] * 32 + 4 * w + t4]);
+                if (TR == TU) sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
             }
             StepIt it0{t_begin, 0, p.ring_slot};
             prep(false);                                       // step 0
@@ -1169,30 +1240,33 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                 TRACE2(0, 1);
                 if (t > t_begin) {                             // the tail CTA has written this sample's indices into ys
                     mbar_wait(s_yfull, (uint32_t)(t - t_begin - 1) & 1);
-                    if (tid == 0 && t + 1 < t_end) mbar_arrive_expect_tx(s_yfull, 2 * TU * 4);          // arm the next hand-back
+                    if (tid == 0 && t + 1 < t_end) mbar_arrive_expect_tx(s_yfull, 2 * TR * 4);          // arm the next hand-back
                 }
                 {   // embedding (reference.cpp:42-57), this warp's 8 channels
-                    const int yc0 = ys[g], yc1 = ys[g + 8];
-                    const uint32_t eo = sm + M::C_EPBUF + epar * (TU * EROW * 4);
-                    const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4)), a1 = unpack_h2(lds32(eo + ((g + 8) * EROW + 4 * w + t4) * 4));
-                    const float2 c0 = unpack_h2(lds32(sm + M::C_EMB + (yc0 * EROW + 4 * w + t4) * 4)), c1 = unpack_h2(lds32(sm + M::C_EMB + (yc1 * EROW + 4 * w + t4) * 4));
-                    xres[0] = a0.x + c0.x; xres[1] = a0.y + c0.y; xres[2] = a1.x + c1.x; xres[3] = a1.y + c1.y;
+                    const int yc0 = ys[g], yc1 = TR == TU ? ys[g + 8] : 0;
+                    const uint32_t eo = sm + M::C_EPBUF + epar * (TR * EROW * 4);
+                    const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
+                    const uint32_t en = sm + M::C_EPBUF + (epar ^ 1) * (TR * EROW * 4);
+                    const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4));
+                    const float2 c0 = unpack_h2(lds32(sm + M::C_EMB + (yc0 * EROW + 4 * w + t4) * 4));
+                    xres[0] = a0.x + c0.x; xres[1] = a0.y + c0.y;
+                    if (TR == TU) {
+                        const float2 a1 = unpack_h2(lds32(eo + ((g + 8) * EROW + 4 * w + t4) * 4));
+                        const float2 c1 = unpack_h2(lds32(sm + M::C_EMB + (yc1 * EROW + 4 * w + t4) * 4));
+                        xres[2] = a1.x + c1.x; xres[3] = a1.y + c1.y;
+                    }
                     if (p.tanhEmbed) {
 #pragma unroll
-                        for (int i = 0; i < 4; i++) xres[i] = wn::tanhf_fast(xres[i]);
+                        for (int i = 0; i < (TR == TU ? 4 : 2); i++) xres[i] = wn::tanhf_fast(xres[i]);
                     }
-                    const uint32_t x01 = pack_h2(xres[0], xres[1]), x23 = pack_h2(xres[2], xres[3]);
-                    sts64(sm + M::C_XBUF + xchg, x01, x23);
-                    stg_v2(gring + lane16 + (size_t)((uint32_t)(it0.slot * L) * rstride) + jw * 512 + hw * 8, x01, x23);
-                    const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
-                    const uint32_t en = sm + M::C_EPBUF + (epar ^ 1) * (TU * EROW * 4);
+                    store_x<TR>(xres, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L), rstride, w);
                     cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
-                    cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
+                    if (TR == TU) cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
                     cp_async_commit();                         // landed long before the next sample starts (waited for at the end of this one)
                 }
                 bar_compute();
 #pragma unroll
-                for (int j = 0; j < 4; j++) load_a(xa[j], sm + M::C_XBUF + j * 512 + lane16);
+                for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
                 TRACE2(0, 2);
 
                 for (int l = 0; l < L; l++, pc++) {
@@ -1212,10 +1286,11 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     const uint4 bw0 = lds128(p1 + o_res), bw1 = lds128(p1 + o_res + 512);
                     {
                         uint32_t h01, h23;
-                        gate(accp, sm + M::C_HBUF + xchg, h01, h23);
+                        gate<TR>(accp, sm + M::C_HBUF + xchg, h01, h23);
                         // the tail CTA's copy: buffer hcnt & 1, free once the tail has read the tile of two steps ago
                         if (!ok_hf) mbar_wait(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
-                        st_async_v2(r_hbuf + (hcnt & 1) * 2048, h01, h23, r_hfull + 8 * (hcnt & 1));
+                        if (TR == TU) st_async_v2(r_hbuf + (hcnt & 1) * M::XT, h01, h23, r_hfull + 8 * (hcnt & 1));
+                        else st_async_b32(r_hbuf + (hcnt & 1) * M::XT, h01, r_hfull + 8 * (hcnt & 1));
                         hcnt++;
                     }
                     TRACE2(0, 12);
@@ -1223,12 +1298,12 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     bar_compute();
                     uint32_t ha[4][4];
 #pragma unroll
-                    for (int j = 0; j < 4; j++) load_a(ha[j], sm + M::C_HBUF + j * 512 + lane16);
+                    for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], sm + M::C_HBUF, j, lane);
                     TRACE2(0, 10);
                     float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
                     hmma_res(ra, rb, ha, bw0, bw1);
                     release(s_empty + 8 * sl);
-                    residual(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
+                    residual<TR>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
                     TRACE2(0, 14);
                     dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
                     {   // look at the coming step's barriers
@@ -1241,7 +1316,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     if (l + 1 < L) {
                         bar_compute();
 #pragma unroll
-                        for (int j = 0; j < 4; j++) load_a(xa[j], sm + M::C_XBUF + j * 512 + lane16);
+                        for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
                     }
                     TRACE2(0, 11);
                 }
@@ -1276,15 +1351,17 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             for (int i = 0; i < C::NSK; i++) sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
             uint32_t pc = 0, hcnt = 0;
             for (int t = t_begin; t < t_end; t++) {
-                const float sel0 = (2 * w + 0 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w] : 0.5f;
-                const float sel1 = (2 * w + 1 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w + 1] : 0.5f;
+                constexpr int RPW = M::RPW;
+                float sel[RPW];                                   // selectors of this warp's rows ub + RPW w + r
+#pragma unroll
+                for (int r = 0; r < RPW; r++) sel[r] = (ub + RPW * w + r) < B ? p.sel[(size_t)t * B + ub + RPW * w + r] : 0.5f;
                 for (int l = 0; l < L; l++, pc++, hcnt++) {
-                    const uint32_t hb = sm + M::T_HBUF + (hcnt & 1) * 2048;
+                    const uint32_t hb = sm + M::T_HBUF + (hcnt & 1) * M::XT;
                     mbar_wait(s_hfull + 8 * (hcnt & 1), (hcnt >> 1) & 1);
                     TRACE2(1, 16);
                     uint32_t ha[4][4];
 #pragma unroll
-                    for (int j = 0; j < 4; j++) load_a(ha[j], hb + j * 512 + lane16);
+                    for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], hb, j, lane);
                     const uint32_t sl = pc % M::NSLOT1, p2 = sm + M::T_RING + sl * M::SLOT1;
                     mbar_wait(s_full + 8 * sl, (pc / M::NSLOT1) & 1);
 #pragma unroll
@@ -1299,7 +1376,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     }
                     // the h tile has been read (the HMMAs above hold its values): arm its barrier for the tile after next (one thread,
                     // ordered before this warp's "free" signal), then hand the buffer back to the chain CTA
-                    if (tid == 0) mbar_arrive_expect_tx(s_hfull + 8 * (hcnt & 1), 2048);
+                    if (tid == 0) mbar_arrive_expect_tx(s_hfull + 8 * (hcnt & 1), M::XT);
                     release_remote(s_hfree + 8 * (hcnt & 1), 0);
                     release(s_empty + 8 * sl);
                     TRACE2(1, 15);
@@ -1316,8 +1393,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     }
                 }
                 // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
-                {   // relu(skip + Bskip): 16 B per pair of skip n-tiles, into this CTA's OB0 and the prep CTA's (free once the prep's
-                    // warps have read the previous sample's)
+                {   // relu(skip + Bskip): TR bytes per pair of skip n-tiles, into this CTA's OB0 and the prep CTA's (free once the
+                    // prep's warps have read the previous sample's)
                     uint4 v[C::NSK / 2];
 #pragma unroll
                     for (int i = 0; i < C::NSK; i++) {
@@ -1329,9 +1406,14 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     const uint32_t r_ob0full = mapa_u32(s_ob0full, 2);
 #pragma unroll
                     for (int j = 0; j < C::NSK / 2; j++) {
-                        const uint32_t o = (w * C::NSK / 2 + j) * 512 + lane16;
-                        sts128(sm + M::T_OB0 + o, v[j]);
-                        st_async_v4(mapa_u32(sm + M::P_OB0 + o, 2), v[j], r_ob0full);
+                        const uint32_t o = (uint32_t)((w * C::NSK / 2 + j) * 32 * TR + lane * TR);
+                        if (TR == TU) {
+                            sts128(sm + M::T_OB0 + o, v[j]);
+                            st_async_v4(mapa_u32(sm + M::P_OB0 + o, 2), v[j], r_ob0full);
+                        } else {                               // rows g: a0 a2
+                            sts64(sm + M::T_OB0 + o, v[j].x, v[j].z);
+                            st_async_v2(mapa_u32(sm + M::P_OB0 + o, 2), v[j].x, v[j].z, r_ob0full);
+                        }
                     }
                 }
                 bar_compute();
@@ -1342,16 +1424,18 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                 for (int i = 0; i < 2; i++) {
                     const int c = 8 * (2 * w + i) + 2 * t4;
                     sts64(sm + M::T_LBUF + (g * LROW + c) * 4, __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]));
-                    sts64(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
+                    if (TR == TU) sts64(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
                 }
                 bar_compute();
                 mbar_wait(s_lfull, (uint32_t)(t - t_begin) & 1);  // columns 128-255 from the prep CTA
                 TRACE2(1, 22);
-                {   // softmax + categorical sample: warp w serves utterances 2w and 2w+1; lane holds 8 consecutive classes of each
-                    float e[2][8], m[2] = {0.f, 0.f};
+                {   // softmax + categorical sample: warp w serves utterances RPW w .. RPW w + RPW - 1 of the tile (two of 16, one of 8);
+                    // lane holds 8 consecutive classes of each
+                    float e[RPW][8], m[RPW];
 #pragma unroll
-                    for (int r = 0; r < 2; r++) {
-                        const uint4 u0 = lds128(sm + M::T_LBUF + ((2 * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + M::T_LBUF + ((2 * w + r) * LROW + 8 * lane + 4) * 4);
+                    for (int r = 0; r < RPW; r++) {
+                        m[r] = 0.f;                               // the reference starts the max at 0 (matrix.cpp:171)
+                        const uint4 u0 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane + 4) * 4);
                         e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
                         e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
 #pragma unroll
@@ -1359,33 +1443,37 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     }
 #pragma unroll
                     for (int o = 16; o >= 1; o >>= 1) {
-                        m[0] = fmaxf(m[0], __shfl_xor_sync(0xffffffffu, m[0], o));
-                        m[1] = fmaxf(m[1], __shfl_xor_sync(0xffffffffu, m[1], o));
+#pragma unroll
+                        for (int r = 0; r < RPW; r++) m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], o));
                     }
                     // the logits have been read: arm lfull for the prep's next half, then hand the buffer back to it
-                    if (tid == 0) mbar_arrive_expect_tx(s_lfull, TU * 128 * 4);
+                    if (tid == 0) mbar_arrive_expect_tx(s_lfull, TR * 128 * 4);
                     release_remote(s_lfree, 2);
-                    float incl[2];
+                    float incl[RPW], tot_lane[RPW];
 #pragma unroll
-                    for (int r = 0; r < 2; r++) {
+                    for (int r = 0; r < RPW; r++) {
                         const float ms = m[r] * 1.4426950408889634f;
                         float run = 0.f;
 #pragma unroll
                         for (int k = 0; k < 8; k++) { run += wn::exp2f_fast(fmaf(e[r][k], 1.4426950408889634f, -ms)); e[r][k] = run; }
-                        incl[r] = run;
+                        incl[r] = tot_lane[r] = run;
                     }
-                    const float tot_lane[2] = {incl[0], incl[1]};
 #pragma unroll
                     for (int o = 1; o < 32; o <<= 1) {
-                        const float a0 = __shfl_up_sync(0xffffffffu, incl[0], o), a1 = __shfl_up_sync(0xffffffffu, incl[1], o);
-                        if (lane >= o) { incl[0] += a0; incl[1] += a1; }
-                    }
-                    int yv[2];                                    // the sampled index of each row
+                        float a[RPW];
 #pragma unroll
-                    for (int r = 0; r < 2; r++) {
+                        for (int r = 0; r < RPW; r++) a[r] = __shfl_up_sync(0xffffffffu, incl[r], o);
+                        if (lane >= o) {
+#pragma unroll
+                            for (int r = 0; r < RPW; r++) incl[r] += a[r];
+                        }
+                    }
+                    int yv[RPW];                                  // the sampled index of each row
+#pragma unroll
+                    for (int r = 0; r < RPW; r++) {
                         const float total = __shfl_sync(0xffffffffu, incl[r], 31);
                         const float excl = incl[r] - tot_lane[r];
-                        const float target = (r == 0 ? sel0 : sel1) * total;
+                        const float target = sel[r] * total;
                         int cntk = 0;
 #pragma unroll
                         for (int k = 0; k < 8; k++) cntk += (target < excl + e[r][k]) ? 0 : 1;
@@ -1393,7 +1481,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                         const int lf = ball ? __ffs(ball) - 1 : 31;
                         const int ck = __shfl_sync(0xffffffffu, cntk, lf);
                         yv[r] = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
-                        const int b = tile * TU + 2 * w + r;
+                        const int b = ub + RPW * w + r;
                         if (DUMP && b < B) {
                             const float inv = 1.f / total;
                             float prevv = 0.f;
@@ -1404,30 +1492,36 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                     // both rows' indices are chosen before lane 0 stores anything: the shuffles of the second row cannot move past the
                     // first row's stores, so selecting and storing row by row would run the two selections one after the other
                     if (lane == 0) {
-                        int fbk[2], yold[2];
+                        int fbk[RPW], yold[RPW];
 #pragma unroll
-                        for (int r = 0; r < 2; r++) {
-                            const int b = tile * TU + 2 * w + r;
+                        for (int r = 0; r < RPW; r++) {
+                            const int b = ub + RPW * w + r;
                             fbk[r] = yv[r];
                             if (b < B) {
                                 p.yOut[(size_t)b * p.N + t] = yv[r];
                                 if (p.forced) fbk[r] = p.forced[(size_t)b * p.N + t];
                             } else fbk[r] = 128;
-                            yold[r] = ys[2 * w + r];
-                            ys[TU + 2 * w + r] = yold[r];
-                            ys[2 * w + r] = fbk[r];
+                            yold[r] = ys[RPW * w + r];
+                            ys[TR + RPW * w + r] = yold[r];
+                            ys[RPW * w + r] = fbk[r];
                         }
                         if (t + 1 < t_end) {                      // the chain CTA's copy: data + completion on its yfull barrier
                             const uint32_t rb = mapa_u32(s_yfull, 0);
-                            st_async_v2(mapa_u32(sm + M::O_YS + (TU + 2 * w) * 4, 0), (uint32_t)yold[0], (uint32_t)yold[1], rb);
-                            st_async_v2(mapa_u32(sm + M::O_YS + (2 * w) * 4, 0), (uint32_t)fbk[0], (uint32_t)fbk[1], rb);
+                            const uint32_t ryold = mapa_u32(sm + M::O_YS + (TR + RPW * w) * 4, 0), rycur = mapa_u32(sm + M::O_YS + (RPW * w) * 4, 0);
+                            if (RPW == 2) {
+                                st_async_v2(ryold, (uint32_t)yold[0], (uint32_t)yold[RPW - 1], rb);
+                                st_async_v2(rycur, (uint32_t)fbk[0], (uint32_t)fbk[RPW - 1], rb);
+                            } else {
+                                st_async_b32(ryold, (uint32_t)yold[0], rb);
+                                st_async_b32(rycur, (uint32_t)fbk[0], rb);
+                            }
                         }
                     }
                 }
                 TRACE2(1, 23);
                 bar_compute();
             }
-            store_ys(p, B, ys, tile, tid);
+            store_ys<TR>(p, B, ys, ub, tid);
         }
     } else {
         // ===================================================================================== prep CTA
@@ -1451,15 +1545,19 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u, cstride = (uint32_t)ntiles_alloc * 4096u;
             const unsigned char* gring = static_cast<const unsigned char*>(p.ring) + (size_t)tile * 2048;
             const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16;
-            const uint32_t r_ap = mapa_u32(sm + M::C_AP + (uint32_t)(w * 32 + lane) * 32, 0);   // this thread's 8 floats of the chain CTA's tiles
+            const uint32_t r_ap = mapa_u32(sm + M::C_AP + (uint32_t)tid * (2 * TR), 0);   // this thread's 2 TR / 4 floats of the chain CTA's tiles
             const uint32_t r_apfull = mapa_u32(s_apfull, 0);
-            const uint32_t s_cond = sm + M::P_COND + (uint32_t)(w * 32 + lane) * 16;  // this thread's 16 B of a conditioning tile (+ 4 KB per slot)
+            const uint32_t s_cond = sm + M::P_COND + (uint32_t)tid * 16;              // this thread's 16 B of a conditioning tile (+ 4 KB per slot)
             const uint32_t s_bias = sm + M::P_BIAS + (uint32_t)(w * 4 + t4) * 16;     // this thread's Bh of layer 0 (+ 512 B per layer)
             // Staging of the step `itp`, three steps before its use, no register and no scoreboard involved:
             //  * its conditioning tile: every thread copies the 16 bytes it will read back itself (cp.async; completion = the thread's
             //    own cp.async group, no barrier);
             //  * its dilated history x_l[t-d] (zero before the start of the utterance, nv_wavenet.cuh:106): warps 0-3, 128 x 16 B,
             //    completion on an mbarrier (every warp reads the whole tile).
+            // Both are copied as whole 16-byte groups of the 16-row store layouts with cp.async.cg, which bypasses L1, at either tile
+            // height; an 8-row tile picks its rows' words when it reads them back (own_rows).  The history ring is rewritten during the
+            // launch by the chain CTA on another SM with plain stores, and L1 is not coherent across SMs: a narrower copy through L1
+            // (cp.async.ca, the only form below 16 bytes) could find the line of the slot's previous occupant, maxDil + 1 samples old.
             // NPS = 8 slots: a slot is staged again five steps after its use, and the weight ring (4 pieces) keeps the warps within four.
             // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
             StepIt itp{p.hist_t, 0, p.ring_slot};
@@ -1499,7 +1597,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                 for (int i = 0; i < 2; i++) {
                     const int c = 8 * (16 + 2 * w + i) + 2 * t4;
                     st_async_v2(mapa_u32(sm + M::T_LBUF + (g * LROW + c) * 4, 1), __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]), r_lfull);
-                    st_async_v2(mapa_u32(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, 1), __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]), r_lfull);
+                    if (TR == TU) st_async_v2(mapa_u32(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, 1), __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]), r_lfull);
                 }
                 TRACE2(2, 33);
             };
@@ -1508,14 +1606,18 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
             for (int n = 0; n < nsteps; n++) {
                 const uint32_t sl = n & 3, pa = sm + M::P_RING + sl * 16384, slot = n & (M::NPS - 1), buf = n & (M::NAP - 1);
                 cp_async_wait_pending<2>();                    // this thread's conditioning of step n has landed (two later groups may be in flight)
-                const uint4 cb = lds128(s_cond + slot * 4096);
+                // (tanh, tanh, sigmoid, sigmoid) of rows (g, g + 8, g, g + 8); 8-row tiles: (tanh, 0, sigmoid, 0) of their row
+                const uint4 cb = own_rows<TR>(lds128(s_cond + slot * 4096), hw4 != 0);
                 const uint4 bq = lds128(s_bias + l1 * 512);
                 mbar_wait(s_full + 8 * sl, (n >> 2) & 1);
                 const GateW bw = lds_gate_w(pa, o_t0, o_g0);
                 mbar_wait(s_pfull + 8 * slot, (n >> 3) & 1);
                 uint32_t pb[4][4];
 #pragma unroll
-                for (int j = 0; j < 4; j++) load_a(pb[j], sm + M::P_PST + slot * 2048 + j * 512 + lane16);
+                for (int j = 0; j < 4; j++) {
+                    const uint4 v = own_rows<TR>(lds128(sm + M::P_PST + slot * 2048 + j * 512 + lane16), hw4 != 0);
+                    pb[j][0] = v.x; pb[j][1] = v.y; pb[j][2] = v.z; pb[j][3] = v.w;
+                }
                 const float4 bh = make_float4(__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w));
                 const float2 c0 = unpack_h2(cb.x), c1 = unpack_h2(cb.y), c2 = unpack_h2(cb.z), c3 = unpack_h2(cb.w);
                 float a[2][4] = {{bh.x + c0.x, bh.y + c0.y, bh.x + c1.x, bh.y + c1.y}, {bh.z + c2.x, bh.w + c2.y, bh.z + c3.x, bh.w + c3.y}};
@@ -1524,8 +1626,12 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
                 release(s_empty + 8 * sl);
                 // the chain CTA's tile buffer n % NAP is free once it has read tile n - NAP
                 mbar_wait(s_apfree + 8 * buf, ((n / M::NAP) & 1) ^ 1);
-                st_async_v4(r_ap + buf * 8192, a[0][0] + u[0][0], a[0][1] + u[0][1], a[0][2] + u[0][2], a[0][3] + u[0][3], r_apfull + 8 * buf);
-                st_async_v4(r_ap + buf * 8192 + 16, a[1][0] + u[1][0], a[1][1] + u[1][1], a[1][2] + u[1][2], a[1][3] + u[1][3], r_apfull + 8 * buf);
+                if (TR == TU) {
+                    st_async_v4(r_ap + buf * M::AP, a[0][0] + u[0][0], a[0][1] + u[0][1], a[0][2] + u[0][2], a[0][3] + u[0][3], r_apfull + 8 * buf);
+                    st_async_v4(r_ap + buf * M::AP + 16, a[1][0] + u[1][0], a[1][1] + u[1][1], a[1][2] + u[1][2], a[1][3] + u[1][3], r_apfull + 8 * buf);
+                } else {                                       // row g: tanh pair, sigmoid pair
+                    st_async_v4(r_ap + buf * M::AP, a[0][0] + u[0][0], a[0][1] + u[0][1], a[1][0] + u[1][0], a[1][1] + u[1][1], r_apfull + 8 * buf);
+                }
                 stage();
                 if (++l1 == L) l1 = 0;
                 // the output half of sample tout: after step (tout + 1, 1) has been shipped, so that the chain CTA starts sample
@@ -1599,13 +1705,13 @@ static cudaError_t lat_go(const WnParams& p, const unsigned char* im8, int tiles
 }
 
 // the cluster variant: grid = NCL x `clusters` CTAs, cluster (NCL, 1, 1); `at` receives the cluster attribute the config points to
-template <int S>
+template <int S, int TR>
 static cudaLaunchConfig_t lat2_config(int clusters, cudaStream_t stream, cudaLaunchAttribute& at)
 {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(NCL * clusters, 1, 1);
     cfg.blockDim = dim3(NT, 1, 1);
-    cfg.dynamicSmemBytes = CfgC<S>::SMEM;
+    cfg.dynamicSmemBytes = CfgC<S, TR>::SMEM;
     cfg.stream = stream;
     at.id = cudaLaunchAttributeClusterDimension;
     at.val.clusterDim.x = NCL; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
@@ -1613,27 +1719,27 @@ static cudaLaunchConfig_t lat2_config(int clusters, cudaStream_t stream, cudaLau
     cfg.numAttrs = 1;
     return cfg;
 }
-template <int S, bool DUMP, bool TRC>
-static cudaError_t lat2_go(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
+template <int S, int TR, bool DUMP, bool TRC>
+static cudaError_t lat2_go(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream)
 {
-    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, TR, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM);
     if (e != cudaSuccess) return e;
     cudaLaunchAttribute at;
-    const cudaLaunchConfig_t cfg = lat2_config<S>(tiles, stream, at);
-    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, DUMP, TRC>, p, im8, ntiles_alloc);
+    const cudaLaunchConfig_t cfg = lat2_config<S, TR>(clusters, stream, at);
+    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, TR, DUMP, TRC>, p, im8, ntiles_alloc);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 // how many clusters the device runs at once (a cluster needs NCL SMs of one GPC: fewer than 132 / NCL fit on an H100); 0 if the query fails
-template <int S>
+template <int S, int TR>
 static int lat2_max_clusters()
 {
     static int cached = -1;
     if (cached >= 0) return cached;
-    if (cudaFuncSetAttribute(wn_lat2_kernel<S, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
+    if (cudaFuncSetAttribute(wn_lat2_kernel<S, TR, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
     cudaLaunchAttribute at;
-    const cudaLaunchConfig_t cfg = lat2_config<S>(48, 0, at);
+    const cudaLaunchConfig_t cfg = lat2_config<S, TR>(48, 0, at);
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+    if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, TR, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
     return cached = n;
 }
 
@@ -1655,18 +1761,23 @@ static cudaError_t lat_launch_S(const WnParams& p, const unsigned char* im8, int
     *smem_out = Cfg<S>::SMEM;
     return lat_launch_split(p, lat_go<S, false, false>, lat_go<S, false, true>, lat_go<S, true, false>, im8, tiles, ntiles_alloc, stream);
 }
-template <int S>
-static cudaError_t lat2_launch_S(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
+template <int S, int TR>
+static cudaError_t lat2_launch_S(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
 {
-    *smem_out = CfgC<S>::SMEM;
-    return lat_launch_split(p, lat2_go<S, false, false>, lat2_go<S, false, true>, lat2_go<S, true, false>, im8, tiles, ntiles_alloc, stream);
+    *smem_out = CfgC<S, TR>::SMEM;
+    return lat_launch_split(p, lat2_go<S, TR, false, false>, lat2_go<S, TR, false, true>, lat2_go<S, TR, true, false>, im8, clusters, ntiles_alloc, stream);
 }
 
-int wn_lat_max_clusters(int S) { return S == 256 ? lat2_max_clusters<256>() : S == 128 ? lat2_max_clusters<128>() : 0; }
+template <int TR>
+static int lat2_fit(int S) { return S == 256 ? lat2_max_clusters<256, TR>() : S == 128 ? lat2_max_clusters<128, TR>() : 0; }
+int wn_lat_max_clusters(int S, int rows) { return rows == 8 ? lat2_fit<8>(S) : rows == TU ? lat2_fit<TU>(S) : 0; }
 
-// c.lat_cluster: serve every 16-utterance tile with a cluster of three CTAs (chain / tail / prep) instead of one.  A run of fewer
-// utterances than the engine holds takes the first p.B of them: the conditioning store and the history ring stay laid out per
-// 16-utterance tile of the engine's batch.
+// c.lat_cluster: serve the utterances with clusters of three CTAs (chain / tail / prep) instead of one CTA per 16-utterance tile.
+// A cluster takes 8 utterances while all of them are resident at once, else 16 (a second wave would halve the rate): an 8-row
+// cluster does half the per-row work of a 16-row one (tile reads, gate, residual, output epilogues, softmax) on the same HMMAs and
+// weight reads, so it is faster per utterance as long as there are SMs for twice the clusters.  A run of fewer utterances than the
+// engine holds takes the first p.B of them: the conditioning store and the history ring stay laid out per 16-utterance tile of the
+// engine's batch, whichever tile height runs.
 static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info)
 {
     const bool cluster = c.lat_cluster;
@@ -1675,14 +1786,18 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
     size_t smem = 0;
     cudaError_t e;
     // the cluster kernel's prep CTA reads history tiles the chain CTA wrote at least L - 9 steps earlier: it wants a few steps of margin
-    const int fit = cluster ? wn_lat_max_clusters(p.S) : 0;
-    if (cluster && p.L >= 12 && grid <= fit) {               // every cluster must be resident at once: a second wave would halve the rate
-        if (p.S == 256) e = lat2_launch_S<256>(p, im8, grid, ntiles_alloc, stream, &smem);
-        else if (p.S == 128) e = lat2_launch_S<128>(p, im8, grid, ntiles_alloc, stream, &smem);
-        else return cudaErrorInvalidValue;
-        if (e != cudaSuccess) return e;
-        if (info) { info->kernel = NVWN_KERNEL_LATENCY; info->grid = NCL * grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = TU; info->cluster = NCL; }
-        return cudaGetLastError();
+    if (cluster && p.L >= 12 && (p.S == 256 || p.S == 128)) {
+        const int c8 = (p.B + 7) / 8;
+        int tr = 0, clusters = 0;
+        if (c8 <= lat2_fit<8>(p.S)) { tr = 8; clusters = c8; }
+        else if (grid <= lat2_fit<TU>(p.S)) { tr = TU; clusters = grid; }
+        if (tr == 8) e = p.S == 256 ? lat2_launch_S<256, 8>(p, im8, clusters, ntiles_alloc, stream, &smem) : lat2_launch_S<128, 8>(p, im8, clusters, ntiles_alloc, stream, &smem);
+        else if (tr == TU) e = p.S == 256 ? lat2_launch_S<256, TU>(p, im8, clusters, ntiles_alloc, stream, &smem) : lat2_launch_S<128, TU>(p, im8, clusters, ntiles_alloc, stream, &smem);
+        if (tr) {
+            if (e != cudaSuccess) return e;
+            if (info) { info->kernel = NVWN_KERNEL_LATENCY; info->grid = NCL * clusters; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = tr; info->cluster = NCL; }
+            return cudaGetLastError();
+        }
     }
     if (p.S == 256) e = lat_launch_S<256>(p, im8, grid, ntiles_alloc, stream, &smem);
     else if (p.S == 128) e = lat_launch_S<128>(p, im8, grid, ntiles_alloc, stream, &smem);

@@ -12,6 +12,9 @@ what a passing GPU run cannot show:
   * history visibility: the prep CTA stages x_l[t-d] from global memory with plain loads -- the chain CTA must have finished the step
     that wrote it; the model reports the smallest distance (in chain steps) it saw, which is what `L >= 12` in wn_launch_lat buys.
 
+Byte counts are those of a cluster of `rows` utterances (16, or 8 when all 8-row clusters are resident): every flow moves
+rows / 16 of its 16-row bytes, with the same arrival counts.
+
 Pure Python, no GPU.  `python tools/lat2_protocol_model.py [runs]` runs random trials; tests/test_lat2_protocol_model.py runs a
 bounded number plus mutations (each re-introduces a defect and the model must see it).  Keep in step with the kernel source.
 """
@@ -74,8 +77,9 @@ class Proc:
 
 
 class Sim:
-    def __init__(self, L=12, T=3, seed=0, slow=None, bug=None, max_dil=4):
-        self.L, self.T = L, T
+    def __init__(self, L=12, T=3, seed=0, slow=None, bug=None, max_dil=4, rows=16):
+        assert rows in (8, 16)
+        self.L, self.T, self.rows = L, T, rows
         self.rng = random.Random(seed)
         self.slow = slow or {}
         self.bug = bug
@@ -109,15 +113,15 @@ class Sim:
         self.pfull = [B(f"prep.pfull{i}", 4) for i in range(NPS)]          # warps 0-3 stage the history tile (128 thread arrivals)
         self.apfree = [B(f"prep.apfree{i}", NCW) for i in range(NAP)]
         # armed by their owners one phase ahead (kernel prologue)
-        self.yfull.expect_tx(128)
+        self.yfull.expect_tx(self.nb(128))
         for b in self.apfull:
-            b.expect_tx(8192)
+            b.expect_tx(self.nb(8192))
         for b in self.hfull:
-            b.expect_tx(2048)
-        self.ob0full.expect_tx(8192)
+            b.expect_tx(self.nb(2048))
+        self.ob0full.expect_tx(self.nb(8192))
         for b in self.ob1full.values():
-            b.expect_tx(4096)
-        self.lfull.expect_tx(8192)
+            b.expect_tx(self.nb(4096))
+        self.lfull.expect_tx(self.nb(8192))
         # buffers: occupant tag + how many warps have read it
         self.slot = {}                                       # name -> [tag, reads]
         self.chain_steps_done = 0                            # steps whose x output (history ring write) is complete, all warps
@@ -125,6 +129,9 @@ class Sim:
         self.emb_done = {}                                   # sample -> warps that wrote the embedding
         self.min_history_margin = None
         self.nsteps = T * L
+
+    def nb(self, bytes16):                                   # bytes of a flow that moves `bytes16` for 16 rows
+        return bytes16 * self.rows // 16
 
     # ------------------------------------------------------------------ engine
     def lat(self, lo, hi, who=None):
@@ -218,7 +225,7 @@ class Sim:
                 self.read(who, f"ap{b}", pn)
                 yield ("delay", self.lat(20, 40, who))
                 if w == 0:
-                    self.apfull[b].expect_tx(8192)           # armed for the tile NAP steps on, before this warp's "free" signal
+                    self.apfull[b].expect_tx(self.nb(8192))  # armed for the tile NAP steps on, before this warp's "free" signal
                 if self.bug != "no_apfree":
                     self.after(self.lat(150, 400), self.apfree[b].arrive)
             pn += 1
@@ -230,7 +237,7 @@ class Sim:
             if t > 0:
                 yield ("wait", self.yfull, t - 1)
                 if w == 0 and t + 1 < T:
-                    self.yfull.expect_tx(128)
+                    self.yfull.expect_tx(self.nb(128))
             yield ("delay", self.lat(150, 300, who))         # embedding, history write of (t, layer 0)
             self.emb_done[t] = self.emb_done.get(t, 0) + 1
             yield from self.cta_bar("chain", who)
@@ -242,9 +249,9 @@ class Sim:
                     yield ("wait", self.hfree[hc & 1], (hc >> 1) - 1)
 
 
-                def land_h(hc=hc):                           # this warp's 256 bytes of the h tile + their complete_tx
+                def land_h(hc=hc):                           # this warp's 256 (8 rows: 128) bytes of the h tile + their complete_tx
                     self.touch(f"h{hc & 1}", hc, NCW)
-                    self.hfull[hc & 1].complete_tx(256)
+                    self.hfull[hc & 1].complete_tx(self.nb(256))
                 self.after(self.lat(200, 700), land_h)
                 hc += 1
                 yield from prep()
@@ -279,17 +286,17 @@ class Sim:
                 self.read(who, f"tring{pc % TSLOTS}", pc)
                 yield ("delay", self.lat(250, 500, who))     # skip GEMM
                 if w == 0:
-                    self.hfull[hc & 1].expect_tx(2048)       # armed for the tile after next, before this warp's "free" signal
+                    self.hfull[hc & 1].expect_tx(self.nb(2048))   # armed for the tile after next, before this warp's "free" signal
                 self.after(self.lat(150, 400), self.hfree[hc & 1].arrive)
                 self.t_empty[pc % TSLOTS].arrive()
                 pc += 1
                 hc += 1
-            # relu(skip + Bskip): this warp's 1 KB into the prep CTA's OB0 (and its own, ordered by the CTA barrier)
+            # relu(skip + Bskip): this warp's 1 KB (8 rows: 512 B) into the prep CTA's OB0 (and its own, ordered by the CTA barrier)
             yield ("wait", self.ob0free, t - 1)
 
             def land_ob0(t=t):
                 self.touch("prep.ob0", t, NCW)
-                self.ob0full.complete_tx(1024)
+                self.ob0full.complete_tx(self.nb(1024))
             self.after(self.lat(200, 700), land_ob0)
             yield from self.cta_bar("tail", who)
             yield from self.out_half("tail", w, t)
@@ -297,12 +304,12 @@ class Sim:
             yield from self.cta_bar("tail", who)
             yield ("wait", self.lfull, t)                    # columns 128-255 from the prep CTA
             self.read(who, "tail.lbuf", t)
-            yield ("delay", self.lat(800, 1500, who))        # softmax + sampling of this warp's two utterances
+            yield ("delay", self.lat(800, 1500, who))        # softmax + sampling of this warp's two utterances (8 rows: one)
             if w == 0:
-                self.lfull.expect_tx(8192)                   # armed for the next sample, before this warp's "free" signal
+                self.lfull.expect_tx(self.nb(8192))                   # armed for the next sample, before this warp's "free" signal
             self.after(self.lat(150, 400), self.lfree.arrive)
             if t + 1 < T:
-                self.after(self.lat(200, 700), lambda: self.yfull.complete_tx(16))
+                self.after(self.lat(200, 700), lambda: self.yfull.complete_tx(self.nb(16)))
             yield from self.cta_bar("tail", who)
 
     def out_half(self, cta, w, t):
@@ -314,14 +321,14 @@ class Sim:
         yield ("delay", self.lat(300, 700, who))             # Zs GEMM, weights resident
         if cta == "prep":
             if w == 0:
-                self.ob0full.expect_tx(8192)
+                self.ob0full.expect_tx(self.nb(8192))
             self.after(self.lat(150, 400), self.ob0free.arrive)
         yield ("wait", self.ob1free[cta], t - 1)
-        self.touch(f"{cta}.ob1", t, NCW)                     # this warp's 16 B per thread, locally ...
+        self.touch(f"{cta}.ob1", t, NCW)                     # this warp's 16 B (8 rows: 8 B) per thread, locally ...
 
         def land_ob1(t=t):                                   # ... and into the peer's OB1
             self.touch(f"{peer}.ob1", t, NCW)
-            self.ob1full[peer].complete_tx(512)
+            self.ob1full[peer].complete_tx(self.nb(512))
         self.after(self.lat(200, 700), land_ob1)
         yield from self.cta_bar(cta, who)
         if self.bug != "no_ob1full_wait":
@@ -329,7 +336,7 @@ class Sim:
         self.read(who, f"{cta}.ob1", t)
         yield ("delay", self.lat(300, 900, who))             # Za GEMM
         if w == 0:
-            self.ob1full[cta].expect_tx(4096)
+            self.ob1full[cta].expect_tx(self.nb(4096))
         self.ob1free[cta].arrive()
         self.after(self.lat(150, 400), self.ob1free[peer].arrive)
 
@@ -337,9 +344,9 @@ class Sim:
         yield from self.out_half("prep", w, t)
         yield ("wait", self.lfree, t - 1)
 
-        def land_l(t=t):                                     # this warp's 1 KB of logits into the tail CTA's buffer
+        def land_l(t=t):                                     # this warp's 1 KB (8 rows: 512 B) of logits into the tail CTA's buffer
             self.touch("tail.lbuf", t, NCW)
-            self.lfull.complete_tx(1024)
+            self.lfull.complete_tx(self.nb(1024))
         self.after(self.lat(200, 700), land_l)
 
     def prep_warp(self, w):
@@ -353,7 +360,7 @@ class Sim:
             slot = pcnt % NPS
             if pcnt < self.nsteps:
                 t, l = divmod(pcnt, L)
-                # conditioning: this warp's own 512 bytes; history: warps 0-3 copy the tile and arrive on pfull
+                # conditioning: this warp's own 512 (8 rows: 256) bytes; history: warps 0-3 copy the tile and arrive on pfull
                 self.write(f"cond{slot}.w{w}", pcnt, 1)
                 if w < 4:
                     d = self.dil[l]
@@ -389,9 +396,9 @@ class Sim:
             if self.bug != "no_apfree_wait":
                 yield ("wait", self.apfree[b], n // NAP - 1)
 
-            def land_ap(n=n, b=b):                           # this warp's 1 KB of the pre-activation tile + their complete_tx
+            def land_ap(n=n, b=b):                           # this warp's 1 KB (8 rows: 512 B) of the pre-activation tile + their complete_tx
                 self.touch(f"ap{b}", n, NCW)
-                self.apfull[b].complete_tx(1024)
+                self.apfull[b].complete_tx(self.nb(1024))
             self.after(self.lat(300, 900), land_ap)
             yield ("delay", self.lat(100, 400, who))         # the remote stores occupy this CTA's load/store pipe
             stage()
@@ -422,9 +429,10 @@ def trial(seed, **kw):
     L = kw.pop("L", rng.choice([12, 13, 16, 20]))
     T = kw.pop("T", rng.choice([2, 3, 4]))
     slow = kw.pop("slow", None)
+    rows = kw.pop("rows", 8 if seed % 2 == 0 else 16)        # (no draw from rng: the latencies of a seed do not depend on it)
     if slow is None and rng.random() < 0.6:
         slow = {rng.choice(["chain.w0", "chain.w5", "tail.w3", "prep.w1", "prep.w6", "chain.producer", "tail.producer", "prep.producer"]): rng.choice([0.3, 3.0, 10.0])}
-    sim = Sim(L=L, T=T, seed=seed, slow=slow, max_dil=kw.pop("max_dil", rng.choice([1, 4, 512])), **kw).build()
+    sim = Sim(L=L, T=T, seed=seed, slow=slow, max_dil=kw.pop("max_dil", rng.choice([1, 4, 512])), rows=rows, **kw).build()
     sim.run()
     return sim
 

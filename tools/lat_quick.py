@@ -15,7 +15,7 @@ L, R, S, A, md = 20, 64, int(os.environ.get("S", 256)), 256, 512
 N = int(os.environ.get("N", 4000))
 Bs = [int(a) for a in sys.argv[1:]] or [64]
 from nv_wavenet_b200 import _lib
-print(json.dumps({"three_cta_clusters_resident_at_once": _lib.lib().nvwn_debug_lat_max_clusters(S)}))
+print(json.dumps({"three_cta_clusters_resident_at_once": {f"{rows}_rows": _lib.lib().nvwn_debug_lat_max_clusters(S, rows) for rows in (8, 16)}}))
 for B in Bs:
     w = refgen.lively_inputs(3, R, S, A, L, min(B, 16), 8)
     rng = np.random.default_rng(0)
