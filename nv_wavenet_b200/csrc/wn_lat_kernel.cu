@@ -25,6 +25,9 @@
 // K = 64 gate GEMM (except the chain CTA's Wcur.x), the gate, the residual GEMM and update with the x-tile / history-ring store, the xtOut dump, the relu(skip + Bskip)
 // packing and the final index store are defined once ("stages of both latency kernels") and called by both, with the trace
 // points between the calls; the mbarrier / bulk-TMA wrappers come from wn_sm90.cuh.
+// Each kernel body is a prologue (barriers, tables) and a dispatch to one function per role: lat_producer / lat_compute, and
+// chain_cta / tail_cta / prep_cta of the cluster, which share load_out_w and out_half.  What the roles share is set once, in a
+// LatCta / ClusterCta; the mbarrier maps (Cfg::B_*, CfgC::B_*) and the slot arithmetic follow from the slot counts.
 //
 // Replaces nv_wavenet_{singleblock,dualblock,persistent}.cuh + matrix_math.cuh + softmax.cuh of the reference for
 // T_data = half while the batch is small enough to be latency-bound.  Numerical contract: oracle/wavenet_oracle.c
@@ -56,21 +59,24 @@ struct Cfg {
     static constexpr int W_CUR = 0, W_PREV = 16384, W_RES = 32768, W_SKIP = 40960;
     static constexpr int P1_BYTES = 32768, P2_BYTES = 8192 + S * 128;
     // output GEMMs: 4 + 4 ring pieces per sample, each all 32 n-tiles x OJP k-step pairs
-    static constexpr int NQ_ZS = 4, NQ_ZA = 4;
+    static constexpr int NQ_ZS = 4, NQ_ZA = 4, NQ = NQ_ZS + NQ_ZA;
+    static_assert(NQ == 8, "the ring bookkeeping assumes 8 output pieces per sample");
     static constexpr int OJP_ZS = S / 128, OJP_ZA = A / 128;         // k-step pairs per piece
     static constexpr int ZS_PIECE = 32 * OJP_ZS * 512, ZA_PIECE = 32 * OJP_ZA * 512;
     static constexpr int OPIECE = ZA_PIECE > ZS_PIECE ? ZA_PIECE : ZS_PIECE;
     static constexpr int NSK = S / 64;                               // skip n-tiles per warp
     // ring: two slots per piece type; output pieces alternate between the two types
     static constexpr int SLOT1 = P1_BYTES, SLOT2 = P2_BYTES > OPIECE ? P2_BYTES : OPIECE;
+    static constexpr int NSLOT = 4;                                  // ring slots of both types: piece n sits in slot (n >> 1) & 1 of type n & 1
+    static constexpr int NPST = 3;                                   // staged history tiles
     // shared memory map
     static constexpr uint32_t O_RING1 = 0;                           // 2 x SLOT1
     static constexpr uint32_t O_RING2 = 2 * SLOT1;                   // 2 x SLOT2
     static constexpr uint32_t O_EMB = O_RING2 + 2 * SLOT2;
     static constexpr uint32_t O_BOUT = O_EMB + A * EROW * 4;         // fp32: Bskip total [S], Bzs [A], Bza [A]
     static constexpr uint32_t O_EPBUF = O_BOUT + (S + 2 * A) * 4;           // two [16 rows][33 words] buffers (sample parity)
-    static constexpr uint32_t O_PST = O_EPBUF + 2 * TU * EROW * 4;          // 3 x 2 KB: staged history tiles x[t-d] (A-fragment order)
-    static constexpr uint32_t O_OB0 = O_PST + 3 * 2048;
+    static constexpr uint32_t O_PST = O_EPBUF + 2 * TU * EROW * 4;          // NPST x 2 KB: staged history tiles x[t-d] (A-fragment order)
+    static constexpr uint32_t O_OB0 = O_PST + NPST * 2048;
     static constexpr uint32_t O_OB1 = O_OB0 + (S / 16) * 512;
     static constexpr uint32_t O_LBUF = O_OB1 + (A / 16) * 512;              // transposed logits; its first 4 KB double as ...
     static constexpr uint32_t O_XBUF = O_LBUF, O_HBUF = O_LBUF + 2048;      // ... the x and h exchange tiles (dead while the logits live)
@@ -78,6 +84,11 @@ struct Cfg {
     static constexpr uint32_t O_YS = O_DIL + MAXL * 4;
     static constexpr uint32_t O_BAR = O_YS + 2 * TU * 4;
     static constexpr uint32_t SMEM = O_BAR + 16 * 8;
+    // mbarriers at O_BAR: ring full[NSLOT] / empty[NSLOT] (slot i of piece type k: k * 2 + i), pfull[NPST] (staged history tiles)
+    static constexpr uint32_t B_FULL = 0, B_EMPTY = B_FULL + NSLOT * 8, B_PFULL = B_EMPTY + NSLOT * 8, B_END = B_PFULL + NPST * 8;
+    static_assert(O_BAR + B_END <= SMEM, "the mbarriers outgrow their reservation");
+    // offset of the barrier of slot i of piece type k inside full[] / empty[]
+    static __device__ __forceinline__ uint32_t ring_bar(uint32_t k, uint32_t i) { return (k * 2 + i) * 8; }
 };
 
 struct LatImage {
@@ -412,6 +423,451 @@ __device__ __forceinline__ void relu_skip(float (&sk)[4], const float* bskip, in
 
 // ------------------------------------------------------------------------------------------------ the kernel
 
+// What both roles of wn_lat_kernel (the TMA producer lane and the compute warps) use; set once, by the kernel's prologue.
+struct LatCta {
+    const WnParams& p;
+    const unsigned char* img;
+    LatImage im;
+    uint32_t sm;                                // shared-memory base
+    int L, B, tid, w, lane, tile, slots, t_begin, t_end;
+    const float* gbias;
+    uint32_t s_full, s_empty, s_pfull;          // mbarriers: Cfg::B_*
+    int* dil;
+    int* ys;                                    // [TU] current index, [TU] previous index
+    float* s_bout;
+    // debug timeline: role 0 = compute thread 0, role 2 = producer; words (tag << 48 | clock)
+    unsigned long long* trc;
+    int tr_t;
+};
+#define TRACE(role, tag) do { if (TRC && trc && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
+
+// TMA producer (one lane): the pieces in consumption order, each refilled as soon as ITS previous occupant has been consumed (two
+// layers of lead for every piece)
+template <int S, bool TRC>
+__device__ __forceinline__ void lat_producer(const LatCta& c, int& trn)
+{
+    using C = Cfg<S>;
+    const unsigned char* img = c.img;
+    const LatImage& im = c.im;
+    const uint32_t sm = c.sm, s_full = c.s_full, s_empty = c.s_empty;
+    const int L = c.L, t_begin = c.t_begin, t_end = c.t_end;
+    unsigned long long* trc = c.trc;
+    const int tr_t = c.tr_t;
+    uint32_t pc = 0;
+    auto put = [&](const unsigned char* src, uint32_t bytes) {
+        const uint32_t idx = (pc >> 1) & 1, bo = C::ring_bar(pc & 1, idx);
+        const uint32_t dst = (pc & 1) ? sm + C::O_RING2 + idx * C::SLOT2 : sm + C::O_RING1 + idx * C::SLOT1;
+        mbar_wait(s_empty + bo, ((pc / C::NSLOT) & 1) ^ 1);
+        mbar_arrive_expect_tx(s_full + bo, bytes);
+        tma_load_1d(dst, src, bytes, s_full + bo);
+        pc++;
+    };
+    for (int t = t_begin; t < t_end; t++) {
+        for (int l = 0; l < L; l++) {
+            const unsigned char* src = img + (size_t)l * im.layer_bytes;
+            put(src, C::P1_BYTES);
+            put(src + C::P1_BYTES, C::P2_BYTES);
+            TRACE(2, 100 + l);
+        }
+        for (int q = 0; q < C::NQ; q++) {
+            put(q < C::NQ_ZS ? img + im.off_zs + (size_t)q * C::ZS_PIECE : img + im.off_za + (size_t)(q - C::NQ_ZS) * C::ZA_PIECE,
+                q < C::NQ_ZS ? C::ZS_PIECE : C::ZA_PIECE);
+            TRACE(2, 200 + q);
+        }
+    }
+}
+
+// the eight compute warps
+template <int S, bool DUMP, bool TRC>
+__device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int ntiles_alloc)
+{
+    using C = Cfg<S>;
+    const WnParams& p = c.p;
+    const unsigned char* img = c.img;
+    const LatImage& im = c.im;
+    const uint32_t sm = c.sm, s_full = c.s_full, s_empty = c.s_empty, s_pfull = c.s_pfull;
+    const int L = c.L, B = c.B, tid = c.tid, lane = c.lane, tile = c.tile, slots = c.slots, t_begin = c.t_begin, t_end = c.t_end;
+    const float* gbias = c.gbias;
+    const int* dil = c.dil;
+    int* ys = c.ys;
+    const float* s_bout = c.s_bout;
+    unsigned long long* trc = c.trc;
+    const int tr_t = c.tr_t;
+    const int w = c.w, g = lane >> 2, t4 = lane & 3;
+    const int b0 = tile * TU + g, b1 = b0 + 8;
+    const bool v0 = b0 < B, v1 = b1 < B;
+    const uint32_t cstride = (uint32_t)ntiles_alloc * 4096u, rstride = (uint32_t)ntiles_alloc * 2048u;
+    const unsigned char* gcond = static_cast<const unsigned char*>(p.Lh) + (size_t)tile * 4096 + (size_t)(w * 32 + lane) * 16;
+    unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048 + (size_t)lane * 16;
+    const float* gbl = gbias + im.b_layer + (size_t)(w * 4 + t4) * 8;
+    const int jw = w >> 1, hw = w & 1;             // this warp's 8 channels = k-step jw, half hw of an activation tile
+    const uint32_t lane16 = (uint32_t)lane * 16;
+    const uint32_t xchg = (uint32_t)(jw * 512 + hw * 8) + lane16;
+    const int cw = 8 * w + 2 * t4;                 // first of the thread's two channels inside the warp's slice
+    // this thread's B-fragment offsets inside the ring pieces
+    const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16;   // + 512 for the second k-step pair
+    const uint32_t o_res = (uint32_t)(w * 2) * 512 + lane16, o_skip = 8192u + (uint32_t)(w * C::NSK * 2) * 512 + lane16;
+    const uint32_t o_out = (uint32_t)(4 * w) * 512;                                                         // output pieces: x OJP, + lane16
+
+    auto advance = [&](StepIt& it) { if (++it.l == L) { it.l = 0; it.t++; if (++it.slot == slots) it.slot = 0; } };
+    auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+    // Every mbarrier wait costs ~90 cycles even when the phase completed long ago (TRYWAIT latency).  The barriers of the coming
+    // step are therefore looked at once, at the end of the running step (measured: 40.1 kHz at C3 B=64 against 38.4 kHz with
+    // plain waits at the point of use, and 35.9 kHz with blocking waits moved behind the preceding HMMA batches).
+    auto probe = [&](uint32_t bar, uint32_t parity) -> bool { return mbar_try_wait(bar, parity); };
+    auto ensure = [&](bool ok, uint32_t bar, uint32_t parity) { if (!ok) mbar_wait(bar, parity); };
+
+    // dilated history x_l[t - d] (zero before the start of the utterance, nv_wavenet.cuh:106) of the step `itp`: staged three
+    // steps ahead into a 3-slot shared-memory ring by warps 0-3 (128 threads x 16 B, cp.async; completion on an mbarrier).
+    // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
+    StepIt itp{p.hist_t, 0, p.ring_slot};
+    const int h_end = p.hist_t + p.count;
+    uint32_t pcnt = 0;                             // tiles staged so far (slot = pcnt % NPST)
+    auto stage_history = [&]() {
+        if (w < 4) {
+            const uint32_t slot3 = pcnt % C::NPST;
+            const int d = dil[itp.l];
+            const uint32_t dst = sm + C::O_PST + slot3 * 2048 + (uint32_t)(w * 32 + lane) * 16;
+            if (itp.t >= h_end || itp.t < d) {
+                sts128(dst, make_uint4(0, 0, 0, 0));
+                mbar_arrive(s_pfull + 8 * slot3);
+            } else {
+                int sl = itp.slot - d; if (sl < 0) sl += slots;
+                cp_async16(dst, gring - lane16 + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
+                cp_async_arrive_noinc(s_pfull + 8 * slot3);
+            }
+        }
+        pcnt++;
+        advance(itp);
+    };
+
+    uint32_t xa[4][4];
+    uint4 cbA = make_uint4(0, 0, 0, 0), cbB = make_uint4(0, 0, 0, 0);
+    float accp[2][4];                              // pre-activation of the coming step: Wprev.x[t-d] + Bh + Lh
+    float2 brn;                                    // Bres pair of the coming step
+    float4 bh_next = make_float4(0.f, 0.f, 0.f, 0.f); float2 br_next = make_float2(0.f, 0.f);            // Bh / Bres pairs of the step after (prefetched a layer ahead)
+    float xres[4] = {0.f, 0.f, 0.f, 0.f};
+    float sk[C::NSK][4];
+#pragma unroll
+    for (int i = 0; i < C::NSK; i++) sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
+    const unsigned char* cptr = gcond + (size_t)t_begin * L * cstride;      // conditioning of step it3 (steps are consecutive in memory)
+
+    // accp <- (Bh + Lh) + Wprev . x[t-d] for the coming step `it1` (its staged history tile is number `pn`, its conditioning
+    // sits in cbA / cbB by parity); Wprev rides in the SAME ring piece as the current layer's Wcur (`p1`; the very first
+    // one comes from global memory).  Then the conditioning of step it3 is fetched.  Independent of the current layer's data.
+    StepIt it1{0, 0, 0}, it3{0, 0, 0};
+    uint32_t pn = 0, kp = 0;                       // kp = parity of the running step
+    auto prep = [&](const uint32_t p1, const bool from_global, const bool pf_ok) {
+        brn = br_next;
+        const uint4 cb = kp ? cbA : cbB;           // step k consumes the buffer of parity (k + 1) & 1 ...
+        {
+            const float2 c0 = unpack_h2(cb.x), c1 = unpack_h2(cb.y), c2 = unpack_h2(cb.z), c3 = unpack_h2(cb.w);
+            accp[0][0] = bh_next.x + c0.x; accp[0][1] = bh_next.y + c0.y; accp[0][2] = bh_next.x + c1.x; accp[0][3] = bh_next.y + c1.y;
+            accp[1][0] = bh_next.z + c2.x; accp[1][1] = bh_next.w + c2.y; accp[1][2] = bh_next.z + c3.x; accp[1][3] = bh_next.w + c3.y;
+        }
+        const uint32_t slot3 = pn % C::NPST;
+        if (it1.t < t_end) {
+            GateW bw;
+            if (from_global) {
+                const unsigned char* gp = img + (size_t)(L - 1) * im.layer_bytes + C::W_PREV;
+                bw = {ldg_nc_v4(gp + o_t0), ldg_nc_v4(gp + o_g0), ldg_nc_v4(gp + o_t0 + 512), ldg_nc_v4(gp + o_g0 + 512)};
+            } else {
+                bw = lds_gate_w(p1 + C::W_PREV, o_t0, o_g0);
+            }
+            ensure(pf_ok, s_pfull + 8 * slot3, (pn / C::NPST) & 1);
+            uint32_t pb[4][4];
+#pragma unroll
+            for (int j = 0; j < 4; j++) load_a(pb[j], sm + C::O_PST + slot3 * 2048 + j * 512 + lane16);
+            gemm_k64(accp, pb, bw);
+        }
+        pn++;
+        {   // ... and refills it with the conditioning of step k + 3
+            const unsigned char* src = cptr;
+            cptr += cstride;
+            const bool live = it3.t < t_end;       // past the end the stale value is never used (the prep of such a step is skipped)
+            ldg_nc_v4_if(cbA, src, live && kp != 0);
+            ldg_nc_v4_if(cbB, src, live && kp == 0);
+        }
+        advance(it1); advance(it3);
+        bh_next = *reinterpret_cast<const float4*>(gbl + it1.l * 256);
+        br_next = *reinterpret_cast<const float2*>(gbl + it1.l * 256 + 4);
+    };
+
+    // ---------------- prologue: previous-index rows of the first sample, prefetch pipeline
+    {
+        const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
+        sts32(sm + C::O_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TU + g] * 32 + 4 * w + t4]);
+        sts32(sm + C::O_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
+    }
+    StepIt it0{t_begin, 0, p.ring_slot};
+    stage_history(); stage_history(); stage_history();              // history tiles of steps 0, 1, 2
+    {
+        it1 = it0; it3 = it0;
+        kp = 1;                                                     // the prologue plays "step -1": consumes cbA (step 0), refills it with step 2
+        cbA = ldg_nc_v4(cptr); cptr += cstride;
+        { StepIt i1 = it0; advance(i1); cbB = i1.t < t_end ? ldg_nc_v4(cptr) : make_uint4(0, 0, 0, 0); cptr += cstride; }
+        advance(it3); advance(it3);
+        bh_next = *reinterpret_cast<const float4*>(gbl); br_next = *reinterpret_cast<const float2*>(gbl + 4);
+        prep(0, true, false);                                       // leaves it1 = step 1, it3 = step 3
+        kp = 0;
+    }
+    bar_compute();
+
+    // ring bookkeeping: a layer step uses slot `sb` of both piece types; the parity of its barriers is `fph`
+    uint32_t sb = 0, fph = 0;
+
+    bool ok_f1 = false, ok_f2 = false, ok_pf = false;          // what the look at the coming step's barriers returned
+    // one layer step
+    auto step = [&](const int t, const int l) {
+        const uint32_t p1 = sm + C::O_RING1 + sb * C::SLOT1, p2 = sm + C::O_RING2 + sb * C::SLOT2;
+        const uint32_t f1 = s_full + C::ring_bar(0, sb), f2 = s_full + C::ring_bar(1, sb), e1 = s_empty + C::ring_bar(0, sb), e2 = s_empty + C::ring_bar(1, sb);
+        const float2 br = brn;
+        // ---- a = Wcur.x + [Wprev.x[t-d] + Bh + Lh]   (nv_wavenet.cuh:131-157); the two halves of K as independent chains
+        ensure(ok_f1, f1, fph);
+        gemm_k64(accp, xa, lds_gate_w(p1, o_t0, o_g0));
+        // ---- h = tanh(a[:R]) * sigmoid(a[R:])
+        {
+            uint32_t h01, h23;
+            gate(accp, sm + C::O_HBUF + xchg, h01, h23);
+        }
+        if (tid == 0) TRACE(0, 12);
+        // ---- while the other warps finish their part of h: the dilated-history half of the next step's pre-activation
+        // (after the last layer: layer 0 of the next sample); then this piece of the ring is free
+        prep(p1, false, ok_pf);
+        release(e1);
+        bar_compute();
+        uint32_t ha[4][4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) load_a(ha[j], sm + C::O_HBUF + j * 512 + lane16);
+        if (tid == 0) TRACE(0, 10);
+        // ---- x' = Wres.h + Bres + x   (nv_wavenet.cuh:185-207); two half-K chains
+        float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
+        ensure(ok_f2, f2, fph);
+        {
+            const uint4 bw0 = lds128(p2 + o_res), bw1 = lds128(p2 + o_res + 512);
+            hmma_res(ra, rb, ha, bw0, bw1);
+        }
+        residual(xres, ra, rb, br, l + 1 < L, sm + C::O_XBUF + xchg, gring, (uint32_t)(it0.slot * L + l + 1), rstride, w);
+        if (tid == 0) TRACE(0, 14);
+        dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
+        // ---- while the other warps finish their part of x': skip += Wskip.h   (biases are added once, after the last layer)
+#pragma unroll
+        for (int jp = 0; jp < 2; jp++) {
+            uint4 bw[C::NSK];
+#pragma unroll
+            for (int i = 0; i < C::NSK; i++) bw[i] = lds128(p2 + o_skip + (i * 2 + jp) * 512);
+#pragma unroll
+            for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp], bw[i].x, bw[i].y);
+#pragma unroll
+            for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp + 1], bw[i].z, bw[i].w);
+        }
+        release(e2);
+        stage_history();                           // the history tile of three steps ahead
+        {   // look at the coming step's barriers now; the answers are consumed a barrier later
+            const uint32_t nsb = sb ^ 1, nph = fph ^ sb;
+            mbar_try_wait3(s_full + C::ring_bar(0, nsb), nph, s_full + C::ring_bar(1, nsb), nph, s_pfull + 8 * (pn % C::NPST), (pn / C::NPST) & 1, ok_f1, ok_f2, ok_pf);
+        }
+        if (tid == 0) TRACE(0, 15);
+        if (DUMP) {
+            const float* pre = gbias + im.b_skpre + (size_t)l * S;
+#pragma unroll
+            for (int i = 0; i < C::NSK; i++) {
+                const int c = 8 * (w * C::NSK + i) + 2 * t4;
+                float o0 = sk[i][0] + pre[c], o1 = sk[i][1] + pre[c + 1], o2 = sk[i][2] + pre[c], o3 = sk[i][3] + pre[c + 1];
+                if (l == L - 1) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); o2 = fmaxf(o2, 0.f); o3 = fmaxf(o3, 0.f); }
+                if (v0) { p.skipOut[((size_t)l * B + b0) * S + c] = o0; p.skipOut[((size_t)l * B + b0) * S + c + 1] = o1; }
+                if (v1) { p.skipOut[((size_t)l * B + b1) * S + c] = o2; p.skipOut[((size_t)l * B + b1) * S + c + 1] = o3; }
+            }
+        }
+        if (l + 1 < L) {
+            bar_compute();
+#pragma unroll
+            for (int j = 0; j < 4; j++) load_a(xa[j], sm + C::O_XBUF + j * 512 + lane16);
+        }
+        if (tid == 0) TRACE(0, 11);
+        fph ^= sb; sb ^= 1; kp ^= 1;               // slot alternates every step, barrier parity every second step
+    };
+
+    uint32_t epar = 0;                             // parity of the sample (epbuf buffer)
+    for (int t = t_begin; t < t_end; t++) {
+        // ---------------- embedding (reference.cpp:42-57): x0 = [tanh](embPrev[yPrev] + embCur[yCur]), this warp's 8 channels
+        if (tid == 0) TRACE(0, 1);
+        const float sel0 = (2 * w + 0 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w] : 0.5f;
+        const float sel1 = (2 * w + 1 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w + 1] : 0.5f;
+        {
+            const int yc0 = ys[g], yc1 = ys[g + 8];
+            const uint32_t eo = sm + C::O_EPBUF + epar * (TU * EROW * 4);
+            const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4)), a1 = unpack_h2(lds32(eo + ((g + 8) * EROW + 4 * w + t4) * 4));
+            const float2 c0 = unpack_h2(lds32(sm + C::O_EMB + (yc0 * EROW + 4 * w + t4) * 4)), c1 = unpack_h2(lds32(sm + C::O_EMB + (yc1 * EROW + 4 * w + t4) * 4));
+            xres[0] = a0.x + c0.x; xres[1] = a0.y + c0.y; xres[2] = a1.x + c1.x; xres[3] = a1.y + c1.y;
+            if (p.tanhEmbed) {
+#pragma unroll
+                for (int i = 0; i < 4; i++) xres[i] = wn::tanhf_fast(xres[i]);
+            }
+            const uint32_t x01 = pack_h2(xres[0], xres[1]), x23 = pack_h2(xres[2], xres[3]);
+            sts64(sm + C::O_XBUF + xchg, x01, x23);
+            stg_v2(gring + (size_t)((uint32_t)(it0.slot * L) * rstride) + jw * 512 + hw * 8, x01, x23);
+            // previous-index rows of the NEXT sample (= this sample's current index): global -> shared, asynchronously
+            const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
+            const uint32_t en = sm + C::O_EPBUF + (epar ^ 1) * (TU * EROW * 4);
+            cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
+            cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
+            cp_async_commit();
+        }
+        bar_compute();
+#pragma unroll
+        for (int j = 0; j < 4; j++) load_a(xa[j], sm + C::O_XBUF + j * 512 + lane16);
+        if (tid == 0) TRACE(0, 2);
+
+        for (int l = 0; l < L; l++) step(t, l);
+        ok_f1 = ok_f2 = false;                     // those looks were at slots the output pieces use first (same parity): stale
+
+        // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
+#pragma unroll
+        for (int i = 0; i < C::NSK; i++) {
+            const int nt = w * C::NSK + i;
+            uint32_t lo, hi;
+            relu_skip(sk[i], s_bout, 8 * nt + 2 * t4, lo, hi);
+            sts64(sm + C::O_OB0 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8, lo, hi);
+        }
+        bar_compute();
+        if (tid == 0) TRACE(0, 20);
+        float zz[4][4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int c = 32 * w + 8 * i + 2 * t4;
+            zz[i][0] = zz[i][2] = s_bout[S + c]; zz[i][1] = zz[i][3] = s_bout[S + c + 1];
+        }
+        // the 8 output pieces continue the ring sequence: piece q sits in slot type q & 1, slot sb ^ (q >> 1 & 1)
+        auto out_gemm = [&](const int q, const int ojp, const uint32_t abuf, const int kp0) {
+            const uint32_t idx = sb ^ ((q >> 1) & 1), bo = C::ring_bar(q & 1, idx);
+            const uint32_t st = ((q & 1) ? sm + C::O_RING2 + idx * C::SLOT2 : sm + C::O_RING1 + idx * C::SLOT1) + o_out * ojp + lane16;
+            mbar_wait(s_full + bo, fph ^ (((sb + (q >> 1)) >> 1) & 1));
+            for (int jp = 0; jp < ojp; jp++) {
+                uint32_t a0[4], a1[4];
+                load_a(a0, abuf + ((kp0 + jp) * 2) * 512 + lane16);
+                load_a(a1, abuf + ((kp0 + jp) * 2 + 1) * 512 + lane16);
+                uint4 bw[4];
+#pragma unroll
+                for (int i = 0; i < 4; i++) bw[i] = lds128(st + (i * ojp + jp) * 512);
+#pragma unroll
+                for (int i = 0; i < 4; i++) hmma(zz[i], a0, bw[i].x, bw[i].y);
+#pragma unroll
+                for (int i = 0; i < 4; i++) hmma(zz[i], a1, bw[i].z, bw[i].w);
+            }
+            release(s_empty + bo);
+        };
+#pragma unroll
+        for (int q = 0; q < C::NQ_ZS; q++) out_gemm(q, C::OJP_ZS, sm + C::O_OB0, q * C::OJP_ZS);
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int nt = 4 * w + i, c = 8 * nt + 2 * t4;
+            const float z0 = fmaxf(zz[i][0], 0.f), z1 = fmaxf(zz[i][1], 0.f), z2 = fmaxf(zz[i][2], 0.f), z3 = fmaxf(zz[i][3], 0.f);
+            sts64(sm + C::O_OB1 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8, pack_h2(z0, z1), pack_h2(z2, z3));
+            if (DUMP) {
+                if (v0) { p.Zs[(size_t)b0 * A + c] = z0; p.Zs[(size_t)b0 * A + c + 1] = z1; }
+                if (v1) { p.Zs[(size_t)b1 * A + c] = z2; p.Zs[(size_t)b1 * A + c + 1] = z3; }
+            }
+            zz[i][0] = zz[i][2] = s_bout[S + A + c]; zz[i][1] = zz[i][3] = s_bout[S + A + c + 1];
+        }
+        bar_compute();
+        if (tid == 0) TRACE(0, 21);
+#pragma unroll
+        for (int q = 0; q < C::NQ_ZA; q++) out_gemm(C::NQ_ZS + q, C::OJP_ZA, sm + C::O_OB1, q * C::OJP_ZA);
+        // 8 pieces = 4 slot pairs later: same slot, same barrier parity as before the output phase
+        // logits (fp32) -> transposed buffer: row = utterance, 256 contiguous classes
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int c = 32 * w + 8 * i + 2 * t4;
+            sts64(sm + C::O_LBUF + (g * LROW + c) * 4, __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]));
+            sts64(sm + C::O_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
+            if (DUMP) {
+                if (v0) { p.Za[(size_t)b0 * A + c] = zz[i][0]; p.Za[(size_t)b0 * A + c + 1] = zz[i][1]; }
+                if (v1) { p.Za[(size_t)b1 * A + c] = zz[i][2]; p.Za[(size_t)b1 * A + c + 1] = zz[i][3]; }
+            }
+        }
+        bar_compute();
+        if (tid == 0) TRACE(0, 22);
+        if (t + 1 < t_end) {                       // every output piece is consumed: the first pieces of the next sample
+            ok_f1 = probe(s_full + C::ring_bar(0, sb), fph);
+            ok_f2 = probe(s_full + C::ring_bar(1, sb), fph);
+        }
+        // ---------------- softmax + categorical sample (matrix.cpp:167-183, reference.cpp:106-121): warp w serves
+        // utterances 2w and 2w+1; lane holds 8 consecutive classes of each
+        {
+            float e[2][8], m[2] = {0.f, 0.f};                          // the reference starts the max at 0 (matrix.cpp:171)
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const uint4 u0 = lds128(sm + C::O_LBUF + ((2 * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + C::O_LBUF + ((2 * w + r) * LROW + 8 * lane + 4) * 4);
+                e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
+                e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
+#pragma unroll
+                for (int k = 0; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
+            }
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) {
+                m[0] = fmaxf(m[0], __shfl_xor_sync(0xffffffffu, m[0], o));
+                m[1] = fmaxf(m[1], __shfl_xor_sync(0xffffffffu, m[1], o));
+            }
+            float incl[2];
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const float ms = m[r] * 1.4426950408889634f;
+                float run = 0.f;
+#pragma unroll
+                for (int k = 0; k < 8; k++) {
+                    const float ev = wn::exp2f_fast(fmaf(e[r][k], 1.4426950408889634f, -ms));
+                    run += ev;
+                    e[r][k] = run;                                     // inclusive running sum inside the lane
+                }
+                incl[r] = run;
+            }
+            const float tot_lane[2] = {incl[0], incl[1]};
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const float a0 = __shfl_up_sync(0xffffffffu, incl[0], o), a1 = __shfl_up_sync(0xffffffffu, incl[1], o);
+                if (lane >= o) { incl[0] += a0; incl[1] += a1; }
+            }
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const float total = __shfl_sync(0xffffffffu, incl[r], 31);
+                const float excl = incl[r] - tot_lane[r];
+                const float target = (r == 0 ? sel0 : sel1) * total;
+                int cntk = 0;
+#pragma unroll
+                for (int k = 0; k < 8; k++) cntk += (target < excl + e[r][k]) ? 0 : 1;
+                const unsigned ball = __ballot_sync(0xffffffffu, target < incl[r]);
+                const int lf = ball ? __ffs(ball) - 1 : 31;
+                const int ck = __shfl_sync(0xffffffffu, cntk, lf);
+                const int y = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
+                const int b = tile * TU + 2 * w + r;
+                if (DUMP && b < B) {
+                    const float inv = 1.f / total;
+                    float prevv = 0.f;
+#pragma unroll
+                    for (int k = 0; k < 8; k++) { p.P[(size_t)b * A + 8 * lane + k] = (e[r][k] - prevv) * inv; prevv = e[r][k]; }
+                }
+                if (lane == 0) {
+                    int fbk = y;
+                    if (b < B) {
+                        p.yOut[(size_t)b * p.N + t] = y;
+                        if (p.forced) fbk = p.forced[(size_t)b * p.N + t];
+                    } else fbk = 128;
+                    ys[TU + 2 * w + r] = ys[2 * w + r];
+                    ys[2 * w + r] = fbk;
+                }
+            }
+        }
+        cp_async_wait_all();                       // the next sample's previous-index rows have landed
+        bar_compute();
+        if (tid == 0) TRACE(0, 23);
+        epar ^= 1;
+        if (++it0.slot == slots) it0.slot = 0;
+        it0.t++;
+    }
+    store_ys(p, B, ys, tile * TU, tid);
+}
+
 // DUMP: write the last-sample activations (the host runs the final sample of a dumping launch with this variant).
 // TRC:  record the clock64 timeline (debug; tools/lat_trace.py).
 template <int S, bool DUMP, bool TRC>
@@ -427,24 +883,17 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
-
-    // mbarriers of the weight ring: piece n lives in slot (n >> 1) & 1 of slot type n & 1; one full / empty pair per slot
-    const uint32_t s_full = sm + C::O_BAR, s_empty = s_full + 32, s_pfull = s_full + 64;       // [4], [4], [3]
+    const uint32_t s_full = sm + C::O_BAR + C::B_FULL, s_empty = sm + C::O_BAR + C::B_EMPTY, s_pfull = sm + C::O_BAR + C::B_PFULL;
     int* dil = reinterpret_cast<int*>(smem_raw + C::O_DIL);
-    int* ys = reinterpret_cast<int*>(smem_raw + C::O_YS);      // [TU] current index, [TU] previous index
+    int* ys = reinterpret_cast<int*>(smem_raw + C::O_YS);
     float* s_bout = reinterpret_cast<float*>(smem_raw + C::O_BOUT);
-    constexpr int NQ = C::NQ_ZS + C::NQ_ZA;
-    static_assert(NQ == 8, "the ring bookkeeping assumes 8 output pieces per sample");
-
-    // debug timeline: role 0 = compute thread 0, role 2 = producer; words (tag << 48 | clock)
     unsigned long long* trc = (TRC && p.trace && blockIdx.x == 0) ? p.trace : nullptr;
     int trn = 0;
     const int tr_t = p.trace_t & 0xFFFF;
-#define TRACE(role, tag) do { if (TRC && trc && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
 
     if (tid == 0) {
-        for (int i = 0; i < 4; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
-        for (int i = 0; i < 3; i++) mbar_init(s_pfull + 8 * i, 128);
+        for (int i = 0; i < C::NSLOT; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
+        for (int i = 0; i < C::NPST; i++) mbar_init(s_pfull + 8 * i, 128);
         fence_mbar_init();
         int d = 1;                                     // dilation of layer l (nv_wavenet.cuh:99-111): 1,2,4..maxDil,1,2,...
         for (int l = 0; l < L; l++) { dil[l] = d; d <<= 1; if (d > p.maxDil) d = 1; }
@@ -463,411 +912,14 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
     }
     __syncthreads();
 
+    const LatCta c{p, img, im, sm, L, B, tid, warp, lane, tile, slots, t_begin, t_end, gbias, s_full, s_empty, s_pfull, dil, ys, s_bout, trc, tr_t};
     if (warp == NCW) {
-        // =============================================================== TMA producer (one lane): the pieces in consumption order,
-        // each refilled as soon as ITS previous occupant has been consumed (two layers of lead for every piece)
-        if (lane == 0) {
-            uint32_t pc = 0;
-            auto put = [&](const unsigned char* src, uint32_t bytes) {
-                const uint32_t idx = (pc >> 1) & 1, bo = ((pc & 1) * 2 + idx) * 8;
-                const uint32_t dst = (pc & 1) ? sm + C::O_RING2 + idx * C::SLOT2 : sm + C::O_RING1 + idx * C::SLOT1;
-                mbar_wait(s_empty + bo, ((pc >> 2) & 1) ^ 1);
-                mbar_arrive_expect_tx(s_full + bo, bytes);
-                tma_load_1d(dst, src, bytes, s_full + bo);
-                pc++;
-            };
-            for (int t = t_begin; t < t_end; t++) {
-                for (int l = 0; l < L; l++) {
-                    const unsigned char* src = img + (size_t)l * im.layer_bytes;
-                    put(src, C::P1_BYTES);
-                    put(src + C::P1_BYTES, C::P2_BYTES);
-                    TRACE(2, 100 + l);
-                }
-                for (int q = 0; q < NQ; q++) {
-                    put(q < C::NQ_ZS ? img + im.off_zs + (size_t)q * C::ZS_PIECE : img + im.off_za + (size_t)(q - C::NQ_ZS) * C::ZA_PIECE,
-                        q < C::NQ_ZS ? C::ZS_PIECE : C::ZA_PIECE);
-                    TRACE(2, 200 + q);
-                }
-            }
-        }
+        if (lane == 0) lat_producer<S, TRC>(c, trn);
     } else {
-        // =============================================================== compute warps
-        const int w = warp, g = lane >> 2, t4 = lane & 3;
-        const int b0 = tile * TU + g, b1 = b0 + 8;
-        const bool v0 = b0 < B, v1 = b1 < B;
-        const uint32_t cstride = (uint32_t)ntiles_alloc * 4096u, rstride = (uint32_t)ntiles_alloc * 2048u;
-        const unsigned char* gcond = static_cast<const unsigned char*>(p.Lh) + (size_t)tile * 4096 + (size_t)(w * 32 + lane) * 16;
-        unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048 + (size_t)lane * 16;
-        const float* gbl = gbias + im.b_layer + (size_t)(w * 4 + t4) * 8;
-        const int jw = w >> 1, hw = w & 1;             // this warp's 8 channels = k-step jw, half hw of an activation tile
-        const uint32_t lane16 = (uint32_t)lane * 16;
-        const uint32_t xchg = (uint32_t)(jw * 512 + hw * 8) + lane16;
-        const int cw = 8 * w + 2 * t4;                 // first of the thread's two channels inside the warp's slice
-        // this thread's B-fragment offsets inside the ring pieces
-        const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16;   // + 512 for the second k-step pair
-        const uint32_t o_res = (uint32_t)(w * 2) * 512 + lane16, o_skip = 8192u + (uint32_t)(w * C::NSK * 2) * 512 + lane16;
-        const uint32_t o_out = (uint32_t)(4 * w) * 512;                                                         // output pieces: x OJP, + lane16
-
-        auto advance = [&](StepIt& it) { if (++it.l == L) { it.l = 0; it.t++; if (++it.slot == slots) it.slot = 0; } };
-        auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
-        // Every mbarrier wait costs ~90 cycles even when the phase completed long ago (TRYWAIT latency).  The barriers of the coming
-        // step are therefore looked at once, at the end of the running step (measured: 40.1 kHz at C3 B=64 against 38.4 kHz with
-        // plain waits at the point of use, and 35.9 kHz with blocking waits moved behind the preceding HMMA batches).
-        auto probe = [&](uint32_t bar, uint32_t parity) -> bool { return mbar_try_wait(bar, parity); };
-        auto ensure = [&](bool ok, uint32_t bar, uint32_t parity) { if (!ok) mbar_wait(bar, parity); };
-
-        // dilated history x_l[t - d] (zero before the start of the utterance, nv_wavenet.cuh:106) of the step `itp`: staged three
-        // steps ahead into a 3-slot shared-memory ring by warps 0-3 (128 threads x 16 B, cp.async; completion on an mbarrier).
-        // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
-        StepIt itp{p.hist_t, 0, p.ring_slot};
-        const int h_end = p.hist_t + p.count;
-        uint32_t pcnt = 0;                             // tiles staged so far (slot = pcnt % 3)
-        auto stage_history = [&]() {
-            if (w < 4) {
-                const uint32_t slot3 = pcnt % 3;
-                const int d = dil[itp.l];
-                const uint32_t dst = sm + C::O_PST + slot3 * 2048 + (uint32_t)(w * 32 + lane) * 16;
-                if (itp.t >= h_end || itp.t < d) {
-                    sts128(dst, make_uint4(0, 0, 0, 0));
-                    mbar_arrive(s_pfull + 8 * slot3);
-                } else {
-                    int sl = itp.slot - d; if (sl < 0) sl += slots;
-                    cp_async16(dst, gring - lane16 + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
-                    cp_async_arrive_noinc(s_pfull + 8 * slot3);
-                }
-            }
-            pcnt++;
-            advance(itp);
-        };
-
-        uint32_t xa[4][4];
-        uint4 cbA = make_uint4(0, 0, 0, 0), cbB = make_uint4(0, 0, 0, 0);
-        float accp[2][4];                              // pre-activation of the coming step: Wprev.x[t-d] + Bh + Lh
-        float2 brn;                                    // Bres pair of the coming step
-        float4 bh_next; float2 br_next;                // Bh / Bres pairs of the step after (prefetched a layer ahead)
-        float xres[4] = {0.f, 0.f, 0.f, 0.f};
-        float sk[C::NSK][4];
-#pragma unroll
-        for (int i = 0; i < C::NSK; i++) sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
-        const unsigned char* cptr = gcond + (size_t)t_begin * L * cstride;      // conditioning of step it3 (steps are consecutive in memory)
-
-        // accp <- (Bh + Lh) + Wprev . x[t-d] for the coming step `it1` (its staged history tile is number `pn`, its conditioning
-        // sits in cbA / cbB by parity); Wprev rides in the SAME ring piece as the current layer's Wcur (`p1`; the very first
-        // one comes from global memory).  Then the conditioning of step it3 is fetched.  Independent of the current layer's data.
-        StepIt it1{0, 0, 0}, it3{0, 0, 0};
-        uint32_t pn = 0, kp = 0;                       // kp = parity of the running step
-        auto prep = [&](const uint32_t p1, const bool from_global, const bool pf_ok) {
-            brn = br_next;
-            const uint4 cb = kp ? cbA : cbB;           // step k consumes the buffer of parity (k + 1) & 1 ...
-            {
-                const float2 c0 = unpack_h2(cb.x), c1 = unpack_h2(cb.y), c2 = unpack_h2(cb.z), c3 = unpack_h2(cb.w);
-                accp[0][0] = bh_next.x + c0.x; accp[0][1] = bh_next.y + c0.y; accp[0][2] = bh_next.x + c1.x; accp[0][3] = bh_next.y + c1.y;
-                accp[1][0] = bh_next.z + c2.x; accp[1][1] = bh_next.w + c2.y; accp[1][2] = bh_next.z + c3.x; accp[1][3] = bh_next.w + c3.y;
-            }
-            const uint32_t slot3 = pn % 3;
-            if (it1.t < t_end) {
-                GateW bw;
-                if (from_global) {
-                    const unsigned char* gp = img + (size_t)(L - 1) * im.layer_bytes + C::W_PREV;
-                    bw = {ldg_nc_v4(gp + o_t0), ldg_nc_v4(gp + o_g0), ldg_nc_v4(gp + o_t0 + 512), ldg_nc_v4(gp + o_g0 + 512)};
-                } else {
-                    bw = lds_gate_w(p1 + C::W_PREV, o_t0, o_g0);
-                }
-                ensure(pf_ok, s_pfull + 8 * slot3, (pn / 3) & 1);
-                uint32_t pb[4][4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) load_a(pb[j], sm + C::O_PST + slot3 * 2048 + j * 512 + lane16);
-                gemm_k64(accp, pb, bw);
-            }
-            pn++;
-            {   // ... and refills it with the conditioning of step k + 3
-                const unsigned char* src = cptr;
-                cptr += cstride;
-                const bool live = it3.t < t_end;       // past the end the stale value is never used (the prep of such a step is skipped)
-                ldg_nc_v4_if(cbA, src, live && kp != 0);
-                ldg_nc_v4_if(cbB, src, live && kp == 0);
-            }
-            advance(it1); advance(it3);
-            bh_next = *reinterpret_cast<const float4*>(gbl + it1.l * 256);
-            br_next = *reinterpret_cast<const float2*>(gbl + it1.l * 256 + 4);
-        };
-
-        // ---------------- prologue: previous-index rows of the first sample, prefetch pipeline
-        {
-            const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
-            sts32(sm + C::O_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TU + g] * 32 + 4 * w + t4]);
-            sts32(sm + C::O_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
-        }
-        StepIt it0{t_begin, 0, p.ring_slot};
-        stage_history(); stage_history(); stage_history();              // history tiles of steps 0, 1, 2
-        {
-            it1 = it0; it3 = it0;
-            kp = 1;                                                     // the prologue plays "step -1": consumes cbA (step 0), refills it with step 2
-            cbA = ldg_nc_v4(cptr); cptr += cstride;
-            { StepIt i1 = it0; advance(i1); cbB = i1.t < t_end ? ldg_nc_v4(cptr) : make_uint4(0, 0, 0, 0); cptr += cstride; }
-            advance(it3); advance(it3);
-            bh_next = *reinterpret_cast<const float4*>(gbl); br_next = *reinterpret_cast<const float2*>(gbl + 4);
-            prep(0, true, false);                                       // leaves it1 = step 1, it3 = step 3
-            kp = 0;
-        }
-        bar_compute();
-
-        // ring bookkeeping: a layer step uses slot `sb` of both piece types; the parity of its barriers is `fph`
-        uint32_t sb = 0, fph = 0;
-
-        bool ok_f1 = false, ok_f2 = false, ok_pf = false;          // what the look at the coming step's barriers returned
-        // one layer step
-        auto step = [&](const int t, const int l) {
-            const uint32_t p1 = sm + C::O_RING1 + sb * C::SLOT1, p2 = sm + C::O_RING2 + sb * C::SLOT2;
-            const uint32_t f1 = s_full + sb * 8, f2 = s_full + 16 + sb * 8, e1 = s_empty + sb * 8, e2 = s_empty + 16 + sb * 8;
-            const float2 br = brn;
-            // ---- a = Wcur.x + [Wprev.x[t-d] + Bh + Lh]   (nv_wavenet.cuh:131-157); the two halves of K as independent chains
-            ensure(ok_f1, f1, fph);
-            gemm_k64(accp, xa, lds_gate_w(p1, o_t0, o_g0));
-            // ---- h = tanh(a[:R]) * sigmoid(a[R:])
-            {
-                uint32_t h01, h23;
-                gate(accp, sm + C::O_HBUF + xchg, h01, h23);
-            }
-            if (tid == 0) TRACE(0, 12);
-            // ---- while the other warps finish their part of h: the dilated-history half of the next step's pre-activation
-            // (after the last layer: layer 0 of the next sample); then this piece of the ring is free
-            prep(p1, false, ok_pf);
-            release(e1);
-            bar_compute();
-            uint32_t ha[4][4];
-#pragma unroll
-            for (int j = 0; j < 4; j++) load_a(ha[j], sm + C::O_HBUF + j * 512 + lane16);
-            if (tid == 0) TRACE(0, 10);
-            // ---- x' = Wres.h + Bres + x   (nv_wavenet.cuh:185-207); two half-K chains
-            float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
-            ensure(ok_f2, f2, fph);
-            {
-                const uint4 bw0 = lds128(p2 + o_res), bw1 = lds128(p2 + o_res + 512);
-                hmma_res(ra, rb, ha, bw0, bw1);
-            }
-            residual(xres, ra, rb, br, l + 1 < L, sm + C::O_XBUF + xchg, gring, (uint32_t)(it0.slot * L + l + 1), rstride, w);
-            if (tid == 0) TRACE(0, 14);
-            dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
-            // ---- while the other warps finish their part of x': skip += Wskip.h   (biases are added once, after the last layer)
-#pragma unroll
-            for (int jp = 0; jp < 2; jp++) {
-                uint4 bw[C::NSK];
-#pragma unroll
-                for (int i = 0; i < C::NSK; i++) bw[i] = lds128(p2 + o_skip + (i * 2 + jp) * 512);
-#pragma unroll
-                for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp], bw[i].x, bw[i].y);
-#pragma unroll
-                for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp + 1], bw[i].z, bw[i].w);
-            }
-            release(e2);
-            stage_history();                           // the history tile of three steps ahead
-            {   // look at the coming step's barriers now; the answers are consumed a barrier later
-                const uint32_t nsb = sb ^ 1, nph = fph ^ sb;
-                mbar_try_wait3(s_full + nsb * 8, nph, s_full + 16 + nsb * 8, nph, s_pfull + 8 * (pn % 3), (pn / 3) & 1, ok_f1, ok_f2, ok_pf);
-            }
-            if (tid == 0) TRACE(0, 15);
-            if (DUMP) {
-                const float* pre = gbias + im.b_skpre + (size_t)l * S;
-#pragma unroll
-                for (int i = 0; i < C::NSK; i++) {
-                    const int c = 8 * (w * C::NSK + i) + 2 * t4;
-                    float o0 = sk[i][0] + pre[c], o1 = sk[i][1] + pre[c + 1], o2 = sk[i][2] + pre[c], o3 = sk[i][3] + pre[c + 1];
-                    if (l == L - 1) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); o2 = fmaxf(o2, 0.f); o3 = fmaxf(o3, 0.f); }
-                    if (v0) { p.skipOut[((size_t)l * B + b0) * S + c] = o0; p.skipOut[((size_t)l * B + b0) * S + c + 1] = o1; }
-                    if (v1) { p.skipOut[((size_t)l * B + b1) * S + c] = o2; p.skipOut[((size_t)l * B + b1) * S + c + 1] = o3; }
-                }
-            }
-            if (l + 1 < L) {
-                bar_compute();
-#pragma unroll
-                for (int j = 0; j < 4; j++) load_a(xa[j], sm + C::O_XBUF + j * 512 + lane16);
-            }
-            if (tid == 0) TRACE(0, 11);
-            fph ^= sb; sb ^= 1; kp ^= 1;               // slot alternates every step, barrier parity every second step
-        };
-
-        uint32_t epar = 0;                             // parity of the sample (epbuf buffer)
-        for (int t = t_begin; t < t_end; t++) {
-            // ---------------- embedding (reference.cpp:42-57): x0 = [tanh](embPrev[yPrev] + embCur[yCur]), this warp's 8 channels
-            if (tid == 0) TRACE(0, 1);
-            const float sel0 = (2 * w + 0 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w] : 0.5f;
-            const float sel1 = (2 * w + 1 + tile * TU) < B ? p.sel[(size_t)t * B + tile * TU + 2 * w + 1] : 0.5f;
-            {
-                const int yc0 = ys[g], yc1 = ys[g + 8];
-                const uint32_t eo = sm + C::O_EPBUF + epar * (TU * EROW * 4);
-                const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4)), a1 = unpack_h2(lds32(eo + ((g + 8) * EROW + 4 * w + t4) * 4));
-                const float2 c0 = unpack_h2(lds32(sm + C::O_EMB + (yc0 * EROW + 4 * w + t4) * 4)), c1 = unpack_h2(lds32(sm + C::O_EMB + (yc1 * EROW + 4 * w + t4) * 4));
-                xres[0] = a0.x + c0.x; xres[1] = a0.y + c0.y; xres[2] = a1.x + c1.x; xres[3] = a1.y + c1.y;
-                if (p.tanhEmbed) {
-#pragma unroll
-                    for (int i = 0; i < 4; i++) xres[i] = wn::tanhf_fast(xres[i]);
-                }
-                const uint32_t x01 = pack_h2(xres[0], xres[1]), x23 = pack_h2(xres[2], xres[3]);
-                sts64(sm + C::O_XBUF + xchg, x01, x23);
-                stg_v2(gring + (size_t)((uint32_t)(it0.slot * L) * rstride) + jw * 512 + hw * 8, x01, x23);
-                // previous-index rows of the NEXT sample (= this sample's current index): global -> shared, asynchronously
-                const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
-                const uint32_t en = sm + C::O_EPBUF + (epar ^ 1) * (TU * EROW * 4);
-                cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
-                cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
-                cp_async_commit();
-            }
-            bar_compute();
-#pragma unroll
-            for (int j = 0; j < 4; j++) load_a(xa[j], sm + C::O_XBUF + j * 512 + lane16);
-            if (tid == 0) TRACE(0, 2);
-
-            for (int l = 0; l < L; l++) step(t, l);
-            ok_f1 = ok_f2 = false;                     // those looks were at slots the output pieces use first (same parity): stale
-
-            // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
-#pragma unroll
-            for (int i = 0; i < C::NSK; i++) {
-                const int nt = w * C::NSK + i;
-                uint32_t lo, hi;
-                relu_skip(sk[i], s_bout, 8 * nt + 2 * t4, lo, hi);
-                sts64(sm + C::O_OB0 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8, lo, hi);
-            }
-            bar_compute();
-            if (tid == 0) TRACE(0, 20);
-            float zz[4][4];
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int c = 32 * w + 8 * i + 2 * t4;
-                zz[i][0] = zz[i][2] = s_bout[S + c]; zz[i][1] = zz[i][3] = s_bout[S + c + 1];
-            }
-            // the 8 output pieces continue the ring sequence: piece q sits in slot type q & 1, slot sb ^ (q >> 1 & 1)
-            auto out_gemm = [&](const int q, const int ojp, const uint32_t abuf, const int kp0) {
-                const uint32_t idx = sb ^ ((q >> 1) & 1), bo = ((q & 1) * 2 + idx) * 8;
-                const uint32_t st = ((q & 1) ? sm + C::O_RING2 + idx * C::SLOT2 : sm + C::O_RING1 + idx * C::SLOT1) + o_out * ojp + lane16;
-                mbar_wait(s_full + bo, fph ^ (((sb + (q >> 1)) >> 1) & 1));
-                for (int jp = 0; jp < ojp; jp++) {
-                    uint32_t a0[4], a1[4];
-                    load_a(a0, abuf + ((kp0 + jp) * 2) * 512 + lane16);
-                    load_a(a1, abuf + ((kp0 + jp) * 2 + 1) * 512 + lane16);
-                    uint4 bw[4];
-#pragma unroll
-                    for (int i = 0; i < 4; i++) bw[i] = lds128(st + (i * ojp + jp) * 512);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) hmma(zz[i], a0, bw[i].x, bw[i].y);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) hmma(zz[i], a1, bw[i].z, bw[i].w);
-                }
-                release(s_empty + bo);
-            };
-#pragma unroll
-            for (int q = 0; q < C::NQ_ZS; q++) out_gemm(q, C::OJP_ZS, sm + C::O_OB0, q * C::OJP_ZS);
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int nt = 4 * w + i, c = 8 * nt + 2 * t4;
-                const float z0 = fmaxf(zz[i][0], 0.f), z1 = fmaxf(zz[i][1], 0.f), z2 = fmaxf(zz[i][2], 0.f), z3 = fmaxf(zz[i][3], 0.f);
-                sts64(sm + C::O_OB1 + (nt >> 1) * 512 + lane16 + (nt & 1) * 8, pack_h2(z0, z1), pack_h2(z2, z3));
-                if (DUMP) {
-                    if (v0) { p.Zs[(size_t)b0 * A + c] = z0; p.Zs[(size_t)b0 * A + c + 1] = z1; }
-                    if (v1) { p.Zs[(size_t)b1 * A + c] = z2; p.Zs[(size_t)b1 * A + c + 1] = z3; }
-                }
-                zz[i][0] = zz[i][2] = s_bout[S + A + c]; zz[i][1] = zz[i][3] = s_bout[S + A + c + 1];
-            }
-            bar_compute();
-            if (tid == 0) TRACE(0, 21);
-#pragma unroll
-            for (int q = 0; q < C::NQ_ZA; q++) out_gemm(C::NQ_ZS + q, C::OJP_ZA, sm + C::O_OB1, q * C::OJP_ZA);
-            // 8 pieces = 4 slot pairs later: same slot, same barrier parity as before the output phase
-            // logits (fp32) -> transposed buffer: row = utterance, 256 contiguous classes
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int c = 32 * w + 8 * i + 2 * t4;
-                sts64(sm + C::O_LBUF + (g * LROW + c) * 4, __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]));
-                sts64(sm + C::O_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
-                if (DUMP) {
-                    if (v0) { p.Za[(size_t)b0 * A + c] = zz[i][0]; p.Za[(size_t)b0 * A + c + 1] = zz[i][1]; }
-                    if (v1) { p.Za[(size_t)b1 * A + c] = zz[i][2]; p.Za[(size_t)b1 * A + c + 1] = zz[i][3]; }
-                }
-            }
-            bar_compute();
-            if (tid == 0) TRACE(0, 22);
-            if (t + 1 < t_end) {                       // every output piece is consumed: the first pieces of the next sample
-                ok_f1 = probe(s_full + sb * 8, fph);
-                ok_f2 = probe(s_full + 16 + sb * 8, fph);
-            }
-            // ---------------- softmax + categorical sample (matrix.cpp:167-183, reference.cpp:106-121): warp w serves
-            // utterances 2w and 2w+1; lane holds 8 consecutive classes of each
-            {
-                float e[2][8], m[2] = {0.f, 0.f};                          // the reference starts the max at 0 (matrix.cpp:171)
-#pragma unroll
-                for (int r = 0; r < 2; r++) {
-                    const uint4 u0 = lds128(sm + C::O_LBUF + ((2 * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + C::O_LBUF + ((2 * w + r) * LROW + 8 * lane + 4) * 4);
-                    e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
-                    e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
-#pragma unroll
-                    for (int k = 0; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
-                }
-#pragma unroll
-                for (int o = 16; o >= 1; o >>= 1) {
-                    m[0] = fmaxf(m[0], __shfl_xor_sync(0xffffffffu, m[0], o));
-                    m[1] = fmaxf(m[1], __shfl_xor_sync(0xffffffffu, m[1], o));
-                }
-                float incl[2];
-#pragma unroll
-                for (int r = 0; r < 2; r++) {
-                    const float ms = m[r] * 1.4426950408889634f;
-                    float run = 0.f;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) {
-                        const float ev = wn::exp2f_fast(fmaf(e[r][k], 1.4426950408889634f, -ms));
-                        run += ev;
-                        e[r][k] = run;                                     // inclusive running sum inside the lane
-                    }
-                    incl[r] = run;
-                }
-                const float tot_lane[2] = {incl[0], incl[1]};
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const float a0 = __shfl_up_sync(0xffffffffu, incl[0], o), a1 = __shfl_up_sync(0xffffffffu, incl[1], o);
-                    if (lane >= o) { incl[0] += a0; incl[1] += a1; }
-                }
-#pragma unroll
-                for (int r = 0; r < 2; r++) {
-                    const float total = __shfl_sync(0xffffffffu, incl[r], 31);
-                    const float excl = incl[r] - tot_lane[r];
-                    const float target = (r == 0 ? sel0 : sel1) * total;
-                    int cntk = 0;
-#pragma unroll
-                    for (int k = 0; k < 8; k++) cntk += (target < excl + e[r][k]) ? 0 : 1;
-                    const unsigned ball = __ballot_sync(0xffffffffu, target < incl[r]);
-                    const int lf = ball ? __ffs(ball) - 1 : 31;
-                    const int ck = __shfl_sync(0xffffffffu, cntk, lf);
-                    const int y = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
-                    const int b = tile * TU + 2 * w + r;
-                    if (DUMP && b < B) {
-                        const float inv = 1.f / total;
-                        float prevv = 0.f;
-#pragma unroll
-                        for (int k = 0; k < 8; k++) { p.P[(size_t)b * A + 8 * lane + k] = (e[r][k] - prevv) * inv; prevv = e[r][k]; }
-                    }
-                    if (lane == 0) {
-                        int fbk = y;
-                        if (b < B) {
-                            p.yOut[(size_t)b * p.N + t] = y;
-                            if (p.forced) fbk = p.forced[(size_t)b * p.N + t];
-                        } else fbk = 128;
-                        ys[TU + 2 * w + r] = ys[2 * w + r];
-                        ys[2 * w + r] = fbk;
-                    }
-                }
-            }
-            cp_async_wait_all();                       // the next sample's previous-index rows have landed
-            bar_compute();
-            if (tid == 0) TRACE(0, 23);
-            epar ^= 1;
-            if (++it0.slot == slots) it0.slot = 0;
-            it0.t++;
-        }
-        store_ys(p, B, ys, tile * TU, tid);
+        lat_compute<S, DUMP, TRC>(c, trn, ntiles_alloc);
     }
-#undef TRACE
 }
+#undef TRACE
 
 // ================================================================================================ three-CTA cluster variant
 // The single-CTA kernel above runs at ~83 % of its SM's shared-memory bandwidth (per layer step: 72 KB written by TMA, 72 KB of
@@ -898,6 +950,11 @@ struct CfgC {
     static constexpr int NSLOT1 = 3;
     static constexpr int NAP = 4;                                          // pre-activation tiles in flight from the prep CTA to the chain CTA
     static constexpr int NPS = 8;                                          // staged history / conditioning tiles of the prep CTA
+    static constexpr int NPRING = 4;                                       // Wprev ring slots of the prep CTA
+    static constexpr int NHB = 2;                                          // h tiles in flight from the chain CTA to the tail CTA
+    static constexpr int NRING = NSLOT1 > NPRING ? NSLOT1 : NPRING;        // weight-ring barrier pairs (the chain uses two)
+    static_assert((NAP & (NAP - 1)) == 0 && (NPS & (NPS - 1)) == 0 && (NPRING & (NPRING - 1)) == 0 && (NHB & (NHB - 1)) == 0,
+                  "slot counts are powers of two, so that slot and parity arithmetic stays a mask and a shift");
     static constexpr int RPW = TR / NCW;                                   // rows sampled per tail warp
     static constexpr uint32_t XT = TR * 128;                               // activation tile (x, h, x[t-d]): TR rows x 64 channels fp16
     static constexpr uint32_t AP = TR * 512;                               // pre-activation tile: TR rows x 128 channels fp32
@@ -915,17 +972,17 @@ struct CfgC {
     // the tail, 8-15 from the prep; each CTA writes into the other's), ZA = this CTA's half of Wza in B-fragment order, resident.
     static constexpr uint32_t OB0_BYTES = (S / 16) * 32 * TR, OB1_BYTES = (A / 16) * 32 * TR, ZA_BYTES = 16 * (A / 32) * 512;
     static constexpr uint32_t T_RING = 0;                                  // NSLOT1 x SLOT1
-    static constexpr uint32_t T_HBUF = NSLOT1 * SLOT1;                     // 2 x XT, written by the chain CTA
-    static constexpr uint32_t T_LBUF = T_HBUF + 2 * XT;                    // transposed logits; columns 128-255 written by the prep CTA
+    static constexpr uint32_t T_HBUF = NSLOT1 * SLOT1;                     // NHB x XT, written by the chain CTA
+    static constexpr uint32_t T_LBUF = T_HBUF + NHB * XT;                    // transposed logits; columns 128-255 written by the prep CTA
     static constexpr uint32_t T_BOUT = T_LBUF + TR * LROW * 4;             // fp32: Bskip total [S], Bzs [A], Bza [A]
     static constexpr uint32_t T_OB0 = T_BOUT + (S + 2 * A) * 4;
     static constexpr uint32_t T_OB1 = T_OB0 + OB0_BYTES;
     static constexpr uint32_t T_ZA = T_OB1 + OB1_BYTES;
     static constexpr uint32_t T_END = T_ZA + ZA_BYTES;
     // prep CTA
-    static constexpr uint32_t P_RING = 0;                                  // 4 x 16 KB: Wprev_l
+    static constexpr uint32_t P_RING = 0;                                  // NPRING x 16 KB: Wprev_l
     // (both staged as whole 16-row tiles at either height: see the prep CTA's staging)
-    static constexpr uint32_t P_PST = 4 * 16384;                           // NPS x 2 KB: staged history tiles x[t-d] (A-fragment order)
+    static constexpr uint32_t P_PST = NPRING * 16384;                      // NPS x 2 KB: staged history tiles x[t-d] (A-fragment order)
     static constexpr uint32_t P_COND = P_PST + NPS * 2048;                 // NPS x 4 KB: conditioning tiles, staged with the history tiles (cp.async)
     static constexpr uint32_t P_BIAS = P_COND + NPS * 4096;                // [L][8 warps][4][4] fp32: this thread's Bh
     static constexpr uint32_t P_DIL = P_BIAS + MAXL * 512;
@@ -939,6 +996,13 @@ struct CfgC {
     static constexpr uint32_t O_BAR = O_YS + 2 * TR * 4;
     static constexpr uint32_t SMEM = O_BAR + 40 * 8;
     static_assert(SMEM <= 227 * 1024, "the cluster kernel's shared-memory map exceeds the 227 KB an H100 CTA may use");
+    // mbarriers at O_BAR (what each one guards: wn_lat2_kernel)
+    static constexpr uint32_t B_FULL = 0, B_EMPTY = B_FULL + NRING * 8, B_PFULL = B_EMPTY + NRING * 8;
+    static constexpr uint32_t B_HFULL = B_PFULL + NPS * 8, B_HFREE = B_HFULL + NHB * 8, B_YFULL = B_HFREE + NHB * 8;
+    static constexpr uint32_t B_APFULL = B_YFULL + 8, B_APFREE = B_APFULL + NAP * 8;
+    static constexpr uint32_t B_OB0FULL = B_APFREE + NAP * 8, B_OB0FREE = B_OB0FULL + 8, B_OB1FULL = B_OB0FREE + 8, B_OB1FREE = B_OB1FULL + 8;
+    static constexpr uint32_t B_LFULL = B_OB1FREE + 8, B_LFREE = B_LFULL + 8, B_END = B_LFREE + 8;
+    static_assert(O_BAR + B_END <= SMEM, "the mbarriers outgrow their reservation");
 };
 constexpr int NCL = 3;                       // CTAs per cluster
 
@@ -973,14 +1037,703 @@ __device__ __forceinline__ void cluster_sync_all()
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// the warp is done with a buffer: one arrival (lane 0, after the warp's reads) on its barrier here / in cluster CTA `rank`
+__device__ __forceinline__ void release(uint32_t bar, int lane) { __syncwarp(); if (lane == 0) mbar_arrive(bar); }
+__device__ __forceinline__ void release_remote(uint32_t local_bar, uint32_t rank, int lane)
+{
+    __syncwarp();
+    if (lane == 0) mbar_arrive_remote(mapa_u32(local_bar, rank));
+}
+
+// What more than one role of wn_lat2_kernel uses; set once, by the kernel's prologue.
+struct ClusterCta {
+    const WnParams& p;
+    const unsigned char* img;
+    LatImage im;
+    unsigned char* smem;                        // shared memory, and its shared-window address
+    uint32_t sm;
+    int L, B, tid;
+    uint32_t crank;                             // cluster rank: 0 chain, 1 tail, 2 prep
+    int ub, tile;                               // utterances ub .. ub + TR - 1, in 16-row tile `tile` (hw4: see the kernel)
+    uint32_t hw4;
+    int slots, t_begin, t_end, ntiles_alloc;
+    const float* gbias;
+    uint32_t s_full, s_empty, s_pfull, s_hfull, s_hfree, s_yfull, s_apfull, s_apfree;      // mbarriers: CfgC::B_*
+    uint32_t s_ob0full, s_ob0free, s_ob1full, s_ob1free, s_lfull, s_lfree;
+    int* ys;                                    // [TR] current index, [TR] previous index
+    // this thread: warp w, lane = 4 g + t4, rows b0 and b1 (v0, v1: inside the batch), lane16 = 16 lane, its slot of an activation tile
+    int w, lane, g, t4, b0, b1;
+    bool v0, v1;
+    uint32_t lane16, xchg;
+    unsigned long long* trc;                    // debug timeline: see the kernel
+    int tr_t;
+};
+#define TRACE2(role, tag) do { if (TRC && trc && threadIdx.x == 0 && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
+
+// ---------------- output layers, tail (half 0) and prep (half 1) CTAs: n-tiles 16 half + 2w and 16 half + 2w + 1 of Zs and Za.
+// Their B fragments (lat_pack_kernel: piece q of a matrix = k-step pairs [q OJP, (q+1) OJP) of all 32 n-tiles, fragment
+// (n-tile OJP + jp) x 512 + lane x 16) are loaded once, at kernel start: Wzs into registers (S / 4 per thread), Wza into this
+// CTA's ZA region, where every thread reads back only the 16 B it stored itself (fragment (2w + i) x A/32 + jp).  Wza resident
+// in registers as well would not fit: nine warps leave 168 registers per thread (three warps share a sub-partition's 64 KB),
+// and the tail's skip loop and the prep's step loop would spill ~300 B at S = 256.
+template <int S, int TR>
+__device__ __forceinline__ void load_out_w(const ClusterCta& c, uint4 (&zsw)[2][S / 32], const uint32_t half)
+{
+    using C = Cfg<S>;
+    using M = CfgC<S, TR>;
+    const unsigned char* img = c.img;
+    const LatImage& im = c.im;
+    const uint32_t sm = c.sm, lane16 = c.lane16;
+    const int w = c.w;
+    const uint32_t za = sm + (half ? M::P_ZA : M::T_ZA) + lane16;
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int nt = 16 * half + 2 * w + i;
+#pragma unroll
+        for (int jp = 0; jp < S / 32; jp++)
+            zsw[i][jp] = ldg_nc_v4(img + im.off_zs + (size_t)(jp / C::OJP_ZS) * C::ZS_PIECE + (size_t)(nt * C::OJP_ZS + jp % C::OJP_ZS) * 512 + lane16);
+        for (int jp = 0; jp < A / 32; jp++)
+            sts128(za + ((2 * w + i) * (A / 32) + jp) * 512,
+                   ldg_nc_v4(img + im.off_za + (size_t)(jp / C::OJP_ZA) * C::ZA_PIECE + (size_t)(nt * C::OJP_ZA + jp % C::OJP_ZA) * 512 + lane16));
+    }
+}
+// relu(skip + Bskip) is in this CTA's OB0 (the prep waits for it here).  Per n-tile the HMMAs run from the bias through the
+// k-steps in order on one accumulator, as in the single-CTA kernel.  relu(Zs) of the two n-tiles is k-step 8 half + w of the
+// Za GEMM's A operand: 16 B per thread into this CTA's OB1 and the peer's.  Leaves the logits of the two n-tiles in zz.
+template <int S, int TR, bool DUMP, bool TRC>
+__device__ __forceinline__ void out_half(const ClusterCta& c, int& trn, const int t, const uint4 (&zsw)[2][S / 32], const uint32_t half, float (&zz)[2][4])
+{
+    using M = CfgC<S, TR>;
+    const WnParams& p = c.p;
+    unsigned char* smem_raw = c.smem;
+    const uint32_t sm = c.sm, crank = c.crank, lane16 = c.lane16;
+    const uint32_t s_ob0full = c.s_ob0full, s_ob0free = c.s_ob0free, s_ob1full = c.s_ob1full, s_ob1free = c.s_ob1free;
+    const int tid = c.tid, t_begin = c.t_begin, w = c.w, lane = c.lane, t4 = c.t4, b0 = c.b0, b1 = c.b1;
+    const bool v0 = c.v0, v1 = c.v1;
+    unsigned long long* trc = c.trc;
+    const int tr_t = c.tr_t;
+    const uint32_t peer = half ? 1 : 2, par = (uint32_t)(t - t_begin) & 1;
+    const float* bz = reinterpret_cast<const float*>(smem_raw + (half ? M::P_BOUT : M::T_BOUT + S * 4));   // Bzs [A], Bza [A]
+    const uint32_t ob0 = sm + (half ? M::P_OB0 : M::T_OB0), ob1 = sm + (half ? M::P_OB1 : M::T_OB1), za = sm + (half ? M::P_ZA : M::T_ZA);
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
+        zz[i][0] = zz[i][2] = bz[c]; zz[i][1] = zz[i][3] = bz[c + 1];
+    }
+    // the Wza fragments of the first half of K (32 registers) are read while the CTA would wait anyway: the prep before relu(skip)
+    // arrives, the tail after its Zs HMMAs, while the prep's relu(Zs) half is still on its way; those of the second half inside
+    // the Za GEMM (three quarters or more up front spill at S = 256)
+    constexpr int ZPRE = A / 64;
+    uint4 zab[2][A / 32];
+    auto load_za = [&]() {
+#pragma unroll
+        for (int jp = 0; jp < ZPRE; jp++)
+#pragma unroll
+            for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
+    };
+    if (half) { load_za(); mbar_wait(s_ob0full, par); }
+#pragma unroll
+    for (int jp = 0; jp < S / 32; jp++) {
+        uint32_t a0[4], a1[4];
+        load_a_rows<TR>(a0, ob0, 2 * jp, lane);
+        load_a_rows<TR>(a1, ob0, 2 * jp + 1, lane);
+#pragma unroll
+        for (int i = 0; i < 2; i++) hmma(zz[i], a0, zsw[i][jp].x, zsw[i][jp].y);
+#pragma unroll
+        for (int i = 0; i < 2; i++) hmma(zz[i], a1, zsw[i][jp].z, zsw[i][jp].w);
+    }
+    if (!half) load_za();
+    if (half) {                                    // OB0 has been read: arm its barrier for the next sample, then free it
+        if (tid == 0) mbar_arrive_expect_tx(s_ob0full, TR * S * 2);
+        release_remote(s_ob0free, 1, lane);
+    }
+    TRACE2(crank, 24);
+    uint32_t zp[4];
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+        const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
+        const float z0 = fmaxf(zz[i][0], 0.f), z1 = fmaxf(zz[i][1], 0.f), z2 = fmaxf(zz[i][2], 0.f), z3 = fmaxf(zz[i][3], 0.f);
+        zp[2 * i] = pack_h2(z0, z1); zp[2 * i + 1] = pack_h2(z2, z3);
+        if (DUMP) {
+            if (v0) { p.Zs[(size_t)b0 * A + c] = z0; p.Zs[(size_t)b0 * A + c + 1] = z1; }
+            if (v1) { p.Zs[(size_t)b1 * A + c] = z2; p.Zs[(size_t)b1 * A + c + 1] = z3; }
+        }
+        zz[i][0] = zz[i][2] = bz[A + c]; zz[i][1] = zz[i][3] = bz[A + c + 1];
+    }
+    {   // both CTAs' warps have read the previous sample's OB1
+        const uint32_t o = (uint32_t)((8 * half + w) * 32 * TR + lane * TR);      // k-step 8 half + w of OB1
+        const uint32_t ro = mapa_u32(sm + (half ? M::T_OB1 : M::P_OB1) + o, peer), rbar = mapa_u32(s_ob1full, peer);
+        mbar_wait(s_ob1free, par ^ 1);
+        if (TR == TU) {
+            const uint4 v = make_uint4(zp[0], zp[1], zp[2], zp[3]);
+            sts128(ob1 + o, v);
+            st_async_v4(ro, v, rbar);
+        } else {
+            sts64(ob1 + o, zp[0], zp[2]);
+            st_async_v2(ro, zp[0], zp[2], rbar);
+        }
+    }
+    bar_compute();
+    mbar_wait(s_ob1full, par);
+    TRACE2(crank, 21);
+#pragma unroll
+    for (int jp = 0; jp < A / 32; jp++) {
+        uint32_t a0[4], a1[4];
+        load_a_rows<TR>(a0, ob1, 2 * jp, lane);
+        load_a_rows<TR>(a1, ob1, 2 * jp + 1, lane);
+        if (jp >= ZPRE) {
+#pragma unroll
+            for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
+        }
+#pragma unroll
+        for (int i = 0; i < 2; i++) hmma(zz[i], a0, zab[i][jp].x, zab[i][jp].y);
+#pragma unroll
+        for (int i = 0; i < 2; i++) hmma(zz[i], a1, zab[i][jp].z, zab[i][jp].w);
+    }
+    // OB1 has been read: arm its barrier for the peer's next half, then free it for both CTAs
+    if (tid == 0) mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2);
+    release(s_ob1free, lane);
+    release_remote(s_ob1free, peer, lane);
+    if (DUMP) {
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+            const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
+            if (v0) { p.Za[(size_t)b0 * A + c] = zz[i][0]; p.Za[(size_t)b0 * A + c + 1] = zz[i][1]; }
+            if (v1) { p.Za[(size_t)b1 * A + c] = zz[i][2]; p.Za[(size_t)b1 * A + c + 1] = zz[i][3]; }
+        }
+    }
+}
+
+// ===================================================================================== chain CTA
+template <int S, int TR, bool DUMP, bool TRC>
+__device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
+{
+    using C = Cfg<S>;
+    using M = CfgC<S, TR>;
+    const WnParams& p = c.p;
+    const unsigned char* img = c.img;
+    const LatImage& im = c.im;
+    const uint32_t sm = c.sm, hw4 = c.hw4, lane16 = c.lane16, xchg = c.xchg;
+    const uint32_t s_full = c.s_full, s_empty = c.s_empty, s_hfull = c.s_hfull, s_hfree = c.s_hfree, s_yfull = c.s_yfull;
+    const uint32_t s_apfull = c.s_apfull, s_apfree = c.s_apfree;
+    const int L = c.L, B = c.B, tid = c.tid, tile = c.tile, slots = c.slots, t_begin = c.t_begin, t_end = c.t_end, ntiles_alloc = c.ntiles_alloc;
+    const int w = c.w, lane = c.lane, g = c.g, t4 = c.t4, b0 = c.b0, b1 = c.b1;
+    const int* ys = c.ys;
+    unsigned long long* trc = c.trc;
+    const int tr_t = c.tr_t;
+    if (w == NCW) {
+        if (lane == 0) {
+            uint32_t pc = 0;
+            for (int t = t_begin; t < t_end; t++)
+                for (int l = 0; l < L; l++, pc++) {
+                    const uint32_t sl = pc & 1;
+                    mbar_wait(s_empty + 8 * sl, ((pc >> 1) & 1) ^ 1);
+                    mbar_arrive_expect_tx(s_full + 8 * sl, M::PIECE0);
+                    tma_load_1d(sm + M::C_RING + sl * M::PIECE0, img + (size_t)l * im.layer_bytes + C::W_CUR, 16384, s_full + 8 * sl);
+                    tma_load_1d(sm + M::C_RING + sl * M::PIECE0 + 16384, img + (size_t)l * im.layer_bytes + C::W_RES, 8192, s_full + 8 * sl);
+                }
+        }
+    } else {
+        const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u;
+        unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048 + hw4;
+        const int cw = 8 * w + 2 * t4;
+        const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16, o_res = 16384u + (uint32_t)(w * 2) * 512 + lane16;
+        const uint32_t r_hbuf = mapa_u32(sm + M::T_HBUF + xchg, 1);            // this thread's slot of the tail CTA's h tiles
+        const uint32_t r_hfull = mapa_u32(s_hfull, 1);
+        const uint32_t s_bias = sm + M::C_BIAS + (uint32_t)(w * 4 + t4) * 32;   // this thread's Bh / Bres pairs of layer 0 (+ 1 KB per layer)
+        const uint32_t s_ap = sm + M::C_AP + (uint32_t)tid * (2 * TR);         // this thread's 2 TR / 4 floats of a pre-activation tile (+ AP per buffer)
+        uint32_t xa[4][4];
+        float accp[2][4];
+        float2 brn = make_float2(0.f, 0.f);
+        float xres[4] = {0.f, 0.f, 0.f, 0.f};
+        int t1 = t_begin, l1 = 0;                          // the coming step (number pn)
+        uint32_t pn = 0;
+        // accp <- (Bh + Lh) + Wprev . x[t-d] of the coming step: computed by the prep CTA, read from this CTA's shared memory
+        auto prep = [&](const bool ap_ok) {
+            if (t1 < t_end) {
+                const uint2 b2 = lds64(s_bias + l1 * 1024 + 16);
+                if (!ap_ok) mbar_wait(s_apfull + 8 * (pn % M::NAP), (pn / M::NAP) & 1);
+                const uint4 a0 = lds128(s_ap + (pn % M::NAP) * M::AP);
+                brn = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
+                if (TR == TU) {
+                    const uint4 a1 = lds128(s_ap + (pn % M::NAP) * M::AP + 16);
+                    accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
+                    accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
+                } else {                                   // row g only: tanh pair, sigmoid pair
+                    accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[1][0] = __uint_as_float(a0.z); accp[1][1] = __uint_as_float(a0.w);
+                    accp[0][2] = accp[0][3] = accp[1][2] = accp[1][3] = 0.f;
+                }
+                // the tile has been read: arm its barrier for the tile NAP steps on (one thread, ordered before this warp's "free"
+                // signal), then hand the buffer back to the prep CTA
+                if (tid == 0) mbar_arrive_expect_tx(s_apfull + 8 * (pn % M::NAP), M::AP);
+                release_remote(s_apfree + 8 * (pn % M::NAP), 2, lane);
+            }
+            pn++;
+            if (++l1 == L) { l1 = 0; t1++; }
+        };
+        {   // prologue: previous-index rows of the first sample; staging of steps 0, 1, 2; pre-activation of step 0
+            const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
+            sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TR + g] * 32 + 4 * w + t4]);
+            if (TR == TU) sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
+        }
+        StepIt it0{t_begin, 0, p.ring_slot};
+        prep(false);                                       // step 0
+        bar_compute();
+
+        uint32_t pc = 0, epar = 0, hcnt = 0;               // ring piece counter, sample parity, h tiles handed over
+        bool ok_f = false, ok_ap = false, ok_hf = false;
+        for (int t = t_begin; t < t_end; t++) {
+            TRACE2(0, 1);
+            if (t > t_begin) {                             // the tail CTA has written this sample's indices into ys
+                mbar_wait(s_yfull, (uint32_t)(t - t_begin - 1) & 1);
+                if (tid == 0 && t + 1 < t_end) mbar_arrive_expect_tx(s_yfull, 2 * TR * 4);          // arm the next hand-back
+            }
+            {   // embedding (reference.cpp:42-57), this warp's 8 channels
+                const int yc0 = ys[g], yc1 = TR == TU ? ys[g + 8] : 0;
+                const uint32_t eo = sm + M::C_EPBUF + epar * (TR * EROW * 4);
+                const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
+                const uint32_t en = sm + M::C_EPBUF + (epar ^ 1) * (TR * EROW * 4);
+                const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4));
+                const float2 c0 = unpack_h2(lds32(sm + M::C_EMB + (yc0 * EROW + 4 * w + t4) * 4));
+                xres[0] = a0.x + c0.x; xres[1] = a0.y + c0.y;
+                if (TR == TU) {
+                    const float2 a1 = unpack_h2(lds32(eo + ((g + 8) * EROW + 4 * w + t4) * 4));
+                    const float2 c1 = unpack_h2(lds32(sm + M::C_EMB + (yc1 * EROW + 4 * w + t4) * 4));
+                    xres[2] = a1.x + c1.x; xres[3] = a1.y + c1.y;
+                }
+                if (p.tanhEmbed) {
+#pragma unroll
+                    for (int i = 0; i < (TR == TU ? 4 : 2); i++) xres[i] = wn::tanhf_fast(xres[i]);
+                }
+                store_x<TR>(xres, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L), rstride, w);
+                cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
+                if (TR == TU) cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
+                cp_async_commit();                         // landed long before the next sample starts (waited for at the end of this one)
+            }
+            bar_compute();
+#pragma unroll
+            for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
+            TRACE2(0, 2);
+
+            for (int l = 0; l < L; l++, pc++) {
+                const uint32_t sl = pc & 1, p1 = sm + M::C_RING + sl * M::PIECE0, fph = (pc >> 1) & 1;
+                const float2 br = brn;
+                if (!ok_f) mbar_wait(s_full + 8 * sl, fph);
+                {
+                    const uint4 bt0 = lds128(p1 + o_t0), bg0 = lds128(p1 + o_g0), bt1 = lds128(p1 + o_t0 + 512), bg1 = lds128(p1 + o_g0 + 512);
+                    float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
+                    hmma(accp[0], xa[0], bt0.x, bt0.y); hmma(accp[1], xa[0], bg0.x, bg0.y); hmma(u0, xa[2], bt1.x, bt1.y); hmma(u1, xa[2], bg1.x, bg1.y);
+                    hmma(accp[0], xa[1], bt0.z, bt0.w); hmma(accp[1], xa[1], bg0.z, bg0.w); hmma(u0, xa[3], bt1.z, bt1.w); hmma(u1, xa[3], bg1.z, bg1.w);
+#pragma unroll
+                    for (int i = 0; i < 4; i++) { accp[0][i] += u0[i]; accp[1][i] += u1[i]; }
+                }
+                // the res GEMM's B fragments (same ring piece), read while the shared-memory pipe is idle under the HMMAs and the
+                // gate, so that only the h tile is read between the barrier below and the res HMMAs
+                const uint4 bw0 = lds128(p1 + o_res), bw1 = lds128(p1 + o_res + 512);
+                {
+                    uint32_t h01, h23;
+                    gate<TR>(accp, sm + M::C_HBUF + xchg, h01, h23);
+                    // the tail CTA's copy: buffer hcnt % NHB, free once the tail has read the tile of two steps ago
+                    if (!ok_hf) mbar_wait(s_hfree + 8 * (hcnt % M::NHB), ((hcnt / M::NHB) & 1) ^ 1);
+                    if (TR == TU) st_async_v2(r_hbuf + (hcnt % M::NHB) * M::XT, h01, h23, r_hfull + 8 * (hcnt % M::NHB));
+                    else st_async_b32(r_hbuf + (hcnt % M::NHB) * M::XT, h01, r_hfull + 8 * (hcnt % M::NHB));
+                    hcnt++;
+                }
+                TRACE2(0, 12);
+                prep(ok_ap);
+                bar_compute();
+                uint32_t ha[4][4];
+#pragma unroll
+                for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], sm + M::C_HBUF, j, lane);
+                TRACE2(0, 10);
+                float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
+                hmma_res(ra, rb, ha, bw0, bw1);
+                release(s_empty + 8 * sl, lane);
+                residual<TR>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
+                TRACE2(0, 14);
+                dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
+                {   // look at the coming step's barriers
+                    const uint32_t npc = pc + 1;
+                    ok_f = mbar_test_wait(s_full + 8 * (npc & 1), (npc >> 1) & 1);
+                    ok_ap = mbar_test_wait(s_apfull + 8 * (pn % M::NAP), (pn / M::NAP) & 1);
+                    ok_hf = mbar_test_wait(s_hfree + 8 * (hcnt % M::NHB), ((hcnt / M::NHB) & 1) ^ 1);
+                }
+                TRACE2(0, 13);
+                if (l + 1 < L) {
+                    bar_compute();
+#pragma unroll
+                    for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
+                }
+                TRACE2(0, 11);
+            }
+            cp_async_wait_all();                           // the previous-index rows of the next sample
+            epar ^= 1;
+            if (++it0.slot == slots) it0.slot = 0;
+            it0.t++;
+        }
+    }
+}
+
+// ===================================================================================== tail CTA
+template <int S, int TR, bool DUMP, bool TRC>
+__device__ __forceinline__ void tail_cta(const ClusterCta& c, int& trn)
+{
+    using C = Cfg<S>;
+    using M = CfgC<S, TR>;
+    const WnParams& p = c.p;
+    const unsigned char* img = c.img;
+    const LatImage& im = c.im;
+    unsigned char* smem_raw = c.smem;
+    const uint32_t sm = c.sm, lane16 = c.lane16;
+    const uint32_t s_full = c.s_full, s_empty = c.s_empty, s_hfull = c.s_hfull, s_hfree = c.s_hfree, s_yfull = c.s_yfull;
+    const uint32_t s_ob0full = c.s_ob0full, s_ob0free = c.s_ob0free, s_lfull = c.s_lfull, s_lfree = c.s_lfree;
+    const int L = c.L, B = c.B, tid = c.tid, ub = c.ub, t_begin = c.t_begin, t_end = c.t_end;
+    const int w = c.w, lane = c.lane, g = c.g, t4 = c.t4, b0 = c.b0, b1 = c.b1;
+    const bool v0 = c.v0, v1 = c.v1;
+    const float* gbias = c.gbias;
+    int* ys = c.ys;
+    unsigned long long* trc = c.trc;
+    const int tr_t = c.tr_t;
+    if (w == NCW) {
+        if (lane == 0) {
+            uint32_t pc = 0;
+            auto put = [&](const unsigned char* src, uint32_t bytes) {
+                const uint32_t sl = pc % M::NSLOT1;
+                mbar_wait(s_empty + 8 * sl, ((pc / M::NSLOT1) & 1) ^ 1);
+                mbar_arrive_expect_tx(s_full + 8 * sl, bytes);
+                tma_load_1d(sm + M::T_RING + sl * M::SLOT1, src, bytes, s_full + 8 * sl);
+                pc++;
+            };
+            for (int t = t_begin; t < t_end; t++)
+                for (int l = 0; l < L; l++) put(img + (size_t)l * im.layer_bytes + C::W_SKIP, S * 128);
+        }
+    } else {
+        const float* s_bout = reinterpret_cast<const float*>(smem_raw + M::T_BOUT);
+        const uint32_t o_skip = (uint32_t)(w * C::NSK * 2) * 512 + lane16;
+        uint4 zsw[2][S / 32];
+        load_out_w<S, TR>(c, zsw, 0);
+        float sk[C::NSK][4];
+#pragma unroll
+        for (int i = 0; i < C::NSK; i++) sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
+        uint32_t pc = 0, hcnt = 0;
+        for (int t = t_begin; t < t_end; t++) {
+            constexpr int RPW = M::RPW;
+            float sel[RPW];                                   // selectors of this warp's rows ub + RPW w + r
+#pragma unroll
+            for (int r = 0; r < RPW; r++) sel[r] = (ub + RPW * w + r) < B ? p.sel[(size_t)t * B + ub + RPW * w + r] : 0.5f;
+            for (int l = 0; l < L; l++, pc++, hcnt++) {
+                const uint32_t hb = sm + M::T_HBUF + (hcnt % M::NHB) * M::XT;
+                mbar_wait(s_hfull + 8 * (hcnt % M::NHB), (hcnt / M::NHB) & 1);
+                TRACE2(1, 16);
+                uint32_t ha[4][4];
+#pragma unroll
+                for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], hb, j, lane);
+                const uint32_t sl = pc % M::NSLOT1, p2 = sm + M::T_RING + sl * M::SLOT1;
+                mbar_wait(s_full + 8 * sl, (pc / M::NSLOT1) & 1);
+#pragma unroll
+                for (int jp = 0; jp < 2; jp++) {
+                    uint4 bw[C::NSK];
+#pragma unroll
+                    for (int i = 0; i < C::NSK; i++) bw[i] = lds128(p2 + o_skip + (i * 2 + jp) * 512);
+#pragma unroll
+                    for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp], bw[i].x, bw[i].y);
+#pragma unroll
+                    for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp + 1], bw[i].z, bw[i].w);
+                }
+                // the h tile has been read (the HMMAs above hold its values): arm its barrier for the tile after next (one thread,
+                // ordered before this warp's "free" signal), then hand the buffer back to the chain CTA
+                if (tid == 0) mbar_arrive_expect_tx(s_hfull + 8 * (hcnt % M::NHB), M::XT);
+                release_remote(s_hfree + 8 * (hcnt % M::NHB), 0, lane);
+                release(s_empty + 8 * sl, lane);
+                TRACE2(1, 15);
+                if (DUMP) {
+                    const float* pre = gbias + im.b_skpre + (size_t)l * S;
+#pragma unroll
+                    for (int i = 0; i < C::NSK; i++) {
+                        const int c = 8 * (w * C::NSK + i) + 2 * t4;
+                        float o0 = sk[i][0] + pre[c], o1 = sk[i][1] + pre[c + 1], o2 = sk[i][2] + pre[c], o3 = sk[i][3] + pre[c + 1];
+                        if (l == L - 1) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); o2 = fmaxf(o2, 0.f); o3 = fmaxf(o3, 0.f); }
+                        if (v0) { p.skipOut[((size_t)l * B + b0) * S + c] = o0; p.skipOut[((size_t)l * B + b0) * S + c + 1] = o1; }
+                        if (v1) { p.skipOut[((size_t)l * B + b1) * S + c] = o2; p.skipOut[((size_t)l * B + b1) * S + c + 1] = o3; }
+                    }
+                }
+            }
+            // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
+            {   // relu(skip + Bskip): TR bytes per pair of skip n-tiles, into this CTA's OB0 and the prep CTA's (free once the
+                // prep's warps have read the previous sample's)
+                uint4 v[C::NSK / 2];
+#pragma unroll
+                for (int i = 0; i < C::NSK; i++) {
+                    uint32_t lo, hi;
+                    relu_skip(sk[i], s_bout, 8 * (w * C::NSK + i) + 2 * t4, lo, hi);
+                    if (i & 1) { v[i >> 1].z = lo; v[i >> 1].w = hi; } else { v[i >> 1].x = lo; v[i >> 1].y = hi; }
+                }
+                mbar_wait(s_ob0free, ((uint32_t)(t - t_begin) & 1) ^ 1);
+                const uint32_t r_ob0full = mapa_u32(s_ob0full, 2);
+#pragma unroll
+                for (int j = 0; j < C::NSK / 2; j++) {
+                    const uint32_t o = (uint32_t)((w * C::NSK / 2 + j) * 32 * TR + lane * TR);
+                    if (TR == TU) {
+                        sts128(sm + M::T_OB0 + o, v[j]);
+                        st_async_v4(mapa_u32(sm + M::P_OB0 + o, 2), v[j], r_ob0full);
+                    } else {                               // rows g: a0 a2
+                        sts64(sm + M::T_OB0 + o, v[j].x, v[j].z);
+                        st_async_v2(mapa_u32(sm + M::P_OB0 + o, 2), v[j].x, v[j].z, r_ob0full);
+                    }
+                }
+            }
+            bar_compute();
+            TRACE2(1, 20);
+            float zz[2][4];
+            out_half<S, TR, DUMP, TRC>(c, trn, t, zsw, 0, zz);
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                const int c = 8 * (2 * w + i) + 2 * t4;
+                sts64(sm + M::T_LBUF + (g * LROW + c) * 4, __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]));
+                if (TR == TU) sts64(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
+            }
+            bar_compute();
+            mbar_wait(s_lfull, (uint32_t)(t - t_begin) & 1);  // columns 128-255 from the prep CTA
+            TRACE2(1, 22);
+            {   // softmax + categorical sample: warp w serves utterances RPW w .. RPW w + RPW - 1 of the tile (two of 16, one of 8);
+                // lane holds 8 consecutive classes of each
+                float e[RPW][8], m[RPW];
+#pragma unroll
+                for (int r = 0; r < RPW; r++) {
+                    m[r] = 0.f;                               // the reference starts the max at 0 (matrix.cpp:171)
+                    const uint4 u0 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane + 4) * 4);
+                    e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
+                    e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
+#pragma unroll
+                    for (int k = 0; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
+                }
+#pragma unroll
+                for (int o = 16; o >= 1; o >>= 1) {
+#pragma unroll
+                    for (int r = 0; r < RPW; r++) m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], o));
+                }
+                // the logits have been read: arm lfull for the prep's next half, then hand the buffer back to it
+                if (tid == 0) mbar_arrive_expect_tx(s_lfull, TR * 128 * 4);
+                release_remote(s_lfree, 2, lane);
+                float incl[RPW], tot_lane[RPW];
+#pragma unroll
+                for (int r = 0; r < RPW; r++) {
+                    const float ms = m[r] * 1.4426950408889634f;
+                    float run = 0.f;
+#pragma unroll
+                    for (int k = 0; k < 8; k++) { run += wn::exp2f_fast(fmaf(e[r][k], 1.4426950408889634f, -ms)); e[r][k] = run; }
+                    incl[r] = tot_lane[r] = run;
+                }
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    float a[RPW];
+#pragma unroll
+                    for (int r = 0; r < RPW; r++) a[r] = __shfl_up_sync(0xffffffffu, incl[r], o);
+                    if (lane >= o) {
+#pragma unroll
+                        for (int r = 0; r < RPW; r++) incl[r] += a[r];
+                    }
+                }
+                int yv[RPW];                                  // the sampled index of each row
+#pragma unroll
+                for (int r = 0; r < RPW; r++) {
+                    const float total = __shfl_sync(0xffffffffu, incl[r], 31);
+                    const float excl = incl[r] - tot_lane[r];
+                    const float target = sel[r] * total;
+                    int cntk = 0;
+#pragma unroll
+                    for (int k = 0; k < 8; k++) cntk += (target < excl + e[r][k]) ? 0 : 1;
+                    const unsigned ball = __ballot_sync(0xffffffffu, target < incl[r]);
+                    const int lf = ball ? __ffs(ball) - 1 : 31;
+                    const int ck = __shfl_sync(0xffffffffu, cntk, lf);
+                    yv[r] = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
+                    const int b = ub + RPW * w + r;
+                    if (DUMP && b < B) {
+                        const float inv = 1.f / total;
+                        float prevv = 0.f;
+#pragma unroll
+                        for (int k = 0; k < 8; k++) { p.P[(size_t)b * A + 8 * lane + k] = (e[r][k] - prevv) * inv; prevv = e[r][k]; }
+                    }
+                }
+                // both rows' indices are chosen before lane 0 stores anything: the shuffles of the second row cannot move past the
+                // first row's stores, so selecting and storing row by row would run the two selections one after the other
+                if (lane == 0) {
+                    int fbk[RPW], yold[RPW];
+#pragma unroll
+                    for (int r = 0; r < RPW; r++) {
+                        const int b = ub + RPW * w + r;
+                        fbk[r] = yv[r];
+                        if (b < B) {
+                            p.yOut[(size_t)b * p.N + t] = yv[r];
+                            if (p.forced) fbk[r] = p.forced[(size_t)b * p.N + t];
+                        } else fbk[r] = 128;
+                        yold[r] = ys[RPW * w + r];
+                        ys[TR + RPW * w + r] = yold[r];
+                        ys[RPW * w + r] = fbk[r];
+                    }
+                    if (t + 1 < t_end) {                      // the chain CTA's copy: data + completion on its yfull barrier
+                        const uint32_t rb = mapa_u32(s_yfull, 0);
+                        const uint32_t ryold = mapa_u32(sm + M::O_YS + (TR + RPW * w) * 4, 0), rycur = mapa_u32(sm + M::O_YS + (RPW * w) * 4, 0);
+                        if (RPW == 2) {
+                            st_async_v2(ryold, (uint32_t)yold[0], (uint32_t)yold[RPW - 1], rb);
+                            st_async_v2(rycur, (uint32_t)fbk[0], (uint32_t)fbk[RPW - 1], rb);
+                        } else {
+                            st_async_b32(ryold, (uint32_t)yold[0], rb);
+                            st_async_b32(rycur, (uint32_t)fbk[0], rb);
+                        }
+                    }
+                }
+            }
+            TRACE2(1, 23);
+            bar_compute();
+        }
+        store_ys<TR>(p, B, ys, ub, tid);
+    }
+}
+
+// ===================================================================================== prep CTA
+// (Bh + Lh) + Wprev . x[t-d] of every step, as far ahead of the chain CTA as its NAP tile buffers allow.  Nothing here depends on
+// the current sample: the history it reads was written by the chain CTA at least L - 9 steps earlier (wn_launch_lat asks for L >= 12).
+template <int S, int TR, bool DUMP, bool TRC>
+__device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
+{
+    using C = Cfg<S>;
+    using M = CfgC<S, TR>;
+    const WnParams& p = c.p;
+    const unsigned char* img = c.img;
+    const LatImage& im = c.im;
+    unsigned char* smem_raw = c.smem;
+    const uint32_t sm = c.sm, hw4 = c.hw4, lane16 = c.lane16;
+    const uint32_t s_full = c.s_full, s_empty = c.s_empty, s_pfull = c.s_pfull, s_apfull = c.s_apfull, s_apfree = c.s_apfree;
+    const uint32_t s_lfull = c.s_lfull, s_lfree = c.s_lfree;
+    const int L = c.L, tid = c.tid, tile = c.tile, slots = c.slots, t_begin = c.t_begin, t_end = c.t_end, ntiles_alloc = c.ntiles_alloc;
+    const int w = c.w, lane = c.lane, g = c.g, t4 = c.t4;
+    unsigned long long* trc = c.trc;
+    const int tr_t = c.tr_t;
+    const int nsteps = p.count * L;
+    if (w == NCW) {
+        if (lane == 0) {
+            int l = 0;
+            for (int n = 0; n < nsteps; n++) {
+                const uint32_t sl = (uint32_t)n % M::NPRING;
+                mbar_wait(s_empty + 8 * sl, (((uint32_t)n / M::NPRING) & 1) ^ 1);
+                mbar_arrive_expect_tx(s_full + 8 * sl, 16384);
+                // Wprev of layer l lives in the block of the layer before it (lat_pack_kernel)
+                tma_load_1d(sm + M::P_RING + sl * 16384, img + (size_t)((l + L - 1) % L) * im.layer_bytes + C::W_PREV, 16384, s_full + 8 * sl);
+                if (++l == L) l = 0;
+            }
+        }
+    } else {
+        int* dil = reinterpret_cast<int*>(smem_raw + M::P_DIL);
+        const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u, cstride = (uint32_t)ntiles_alloc * 4096u;
+        const unsigned char* gring = static_cast<const unsigned char*>(p.ring) + (size_t)tile * 2048;
+        const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16;
+        const uint32_t r_ap = mapa_u32(sm + M::C_AP + (uint32_t)tid * (2 * TR), 0);   // this thread's 2 TR / 4 floats of the chain CTA's tiles
+        const uint32_t r_apfull = mapa_u32(s_apfull, 0);
+        const uint32_t s_cond = sm + M::P_COND + (uint32_t)tid * 16;              // this thread's 16 B of a conditioning tile (+ 4 KB per slot)
+        const uint32_t s_bias = sm + M::P_BIAS + (uint32_t)(w * 4 + t4) * 16;     // this thread's Bh of layer 0 (+ 512 B per layer)
+        // Staging of the step `itp`, three steps before its use, no register and no scoreboard involved:
+        //  * its conditioning tile: every thread copies the 16 bytes it will read back itself (cp.async; completion = the thread's
+        //    own cp.async group, no barrier);
+        //  * its dilated history x_l[t-d] (zero before the start of the utterance, nv_wavenet.cuh:106): warps 0-3, 128 x 16 B,
+        //    completion on an mbarrier (every warp reads the whole tile).
+        // Both are copied as whole 16-byte groups of the 16-row store layouts with cp.async.cg, which bypasses L1, at either tile
+        // height; an 8-row tile picks its rows' words when it reads them back (own_rows).  The history ring is rewritten during the
+        // launch by the chain CTA on another SM with plain stores, and L1 is not coherent across SMs: a narrower copy through L1
+        // (cp.async.ca, the only form below 16 bytes) could find the line of the slot's previous occupant, maxDil + 1 samples old.
+        // NPS = 8 slots: a slot is staged again five steps after its use, and the weight ring (NPRING = 4 pieces) keeps the warps within four.
+        // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
+        StepIt itp{p.hist_t, 0, p.ring_slot};
+        const int h_end = p.hist_t + p.count;
+        uint32_t pcnt = 0;
+        const unsigned char* cptr = static_cast<const unsigned char*>(p.Lh) + (size_t)tile * 4096 + (size_t)(w * 32 + lane) * 16 + (size_t)t_begin * L * cstride;
+        auto stage = [&]() {
+            const uint32_t slot = pcnt % M::NPS;
+            if (itp.t < h_end) cp_async16(s_cond + slot * 4096, cptr);
+            cptr += cstride;
+            if (w < 4) {
+                const int d = dil[itp.l];
+                const uint32_t dst = sm + M::P_PST + slot * 2048 + (uint32_t)(w * 32 + lane) * 16;
+                if (itp.t >= h_end || itp.t < d) {
+                    sts128(dst, make_uint4(0, 0, 0, 0));
+                    mbar_arrive(s_pfull + 8 * slot);
+                } else {
+                    int sl = itp.slot - d; if (sl < 0) sl += slots;
+                    cp_async16(dst, gring + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
+                    cp_async_arrive_noinc(s_pfull + 8 * slot);
+                }
+            }
+            cp_async_commit();
+            pcnt++;
+            if (++itp.l == L) { itp.l = 0; itp.t++; if (++itp.slot == slots) itp.slot = 0; }
+        };
+        uint4 zsw[2][S / 32];
+        load_out_w<S, TR>(c, zsw, 1);
+        // output columns 128-255 of sample t; the logits go to the tail CTA (free once its softmax has read the previous ones)
+        auto out_prep = [&](const int t) {
+            float zz[2][4];
+            TRACE2(2, 30);
+            out_half<S, TR, DUMP, TRC>(c, trn, t, zsw, 1, zz);
+            const uint32_t r_lfull = mapa_u32(s_lfull, 1);
+            mbar_wait(s_lfree, ((uint32_t)(t - t_begin) & 1) ^ 1);
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                const int c = 8 * (16 + 2 * w + i) + 2 * t4;
+                st_async_v2(mapa_u32(sm + M::T_LBUF + (g * LROW + c) * 4, 1), __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]), r_lfull);
+                if (TR == TU) st_async_v2(mapa_u32(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, 1), __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]), r_lfull);
+            }
+            TRACE2(2, 33);
+        };
+        stage(); stage(); stage();
+        int l1 = 0, tout = t_begin;                        // tout: the next sample whose output half is due
+        for (int n = 0; n < nsteps; n++) {
+            const uint32_t sl = (uint32_t)n % M::NPRING, pa = sm + M::P_RING + sl * 16384, slot = (uint32_t)n % M::NPS, buf = (uint32_t)n % M::NAP;
+            cp_async_wait_pending<2>();                    // this thread's conditioning of step n has landed (two later groups may be in flight)
+            // (tanh, tanh, sigmoid, sigmoid) of rows (g, g + 8, g, g + 8); 8-row tiles: (tanh, 0, sigmoid, 0) of their row
+            const uint4 cb = own_rows<TR>(lds128(s_cond + slot * 4096), hw4 != 0);
+            const uint4 bq = lds128(s_bias + l1 * 512);
+            mbar_wait(s_full + 8 * sl, ((uint32_t)n / M::NPRING) & 1);
+            const GateW bw = lds_gate_w(pa, o_t0, o_g0);
+            mbar_wait(s_pfull + 8 * slot, ((uint32_t)n / M::NPS) & 1);
+            uint32_t pb[4][4];
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const uint4 v = own_rows<TR>(lds128(sm + M::P_PST + slot * 2048 + j * 512 + lane16), hw4 != 0);
+                pb[j][0] = v.x; pb[j][1] = v.y; pb[j][2] = v.z; pb[j][3] = v.w;
+            }
+            const float4 bh = make_float4(__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w));
+            const float2 c0 = unpack_h2(cb.x), c1 = unpack_h2(cb.y), c2 = unpack_h2(cb.z), c3 = unpack_h2(cb.w);
+            float a[2][4] = {{bh.x + c0.x, bh.y + c0.y, bh.x + c1.x, bh.y + c1.y}, {bh.z + c2.x, bh.w + c2.y, bh.z + c3.x, bh.w + c3.y}};
+            float u[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+            hmma_k64(a, u, pb, bw);
+            release(s_empty + 8 * sl, lane);
+            // the chain CTA's tile buffer n % NAP is free once it has read tile n - NAP
+            mbar_wait(s_apfree + 8 * buf, ((n / M::NAP) & 1) ^ 1);
+            if (TR == TU) {
+                st_async_v4(r_ap + buf * M::AP, a[0][0] + u[0][0], a[0][1] + u[0][1], a[0][2] + u[0][2], a[0][3] + u[0][3], r_apfull + 8 * buf);
+                st_async_v4(r_ap + buf * M::AP + 16, a[1][0] + u[1][0], a[1][1] + u[1][1], a[1][2] + u[1][2], a[1][3] + u[1][3], r_apfull + 8 * buf);
+            } else {                                       // row g: tanh pair, sigmoid pair
+                st_async_v4(r_ap + buf * M::AP, a[0][0] + u[0][0], a[0][1] + u[0][1], a[1][0] + u[1][0], a[1][1] + u[1][1], r_apfull + 8 * buf);
+            }
+            stage();
+            if (++l1 == L) l1 = 0;
+            // the output half of sample tout: after step (tout + 1, 1) has been shipped, so that the chain CTA starts sample
+            // tout + 1 with its first two pre-activation tiles at hand, and before the wait for the buffer of step
+            // (tout + 1, NAP + 1), which the chain CTA frees only inside sample tout + 1
+            if (n == (tout - t_begin + 1) * L + 1) out_prep(tout++);
+        }
+        while (tout < t_end) out_prep(tout++);             // the last sample: no steps follow it
+        cp_async_wait_all();
+    }
+}
+
 template <int S, int TR, bool DUMP, bool TRC>
 __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
 {
-    // debug timeline (tools/lat_trace.py): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
+    // debug timeline (tools/lat_trace.py, TRACE2): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
     unsigned long long* trc = (TRC && p.trace && blockIdx.x < NCL) ? p.trace : nullptr;
     int trn = 0;
     const int tr_t = p.trace_t & 0xFFFF;
-#define TRACE2(role, tag) do { if (TRC && trc && threadIdx.x == 0 && t == tr_t && trn < 1023) trc[(role) * 1024 + trn++] = ((unsigned long long)(tag) << 48) | (clock64() & 0xFFFFFFFFFFFFull); } while (0)
     using C = Cfg<S>;
     using M = CfgC<S, TR>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -999,22 +1752,23 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
 
-    // barriers (same offsets in every CTA): ring full[4] / empty[4] (the chain uses two of each, the tail three); pfull[NPS] (prep: staged history
-    // tiles); hfull[2] (tail: h tiles, bytes from the chain); hfree[2], yfull, apfull[NAP] (chain: bytes from the tail / the prep CTA);
+    // barriers (same offsets in every CTA): ring full[NRING] / empty[NRING] (the chain uses two of each, the tail NSLOT1, the prep NPRING);
+    // pfull[NPS] (prep: staged history tiles); hfull[NHB] (tail: h tiles, bytes from the chain); hfree[NHB], yfull, apfull[NAP] (chain: bytes from the tail / the prep CTA);
     // apfree[NAP] (prep: arrived by the chain's warps).  Output layers, once per sample: ob0full (prep: relu(skip) bytes from the
     // tail); ob0free (tail: arrived by the prep's warps); ob1full (tail and prep: the peer's relu(Zs) half); ob1free (tail and prep:
     // arrived by the warps of both CTAs once they have read OB1); lfull (tail: the prep's logits bytes); lfree (prep: arrived by the
     // tail's warps once the softmax has read the logits)
-    const uint32_t s_full = sm + M::O_BAR, s_empty = s_full + 32, s_pfull = s_full + 64, s_hfull = s_full + 128, s_hfree = s_full + 144, s_yfull = s_full + 160;
-    const uint32_t s_apfull = s_full + 168, s_apfree = s_full + 200;
-    const uint32_t s_ob0full = s_full + 232, s_ob0free = s_full + 240, s_ob1full = s_full + 248, s_ob1free = s_full + 256;
-    const uint32_t s_lfull = s_full + 264, s_lfree = s_full + 272;
+    const uint32_t bar = sm + M::O_BAR;
+    const uint32_t s_full = bar + M::B_FULL, s_empty = bar + M::B_EMPTY, s_pfull = bar + M::B_PFULL, s_hfull = bar + M::B_HFULL, s_hfree = bar + M::B_HFREE;
+    const uint32_t s_yfull = bar + M::B_YFULL, s_apfull = bar + M::B_APFULL, s_apfree = bar + M::B_APFREE;
+    const uint32_t s_ob0full = bar + M::B_OB0FULL, s_ob0free = bar + M::B_OB0FREE, s_ob1full = bar + M::B_OB1FULL, s_ob1free = bar + M::B_OB1FREE;
+    const uint32_t s_lfull = bar + M::B_LFULL, s_lfree = bar + M::B_LFREE;
     int* ys = reinterpret_cast<int*>(smem_raw + M::O_YS);
 
     if (tid == 0) {
-        for (int i = 0; i < 4; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
+        for (int i = 0; i < M::NRING; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
         for (int i = 0; i < M::NPS; i++) mbar_init(s_pfull + 8 * i, 128);
-        for (int i = 0; i < 2; i++) { mbar_init(s_hfull + 8 * i, 1); mbar_init(s_hfree + 8 * i, NCW); }
+        for (int i = 0; i < M::NHB; i++) { mbar_init(s_hfull + 8 * i, 1); mbar_init(s_hfree + 8 * i, NCW); }
         for (int i = 0; i < M::NAP; i++) { mbar_init(s_apfull + 8 * i, 1); mbar_init(s_apfree + 8 * i, NCW); }
         mbar_init(s_yfull, 1);
         mbar_init(s_ob0full, 1); mbar_init(s_ob0free, NCW); mbar_init(s_ob1full, 1); mbar_init(s_ob1free, 2 * NCW);
@@ -1024,7 +1778,10 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
         // the sampled indices (2 x TR x 4 B) and a pre-activation tile per step (TR x 512 B); once per sample the prep expects relu(skip)
         // and a relu(Zs) half, the tail a relu(Zs) half and the logits half
         if (is_chain) { mbar_arrive_expect_tx(s_yfull, 2 * TR * 4); for (int i = 0; i < M::NAP; i++) mbar_arrive_expect_tx(s_apfull + 8 * i, M::AP); }
-        else if (is_tail) { mbar_arrive_expect_tx(s_hfull, M::XT); mbar_arrive_expect_tx(s_hfull + 8, M::XT); mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2); mbar_arrive_expect_tx(s_lfull, TR * 128 * 4); }
+        else if (is_tail) {
+            for (int i = 0; i < M::NHB; i++) mbar_arrive_expect_tx(s_hfull + 8 * i, M::XT);
+            mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2); mbar_arrive_expect_tx(s_lfull, TR * 128 * 4);
+        }
         else { mbar_arrive_expect_tx(s_ob0full, TR * S * 2); mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2); }
     }
     if (tid < TR) {
@@ -1055,598 +1812,16 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     const bool v0 = b0 < B, v1 = b1 < B;
     const uint32_t lane16 = (uint32_t)lane * 16;
     const uint32_t xchg = xslot<TR>(w, lane);                // this thread's slot of an activation tile
-    auto release = [&](uint32_t bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
-    auto release_remote = [&](uint32_t local_bar, uint32_t rank) { __syncwarp(); if (lane == 0) mbar_arrive_remote(mapa_u32(local_bar, rank)); };
-
-    // ---------------- output layers, tail (half 0) and prep (half 1) CTAs: n-tiles 16 half + 2w and 16 half + 2w + 1 of Zs and Za.
-    // Their B fragments (lat_pack_kernel: piece q of a matrix = k-step pairs [q OJP, (q+1) OJP) of all 32 n-tiles, fragment
-    // (n-tile OJP + jp) x 512 + lane x 16) are loaded once, at kernel start: Wzs into registers (S / 4 per thread), Wza into this
-    // CTA's ZA region, where every thread reads back only the 16 B it stored itself (fragment (2w + i) x A/32 + jp).  Wza resident
-    // in registers as well would not fit: nine warps leave 168 registers per thread (three warps share a sub-partition's 64 KB),
-    // and the tail's skip loop and the prep's step loop would spill ~300 B at S = 256.
-    auto load_out_w = [&](uint4 (&zsw)[2][S / 32], const uint32_t half) {
-        const uint32_t za = sm + (half ? M::P_ZA : M::T_ZA) + lane16;
-#pragma unroll
-        for (int i = 0; i < 2; i++) {
-            const int nt = 16 * half + 2 * w + i;
-#pragma unroll
-            for (int jp = 0; jp < S / 32; jp++)
-                zsw[i][jp] = ldg_nc_v4(img + im.off_zs + (size_t)(jp / C::OJP_ZS) * C::ZS_PIECE + (size_t)(nt * C::OJP_ZS + jp % C::OJP_ZS) * 512 + lane16);
-            for (int jp = 0; jp < A / 32; jp++)
-                sts128(za + ((2 * w + i) * (A / 32) + jp) * 512,
-                       ldg_nc_v4(img + im.off_za + (size_t)(jp / C::OJP_ZA) * C::ZA_PIECE + (size_t)(nt * C::OJP_ZA + jp % C::OJP_ZA) * 512 + lane16));
-        }
-    };
-    // relu(skip + Bskip) is in this CTA's OB0 (the prep waits for it here).  Per n-tile the HMMAs run from the bias through the
-    // k-steps in order on one accumulator, as in the single-CTA kernel.  relu(Zs) of the two n-tiles is k-step 8 half + w of the
-    // Za GEMM's A operand: 16 B per thread into this CTA's OB1 and the peer's.  Leaves the logits of the two n-tiles in zz.
-    auto out_half = [&](const int t, const uint4 (&zsw)[2][S / 32], const uint32_t half, float (&zz)[2][4]) {
-        const uint32_t peer = half ? 1 : 2, par = (uint32_t)(t - t_begin) & 1;
-        const float* bz = reinterpret_cast<const float*>(smem_raw + (half ? M::P_BOUT : M::T_BOUT + S * 4));   // Bzs [A], Bza [A]
-        const uint32_t ob0 = sm + (half ? M::P_OB0 : M::T_OB0), ob1 = sm + (half ? M::P_OB1 : M::T_OB1), za = sm + (half ? M::P_ZA : M::T_ZA);
-#pragma unroll
-        for (int i = 0; i < 2; i++) {
-            const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
-            zz[i][0] = zz[i][2] = bz[c]; zz[i][1] = zz[i][3] = bz[c + 1];
-        }
-        // the Wza fragments of the first half of K (32 registers) are read while the CTA would wait anyway: the prep before relu(skip)
-        // arrives, the tail after its Zs HMMAs, while the prep's relu(Zs) half is still on its way; those of the second half inside
-        // the Za GEMM (three quarters or more up front spill at S = 256)
-        constexpr int ZPRE = A / 64;
-        uint4 zab[2][A / 32];
-        auto load_za = [&]() {
-#pragma unroll
-            for (int jp = 0; jp < ZPRE; jp++)
-#pragma unroll
-                for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
-        };
-        if (half) { load_za(); mbar_wait(s_ob0full, par); }
-#pragma unroll
-        for (int jp = 0; jp < S / 32; jp++) {
-            uint32_t a0[4], a1[4];
-            load_a_rows<TR>(a0, ob0, 2 * jp, lane);
-            load_a_rows<TR>(a1, ob0, 2 * jp + 1, lane);
-#pragma unroll
-            for (int i = 0; i < 2; i++) hmma(zz[i], a0, zsw[i][jp].x, zsw[i][jp].y);
-#pragma unroll
-            for (int i = 0; i < 2; i++) hmma(zz[i], a1, zsw[i][jp].z, zsw[i][jp].w);
-        }
-        if (!half) load_za();
-        if (half) {                                    // OB0 has been read: arm its barrier for the next sample, then free it
-            if (tid == 0) mbar_arrive_expect_tx(s_ob0full, TR * S * 2);
-            release_remote(s_ob0free, 1);
-        }
-        TRACE2(crank, 24);
-        uint32_t zp[4];
-#pragma unroll
-        for (int i = 0; i < 2; i++) {
-            const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
-            const float z0 = fmaxf(zz[i][0], 0.f), z1 = fmaxf(zz[i][1], 0.f), z2 = fmaxf(zz[i][2], 0.f), z3 = fmaxf(zz[i][3], 0.f);
-            zp[2 * i] = pack_h2(z0, z1); zp[2 * i + 1] = pack_h2(z2, z3);
-            if (DUMP) {
-                if (v0) { p.Zs[(size_t)b0 * A + c] = z0; p.Zs[(size_t)b0 * A + c + 1] = z1; }
-                if (v1) { p.Zs[(size_t)b1 * A + c] = z2; p.Zs[(size_t)b1 * A + c + 1] = z3; }
-            }
-            zz[i][0] = zz[i][2] = bz[A + c]; zz[i][1] = zz[i][3] = bz[A + c + 1];
-        }
-        {   // both CTAs' warps have read the previous sample's OB1
-            const uint32_t o = (uint32_t)((8 * half + w) * 32 * TR + lane * TR);      // k-step 8 half + w of OB1
-            const uint32_t ro = mapa_u32(sm + (half ? M::T_OB1 : M::P_OB1) + o, peer), rbar = mapa_u32(s_ob1full, peer);
-            mbar_wait(s_ob1free, par ^ 1);
-            if (TR == TU) {
-                const uint4 v = make_uint4(zp[0], zp[1], zp[2], zp[3]);
-                sts128(ob1 + o, v);
-                st_async_v4(ro, v, rbar);
-            } else {
-                sts64(ob1 + o, zp[0], zp[2]);
-                st_async_v2(ro, zp[0], zp[2], rbar);
-            }
-        }
-        bar_compute();
-        mbar_wait(s_ob1full, par);
-        TRACE2(crank, 21);
-#pragma unroll
-        for (int jp = 0; jp < A / 32; jp++) {
-            uint32_t a0[4], a1[4];
-            load_a_rows<TR>(a0, ob1, 2 * jp, lane);
-            load_a_rows<TR>(a1, ob1, 2 * jp + 1, lane);
-            if (jp >= ZPRE) {
-#pragma unroll
-                for (int i = 0; i < 2; i++) zab[i][jp] = lds128(za + ((2 * w + i) * (A / 32) + jp) * 512 + lane16);
-            }
-#pragma unroll
-            for (int i = 0; i < 2; i++) hmma(zz[i], a0, zab[i][jp].x, zab[i][jp].y);
-#pragma unroll
-            for (int i = 0; i < 2; i++) hmma(zz[i], a1, zab[i][jp].z, zab[i][jp].w);
-        }
-        // OB1 has been read: arm its barrier for the peer's next half, then free it for both CTAs
-        if (tid == 0) mbar_arrive_expect_tx(s_ob1full, TR * 128 * 2);
-        release(s_ob1free);
-        release_remote(s_ob1free, peer);
-        if (DUMP) {
-#pragma unroll
-            for (int i = 0; i < 2; i++) {
-                const int c = 8 * (16 * (int)half + 2 * w + i) + 2 * t4;
-                if (v0) { p.Za[(size_t)b0 * A + c] = zz[i][0]; p.Za[(size_t)b0 * A + c + 1] = zz[i][1]; }
-                if (v1) { p.Za[(size_t)b1 * A + c] = zz[i][2]; p.Za[(size_t)b1 * A + c + 1] = zz[i][3]; }
-            }
-        }
-    };
-
-    if (is_chain) {
-        // ===================================================================================== chain CTA
-        if (warp == NCW) {
-            if (lane == 0) {
-                uint32_t pc = 0;
-                for (int t = t_begin; t < t_end; t++)
-                    for (int l = 0; l < L; l++, pc++) {
-                        const uint32_t sl = pc & 1;
-                        mbar_wait(s_empty + 8 * sl, ((pc >> 1) & 1) ^ 1);
-                        mbar_arrive_expect_tx(s_full + 8 * sl, M::PIECE0);
-                        tma_load_1d(sm + M::C_RING + sl * M::PIECE0, img + (size_t)l * im.layer_bytes + C::W_CUR, 16384, s_full + 8 * sl);
-                        tma_load_1d(sm + M::C_RING + sl * M::PIECE0 + 16384, img + (size_t)l * im.layer_bytes + C::W_RES, 8192, s_full + 8 * sl);
-                    }
-            }
-        } else {
-            const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u;
-            unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048 + hw4;
-            const int cw = 8 * w + 2 * t4;
-            const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16, o_res = 16384u + (uint32_t)(w * 2) * 512 + lane16;
-            const uint32_t r_hbuf = mapa_u32(sm + M::T_HBUF + xchg, 1);            // this thread's slot of the tail CTA's h tiles
-            const uint32_t r_hfull = mapa_u32(s_hfull, 1);
-            const uint32_t s_bias = sm + M::C_BIAS + (uint32_t)(w * 4 + t4) * 32;   // this thread's Bh / Bres pairs of layer 0 (+ 1 KB per layer)
-            const uint32_t s_ap = sm + M::C_AP + (uint32_t)tid * (2 * TR);         // this thread's 2 TR / 4 floats of a pre-activation tile (+ AP per buffer)
-            uint32_t xa[4][4];
-            float accp[2][4];
-            float2 brn = make_float2(0.f, 0.f);
-            float xres[4] = {0.f, 0.f, 0.f, 0.f};
-            int t1 = t_begin, l1 = 0;                          // the coming step (number pn)
-            uint32_t pn = 0;
-            // accp <- (Bh + Lh) + Wprev . x[t-d] of the coming step: computed by the prep CTA, read from this CTA's shared memory
-            auto prep = [&](const bool ap_ok) {
-                if (t1 < t_end) {
-                    const uint2 b2 = lds64(s_bias + l1 * 1024 + 16);
-                    if (!ap_ok) mbar_wait(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
-                    const uint4 a0 = lds128(s_ap + (pn & 3) * M::AP);
-                    brn = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
-                    if (TR == TU) {
-                        const uint4 a1 = lds128(s_ap + (pn & 3) * M::AP + 16);
-                        accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
-                        accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
-                    } else {                                   // row g only: tanh pair, sigmoid pair
-                        accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[1][0] = __uint_as_float(a0.z); accp[1][1] = __uint_as_float(a0.w);
-                        accp[0][2] = accp[0][3] = accp[1][2] = accp[1][3] = 0.f;
-                    }
-                    // the tile has been read: arm its barrier for the tile NAP steps on (one thread, ordered before this warp's "free"
-                    // signal), then hand the buffer back to the prep CTA
-                    if (tid == 0) mbar_arrive_expect_tx(s_apfull + 8 * (pn & 3), M::AP);
-                    release_remote(s_apfree + 8 * (pn & 3), 2);
-                }
-                pn++;
-                if (++l1 == L) { l1 = 0; t1++; }
-            };
-            {   // prologue: previous-index rows of the first sample; staging of steps 0, 1, 2; pre-activation of step 0
-                const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
-                sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TR + g] * 32 + 4 * w + t4]);
-                if (TR == TU) sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
-            }
-            StepIt it0{t_begin, 0, p.ring_slot};
-            prep(false);                                       // step 0
-            bar_compute();
-
-            uint32_t pc = 0, epar = 0, hcnt = 0;               // ring piece counter, sample parity, h tiles handed over
-            bool ok_f = false, ok_ap = false, ok_hf = false;
-            for (int t = t_begin; t < t_end; t++) {
-                TRACE2(0, 1);
-                if (t > t_begin) {                             // the tail CTA has written this sample's indices into ys
-                    mbar_wait(s_yfull, (uint32_t)(t - t_begin - 1) & 1);
-                    if (tid == 0 && t + 1 < t_end) mbar_arrive_expect_tx(s_yfull, 2 * TR * 4);          // arm the next hand-back
-                }
-                {   // embedding (reference.cpp:42-57), this warp's 8 channels
-                    const int yc0 = ys[g], yc1 = TR == TU ? ys[g + 8] : 0;
-                    const uint32_t eo = sm + M::C_EPBUF + epar * (TR * EROW * 4);
-                    const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
-                    const uint32_t en = sm + M::C_EPBUF + (epar ^ 1) * (TR * EROW * 4);
-                    const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4));
-                    const float2 c0 = unpack_h2(lds32(sm + M::C_EMB + (yc0 * EROW + 4 * w + t4) * 4));
-                    xres[0] = a0.x + c0.x; xres[1] = a0.y + c0.y;
-                    if (TR == TU) {
-                        const float2 a1 = unpack_h2(lds32(eo + ((g + 8) * EROW + 4 * w + t4) * 4));
-                        const float2 c1 = unpack_h2(lds32(sm + M::C_EMB + (yc1 * EROW + 4 * w + t4) * 4));
-                        xres[2] = a1.x + c1.x; xres[3] = a1.y + c1.y;
-                    }
-                    if (p.tanhEmbed) {
-#pragma unroll
-                        for (int i = 0; i < (TR == TU ? 4 : 2); i++) xres[i] = wn::tanhf_fast(xres[i]);
-                    }
-                    store_x<TR>(xres, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L), rstride, w);
-                    cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
-                    if (TR == TU) cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
-                    cp_async_commit();                         // landed long before the next sample starts (waited for at the end of this one)
-                }
-                bar_compute();
-#pragma unroll
-                for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
-                TRACE2(0, 2);
-
-                for (int l = 0; l < L; l++, pc++) {
-                    const uint32_t sl = pc & 1, p1 = sm + M::C_RING + sl * M::PIECE0, fph = (pc >> 1) & 1;
-                    const float2 br = brn;
-                    if (!ok_f) mbar_wait(s_full + 8 * sl, fph);
-                    {
-                        const uint4 bt0 = lds128(p1 + o_t0), bg0 = lds128(p1 + o_g0), bt1 = lds128(p1 + o_t0 + 512), bg1 = lds128(p1 + o_g0 + 512);
-                        float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
-                        hmma(accp[0], xa[0], bt0.x, bt0.y); hmma(accp[1], xa[0], bg0.x, bg0.y); hmma(u0, xa[2], bt1.x, bt1.y); hmma(u1, xa[2], bg1.x, bg1.y);
-                        hmma(accp[0], xa[1], bt0.z, bt0.w); hmma(accp[1], xa[1], bg0.z, bg0.w); hmma(u0, xa[3], bt1.z, bt1.w); hmma(u1, xa[3], bg1.z, bg1.w);
-#pragma unroll
-                        for (int i = 0; i < 4; i++) { accp[0][i] += u0[i]; accp[1][i] += u1[i]; }
-                    }
-                    // the res GEMM's B fragments (same ring piece), read while the shared-memory pipe is idle under the HMMAs and the
-                    // gate, so that only the h tile is read between the barrier below and the res HMMAs
-                    const uint4 bw0 = lds128(p1 + o_res), bw1 = lds128(p1 + o_res + 512);
-                    {
-                        uint32_t h01, h23;
-                        gate<TR>(accp, sm + M::C_HBUF + xchg, h01, h23);
-                        // the tail CTA's copy: buffer hcnt & 1, free once the tail has read the tile of two steps ago
-                        if (!ok_hf) mbar_wait(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
-                        if (TR == TU) st_async_v2(r_hbuf + (hcnt & 1) * M::XT, h01, h23, r_hfull + 8 * (hcnt & 1));
-                        else st_async_b32(r_hbuf + (hcnt & 1) * M::XT, h01, r_hfull + 8 * (hcnt & 1));
-                        hcnt++;
-                    }
-                    TRACE2(0, 12);
-                    prep(ok_ap);
-                    bar_compute();
-                    uint32_t ha[4][4];
-#pragma unroll
-                    for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], sm + M::C_HBUF, j, lane);
-                    TRACE2(0, 10);
-                    float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
-                    hmma_res(ra, rb, ha, bw0, bw1);
-                    release(s_empty + 8 * sl);
-                    residual<TR>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
-                    TRACE2(0, 14);
-                    dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
-                    {   // look at the coming step's barriers
-                        const uint32_t npc = pc + 1;
-                        ok_f = mbar_test_wait(s_full + 8 * (npc & 1), (npc >> 1) & 1);
-                        ok_ap = mbar_test_wait(s_apfull + 8 * (pn & 3), (pn >> 2) & 1);
-                        ok_hf = mbar_test_wait(s_hfree + 8 * (hcnt & 1), ((hcnt >> 1) & 1) ^ 1);
-                    }
-                    TRACE2(0, 13);
-                    if (l + 1 < L) {
-                        bar_compute();
-#pragma unroll
-                        for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
-                    }
-                    TRACE2(0, 11);
-                }
-                cp_async_wait_all();                           // the previous-index rows of the next sample
-                epar ^= 1;
-                if (++it0.slot == slots) it0.slot = 0;
-                it0.t++;
-            }
-        }
-    } else if (is_tail) {
-        // ===================================================================================== tail CTA
-        if (warp == NCW) {
-            if (lane == 0) {
-                uint32_t pc = 0;
-                auto put = [&](const unsigned char* src, uint32_t bytes) {
-                    const uint32_t sl = pc % M::NSLOT1;
-                    mbar_wait(s_empty + 8 * sl, ((pc / M::NSLOT1) & 1) ^ 1);
-                    mbar_arrive_expect_tx(s_full + 8 * sl, bytes);
-                    tma_load_1d(sm + M::T_RING + sl * M::SLOT1, src, bytes, s_full + 8 * sl);
-                    pc++;
-                };
-                for (int t = t_begin; t < t_end; t++)
-                    for (int l = 0; l < L; l++) put(img + (size_t)l * im.layer_bytes + C::W_SKIP, S * 128);
-            }
-        } else {
-            const float* s_bout = reinterpret_cast<const float*>(smem_raw + M::T_BOUT);
-            const uint32_t o_skip = (uint32_t)(w * C::NSK * 2) * 512 + lane16;
-            uint4 zsw[2][S / 32];
-            load_out_w(zsw, 0);
-            float sk[C::NSK][4];
-#pragma unroll
-            for (int i = 0; i < C::NSK; i++) sk[i][0] = sk[i][1] = sk[i][2] = sk[i][3] = 0.f;
-            uint32_t pc = 0, hcnt = 0;
-            for (int t = t_begin; t < t_end; t++) {
-                constexpr int RPW = M::RPW;
-                float sel[RPW];                                   // selectors of this warp's rows ub + RPW w + r
-#pragma unroll
-                for (int r = 0; r < RPW; r++) sel[r] = (ub + RPW * w + r) < B ? p.sel[(size_t)t * B + ub + RPW * w + r] : 0.5f;
-                for (int l = 0; l < L; l++, pc++, hcnt++) {
-                    const uint32_t hb = sm + M::T_HBUF + (hcnt & 1) * M::XT;
-                    mbar_wait(s_hfull + 8 * (hcnt & 1), (hcnt >> 1) & 1);
-                    TRACE2(1, 16);
-                    uint32_t ha[4][4];
-#pragma unroll
-                    for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], hb, j, lane);
-                    const uint32_t sl = pc % M::NSLOT1, p2 = sm + M::T_RING + sl * M::SLOT1;
-                    mbar_wait(s_full + 8 * sl, (pc / M::NSLOT1) & 1);
-#pragma unroll
-                    for (int jp = 0; jp < 2; jp++) {
-                        uint4 bw[C::NSK];
-#pragma unroll
-                        for (int i = 0; i < C::NSK; i++) bw[i] = lds128(p2 + o_skip + (i * 2 + jp) * 512);
-#pragma unroll
-                        for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp], bw[i].x, bw[i].y);
-#pragma unroll
-                        for (int i = 0; i < C::NSK; i++) hmma(sk[i], ha[2 * jp + 1], bw[i].z, bw[i].w);
-                    }
-                    // the h tile has been read (the HMMAs above hold its values): arm its barrier for the tile after next (one thread,
-                    // ordered before this warp's "free" signal), then hand the buffer back to the chain CTA
-                    if (tid == 0) mbar_arrive_expect_tx(s_hfull + 8 * (hcnt & 1), M::XT);
-                    release_remote(s_hfree + 8 * (hcnt & 1), 0);
-                    release(s_empty + 8 * sl);
-                    TRACE2(1, 15);
-                    if (DUMP) {
-                        const float* pre = gbias + im.b_skpre + (size_t)l * S;
-#pragma unroll
-                        for (int i = 0; i < C::NSK; i++) {
-                            const int c = 8 * (w * C::NSK + i) + 2 * t4;
-                            float o0 = sk[i][0] + pre[c], o1 = sk[i][1] + pre[c + 1], o2 = sk[i][2] + pre[c], o3 = sk[i][3] + pre[c + 1];
-                            if (l == L - 1) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); o2 = fmaxf(o2, 0.f); o3 = fmaxf(o3, 0.f); }
-                            if (v0) { p.skipOut[((size_t)l * B + b0) * S + c] = o0; p.skipOut[((size_t)l * B + b0) * S + c + 1] = o1; }
-                            if (v1) { p.skipOut[((size_t)l * B + b1) * S + c] = o2; p.skipOut[((size_t)l * B + b1) * S + c + 1] = o3; }
-                        }
-                    }
-                }
-                // ---------------- relu(skip + bias) -> Zs -> Za   (reference.cpp:93-104)
-                {   // relu(skip + Bskip): TR bytes per pair of skip n-tiles, into this CTA's OB0 and the prep CTA's (free once the
-                    // prep's warps have read the previous sample's)
-                    uint4 v[C::NSK / 2];
-#pragma unroll
-                    for (int i = 0; i < C::NSK; i++) {
-                        uint32_t lo, hi;
-                        relu_skip(sk[i], s_bout, 8 * (w * C::NSK + i) + 2 * t4, lo, hi);
-                        if (i & 1) { v[i >> 1].z = lo; v[i >> 1].w = hi; } else { v[i >> 1].x = lo; v[i >> 1].y = hi; }
-                    }
-                    mbar_wait(s_ob0free, ((uint32_t)(t - t_begin) & 1) ^ 1);
-                    const uint32_t r_ob0full = mapa_u32(s_ob0full, 2);
-#pragma unroll
-                    for (int j = 0; j < C::NSK / 2; j++) {
-                        const uint32_t o = (uint32_t)((w * C::NSK / 2 + j) * 32 * TR + lane * TR);
-                        if (TR == TU) {
-                            sts128(sm + M::T_OB0 + o, v[j]);
-                            st_async_v4(mapa_u32(sm + M::P_OB0 + o, 2), v[j], r_ob0full);
-                        } else {                               // rows g: a0 a2
-                            sts64(sm + M::T_OB0 + o, v[j].x, v[j].z);
-                            st_async_v2(mapa_u32(sm + M::P_OB0 + o, 2), v[j].x, v[j].z, r_ob0full);
-                        }
-                    }
-                }
-                bar_compute();
-                TRACE2(1, 20);
-                float zz[2][4];
-                out_half(t, zsw, 0, zz);
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const int c = 8 * (2 * w + i) + 2 * t4;
-                    sts64(sm + M::T_LBUF + (g * LROW + c) * 4, __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]));
-                    if (TR == TU) sts64(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]));
-                }
-                bar_compute();
-                mbar_wait(s_lfull, (uint32_t)(t - t_begin) & 1);  // columns 128-255 from the prep CTA
-                TRACE2(1, 22);
-                {   // softmax + categorical sample: warp w serves utterances RPW w .. RPW w + RPW - 1 of the tile (two of 16, one of 8);
-                    // lane holds 8 consecutive classes of each
-                    float e[RPW][8], m[RPW];
-#pragma unroll
-                    for (int r = 0; r < RPW; r++) {
-                        m[r] = 0.f;                               // the reference starts the max at 0 (matrix.cpp:171)
-                        const uint4 u0 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane + 4) * 4);
-                        e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
-                        e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
-#pragma unroll
-                        for (int k = 0; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
-                    }
-#pragma unroll
-                    for (int o = 16; o >= 1; o >>= 1) {
-#pragma unroll
-                        for (int r = 0; r < RPW; r++) m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], o));
-                    }
-                    // the logits have been read: arm lfull for the prep's next half, then hand the buffer back to it
-                    if (tid == 0) mbar_arrive_expect_tx(s_lfull, TR * 128 * 4);
-                    release_remote(s_lfree, 2);
-                    float incl[RPW], tot_lane[RPW];
-#pragma unroll
-                    for (int r = 0; r < RPW; r++) {
-                        const float ms = m[r] * 1.4426950408889634f;
-                        float run = 0.f;
-#pragma unroll
-                        for (int k = 0; k < 8; k++) { run += wn::exp2f_fast(fmaf(e[r][k], 1.4426950408889634f, -ms)); e[r][k] = run; }
-                        incl[r] = tot_lane[r] = run;
-                    }
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) {
-                        float a[RPW];
-#pragma unroll
-                        for (int r = 0; r < RPW; r++) a[r] = __shfl_up_sync(0xffffffffu, incl[r], o);
-                        if (lane >= o) {
-#pragma unroll
-                            for (int r = 0; r < RPW; r++) incl[r] += a[r];
-                        }
-                    }
-                    int yv[RPW];                                  // the sampled index of each row
-#pragma unroll
-                    for (int r = 0; r < RPW; r++) {
-                        const float total = __shfl_sync(0xffffffffu, incl[r], 31);
-                        const float excl = incl[r] - tot_lane[r];
-                        const float target = sel[r] * total;
-                        int cntk = 0;
-#pragma unroll
-                        for (int k = 0; k < 8; k++) cntk += (target < excl + e[r][k]) ? 0 : 1;
-                        const unsigned ball = __ballot_sync(0xffffffffu, target < incl[r]);
-                        const int lf = ball ? __ffs(ball) - 1 : 31;
-                        const int ck = __shfl_sync(0xffffffffu, cntk, lf);
-                        yv[r] = ball ? 8 * lf + (ck < 7 ? ck : 7) : A - 1;
-                        const int b = ub + RPW * w + r;
-                        if (DUMP && b < B) {
-                            const float inv = 1.f / total;
-                            float prevv = 0.f;
-#pragma unroll
-                            for (int k = 0; k < 8; k++) { p.P[(size_t)b * A + 8 * lane + k] = (e[r][k] - prevv) * inv; prevv = e[r][k]; }
-                        }
-                    }
-                    // both rows' indices are chosen before lane 0 stores anything: the shuffles of the second row cannot move past the
-                    // first row's stores, so selecting and storing row by row would run the two selections one after the other
-                    if (lane == 0) {
-                        int fbk[RPW], yold[RPW];
-#pragma unroll
-                        for (int r = 0; r < RPW; r++) {
-                            const int b = ub + RPW * w + r;
-                            fbk[r] = yv[r];
-                            if (b < B) {
-                                p.yOut[(size_t)b * p.N + t] = yv[r];
-                                if (p.forced) fbk[r] = p.forced[(size_t)b * p.N + t];
-                            } else fbk[r] = 128;
-                            yold[r] = ys[RPW * w + r];
-                            ys[TR + RPW * w + r] = yold[r];
-                            ys[RPW * w + r] = fbk[r];
-                        }
-                        if (t + 1 < t_end) {                      // the chain CTA's copy: data + completion on its yfull barrier
-                            const uint32_t rb = mapa_u32(s_yfull, 0);
-                            const uint32_t ryold = mapa_u32(sm + M::O_YS + (TR + RPW * w) * 4, 0), rycur = mapa_u32(sm + M::O_YS + (RPW * w) * 4, 0);
-                            if (RPW == 2) {
-                                st_async_v2(ryold, (uint32_t)yold[0], (uint32_t)yold[RPW - 1], rb);
-                                st_async_v2(rycur, (uint32_t)fbk[0], (uint32_t)fbk[RPW - 1], rb);
-                            } else {
-                                st_async_b32(ryold, (uint32_t)yold[0], rb);
-                                st_async_b32(rycur, (uint32_t)fbk[0], rb);
-                            }
-                        }
-                    }
-                }
-                TRACE2(1, 23);
-                bar_compute();
-            }
-            store_ys<TR>(p, B, ys, ub, tid);
-        }
-    } else {
-        // ===================================================================================== prep CTA
-        // (Bh + Lh) + Wprev . x[t-d] of every step, as far ahead of the chain CTA as its NAP tile buffers allow.  Nothing here depends on
-        // the current sample: the history it reads was written by the chain CTA at least L - 9 steps earlier (wn_launch_lat asks for L >= 12).
-        const int nsteps = p.count * L;
-        if (warp == NCW) {
-            if (lane == 0) {
-                int l = 0;
-                for (int n = 0; n < nsteps; n++) {
-                    const uint32_t sl = n & 3;
-                    mbar_wait(s_empty + 8 * sl, ((n >> 2) & 1) ^ 1);
-                    mbar_arrive_expect_tx(s_full + 8 * sl, 16384);
-                    // Wprev of layer l lives in the block of the layer before it (lat_pack_kernel)
-                    tma_load_1d(sm + M::P_RING + sl * 16384, img + (size_t)((l + L - 1) % L) * im.layer_bytes + C::W_PREV, 16384, s_full + 8 * sl);
-                    if (++l == L) l = 0;
-                }
-            }
-        } else {
-            int* dil = reinterpret_cast<int*>(smem_raw + M::P_DIL);
-            const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u, cstride = (uint32_t)ntiles_alloc * 4096u;
-            const unsigned char* gring = static_cast<const unsigned char*>(p.ring) + (size_t)tile * 2048;
-            const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16;
-            const uint32_t r_ap = mapa_u32(sm + M::C_AP + (uint32_t)tid * (2 * TR), 0);   // this thread's 2 TR / 4 floats of the chain CTA's tiles
-            const uint32_t r_apfull = mapa_u32(s_apfull, 0);
-            const uint32_t s_cond = sm + M::P_COND + (uint32_t)tid * 16;              // this thread's 16 B of a conditioning tile (+ 4 KB per slot)
-            const uint32_t s_bias = sm + M::P_BIAS + (uint32_t)(w * 4 + t4) * 16;     // this thread's Bh of layer 0 (+ 512 B per layer)
-            // Staging of the step `itp`, three steps before its use, no register and no scoreboard involved:
-            //  * its conditioning tile: every thread copies the 16 bytes it will read back itself (cp.async; completion = the thread's
-            //    own cp.async group, no barrier);
-            //  * its dilated history x_l[t-d] (zero before the start of the utterance, nv_wavenet.cuh:106): warps 0-3, 128 x 16 B,
-            //    completion on an mbarrier (every warp reads the whole tile).
-            // Both are copied as whole 16-byte groups of the 16-row store layouts with cp.async.cg, which bypasses L1, at either tile
-            // height; an 8-row tile picks its rows' words when it reads them back (own_rows).  The history ring is rewritten during the
-            // launch by the chain CTA on another SM with plain stores, and L1 is not coherent across SMs: a narrower copy through L1
-            // (cp.async.ca, the only form below 16 bytes) could find the line of the slot's previous occupant, maxDil + 1 samples old.
-            // NPS = 8 slots: a slot is staged again five steps after its use, and the weight ring (4 pieces) keeps the warps within four.
-            // itp.t counts the (clamped) absolute time of the WnParams, so the test against d is the utterance's.
-            StepIt itp{p.hist_t, 0, p.ring_slot};
-            const int h_end = p.hist_t + p.count;
-            uint32_t pcnt = 0;
-            const unsigned char* cptr = static_cast<const unsigned char*>(p.Lh) + (size_t)tile * 4096 + (size_t)(w * 32 + lane) * 16 + (size_t)t_begin * L * cstride;
-            auto stage = [&]() {
-                const uint32_t slot = pcnt & (M::NPS - 1);
-                if (itp.t < h_end) cp_async16(s_cond + slot * 4096, cptr);
-                cptr += cstride;
-                if (w < 4) {
-                    const int d = dil[itp.l];
-                    const uint32_t dst = sm + M::P_PST + slot * 2048 + (uint32_t)(w * 32 + lane) * 16;
-                    if (itp.t >= h_end || itp.t < d) {
-                        sts128(dst, make_uint4(0, 0, 0, 0));
-                        mbar_arrive(s_pfull + 8 * slot);
-                    } else {
-                        int sl = itp.slot - d; if (sl < 0) sl += slots;
-                        cp_async16(dst, gring + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
-                        cp_async_arrive_noinc(s_pfull + 8 * slot);
-                    }
-                }
-                cp_async_commit();
-                pcnt++;
-                if (++itp.l == L) { itp.l = 0; itp.t++; if (++itp.slot == slots) itp.slot = 0; }
-            };
-            uint4 zsw[2][S / 32];
-            load_out_w(zsw, 1);
-            // output columns 128-255 of sample t; the logits go to the tail CTA (free once its softmax has read the previous ones)
-            auto out_prep = [&](const int t) {
-                float zz[2][4];
-                TRACE2(2, 30);
-                out_half(t, zsw, 1, zz);
-                const uint32_t r_lfull = mapa_u32(s_lfull, 1);
-                mbar_wait(s_lfree, ((uint32_t)(t - t_begin) & 1) ^ 1);
-#pragma unroll
-                for (int i = 0; i < 2; i++) {
-                    const int c = 8 * (16 + 2 * w + i) + 2 * t4;
-                    st_async_v2(mapa_u32(sm + M::T_LBUF + (g * LROW + c) * 4, 1), __float_as_uint(zz[i][0]), __float_as_uint(zz[i][1]), r_lfull);
-                    if (TR == TU) st_async_v2(mapa_u32(sm + M::T_LBUF + ((g + 8) * LROW + c) * 4, 1), __float_as_uint(zz[i][2]), __float_as_uint(zz[i][3]), r_lfull);
-                }
-                TRACE2(2, 33);
-            };
-            stage(); stage(); stage();
-            int l1 = 0, tout = t_begin;                        // tout: the next sample whose output half is due
-            for (int n = 0; n < nsteps; n++) {
-                const uint32_t sl = n & 3, pa = sm + M::P_RING + sl * 16384, slot = n & (M::NPS - 1), buf = n & (M::NAP - 1);
-                cp_async_wait_pending<2>();                    // this thread's conditioning of step n has landed (two later groups may be in flight)
-                // (tanh, tanh, sigmoid, sigmoid) of rows (g, g + 8, g, g + 8); 8-row tiles: (tanh, 0, sigmoid, 0) of their row
-                const uint4 cb = own_rows<TR>(lds128(s_cond + slot * 4096), hw4 != 0);
-                const uint4 bq = lds128(s_bias + l1 * 512);
-                mbar_wait(s_full + 8 * sl, (n >> 2) & 1);
-                const GateW bw = lds_gate_w(pa, o_t0, o_g0);
-                mbar_wait(s_pfull + 8 * slot, (n >> 3) & 1);
-                uint32_t pb[4][4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    const uint4 v = own_rows<TR>(lds128(sm + M::P_PST + slot * 2048 + j * 512 + lane16), hw4 != 0);
-                    pb[j][0] = v.x; pb[j][1] = v.y; pb[j][2] = v.z; pb[j][3] = v.w;
-                }
-                const float4 bh = make_float4(__uint_as_float(bq.x), __uint_as_float(bq.y), __uint_as_float(bq.z), __uint_as_float(bq.w));
-                const float2 c0 = unpack_h2(cb.x), c1 = unpack_h2(cb.y), c2 = unpack_h2(cb.z), c3 = unpack_h2(cb.w);
-                float a[2][4] = {{bh.x + c0.x, bh.y + c0.y, bh.x + c1.x, bh.y + c1.y}, {bh.z + c2.x, bh.w + c2.y, bh.z + c3.x, bh.w + c3.y}};
-                float u[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-                hmma_k64(a, u, pb, bw);
-                release(s_empty + 8 * sl);
-                // the chain CTA's tile buffer n % NAP is free once it has read tile n - NAP
-                mbar_wait(s_apfree + 8 * buf, ((n / M::NAP) & 1) ^ 1);
-                if (TR == TU) {
-                    st_async_v4(r_ap + buf * M::AP, a[0][0] + u[0][0], a[0][1] + u[0][1], a[0][2] + u[0][2], a[0][3] + u[0][3], r_apfull + 8 * buf);
-                    st_async_v4(r_ap + buf * M::AP + 16, a[1][0] + u[1][0], a[1][1] + u[1][1], a[1][2] + u[1][2], a[1][3] + u[1][3], r_apfull + 8 * buf);
-                } else {                                       // row g: tanh pair, sigmoid pair
-                    st_async_v4(r_ap + buf * M::AP, a[0][0] + u[0][0], a[0][1] + u[0][1], a[1][0] + u[1][0], a[1][1] + u[1][1], r_apfull + 8 * buf);
-                }
-                stage();
-                if (++l1 == L) l1 = 0;
-                // the output half of sample tout: after step (tout + 1, 1) has been shipped, so that the chain CTA starts sample
-                // tout + 1 with its first two pre-activation tiles at hand, and before the wait for the buffer of step
-                // (tout + 1, NAP + 1), which the chain CTA frees only inside sample tout + 1
-                if (n == (tout - t_begin + 1) * L + 1) out_prep(tout++);
-            }
-            while (tout < t_end) out_prep(tout++);             // the last sample: no steps follow it
-            cp_async_wait_all();
-        }
-    }
-#undef TRACE2
+    const ClusterCta c{p, img, im, smem_raw, sm, L, B, tid, crank, ub, tile, hw4, slots, t_begin, t_end, ntiles_alloc, gbias,
+                       s_full, s_empty, s_pfull, s_hfull, s_hfree, s_yfull, s_apfull, s_apfree, s_ob0full, s_ob0free, s_ob1full, s_ob1free, s_lfull, s_lfree,
+                       ys, w, lane, g, t4, b0, b1, v0, v1, lane16, xchg, trc, tr_t};
+    if (is_chain) chain_cta<S, TR, DUMP, TRC>(c, trn);
+    else if (is_tail) tail_cta<S, TR, DUMP, TRC>(c, trn);
+    else prep_cta<S, TR, DUMP, TRC>(c, trn);
     // nobody leaves while the peer may still write into this CTA's shared memory or arrive on its barriers
     cluster_sync_all();
 }
+#undef TRACE2
 
 }  // namespace
 
