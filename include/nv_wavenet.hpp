@@ -135,6 +135,27 @@ public:
         return rc == 0;
     }
 
+    /* Not in the reference class: continuous batching over the rows of a streaming engine (slots); see nvwn_restart_slots,
+     * nvwn_set_conditioning_slots and nvwn_set_selectors_random_slots. */
+    bool restart_slots(const int* slots, int n, const unsigned long long* seeds = NULL, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_restart_slots(m_engine, slots, n, seeds, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool set_conditioning_slots(const float* Lh, const int* slots, int n, long long first_sample, int num_samples, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_set_conditioning_slots(m_engine, Lh, slots, n, first_sample, num_samples, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool set_selectors_random_slots(long long first_sample, int num_samples, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_set_selectors_random_slots(m_engine, first_sample, num_samples, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
     /* Not in the reference class: teacher-forced scoring, logp[b * num_samples + t] = log p(audio[b][t] | audio[b][0..t),
      * conditioning) for every step at once, and optionally the fp32 logits; see nvwn_score.  fp16 engines only. */
     bool score(const int* audio, int num_samples, int batch_size, float* logp, float* logits = NULL, cudaStream_t stream = 0)

@@ -110,6 +110,27 @@ int nvwn_run(nvwn_engine* e, int num_samples, int batch_size, int* yOut, int dum
  * Fill the positions of a range (conditioning, selectors, forced indices) before the call, and read them (nvwn_get_yout,
  * nvwn_get_audio) before a later call overwrites them. */
 int nvwn_run_stream(nvwn_engine* e, long long first_sample, int count, int batch_size, int dump_activations, void* stream);
+/* Continuous batching: the B rows of a streaming engine are slots, each serving one utterance after another.  Between launches a
+ * slot's whole state is its row of the history ring and its two fed-back indices, so a new utterance starts in a slot while the
+ * others keep going.  slots / seeds are host arrays of n distinct slots in [0, B), 1 <= n <= B, copied before return (the caller
+ * may reuse them at once, pinned or not).  The rows these calls write (history, conditioning, selectors) are laid out for runs of
+ * the whole batch: after any of them, and until nvwn_reset_history, nvwn_run_stream / nvwn_run_partial with batch_size != B is
+ * NVWN_EINVAL.  The calls share the engine's slot scratch: issue them on one stream, or order them.
+ *
+ * Start a new utterance in each of slots[0..n) at the engine's next sample t0 (the first_sample the next nvwn_run_stream takes):
+ * that row's history is cleared and its fed-back indices set to 128, exactly as at a fresh start; the other rows are not touched.
+ * seeds (NULL = all 0) key the slot's selectors for nvwn_set_selectors_random_slots.  Stream-ordered on `stream`: issue it
+ * after the launch that ends at t0.  nvwn_reset_history sets every slot's start to 0 and its seed to 0. */
+int nvwn_restart_slots(nvwn_engine* e, const int* slots, int n, const unsigned long long* seeds, void* stream);
+/* Lh [num_samples][L][n][2R] fp32 (host or device): conditioning of absolute samples [first_sample, +num_samples) for rows
+ * slots[0..n) only, sample t at position t mod N; num_samples <= N (split at the wrap inside).  A host Lh is staged and the call
+ * returns when it may be released; a device Lh is converted asynchronously on `stream`. */
+int nvwn_set_conditioning_slots(nvwn_engine* e, const float* Lh, const int* slots, int n, long long first_sample, int num_samples, void* stream);
+/* selectors of absolute samples [first_sample, +num_samples), num_samples <= N, for every slot from its (seed, origin): slot b at
+ * sample t gets the Philox draw of counter t - origin[b] under key seed[b] (mapped as nvwn_set_selectors_random), which is what
+ * nvwn_set_selectors_random_stream(seed[b], ...) gives a one-utterance engine at sample t - origin[b]: an utterance's selectors do
+ * not depend on its slot, its start or the batch it shares.  Asynchronous on `stream`. */
+int nvwn_set_selectors_random_slots(nvwn_engine* e, long long first_sample, int num_samples, void* stream);
 /* nv_wavenet.cuh:439-444: 2-D copy of yOut[b][offset .. offset+size) for every b */
 int nvwn_get_yout(nvwn_engine* e, int* yOut, int offset, int size, void* stream);
 /* Output side (SURVEY.md 8f next-3): replaces the host post-processing of pytorch/nv_wavenet_inference.py:55-60 --

@@ -73,6 +73,13 @@ struct WnFamily {
     size_t (*image_bytes)(const WnConfig& c);       // NULL when pack is
     cudaError_t (*convert)(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
     cudaError_t (*readback)(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
+    // Per-utterance-row twins (continuous batching, DESIGN.md §6), rows_dev: n distinct rows in [0, c.B), device memory.
+    // clear_rows zeroes every byte of rows rows_dev[i] in all (maxDil+1) x L history-ring entries and no other byte;
+    // convert_rows converts fp32 [num_pos][L][n][2R] (device) into rows rows_dev[i] of store positions [first_pos, +num_pos),
+    // bit for bit as convert does, and leaves every other row alone.
+    cudaError_t (*clear_rows)(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream);
+    cudaError_t (*convert_rows)(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
+                                cudaStream_t stream);
     cudaError_t (*pack)(void* image, const WnParams& p, cudaStream_t stream);      // weight blob -> image; NULL: the kernels read the blob
     cudaError_t (*launch)(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info);
     bool whole_batch;                               // a run must take all c.B utterances
@@ -89,6 +96,10 @@ int wn_lat_max_clusters(int S, int rows);          // three-CTA clusters of `row
 size_t wn_plain_store_bytes(const WnConfig& c);
 cudaError_t wn_plain_convert(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
 cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
+// ... and its history ring [(maxDil+1)][L][B][R], fp16 on NVWN_FP16 engines, else fp32: the per-row operations of WnFamily
+cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream);
+cudaError_t wn_plain_convert_rows(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
+                                  cudaStream_t stream);
 
 // teacher-forced scoring (wn_score_kernel.cu, DESIGN.md §5.4): one time chunk of T steps x Bs utterances, rows m = (t - t0) * Bs + b
 struct WnScoreChunk {
@@ -119,6 +130,12 @@ cudaError_t wn_f32_to_f16(__half* dst, const float* src_dev, size_t n, cudaStrea
 cudaError_t wn_f16_to_f32(float* dst, const __half* src_dev, size_t n, cudaStream_t stream);
 cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, unsigned long long first, cudaStream_t stream);
 cudaError_t wn_fill_int(int* dst, int value, size_t n, cudaStream_t stream);
+// per-slot selectors: dst[p * B + b], p in [0, n), = the selector of counter first_t + p - origin[b] under key seed[b]
+cudaError_t wn_fill_selectors_slots(float* dst, int n, int B, long long first_t, const long long* origin, const unsigned long long* seed,
+                                    cudaStream_t stream);
+// restart of rows rows[0..n): yPrev = yCur = 128, origin = t0, seed = seeds[i] (seeds NULL: 0)
+cudaError_t wn_restart_rows(const int* rows, int n, const unsigned long long* seeds, long long t0, int* yPrev, int* yCur, long long* origin,
+                            unsigned long long* seed, cudaStream_t stream);
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream);
 

@@ -90,6 +90,48 @@ cudaError_t wn_fill_selectors(float* dst, size_t n, unsigned long long seed, uns
     return cudaGetLastError();
 }
 
+// Per-slot selectors (continuous batching): slot b at absolute sample t draws counter t - origin[b] under key seed[b], which is
+// what a one-utterance engine draws at sample t - origin[b] (counter sample * 1 + 0): an utterance's selectors do not depend on
+// its slot, its start time or the batch it shares.
+__global__ void selectors_slots_kernel(float* __restrict__ dst, size_t n, int B, long long first_t, const long long* __restrict__ origin,
+                                       const unsigned long long* __restrict__ seed)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int b = (int)(i % B);
+        const long long t = first_t + (long long)(i / B);
+        dst[i] = (float)(wn_philox_first((unsigned long long)(t - origin[b]), seed[b]) >> 8) * (1.0f / 16777216.0f);
+    }
+}
+cudaError_t wn_fill_selectors_slots(float* dst, int n, int B, long long first_t, const long long* origin, const unsigned long long* seed,
+                                    cudaStream_t stream)
+{
+    const size_t total = (size_t)n * B;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    selectors_slots_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, total, B, first_t, origin, seed);
+    return cudaGetLastError();
+}
+
+__global__ void restart_rows_kernel(const int* __restrict__ rows, int n, const unsigned long long* __restrict__ seeds, long long t0,
+                                    int* yPrev, int* yCur, long long* origin, unsigned long long* seed)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int b = rows[i];
+        yPrev[b] = 128;                   // silence, as nvwn_reset_history
+        yCur[b] = 128;
+        origin[b] = t0;
+        seed[b] = seeds ? seeds[i] : 0ull;
+    }
+}
+cudaError_t wn_restart_rows(const int* rows, int n, const unsigned long long* seeds, long long t0, int* yPrev, int* yCur, long long* origin,
+                            unsigned long long* seed, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    restart_rows_kernel<<<(n + 255) / 256, 256, 0, stream>>>(rows, n, seeds, t0, yPrev, yCur, origin, seed);
+    return cudaGetLastError();
+}
+
 cudaError_t wn_fill_int(int* dst, int value, size_t n, cudaStream_t stream)
 {
     if (n == 0) return cudaSuccess;
@@ -116,6 +158,63 @@ cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* sto
     const size_t per = (size_t)c.L * c.B * 2 * c.R, n = per * num_samples;
     if (c.dtype == NVWN_FP16) return wn_f16_to_f32(dst_dev, static_cast<const __half*>(store) + (size_t)first_sample * per, n, stream);
     return cudaMemcpyAsync(dst_dev, static_cast<const float*>(store) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
+}
+
+// ring row (entry e = slot * L + layer, utterance rows[i]) = R elements of TD, zeroed as 16-byte words (R * sizeof(TD) >= 64)
+__global__ void plain_clear_rows_kernel(uint4* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int B, int words)
+{
+    const size_t total = (size_t)entries * n * words;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int k = (int)(i % words);
+        const size_t ei = i / words;                              // e * n + i
+        const int r = (int)(ei % n);
+        const size_t e = ei / n;
+        ring[(e * B + rows[r]) * words + k] = make_uint4(0, 0, 0, 0);
+    }
+}
+cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    const int words = c.R * (c.dtype == NVWN_FP16 ? (int)sizeof(__half) : (int)sizeof(float)) / 16;
+    const size_t total = (size_t)(c.maxDil + 1) * c.L * n * words;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    plain_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<uint4*>(ring), rows_dev, n, (c.maxDil + 1) * c.L, c.B, words);
+    return cudaGetLastError();
+}
+
+// fp32 [num_pos][L][n][2R] -> rows rows[i] of the plain store at positions [first_pos, +num_pos); TD = __half rounds as
+// f32_to_f16_kernel does (round to nearest even, element by element)
+template <typename TD>
+__global__ void plain_convert_rows_kernel(TD* __restrict__ dst, const float* __restrict__ src, const int* __restrict__ rows, int n, int first_pos,
+                                          int num_pos, int L, int B, int R2)
+{
+    const size_t total = (size_t)num_pos * L * n * R2;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int k = (int)(i % R2);
+        const size_t row = i / R2;                                // (s * L + l) * n + r
+        const int r = (int)(row % n);
+        const size_t sl = row / n;                                // s * L + l
+        const float v = src[i];
+        TD* d = dst + (((size_t)first_pos * L + sl) * B + rows[r]) * R2 + k;
+        if constexpr (sizeof(TD) == 2) *d = __float2half_rn(v);
+        else *d = v;
+    }
+}
+cudaError_t wn_plain_convert_rows(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
+                                  cudaStream_t stream)
+{
+    const size_t total = (size_t)num_pos * c.L * n * 2 * c.R;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    if (c.dtype == NVWN_FP16)
+        plain_convert_rows_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(static_cast<__half*>(store), src, rows_dev, n, first_pos, num_pos,
+                                                                                 c.L, c.B, 2 * c.R);
+    else
+        plain_convert_rows_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(static_cast<float*>(store), src, rows_dev, n, first_pos, num_pos,
+                                                                                c.L, c.B, 2 * c.R);
+    return cudaGetLastError();
 }
 
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,

@@ -67,6 +67,18 @@ struct nvwn_engine : WnConfig {
     float* stage_dev = nullptr;              // device fp32 staging for host->fp16 uploads (fp16 engines only)
     size_t stage_elems = 0;
 
+    // continuous batching (nvwn_restart_slots): per slot, the absolute sample its utterance started at and its selector key; the
+    // slot indices and seeds of the last per-slot call; fp32 staging of host conditioning for slot rows on engines without stage_dev
+    long long* origin = nullptr;             // [B]
+    unsigned long long* seed = nullptr;      // [B]
+    int* slot_rows = nullptr;                // [B]
+    unsigned long long* slot_seeds = nullptr;    // [B]
+    float* row_stage = nullptr;
+    size_t row_stage_elems = 0;
+    // a per-slot call since the last nvwn_reset_history: its rows (history, conditioning, selectors) sit at the engine's batch
+    // stride, which the kernels read at the run's, so until the next reset a run must take the whole batch
+    bool slot_rows_used = false;
+
     void* image = nullptr;                   // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
 
@@ -97,21 +109,53 @@ namespace {
 // host source through the device staging buffer, whole units at a time, and wait for those copies: the buffer and the source are
 // free again on return.  fp32 engines have no staging buffer: their conversions are copies that also read host memory.
 template <typename Convert>
-int feed(nvwn_engine* e, const float* src, size_t n, size_t unit, cudaStream_t stream, Convert convert)
+int feed_via(float* stage, size_t stage_elems, const float* src, size_t n, size_t unit, cudaStream_t stream, Convert convert)
 {
     if (n == 0) return 0;
-    if (!e->stage_dev || is_device_ptr(src)) {
+    if (!stage || is_device_ptr(src)) {
         CK(convert(src, 0, n));
         return 0;
     }
-    const size_t chunk = e->stage_elems / unit;                              // >= 1: nvwn_create sizes the buffer for it
+    const size_t chunk = stage_elems / unit;                                 // >= 1: the callers size the buffer for it
     for (size_t done = 0; done < n; done += chunk) {
         const size_t m = n - done < chunk ? n - done : chunk;
-        CK(cudaMemcpyAsync(e->stage_dev, src + done * unit, m * unit * sizeof(float), cudaMemcpyHostToDevice, stream));
-        CK(convert(e->stage_dev, done, m));
+        CK(cudaMemcpyAsync(stage, src + done * unit, m * unit * sizeof(float), cudaMemcpyHostToDevice, stream));
+        CK(convert(stage, done, m));
     }
     CK(cudaStreamSynchronize(stream));
     return 0;
+}
+template <typename Convert>
+int feed(nvwn_engine* e, const float* src, size_t n, size_t unit, cudaStream_t stream, Convert convert)
+{
+    return feed_via(e->stage_dev, e->stage_elems, src, n, unit, stream, convert);
+}
+
+// Host array -> device scratch, stream-ordered, through a snapshot in pageable memory: a pageable source is staged before
+// cudaMemcpyAsync returns, so the caller's array (pinned or not) is free again on return.
+template <typename T>
+int copy_snapshot(T* dst_dev, const T* src, int n, cudaStream_t stream)
+{
+    const std::vector<T> snap(src, src + n);
+    CK(cudaMemcpyAsync(dst_dev, snap.data(), (size_t)n * sizeof(T), cudaMemcpyHostToDevice, stream));
+    return 0;
+}
+
+// Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.  Then copies it to the
+// device scratch slot_rows, stream-ordered, and marks the engine's rows as laid out for runs of the whole batch.
+int take_slots(nvwn_engine* e, const char* who, const int* slots, int n, cudaStream_t stream)
+{
+    if (!slots) return fail(NVWN_EINVAL, std::string(who) + ": slots is NULL");
+    if (n < 1 || n > e->B) return fail(NVWN_EINVAL, std::string(who) + ": need 1 <= n <= B (" + std::to_string(e->B) + "); got n = " + std::to_string(n));
+    std::vector<char> seen(e->B, 0);
+    for (int i = 0; i < n; i++) {
+        if (slots[i] < 0 || slots[i] >= e->B)
+            return fail(NVWN_EINVAL, std::string(who) + ": slot " + std::to_string(slots[i]) + " is outside [0, " + std::to_string(e->B) + ")");
+        if (seen[slots[i]]) return fail(NVWN_EINVAL, std::string(who) + ": slot " + std::to_string(slots[i]) + " is given twice");
+        seen[slots[i]] = 1;
+    }
+    e->slot_rows_used = true;
+    return copy_snapshot(e->slot_rows, slots, n, stream);
 }
 
 // dst (TD, device) <- src (fp32, host or device), n elements
@@ -194,6 +238,10 @@ int launch_steps(nvwn_engine* e, const char* who, int pos, long long t_abs, int 
     if (count > 0) {
         if (e->family->whole_batch && batch != e->B)
             return fail(NVWN_EINVAL, std::string(who) + ": the tensor-core path needs batch_size equal to the engine's batch size");
+        if (e->slot_rows_used && batch != e->B)
+            return fail(NVWN_EINVAL, std::string(who) + ": after a per-slot call (nvwn_restart_slots, nvwn_set_conditioning_slots, "
+                                     "nvwn_set_selectors_random_slots) runs need batch_size equal to the engine's batch size (" +
+                                     std::to_string(e->B) + ") until nvwn_reset_history");
         if (e->family->pack && e->image_dirty) {
             CK(e->family->pack(e->image, p, stream));
             e->image_dirty = false;
@@ -310,12 +358,18 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     ALLOC(e->Zs, Bz * A * sizeof(float));
     ALLOC(e->Za, Bz * A * sizeof(float));
     ALLOC(e->P, Bz * A * sizeof(float));
+    ALLOC(e->origin, Bz * sizeof(long long));
+    ALLOC(e->seed, Bz * sizeof(unsigned long long));
+    ALLOC(e->slot_rows, Bz * sizeof(int));
+    ALLOC(e->slot_seeds, Bz * sizeof(unsigned long long));
     if (e->stage_elems) ALLOC(e->stage_dev, e->stage_elems * sizeof(float));
     if (e->family->pack) ALLOC(e->image, e->family->image_bytes(*e));
 #undef ALLOC
     cudaMemsetAsync(e->blob, 0, e->blob_bytes, 0);
     cudaMemsetAsync(e->yOut, 0, Nz * Bz * sizeof(int), 0);
     cudaMemsetAsync(e->ring, 0, ring_bytes, 0);
+    cudaMemsetAsync(e->origin, 0, Bz * sizeof(long long), 0);
+    cudaMemsetAsync(e->seed, 0, Bz * sizeof(unsigned long long), 0);
     wn_fill_int(e->yPrev, 128, Bz, 0);
     wn_fill_int(e->yCur, 128, Bz, 0);
     cudaError_t se = cudaDeviceSynchronize();
@@ -328,7 +382,8 @@ int nvwn_destroy(nvwn_engine* e)
 {
     if (!e) return 0;
     void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
-                    e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch};
+                    e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch,
+                    e->origin, e->seed, e->slot_rows, e->slot_seeds, e->row_stage};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
@@ -493,7 +548,75 @@ int nvwn_reset_history(nvwn_engine* e)
     if (!e) return fail(NVWN_EINVAL, "nvwn_reset_history: NULL engine");
     CK(wn_fill_int(e->yPrev, 128, e->B, 0));      // silenceInputs, nv_wavenet.cuh:213-218
     CK(wn_fill_int(e->yCur, 128, e->B, 0));
+    CK(cudaMemsetAsync(e->origin, 0, (size_t)e->B * sizeof(long long), 0));
+    CK(cudaMemsetAsync(e->seed, 0, (size_t)e->B * sizeof(unsigned long long), 0));
     e->next_t = 0;
+    e->slot_rows_used = false;
+    return 0;
+}
+
+int nvwn_restart_slots(nvwn_engine* e, const int* slots, int n, const unsigned long long* seeds, void* stream)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_restart_slots: NULL engine");
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = take_slots(e, "nvwn_restart_slots", slots, n, st);
+    if (rc != 0) return rc;
+    if (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st))) return rc;
+    // a zero history row and silence fed back are exactly the state of a fresh start (DESIGN.md §6)
+    CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
+    CK(wn_restart_rows(e->slot_rows, n, seeds ? e->slot_seeds : nullptr, e->next_t, e->yPrev, e->yCur, e->origin, e->seed, st));
+    return 0;
+}
+
+int nvwn_set_conditioning_slots(nvwn_engine* e, const float* Lh, const int* slots, int n, long long first_sample, int num_samples, void* stream)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_set_conditioning_slots: NULL engine");
+    if (!Lh) return fail(NVWN_EINVAL, "nvwn_set_conditioning_slots: Lh is NULL");
+    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
+        return fail(NVWN_EINVAL, "nvwn_set_conditioning_slots: need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) +
+                                     ") of the engine");
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = take_slots(e, "nvwn_set_conditioning_slots", slots, n, st);
+    if (rc != 0) return rc;
+    const size_t unit = (size_t)e->L * n * 2 * e->R;                        // floats per sample
+    float* stage = e->stage_dev;
+    size_t stage_elems = e->stage_elems;
+    if (!stage && num_samples > 0 && !is_device_ptr(Lh)) {
+        // the row conversions are kernels: a host source goes through device memory on fp32 engines too
+        size_t want = (size_t)num_samples * unit;
+        if (want > ((size_t)16 << 20)) want = unit > ((size_t)16 << 20) ? unit : ((size_t)16 << 20);
+        if (want > e->row_stage_elems) {
+            if (e->row_stage) { CK(cudaStreamSynchronize(st)); cudaFree(e->row_stage); e->row_stage = nullptr; e->row_stage_elems = 0; }
+            CK(cudaMalloc((void**)&e->row_stage, want * sizeof(float)));
+            e->row_stage_elems = want;
+        }
+        stage = e->row_stage;
+        stage_elems = e->row_stage_elems;
+    }
+    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
+    const int piece_pos[2] = {pos, 0}, piece_len[2] = {head, num_samples - head};
+    const float* src = Lh;
+    for (int k = 0; k < 2 && rc == 0; k++) {
+        rc = feed_via(stage, stage_elems, src, (size_t)piece_len[k], unit, st, [&](const float* s, size_t first, size_t m) {
+            return e->family->convert_rows(*e, e->Lh, s, e->slot_rows, n, piece_pos[k] + (int)first, (int)m, st);
+        });
+        src += (size_t)piece_len[k] * unit;
+    }
+    return rc;
+}
+
+int nvwn_set_selectors_random_slots(nvwn_engine* e, long long first_sample, int num_samples, void* stream)
+{
+    if (!e) return fail(NVWN_EINVAL, "nvwn_set_selectors_random_slots: NULL engine");
+    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
+        return fail(NVWN_EINVAL, "nvwn_set_selectors_random_slots: need first_sample >= 0 and 0 <= num_samples <= num_samples (" +
+                                     std::to_string(e->N) + ") of the engine");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t B = e->B;
+    e->slot_rows_used = true;
+    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
+    CK(wn_fill_selectors_slots(e->sel + (size_t)pos * B, head, e->B, first_sample, e->origin, e->seed, st));
+    CK(wn_fill_selectors_slots(e->sel, num_samples - head, e->B, first_sample + head, e->origin, e->seed, st));
     return 0;
 }
 

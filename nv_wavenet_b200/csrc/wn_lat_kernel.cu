@@ -219,6 +219,43 @@ __global__ void lat_cond_readback_kernel(float* __restrict__ dst, const unsigned
     }
 }
 
+// the row-indexed twin of lat_cond_kernel (continuous batching): fp32 [nsamples][L][n][2R] -> utterances rows[i] of store positions
+// [first_sample, +nsamples).  A row's channel pairs are whole words of the uint4s (.x / .z for rows g, .y / .w for rows g + 8), so
+// the other rows are not touched.
+__global__ void lat_cond_rows_kernel(unsigned char* __restrict__ dst, const float* __restrict__ src, const int* __restrict__ rows, int n,
+                                     int first_sample, int nsamples, int L, int ntiles)
+{
+    const size_t total = (size_t)nsamples * L * n * 64;            // one thread per channel pair
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int c2 = (int)(i & 63);
+        const size_t row = i >> 6;                                  // (s * L + l) * n + r
+        const int b = rows[row % n];
+        const size_t sl = row / n;
+        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3;
+        const int sig = c2 >= 32, cc = (c2 & 31) * 2, w = cc >> 3, t = (cc & 7) >> 1;
+        const float2 f = *reinterpret_cast<const float2*>(src + row * 128 + sig * 64 + cc);
+        const __half2 v = __floats2half2_rn(f.x, f.y);
+        const size_t off = (((size_t)first_sample * L + sl) * ntiles + tile) * 4096 + (size_t)(w * 32 + g * 4 + t) * 16 + (size_t)(2 * sig + hi) * 4;
+        *reinterpret_cast<uint32_t*>(dst + off) = *reinterpret_cast<const uint32_t*>(&v);
+    }
+}
+
+// zero utterances rows[i] in every history-ring entry (slot x L + layer; rstride = ntiles x 2 KB): a row is the 32 words that
+// store_x and the embedding store write for it, k-step j, lane 4 g + t, word 2 half + (row >= 8) of each 16-byte group
+__global__ void lat_ring_clear_rows_kernel(unsigned char* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles)
+{
+    const size_t total = (size_t)entries * n * 32;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int k = (int)(i & 31), j = k >> 3, t = (k >> 1) & 3, half = k & 1;
+        const size_t ei = i >> 5;                                   // e * n + r
+        const int b = rows[ei % n];
+        const size_t e = ei / n;
+        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3;
+        const size_t off = (e * ntiles + tile) * 2048 + (size_t)j * 512 + (size_t)(4 * g + t) * 16 + (size_t)(2 * half + hi) * 4;
+        *reinterpret_cast<uint32_t*>(ring + off) = 0u;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ pack
 // blob (fp16, column-major M x K matrices as uploaded) -> weight image in mma.m16n8k16 B-fragment order.
 // Element (n-tile nt, k-step pair jp, lane = 4 g + t) of a matrix W[M][K] is the uint4
@@ -1856,6 +1893,29 @@ static cudaError_t cond_readback(const WnConfig& c, float* dst_dev, const void* 
     return cudaGetLastError();
 }
 
+static cudaError_t cond_convert_rows(const WnConfig& c, void* store, const float* src_dev, const int* rows_dev, int n, int first_pos, int num_pos,
+                                     cudaStream_t stream)
+{
+    const size_t total = (size_t)num_pos * c.L * n * 64;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 32) blocks = 132 * 32;
+    lat_cond_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(store), src_dev, rows_dev, n, first_pos, num_pos, c.L,
+                                                               lat_tiles(c.B));
+    return cudaGetLastError();
+}
+
+static cudaError_t ring_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
+{
+    const int entries = (c.maxDil + 1) * c.L;
+    const size_t total = (size_t)entries * n * 32;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    lat_ring_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), rows_dev, n, entries, lat_tiles(c.B));
+    return cudaGetLastError();
+}
+
 static cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream)
 {
     const LatImage im = lat_image(p.S, p.L);
@@ -1982,4 +2042,5 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
     return cudaGetLastError();
 }
 
-const WnFamily wn_lat_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, wn_lat_pack, wn_launch_lat, false};
+const WnFamily wn_lat_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, ring_clear_rows, cond_convert_rows,
+                                wn_lat_pack, wn_launch_lat, false};

@@ -113,6 +113,45 @@ __global__ void tc_cond_readback_kernel(float* __restrict__ dst, const unsigned 
     }
 }
 
+// the row-indexed twin of tc_cond_kernel (continuous batching): fp32 [nsamples][L][n][2R] -> utterances rows[i] of store positions
+// [first_sample, +nsamples); a row is whole 16-byte chunks, so the other rows are not touched
+__global__ void tc_cond_rows_kernel(unsigned char* __restrict__ dst, const float* __restrict__ src, const int* __restrict__ rows, int n,
+                                    int first_sample, int nsamples, int L, int B, int TU)
+{
+    const size_t total = (size_t)nsamples * L * n * 16;
+    const size_t bpad = cond_bpad(B, TU);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int c = (int)(i & 15);
+        const size_t rowi = i >> 4;                       // (s * L + l) * n + r
+        const int b = rows[rowi % n];
+        const size_t sl = rowi / n;                       // s * L + l
+        const float4 f0 = *reinterpret_cast<const float4*>(src + rowi * 128 + c * 8);
+        const float4 f1 = *reinterpret_cast<const float4*>(src + rowi * 128 + c * 8 + 4);
+        __half2 h0 = __floats2half2_rn(f0.x, f0.y), h1 = __floats2half2_rn(f0.z, f0.w), h2 = __floats2half2_rn(f1.x, f1.y), h3 = __floats2half2_rn(f1.z, f1.w);
+        uint4 o;
+        o.x = *reinterpret_cast<unsigned*>(&h0); o.y = *reinterpret_cast<unsigned*>(&h1);
+        o.z = *reinterpret_cast<unsigned*>(&h2); o.w = *reinterpret_cast<unsigned*>(&h3);
+        const int tile = b / TU, r = b % TU, half = c >> 3, q = c & 7;
+        const size_t off = (((size_t)first_sample * L + sl) * bpad + (size_t)tile * TU) * 256 + (size_t)half * cond_rows(B, tile, TU) * 128 +
+                           (size_t)r * 128 + (size_t)((q ^ (r & 7)) << 4);
+        *reinterpret_cast<uint4*>(dst + off) = o;
+    }
+}
+
+// zero utterances rows[i] in every history-ring entry (slot x L + layer): each entry holds one 16 KB SW128 tile image per TU
+// utterances, row r of a tile at bytes [128 r, 128 r + 128) (its 16-byte chunks permuted by r & 7 inside them)
+__global__ void tc_ring_clear_rows_kernel(uint4* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles, int TU)
+{
+    const size_t total = (size_t)entries * n * 8;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int q = (int)(i & 7);
+        const size_t ei = i >> 3;                         // e * n + r
+        const int b = rows[ei % n];
+        const size_t e = ei / n;
+        ring[((e * ntiles + b / TU) * TILE + (size_t)(b % TU) * 128) / 16 + q] = make_uint4(0, 0, 0, 0);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ pack
 // blob (fp16, column-major matrices as uploaded) -> tiled / swizzled weight image + fp32 bias block
 __global__ void tc_pack_kernel(WnParams p, unsigned char* __restrict__ img, TcImage im)
@@ -683,6 +722,30 @@ cudaError_t cond_readback(const WnConfig& c, float* dst_dev, const void* store, 
     return cudaGetLastError();
 }
 
+cudaError_t cond_convert_rows(const WnConfig& c, void* store, const float* src_dev, const int* rows_dev, int n, int first_pos, int num_pos,
+                              cudaStream_t stream)
+{
+    const size_t total = (size_t)num_pos * c.L * n * 16;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 4096) blocks = 4096;
+    tc_cond_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(store), src_dev, rows_dev, n, first_pos, num_pos, c.L, c.B,
+                                                              c.tc_tile);
+    return cudaGetLastError();
+}
+
+cudaError_t ring_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
+{
+    const int entries = (c.maxDil + 1) * c.L;
+    const size_t total = (size_t)entries * n * 8;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    tc_ring_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<uint4*>(ring), rows_dev, n, entries, (c.B + c.tc_tile - 1) / c.tc_tile,
+                                                                    c.tc_tile);
+    return cudaGetLastError();
+}
+
 cudaError_t wn_tc_pack(void* image, const WnParams& p, cudaStream_t stream)
 {
     const TcImage im = tc_image(p.S, p.L);
@@ -722,4 +785,5 @@ bool wn_tc_supported(int R_, int S, int A_, int, int)
     return R_ == R && A_ == A && (S == 128 || S == 256);
 }
 
-const WnFamily wn_tc_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, wn_tc_pack, wn_launch_tc, true};
+const WnFamily wn_tc_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, ring_clear_rows, cond_convert_rows,
+                               wn_tc_pack, wn_launch_tc, true};

@@ -197,6 +197,42 @@ class NVWavenetInfer:
         check(self._l.nvwn_run_stream(self._h, first_sample, count, batch_size, int(dump_activations), _stream(stream)), "run_stream")
         return True
 
+    # ---- continuous batching: the B rows are slots, each restarted with a new utterance at a launch boundary ----
+    def _slots(self, slots):
+        s = np.ascontiguousarray(np.asarray(slots, dtype=np.int64).reshape(-1)).astype(np.int32)
+        return C.c_void_p(s.ctypes.data), s
+
+    def restart_slots(self, slots, seeds=None, stream=None):
+        """Starts a new utterance in each of `slots` at the engine's next sample: their history is cleared and silence fed back,
+        the other slots are not touched.  seeds (one per slot, None = 0) key the slots' selectors for
+        set_selectors_random_slots.  Asynchronous on `stream`."""
+        p, s = self._slots(slots)
+        k = None
+        if seeds is not None:
+            k = np.ascontiguousarray([int(v) & (2 ** 64 - 1) for v in seeds], dtype=np.uint64)
+            if k.size != s.size:
+                raise ValueError(f"restart_slots: {s.size} slots but {k.size} seeds")
+        check(self._l.nvwn_restart_slots(self._h, p, s.size, None if k is None else C.c_void_p(k.ctypes.data), _stream(stream)),
+              "restartSlots")
+
+    def set_conditioning_slots(self, Lh, slots, first_sample, stream=None):
+        """Lh [n][L][k][2R] (numpy array or CUDA tensor): the conditioning of absolute samples [first_sample, first_sample + n)
+        for the k slots `slots` only, n <= N.  A CUDA tensor is converted asynchronously on `stream` (keep it alive until then:
+        it is returned)."""
+        p, s = self._slots(slots)
+        shape = tuple(int(v) for v in Lh.shape)
+        if len(shape) != 4 or shape[1:] != (self.L, s.size, 2 * self.R):
+            raise ValueError(f"set_conditioning_slots: Lh must be [n][{self.L}][{s.size}][{2 * self.R}] for {s.size} slots; got {shape}")
+        a, keep = _ptr(Lh, np.float32)
+        n = shape[0]
+        check(self._l.nvwn_set_conditioning_slots(self._h, a, p, s.size, first_sample, n, _stream(stream)), "setConditioningSlots")
+        return keep
+
+    def set_selectors_random_slots(self, first_sample, n, stream=None):
+        """Device selectors of absolute samples [first_sample, first_sample + n) for every slot from its seed and start: an
+        utterance draws what a one-utterance engine draws for it."""
+        check(self._l.nvwn_set_selectors_random_slots(self._h, first_sample, n, _stream(stream)), "setSelectorsRandomSlots")
+
     def reset_history(self):
         check(self._l.nvwn_reset_history(self._h), "resetHistory")
 

@@ -46,6 +46,28 @@ def column_major(x):
     raise AssertionError(f"column_major: unsupported rank {nd}")
 
 
+def plan_slots(lengths, slots, window):
+    """Continuous batching schedule of infer_many: utterances of `lengths` samples, in arrival order, through `slots` slots
+    restarted only at multiples of `window`.  At each window boundary the free slots (lowest first) take the next queued
+    utterances; a slot is free once its utterance has ended.  Returns [(slot, start)] per utterance, start a multiple of window."""
+    if slots < 1 or window < 1:
+        raise ValueError(f"need slots >= 1 and window >= 1; got {slots}, {window}")
+    if any(n < 1 for n in lengths):
+        raise ValueError("every utterance needs at least one sample")
+    ends = [0] * slots                              # sample at which each slot's current utterance ends
+    plan, t = [], 0
+    for n in lengths:
+        while True:
+            free = [s for s in range(slots) if ends[s] <= t]
+            if free:
+                break
+            t = (min(ends) + window - 1) // window * window       # the first boundary at which a slot is free
+        s = free[0]
+        plan.append((s, t))
+        ends[s] = t + n
+    return plan
+
+
 def _expect(name, tensor, shape):
     got = tuple(tensor.size())[:len(shape)]
     if got != tuple(shape):
@@ -154,6 +176,70 @@ class NVWaveNet:
                 eng.get_yout_stream(samples[:, first:first + n], first, n)
         torch.cuda.synchronize()
         return samples
+
+    def infer_many(self, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None):
+        """Continuous batching: generates a queue of utterances of different lengths through one engine of `slots` utterances and
+        `window` samples.  cond_inputs: per utterance, conditioning [2R][L][n_u] (channels x num_layers x samples); seeds: one
+        integer per utterance (device selectors, as infer(seed=...)).  Returns int32 CUDA tensors [n_u], each bit-identical to
+        infer() of that utterance alone with its seed.  The engine runs in windows of `window` samples; at each window boundary
+        the slots whose utterance has ended take the next queued ones in arrival order (plan_slots).  A slot with nothing to do
+        keeps running on stale inputs and its output is discarded.  timing: a dict, or None; if given, receives the GPU seconds
+        spent in restarts and per-slot uploads ("restart_upload_s") and in generation ("generate_s")."""
+        if len(cond_inputs) != len(seeds):
+            raise AssertionError(f"{len(cond_inputs)} utterances but {len(seeds)} seeds")
+        for c in cond_inputs:
+            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * self.R, self.num_layers):
+                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
+        lengths = [int(c.size(2)) for c in cond_inputs]
+        plan = plan_slots(lengths, slots, window)
+        eng = self._engine(slots, window, fp16)
+        eng.reset_history()
+        outs = [torch.empty(n, dtype=torch.int32, device="cuda") for n in lengths]
+        stage = torch.empty((slots, window), dtype=torch.int32, device="cuda")
+        end = max((start + n for (_, start), n in zip(plan, lengths)), default=0)
+        by_start = {}
+        for u, (s, start) in enumerate(plan):
+            by_start.setdefault(start, []).append(u)
+        active = {}                                                   # slot -> utterance
+        events = []
+        for first in range(0, end, window):
+            count = min(window, end - first)
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)] if timing is not None else None
+            if ev:
+                ev[0].record()
+            starting = by_start.get(first, [])
+            for u in starting:
+                active[plan[u][0]] = u
+            if starting:
+                eng.restart_slots([plan[u][0] for u in starting], [seeds[u] for u in starting])
+            live = sorted(s for s, u in active.items() if plan[u][1] + lengths[u] > first)
+            if live:
+                # this window's conditioning of the live slots, [count][L][slots][2R], zero past an utterance's end
+                lh = torch.zeros((count, self.num_layers, len(live), 2 * self.R), dtype=torch.float32, device="cuda")
+                for j, s in enumerate(live):
+                    u = active[s]
+                    a = first - plan[u][1]
+                    m = min(count, lengths[u] - a)
+                    lh[:m, :, j].copy_(cond_inputs[u][:, :, a:a + m].permute(2, 1, 0))
+                eng.set_conditioning_slots(lh, live, first)
+            eng.set_selectors_random_slots(first, count)
+            if ev:
+                ev[1].record()
+            eng.run_stream(first, count, slots)
+            eng.get_yout(stage, 0, count)
+            for s in live:
+                u = active[s]
+                a = first - plan[u][1]
+                m = min(count, lengths[u] - a)
+                outs[u][a:a + m].copy_(stage[s, :m])
+            if ev:
+                ev[2].record()
+                events.append(ev)
+        torch.cuda.synchronize()
+        if timing is not None:
+            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[1]) for e in events) / 1e3
+            timing["generate_s"] = sum(e[1].elapsed_time(e[2]) for e in events) / 1e3
+        return outs
 
     def log_likelihood(self, cond_input, audio):
         """Per-sample log-likelihood of `audio` (int mu-law codes [batch][samples]) given `cond_input` (channels x batch x
