@@ -832,14 +832,17 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
         // ---------------- softmax + categorical sample (matrix.cpp:167-183, reference.cpp:106-121): warp w serves
         // utterances 2w and 2w+1; lane holds 8 consecutive classes of each
         {
-            float e[2][8], m[2] = {0.f, 0.f};                          // the reference starts the max at 0 (matrix.cpp:171)
+            // the max starts from the row's own logits, not at 0 as the CPU model's does (matrix.cpp:171): ex2.approx.ftz flushes
+            // 2^(z - m) below 2^-126, so with a start at 0 a row whose logits all lie below about -87 would sum to 0
+            float e[2][8], m[2];
 #pragma unroll
             for (int r = 0; r < 2; r++) {
                 const uint4 u0 = lds128(sm + C::O_LBUF + ((2 * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + C::O_LBUF + ((2 * w + r) * LROW + 8 * lane + 4) * 4);
                 e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
                 e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
+                m[r] = e[r][0];
 #pragma unroll
-                for (int k = 0; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
+                for (int k = 1; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
             }
 #pragma unroll
             for (int o = 16; o >= 1; o >>= 1) {
@@ -1537,12 +1540,12 @@ __device__ __forceinline__ void tail_cta(const ClusterCta& c, int& trn)
                 float e[RPW][8], m[RPW];
 #pragma unroll
                 for (int r = 0; r < RPW; r++) {
-                    m[r] = 0.f;                               // the reference starts the max at 0 (matrix.cpp:171)
                     const uint4 u0 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane) * 4), u1 = lds128(sm + M::T_LBUF + ((RPW * w + r) * LROW + 8 * lane + 4) * 4);
                     e[r][0] = __uint_as_float(u0.x); e[r][1] = __uint_as_float(u0.y); e[r][2] = __uint_as_float(u0.z); e[r][3] = __uint_as_float(u0.w);
                     e[r][4] = __uint_as_float(u1.x); e[r][5] = __uint_as_float(u1.y); e[r][6] = __uint_as_float(u1.z); e[r][7] = __uint_as_float(u1.w);
+                    m[r] = e[r][0];                           // the row's own logits, not 0 as in the CPU model: see lat_compute
 #pragma unroll
-                    for (int k = 0; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
+                    for (int k = 1; k < 8; k++) m[r] = fmaxf(m[r], e[r][k]);
                 }
 #pragma unroll
                 for (int o = 16; o >= 1; o >>= 1) {

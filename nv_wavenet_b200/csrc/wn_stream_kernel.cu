@@ -555,8 +555,8 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
             if (warp < BT) {
                 const int per = A / 32;
                 const float* z = za + warp * A + lane * per;
-                float mx = 0.f;
-                for (int j = 0; j < per; j++) mx = fmaxf(mx, z[j]);
+                float mx = z[0];                                    // the row's own max, not 0: exp2f_fast flushes below 2^-126
+                for (int j = 1; j < per; j++) mx = fmaxf(mx, z[j]);
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
                 float* e = ex + warp * A + lane * per;
