@@ -156,6 +156,30 @@ public:
         return rc == 0;
     }
 
+    /* Not in the reference class: each slot's conditioning produced on the device from its own utterance's mel frames; see
+     * nvwn_cond_producer_set_weights, nvwn_cond_producer_set_slots and nvwn_cond_producer_run_slots. */
+    bool cond_producer_set_weights(int n_cond_channels, const float* upsample_weight, const float* upsample_bias, int window, int stride,
+                                   const float* cond_weight, const float* cond_bias, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_set_weights(m_engine, n_cond_channels, upsample_weight, upsample_bias, window, stride, cond_weight,
+                                                      cond_bias, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool cond_producer_set_slots(const int* slots, int n, const float* const* features, const int* num_frames, const long long* starts,
+                                 cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_set_slots(m_engine, slots, n, features, num_frames, starts, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool cond_producer_run_slots(const int* slots, int n, long long first_sample, int num_samples, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_run_slots(m_engine, slots, n, first_sample, num_samples, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
     /* Not in the reference class: teacher-forced scoring, logp[b * num_samples + t] = log p(audio[b][t] | audio[b][0..t),
      * conditioning) for every step at once, and optionally the fp32 logits; see nvwn_score.  fp16 engines only. */
     bool score(const int* audio, int num_samples, int batch_size, float* logp, float* logits = NULL, cudaStream_t stream = 0)

@@ -131,6 +131,27 @@ int nvwn_set_conditioning_slots(nvwn_engine* e, const float* Lh, const int* slot
  * nvwn_set_selectors_random_stream(seed[b], ...) gives a one-utterance engine at sample t - origin[b]: an utterance's selectors do
  * not depend on its slot, its start or the batch it shares.  Asynchronous on `stream`. */
 int nvwn_set_selectors_random_slots(nvwn_engine* e, long long first_sample, int num_samples, void* stream);
+/* Per-slot conditioning producer: each slot's conditioning made on the device from its own utterance's mel frames, straight into
+ * that slot's rows of the store (the arithmetic of nvwn_set_conditioning_from_features, utterance by utterance).  The three calls
+ * have their own weights and scratch, apart from nvwn_cond_producer_load / _run, and use neither the slot scratch of the calls
+ * above nor the restart state: they may run on a side stream while the generating stream restarts slots and generates, ordered
+ * only by events (issue the three on one stream: they share scratch).  _set_slots and _run_slots count as per-slot calls for the
+ * whole-batch rule above.
+ *
+ * The conditioning network, as for nvwn_set_conditioning_from_features (host or device memory).  Returns when the sources may be
+ * released.  Forgets the frames attached to every slot. */
+int nvwn_cond_producer_set_weights(nvwn_engine* e, int n_cond_channels, const float* upsample_weight, const float* upsample_bias, int window,
+                                   int stride, const float* cond_weight, const float* cond_bias, void* stream);
+/* Attaches utterance i, frames features[i] [n_cond_channels][num_frames[i]] (num_frames[i] >= 1), to slot slots[i]; its sample 0 is
+ * absolute sample starts[i] >= 0 and it has num_frames[i] * stride samples.  The frames are copied into engine memory: host frames
+ * are staged and may be released on return, device frames are copied in stream order on `stream`.  The host arrays (slots,
+ * features, num_frames, starts) may be reused on return, pinned or not.  nvwn_reset_history forgets every attached utterance. */
+int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const float* const* features, const int* num_frames,
+                                 const long long* starts, void* stream);
+/* Conditioning of absolute samples [first_sample, first_sample + num_samples), num_samples <= N, for rows slots[0..n) only, sample t
+ * at position t mod N: slot s gets sample t - start of its utterance, and 0 at or past that utterance's end.  Every listed slot needs
+ * an attached utterance with start <= first_sample.  Asynchronous on `stream`; other rows are not touched. */
+int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long long first_sample, int num_samples, void* stream);
 /* nv_wavenet.cuh:439-444: 2-D copy of yOut[b][offset .. offset+size) for every b */
 int nvwn_get_yout(nvwn_engine* e, int* yOut, int offset, int size, void* stream);
 /* Output side (SURVEY.md 8f next-3): replaces the host post-processing of pytorch/nv_wavenet_inference.py:55-60 --

@@ -44,6 +44,9 @@ SYMBOLS = {
     "nvwn_restart_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "nvwn_set_conditioning_slots": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_longlong, C.c_int, _vp]),
     "nvwn_set_selectors_random_slots": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp]),
+    "nvwn_cond_producer_set_weights": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "nvwn_cond_producer_set_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp]),
+    "nvwn_cond_producer_run_slots": (C.c_int, [_vp, _vp, C.c_int, C.c_longlong, C.c_int, _vp]),
     "nvwn_get_yout": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp]),
     "nvwn_get_audio": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "nvwn_mulaw_table": (C.c_int, [C.c_int, _vp, _vp, _vp]),

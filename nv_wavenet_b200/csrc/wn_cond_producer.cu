@@ -13,6 +13,8 @@
 // fp32 FMA, every output element accumulated in the order of the shared element functions (so host reference, simple kernels
 // and the tiled kernel below agree bit for bit).  The projection is 94 % of the flops (C3: 0.42 TFLOP per 16000 samples x 64
 // utterances): a register-tiled kernel (128 x 128 outputs per CTA, 8 x 8 per thread, operands through shared memory).
+// The per-slot producer (wn_cond_produce_slots, continuous batching) differs only in the upsampling: each row of a chunk reads its
+// own utterance's frames at its own sample offset; the projection is the same kernel with B = the number of slots.
 #include "wn_common.h"
 
 namespace {
@@ -62,6 +64,36 @@ __global__ void upsample_kernel(float* __restrict__ U, const float* __restrict__
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int co = (int)(i % C), j = (int)((i / C) % m), b = (int)(i / ((size_t)C * m));
         U[i] = upsample_element<true>(feat, WuT, bu, C, T, K, stride, b, co, n0 + j);
+    }
+}
+
+// Per-slot twin of upsample_kernel: U[i][j][co] for the k rows of a chunk, row i = absolute sample n0 + j of the utterance in
+// tab[i], i.e. sample n0 + j - start of its own frames [C][T] at frames + foff.  Samples at or past its end (T * stride) are left
+// at 0: mask_slots_kernel zeroes their projected rows.
+__global__ void upsample_slots_kernel(float* __restrict__ U, const float* __restrict__ frames, const WnCondSlot* __restrict__ tab,
+                                      const float* __restrict__ WuT, const float* __restrict__ bu, int k, int C, int K, int stride, long long n0, int m)
+{
+    const size_t total = (size_t)k * m * C;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int co = (int)(i % C), j = (int)((i / C) % m), r = (int)(i / ((size_t)C * m));
+        const WnCondSlot s = tab[r];
+        const long long n = n0 + j - s.start;
+        U[i] = n < (long long)s.T * stride ? upsample_element<true>(frames + s.foff, WuT, bu, C, s.T, K, stride, 0, co, (int)n) : 0.f;
+    }
+}
+
+// zeroes out[j][l][r][c] for every (j, r) whose sample n0 + j is at or past the end of row r's utterance (the projection of a zero
+// U row is the bias, not 0).  One thread per (j, r): only an utterance's last window has such rows, so almost every thread returns.
+__global__ void mask_slots_kernel(float* __restrict__ out, const WnCondSlot* __restrict__ tab, int k, int L, int R2, int stride, long long n0, int m)
+{
+    const size_t total = (size_t)m * k;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int r = (int)(i % k), j = (int)(i / k);
+        if (n0 + j - tab[r].start < (long long)tab[r].T * stride) continue;
+        for (int l = 0; l < L; l++) {
+            float* row = out + (((size_t)j * L + l) * k + r) * R2;
+            for (int c = 0; c < R2; c++) row[c] = 0.f;
+        }
     }
 }
 
@@ -147,6 +179,19 @@ unsigned grid_for(size_t total)
     return (unsigned)(blocks ? blocks : 1);
 }
 
+// out[j][l][b][2R] from U[b][j][C], j < m: the tiled kernel where its float4 stores fit, else the simple one
+cudaError_t project(float* out, const float* U, const float* Wc, const float* bc, int B, int C, int L, int R, int m, cudaStream_t stream)
+{
+    const int R2 = 2 * R;
+    if (R2 % 4 == 0 && (((size_t)out) & 15) == 0) {
+        const dim3 grid((unsigned)(((size_t)m * B + PT - 1) / PT), (unsigned)((L * R2 + PT - 1) / PT));
+        project_tiled_kernel<<<grid, 256, 0, stream>>>(out, U, Wc, bc, B, C, L, R2, m);
+    } else {
+        project_kernel<<<grid_for((size_t)m * L * B * R2), 256, 0, stream>>>(out, U, Wc, bc, B, C, L, R2, m);
+    }
+    return cudaGetLastError();
+}
+
 }  // namespace
 
 // device pointers throughout; WuT = [K][C][C] transpose made by wn_cond_transpose_wu; U scratch holds B * m * C floats
@@ -163,13 +208,18 @@ cudaError_t wn_cond_produce(float* out, float* U, const float* feat, const float
     upsample_kernel<<<grid_for((size_t)B * m * C), 256, 0, stream>>>(U, feat, WuT, bu, B, C, T, K, stride, n0, m);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    const int R2 = 2 * R;
-    if (R2 % 4 == 0 && (((size_t)out) & 15) == 0) {
-        const dim3 grid((unsigned)(((size_t)m * B + PT - 1) / PT), (unsigned)((L * R2 + PT - 1) / PT));
-        project_tiled_kernel<<<grid, 256, 0, stream>>>(out, U, Wc, bc, B, C, L, R2, m);
-    } else {
-        project_kernel<<<grid_for((size_t)m * L * B * R2), 256, 0, stream>>>(out, U, Wc, bc, B, C, L, R2, m);
-    }
+    return project(out, U, Wc, bc, B, C, L, R, m, stream);
+}
+
+cudaError_t wn_cond_produce_slots(float* out, float* U, const float* frames, const WnCondSlot* tab, const float* WuT, const float* bu, const float* Wc,
+                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, cudaStream_t stream)
+{
+    if (m <= 0) return cudaSuccess;
+    upsample_slots_kernel<<<grid_for((size_t)k * m * C), 256, 0, stream>>>(U, frames, tab, WuT, bu, k, C, K, stride, n0, m);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = project(out, U, Wc, bc, k, C, L, R, m, stream);     // rows b * m + j -> out[j][l][b][2R]: the chunk's layout
+    if (e != cudaSuccess) return e;
+    mask_slots_kernel<<<grid_for((size_t)m * k), 256, 0, stream>>>(out, tab, k, L, 2 * R, stride, n0, m);
     return cudaGetLastError();
 }
 

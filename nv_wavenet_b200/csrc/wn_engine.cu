@@ -87,6 +87,18 @@ struct nvwn_engine : WnConfig {
     size_t cp_floats = 0;
     int cp_C = 0, cp_T = 0, cp_K = 0, cp_stride = 0, cp_chunk = 0;
 
+    // per-slot conditioning producer (nvwn_cond_producer_set_weights / _set_slots / _run_slots), apart from the one above:
+    // Wu | WuT | bu | Wc | bc | U chunk | Lh chunk in one allocation, chunks of up to cs_rows (slot, sample) rows; the frames of
+    // slot b's utterance at cs_frames + b * cs_cap * C; the slot list and WnCondSlot table of the last _run_slots (device); per slot
+    // on the host, the attached utterance's frames (0: none) and absolute start
+    float* cs_scratch = nullptr;
+    int cs_C = 0, cs_K = 0, cs_stride = 0, cs_rows = 0;
+    float* cs_frames = nullptr;
+    int cs_cap = 0;
+    char* cs_tables = nullptr;               // int [B] slots, then WnCondSlot [B]
+    std::vector<int> cs_T;
+    std::vector<long long> cs_start;
+
     // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
     void* score_image = nullptr;
     bool score_dirty = true;                 // set wherever image_dirty is: the image is repacked on the next nvwn_score
@@ -134,16 +146,35 @@ int feed(nvwn_engine* e, const float* src, size_t n, size_t unit, cudaStream_t s
 // Host array -> device scratch, stream-ordered, through a snapshot in pageable memory: a pageable source is staged before
 // cudaMemcpyAsync returns, so the caller's array (pinned or not) is free again on return.
 template <typename T>
-int copy_snapshot(T* dst_dev, const T* src, int n, cudaStream_t stream)
+int copy_snapshot(T* dst_dev, const T* src, size_t n, cudaStream_t stream)
 {
     const std::vector<T> snap(src, src + n);
-    CK(cudaMemcpyAsync(dst_dev, snap.data(), (size_t)n * sizeof(T), cudaMemcpyHostToDevice, stream));
+    CK(cudaMemcpyAsync(dst_dev, snap.data(), n * sizeof(T), cudaMemcpyHostToDevice, stream));
     return 0;
 }
 
-// Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.  Then copies it to the
-// device scratch slot_rows, stream-ordered, and marks the engine's rows as laid out for runs of the whole batch.
-int take_slots(nvwn_engine* e, const char* who, const int* slots, int n, cudaStream_t stream)
+// Floats of the conditioning network in engine memory: Wu [C][C][K] | its [K][C][C] transpose WuT | bu [C] | Wc [L*2R][C] | bc [L*2R]
+size_t cond_weight_floats(const nvwn_engine* e, int C, int K)
+{
+    return 2 * (size_t)C * C * K + C + (size_t)e->L * 2 * e->R * (C + 1);
+}
+
+// The conditioning network into that layout at `w`, from host or device sources, and the transpose the kernels read.  Stream-ordered
+// on `st`: the caller synchronises before the sources may be released.  Both producers load their weights through it.
+cudaError_t put_cond_weights(const nvwn_engine* e, float* w, const float* Wu, const float* bu, const float* Wc, const float* bc, int C, int K,
+                             cudaStream_t st)
+{
+    const size_t n_wu = (size_t)C * C * K, n_wc = (size_t)e->L * 2 * e->R * C, n_bc = (size_t)e->L * 2 * e->R;
+    float* d_wu = w; float* d_wut = d_wu + n_wu; float* d_bu = d_wut + n_wu; float* d_wc = d_bu + C; float* d_bc = d_wc + n_wc;
+    cudaError_t ce = cudaSuccess;
+    auto put = [&](float* dst, const float* src, size_t n) { if (ce == cudaSuccess) ce = cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDefault, st); };
+    put(d_wu, Wu, n_wu); put(d_bu, bu, C); put(d_wc, Wc, n_wc); put(d_bc, bc, n_bc);
+    if (ce == cudaSuccess) ce = wn_cond_transpose_wu(d_wut, d_wu, C, K, st);
+    return ce;
+}
+
+// Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.
+int check_slots(nvwn_engine* e, const char* who, const int* slots, int n)
 {
     if (!slots) return fail(NVWN_EINVAL, std::string(who) + ": slots is NULL");
     if (n < 1 || n > e->B) return fail(NVWN_EINVAL, std::string(who) + ": need 1 <= n <= B (" + std::to_string(e->B) + "); got n = " + std::to_string(n));
@@ -154,6 +185,15 @@ int take_slots(nvwn_engine* e, const char* who, const int* slots, int n, cudaStr
         if (seen[slots[i]]) return fail(NVWN_EINVAL, std::string(who) + ": slot " + std::to_string(slots[i]) + " is given twice");
         seen[slots[i]] = 1;
     }
+    return 0;
+}
+
+// check_slots, then copies the list to the device scratch slot_rows, stream-ordered, and marks the engine's rows as laid out for
+// runs of the whole batch.
+int take_slots(nvwn_engine* e, const char* who, const int* slots, int n, cudaStream_t stream)
+{
+    const int rc = check_slots(e, who, slots, n);
+    if (rc != 0) return rc;
     e->slot_rows_used = true;
     return copy_snapshot(e->slot_rows, slots, n, stream);
 }
@@ -370,6 +410,8 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     cudaMemsetAsync(e->ring, 0, ring_bytes, 0);
     cudaMemsetAsync(e->origin, 0, Bz * sizeof(long long), 0);
     cudaMemsetAsync(e->seed, 0, Bz * sizeof(unsigned long long), 0);
+    e->cs_T.assign(Bz, 0);
+    e->cs_start.assign(Bz, 0);
     wn_fill_int(e->yPrev, 128, Bz, 0);
     wn_fill_int(e->yCur, 128, Bz, 0);
     cudaError_t se = cudaDeviceSynchronize();
@@ -383,7 +425,7 @@ int nvwn_destroy(nvwn_engine* e)
     if (!e) return 0;
     void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
                     e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch,
-                    e->origin, e->seed, e->slot_rows, e->slot_seeds, e->row_stage};
+                    e->origin, e->seed, e->slot_rows, e->slot_seeds, e->row_stage, e->cs_scratch, e->cs_frames, e->cs_tables};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
@@ -455,20 +497,17 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
     const size_t per = (size_t)e->L * e->B * 2 * e->R;                       // floats of conditioning per sample
     int chunk = (int)(((size_t)16 << 20) / per);                             // chunk of whole samples: ~64 MB of fp32 at a time
     if (chunk < 1) chunk = 1;
-    const size_t n_feat = (size_t)e->B * C * T, n_wu = (size_t)C * C * K, n_wc = (size_t)e->L * 2 * e->R * C, n_bc = (size_t)e->L * 2 * e->R;
-    const size_t floats = n_feat + 2 * n_wu + C + n_wc + n_bc + (size_t)e->B * chunk * C + (size_t)chunk * per + 16;
+    const size_t n_feat = (size_t)e->B * C * T;
+    const size_t floats = n_feat + cond_weight_floats(e, C, K) + (size_t)e->B * chunk * C + (size_t)chunk * per + 16;
     if (floats > e->cp_floats) {
         if (e->cp_scratch) { CK(cudaDeviceSynchronize()); cudaFree(e->cp_scratch); e->cp_scratch = nullptr; e->cp_floats = 0; }
         CK(cudaMalloc((void**)&e->cp_scratch, floats * sizeof(float)));
         e->cp_floats = floats;
     }
     e->cp_C = C; e->cp_T = T; e->cp_K = K; e->cp_stride = stride; e->cp_chunk = chunk;
-    float* d_feat = e->cp_scratch; float* d_wu = d_feat + n_feat; float* d_wut = d_wu + n_wu; float* d_bu = d_wut + n_wu;
-    float* d_wc = d_bu + C; float* d_bc = d_wc + n_wc;
-    cudaError_t ce = cudaSuccess;
-    auto put = [&](float* dst, const float* src, size_t n) { if (ce == cudaSuccess) ce = cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDefault, st); };
-    put(d_feat, features, n_feat); put(d_wu, upsample_weight, n_wu); put(d_bu, upsample_bias, C); put(d_wc, cond_weight, n_wc); put(d_bc, cond_bias, n_bc);
-    if (ce == cudaSuccess) ce = wn_cond_transpose_wu(d_wut, d_wu, C, K, st);
+    float* d_feat = e->cp_scratch;
+    cudaError_t ce = cudaMemcpyAsync(d_feat, features, n_feat * sizeof(float), cudaMemcpyDefault, st);
+    if (ce == cudaSuccess) ce = put_cond_weights(e, d_feat + n_feat, upsample_weight, upsample_bias, cond_weight, cond_bias, C, K, st);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);                   // host sources may be released by the caller now
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_cond_producer_load: ") + cudaGetErrorString(ce));
     return 0;
@@ -543,6 +582,135 @@ int nvwn_set_conditioning_from_features(nvwn_engine* e, const float* features, i
     return 0;
 }
 
+int nvwn_cond_producer_set_weights(nvwn_engine* e, int n_cond_channels, const float* upsample_weight, const float* upsample_bias, int window,
+                                   int stride, const float* cond_weight, const float* cond_bias, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_set_weights";
+    if (!e || !upsample_weight || !upsample_bias || !cond_weight || !cond_bias) return fail(NVWN_EINVAL, who + ": NULL argument");
+    const int C = n_cond_channels, K = window;
+    if (C < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, who + ": bad sizes (need n_cond_channels >= 1 and window >= stride >= 1)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t lrow = (size_t)e->L * 2 * e->R;                             // floats of one (slot, sample) row of conditioning
+    size_t rows = ((size_t)16 << 20) / lrow;                                  // chunks of ~64 MB of fp32, and of at least one sample
+    if (rows < (size_t)e->B) rows = e->B;                                     // of every slot
+    if (!e->cs_scratch || C != e->cs_C || K != e->cs_K) {
+        if (e->cs_scratch || e->cs_frames) CK(cudaDeviceSynchronize());
+        if (e->cs_scratch) { cudaFree(e->cs_scratch); e->cs_scratch = nullptr; }
+        if (e->cs_frames) { cudaFree(e->cs_frames); e->cs_frames = nullptr; e->cs_cap = 0; }      // sized for the old channel count
+        if (!e->cs_tables) CK(cudaMalloc((void**)&e->cs_tables, align_up((size_t)e->B * sizeof(int), 16) + (size_t)e->B * sizeof(WnCondSlot)));
+        CK(cudaMalloc((void**)&e->cs_scratch, (cond_weight_floats(e, C, K) + rows * (C + lrow) + 16) * sizeof(float)));
+    }
+    e->cs_C = C; e->cs_K = K; e->cs_stride = stride; e->cs_rows = (int)rows;
+    e->cs_T.assign(e->B, 0);                                                  // frames attached under the old network are forgotten
+    cudaError_t ce = put_cond_weights(e, e->cs_scratch, upsample_weight, upsample_bias, cond_weight, cond_bias, C, K, st);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);                   // host sources may be released by the caller now
+    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
+    return 0;
+}
+
+int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const float* const* features, const int* num_frames,
+                                 const long long* starts, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_set_slots";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (!e->cs_scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
+    int rc = check_slots(e, who.c_str(), slots, n);
+    if (rc != 0) return rc;
+    if (!features || !num_frames || !starts) return fail(NVWN_EINVAL, who + ": features, num_frames or starts is NULL");
+    const int C = e->cs_C;
+    int most = 0;
+    for (int i = 0; i < n; i++) {
+        const std::string u = "utterance " + std::to_string(i) + " (slot " + std::to_string(slots[i]) + ")";
+        if (!features[i]) return fail(NVWN_EINVAL, who + ": the frames of " + u + " are NULL");
+        if (num_frames[i] < 1) return fail(NVWN_EINVAL, who + ": " + u + " has num_frames = " + std::to_string(num_frames[i]) + "; need >= 1");
+        if ((long long)num_frames[i] * e->cs_stride > INT_MAX) return fail(NVWN_EINVAL, who + ": " + u + " has more than INT_MAX samples");
+        if (starts[i] < 0) return fail(NVWN_EINVAL, who + ": " + u + " starts at " + std::to_string(starts[i]) + " < 0");
+        if (num_frames[i] > most) most = num_frames[i];
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (most > e->cs_cap) {
+        // a larger arena; the frames of the other slots move with it
+        const int cap = most > 2 * e->cs_cap ? most : 2 * e->cs_cap;
+        float* grown = nullptr;
+        CK(cudaMalloc((void**)&grown, (size_t)e->B * cap * C * sizeof(float)));
+        if (e->cs_frames) {
+            const size_t old_pitch = (size_t)e->cs_cap * C * sizeof(float);
+            cudaError_t ce = cudaMemcpy2DAsync(grown, (size_t)cap * C * sizeof(float), e->cs_frames, old_pitch, old_pitch, e->B, cudaMemcpyDeviceToDevice, st);
+            if (ce == cudaSuccess) ce = cudaDeviceSynchronize();             // no launch reads the old arena any more
+            if (ce != cudaSuccess) { cudaFree(grown); return fail((int)ce, who + ": " + cudaGetErrorString(ce)); }
+            cudaFree(e->cs_frames);
+        }
+        e->cs_frames = grown;
+        e->cs_cap = cap;
+    }
+    for (int i = 0; i < n; i++) {
+        float* dst = e->cs_frames + (size_t)slots[i] * e->cs_cap * C;
+        const size_t count = (size_t)C * num_frames[i];
+        if (is_device_ptr(features[i])) CK(cudaMemcpyAsync(dst, features[i], count * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        else if ((rc = copy_snapshot(dst, features[i], count, st))) return rc;     // staged: the caller may reuse its memory on return
+    }
+    for (int i = 0; i < n; i++) {
+        e->cs_T[slots[i]] = num_frames[i];
+        e->cs_start[slots[i]] = starts[i];
+    }
+    e->slot_rows_used = true;
+    return 0;
+}
+
+int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long long first_sample, int num_samples, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_run_slots";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (!e->cs_scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
+    int rc = check_slots(e, who.c_str(), slots, n);
+    if (rc != 0) return rc;
+    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
+        return fail(NVWN_EINVAL, who + ": need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) + ") of the engine");
+    const int C = e->cs_C, L = e->L, R = e->R;
+    std::vector<WnCondSlot> tab(n);
+    for (int i = 0; i < n; i++) {
+        const int s = slots[i];
+        if (e->cs_T[s] < 1)
+            return fail(NVWN_EINVAL, who + ": slot " + std::to_string(s) + " has no frames attached (nvwn_cond_producer_set_slots; nvwn_reset_history "
+                                           "and nvwn_cond_producer_set_weights forget them)");
+        if (first_sample < e->cs_start[s])
+            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " is before the start " + std::to_string(e->cs_start[s]) +
+                                         " of slot " + std::to_string(s) + "'s utterance");
+        tab[i] = {(long long)s * e->cs_cap * C, e->cs_start[s], e->cs_T[s], 0};
+    }
+    e->slot_rows_used = true;
+    if (num_samples == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    // the slot list and the table in one copy, staged from pageable memory: the caller's arrays are free again on return
+    const size_t tab_off = align_up((size_t)e->B * sizeof(int), 16);
+    std::vector<char> host(tab_off + (size_t)n * sizeof(WnCondSlot));
+    memcpy(host.data(), slots, (size_t)n * sizeof(int));
+    memcpy(host.data() + tab_off, tab.data(), (size_t)n * sizeof(WnCondSlot));
+    CK(cudaMemcpyAsync(e->cs_tables, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+    const int* d_slots = reinterpret_cast<const int*>(e->cs_tables);
+    const WnCondSlot* d_tab = reinterpret_cast<const WnCondSlot*>(e->cs_tables + tab_off);
+
+    const size_t n_wu = (size_t)C * C * e->cs_K, n_wc = (size_t)L * 2 * R * C, n_bc = (size_t)L * 2 * R;
+    const float* d_wut = e->cs_scratch + n_wu; const float* d_bu = d_wut + n_wu; const float* d_wc = d_bu + C; const float* d_bc = d_wc + n_wc;
+    float* d_u = e->cs_scratch + 2 * n_wu + C + n_wc + n_bc;
+    float* d_out = d_u + (size_t)e->cs_rows * C;
+    d_out += (4 - ((size_t)(d_out - e->cs_scratch) & 3)) & 3;                 // 16-byte aligned rows for the tiled projection's float4 stores
+    const int chunk = e->cs_rows / n;                                         // whole samples of every listed slot; >= 1 as cs_rows >= B
+    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
+    const int piece_pos[2] = {pos, 0}, piece_len[2] = {head, num_samples - head};
+    cudaError_t ce = cudaSuccess;
+    for (int p = 0; p < 2; p++) {
+        const long long t0 = first_sample + (p ? head : 0);
+        for (int done = 0; done < piece_len[p] && ce == cudaSuccess; done += chunk) {
+            const int m = piece_len[p] - done < chunk ? piece_len[p] - done : chunk;
+            ce = wn_cond_produce_slots(d_out, d_u, e->cs_frames, d_tab, d_wut, d_bu, d_wc, d_bc, n, C, e->cs_K, e->cs_stride, L, R, t0 + done, m, st);
+            if (ce == cudaSuccess) ce = e->family->convert_rows(*e, e->Lh, d_out, d_slots, n, piece_pos[p] + done, m, st);
+        }
+    }
+    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
+    return 0;
+}
+
 int nvwn_reset_history(nvwn_engine* e)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_reset_history: NULL engine");
@@ -552,6 +720,7 @@ int nvwn_reset_history(nvwn_engine* e)
     CK(cudaMemsetAsync(e->seed, 0, (size_t)e->B * sizeof(unsigned long long), 0));
     e->next_t = 0;
     e->slot_rows_used = false;
+    e->cs_T.assign(e->B, 0);                      // attached frames: their starts are absolute samples of the old timeline
     return 0;
 }
 

@@ -233,6 +233,56 @@ class NVWavenetInfer:
         utterance draws what a one-utterance engine draws for it."""
         check(self._l.nvwn_set_selectors_random_slots(self._h, first_sample, n, _stream(stream)), "setSelectorsRandomSlots")
 
+    # ---- per-slot conditioning producer: each slot's conditioning from its own utterance's mel frames, on the device ----
+    def cond_producer_set_weights(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, stream=None):
+        """The conditioning network of set_conditioning_from_features (upsample_weight [C][C][window], upsample_bias [C],
+        cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]), for cond_producer_run_slots.  Forgets every attached utterance."""
+        shp = lambda a: tuple(int(v) for v in a.shape)
+        Cc = shp(upsample_weight)[0]
+        if (len(shp(upsample_weight)) != 3 or shp(upsample_weight)[1] != Cc or shp(upsample_bias) != (Cc,)
+                or shp(cond_weight)[:2] != (self.L * 2 * self.R, Cc) or shp(cond_bias) != (self.L * 2 * self.R,)):
+            raise ValueError(f"cond_producer_set_weights: need upsample_weight [C][C][window], upsample_bias [C], cond_weight "
+                             f"[{self.L * 2 * self.R}][C], cond_bias [{self.L * 2 * self.R}]; got {shp(upsample_weight)}, {shp(upsample_bias)}, "
+                             f"{shp(cond_weight)}, {shp(cond_bias)}")
+        window = shp(upsample_weight)[2]
+        wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
+        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
+        check(self._l.nvwn_cond_producer_set_weights(self._h, Cc, wu, bu, window, stride, wc, bc, _stream(stream)), "condProducerSetWeights")
+        self._cond_channels = Cc
+
+    def cond_producer_set_slots(self, slots, features, starts, stream=None):
+        """Attaches utterance i, mel frames features[i] [C][T_i] (numpy array or torch tensor), to slot slots[i], its sample 0 at
+        absolute sample starts[i].  Host frames are copied before return; CUDA frames are copied in order on `stream`: keep what
+        this returns alive until then."""
+        p, s = self._slots(slots)
+        if len(features) != s.size or len(starts) != s.size:
+            raise ValueError(f"cond_producer_set_slots: {s.size} slots, {len(features)} frame arrays and {len(starts)} starts")
+        keep, ptrs = [], (C.c_void_p * s.size)()
+        counts = np.empty(s.size, np.int32)
+        import contextlib
+        on_stream = contextlib.nullcontext()
+        if hasattr(stream, "cuda_stream"):                 # CUDA frames that need a contiguous fp32 copy get it on `stream`
+            import torch
+            on_stream = torch.cuda.stream(stream)
+        with on_stream:
+            for i, f in enumerate(features):
+                shape = tuple(int(v) for v in f.shape)
+                if len(shape) != 2 or shape[0] != getattr(self, "_cond_channels", shape[0]):
+                    raise ValueError(f"cond_producer_set_slots: frames must be [C][T] with the C of cond_producer_set_weights; got {shape}")
+                a, k = _ptr(f, np.float32)
+                ptrs[i], counts[i] = a, shape[1]
+                keep.append(k)
+        st = np.ascontiguousarray([int(v) for v in starts], dtype=np.int64)
+        check(self._l.nvwn_cond_producer_set_slots(self._h, p, s.size, ptrs, C.c_void_p(counts.ctypes.data), C.c_void_p(st.ctypes.data),
+                                                   _stream(stream)), "condProducerSetSlots")
+        return keep
+
+    def cond_producer_run_slots(self, slots, first_sample, num_samples, stream=None):
+        """Conditioning of absolute samples [first_sample, first_sample + num_samples), num_samples <= N, for `slots` only, from
+        their attached utterances (0 past an utterance's end).  Asynchronous on `stream`."""
+        p, s = self._slots(slots)
+        check(self._l.nvwn_cond_producer_run_slots(self._h, p, s.size, first_sample, num_samples, _stream(stream)), "condProducerRunSlots")
+
     def reset_history(self):
         check(self._l.nvwn_reset_history(self._h), "resetHistory")
 

@@ -68,6 +68,25 @@ def plan_slots(lengths, slots, window):
     return plan
 
 
+def _windows(plan, lengths, window):
+    """The windows of a plan_slots schedule: per window, (first sample, samples, utterances that start there, live slots as
+    [(slot, utterance, its first sample in the window, its samples in the window)], slots ascending)."""
+    end = max((start + n for (_, start), n in zip(plan, lengths)), default=0)
+    by_start = {}
+    for u, (s, start) in enumerate(plan):
+        by_start.setdefault(start, []).append(u)
+    active, out = {}, []                                           # slot -> utterance
+    for first in range(0, end, window):
+        count = min(window, end - first)
+        starting = by_start.get(first, [])
+        for u in starting:
+            active[plan[u][0]] = u
+        live = [(s, u, first - plan[u][1], min(count, plan[u][1] + lengths[u] - first))
+                for s, u in sorted(active.items()) if plan[u][1] + lengths[u] > first]
+        out.append((first, count, starting, live))
+    return out
+
+
 def _expect(name, tensor, shape):
     got = tuple(tensor.size())[:len(shape)]
     if got != tuple(shape):
@@ -192,54 +211,136 @@ class NVWaveNet:
                 raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
         lengths = [int(c.size(2)) for c in cond_inputs]
         plan = plan_slots(lengths, slots, window)
+        windows = _windows(plan, lengths, window)
         eng = self._engine(slots, window, fp16)
         eng.reset_history()
-        outs = [torch.empty(n, dtype=torch.int32, device="cuda") for n in lengths]
-        stage = torch.empty((slots, window), dtype=torch.int32, device="cuda")
-        end = max((start + n for (_, start), n in zip(plan, lengths)), default=0)
-        by_start = {}
-        for u, (s, start) in enumerate(plan):
-            by_start.setdefault(start, []).append(u)
-        active = {}                                                   # slot -> utterance
-        events = []
-        for first in range(0, end, window):
-            count = min(window, end - first)
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)] if timing is not None else None
-            if ev:
-                ev[0].record()
-            starting = by_start.get(first, [])
-            for u in starting:
-                active[plan[u][0]] = u
-            if starting:
-                eng.restart_slots([plan[u][0] for u in starting], [seeds[u] for u in starting])
-            live = sorted(s for s, u in active.items() if plan[u][1] + lengths[u] > first)
+
+        def condition(k):
+            first, count, _, live = windows[k]
             if live:
                 # this window's conditioning of the live slots, [count][L][slots][2R], zero past an utterance's end
                 lh = torch.zeros((count, self.num_layers, len(live), 2 * self.R), dtype=torch.float32, device="cuda")
-                for j, s in enumerate(live):
-                    u = active[s]
-                    a = first - plan[u][1]
-                    m = min(count, lengths[u] - a)
+                for j, (_, u, a, m) in enumerate(live):
                     lh[:m, :, j].copy_(cond_inputs[u][:, :, a:a + m].permute(2, 1, 0))
-                eng.set_conditioning_slots(lh, live, first)
-            eng.set_selectors_random_slots(first, count)
-            if ev:
-                ev[1].record()
-            eng.run_stream(first, count, slots)
-            eng.get_yout(stage, 0, count)
-            for s in live:
-                u = active[s]
-                a = first - plan[u][1]
-                m = min(count, lengths[u] - a)
-                outs[u][a:a + m].copy_(stage[s, :m])
-            if ev:
-                ev[2].record()
-                events.append(ev)
+                eng.set_conditioning_slots(lh, [s for s, _, _, _ in live], first)
+
+        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition)
         torch.cuda.synchronize()
         if timing is not None:
-            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[1]) for e in events) / 1e3
-            timing["generate_s"] = sum(e[1].elapsed_time(e[2]) for e in events) / 1e3
+            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
+            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
         return outs
+
+    def infer_many_from_features(self, features, seeds, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots=64,
+                                 window=4096, fp16=False, timing=None):
+        """Continuous batching from mel frames: infer_many with each utterance given as its frames [C][T_u] instead of expanded
+        conditioning.  Utterance u has T_u * stride samples.  The weights are those of set_conditioning_from_features
+        (upsample_weight [C][C][w], upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]).  Returns int32
+        CUDA tensors [T_u * stride], each bit-identical to infer() of that utterance alone with its seed and the conditioning the
+        producer's arithmetic gives it (nvwn_cond_from_features_host).
+        The schedule is infer_many's, through an engine of two windows: on a side stream the per-slot conditioning producer makes
+        window k + 1 of the slots live then, while the current stream generates window k.  frames and weights may be numpy arrays
+        or torch tensors (CUDA ones are read in stream order).  timing: a dict, or None; if given, receives the GPU seconds of
+        production on the side stream ("produce_s"), the time generation waited for it ("produce_wait_s"), of restarts and
+        selectors ("restart_select_s") and of generation ("generate_s")."""
+        shp = lambda a: tuple(int(v) for v in a.shape)
+        if len(features) != len(seeds):
+            raise AssertionError(f"{len(features)} utterances but {len(seeds)} seeds")
+        lr = self.num_layers * 2 * self.R
+        if len(shp(upsample_weight)) != 3 or shp(upsample_weight)[0] != shp(upsample_weight)[1]:
+            raise AssertionError(f"upsample_weight must be [C][C][window]; got {shp(upsample_weight)}")
+        Cc, window_u = shp(upsample_weight)[0], shp(upsample_weight)[2]
+        if shp(upsample_bias) != (Cc,) or shp(cond_weight) not in ((lr, Cc), (lr, Cc, 1)) or shp(cond_bias) != (lr,):
+            raise AssertionError(f"need upsample_bias [{Cc}], cond_weight [{lr}][{Cc}] and cond_bias [{lr}]; got {shp(upsample_bias)}, "
+                                 f"{shp(cond_weight)}, {shp(cond_bias)}")
+        if stride < 1 or window_u < stride:
+            raise AssertionError(f"need upsampling window >= stride >= 1; got {window_u}, {stride}")
+        for f in features:
+            if len(shp(f)) != 2 or shp(f)[0] != Cc or shp(f)[1] < 1:
+                raise AssertionError(f"each utterance's frames are [{Cc}][T] with T >= 1; got {shp(f)}")
+        lengths = [shp(f)[1] * stride for f in features]
+        # contiguous fp32 frames, made on the current stream before the side stream is ordered after it
+        features = [f.to(torch.float32).contiguous() if isinstance(f, torch.Tensor) else np.ascontiguousarray(f, np.float32) for f in features]
+        plan = plan_slots(lengths, slots, window)
+        windows = _windows(plan, lengths, window)
+        eng = self._engine(slots, 2 * window, fp16)
+        eng.reset_history()
+        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(lr, Cc), cond_bias, stride)
+
+        cur, side = torch.cuda.current_stream(), torch.cuda.Stream()
+        side.wait_stream(cur)                                         # frames made on the current stream
+        ready, read, produced, keep = {}, {}, [], []
+
+        def produce(k):
+            # window k on the side stream, into the positions of window k - 2: after that window has been generated and read
+            if k >= len(windows):
+                return
+            first, count, starting, live = windows[k]
+            if k - 2 in read:
+                side.wait_event(read.pop(k - 2))
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if timing is not None else None
+            if ev:
+                ev[0].record(side)
+            if starting:
+                keep.append(eng.cond_producer_set_slots([plan[u][0] for u in starting], [features[u] for u in starting],
+                                                        [first] * len(starting), stream=side))
+            if live:
+                eng.cond_producer_run_slots([s for s, _, _, _ in live], first, count, stream=side)
+            if ev:
+                ev[1].record(side)
+                produced.append(ev)
+            ready[k] = torch.cuda.Event()
+            ready[k].record(side)
+
+        def condition(k):
+            cur.wait_event(ready.pop(k))
+
+        def after(k):
+            read[k] = torch.cuda.Event()
+            read[k].record(cur)
+            produce(k + 1)                                            # enqueued after window k's generation, which it overlaps
+
+        produce(0)
+        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, after)
+        torch.cuda.synchronize()
+        if timing is not None:
+            timing["produce_s"] = sum(a.elapsed_time(b) for a, b in produced) / 1e3
+            timing["produce_wait_s"] = sum(e[0].elapsed_time(e[1]) for e in events) / 1e3
+            timing["restart_select_s"] = sum(e[1].elapsed_time(e[2]) for e in events) / 1e3
+            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
+        return outs
+
+    def _serve(self, eng, plan, windows, lengths, seeds, timed, condition, after=None):
+        """The window loop of infer_many and infer_many_from_features on the current stream.  Per window k: condition(k), which
+        leaves the conditioning of the window's live slots in the engine or makes the stream wait for it; the restarts of the
+        slots whose utterance starts there; their selectors; the launch; the outputs; then after(k).  Returns the outputs and, if
+        timed, per window four events around those steps (before condition, restarts, launch, and after the outputs)."""
+        outs = [torch.empty(n, dtype=torch.int32, device="cuda") for n in lengths]
+        stage = torch.empty((eng.B, eng.N), dtype=torch.int32, device="cuda")
+        events = []
+        for k, (first, count, starting, live) in enumerate(windows):
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timed else None
+            if ev:
+                ev[0].record()
+            condition(k)
+            if ev:
+                ev[1].record()
+            if starting:
+                eng.restart_slots([plan[u][0] for u in starting], [seeds[u] for u in starting])
+            eng.set_selectors_random_slots(first, count)
+            if ev:
+                ev[2].record()
+            eng.run_stream(first, count, eng.B)
+            pos = first % eng.N                                       # windows start at multiples of the window: no wrap inside
+            eng.get_yout(stage, pos, count)
+            for s, u, a, m in live:
+                outs[u][a:a + m].copy_(stage[s, pos:pos + m])
+            if ev:
+                ev[3].record()
+                events.append(ev)
+            if after is not None:
+                after(k)
+        return outs, events
 
     def log_likelihood(self, cond_input, audio):
         """Per-sample log-likelihood of `audio` (int mu-law codes [batch][samples]) given `cond_input` (channels x batch x

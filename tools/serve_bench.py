@@ -1,19 +1,26 @@
-"""Serving a queue of utterances of different lengths: continuous batching (NVWaveNet.infer_many) against static batches.
+"""Serving a queue of utterances of different lengths: continuous batching (NVWaveNet.infer_many), continuous batching from mel
+frames (NVWaveNet.infer_many_from_features) and static batches.
 
     python tools/serve_bench.py --out DIR [--utterances 256] [--seed 1]
 
 Workload: the C3 model (fp16, R64 / S256 / A256, 20 layers, max dilation 512, lively seeded weights), 64 slots, windows of
-4 000 samples, and a seeded mix of `utterances` utterances with lengths uniform in [16 000, 160 000] samples, each conditioned on a
-slice of one random conditioning tensor.
+4 000 samples, and a seeded mix of `utterances` utterances of whole frames of 200 samples, uniform in [16 000, 160 000] samples.
+The first and third arms condition each utterance on a slice of one random conditioning tensor; the second on its own random
+mel frames (80 channels) through a seeded conditioning network of the reference's geometry (upsampling window 800, stride 200).
   continuous  infer_many(slots=64, window=4000): a slot takes the next queued utterance at the first window boundary after its
               utterance ends.
+  mel         infer_many_from_features(slots=64, window=4000): the same schedule; each window's conditioning is produced on the
+              device from the frames, on a side stream one window ahead of generation.
   static      batches of 64 in arrival order, each generated up to its longest utterance by the loop of infer(window=4000)
               (per window: conditioning of the whole batch, selectors, run_stream, yOut).  The loop is run here with the window's
               conditioning assembled from the same slices, because infer() wants the batch's whole conditioning tensor at once
               (64 x 160 000 samples x 20 x 128 fp32 = 105 GB).
-Reported: useful samples/s of both (the sum of the lengths over the wall time), the padding fraction of the static batches
-(computed from the lengths), the idle slot fraction of the continuous run, and the GPU time infer_many spends in restarts and
-per-slot uploads.  The card's name, power limit and SM clock come from a read-only nvidia-smi query in the same run.
+Reported: useful samples/s of each arm (the sum of the lengths over the wall time), the padding fraction of the static batches
+(computed from the lengths), the idle slot fraction of the continuous run, the GPU time infer_many spends in restarts and
+per-slot uploads, the mel arm's production time per window and the time generation waited for it (zero when production is
+hidden), and the bytes each arm's queued inputs would take (from shapes: fp32 conditioning [2R][L][n] against frames [80][T]).
+A separate phase then times the production of one window of 64 slots alone, and splits it by kernel (upsampling, projection,
+masking, store conversion) under torch.profiler.  The card's name, power limit and SM clock come from a read-only nvidia-smi query in the same run.
 Writes DIR/serve_bench.json and prints it.
 """
 import argparse
@@ -33,6 +40,7 @@ from tests import refgen  # noqa: E402
 R, S, A, L, MD = 64, 256, 256, 20, 512
 SLOTS, WINDOW = 64, 4000
 LO, HI = 16000, 160000
+MEL, UP_WINDOW, STRIDE = 80, 800, 200
 
 
 def card():
@@ -58,6 +66,52 @@ def network(seed):
                      res_biases=[tt(w["Bres"][l]) for l in range(L - 1)],
                      skip_weights=[tt(cm(w["Wskip"][l], S, R)[:, :, None]) for l in range(L)],
                      skip_biases=[tt(w["Bskip"][l]) for l in range(L)], use_embed_tanh=True)
+
+
+def conditioning_network(seed):
+    """Seeded upsampling ConvTranspose1d(80, 80, 800, stride 200) and 1x1 projection to L * 2R, scaled so that the conditioning
+    has a standard deviation of about 0.5 like the slices of the other arms."""
+    rng = np.random.default_rng(seed + 1)
+    taps = UP_WINDOW // STRIDE
+    return ((rng.standard_normal((MEL, MEL, UP_WINDOW)) / np.sqrt(MEL * taps)).astype(np.float32),
+            (0.1 * rng.standard_normal(MEL)).astype(np.float32),
+            (0.5 * rng.standard_normal((L * 2 * R, MEL)) / np.sqrt(MEL)).astype(np.float32),
+            (0.1 * rng.standard_normal(L * 2 * R)).astype(np.float32))
+
+
+def production_split(net, mels, cnet, reps=5):
+    """Production of one window for all SLOTS slots, without generation: event time per window, then its kernels' device time
+    per window under torch.profiler (a run of its own), grouped as upsampling, projection, masking and store conversion."""
+    eng = net._engine(SLOTS, 2 * WINDOW, True)
+    eng.reset_history()
+    eng.cond_producer_set_weights(*cnet, STRIDE)
+    eng.cond_producer_set_slots(range(SLOTS), mels[:SLOTS], [0] * SLOTS)
+    eng.cond_producer_run_slots(range(SLOTS), 0, WINDOW)               # warm-up
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for k in range(reps):
+        eng.cond_producer_run_slots(range(SLOTS), k * WINDOW, WINDOW)
+    b.record()
+    torch.cuda.synchronize()
+    out = {"ms_per_window": a.elapsed_time(b) / reps}
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for k in range(reps):
+            eng.cond_producer_run_slots(range(SLOTS), k * WINDOW, WINDOW)
+        torch.cuda.synchronize()
+    groups = {"upsample": 0.0, "project": 0.0, "mask": 0.0, "convert": 0.0, "other": 0.0}
+    for item in prof.key_averages():
+        us = getattr(item, "self_device_time_total", None)
+        if us is None:
+            us = item.self_cuda_time_total
+        name = item.key
+        g = ("upsample" if "upsample_slots" in name else "project" if "project" in name else "mask" if "mask_slots" in name
+             else "convert" if "convert_rows" in name or "cond_rows" in name else "other")
+        groups[g] += us / 1e3 / reps
+    out["kernel_ms_per_window"] = groups
+    out["kernels"] = sorted({item.key for item in prof.key_averages()})
+    return out
 
 
 def static_batches(net, conds, seeds):
@@ -98,12 +152,15 @@ def main():
         os.environ.pop(k, None)
 
     rng = np.random.default_rng(args.seed)
-    lengths = [int(v) for v in rng.integers(LO, HI + 1, args.utterances)]
+    frames = [int(v) for v in rng.integers(LO // STRIDE, HI // STRIDE + 1, args.utterances)]
+    lengths = [STRIDE * t for t in frames]
     offsets = [int(v) for v in rng.integers(0, HI + 1, args.utterances)]
     seeds = [int(v) for v in rng.integers(0, 2 ** 62, args.utterances)]
     g = torch.Generator(device="cuda").manual_seed(args.seed)
     base = 0.5 * torch.randn((2 * R, L, 2 * HI + 1), generator=g, device="cuda")
     conds = [base[:, :, o:o + n] for o, n in zip(offsets, lengths)]
+    mels = [torch.randn((MEL, t), generator=g, device="cuda") for t in frames]
+    cnet = conditioning_network(args.seed)
     net = network(args.seed)
     info = card()
 
@@ -115,6 +172,8 @@ def main():
     # warm-up: engine creation, weight upload and first launches of both arms
     net.infer_many([c[:, :, :2 * WINDOW] for c in conds[:SLOTS]], seeds[:SLOTS], slots=SLOTS, window=WINDOW, fp16=True)
     static_batches(net, [c[:, :, :WINDOW] for c in conds[:SLOTS]], seeds[:SLOTS])
+    net.infer_many_from_features([m[:, :2 * WINDOW // STRIDE] for m in mels[:SLOTS]], seeds[:SLOTS], *cnet, STRIDE, slots=SLOTS,
+                                 window=WINDOW, fp16=True)
 
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -123,11 +182,20 @@ def main():
     t_cont = time.perf_counter() - t0
     launch = net._engine(SLOTS, WINDOW, True).launch_info()
 
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    mtiming = {}
+    mel = net.infer_many_from_features(mels, seeds, *cnet, STRIDE, slots=SLOTS, window=WINDOW, fp16=True, timing=mtiming)
+    t_mel = time.perf_counter() - t0
+    windows = (steps + WINDOW - 1) // WINDOW
+
     t0 = time.perf_counter()
     stat = static_batches(net, conds, seeds)
     t_stat = time.perf_counter() - t0
-    del cont, stat
+    del cont, stat, mel
+    split = production_split(net, mels, cnet)
     after = card()
+    cond_bytes = sum(lengths) * 2 * R * L * 4
 
     res = {
         "workload": {"model": "C3", "dtype": "fp16", "slots": SLOTS, "window": WINDOW, "utterances": args.utterances,
@@ -136,8 +204,15 @@ def main():
         "continuous": {"seconds": t_cont, "useful_samples_per_s": useful / t_cont, "steps": steps,
                        "idle_slot_fraction": 1.0 - useful / (SLOTS * steps),
                        "restart_upload_s": timing.get("restart_upload_s"), "generate_s": timing.get("generate_s")},
+        "mel": {"seconds": t_mel, "useful_samples_per_s": useful / t_mel, "windows": windows, **mtiming,
+                "produce_ms_per_window": 1e3 * mtiming["produce_s"] / windows,
+                "produce_wait_ms_per_window": 1e3 * mtiming["produce_wait_s"] / windows,
+                "produce_hidden_fraction": 1.0 - mtiming["produce_wait_s"] / mtiming["produce_s"]},
         "static": {"seconds": t_stat, "useful_samples_per_s": useful / t_stat, "padding_fraction": 1.0 - useful / padded},
         "speedup": t_stat / t_cont,
+        "mel_vs_continuous": t_cont / t_mel,
+        "input_bytes": {"continuous": cond_bytes, "static": cond_bytes, "mel": sum(frames) * MEL * 4},
+        "production_alone": split,
     }
     line = json.dumps(res)
     if args.out:
