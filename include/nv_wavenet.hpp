@@ -188,6 +188,14 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Not in the reference class: score of absolute samples [first_sample, first_sample + count) of audio of any length, continuing
+     * the scoring stream (first_sample = 0 starts one); audio, logp and logits cover this call's samples only.  See nvwn_score_stream. */
+    bool score_stream(const int* audio, long long first_sample, int count, int batch_size, float* logp, float* logits = NULL, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_score_stream(m_engine, audio, first_sample, count, batch_size, logp, logits, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
 
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)

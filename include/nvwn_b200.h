@@ -175,9 +175,21 @@ int nvwn_mulaw_table(int A, float* f32, short* i16_wrap, short* i16_saturate);
  * any destination is on the host, device destinations are filled asynchronously on `stream`.  The generation state (history,
  * yOut, selectors, forced indices, dumps, launch info) is left untouched.  Each output (b, t) depends only on audio[b][0..t],
  * the conditioning and the weights, bit for bit.  NVWN_FP16 engines with A = 256 only (else NVWN_EUNSUPPORTED); an audio value
- * outside [0, A) is NVWN_EINVAL and the message names the first offending (b, t). */
+ * outside [0, A) is NVWN_EINVAL and the message names the first offending (b, t).  Ends the scoring stream below. */
 int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size,
                float* logp, float* logits, void* stream);
+/* Streaming scoring: utterances of any length through an engine of num_samples = N, as nvwn_run_stream does for generation.
+ * Scores absolute samples [first_sample, first_sample + count), 1 <= count <= N; audio and logp are [batch_size][count] and
+ * logits (NULL, or [batch_size][count][A]) covers them too.  Sample t uses the conditioning at store position t mod N: fill a range's
+ * positions before the call.  first_sample = 0 starts a scoring stream from silence; any other first_sample must continue it (the
+ * end of the last call of the stream, with the same batch_size), else NVWN_EINVAL.  Between calls the engine keeps each layer's last
+ * d_l inputs and the last two codes, so the results equal nvwn_score of one engine that holds the whole length, bit for bit.
+ * nvwn_score and every weight change (the weight setters, nvwn_weights_updated) end the stream; generation calls leave it alone, and
+ * it leaves the generation state alone.  A call that fails its checks (bad audio included) leaves the stream as it was.  Memory
+ * kinds, completion, the audio check (the message names t as an absolute sample) and the engine kinds as for nvwn_score; the
+ * calls share scratch with nvwn_score: issue them on one stream, or order them. */
+int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, int count, int batch_size,
+                      float* logp, float* logits, void* stream);
 
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);

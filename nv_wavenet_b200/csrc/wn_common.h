@@ -109,6 +109,7 @@ struct WnScoreChunk {
     const void* image;              // scorer weight image (wn_score_pack)
     const void *embPrev, *embCur;   // fp16 [A][R] (engine blob)
     const int* audio;               // device [Bs][N]
+    const int* codes;               // device [Bs][2]: the codes of steps -2 and -1 of the call (128, 128 at a fresh start)
     const float* lh;                // conditioning of the chunk, fp32 [T][L][Be][2R]
     __half* xh;                     // fp16 layer inputs; layer l at wn_score_xh_offset(l): [d_l * Bs history rows | T * Bs rows][R]
     float* xf;                      // fp32 residual stream [T * Bs][R]
@@ -124,6 +125,8 @@ size_t wn_score_image_bytes(int R, int S, int A, int L);
 cudaError_t wn_score_pack(void* image, const WnParams& p, cudaStream_t stream);
 cudaError_t wn_score_check_audio(const int* audio, size_t n, int A, unsigned long long* first_bad, cudaStream_t stream);
 cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t stream);
+// streaming scoring: codes [Bs][2] <- the codes of steps count-2 and count-1 of a call's audio [Bs][N] (count = 1: the pair shifts by one)
+cudaError_t wn_score_carry_codes(int* codes, const int* audio, int N, int count, int Bs, cudaStream_t stream);
 
 // conversions (wn_convert.cu)
 cudaError_t wn_f32_to_f16(__half* dst, const float* src_dev, size_t n, cudaStream_t stream);

@@ -101,9 +101,13 @@ struct nvwn_engine : WnConfig {
 
     // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
     void* score_image = nullptr;
-    bool score_dirty = true;                 // set wherever image_dirty is: the image is repacked on the next nvwn_score
+    bool score_dirty = true;                 // set with image_dirty (weights_changed): the image is repacked on the next scoring call
     char* score_scratch = nullptr;
     int score_T = 0;                         // time steps per chunk: SCORE_ROWS / B
+    // the open scoring stream (nvwn_score_stream): the absolute sample its next call starts at, -1 if none is open, and its
+    // batch_size; its state is the layer fronts and the codes in score_scratch
+    long long score_next = -1;
+    int score_bs = 0;
 
     float* lut_f = nullptr;                  // mu-law decode tables (nvwn_get_audio): A floats, then 2 x A int16 (wrap / saturate)
     unsigned long long* trace = nullptr;     // debug timeline (nvwn_debug_trace)
@@ -196,6 +200,14 @@ int take_slots(nvwn_engine* e, const char* who, const int* slots, int n, cudaStr
     if (rc != 0) return rc;
     e->slot_rows_used = true;
     return copy_snapshot(e->slot_rows, slots, n, stream);
+}
+
+// The weights changed: both images are repacked before their next use, and an open scoring stream ends (its carried layer inputs
+// were computed with the old weights).
+void weights_changed(nvwn_engine* e)
+{
+    e->image_dirty = e->score_dirty = true;
+    e->score_next = -1;
 }
 
 // dst (TD, device) <- src (fp32, host or device), n elements
@@ -298,7 +310,7 @@ constexpr int SCORE_ROWS = 16384;
 
 // byte offsets of the scoring scratch, for the engine's B and N and a chunk of T steps
 struct ScoreScratch {
-    size_t audio, logp, bad, lh, xh, xf, H, lgt, bytes;
+    size_t audio, logp, bad, codes, lh, xh, xf, H, lgt, bytes;
 };
 ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
 {
@@ -309,6 +321,7 @@ ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
     o.audio = take(B * N * sizeof(int));
     o.logp = take(B * N * sizeof(float));
     o.bad = take(sizeof(unsigned long long));
+    o.codes = take(B * 2 * sizeof(int));
     o.lh = take(Tz * L * B * 2 * R * sizeof(float));
     o.xh = take(wn_score_xh_offset(e->L, e->L, e->maxDil, T, e->B, e->R) * sizeof(__half));
     o.xf = take(Tz * B * R * sizeof(float));
@@ -437,7 +450,7 @@ int nvwn_set_embeddings(nvwn_engine* e, const float* embedPrev, const float* emb
     int rc;
     if ((rc = upload(e, e->blob + e->o_embPrev, embedPrev, (size_t)e->A * e->R))) return rc;
     if ((rc = upload(e, e->blob + e->o_embCur, embedCur, (size_t)e->A * e->R))) return rc;
-    e->image_dirty = e->score_dirty = true;
+    weights_changed(e);
     CK(cudaStreamSynchronize(0));
     return 0;
 }
@@ -456,7 +469,7 @@ int nvwn_set_layer_weights(nvwn_engine* e, int layer, const float* Wprev, const 
     if ((rc = upload(e, e->blob + e->o_Bres + l * R * td, Bres, R))) return rc;
     if ((rc = upload(e, e->blob + e->o_Wskip + l * S * R * td, Wskip, S * R))) return rc;
     if ((rc = upload(e, e->blob + e->o_Bskip + l * S * td, Bskip, S))) return rc;
-    e->image_dirty = e->score_dirty = true;
+    weights_changed(e);
     CK(cudaStreamSynchronize(0));       // sources may be freed by the caller right after return
     return 0;
 }
@@ -470,7 +483,7 @@ int nvwn_set_out_weights(nvwn_engine* e, const float* Wzs, const float* Bzs, con
     if ((rc = upload(e, e->blob + e->o_Bzs, Bzs, A))) return rc;
     if ((rc = upload(e, e->blob + e->o_Wza, Wza, A * A))) return rc;
     if ((rc = upload(e, e->blob + e->o_Bza, Bza, A))) return rc;
-    e->image_dirty = e->score_dirty = true;
+    weights_changed(e);
     CK(cudaStreamSynchronize(0));
     return 0;
 }
@@ -873,7 +886,7 @@ int nvwn_weight_blob(nvwn_engine* e, void** dev_ptr, unsigned long long* bytes)
 int nvwn_weights_updated(nvwn_engine* e)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_weights_updated: NULL engine");
-    e->image_dirty = e->score_dirty = true;
+    weights_changed(e);
     return 0;
 }
 
@@ -999,15 +1012,29 @@ int nvwn_get_audio(nvwn_engine* e, float* audio_f32, short* audio_i16, int offse
     return 0;
 }
 
-int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size, float* logp, float* logits, void* stream_)
+}  // extern "C"
+
+namespace {
+
+// The checks nvwn_score and nvwn_score_stream share, in their order: arguments, engine kind, batch_size.
+int score_args(const nvwn_engine* e, const char* who, const int* audio, int batch_size, const float* logp)
 {
-    if (!e || !audio || !logp) return fail(NVWN_EINVAL, "nvwn_score: NULL engine, audio or logp");
-    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, "nvwn_score: only NVWN_FP16 engines can score");
-    if (e->A != 256) return fail(NVWN_EUNSUPPORTED, "nvwn_score: scoring needs A = 256");
-    if (batch_size < 1 || batch_size > e->B) return fail(NVWN_EINVAL, "nvwn_score: batch_size outside [1, B]");
-    if (num_samples < 1 || num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_score: num_samples outside [1, N]");
-    cudaStream_t st = (cudaStream_t)stream_;
-    const int Bs = batch_size, N = num_samples, L = e->L, R = e->R, A = e->A;
+    if (!e || !audio || !logp) return fail(NVWN_EINVAL, std::string(who) + ": NULL engine, audio or logp");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, std::string(who) + ": only NVWN_FP16 engines can score");
+    if (e->A != 256) return fail(NVWN_EUNSUPPORTED, std::string(who) + ": scoring needs A = 256");
+    if (batch_size < 1 || batch_size > e->B) return fail(NVWN_EINVAL, std::string(who) + ": batch_size outside [1, B]");
+    return 0;
+}
+
+// The chunk loop of both scoring calls: absolute samples [first, first + count) of the first Bs utterances, 1 <= count <= N, sample t
+// with the conditioning at store position t mod N; audio, logp and logits hold [Bs][count] (host or device).  first == 0 starts
+// afresh (x_l[t - d] = 0 for t < d, codes 128 / 128); any other first continues from the layer fronts and codes the last call left.
+// keep leaves the call's own fronts and codes there and opens the stream at first + count; otherwise the stream ends.  The caller has
+// checked the arguments; the audio is checked here, before any state changes.
+int score_range(nvwn_engine* e, const char* who, const int* audio, long long first, int count, int Bs, float* logp, float* logits, bool keep,
+                cudaStream_t st)
+{
+    const int N = count, L = e->L, R = e->R, A = e->A;
     if (!e->score_scratch) {
         int T = SCORE_ROWS / e->B;
         if (T < 1) T = 1;
@@ -1023,6 +1050,7 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
     const ScoreScratch o = score_scratch_layout(e, T);
     char* sc = e->score_scratch;
     int* d_audio = reinterpret_cast<int*>(sc + o.audio);
+    int* d_codes = reinterpret_cast<int*>(sc + o.codes);
     unsigned long long* d_bad = reinterpret_cast<unsigned long long*>(sc + o.bad);
     __half* xh = reinterpret_cast<__half*>(sc + o.xh);
 
@@ -1037,9 +1065,10 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
     if (bad != ~0ull) {
         int v = 0;
         CK(cudaMemcpy(&v, d_audio + bad, sizeof v, cudaMemcpyDeviceToHost));
-        return fail(NVWN_EINVAL, "nvwn_score: audio[" + std::to_string(bad / N) + "][" + std::to_string(bad % N) + "] = " + std::to_string(v) +
-                                     " is outside [0, " + std::to_string(A) + ")");
+        return fail(NVWN_EINVAL, std::string(who) + ": audio[" + std::to_string(bad / N) + "][" + std::to_string(first + (long long)(bad % N)) + "] = " +
+                                     std::to_string(v) + " is outside [0, " + std::to_string(A) + ")");
     }
+    e->score_next = -1;                      // reopened below once this call's state is complete
     if (e->score_dirty) {
         WnParams p;
         fill_params(e, p, 0, 0, 0, N, Bs, 0);
@@ -1047,15 +1076,20 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
         e->score_dirty = false;
     }
     const bool logp_dev = is_device_ptr(logp), logits_dev = logits && is_device_ptr(logits);
-    for (int l = 0; l < L; l++)              // x_l[t - d] = 0 for t < d
-        CK(cudaMemsetAsync(xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R), 0,
-                           (size_t)wn_score_dilation(l, e->maxDil) * Bs * R * sizeof(__half), st));
+    if (first == 0) {
+        for (int l = 0; l < L; l++)          // x_l[t - d] = 0 for t < d
+            CK(cudaMemsetAsync(xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R), 0,
+                               (size_t)wn_score_dilation(l, e->maxDil) * Bs * R * sizeof(__half), st));
+        CK(wn_fill_int(d_codes, 128, (size_t)Bs * 2, st));
+    }
     WnScoreChunk c;
     c.L = L; c.R = R; c.S = e->S; c.A = A; c.maxDil = e->maxDil; c.tanhEmbed = e->tanhEmbed;
     c.Bs = Bs; c.Be = e->B; c.N = N; c.Tcap = T;
     c.image = e->score_image; c.embPrev = e->blob + e->o_embPrev; c.embCur = e->blob + e->o_embCur;
     c.audio = d_audio;
-    c.lh = reinterpret_cast<const float*>(sc + o.lh);
+    c.codes = d_codes;
+    float* lh = reinterpret_cast<float*>(sc + o.lh);
+    c.lh = lh;
     c.xh = xh;
     c.xf = reinterpret_cast<float*>(sc + o.xf);
     c.H = reinterpret_cast<__half*>(sc + o.H);
@@ -1063,7 +1097,10 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
     float* lgt = reinterpret_cast<float*>(sc + o.lgt);
     for (int t0 = 0; t0 < N; t0 += T) {
         const int Tc = N - t0 < T ? N - t0 : T;
-        CK(e->family->readback(*e, reinterpret_cast<float*>(sc + o.lh), e->Lh, t0, Tc, st));
+        // the chunk's conditioning, in two pieces where its samples wrap around the store
+        const int pos = (int)((first + t0) % e->N), head = Tc < e->N - pos ? Tc : e->N - pos;
+        CK(e->family->readback(*e, lh, e->Lh, pos, head, st));
+        if (head < Tc) CK(e->family->readback(*e, lh + (size_t)head * L * e->B * 2 * R, e->Lh, 0, Tc - head, st));
         c.t0 = t0; c.T = Tc;
         c.logits = logits ? (logits_dev ? logits : lgt) : nullptr;
         c.logits_ld = logits_dev ? (long long)N * A : (long long)Tc * A;
@@ -1072,8 +1109,9 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
         if (logits && !logits_dev)
             CK(cudaMemcpy2DAsync(logits + (size_t)t0 * A, (size_t)N * A * sizeof(float), lgt, (size_t)Tc * A * sizeof(float),
                                  (size_t)Tc * A * sizeof(float), Bs, cudaMemcpyDeviceToHost, st));
-        if (t0 + Tc < N) {
-            // carry the last d_l steps of every layer's input to the front of its buffer, in pieces that do not overlap
+        if (t0 + Tc < N || keep) {
+            // carry the last d_l steps of every layer's input to the front of its buffer, in pieces that do not overlap; after the
+            // last chunk these are the fronts of the stream's next call
             const size_t piece = (size_t)Tc * Bs;
             for (int l = 0; l < L; l++) {
                 __half* buf = xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R);
@@ -1085,9 +1123,48 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
             }
         }
     }
+    if (keep) {
+        CK(wn_score_carry_codes(d_codes, d_audio, N, N, Bs, st));
+        e->score_next = first + N;
+        e->score_bs = Bs;
+    }
     if (!logp_dev) CK(cudaMemcpyAsync(logp, c.logp, n_audio * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (!logp_dev || (logits && !logits_dev)) CK(cudaStreamSynchronize(st));
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size, float* logp, float* logits, void* stream)
+{
+    int rc = score_args(e, "nvwn_score", audio, batch_size, logp);
+    if (rc != 0) return rc;
+    if (num_samples < 1 || num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_score: num_samples outside [1, N]");
+    return score_range(e, "nvwn_score", audio, 0, num_samples, batch_size, logp, logits, false, (cudaStream_t)stream);
+}
+
+int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, int count, int batch_size, float* logp, float* logits, void* stream)
+{
+    const std::string who = "nvwn_score_stream";
+    int rc = score_args(e, who.c_str(), audio, batch_size, logp);
+    if (rc != 0) return rc;
+    if (count < 1 || count > e->N)
+        return fail(NVWN_EINVAL, who + ": count " + std::to_string(count) + " is outside [1, " + std::to_string(e->N) + "] (num_samples of the engine)");
+    if (first_sample < 0) return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " < 0");
+    if (first_sample != 0) {
+        if (e->score_next < 0)
+            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " continues no scoring stream (nvwn_score and weight "
+                                           "changes end one): start one at first_sample = 0");
+        if (first_sample != e->score_next)
+            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " does not continue the scoring stream: the next sample is " +
+                                         std::to_string(e->score_next) + " (first_sample = 0 starts over)");
+        if (batch_size != e->score_bs)
+            return fail(NVWN_EINVAL, who + ": batch_size " + std::to_string(batch_size) + " differs from the scoring stream's batch_size " +
+                                         std::to_string(e->score_bs) + " (first_sample = 0 starts over)");
+    }
+    return score_range(e, who.c_str(), audio, first_sample, count, batch_size, logp, logits, true, (cudaStream_t)stream);
 }
 
 // debug only (not part of the public ABI): the engine's conditioning store for samples [first_sample, first_sample + num_samples),

@@ -11,9 +11,10 @@
 //           Zs = relu(skip . Wzs^T + Bzs);  Za = Zs . Wza^T + Bza;  logp = Za[a[t]] - logsumexp(Za)      (one launch)
 //
 // Each layer's fp16 input buffer carries the last d_l steps of the previous chunk in front of the chunk, so x_l[t-d] is the
-// same buffer d_l * Bs rows earlier.  Tensor cores through mma.sync.m16n8k16 (fp16 in, fp32 accumulate) from XOR-swizzled
-// shared-memory tiles loaded with cp.async; every output element accumulates its K in one fixed order in one CTA (no
-// split-K, no atomics), so a row's result does not depend on which tile, chunk or batch it is computed in.
+// same buffer d_l * Bs rows earlier.  A scoring stream (nvwn_score_stream) keeps those fronts and the last two codes between
+// calls, so the first chunk of a call continues the previous call's last one.  Tensor cores through mma.sync.m16n8k16 (fp16 in,
+// fp32 accumulate) from XOR-swizzled shared-memory tiles loaded with cp.async; every output element accumulates its K in one
+// fixed order in one CTA (no split-K, no atomics), so a row's result does not depend on which tile, chunk or batch it is computed in.
 #include "wn_common.h"
 #include "wn_math.cuh"
 
@@ -83,6 +84,17 @@ __global__ void pack_bias_kernel(float* __restrict__ Bh, float* __restrict__ Br,
     for (int a = tid; a < A; a += nt) { Bzs[a] = __half2float(bzs[a]); Bza[a] = __half2float(bza[a]); }
 }
 
+// the codes of the next call's steps -2 and -1: the last two of this call's `count` codes (row stride N); with count = 1 the
+// pair shifts by one
+__global__ void carry_codes_kernel(int* __restrict__ codes, const int* __restrict__ audio, int N, int count, int Bs)
+{
+    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < Bs; b += gridDim.x * blockDim.x) {
+        const int prev = count >= 2 ? audio[(size_t)b * N + count - 2] : codes[2 * b + 1];
+        codes[2 * b] = prev;
+        codes[2 * b + 1] = audio[(size_t)b * N + count - 1];
+    }
+}
+
 __global__ void check_audio_kernel(const int* __restrict__ audio, size_t n, int A, unsigned long long* first_bad)
 {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -130,14 +142,15 @@ __device__ __forceinline__ void load_b2(uint32_t (&b)[4], uint32_t base, int nch
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(addr), "r"(v)); }
 __device__ __forceinline__ uint32_t u32(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 
-// ---- embedding: x_0 of every row of the chunk ----
-__global__ void score_embed_kernel(const __half* __restrict__ embPrev, const __half* __restrict__ embCur, const int* __restrict__ audio, int N, int t0,
-                                   int M, int Bs, int R, int tanhEmbed, float* __restrict__ xf, __half* __restrict__ x0)
+// ---- embedding: x_0 of every row of the chunk; the codes of call steps -2 and -1 come from codes[b][0..1] ----
+__global__ void score_embed_kernel(const __half* __restrict__ embPrev, const __half* __restrict__ embCur, const int* __restrict__ audio,
+                                   const int* __restrict__ codes, int N, int t0, int M, int Bs, int R, int tanhEmbed, float* __restrict__ xf,
+                                   __half* __restrict__ x0)
 {
     const size_t n_all = (size_t)M * R;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (size_t)gridDim.x * blockDim.x) {
         const int m = (int)(i / R), r = (int)(i % R), b = m % Bs, t = t0 + m / Bs;
-        const int yp = t >= 2 ? audio[(size_t)b * N + t - 2] : 128, yc = t >= 1 ? audio[(size_t)b * N + t - 1] : 128;
+        const int yp = t >= 2 ? audio[(size_t)b * N + t - 2] : codes[2 * b + t], yc = t >= 1 ? audio[(size_t)b * N + t - 1] : codes[2 * b + 1];
         float v = __half2float(embPrev[(size_t)yp * R + r]) + __half2float(embCur[(size_t)yc * R + r]);
         if (tanhEmbed) v = wn::tanhf_fast(v);         // as the latency kernel (wn_lat_kernel.cu)
         xf[i] = v;
@@ -517,6 +530,12 @@ cudaError_t wn_score_check_audio(const int* audio, size_t n, int A, unsigned lon
     return cudaGetLastError();
 }
 
+cudaError_t wn_score_carry_codes(int* codes, const int* audio, int N, int count, int Bs, cudaStream_t st)
+{
+    carry_codes_kernel<<<(Bs + 255) / 256, 256, 0, st>>>(codes, audio, N, count, Bs);
+    return cudaGetLastError();
+}
+
 cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
 {
     if (c.A != A_OUT || (c.S != 128 && c.S != 256) || (c.R != 32 && c.R != 64 && c.R != 128)) return cudaErrorInvalidValue;
@@ -529,8 +548,8 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
         size_t blocks = (n + 255) / 256;
         if (blocks > 132 * 16) blocks = 132 * 16;
         __half* x0 = c.xh + (size_t)wn_score_dilation(0, c.maxDil) * c.Bs * R;
-        score_embed_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const __half*>(c.embPrev), static_cast<const __half*>(c.embCur), c.audio, c.N,
-                                                            c.t0, M, c.Bs, R, c.tanhEmbed, c.xf, x0);
+        score_embed_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const __half*>(c.embPrev), static_cast<const __half*>(c.embCur), c.audio,
+                                                            c.codes, c.N, c.t0, M, c.Bs, R, c.tanhEmbed, c.xf, x0);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     for (int l = 0; l < c.L; l++) {

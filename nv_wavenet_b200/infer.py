@@ -337,6 +337,20 @@ class NVWavenetInfer:
         audio[b][0..t) fed back and the conditioning already in the engine.  `audio`: int [batch][samples] numpy array
         (numpy results) or CUDA tensor (CUDA tensors, filled asynchronously on `stream`).  Returns logp [batch_size][num_samples],
         or (logp, logits [batch_size][num_samples][A]) with logits=True.  The generation state is left untouched."""
+        return self._score(audio, num_samples, batch_size, logits, "score",
+                           lambda a, n, bs, lp, lg: self._l.nvwn_score(self._h, a, n, bs, lp, lg, _stream(stream)))
+
+    def score_stream(self, audio, first_sample, num_samples=None, batch_size=None, logits=False, stream=None):
+        """Scoring of audio of any length through this engine, a window at a time: the log-likelihood of absolute samples
+        [first_sample, first_sample + num_samples), num_samples <= N, continuing the scoring stream (first_sample 0 starts one).
+        `audio` holds this call's samples only, [batch][num_samples], and sample t uses the conditioning at position t mod N.
+        Arrays and results as for score().  Over the windows the results equal score() of one engine of the whole length."""
+        return self._score(audio, num_samples, batch_size, logits, "score_stream",
+                           lambda a, n, bs, lp, lg: self._l.nvwn_score_stream(self._h, a, first_sample, n, bs, lp, lg, _stream(stream)))
+
+    def _score(self, audio, num_samples, batch_size, logits, what, call):
+        """audio[:batch_size, :num_samples] as int32 and the outputs of score() in matching memory; call(audio, n, bs, logp, logits)
+        with their pointers."""
         n = audio.shape[1] if num_samples is None else num_samples
         bs = audio.shape[0] if batch_size is None else batch_size
         if hasattr(audio, "is_cuda") and audio.is_cuda:
@@ -350,8 +364,7 @@ class NVWavenetInfer:
             lp = np.empty((bs, n), np.float32)
             lg = np.empty((bs, n, self.A), np.float32) if logits else None
             ptrs = (a.ctypes.data, lp.ctypes.data, lg.ctypes.data if logits else None)
-        check(self._l.nvwn_score(self._h, C.c_void_p(ptrs[0]), n, bs, C.c_void_p(ptrs[1]),
-                                 None if ptrs[2] is None else C.c_void_p(ptrs[2]), _stream(stream)), "score")
+        check(call(C.c_void_p(ptrs[0]), n, bs, C.c_void_p(ptrs[1]), None if ptrs[2] is None else C.c_void_p(ptrs[2])), what)
         return (lp, lg) if logits else lp
 
     # ---- run (nv_wavenet.cuh:445-639) ----

@@ -246,15 +246,7 @@ class NVWaveNet:
         shp = lambda a: tuple(int(v) for v in a.shape)
         if len(features) != len(seeds):
             raise AssertionError(f"{len(features)} utterances but {len(seeds)} seeds")
-        lr = self.num_layers * 2 * self.R
-        if len(shp(upsample_weight)) != 3 or shp(upsample_weight)[0] != shp(upsample_weight)[1]:
-            raise AssertionError(f"upsample_weight must be [C][C][window]; got {shp(upsample_weight)}")
-        Cc, window_u = shp(upsample_weight)[0], shp(upsample_weight)[2]
-        if shp(upsample_bias) != (Cc,) or shp(cond_weight) not in ((lr, Cc), (lr, Cc, 1)) or shp(cond_bias) != (lr,):
-            raise AssertionError(f"need upsample_bias [{Cc}], cond_weight [{lr}][{Cc}] and cond_bias [{lr}]; got {shp(upsample_bias)}, "
-                                 f"{shp(cond_weight)}, {shp(cond_bias)}")
-        if stride < 1 or window_u < stride:
-            raise AssertionError(f"need upsampling window >= stride >= 1; got {window_u}, {stride}")
+        Cc, lr = self._cond_network(upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
         for f in features:
             if len(shp(f)) != 2 or shp(f)[0] != Cc or shp(f)[1] < 1:
                 raise AssertionError(f"each utterance's frames are [{Cc}][T] with T >= 1; got {shp(f)}")
@@ -310,6 +302,21 @@ class NVWaveNet:
             timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
         return outs
 
+    def _cond_network(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride):
+        """Checks the shapes of a conditioning network (upsample_weight [C][C][window], upsample_bias [C], cond_weight [L*2R][C] or
+        [L*2R][C][1], cond_bias [L*2R]) and its stride (window >= stride >= 1).  Returns (C, L*2R)."""
+        shp = lambda a: tuple(int(v) for v in a.shape)
+        lr = self.num_layers * 2 * self.R
+        if len(shp(upsample_weight)) != 3 or shp(upsample_weight)[0] != shp(upsample_weight)[1]:
+            raise AssertionError(f"upsample_weight must be [C][C][window]; got {shp(upsample_weight)}")
+        Cc, window_u = shp(upsample_weight)[0], shp(upsample_weight)[2]
+        if shp(upsample_bias) != (Cc,) or shp(cond_weight) not in ((lr, Cc), (lr, Cc, 1)) or shp(cond_bias) != (lr,):
+            raise AssertionError(f"need upsample_bias [{Cc}], cond_weight [{lr}][{Cc}] and cond_bias [{lr}]; got {shp(upsample_bias)}, "
+                                 f"{shp(cond_weight)}, {shp(cond_bias)}")
+        if stride < 1 or window_u < stride:
+            raise AssertionError(f"need upsampling window >= stride >= 1; got {window_u}, {stride}")
+        return Cc, lr
+
     def _serve(self, eng, plan, windows, lengths, seeds, timed, condition, after=None):
         """The window loop of infer_many and infer_many_from_features on the current stream.  Per window k: condition(k), which
         leaves the conditioning of the window's live slots in the engine or makes the stream wait for it; the restarts of the
@@ -342,17 +349,85 @@ class NVWaveNet:
                 after(k)
         return outs, events
 
-    def log_likelihood(self, cond_input, audio):
+    def log_likelihood(self, cond_input, audio, window=None):
         """Per-sample log-likelihood of `audio` (int mu-law codes [batch][samples]) given `cond_input` (channels x batch x
         num_layers x samples, as for infer()): log p(audio[b][t] | audio[b][0..t), conditioning) under the fp16 engine of that
-        size, all steps at once.  Returns a float32 CUDA tensor [batch][samples]."""
+        size, all steps at once.  Returns a float32 CUDA tensor [batch][samples].
+        window=W scores through one fp16 engine of W samples per batch size, whatever the length, a window at a time
+        (nvwn_score_stream): the engine holds W samples of conditioning instead of all of them, and the result is the same as
+        without a window, bit for bit."""
         if (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
             raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
         batch_size, sample_count = cond_input.size(1), cond_input.size(3)
         if tuple(audio.size()) != (batch_size, sample_count):
             raise AssertionError(f"audio must be [batch][samples] = {(batch_size, sample_count)}; got {tuple(audio.size())}")
-        eng = self._engine(batch_size, sample_count, True)
-        eng.set_conditioning(column_major(cond_input).float(), 0, sample_count)
-        logp = eng.score(audio.to(device="cuda", dtype=torch.int32))
+        if window is not None and window < 1:
+            raise AssertionError(f"window must be at least 1; got {window}")
+        audio = audio.to(device="cuda", dtype=torch.int32)
+        if window is None:
+            eng = self._engine(batch_size, sample_count, True)
+            eng.set_conditioning(column_major(cond_input).float(), 0, sample_count)
+            logp = eng.score(audio)
+        else:
+            eng = self._engine(batch_size, window, True)
+            logp = torch.empty((batch_size, sample_count), dtype=torch.float32, device="cuda")
+            # windows start at multiples of W, so each one fills the store from position 0
+            for first in range(0, sample_count, window):
+                n = min(window, sample_count - first)
+                eng.set_conditioning(column_major(cond_input[..., first:first + n]).float(), 0, n)
+                logp[:, first:first + n] = eng.score_stream(audio[:, first:first + n], first)
         torch.cuda.synchronize()
+        return logp
+
+    def log_likelihood_from_features(self, features, audio, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, window=None,
+                                     timing=None):
+        """log_likelihood with the conditioning made on the device from mel frames: features [batch][C][T], audio int mu-law codes
+        [batch][T * stride], and the conditioning network of set_conditioning_from_features (upsample_weight [C][C][w],
+        upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]); numpy arrays or torch tensors.  Returns a
+        float32 CUDA tensor [batch][T * stride], equal bit for bit to log_likelihood of the conditioning the producer's arithmetic
+        gives (nvwn_cond_from_features_host).
+        window=None fills one engine of the whole length; window=W uses one engine of W samples, producing each window's
+        conditioning from the frames just before scoring it, so neither the expanded conditioning nor a store of the whole length
+        ever exists.  timing: a dict, or None; if given, receives the GPU seconds of production ("produce_s") and of scoring
+        ("score_s")."""
+        shp = lambda a: tuple(int(v) for v in a.shape)
+        Cc, lr = self._cond_network(upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
+        if len(shp(features)) != 3 or shp(features)[1] != Cc or shp(features)[2] < 1:
+            raise AssertionError(f"features must be [batch][{Cc}][T] with T >= 1; got {shp(features)}")
+        batch_size, sample_count = shp(features)[0], shp(features)[2] * stride
+        if shp(audio) != (batch_size, sample_count):
+            raise AssertionError(f"audio must be [batch][T * stride] = {(batch_size, sample_count)}; got {shp(audio)}")
+        if window is not None and window < 1:
+            raise AssertionError(f"window must be at least 1; got {window}")
+        audio = torch.as_tensor(audio).to(device="cuda", dtype=torch.int32)
+        net = (upsample_weight, upsample_bias, cond_weight.reshape(lr, Cc), cond_bias, stride)
+        events = []
+
+        def mark():
+            if timing is not None:
+                events.append(torch.cuda.Event(enable_timing=True))
+                events[-1].record()
+
+        if window is None:
+            eng = self._engine(batch_size, sample_count, True)
+            mark()
+            eng.set_conditioning_from_features(features, *net)
+            mark()
+            logp = eng.score(audio)
+            mark()
+        else:
+            eng = self._engine(batch_size, window, True)
+            eng.cond_producer_load(features, *net)
+            logp = torch.empty((batch_size, sample_count), dtype=torch.float32, device="cuda")
+            for first in range(0, sample_count, window):
+                n = min(window, sample_count - first)
+                mark()
+                eng.cond_producer_run_stream(first, n)
+                mark()
+                logp[:, first:first + n] = eng.score_stream(audio[:, first:first + n], first)
+                mark()
+        torch.cuda.synchronize()
+        if timing is not None:
+            timing["produce_s"] = sum(events[i].elapsed_time(events[i + 1]) for i in range(0, len(events), 3)) / 1e3
+            timing["score_s"] = sum(events[i + 1].elapsed_time(events[i + 2]) for i in range(0, len(events), 3)) / 1e3
         return logp
