@@ -196,6 +196,14 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Not in the reference class: after score_stream over a prompt [0, P), generation continues it from sample P (run_stream of
+     * the scoring stream's batch_size).  See nvwn_prime_from_score. */
+    bool prime_from_score(cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_prime_from_score(m_engine, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
 
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)

@@ -190,6 +190,20 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
  * calls share scratch with nvwn_score: issue them on one stream, or order them. */
 int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, int count, int batch_size,
                       float* logp, float* logits, void* stream);
+/* Prompted generation: continue given audio.  Score the prompt, samples [0, P), with nvwn_score_stream (any windows), then this call
+ * moves the open scoring stream's state into generation: for its batch_size Bs utterances, each layer's last d_l inputs go into the
+ * history ring and the last two codes become the fed-back indices, and the engine's next sample becomes P.  Then
+ * nvwn_run_stream(e, P, count, Bs, ...) generates the continuation; with nvwn_set_selectors_random_stream it draws at sample t what
+ * any engine draws at t.  The scoring stream stays open and unchanged; nothing else changes (selectors, conditioning, forced indices,
+ * per-slot state, dumps, launch info).  Stream-ordered on `stream`: issue it on the scoring calls' stream, or order them.
+ * Needs an open scoring stream with P >= 1 (nvwn_score and weight changes end one), else NVWN_EINVAL; NVWN_FP16 engines only (else
+ * NVWN_EUNSUPPORTED).  The tensor-core path, and any engine after a per-slot call, need Bs = B.  After a prime, and until
+ * nvwn_reset_history, runs need batch_size = Bs (NVWN_EINVAL otherwise).  A refused call changes nothing.
+ * Numerics: the primed history holds the scorer's fp16 layer inputs, whose GEMMs sum in another order than any generation kernel's,
+ * so the continuation is not bit-identical to forced generation of the prompt.  It is bit-identical whatever the windows of the
+ * scoring and generation calls, the primed history is the same on every engine kind, and it is within the fp16 contract of the
+ * fp32 model at that history. */
+int nvwn_prime_from_score(nvwn_engine* e, void* stream);
 
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);

@@ -80,6 +80,12 @@ struct WnFamily {
     cudaError_t (*clear_rows)(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream);
     cudaError_t (*convert_rows)(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
                                 cudaStream_t stream);
+    // History writers (priming from a scoring stream, DESIGN.md §5.4).  put_history writes fp16 src [n][batch][R] (device), the
+    // values x_layer[t] of absolute times [t_first, t_first + n), n <= maxDil + 1, rows 0..batch-1, into ring slot t mod (maxDil+1)
+    // of that layer, where a run of batch_size = batch reads them, and no other byte; get_history (debug) reads the whole ring back
+    // as fp32 [(maxDil+1)][L][batch][R] (device), slot by slot, at that stride.
+    cudaError_t (*put_history)(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream);
+    cudaError_t (*get_history)(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream);
     cudaError_t (*pack)(void* image, const WnParams& p, cudaStream_t stream);      // weight blob -> image; NULL: the kernels read the blob
     cudaError_t (*launch)(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info);
     bool whole_batch;                               // a run must take all c.B utterances
@@ -100,6 +106,8 @@ cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* sto
 cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream);
 cudaError_t wn_plain_convert_rows(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
                                   cudaStream_t stream);
+cudaError_t wn_plain_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream);
+cudaError_t wn_plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream);
 
 // teacher-forced scoring (wn_score_kernel.cu, DESIGN.md §5.4): one time chunk of T steps x Bs utterances, rows m = (t - t0) * Bs + b
 struct WnScoreChunk {
@@ -139,6 +147,9 @@ cudaError_t wn_fill_selectors_slots(float* dst, int n, int B, long long first_t,
 // restart of rows rows[0..n): yPrev = yCur = 128, origin = t0, seed = seeds[i] (seeds NULL: 0)
 cudaError_t wn_restart_rows(const int* rows, int n, const unsigned long long* seeds, long long t0, int* yPrev, int* yCur, long long* origin,
                             unsigned long long* seed, cudaStream_t stream);
+// fed-back indices of rows b < n from a scoring stream's codes [n][2] (the codes of steps t-2 and t-1 of its next sample t):
+// yPrev[b] = codes[b][0], yCur[b] = codes[b][1]
+cudaError_t wn_feedback_from_codes(const int* codes, int n, int* yPrev, int* yCur, cudaStream_t stream);
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream);
 

@@ -160,8 +160,14 @@ cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* sto
     return cudaMemcpyAsync(dst_dev, static_cast<const float*>(store) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
 }
 
-// ring row (entry e = slot * L + layer, utterance rows[i]) = R elements of TD, zeroed as 16-byte words (R * sizeof(TD) >= 64)
-__global__ void plain_clear_rows_kernel(uint4* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int B, int words)
+// 16-byte word k of the history-ring row (entry e = slot * L + layer, utterance b) of a run of `batch` utterances: rows of
+// `words` 16-byte words (R elements of TD, R * sizeof(TD) >= 64), entry-major at the run's batch stride
+__device__ __forceinline__ uint4* plain_ring_word(void* ring, size_t e, int batch, int b, int words, int k)
+{
+    return static_cast<uint4*>(ring) + (e * batch + b) * words + k;
+}
+// rows rows[i] zeroed in every entry, at the engine's batch stride B
+__global__ void plain_clear_rows_kernel(void* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int B, int words)
 {
     const size_t total = (size_t)entries * n * words;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -169,7 +175,7 @@ __global__ void plain_clear_rows_kernel(uint4* __restrict__ ring, const int* __r
         const size_t ei = i / words;                              // e * n + i
         const int r = (int)(ei % n);
         const size_t e = ei / n;
-        ring[(e * B + rows[r]) * words + k] = make_uint4(0, 0, 0, 0);
+        *plain_ring_word(ring, e, B, rows[r], words, k) = make_uint4(0, 0, 0, 0);
     }
 }
 cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
@@ -179,7 +185,57 @@ cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_d
     const size_t total = (size_t)(c.maxDil + 1) * c.L * n * words;
     size_t blocks = (total + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    plain_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<uint4*>(ring), rows_dev, n, (c.maxDil + 1) * c.L, c.B, words);
+    plain_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(ring, rows_dev, n, (c.maxDil + 1) * c.L, c.B, words);
+    return cudaGetLastError();
+}
+
+// fp16 src [n][batch][R] (16-byte words, `words` per row) -> rows 0..batch-1 of entries (t mod slots) * L + layer, t = t_first + j
+__global__ void plain_put_history_kernel(void* __restrict__ ring, const uint4* __restrict__ src, int layer, int L, int slots, long long t_first,
+                                         int n, int batch, int words)
+{
+    const size_t total = (size_t)n * batch * words;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int k = (int)(i % words);
+        const size_t row = i / words;                             // j * batch + b
+        const int b = (int)(row % batch);
+        const long long t = t_first + (long long)(row / batch);
+        *plain_ring_word(ring, (size_t)(t % slots) * L + layer, batch, b, words, k) = src[i];
+    }
+}
+cudaError_t wn_plain_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
+{
+    const int words = c.R * (int)sizeof(__half) / 16;
+    const size_t total = (size_t)n * batch * words;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    plain_put_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(ring, reinterpret_cast<const uint4*>(src), layer, c.L, c.maxDil + 1, t_first, n,
+                                                                   batch, words);
+    return cudaGetLastError();
+}
+
+// at the run's batch stride the plain ring already is [(maxDil+1)][L][batch][R]: a conversion of its first elements
+cudaError_t wn_plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
+{
+    const size_t n = (size_t)(c.maxDil + 1) * c.L * batch * c.R;
+    if (c.dtype == NVWN_FP16) return wn_f16_to_f32(dst, static_cast<const __half*>(ring), n, stream);
+    return cudaMemcpyAsync(dst, ring, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
+}
+
+// fed-back indices from the codes of a scoring stream: step t embeds (y[t-2], y[t-1]) = (yPrev, yCur) in generation and
+// (codes[b][0], codes[b][1]) at the first step of the scorer's next call
+__global__ void feedback_from_codes_kernel(const int* __restrict__ codes, int n, int* yPrev, int* yCur)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < n) {
+        yPrev[b] = codes[2 * b];
+        yCur[b] = codes[2 * b + 1];
+    }
+}
+cudaError_t wn_feedback_from_codes(const int* codes, int n, int* yPrev, int* yCur, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    feedback_from_codes_kernel<<<(n + 255) / 256, 256, 0, stream>>>(codes, n, yPrev, yCur);
     return cudaGetLastError();
 }
 

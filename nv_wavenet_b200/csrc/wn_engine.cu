@@ -78,6 +78,9 @@ struct nvwn_engine : WnConfig {
     // a per-slot call since the last nvwn_reset_history: its rows (history, conditioning, selectors) sit at the engine's batch
     // stride, which the kernels read at the run's, so until the next reset a run must take the whole batch
     bool slot_rows_used = false;
+    // the batch_size of the last nvwn_prime_from_score since the last nvwn_reset_history, 0 if none: the plain history ring was
+    // written at that stride, so until the next reset a run must take that batch
+    int prime_bs = 0;
 
     void* image = nullptr;                   // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
@@ -294,6 +297,9 @@ int launch_steps(nvwn_engine* e, const char* who, int pos, long long t_abs, int 
             return fail(NVWN_EINVAL, std::string(who) + ": after a per-slot call (nvwn_restart_slots, nvwn_set_conditioning_slots, "
                                      "nvwn_set_selectors_random_slots) runs need batch_size equal to the engine's batch size (" +
                                      std::to_string(e->B) + ") until nvwn_reset_history");
+        if (e->prime_bs && batch != e->prime_bs)
+            return fail(NVWN_EINVAL, std::string(who) + ": after nvwn_prime_from_score runs need batch_size equal to the primed batch_size (" +
+                                     std::to_string(e->prime_bs) + ") until nvwn_reset_history; got " + std::to_string(batch));
         if (e->family->pack && e->image_dirty) {
             CK(e->family->pack(e->image, p, stream));
             e->image_dirty = false;
@@ -733,6 +739,7 @@ int nvwn_reset_history(nvwn_engine* e)
     CK(cudaMemsetAsync(e->seed, 0, (size_t)e->B * sizeof(unsigned long long), 0));
     e->next_t = 0;
     e->slot_rows_used = false;
+    e->prime_bs = 0;
     e->cs_T.assign(e->B, 0);                      // attached frames: their starts are absolute samples of the old timeline
     return 0;
 }
@@ -1167,6 +1174,40 @@ int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, 
     return score_range(e, who.c_str(), audio, first_sample, count, batch_size, logp, logits, true, (cudaStream_t)stream);
 }
 
+int nvwn_prime_from_score(nvwn_engine* e, void* stream)
+{
+    const std::string who = "nvwn_prime_from_score";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score, so only they can be primed");
+    if (e->score_next < 1)
+        return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompt with nvwn_score_stream "
+                                       "from first_sample = 0 first");
+    const int Bs = e->score_bs;
+    if (e->family->whole_batch && Bs != e->B)
+        return fail(NVWN_EINVAL, who + ": the tensor-core path needs the scoring stream's batch_size (" + std::to_string(Bs) +
+                                     ") equal to the engine's batch size (" + std::to_string(e->B) + ")");
+    if (e->slot_rows_used && Bs != e->B)
+        return fail(NVWN_EINVAL, who + ": after a per-slot call the scoring stream's batch_size (" + std::to_string(Bs) +
+                                     ") must equal the engine's batch size (" + std::to_string(e->B) + ") until nvwn_reset_history");
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long P = e->score_next;
+    const int T = e->score_T, R = e->R, L = e->L;
+    const ScoreScratch o = score_scratch_layout(e, T);
+    const __half* xh = reinterpret_cast<const __half*>(e->score_scratch + o.xh);
+    // layer l's front holds x_l of times [P - d_l, P), d_l rows of Bs utterances: the entries with t >= 0 are the ring entries a
+    // generation from sample P reads (x_l[t - d_l] with t >= P); earlier times are never read (hist_t)
+    for (int l = 0; l < L; l++) {
+        const int d = wn_score_dilation(l, e->maxDil);
+        const long long t_first = P - d > 0 ? P - d : 0;
+        const __half* src = xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R) + (size_t)(t_first - (P - d)) * Bs * R;
+        CK(e->family->put_history(*e, e->ring, src, l, t_first, (int)(P - t_first), Bs, st));
+    }
+    CK(wn_feedback_from_codes(reinterpret_cast<const int*>(e->score_scratch + o.codes), Bs, e->yPrev, e->yCur, st));
+    e->next_t = P;
+    e->prime_bs = Bs;
+    return 0;
+}
+
 // debug only (not part of the public ABI): the engine's conditioning store for samples [first_sample, first_sample + num_samples),
 // converted back to fp32 [num_samples][L][B][2R] whatever the kernel-native layout (plain / tiled fp16 / fragment order) is
 int nvwn_debug_get_conditioning(nvwn_engine* e, float* out, int first_sample, int num_samples)
@@ -1181,6 +1222,22 @@ int nvwn_debug_get_conditioning(nvwn_engine* e, float* out, int first_sample, in
     if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
     cudaFree(tmp);
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_conditioning: ") + cudaGetErrorString(ce));
+    return 0;
+}
+
+// debug only (not part of the public ABI): the whole history ring, read at the stride of a run of `batch` utterances, as fp32
+// [(maxDil+1)][L][batch][R] in slot order, whatever the kernel-native layout
+int nvwn_debug_get_history(nvwn_engine* e, float* out, int batch)
+{
+    if (!e || !out) return fail(NVWN_EINVAL, "nvwn_debug_get_history: NULL argument");
+    if (batch < 1 || batch > e->B) return fail(NVWN_EINVAL, "nvwn_debug_get_history: batch outside [1, B]");
+    const size_t n = (size_t)(e->maxDil + 1) * e->L * batch * e->R;
+    float* tmp = nullptr;
+    CK(cudaMalloc((void**)&tmp, n * sizeof(float)));
+    cudaError_t ce = e->family->get_history(*e, tmp, e->ring, batch, 0);
+    if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
+    cudaFree(tmp);
+    if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_history: ") + cudaGetErrorString(ce));
     return 0;
 }
 

@@ -240,19 +240,47 @@ __global__ void lat_cond_rows_kernel(unsigned char* __restrict__ dst, const floa
     }
 }
 
-// zero utterances rows[i] in every history-ring entry (slot x L + layer; rstride = ntiles x 2 KB): a row is the 32 words that
-// store_x and the embedding store write for it, k-step j, lane 4 g + t, word 2 half + (row >= 8) of each 16-byte group
+// The history ring: per entry (slot x L + layer) one 2 KB image per 16-utterance tile of the engine's batch (ntiles of them).  Row
+// r = b mod 16 of a tile is the 32 words that store_x and the embedding store write for it: channels (c, c + 1), c even, sit at
+// k-step j = c / 16, lane 4 (r mod 8) + (c mod 8) / 2, word 2 ((c / 8) mod 2) + (r >= 8) of the lane's 16-byte group.
+__device__ __forceinline__ uint32_t* lat_ring_word(unsigned char* ring, size_t e, int ntiles, int b, int c)
+{
+    const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3, j = c >> 4, half = (c >> 3) & 1, t = (c & 7) >> 1;
+    return reinterpret_cast<uint32_t*>(ring + (e * ntiles + tile) * 2048 + (size_t)j * 512 + (size_t)(4 * g + t) * 16 + (size_t)(2 * half + hi) * 4);
+}
+
+// zero utterances rows[i] in every history-ring entry
 __global__ void lat_ring_clear_rows_kernel(unsigned char* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles)
 {
     const size_t total = (size_t)entries * n * 32;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int k = (int)(i & 31), j = k >> 3, t = (k >> 1) & 3, half = k & 1;
         const size_t ei = i >> 5;                                   // e * n + r
-        const int b = rows[ei % n];
-        const size_t e = ei / n;
-        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3;
-        const size_t off = (e * ntiles + tile) * 2048 + (size_t)j * 512 + (size_t)(4 * g + t) * 16 + (size_t)(2 * half + hi) * 4;
-        *reinterpret_cast<uint32_t*>(ring + off) = 0u;
+        *lat_ring_word(ring, ei / n, ntiles, rows[ei % n], 2 * (int)(i & 31)) = 0u;
+    }
+}
+
+// fp16 src [n][batch][64] -> rows 0..batch-1 of entries (t mod slots) * L + layer, t = t_first + j; one thread per channel pair
+__global__ void lat_put_history_kernel(unsigned char* __restrict__ ring, const uint32_t* __restrict__ src, int layer, int L, int slots,
+                                       long long t_first, int n, int batch, int ntiles)
+{
+    const size_t total = (size_t)n * batch * 32;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> 5;                                  // j * batch + b
+        const long long t = t_first + (long long)(row / batch);
+        *lat_ring_word(ring, (size_t)(t % slots) * L + layer, ntiles, (int)(row % batch), 2 * (int)(i & 31)) = src[i];
+    }
+}
+
+// the ring -> fp32 [entries][batch][64]
+__global__ void lat_get_history_kernel(float* __restrict__ dst, unsigned char* __restrict__ ring, int entries, int batch, int ntiles)
+{
+    const size_t total = (size_t)entries * batch * 32;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> 5;                                  // e * batch + b
+        const int c = 2 * (int)(i & 31);
+        const float2 v = unpack_h2(*lat_ring_word(ring, row / batch, ntiles, (int)(row % batch), c));
+        dst[row * 64 + c] = v.x;
+        dst[row * 64 + c + 1] = v.y;
     }
 }
 
@@ -1919,6 +1947,29 @@ static cudaError_t ring_clear_rows(const WnConfig& c, void* ring, const int* row
     return cudaGetLastError();
 }
 
+// the tiles are those of the engine's batch whatever the run's (wn_launch_lat: ntiles_alloc)
+static cudaError_t ring_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
+{
+    const size_t total = (size_t)n * batch * 32;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    lat_put_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), reinterpret_cast<const uint32_t*>(src), layer, c.L,
+                                                                 c.maxDil + 1, t_first, n, batch, lat_tiles(c.B));
+    return cudaGetLastError();
+}
+
+static cudaError_t ring_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
+{
+    const int entries = (c.maxDil + 1) * c.L;
+    const size_t total = (size_t)entries * batch * 32;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    lat_get_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, static_cast<unsigned char*>(const_cast<void*>(ring)), entries, batch, lat_tiles(c.B));
+    return cudaGetLastError();
+}
+
 static cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream)
 {
     const LatImage im = lat_image(p.S, p.L);
@@ -2046,4 +2097,4 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
 }
 
 const WnFamily wn_lat_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, ring_clear_rows, cond_convert_rows,
-                                wn_lat_pack, wn_launch_lat, false};
+                                ring_put_history, ring_get_history, wn_lat_pack, wn_launch_lat, false};

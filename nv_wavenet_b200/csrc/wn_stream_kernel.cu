@@ -693,4 +693,4 @@ bool wn_stream_supported(int R, int S, int A, bool)
 
 // the kernels read the weight blob and the plain conditioning store (wn_convert.cu); any batch up to the engine's
 const WnFamily wn_stream_family = {wn_plain_store_bytes, ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, wn_plain_clear_rows,
-                                   wn_plain_convert_rows, nullptr, wn_launch_stream, false};
+                                   wn_plain_convert_rows, wn_plain_put_history, wn_plain_get_history, nullptr, wn_launch_stream, false};

@@ -138,17 +138,51 @@ __global__ void tc_cond_rows_kernel(unsigned char* __restrict__ dst, const float
     }
 }
 
-// zero utterances rows[i] in every history-ring entry (slot x L + layer): each entry holds one 16 KB SW128 tile image per TU
-// utterances, row r of a tile at bytes [128 r, 128 r + 128) (its 16-byte chunks permuted by r & 7 inside them)
-__global__ void tc_ring_clear_rows_kernel(uint4* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles, int TU)
+// The history ring: each entry (slot x L + layer) holds one 16 KB SW128 tile image per TU utterances (ntiles of them), row
+// r = b mod TU of a tile at bytes [128 r, 128 r + 128) in the channel order publish_x writes (its 16-byte chunks permuted by r & 7).
+// The 16 bytes of channels [8 q, 8 q + 8) of utterance b in entry e:
+__device__ __forceinline__ uint4* tc_ring_chunk(unsigned char* ring, size_t e, int ntiles, int TU, int b, int q)
+{
+    return reinterpret_cast<uint4*>(ring + (e * ntiles + b / TU) * TILE + sw128_offset(b % TU, 8 * q));
+}
+
+// zero utterances rows[i] in every history-ring entry
+__global__ void tc_ring_clear_rows_kernel(unsigned char* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles, int TU)
 {
     const size_t total = (size_t)entries * n * 8;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int q = (int)(i & 7);
         const size_t ei = i >> 3;                         // e * n + r
-        const int b = rows[ei % n];
-        const size_t e = ei / n;
-        ring[((e * ntiles + b / TU) * TILE + (size_t)(b % TU) * 128) / 16 + q] = make_uint4(0, 0, 0, 0);
+        *tc_ring_chunk(ring, ei / n, ntiles, TU, rows[ei % n], (int)(i & 7)) = make_uint4(0, 0, 0, 0);
+    }
+}
+
+// fp16 src [n][batch][64] -> rows 0..batch-1 of entries (t mod slots) * L + layer, t = t_first + j; one thread per 16-byte chunk
+__global__ void tc_put_history_kernel(unsigned char* __restrict__ ring, const uint4* __restrict__ src, int layer, int L, int slots, long long t_first,
+                                      int n, int batch, int ntiles, int TU)
+{
+    const size_t total = (size_t)n * batch * 8;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> 3;                        // j * batch + b
+        const long long t = t_first + (long long)(row / batch);
+        *tc_ring_chunk(ring, (size_t)(t % slots) * L + layer, ntiles, TU, (int)(row % batch), (int)(i & 7)) = src[i];
+    }
+}
+
+// the ring -> fp32 [entries][batch][64]
+__global__ void tc_get_history_kernel(float* __restrict__ dst, unsigned char* __restrict__ ring, int entries, int batch, int ntiles, int TU)
+{
+    const size_t total = (size_t)entries * batch * 8;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> 3;                        // e * batch + b
+        const int q = (int)(i & 7);
+        const uint4 v = *tc_ring_chunk(ring, row / batch, ntiles, TU, (int)(row % batch), q);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const float2 f = wn::unpack_h2(w[k]);
+            dst[row * 64 + 8 * q + 2 * k] = f.x;
+            dst[row * 64 + 8 * q + 2 * k + 1] = f.y;
+        }
     }
 }
 
@@ -741,8 +775,31 @@ cudaError_t ring_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, 
     if (total == 0) return cudaSuccess;
     size_t blocks = (total + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    tc_ring_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<uint4*>(ring), rows_dev, n, entries, (c.B + c.tc_tile - 1) / c.tc_tile,
-                                                                    c.tc_tile);
+    tc_ring_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), rows_dev, n, entries,
+                                                                    (c.B + c.tc_tile - 1) / c.tc_tile, c.tc_tile);
+    return cudaGetLastError();
+}
+
+cudaError_t ring_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
+{
+    const size_t total = (size_t)n * batch * 8;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    tc_put_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), reinterpret_cast<const uint4*>(src), layer, c.L,
+                                                                c.maxDil + 1, t_first, n, batch, (c.B + c.tc_tile - 1) / c.tc_tile, c.tc_tile);
+    return cudaGetLastError();
+}
+
+cudaError_t ring_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
+{
+    const int entries = (c.maxDil + 1) * c.L;
+    const size_t total = (size_t)entries * batch * 8;
+    if (total == 0) return cudaSuccess;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    tc_get_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, static_cast<unsigned char*>(const_cast<void*>(ring)), entries, batch,
+                                                                (c.B + c.tc_tile - 1) / c.tc_tile, c.tc_tile);
     return cudaGetLastError();
 }
 
@@ -786,4 +843,4 @@ bool wn_tc_supported(int R_, int S, int A_, int, int)
 }
 
 const WnFamily wn_tc_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, ring_clear_rows, cond_convert_rows,
-                               wn_tc_pack, wn_launch_tc, true};
+                               ring_put_history, ring_get_history, wn_tc_pack, wn_launch_tc, true};

@@ -348,6 +348,11 @@ class NVWavenetInfer:
         return self._score(audio, num_samples, batch_size, logits, "score_stream",
                            lambda a, n, bs, lp, lg: self._l.nvwn_score_stream(self._h, a, first_sample, n, bs, lp, lg, _stream(stream)))
 
+    def prime_from_score(self, stream=None):
+        """After score_stream over a prompt, samples [0, P): generation continues the prompt from sample P, run_stream(P, count, bs)
+        with the scoring stream's batch_size bs.  The scoring stream stays open.  Asynchronous on `stream`; see nvwn_prime_from_score."""
+        check(self._l.nvwn_prime_from_score(self._h, _stream(stream)), "primeFromScore")
+
     def _score(self, audio, num_samples, batch_size, logits, what, call):
         """audio[:batch_size, :num_samples] as int32 and the outputs of score() in matching memory; call(audio, n, bs, logp, logits)
         with their pointers."""

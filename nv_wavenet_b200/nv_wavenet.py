@@ -157,14 +157,30 @@ class NVWaveNet:
             self.engines_created += 1
         return eng
 
-    def infer(self, cond_input, implementation, seed=None, fp16=False, window=None):
+    def infer(self, cond_input, implementation, seed=None, fp16=False, window=None, prompt=None):
         """cond_input: channels x batch x num_layers x samples (pytorch/nv_wavenet.py:172-196); returns int32 [batch][samples].
         `implementation` (Impl.*) is accepted for compatibility: one kernel family serves all of them.
         window=W generates through one engine of W samples per (batch, W, precision), whatever the length, in windows of W
-        samples (nvwn_run_stream); the result is the same as without a window, bit for bit."""
+        samples (nvwn_run_stream); the result is the same as without a window, bit for bit.
+        prompt: int mu-law codes [batch][P], 1 <= P < samples (host or CUDA tensor), fp16 only.  The prompt is scored all steps at
+        once (nvwn_score_stream, a window at a time with a window), generation is primed from the scoring state
+        (nvwn_prime_from_score) and continues with samples [P, samples), drawn with the selectors infer() uses at those samples.
+        The first P columns of the result are the prompt.  The continuation is not bit-identical to forced generation of the
+        prompt (the history holds the scorer's fp16 values, DESIGN.md §5.4); with a window it is bit-identical to without one."""
         if (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
             raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
         batch_size, sample_count = cond_input.size(1), cond_input.size(3)
+        if prompt is not None:
+            prompt = torch.as_tensor(prompt)
+            shape = tuple(prompt.shape)
+            if len(shape) != 2 or shape[0] != batch_size or not 1 <= shape[1] < sample_count:
+                raise AssertionError(f"prompt must be [batch][P] with batch {batch_size} and 1 <= P < {sample_count}; got {shape}")
+            if prompt.dtype.is_floating_point or prompt.dtype.is_complex or prompt.dtype == torch.bool:
+                raise AssertionError(f"prompt must hold integer mu-law codes; got {prompt.dtype}")
+            if not fp16:
+                raise AssertionError("a prompt needs fp16=True: it is scored by the fp16 scorer")
+            if window is not None and window < 1:
+                raise AssertionError(f"window must be at least 1; got {window}")
         eng = self._engine(batch_size, sample_count if window is None else window, fp16)
         lh = column_major(cond_input).float()                       # [samples][layers][batch][2R]
         eng.reset_history()
@@ -173,7 +189,10 @@ class NVWaveNet:
             sel = np.empty(sample_count * batch_size, np.float32)
             _lib.check(self._lib.nvwn_libc_selectors(C.c_void_p(sel.ctypes.data), batch_size, sample_count), "selectors")
         samples = torch.empty((batch_size, sample_count), dtype=torch.int32, device="cuda")
-        if window is None:
+        if prompt is not None:
+            self._continue(eng, lh, prompt.to(device="cuda", dtype=torch.int32), seed, sel, sample_count if window is None else window,
+                           samples)
+        elif window is None:
             eng.set_conditioning(lh, 0, sample_count)
             if sel is None:
                 eng.set_selectors_random(seed)
@@ -195,6 +214,35 @@ class NVWaveNet:
                 eng.get_yout_stream(samples[:, first:first + n], first, n)
         torch.cuda.synchronize()
         return samples
+
+    @staticmethod
+    def _continue(eng, lh, prompt, seed, sel, window, samples):
+        """The prompted path of infer() on a reset engine of `window` samples: windows at multiples of W, each one's conditioning
+        set once; the prompt's part of a window is scored, the engine primed at the prompt's end and the rest of the window
+        generated with the selectors of those samples (Philox under `seed`, or the host draw `sel`)."""
+        batch_size, sample_count = samples.shape
+        P = prompt.shape[1]
+        samples[:, :P] = prompt
+        for first in range(0, sample_count, window):
+            n = min(window, sample_count - first)
+            eng.set_conditioning(lh[first:first + n], 0, n)
+            g0 = first
+            if first < P:
+                g0 = min(first + n, P)
+                eng.score_stream(prompt[:, first:g0], first)
+                if g0 == P:
+                    eng.prime_from_score()
+            k = first + n - g0
+            if k == 0:
+                continue
+            if sel is None:
+                eng.set_selectors_random_stream(seed, g0, k)
+            else:
+                chunk = np.zeros(window * batch_size, np.float32)
+                chunk[(g0 - first) * batch_size:n * batch_size] = sel[g0 * batch_size:(first + n) * batch_size]
+                eng.set_selectors(chunk)
+            eng.run_stream(g0, k, batch_size)
+            eng.get_yout_stream(samples[:, g0:g0 + k], g0, k)
 
     def infer_many(self, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None):
         """Continuous batching: generates a queue of utterances of different lengths through one engine of `slots` utterances and
