@@ -73,7 +73,8 @@ struct WnFamily {
     size_t (*image_bytes)(const WnConfig& c);       // NULL when pack is
     cudaError_t (*convert)(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
     cudaError_t (*readback)(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
-    // Per-utterance-row twins (continuous batching, DESIGN.md §6), rows_dev: n distinct rows in [0, c.B), device memory.
+    // Per-utterance-row operations (continuous batching, DESIGN.md §6), rows_dev: n distinct rows in [0, c.B), device memory.
+    // wn_layout.cuh implements these and the history writers once, over each family's layout.
     // clear_rows zeroes every byte of rows rows_dev[i] in all (maxDil+1) x L history-ring entries and no other byte;
     // convert_rows converts fp32 [num_pos][L][n][2R] (device) into rows rows_dev[i] of store positions [first_pos, +num_pos),
     // bit for bit as convert does, and leaves every other row alone.
@@ -98,16 +99,10 @@ bool wn_tc_supported(int R, int S, int A, int L, int B);
 bool wn_lat_supported(int R, int S, int A, int L);
 int wn_lat_max_clusters(int S, int rows);          // three-CTA clusters of `rows` (8 or 16) utterances the device runs at once
 
-// the plain conditioning store of the stream kernel (wn_convert.cu): [N][L][B][2R], fp16 on NVWN_FP16 engines, else fp32
-size_t wn_plain_store_bytes(const WnConfig& c);
+// the plain conditioning store of the stream kernel, [N][L][B][2R], fp16 on NVWN_FP16 engines, else fp32: whole-store conversions
+// (wn_convert.cu)
 cudaError_t wn_plain_convert(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
 cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
-// ... and its history ring [(maxDil+1)][L][B][R], fp16 on NVWN_FP16 engines, else fp32: the per-row operations of WnFamily
-cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream);
-cudaError_t wn_plain_convert_rows(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
-                                  cudaStream_t stream);
-cudaError_t wn_plain_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream);
-cudaError_t wn_plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream);
 
 // teacher-forced scoring (wn_score_kernel.cu, DESIGN.md §5.4): one time chunk of T steps x Bs utterances, rows m = (t - t0) * Bs + b
 struct WnScoreChunk {

@@ -141,11 +141,6 @@ cudaError_t wn_fill_int(int* dst, int value, size_t n, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-size_t wn_plain_store_bytes(const WnConfig& c)
-{
-    return (size_t)c.N * c.L * c.B * 2 * c.R * (c.dtype == NVWN_FP16 ? sizeof(__half) : sizeof(float));
-}
-
 cudaError_t wn_plain_convert(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream)
 {
     const size_t per = (size_t)c.L * c.B * 2 * c.R, n = per * num_samples;
@@ -158,68 +153,6 @@ cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* sto
     const size_t per = (size_t)c.L * c.B * 2 * c.R, n = per * num_samples;
     if (c.dtype == NVWN_FP16) return wn_f16_to_f32(dst_dev, static_cast<const __half*>(store) + (size_t)first_sample * per, n, stream);
     return cudaMemcpyAsync(dst_dev, static_cast<const float*>(store) + (size_t)first_sample * per, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
-}
-
-// 16-byte word k of the history-ring row (entry e = slot * L + layer, utterance b) of a run of `batch` utterances: rows of
-// `words` 16-byte words (R elements of TD, R * sizeof(TD) >= 64), entry-major at the run's batch stride
-__device__ __forceinline__ uint4* plain_ring_word(void* ring, size_t e, int batch, int b, int words, int k)
-{
-    return static_cast<uint4*>(ring) + (e * batch + b) * words + k;
-}
-// rows rows[i] zeroed in every entry, at the engine's batch stride B
-__global__ void plain_clear_rows_kernel(void* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int B, int words)
-{
-    const size_t total = (size_t)entries * n * words;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int k = (int)(i % words);
-        const size_t ei = i / words;                              // e * n + i
-        const int r = (int)(ei % n);
-        const size_t e = ei / n;
-        *plain_ring_word(ring, e, B, rows[r], words, k) = make_uint4(0, 0, 0, 0);
-    }
-}
-cudaError_t wn_plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
-{
-    if (n <= 0) return cudaSuccess;
-    const int words = c.R * (c.dtype == NVWN_FP16 ? (int)sizeof(__half) : (int)sizeof(float)) / 16;
-    const size_t total = (size_t)(c.maxDil + 1) * c.L * n * words;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    plain_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(ring, rows_dev, n, (c.maxDil + 1) * c.L, c.B, words);
-    return cudaGetLastError();
-}
-
-// fp16 src [n][batch][R] (16-byte words, `words` per row) -> rows 0..batch-1 of entries (t mod slots) * L + layer, t = t_first + j
-__global__ void plain_put_history_kernel(void* __restrict__ ring, const uint4* __restrict__ src, int layer, int L, int slots, long long t_first,
-                                         int n, int batch, int words)
-{
-    const size_t total = (size_t)n * batch * words;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int k = (int)(i % words);
-        const size_t row = i / words;                             // j * batch + b
-        const int b = (int)(row % batch);
-        const long long t = t_first + (long long)(row / batch);
-        *plain_ring_word(ring, (size_t)(t % slots) * L + layer, batch, b, words, k) = src[i];
-    }
-}
-cudaError_t wn_plain_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
-{
-    const int words = c.R * (int)sizeof(__half) / 16;
-    const size_t total = (size_t)n * batch * words;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    plain_put_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(ring, reinterpret_cast<const uint4*>(src), layer, c.L, c.maxDil + 1, t_first, n,
-                                                                   batch, words);
-    return cudaGetLastError();
-}
-
-// at the run's batch stride the plain ring already is [(maxDil+1)][L][batch][R]: a conversion of its first elements
-cudaError_t wn_plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
-{
-    const size_t n = (size_t)(c.maxDil + 1) * c.L * batch * c.R;
-    if (c.dtype == NVWN_FP16) return wn_f16_to_f32(dst, static_cast<const __half*>(ring), n, stream);
-    return cudaMemcpyAsync(dst, ring, n * sizeof(float), cudaMemcpyDeviceToDevice, stream);
 }
 
 // fed-back indices from the codes of a scoring stream: step t embeds (y[t-2], y[t-1]) = (yPrev, yCur) in generation and
@@ -236,40 +169,6 @@ cudaError_t wn_feedback_from_codes(const int* codes, int n, int* yPrev, int* yCu
 {
     if (n <= 0) return cudaSuccess;
     feedback_from_codes_kernel<<<(n + 255) / 256, 256, 0, stream>>>(codes, n, yPrev, yCur);
-    return cudaGetLastError();
-}
-
-// fp32 [num_pos][L][n][2R] -> rows rows[i] of the plain store at positions [first_pos, +num_pos); TD = __half rounds as
-// f32_to_f16_kernel does (round to nearest even, element by element)
-template <typename TD>
-__global__ void plain_convert_rows_kernel(TD* __restrict__ dst, const float* __restrict__ src, const int* __restrict__ rows, int n, int first_pos,
-                                          int num_pos, int L, int B, int R2)
-{
-    const size_t total = (size_t)num_pos * L * n * R2;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int k = (int)(i % R2);
-        const size_t row = i / R2;                                // (s * L + l) * n + r
-        const int r = (int)(row % n);
-        const size_t sl = row / n;                                // s * L + l
-        const float v = src[i];
-        TD* d = dst + (((size_t)first_pos * L + sl) * B + rows[r]) * R2 + k;
-        if constexpr (sizeof(TD) == 2) *d = __float2half_rn(v);
-        else *d = v;
-    }
-}
-cudaError_t wn_plain_convert_rows(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos,
-                                  cudaStream_t stream)
-{
-    const size_t total = (size_t)num_pos * c.L * n * 2 * c.R;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    if (c.dtype == NVWN_FP16)
-        plain_convert_rows_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(static_cast<__half*>(store), src, rows_dev, n, first_pos, num_pos,
-                                                                                 c.L, c.B, 2 * c.R);
-    else
-        plain_convert_rows_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(static_cast<float*>(store), src, rows_dev, n, first_pos, num_pos,
-                                                                                c.L, c.B, 2 * c.R);
     return cudaGetLastError();
 }
 

@@ -36,6 +36,24 @@ int fail(int code, const std::string& msg)
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// Absolute samples [first, first + count) of the engine's N-sample buffers used as rings (count <= N), as at most two pieces
+// (position, offset, length): samples first + off .. first + off + len - 1 sit at positions pos .. pos + len - 1.  The same split
+// as infer.split_at_wrap.
+struct WrapPiece {
+    int pos, off, len;
+};
+struct WrapPieces {
+    WrapPiece piece[2];
+    int n;
+    const WrapPiece* begin() const { return piece; }
+    const WrapPiece* end() const { return piece + n; }
+};
+WrapPieces split_at_wrap(long long first, int count, int N)
+{
+    const int pos = (int)(first % N), head = count < N - pos ? count : N - pos;
+    return {{{pos, 0, head}, {0, head, count - head}}, (head > 0) + (head < count)};
+}
+
 bool is_device_ptr(const void* p)
 {
     cudaPointerAttributes at;
@@ -580,10 +598,11 @@ int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sa
     const long long Nn = (long long)e->cp_T * e->cp_stride;
     if (sample_begin < 0 || sample_count < 0 || sample_begin + sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: sample range outside num_frames * stride");
     if (sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: more samples than the engine's num_samples (" + std::to_string(e->N) + ")");
-    const int pos = (int)(sample_begin % e->N), head = sample_count < e->N - pos ? sample_count : e->N - pos;
-    int rc = cond_produce(e, pos, (int)sample_begin, head, stream);
-    if (rc == 0 && head < sample_count) rc = cond_produce(e, 0, (int)sample_begin + head, sample_count - head, stream);
-    return rc;
+    for (const WrapPiece& w : split_at_wrap(sample_begin, sample_count, e->N)) {
+        const int rc = cond_produce(e, w.pos, (int)sample_begin + w.off, w.len, stream);
+        if (rc != 0) return rc;
+    }
+    return 0;
 }
 
 int nvwn_set_conditioning_from_features(nvwn_engine* e, const float* features, int n_cond_channels, int num_frames,
@@ -715,17 +734,14 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
     float* d_out = d_u + (size_t)e->cs_rows * C;
     d_out += (4 - ((size_t)(d_out - e->cs_scratch) & 3)) & 3;                 // 16-byte aligned rows for the tiled projection's float4 stores
     const int chunk = e->cs_rows / n;                                         // whole samples of every listed slot; >= 1 as cs_rows >= B
-    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
-    const int piece_pos[2] = {pos, 0}, piece_len[2] = {head, num_samples - head};
     cudaError_t ce = cudaSuccess;
-    for (int p = 0; p < 2; p++) {
-        const long long t0 = first_sample + (p ? head : 0);
-        for (int done = 0; done < piece_len[p] && ce == cudaSuccess; done += chunk) {
-            const int m = piece_len[p] - done < chunk ? piece_len[p] - done : chunk;
-            ce = wn_cond_produce_slots(d_out, d_u, e->cs_frames, d_tab, d_wut, d_bu, d_wc, d_bc, n, C, e->cs_K, e->cs_stride, L, R, t0 + done, m, st);
-            if (ce == cudaSuccess) ce = e->family->convert_rows(*e, e->Lh, d_out, d_slots, n, piece_pos[p] + done, m, st);
+    for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
+        for (int done = 0; done < w.len && ce == cudaSuccess; done += chunk) {
+            const int m = w.len - done < chunk ? w.len - done : chunk;
+            ce = wn_cond_produce_slots(d_out, d_u, e->cs_frames, d_tab, d_wut, d_bu, d_wc, d_bc, n, C, e->cs_K, e->cs_stride, L, R,
+                                       first_sample + w.off + done, m, st);
+            if (ce == cudaSuccess) ce = e->family->convert_rows(*e, e->Lh, d_out, d_slots, n, w.pos + done, m, st);
         }
-    }
     if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
     return 0;
 }
@@ -782,16 +798,13 @@ int nvwn_set_conditioning_slots(nvwn_engine* e, const float* Lh, const int* slot
         stage = e->row_stage;
         stage_elems = e->row_stage_elems;
     }
-    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
-    const int piece_pos[2] = {pos, 0}, piece_len[2] = {head, num_samples - head};
-    const float* src = Lh;
-    for (int k = 0; k < 2 && rc == 0; k++) {
-        rc = feed_via(stage, stage_elems, src, (size_t)piece_len[k], unit, st, [&](const float* s, size_t first, size_t m) {
-            return e->family->convert_rows(*e, e->Lh, s, e->slot_rows, n, piece_pos[k] + (int)first, (int)m, st);
+    for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N)) {
+        rc = feed_via(stage, stage_elems, Lh + (size_t)w.off * unit, (size_t)w.len, unit, st, [&](const float* s, size_t first, size_t m) {
+            return e->family->convert_rows(*e, e->Lh, s, e->slot_rows, n, w.pos + (int)first, (int)m, st);
         });
-        src += (size_t)piece_len[k] * unit;
+        if (rc != 0) return rc;
     }
-    return rc;
+    return 0;
 }
 
 int nvwn_set_selectors_random_slots(nvwn_engine* e, long long first_sample, int num_samples, void* stream)
@@ -803,9 +816,8 @@ int nvwn_set_selectors_random_slots(nvwn_engine* e, long long first_sample, int 
     cudaStream_t st = (cudaStream_t)stream;
     const size_t B = e->B;
     e->slot_rows_used = true;
-    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
-    CK(wn_fill_selectors_slots(e->sel + (size_t)pos * B, head, e->B, first_sample, e->origin, e->seed, st));
-    CK(wn_fill_selectors_slots(e->sel, num_samples - head, e->B, first_sample + head, e->origin, e->seed, st));
+    for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
+        CK(wn_fill_selectors_slots(e->sel + (size_t)w.pos * B, w.len, e->B, first_sample + w.off, e->origin, e->seed, st));
     return 0;
 }
 
@@ -846,9 +858,8 @@ int nvwn_set_selectors_random_stream(nvwn_engine* e, unsigned long long seed, lo
     if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
         return fail(NVWN_EINVAL, "nvwn_set_selectors_random_stream: need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) + ") of the engine");
     const size_t B = e->B;
-    const int pos = (int)(first_sample % e->N), head = num_samples < e->N - pos ? num_samples : e->N - pos;
-    CK(wn_fill_selectors(e->sel + (size_t)pos * B, (size_t)head * B, seed, (unsigned long long)first_sample * B, (cudaStream_t)stream));
-    CK(wn_fill_selectors(e->sel, (size_t)(num_samples - head) * B, seed, (unsigned long long)(first_sample + head) * B, (cudaStream_t)stream));
+    for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
+        CK(wn_fill_selectors(e->sel + (size_t)w.pos * B, (size_t)w.len * B, seed, (unsigned long long)(first_sample + w.off) * B, (cudaStream_t)stream));
     return 0;
 }
 
@@ -921,11 +932,12 @@ int nvwn_run_stream(nvwn_engine* e, long long first_sample, int count, int batch
         return fail(NVWN_EINVAL, "nvwn_run_stream: first_sample " + std::to_string(first_sample) + " does not continue the utterance batch: the next sample is " +
                                      std::to_string(e->next_t) + " (nvwn_reset_history starts over at 0)");
     cudaStream_t stream = (cudaStream_t)stream_;
-    const int pos = (int)(first_sample % e->N), head = count < e->N - pos ? count : e->N - pos;
     const int dump = dump_activations ? 1 : 0;
-    int rc = launch_steps(e, "nvwn_run_stream", pos, first_sample, head, e->N, batch_size, head == count ? dump : 0, stream);
-    if (rc == 0 && head < count) rc = launch_steps(e, "nvwn_run_stream", 0, first_sample + head, count - head, e->N, batch_size, dump, stream);
-    return rc;
+    for (const WrapPiece& w : split_at_wrap(first_sample, count, e->N)) {
+        const int rc = launch_steps(e, "nvwn_run_stream", w.pos, first_sample + w.off, w.len, e->N, batch_size, w.off + w.len == count ? dump : 0, stream);
+        if (rc != 0) return rc;
+    }
+    return 0;
 }
 
 int nvwn_run(nvwn_engine* e, int num_samples, int batch_size, int* yOut, int dump_activations, void* stream)
@@ -1105,9 +1117,8 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, long long fir
     for (int t0 = 0; t0 < N; t0 += T) {
         const int Tc = N - t0 < T ? N - t0 : T;
         // the chunk's conditioning, in two pieces where its samples wrap around the store
-        const int pos = (int)((first + t0) % e->N), head = Tc < e->N - pos ? Tc : e->N - pos;
-        CK(e->family->readback(*e, lh, e->Lh, pos, head, st));
-        if (head < Tc) CK(e->family->readback(*e, lh + (size_t)head * L * e->B * 2 * R, e->Lh, 0, Tc - head, st));
+        for (const WrapPiece& w : split_at_wrap(first + t0, Tc, e->N))
+            CK(e->family->readback(*e, lh + (size_t)w.off * L * e->B * 2 * R, e->Lh, w.pos, w.len, st));
         c.t0 = t0; c.T = Tc;
         c.logits = logits ? (logits_dev ? logits : lgt) : nullptr;
         c.logits_ld = logits_dev ? (long long)N * A : (long long)Tc * A;

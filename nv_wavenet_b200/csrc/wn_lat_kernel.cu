@@ -34,6 +34,7 @@
 // WNO_PREC_FP16 (GEMM inputs fp16, fp32 accumulation, fp32 residual stream / skip sum / softmax), gate evaluated with
 // tanh.approx.f16x2; no weight folding.
 #include "wn_common.h"
+#include "wn_layout.cuh"
 #include "wn_math.cuh"
 #include "wn_sm90.cuh"
 
@@ -171,13 +172,41 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait_pending() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// ------------------------------------------------------------------------------------------------ conditioning layout
-// fp16, [N][L][tiles][8 warps][32 lanes][16 B]: the uint4 of thread (w, lane = 4 g + t) holds, as half2 pairs of channels
-// (c, c+1), c = 8 w + 2 t:  .x = (row g, tanh c) .y = (row g+8, tanh c) .z = (row g, sigmoid R+c) .w = (row g+8, sigmoid R+c)
-// i.e. exactly the accumulator fragment the thread adds it to.  Rows past the batch are zero.
-__global__ void lat_cond_kernel(unsigned char* __restrict__ dst, const float* __restrict__ src, int first_sample, int nsamples, int L, int B, int ntiles)
+// ------------------------------------------------------------------------------------------------ layouts
+__host__ __device__ inline int lat_tiles(int B) { return (B + TU - 1) / TU; }
+
+// The latency layouts for wn_layout.cuh, both per 16-utterance tile of the engine's batch; a unit is one 4-byte word of a channel
+// pair (c, c + 1), c even, of one utterance row b: tile b / 16, row r = b mod 16, g = r mod 8.
+struct LatLayout {
+    using TD = __half;
+    static constexpr int STORE_UNIT = 2, RING_UNIT = 2;
+    // Conditioning: fp16, [N][L][tiles][8 warps][32 lanes][16 B]: the uint4 of thread (w, lane = 4 g + t) holds, as half2 pairs of
+    // channels (c, c+1), c = 8 w + 2 t:  .x = (row g, tanh c) .y = (row g+8, tanh c) .z = (row g, sigmoid R+c) .w = (row g+8, sigmoid R+c)
+    // i.e. exactly the accumulator fragment the thread adds it to.  Unit k is channels (2k, 2k + 1) of the 2R; k >= 32: sigmoid.
+    static __device__ WnVec<__half, 2>* store_unit(const WnConfig& c, void* store, size_t sl, int b, int k)
+    {
+        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3, sig = k >> 5, w = (k & 31) >> 2, t = k & 3;
+        return reinterpret_cast<WnVec<__half, 2>*>(static_cast<unsigned char*>(store) + (sl * lat_tiles(c.B) + tile) * 4096 +
+                                                   (size_t)(w * 32 + g * 4 + t) * 16 + (size_t)(2 * sig + hi) * 4);
+    }
+    // The history ring: per entry (slot x L + layer) one 2 KB image per tile.  Row r of a tile is the 32 words that store_x and the
+    // embedding store write for it: channels (c, c + 1) = (2k, 2k + 1) sit at k-step j = c / 16, lane 4 g + (c mod 8) / 2, word
+    // 2 ((c / 8) mod 2) + (r >= 8) of the lane's 16-byte group.
+    static __device__ WnVec<__half, 2>* ring_unit(const WnConfig& c, void* ring, size_t e, int, int b, int k)
+    {
+        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3, j = k >> 3, half = (k >> 2) & 1, t = k & 3;
+        return reinterpret_cast<WnVec<__half, 2>*>(static_cast<unsigned char*>(ring) + (e * lat_tiles(c.B) + tile) * 2048 + (size_t)j * 512 +
+                                                   (size_t)(4 * g + t) * 16 + (size_t)(2 * half + hi) * 4);
+    }
+    static size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * lat_tiles(c.B) * 4096; }
+    static size_t ring_bytes(const WnConfig& c) { return (size_t)(c.maxDil + 1) * c.L * lat_tiles(c.B) * 2048; }
+};
+
+// The whole store, one thread per 16-byte group of the layout: rows g and g + 8 and both gate halves in one store, and zero rows
+// past the batch.  The per-row wn_convert_rows would store the same bytes as four 4-byte words and leave the padding rows alone.
+__global__ void lat_cond_kernel(size_t total, WnConfig cfg, unsigned char* __restrict__ dst, const float* __restrict__ src, int first_sample)
 {
-    const size_t total = (size_t)nsamples * L * ntiles * 256;
+    const int ntiles = lat_tiles(cfg.B);
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int th = (int)(i & 255), w = th >> 5, lane = th & 31, g = lane >> 2, t = lane & 3;
         const size_t slt = i >> 8;                       // (s * L + l) * ntiles + tile
@@ -188,99 +217,16 @@ __global__ void lat_cond_kernel(unsigned char* __restrict__ dst, const float* __
 #pragma unroll
         for (int hi = 0; hi < 2; hi++) {
             const int b = tile * TU + g + 8 * hi;
-            if (b < B) {
-                const float* row = src + (sl * B + b) * 128;
+            if (b < cfg.B) {
+                const float* row = src + (sl * cfg.B + b) * 128;
                 const float2 ft = *reinterpret_cast<const float2*>(row + c), fs = *reinterpret_cast<const float2*>(row + 64 + c);
                 __half2 a = __floats2half2_rn(ft.x, ft.y), s = __floats2half2_rn(fs.x, fs.y);
                 o[hi] = *reinterpret_cast<uint32_t*>(&a);
                 o[2 + hi] = *reinterpret_cast<uint32_t*>(&s);
             }
         }
-        const size_t off = (((size_t)first_sample * L * ntiles) + slt) * 4096 + (size_t)th * 16;
-        *reinterpret_cast<uint4*>(dst + off) = make_uint4(o[0], o[1], o[2], o[3]);
-    }
-}
-
-// inverse of lat_cond_kernel (debug / tests): conditioning store -> fp32 [n][L][B][2R]
-__global__ void lat_cond_readback_kernel(float* __restrict__ dst, const unsigned char* __restrict__ src, int first_sample, int nsamples, int L, int B, int ntiles)
-{
-    const size_t total = (size_t)nsamples * L * B * 64;            // one thread per channel pair
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int c2 = (int)(i & 63);
-        const size_t row = i >> 6;                                  // (s * L + l) * B + b
-        const int b = (int)(row % B);
-        const size_t sl = row / B;
-        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3;
-        const int sig = c2 >= 32, cc = (c2 & 31) * 2, w = cc >> 3, t = (cc & 7) >> 1;
-        const size_t off = (((size_t)first_sample * L + sl) * ntiles + tile) * 4096 + (size_t)(w * 32 + g * 4 + t) * 16 + (size_t)(2 * sig + hi) * 4;
-        const __half2 v = *reinterpret_cast<const __half2*>(src + off);
-        dst[row * 128 + sig * 64 + cc] = __low2float(v);
-        dst[row * 128 + sig * 64 + cc + 1] = __high2float(v);
-    }
-}
-
-// the row-indexed twin of lat_cond_kernel (continuous batching): fp32 [nsamples][L][n][2R] -> utterances rows[i] of store positions
-// [first_sample, +nsamples).  A row's channel pairs are whole words of the uint4s (.x / .z for rows g, .y / .w for rows g + 8), so
-// the other rows are not touched.
-__global__ void lat_cond_rows_kernel(unsigned char* __restrict__ dst, const float* __restrict__ src, const int* __restrict__ rows, int n,
-                                     int first_sample, int nsamples, int L, int ntiles)
-{
-    const size_t total = (size_t)nsamples * L * n * 64;            // one thread per channel pair
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int c2 = (int)(i & 63);
-        const size_t row = i >> 6;                                  // (s * L + l) * n + r
-        const int b = rows[row % n];
-        const size_t sl = row / n;
-        const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3;
-        const int sig = c2 >= 32, cc = (c2 & 31) * 2, w = cc >> 3, t = (cc & 7) >> 1;
-        const float2 f = *reinterpret_cast<const float2*>(src + row * 128 + sig * 64 + cc);
-        const __half2 v = __floats2half2_rn(f.x, f.y);
-        const size_t off = (((size_t)first_sample * L + sl) * ntiles + tile) * 4096 + (size_t)(w * 32 + g * 4 + t) * 16 + (size_t)(2 * sig + hi) * 4;
-        *reinterpret_cast<uint32_t*>(dst + off) = *reinterpret_cast<const uint32_t*>(&v);
-    }
-}
-
-// The history ring: per entry (slot x L + layer) one 2 KB image per 16-utterance tile of the engine's batch (ntiles of them).  Row
-// r = b mod 16 of a tile is the 32 words that store_x and the embedding store write for it: channels (c, c + 1), c even, sit at
-// k-step j = c / 16, lane 4 (r mod 8) + (c mod 8) / 2, word 2 ((c / 8) mod 2) + (r >= 8) of the lane's 16-byte group.
-__device__ __forceinline__ uint32_t* lat_ring_word(unsigned char* ring, size_t e, int ntiles, int b, int c)
-{
-    const int tile = b / TU, r = b % TU, g = r & 7, hi = r >> 3, j = c >> 4, half = (c >> 3) & 1, t = (c & 7) >> 1;
-    return reinterpret_cast<uint32_t*>(ring + (e * ntiles + tile) * 2048 + (size_t)j * 512 + (size_t)(4 * g + t) * 16 + (size_t)(2 * half + hi) * 4);
-}
-
-// zero utterances rows[i] in every history-ring entry
-__global__ void lat_ring_clear_rows_kernel(unsigned char* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles)
-{
-    const size_t total = (size_t)entries * n * 32;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t ei = i >> 5;                                   // e * n + r
-        *lat_ring_word(ring, ei / n, ntiles, rows[ei % n], 2 * (int)(i & 31)) = 0u;
-    }
-}
-
-// fp16 src [n][batch][64] -> rows 0..batch-1 of entries (t mod slots) * L + layer, t = t_first + j; one thread per channel pair
-__global__ void lat_put_history_kernel(unsigned char* __restrict__ ring, const uint32_t* __restrict__ src, int layer, int L, int slots,
-                                       long long t_first, int n, int batch, int ntiles)
-{
-    const size_t total = (size_t)n * batch * 32;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i >> 5;                                  // j * batch + b
-        const long long t = t_first + (long long)(row / batch);
-        *lat_ring_word(ring, (size_t)(t % slots) * L + layer, ntiles, (int)(row % batch), 2 * (int)(i & 31)) = src[i];
-    }
-}
-
-// the ring -> fp32 [entries][batch][64]
-__global__ void lat_get_history_kernel(float* __restrict__ dst, unsigned char* __restrict__ ring, int entries, int batch, int ntiles)
-{
-    const size_t total = (size_t)entries * batch * 32;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i >> 5;                                  // e * batch + b
-        const int c = 2 * (int)(i & 31);
-        const float2 v = unpack_h2(*lat_ring_word(ring, row / batch, ntiles, (int)(row % batch), c));
-        dst[row * 64 + c] = v.x;
-        dst[row * 64 + c + 1] = v.y;
+        // the group starts at the unit of (row g, tanh c)
+        *reinterpret_cast<uint4*>(LatLayout::store_unit(cfg, dst, (size_t)first_sample * cfg.L + sl, tile * TU + g, c / 2)) = make_uint4(o[0], o[1], o[2], o[3]);
     }
 }
 
@@ -1898,76 +1844,12 @@ bool wn_lat_supported(int R_, int S, int A_, int L)
 {
     return R_ == R && A_ == A && (S == 128 || S == 256) && L >= 4 && L <= MAXL;     // L >= 4: history prefetch runs 3 steps ahead (single-CTA kernel)
 }
-static int lat_tiles(int B) { return (B + TU - 1) / TU; }
 static size_t image_bytes(const WnConfig& c) { return lat_image(c.S, c.L).total; }
-static size_t ring_bytes(const WnConfig& c) { return (size_t)(c.maxDil + 1) * c.L * lat_tiles(c.B) * 2048; }
-static size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * lat_tiles(c.B) * 4096; }
 
 static cudaError_t cond_convert(const WnConfig& c, void* dst, const float* src_dev, int first_sample, int nsamples, cudaStream_t stream)
 {
-    if (nsamples <= 0) return cudaSuccess;
-    const int ntiles = lat_tiles(c.B);
-    const size_t total = (size_t)nsamples * c.L * ntiles * 256;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 32) blocks = 132 * 32;
-    lat_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, c.L, c.B, ntiles);
-    return cudaGetLastError();
-}
-
-static cudaError_t cond_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int nsamples, cudaStream_t stream)
-{
-    if (nsamples <= 0) return cudaSuccess;
-    const size_t total = (size_t)nsamples * c.L * c.B * 64;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 32) blocks = 132 * 32;
-    lat_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, c.L, c.B, lat_tiles(c.B));
-    return cudaGetLastError();
-}
-
-static cudaError_t cond_convert_rows(const WnConfig& c, void* store, const float* src_dev, const int* rows_dev, int n, int first_pos, int num_pos,
-                                     cudaStream_t stream)
-{
-    const size_t total = (size_t)num_pos * c.L * n * 64;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 32) blocks = 132 * 32;
-    lat_cond_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(store), src_dev, rows_dev, n, first_pos, num_pos, c.L,
-                                                               lat_tiles(c.B));
-    return cudaGetLastError();
-}
-
-static cudaError_t ring_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
-{
-    const int entries = (c.maxDil + 1) * c.L;
-    const size_t total = (size_t)entries * n * 32;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    lat_ring_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), rows_dev, n, entries, lat_tiles(c.B));
-    return cudaGetLastError();
-}
-
-// the tiles are those of the engine's batch whatever the run's (wn_launch_lat: ntiles_alloc)
-static cudaError_t ring_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
-{
-    const size_t total = (size_t)n * batch * 32;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    lat_put_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), reinterpret_cast<const uint32_t*>(src), layer, c.L,
-                                                                 c.maxDil + 1, t_first, n, batch, lat_tiles(c.B));
-    return cudaGetLastError();
-}
-
-static cudaError_t ring_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
-{
-    const int entries = (c.maxDil + 1) * c.L;
-    const size_t total = (size_t)entries * batch * 32;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    lat_get_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, static_cast<unsigned char*>(const_cast<void*>(ring)), entries, batch, lat_tiles(c.B));
-    return cudaGetLastError();
+    return wn_layout_launch(lat_cond_kernel, (size_t)nsamples * c.L * lat_tiles(c.B) * 256, stream, c, static_cast<unsigned char*>(dst), src_dev,
+                            first_sample);
 }
 
 static cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stream)
@@ -2096,5 +1978,6 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
     return cudaGetLastError();
 }
 
-const WnFamily wn_lat_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, ring_clear_rows, cond_convert_rows,
-                                ring_put_history, ring_get_history, wn_lat_pack, wn_launch_lat, false};
+const WnFamily wn_lat_family = {LatLayout::store_bytes, LatLayout::ring_bytes, image_bytes, cond_convert, wn_readback<LatLayout>,
+                                wn_clear_rows<LatLayout>, wn_convert_rows<LatLayout>, wn_put_history<LatLayout>, wn_get_history<LatLayout>,
+                                wn_lat_pack, wn_launch_lat, false};

@@ -22,6 +22,7 @@
 // and Wza.  A slab of a column-major matrix is contiguous, so every piece is one or two plain 1-D copies; a thread reads its row
 // of the slab with conflict-free 4-byte shared loads.  The arithmetic and its order are untouched (same bits).
 #include "wn_common.h"
+#include "wn_layout.cuh"
 #include "wn_math.cuh"
 #include "wn_sm90.cuh"
 
@@ -669,8 +670,6 @@ int pick_bt(const WnParams& p, bool fp16, int forced)
     return bt;
 }
 
-size_t ring_bytes(const WnConfig& c) { return (size_t)(c.maxDil + 1) * c.L * c.B * c.R * (c.dtype == NVWN_FP16 ? sizeof(__half) : sizeof(float)); }
-
 // NVWN_FP32: bit-exact (CPU model's operation order); NVWN_FP16: fp16 storage; NVWN_FP32_FAST: the reference GPU kernels' arithmetic
 cudaError_t wn_launch_stream(const WnConfig& c, const WnParams& p, const void*, cudaStream_t stream, WnLaunchInfo* info)
 {
@@ -683,6 +682,42 @@ cudaError_t wn_launch_stream(const WnConfig& c, const WnParams& p, const void*, 
                                      : launch_shape<float, false>(p, bt, c.stream_ring, stream, info);
 }
 
+// The plain layouts for wn_layout.cuh, of T = __half on NVWN_FP16 engines, else float: the conditioning store [N][L][B][2R] in
+// units of one channel, and the history ring [(maxDil+1)][L][stride][R] in units of one 16-byte word (R * sizeof(T) >= 64).
+template <typename T>
+struct PlainLayout {
+    using TD = T;
+    static constexpr int STORE_UNIT = 1, RING_UNIT = 16 / sizeof(T);
+    static __device__ WnVec<T, 1>* store_unit(const WnConfig& c, void* store, size_t sl, int b, int k)
+    {
+        return static_cast<WnVec<T, 1>*>(store) + (sl * c.B + b) * 2 * c.R + k;
+    }
+    static __device__ WnVec<T, RING_UNIT>* ring_unit(const WnConfig& c, void* ring, size_t e, int stride, int b, int k)
+    {
+        return static_cast<WnVec<T, RING_UNIT>*>(ring) + (e * stride + b) * (c.R / RING_UNIT) + k;
+    }
+    static size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * c.B * 2 * c.R * sizeof(T); }
+    static size_t ring_bytes(const WnConfig& c) { return (size_t)(c.maxDil + 1) * c.L * c.B * c.R * sizeof(T); }
+};
+using PlainH = PlainLayout<__half>;
+using PlainF = PlainLayout<float>;
+
+size_t plain_store_bytes(const WnConfig& c) { return c.dtype == NVWN_FP16 ? PlainH::store_bytes(c) : PlainF::store_bytes(c); }
+size_t plain_ring_bytes(const WnConfig& c) { return c.dtype == NVWN_FP16 ? PlainH::ring_bytes(c) : PlainF::ring_bytes(c); }
+cudaError_t plain_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
+{
+    return c.dtype == NVWN_FP16 ? wn_clear_rows<PlainH>(c, ring, rows_dev, n, stream) : wn_clear_rows<PlainF>(c, ring, rows_dev, n, stream);
+}
+cudaError_t plain_convert_rows(const WnConfig& c, void* store, const float* src, const int* rows_dev, int n, int first_pos, int num_pos, cudaStream_t stream)
+{
+    return c.dtype == NVWN_FP16 ? wn_convert_rows<PlainH>(c, store, src, rows_dev, n, first_pos, num_pos, stream)
+                                : wn_convert_rows<PlainF>(c, store, src, rows_dev, n, first_pos, num_pos, stream);
+}
+cudaError_t plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
+{
+    return c.dtype == NVWN_FP16 ? wn_get_history<PlainH>(c, dst, ring, batch, stream) : wn_get_history<PlainF>(c, dst, ring, batch, stream);
+}
+
 }  // namespace
 
 bool wn_stream_supported(int R, int S, int A, bool)
@@ -691,6 +726,8 @@ bool wn_stream_supported(int R, int S, int A, bool)
     return shape && A % 32 == 0 && A >= 32 && A <= 4096;
 }
 
-// the kernels read the weight blob and the plain conditioning store (wn_convert.cu); any batch up to the engine's
-const WnFamily wn_stream_family = {wn_plain_store_bytes, ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, wn_plain_clear_rows,
-                                   wn_plain_convert_rows, wn_plain_put_history, wn_plain_get_history, nullptr, wn_launch_stream, false};
+// The kernels read the weight blob and the plain conditioning store; any batch up to the engine's.  convert and readback are
+// contiguous conversions (wn_convert.cu): the plain store already is the source layout, and an fp32 convert also copies from host
+// memory, which no kernel can read.  put_history is fp16 only: the engine primes no other precision.
+const WnFamily wn_stream_family = {plain_store_bytes, plain_ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, plain_clear_rows,
+                                   plain_convert_rows, wn_put_history<PlainH>, plain_get_history, nullptr, wn_launch_stream, false};

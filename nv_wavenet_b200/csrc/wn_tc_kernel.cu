@@ -23,6 +23,7 @@
 // Numerical contract (oracle/wavenet_oracle.c, WNO_PREC_FP16): weights, biases, embeddings, Lh and every GEMM input
 // rounded to fp16; fp32 accumulation; residual stream, skip sum and softmax in fp32.
 #include "wn_common.h"
+#include "wn_layout.cuh"
 #include "wn_math.cuh"
 #include "wn_sm90.cuh"
 
@@ -65,126 +66,40 @@ __host__ __device__ inline size_t tc_smem_bytes(int nstage)
     return 1024 + (size_t)nstage * TILE + 4 * ATILE + 4 * ATILE + (size_t)TU * A * sizeof(float) + TU * sizeof(int) + 2 * (size_t)nstage * 8;
 }
 
-// Conditioning in the tensor-core layout: fp16 [N][L][Bpad rows][2 halves of 64 channels], tiled per 128 utterances;
+// Conditioning in the tensor-core layout: fp16 [N][L][Bpad rows][2 halves of 64 channels], tiled per c.tc_tile utterances;
 // inside a tile: [half][row][128 B], 16-byte chunks XOR-swizzled with (row & 7) -- i.e. exactly the K-major
 // SWIZZLE_128B image of an MMA A-operand tile, so a 1-D bulk TMA copy of rows*128 bytes needs no further shuffling.
 __host__ __device__ inline int cond_rows(int B, int tile, int TU) { const int r = B - tile * TU; return r >= TU ? TU : ((r + 7) & ~7); }
 __host__ __device__ inline size_t cond_bpad(int B, int TU) { const int nt = (B + TU - 1) / TU; return (size_t)(nt - 1) * TU + cond_rows(B, nt - 1, TU); }
 
-__global__ void tc_cond_kernel(unsigned char* __restrict__ dst, const float* __restrict__ src, int first_sample, int nsamples, int L, int B, int TU)
-{
-    // one thread per (sample, layer, utterance, 8-channel chunk): 32 B in, 16 B out
-    const size_t total = (size_t)nsamples * L * B * 16;
-    const size_t bpad = cond_bpad(B, TU);
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int c = (int)(i & 15);
-        const size_t rowi = i >> 4;                       // (s * L + l) * B + b
-        const int b = (int)(rowi % B);
-        const size_t sl = rowi / B;                       // s * L + l
-        const float4 f0 = *reinterpret_cast<const float4*>(src + rowi * 128 + c * 8);
-        const float4 f1 = *reinterpret_cast<const float4*>(src + rowi * 128 + c * 8 + 4);
-        __half2 h0 = __floats2half2_rn(f0.x, f0.y), h1 = __floats2half2_rn(f0.z, f0.w), h2 = __floats2half2_rn(f1.x, f1.y), h3 = __floats2half2_rn(f1.z, f1.w);
-        uint4 o;
-        o.x = *reinterpret_cast<unsigned*>(&h0); o.y = *reinterpret_cast<unsigned*>(&h1);
-        o.z = *reinterpret_cast<unsigned*>(&h2); o.w = *reinterpret_cast<unsigned*>(&h3);
-        const int tile = b / TU, r = b % TU, half = c >> 3, q = c & 7;
-        const size_t off = (((size_t)first_sample * L + sl) * bpad + (size_t)tile * TU) * 256 + (size_t)half * cond_rows(B, tile, TU) * 128 +
-                           (size_t)r * 128 + (size_t)((q ^ (r & 7)) << 4);
-        *reinterpret_cast<uint4*>(dst + off) = o;
+// The tensor-core layouts for wn_layout.cuh: a unit is one 16-byte chunk of 8 channels in both.
+struct TcLayout {
+    using TD = __half;
+    static constexpr int STORE_UNIT = 8, RING_UNIT = 8;
+    // chunk k of the 2R channels of utterance b: half k / 8, chunk k mod 8 of its 128-byte row
+    static __device__ WnVec<__half, 8>* store_unit(const WnConfig& c, void* store, size_t sl, int b, int k)
+    {
+        const int TU = c.tc_tile, tile = b / TU, r = b % TU, half = k >> 3, q = k & 7;
+        return reinterpret_cast<WnVec<__half, 8>*>(static_cast<unsigned char*>(store) + (sl * cond_bpad(c.B, TU) + (size_t)tile * TU) * 256 +
+                                                   (size_t)half * cond_rows(c.B, tile, TU) * 128 + (size_t)r * 128 + (size_t)((q ^ (r & 7)) << 4));
     }
-}
-
-// inverse of tc_cond_kernel (debug / tests): conditioning store -> fp32 [n][L][B][2R]
-__global__ void tc_cond_readback_kernel(float* __restrict__ dst, const unsigned char* __restrict__ src, int first_sample, int nsamples, int L, int B, int TU)
-{
-    const size_t total = (size_t)nsamples * L * B * 16;
-    const size_t bpad = cond_bpad(B, TU);
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int c = (int)(i & 15);
-        const size_t rowi = i >> 4;
-        const int b = (int)(rowi % B);
-        const size_t sl = rowi / B;
-        const int tile = b / TU, r = b % TU, half = c >> 3, q = c & 7;
-        const size_t off = (((size_t)first_sample * L + sl) * bpad + (size_t)tile * TU) * 256 + (size_t)half * cond_rows(B, tile, TU) * 128 +
-                           (size_t)r * 128 + (size_t)((q ^ (r & 7)) << 4);
-        const __half2* v = reinterpret_cast<const __half2*>(src + off);
-#pragma unroll
-        for (int k = 0; k < 4; k++) { dst[rowi * 128 + c * 8 + 2 * k] = __low2float(v[k]); dst[rowi * 128 + c * 8 + 2 * k + 1] = __high2float(v[k]); }
+    // The history ring: each entry (slot x L + layer) holds one 16 KB SW128 tile image per c.tc_tile utterances of the engine's
+    // batch, row r = b mod tc_tile of a tile at bytes [128 r, 128 r + 128) in the channel order publish_x writes (its 16-byte chunks
+    // permuted by r & 7).  Chunk q holds channels [8 q, 8 q + 8).
+    static __device__ WnVec<__half, 8>* ring_unit(const WnConfig& c, void* ring, size_t e, int, int b, int q)
+    {
+        const int TU = c.tc_tile;
+        return reinterpret_cast<WnVec<__half, 8>*>(static_cast<unsigned char*>(ring) + (e * ((c.B + TU - 1) / TU) + b / TU) * TILE +
+                                                   sw128_offset(b % TU, 8 * q));
     }
-}
-
-// the row-indexed twin of tc_cond_kernel (continuous batching): fp32 [nsamples][L][n][2R] -> utterances rows[i] of store positions
-// [first_sample, +nsamples); a row is whole 16-byte chunks, so the other rows are not touched
-__global__ void tc_cond_rows_kernel(unsigned char* __restrict__ dst, const float* __restrict__ src, const int* __restrict__ rows, int n,
-                                    int first_sample, int nsamples, int L, int B, int TU)
-{
-    const size_t total = (size_t)nsamples * L * n * 16;
-    const size_t bpad = cond_bpad(B, TU);
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int c = (int)(i & 15);
-        const size_t rowi = i >> 4;                       // (s * L + l) * n + r
-        const int b = rows[rowi % n];
-        const size_t sl = rowi / n;                       // s * L + l
-        const float4 f0 = *reinterpret_cast<const float4*>(src + rowi * 128 + c * 8);
-        const float4 f1 = *reinterpret_cast<const float4*>(src + rowi * 128 + c * 8 + 4);
-        __half2 h0 = __floats2half2_rn(f0.x, f0.y), h1 = __floats2half2_rn(f0.z, f0.w), h2 = __floats2half2_rn(f1.x, f1.y), h3 = __floats2half2_rn(f1.z, f1.w);
-        uint4 o;
-        o.x = *reinterpret_cast<unsigned*>(&h0); o.y = *reinterpret_cast<unsigned*>(&h1);
-        o.z = *reinterpret_cast<unsigned*>(&h2); o.w = *reinterpret_cast<unsigned*>(&h3);
-        const int tile = b / TU, r = b % TU, half = c >> 3, q = c & 7;
-        const size_t off = (((size_t)first_sample * L + sl) * bpad + (size_t)tile * TU) * 256 + (size_t)half * cond_rows(B, tile, TU) * 128 +
-                           (size_t)r * 128 + (size_t)((q ^ (r & 7)) << 4);
-        *reinterpret_cast<uint4*>(dst + off) = o;
+    static size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * cond_bpad(c.B, c.tc_tile) * 256; }
+    static size_t ring_bytes(const WnConfig& c)
+    {
+        const size_t tiled = (size_t)(c.maxDil + 1) * c.L * ((c.B + c.tc_tile - 1) / c.tc_tile) * TILE;
+        const size_t plain = wn_stream_family.ring_bytes(c);
+        return tiled > plain ? tiled : plain;
     }
-}
-
-// The history ring: each entry (slot x L + layer) holds one 16 KB SW128 tile image per TU utterances (ntiles of them), row
-// r = b mod TU of a tile at bytes [128 r, 128 r + 128) in the channel order publish_x writes (its 16-byte chunks permuted by r & 7).
-// The 16 bytes of channels [8 q, 8 q + 8) of utterance b in entry e:
-__device__ __forceinline__ uint4* tc_ring_chunk(unsigned char* ring, size_t e, int ntiles, int TU, int b, int q)
-{
-    return reinterpret_cast<uint4*>(ring + (e * ntiles + b / TU) * TILE + sw128_offset(b % TU, 8 * q));
-}
-
-// zero utterances rows[i] in every history-ring entry
-__global__ void tc_ring_clear_rows_kernel(unsigned char* __restrict__ ring, const int* __restrict__ rows, int n, int entries, int ntiles, int TU)
-{
-    const size_t total = (size_t)entries * n * 8;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t ei = i >> 3;                         // e * n + r
-        *tc_ring_chunk(ring, ei / n, ntiles, TU, rows[ei % n], (int)(i & 7)) = make_uint4(0, 0, 0, 0);
-    }
-}
-
-// fp16 src [n][batch][64] -> rows 0..batch-1 of entries (t mod slots) * L + layer, t = t_first + j; one thread per 16-byte chunk
-__global__ void tc_put_history_kernel(unsigned char* __restrict__ ring, const uint4* __restrict__ src, int layer, int L, int slots, long long t_first,
-                                      int n, int batch, int ntiles, int TU)
-{
-    const size_t total = (size_t)n * batch * 8;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i >> 3;                        // j * batch + b
-        const long long t = t_first + (long long)(row / batch);
-        *tc_ring_chunk(ring, (size_t)(t % slots) * L + layer, ntiles, TU, (int)(row % batch), (int)(i & 7)) = src[i];
-    }
-}
-
-// the ring -> fp32 [entries][batch][64]
-__global__ void tc_get_history_kernel(float* __restrict__ dst, unsigned char* __restrict__ ring, int entries, int batch, int ntiles, int TU)
-{
-    const size_t total = (size_t)entries * batch * 8;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i >> 3;                        // e * batch + b
-        const int q = (int)(i & 7);
-        const uint4 v = *tc_ring_chunk(ring, row / batch, ntiles, TU, (int)(row % batch), q);
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const float2 f = wn::unpack_h2(w[k]);
-            dst[row * 64 + 8 * q + 2 * k] = f.x;
-            dst[row * 64 + 8 * q + 2 * k + 1] = f.y;
-        }
-    }
-}
+};
 
 // ------------------------------------------------------------------------------------------------ pack
 // blob (fp16, column-major matrices as uploaded) -> tiled / swizzled weight image + fp32 bias block
@@ -307,7 +222,7 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
     auto ring_tile = [&](int t, int l) -> unsigned char* {
         return gring + (((size_t)((t + slot_shift) % slots) * L + l) * ntiles + tile) * (size_t)TILE + (size_t)row0 * 128;
     };
-    // conditioning tile geometry (see tc_cond_kernel): [2 halves][c_rows][128 B]; this CTA's rows of each half land in a ring
+    // conditioning tile geometry (see TcLayout::store_unit): [2 halves][c_rows][128 B]; this CTA's rows of each half land in a ring
     // stage at offsets 0 and ATILE
     const int c_rows = cond_rows(B, tile, tu);
     const uint32_t c_bytes = (uint32_t)c_rows * 128u;
@@ -724,84 +639,7 @@ int pick_nstage()
     return 0;
 }
 
-// the conditioning store and the history ring are laid out per tile of c.tc_tile utterances
-size_t store_bytes(const WnConfig& c) { return (size_t)c.N * c.L * cond_bpad(c.B, c.tc_tile) * 256; }
-
-size_t ring_bytes(const WnConfig& c)
-{
-    const size_t tiled = (size_t)(c.maxDil + 1) * c.L * ((c.B + c.tc_tile - 1) / c.tc_tile) * TILE;
-    const size_t plain = wn_stream_family.ring_bytes(c);
-    return tiled > plain ? tiled : plain;
-}
-
 size_t image_bytes(const WnConfig& c) { return tc_image(c.S, c.L).total; }
-
-cudaError_t cond_convert(const WnConfig& c, void* dst, const float* src_dev, int first_sample, int nsamples, cudaStream_t stream)
-{
-    if (nsamples <= 0) return cudaSuccess;
-    const size_t total = (size_t)nsamples * c.L * c.B * 16;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 4096) blocks = 4096;
-    tc_cond_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(dst), src_dev, first_sample, nsamples, c.L, c.B, c.tc_tile);
-    return cudaGetLastError();
-}
-
-cudaError_t cond_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int nsamples, cudaStream_t stream)
-{
-    if (nsamples <= 0) return cudaSuccess;
-    const size_t total = (size_t)nsamples * c.L * c.B * 16;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 4096) blocks = 4096;
-    tc_cond_readback_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst_dev, static_cast<const unsigned char*>(store), first_sample, nsamples, c.L, c.B, c.tc_tile);
-    return cudaGetLastError();
-}
-
-cudaError_t cond_convert_rows(const WnConfig& c, void* store, const float* src_dev, const int* rows_dev, int n, int first_pos, int num_pos,
-                              cudaStream_t stream)
-{
-    const size_t total = (size_t)num_pos * c.L * n * 16;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 4096) blocks = 4096;
-    tc_cond_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(store), src_dev, rows_dev, n, first_pos, num_pos, c.L, c.B,
-                                                              c.tc_tile);
-    return cudaGetLastError();
-}
-
-cudaError_t ring_clear_rows(const WnConfig& c, void* ring, const int* rows_dev, int n, cudaStream_t stream)
-{
-    const int entries = (c.maxDil + 1) * c.L;
-    const size_t total = (size_t)entries * n * 8;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    tc_ring_clear_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), rows_dev, n, entries,
-                                                                    (c.B + c.tc_tile - 1) / c.tc_tile, c.tc_tile);
-    return cudaGetLastError();
-}
-
-cudaError_t ring_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
-{
-    const size_t total = (size_t)n * batch * 8;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    tc_put_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(static_cast<unsigned char*>(ring), reinterpret_cast<const uint4*>(src), layer, c.L,
-                                                                c.maxDil + 1, t_first, n, batch, (c.B + c.tc_tile - 1) / c.tc_tile, c.tc_tile);
-    return cudaGetLastError();
-}
-
-cudaError_t ring_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
-{
-    const int entries = (c.maxDil + 1) * c.L;
-    const size_t total = (size_t)entries * batch * 8;
-    if (total == 0) return cudaSuccess;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    tc_get_history_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dst, static_cast<unsigned char*>(const_cast<void*>(ring)), entries, batch,
-                                                                (c.B + c.tc_tile - 1) / c.tc_tile, c.tc_tile);
-    return cudaGetLastError();
-}
 
 cudaError_t wn_tc_pack(void* image, const WnParams& p, cudaStream_t stream)
 {
@@ -842,5 +680,7 @@ bool wn_tc_supported(int R_, int S, int A_, int, int)
     return R_ == R && A_ == A && (S == 128 || S == 256);
 }
 
-const WnFamily wn_tc_family = {store_bytes, ring_bytes, image_bytes, cond_convert, cond_readback, ring_clear_rows, cond_convert_rows,
-                               ring_put_history, ring_get_history, wn_tc_pack, wn_launch_tc, true};
+// convert is convert_rows with every row: the whole-store and the per-row paths are one kernel
+const WnFamily wn_tc_family = {TcLayout::store_bytes, TcLayout::ring_bytes, image_bytes, wn_convert<TcLayout>, wn_readback<TcLayout>,
+                               wn_clear_rows<TcLayout>, wn_convert_rows<TcLayout>, wn_put_history<TcLayout>, wn_get_history<TcLayout>, wn_tc_pack,
+                               wn_launch_tc, true};
