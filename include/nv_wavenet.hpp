@@ -204,6 +204,14 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Not in the reference class: after score_stream over prompts [0, P), slot slots[i] continues scoring row rows[i] from the engine's
+     * next sample.  See nvwn_prime_slots_from_score. */
+    bool prime_slots_from_score(const int* rows, const int* slots, int n, const unsigned long long* seeds = NULL, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_prime_slots_from_score(m_engine, rows, slots, n, seeds, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
 
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)

@@ -204,6 +204,21 @@ int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, 
  * scoring and generation calls, the primed history is the same on every engine kind, and it is within the fp16 contract of the
  * fp32 model at that history. */
 int nvwn_prime_from_score(nvwn_engine* e, void* stream);
+/* Prompted continuous batching: prime single slots of a running engine.  With an open scoring stream of batch_size Bs and next sample
+ * P >= 1, and the engine's next sample t0: for each i, slot slots[i] starts an utterance whose samples [0, P) are scoring row rows[i],
+ * its local time tau at engine time t0 - P + tau, so that generation from t0 continues it at tau = P.  The slots' history rows are
+ * cleared, each layer's last d_l inputs of their rows go into them, the rows' last two codes become the fed-back indices, and the
+ * slots' selector origin becomes t0 - P and their key seeds[i] (seeds NULL: 0): the same effect on those slots as nvwn_restart_slots
+ * at t0 - P followed by a prime, so nvwn_set_selectors_random_slots draws counter tau, what an engine of that utterance alone draws.
+ * A per-slot call (whole-batch runs until nvwn_reset_history).  The scoring stream stays open and unchanged, so rows of longer prompts
+ * can be scored on and primed later; next_t does not move; no other slot changes.  Stream-ordered on `stream`.
+ * The first such call since nvwn_reset_history at t0 < maxDil zeroes the history entries of the times [t0 - maxDil - 1, 0) in every
+ * slot, and from then until nvwn_reset_history every launch reads the history at every step (the rows that started at sample 0 read
+ * zeros where they staged zeros: the same bits, DESIGN.md §6).
+ * Refused with NVWN_EINVAL, changing nothing: NULL rows or slots, no open scoring stream, rows outside [0, Bs) or given twice, a bad
+ * slot list (1 <= n <= B, distinct slots in [0, B)).  NVWN_FP16 engines only (else NVWN_EUNSUPPORTED).  Numerics as
+ * nvwn_prime_from_score. */
+int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slots, int n, const unsigned long long* seeds, void* stream);
 
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);

@@ -87,6 +87,14 @@ struct WnFamily {
     // as fp32 [(maxDil+1)][L][batch][R] (device), slot by slot, at that stride.
     cudaError_t (*put_history)(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream);
     cudaError_t (*get_history)(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream);
+    // Per-slot history writers (priming single slots, DESIGN.md §6), at the engine's batch stride, for absolute times t that may be
+    // negative, in ring slot ((t mod M) + M) mod M, M = maxDil + 1.  put_history_rows writes rows src_rows_dev[i] of fp16 src
+    // [n_t][src_batch][R] (device), the values x_layer[t] of times [t_first, t_first + n_t), n_t <= M, into ring rows rows_dev[i]
+    // (n distinct rows in [0, c.B)), and no other byte; clear_times zeroes rows 0..c.B-1 of every layer's entries of times
+    // [t_first, t_first + n_t), n_t <= M, and no other byte.
+    cudaError_t (*put_history_rows)(const WnConfig& c, void* ring, const __half* src, int src_batch, const int* src_rows_dev, const int* rows_dev,
+                                    int n, int layer, long long t_first, int n_t, cudaStream_t stream);
+    cudaError_t (*clear_times)(const WnConfig& c, void* ring, long long t_first, int n_t, cudaStream_t stream);
     cudaError_t (*pack)(void* image, const WnParams& p, cudaStream_t stream);      // weight blob -> image; NULL: the kernels read the blob
     cudaError_t (*launch)(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info);
     bool whole_batch;                               // a run must take all c.B utterances
@@ -145,6 +153,10 @@ cudaError_t wn_restart_rows(const int* rows, int n, const unsigned long long* se
 // fed-back indices of rows b < n from a scoring stream's codes [n][2] (the codes of steps t-2 and t-1 of its next sample t):
 // yPrev[b] = codes[b][0], yCur[b] = codes[b][1]
 cudaError_t wn_feedback_from_codes(const int* codes, int n, int* yPrev, int* yCur, cudaStream_t stream);
+// state of slots slots[0..n) primed from scoring rows rows[i]: yPrev = codes[rows[i]][0], yCur = codes[rows[i]][1], origin = t_origin,
+// seed = seeds[i] (seeds NULL: 0)
+cudaError_t wn_prime_rows(const int* codes, const int* rows, const int* slots, int n, const unsigned long long* seeds, long long t_origin, int* yPrev,
+                          int* yCur, long long* origin, unsigned long long* seed, cudaStream_t stream);
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream);
 

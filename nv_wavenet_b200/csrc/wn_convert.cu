@@ -172,6 +172,27 @@ cudaError_t wn_feedback_from_codes(const int* codes, int n, int* yPrev, int* yCu
     return cudaGetLastError();
 }
 
+// the per-slot prime's state: restart_rows_kernel with the fed-back indices of feedback_from_codes_kernel
+__global__ void prime_rows_kernel(const int* __restrict__ codes, const int* __restrict__ rows, const int* __restrict__ slots, int n,
+                                  const unsigned long long* __restrict__ seeds, long long t_origin, int* yPrev, int* yCur, long long* origin,
+                                  unsigned long long* seed)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int b = slots[i], r = rows[i];
+        yPrev[b] = codes[2 * r];
+        yCur[b] = codes[2 * r + 1];
+        origin[b] = t_origin;
+        seed[b] = seeds ? seeds[i] : 0ull;
+    }
+}
+cudaError_t wn_prime_rows(const int* codes, const int* rows, const int* slots, int n, const unsigned long long* seeds, long long t_origin, int* yPrev,
+                          int* yCur, long long* origin, unsigned long long* seed, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    prime_rows_kernel<<<(n + 255) / 256, 256, 0, stream>>>(codes, rows, slots, n, seeds, t_origin, yPrev, yCur, origin, seed);
+    return cudaGetLastError();
+}
+
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream)
 {

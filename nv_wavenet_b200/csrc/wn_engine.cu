@@ -99,6 +99,12 @@ struct nvwn_engine : WnConfig {
     // the batch_size of the last nvwn_prime_from_score since the last nvwn_reset_history, 0 if none: the plain history ring was
     // written at that stride, so until the next reset a run must take that batch
     int prime_bs = 0;
+    // per-slot primes (nvwn_prime_slots_from_score): the scoring rows of the last call (device, [B]); and whether a slot was primed
+    // before sample maxDil since the last nvwn_reset_history.  Such a slot's history holds real values at times the kernels would
+    // skip as "before the start" (t < d_l), so while this is set every launch reads the ring at every step (fill_params), and the
+    // entries of the negative times were zeroed in every row.
+    int* prime_rows = nullptr;
+    bool early_prime = false;
 
     void* image = nullptr;                   // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
@@ -290,7 +296,7 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, long long t
     p.L = e->L; p.R = e->R; p.S = e->S; p.A = e->A; p.maxDil = e->maxDil;
     p.B = batch; p.N = num_samples; p.init_sample = init_sample; p.count = count;
     p.ring_slot = (int)(t_abs % (e->maxDil + 1));
-    p.hist_t = (int)(t_abs < e->maxDil ? t_abs : e->maxDil);
+    p.hist_t = (int)(t_abs < e->maxDil && !e->early_prime ? t_abs : e->maxDil);
     p.tanhEmbed = e->tanhEmbed; p.dump = dump;
     p.embPrev = e->blob + e->o_embPrev; p.embCur = e->blob + e->o_embCur;
     p.Wprev = e->blob + e->o_Wprev; p.Wcur = e->blob + e->o_Wcur; p.Wres = e->blob + e->o_Wres; p.Wskip = e->blob + e->o_Wskip;
@@ -439,6 +445,7 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     ALLOC(e->seed, Bz * sizeof(unsigned long long));
     ALLOC(e->slot_rows, Bz * sizeof(int));
     ALLOC(e->slot_seeds, Bz * sizeof(unsigned long long));
+    ALLOC(e->prime_rows, Bz * sizeof(int));
     if (e->stage_elems) ALLOC(e->stage_dev, e->stage_elems * sizeof(float));
     if (e->family->pack) ALLOC(e->image, e->family->image_bytes(*e));
 #undef ALLOC
@@ -462,7 +469,7 @@ int nvwn_destroy(nvwn_engine* e)
     if (!e) return 0;
     void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
                     e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch,
-                    e->origin, e->seed, e->slot_rows, e->slot_seeds, e->row_stage, e->cs_scratch, e->cs_frames, e->cs_tables};
+                    e->origin, e->seed, e->slot_rows, e->slot_seeds, e->row_stage, e->cs_scratch, e->cs_frames, e->cs_tables, e->prime_rows};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
@@ -756,6 +763,7 @@ int nvwn_reset_history(nvwn_engine* e)
     e->next_t = 0;
     e->slot_rows_used = false;
     e->prime_bs = 0;
+    e->early_prime = false;
     e->cs_T.assign(e->B, 0);                      // attached frames: their starts are absolute samples of the old timeline
     return 0;
 }
@@ -1216,6 +1224,52 @@ int nvwn_prime_from_score(nvwn_engine* e, void* stream)
     CK(wn_feedback_from_codes(reinterpret_cast<const int*>(e->score_scratch + o.codes), Bs, e->yPrev, e->yCur, st));
     e->next_t = P;
     e->prime_bs = Bs;
+    return 0;
+}
+
+int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slots, int n, const unsigned long long* seeds, void* stream)
+{
+    const std::string who = "nvwn_prime_slots_from_score";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score, so only they can be primed");
+    if (!rows) return fail(NVWN_EINVAL, who + ": rows is NULL");
+    if (e->score_next < 1)
+        return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompts with nvwn_score_stream "
+                                       "from first_sample = 0 first");
+    int rc = check_slots(e, who.c_str(), slots, n);
+    if (rc != 0) return rc;
+    const int Bs = e->score_bs;
+    std::vector<char> seen(Bs, 0);
+    for (int i = 0; i < n; i++) {
+        if (rows[i] < 0 || rows[i] >= Bs)
+            return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is outside [0, " + std::to_string(Bs) + ") (the scoring stream's batch_size)");
+        if (seen[rows[i]]) return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is given twice");
+        seen[rows[i]] = 1;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = take_slots(e, who.c_str(), slots, n, st)) || (rc = copy_snapshot(e->prime_rows, rows, n, st))) return rc;
+    if (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st))) return rc;
+    const long long P = e->score_next, t0 = e->next_t, origin = t0 - P;
+    const int M = e->maxDil + 1, T = e->score_T, R = e->R, L = e->L;
+    if (t0 < e->maxDil && !e->early_prime) {
+        // from now on every launch reads the ring at every step: the entries of the negative times, which no row has written since
+        // the reset, must read as the zeros the kernels stage for "before the start"
+        CK(e->family->clear_times(*e, e->ring, t0 - M, (int)(M - t0), st));
+        e->early_prime = true;
+    }
+    // what nvwn_restart_slots at t0 - P does to these slots, then nvwn_prime_from_score of their rows with local time tau at engine
+    // time t0 - P + tau: layer l's front of times tau in [max(0, P - d_l), P)
+    CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
+    const ScoreScratch o = score_scratch_layout(e, T);
+    const __half* xh = reinterpret_cast<const __half*>(e->score_scratch + o.xh);
+    for (int l = 0; l < L; l++) {
+        const int d = wn_score_dilation(l, e->maxDil);
+        const long long tau = P - d > 0 ? P - d : 0;
+        const __half* src = xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R) + (size_t)(tau - (P - d)) * Bs * R;
+        CK(e->family->put_history_rows(*e, e->ring, src, Bs, e->prime_rows, e->slot_rows, n, l, origin + tau, (int)(P - tau), st));
+    }
+    CK(wn_prime_rows(reinterpret_cast<const int*>(e->score_scratch + o.codes), e->prime_rows, e->slot_rows, n, seeds ? e->slot_seeds : nullptr, origin,
+                     e->yPrev, e->yCur, e->origin, e->seed, st));
     return 0;
 }
 

@@ -6,8 +6,8 @@
 //   STORE_UNIT, RING_UNIT                 channels per unit; a unit is a WnVec<TD, UNIT>
 //   store_unit(c, store, sl, b, k)        unit k of row b of the store at sl = position * L + layer, at the engine's batch c.B
 //   ring_unit(c, ring, e, stride, b, k)   unit k of row b of ring entry e = slot * L + layer; stride is the batch stride of the plain
-//                                         ring (the engine's B for clear_rows, the run's batch for the history writers), which the
-//                                         tiled layouts ignore
+//                                         ring (the engine's B for clear_rows and the per-slot writers, the run's batch for the
+//                                         whole-batch history writers), which the tiled layouts ignore
 //   store_bytes(c), ring_bytes(c)
 // Every operation below finds its units through these two functions and nothing else.  So convert_rows writes what convert writes,
 // bit for bit, and a row operation touches the units of its rows and no other byte.
@@ -120,6 +120,42 @@ __global__ void wn_put_history_kernel(size_t total, WnConfig c, void* ring, cons
     }
 }
 
+// The ring slot of absolute time t, which may be negative here (a slot primed before the engine's sample 0, DESIGN.md §6):
+// ((t mod M) + M) mod M, M = maxDil + 1.  wn_put_history_kernel's t % M is only right for t >= 0.
+__device__ __forceinline__ int wn_ring_slot(long long t, int M) { return (int)((t % M + M) % M); }
+
+// fp16 rows src_rows[r] of a front src [n_t][src_batch][R] -> ring rows rows[r] of entries slot(t) * L + layer, t = t_first + j, at
+// the engine's batch stride
+template <class Lay>
+__global__ void wn_put_history_rows_kernel(size_t total, WnConfig c, void* ring, const __half* __restrict__ src, int src_batch,
+                                           const int* __restrict__ src_rows, const int* __restrict__ rows, int n, int layer, long long t_first)
+{
+    constexpr int U = Lay::RING_UNIT;
+    const int units = c.R / U, lg = wn_log2(units);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> lg;                                   // j * n + r
+        const int r = (int)(row % n), k = (int)i & (units - 1);
+        const size_t j = row / n;
+        *Lay::ring_unit(c, ring, (size_t)wn_ring_slot(t_first + (long long)j, c.maxDil + 1) * c.L + layer, c.B, rows[r], k) =
+            wn_vec_cast<typename Lay::TD>(wn_load(reinterpret_cast<const WnVec<__half, U>*>(src) + ((j * src_batch + src_rows[r]) << lg) + k));
+    }
+}
+
+// every row 0..B-1 of every layer's entries slot(t), t in [t_first, t_first + n_t), zeroed at the engine's batch stride
+template <class Lay>
+__global__ void wn_clear_times_kernel(size_t total, WnConfig c, void* ring, long long t_first)
+{
+    const int units = c.R / Lay::RING_UNIT, lg = wn_log2(units);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> lg;                                   // (j * L + l) * B + b
+        const size_t jl = row / c.B;
+        const int l = (int)(jl % c.L);
+        const long long t = t_first + (long long)(jl / c.L);
+        *Lay::ring_unit(c, ring, (size_t)wn_ring_slot(t, c.maxDil + 1) * c.L + l, c.B, (int)(row % c.B), (int)i & (units - 1)) =
+            WnVec<typename Lay::TD, Lay::RING_UNIT>{};
+    }
+}
+
 // every ring entry -> fp32 [entries][batch][R], at the batch stride `batch`
 template <class Lay>
 __global__ void wn_get_history_kernel(size_t total, WnConfig c, float* __restrict__ dst, const void* ring, int batch)
@@ -160,6 +196,18 @@ template <class Lay>
 cudaError_t wn_put_history(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream)
 {
     return wn_layout_launch(wn_put_history_kernel<Lay>, (size_t)n * batch * (c.R / Lay::RING_UNIT), stream, c, ring, src, layer, t_first, batch);
+}
+template <class Lay>
+cudaError_t wn_put_history_rows(const WnConfig& c, void* ring, const __half* src, int src_batch, const int* src_rows_dev, const int* rows_dev, int n,
+                                int layer, long long t_first, int n_t, cudaStream_t stream)
+{
+    return wn_layout_launch(wn_put_history_rows_kernel<Lay>, (size_t)n_t * n * (c.R / Lay::RING_UNIT), stream, c, ring, src, src_batch, src_rows_dev,
+                            rows_dev, n, layer, t_first);
+}
+template <class Lay>
+cudaError_t wn_clear_times(const WnConfig& c, void* ring, long long t_first, int n_t, cudaStream_t stream)
+{
+    return wn_layout_launch(wn_clear_times_kernel<Lay>, (size_t)n_t * c.L * c.B * (c.R / Lay::RING_UNIT), stream, c, ring, t_first);
 }
 template <class Lay>
 cudaError_t wn_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)

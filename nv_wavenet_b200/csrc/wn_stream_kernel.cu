@@ -728,6 +728,7 @@ bool wn_stream_supported(int R, int S, int A, bool)
 
 // The kernels read the weight blob and the plain conditioning store; any batch up to the engine's.  convert and readback are
 // contiguous conversions (wn_convert.cu): the plain store already is the source layout, and an fp32 convert also copies from host
-// memory, which no kernel can read.  put_history is fp16 only: the engine primes no other precision.
+// memory, which no kernel can read.  put_history, put_history_rows and clear_times are fp16 only: the engine primes no other precision.
 const WnFamily wn_stream_family = {plain_store_bytes, plain_ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, plain_clear_rows,
-                                   plain_convert_rows, wn_put_history<PlainH>, plain_get_history, nullptr, wn_launch_stream, false};
+                                   plain_convert_rows, wn_put_history<PlainH>, plain_get_history, wn_put_history_rows<PlainH>, wn_clear_times<PlainH>,
+                                   nullptr, wn_launch_stream, false};

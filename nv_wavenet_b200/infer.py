@@ -353,6 +353,22 @@ class NVWavenetInfer:
         with the scoring stream's batch_size bs.  The scoring stream stays open.  Asynchronous on `stream`; see nvwn_prime_from_score."""
         check(self._l.nvwn_prime_from_score(self._h, _stream(stream)), "primeFromScore")
 
+    def prime_slots_from_score(self, rows, slots, seeds=None, stream=None):
+        """After score_stream over prompts [0, P): slot slots[i] starts an utterance whose samples [0, P) are scoring row rows[i],
+        continued by generation from the engine's next sample t0 (its sample P at t0).  seeds (one per slot, None = 0) key the slots'
+        selectors as restart_slots does.  The scoring stream stays open.  Asynchronous on `stream`; see nvwn_prime_slots_from_score."""
+        p, s = self._slots(slots)
+        r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1)).astype(np.int32)
+        if r.size != s.size:
+            raise ValueError(f"prime_slots_from_score: {s.size} slots but {r.size} rows")
+        k = None
+        if seeds is not None:
+            k = np.ascontiguousarray([int(v) & (2 ** 64 - 1) for v in seeds], dtype=np.uint64)
+            if k.size != s.size:
+                raise ValueError(f"prime_slots_from_score: {s.size} slots but {k.size} seeds")
+        check(self._l.nvwn_prime_slots_from_score(self._h, C.c_void_p(r.ctypes.data), p, s.size, None if k is None else C.c_void_p(k.ctypes.data),
+                                                  _stream(stream)), "primeSlotsFromScore")
+
     def _score(self, audio, num_samples, batch_size, logits, what, call):
         """audio[:batch_size, :num_samples] as int32 and the outputs of score() in matching memory; call(audio, n, bs, logp, logits)
         with their pointers."""

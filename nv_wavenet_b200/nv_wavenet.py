@@ -244,24 +244,64 @@ class NVWaveNet:
             eng.run_stream(g0, k, batch_size)
             eng.get_yout_stream(samples[:, g0:g0 + k], g0, k)
 
-    def infer_many(self, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None):
+    def infer_many(self, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None, prompts=None):
         """Continuous batching: generates a queue of utterances of different lengths through one engine of `slots` utterances and
         `window` samples.  cond_inputs: per utterance, conditioning [2R][L][n_u] (channels x num_layers x samples); seeds: one
         integer per utterance (device selectors, as infer(seed=...)).  Returns int32 CUDA tensors [n_u], each bit-identical to
         infer() of that utterance alone with its seed.  The engine runs in windows of `window` samples; at each window boundary
         the slots whose utterance has ended take the next queued ones in arrival order (plan_slots).  A slot with nothing to do
-        keeps running on stale inputs and its output is discarded.  timing: a dict, or None; if given, receives the GPU seconds
-        spent in restarts and per-slot uploads ("restart_upload_s") and in generation ("generate_s")."""
+        keeps running on stale inputs and its output is discarded.
+        prompts: None, or per utterance None or int mu-law codes [P_u], 1 <= P_u < n_u (host or CUDA tensor), fp16 only; cond_inputs
+        still cover the whole utterance.  A prompted utterance generates n_u - P_u samples (the schedule is plan_slots of those),
+        and is bit-identical to infer(cond_u, seed=s_u, fp16=True, prompt=p_u) of it alone: at the boundary where it starts, the
+        prompted utterances starting there are scored together through the engine's own conditioning store (nvwn_score_stream) and
+        each slot is primed from its row once its prompt has been scored (nvwn_prime_slots_from_score).  The first P_u outputs
+        are the prompt.  timing: a dict, or None; if given, receives the GPU seconds spent in restarts and per-slot uploads
+        ("restart_upload_s"), in generation ("generate_s") and in scoring and priming prompts ("prime_s")."""
         if len(cond_inputs) != len(seeds):
             raise AssertionError(f"{len(cond_inputs)} utterances but {len(seeds)} seeds")
         for c in cond_inputs:
             if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * self.R, self.num_layers):
                 raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
         lengths = [int(c.size(2)) for c in cond_inputs]
-        plan = plan_slots(lengths, slots, window)
-        windows = _windows(plan, lengths, window)
+        prompts = self._slot_prompts(prompts, lengths, fp16)
+        skip = [0 if p is None else int(p.numel()) for p in prompts]                  # samples before the generated ones
+        plan = plan_slots([n - P for n, P in zip(lengths, skip)], slots, window)
+        windows = _windows(plan, [n - P for n, P in zip(lengths, skip)], window)
         eng = self._engine(slots, window, fp16)
         eng.reset_history()
+        primes = []
+
+        def prime(k):
+            # the prompted utterances starting at this boundary, by prompt length: scoring rows 0..g-1, in pieces that end at each
+            # distinct P_u and at multiples of the window (the store holds one window, free now that the last one was generated)
+            first, _, starting, _ = windows[k]
+            group = sorted((u for u in starting if prompts[u] is not None), key=lambda u: skip[u])
+            if not group:
+                return
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if timing is not None else None
+            if ev:
+                ev[0].record()
+            g, a = len(group), 0
+            for end in sorted({skip[u] for u in group}):
+                while a < end:
+                    m = min(end - a, window - a % window)
+                    # rows whose prompt has ended are scored on padding (codes 128, zero conditioning); their results are unused
+                    lh = torch.zeros((m, self.num_layers, g, 2 * self.R), dtype=torch.float32, device="cuda")
+                    codes = torch.full((g, m), 128, dtype=torch.int32, device="cuda")
+                    for j, u in enumerate(group):
+                        e = min(skip[u], a + m)
+                        if e > a:
+                            lh[:e - a, :, j].copy_(cond_inputs[u][:, :, a:e].permute(2, 1, 0))
+                            codes[j, :e - a] = prompts[u][a:e]
+                    eng.set_conditioning_slots(lh, list(range(g)), a)
+                    eng.score_stream(codes, a)
+                    a += m
+                done = [j for j, u in enumerate(group) if skip[u] == end]
+                eng.prime_slots_from_score(done, [plan[group[j]][0] for j in done], [seeds[group[j]] for j in done])
+            if ev:
+                ev[1].record()
+                primes.append(ev)
 
         def condition(k):
             first, count, _, live = windows[k]
@@ -269,15 +309,40 @@ class NVWaveNet:
                 # this window's conditioning of the live slots, [count][L][slots][2R], zero past an utterance's end
                 lh = torch.zeros((count, self.num_layers, len(live), 2 * self.R), dtype=torch.float32, device="cuda")
                 for j, (_, u, a, m) in enumerate(live):
-                    lh[:m, :, j].copy_(cond_inputs[u][:, :, a:a + m].permute(2, 1, 0))
+                    lh[:m, :, j].copy_(cond_inputs[u][:, :, skip[u] + a:skip[u] + a + m].permute(2, 1, 0))
                 eng.set_conditioning_slots(lh, [s for s, _, _, _ in live], first)
 
-        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition)
+        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, before=prime, prompts=prompts)
         torch.cuda.synchronize()
         if timing is not None:
             timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
             timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
+            timing["prime_s"] = sum(a.elapsed_time(b) for a, b in primes) / 1e3
         return outs
+
+    def _slot_prompts(self, prompts, lengths, fp16):
+        """infer_many's prompts checked: per utterance None or int32 CUDA codes [P_u], 1 <= P_u < n_u, each in [0, A), and fp16 if any
+        is given.  Returns the list (all None without prompts)."""
+        if prompts is None:
+            return [None] * len(lengths)
+        if len(prompts) != len(lengths):
+            raise AssertionError(f"{len(lengths)} utterances but {len(prompts)} prompts")
+        out = []
+        for u, p in enumerate(prompts):
+            if p is None:
+                out.append(None)
+                continue
+            p = torch.as_tensor(p)
+            if p.dim() != 1 or not 1 <= p.numel() < lengths[u]:
+                raise AssertionError(f"prompt {u} must be [P] with 1 <= P < {lengths[u]} (its utterance's samples); got {tuple(p.shape)}")
+            if p.dtype.is_floating_point or p.dtype.is_complex or p.dtype == torch.bool:
+                raise AssertionError(f"prompt {u} must hold integer mu-law codes; got {p.dtype}")
+            if int(p.min()) < 0 or int(p.max()) >= self.A:
+                raise AssertionError(f"prompt {u} holds codes outside [0, {self.A})")
+            out.append(p)
+        if any(p is not None for p in out) and not fp16:
+            raise AssertionError("prompts need fp16=True: they are scored by the fp16 scorer")
+        return [None if p is None else p.to(device="cuda", dtype=torch.int32) for p in out]
 
     def infer_many_from_features(self, features, seeds, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots=64,
                                  window=4096, fp16=False, timing=None):
@@ -365,23 +430,35 @@ class NVWaveNet:
             raise AssertionError(f"need upsampling window >= stride >= 1; got {window_u}, {stride}")
         return Cc, lr
 
-    def _serve(self, eng, plan, windows, lengths, seeds, timed, condition, after=None):
-        """The window loop of infer_many and infer_many_from_features on the current stream.  Per window k: condition(k), which
-        leaves the conditioning of the window's live slots in the engine or makes the stream wait for it; the restarts of the
-        slots whose utterance starts there; their selectors; the launch; the outputs; then after(k).  Returns the outputs and, if
-        timed, per window four events around those steps (before condition, restarts, launch, and after the outputs)."""
+    def _serve(self, eng, plan, windows, lengths, seeds, timed, condition, after=None, before=None, prompts=None):
+        """The window loop of infer_many and infer_many_from_features on the current stream.  Per window k: before(k), which
+        primes the prompted slots that start there; condition(k), which leaves the conditioning of the window's live slots in the
+        engine or makes the stream wait for it; the restarts of the other slots whose utterance starts there; their selectors;
+        the launch; the outputs; then after(k).  prompts: None, or per utterance its prompt [P_u] (CUDA) or None: the output's
+        first P_u samples, generated ones after them (windows and lengths count generated samples; outputs have `lengths`).
+        Returns the outputs and, if timed, per window four events around those steps (before condition, restarts, launch, and
+        after the outputs)."""
+        prompts = prompts or [None] * len(lengths)
         outs = [torch.empty(n, dtype=torch.int32, device="cuda") for n in lengths]
+        skip = []
+        for o, p in zip(outs, prompts):
+            skip.append(0 if p is None else p.numel())
+            if p is not None:
+                o[:p.numel()].copy_(p)
         stage = torch.empty((eng.B, eng.N), dtype=torch.int32, device="cuda")
         events = []
         for k, (first, count, starting, live) in enumerate(windows):
+            if before is not None:
+                before(k)
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timed else None
             if ev:
                 ev[0].record()
             condition(k)
             if ev:
                 ev[1].record()
-            if starting:
-                eng.restart_slots([plan[u][0] for u in starting], [seeds[u] for u in starting])
+            restart = [u for u in starting if prompts[u] is None]
+            if restart:
+                eng.restart_slots([plan[u][0] for u in restart], [seeds[u] for u in restart])
             eng.set_selectors_random_slots(first, count)
             if ev:
                 ev[2].record()
@@ -389,7 +466,7 @@ class NVWaveNet:
             pos = first % eng.N                                       # windows start at multiples of the window: no wrap inside
             eng.get_yout(stage, pos, count)
             for s, u, a, m in live:
-                outs[u][a:a + m].copy_(stage[s, pos:pos + m])
+                outs[u][skip[u] + a:skip[u] + a + m].copy_(stage[s, pos:pos + m])
             if ev:
                 ev[3].record()
                 events.append(ev)
