@@ -159,6 +159,8 @@ __device__ __forceinline__ void ldg_nc_v4_if(uint4& d, const void* p, bool pred)
 __device__ __forceinline__ void stg_v2(void* p, uint32_t a, uint32_t b) { asm volatile("st.global.v2.u32 [%0], {%1,%2};" ::"l"(p), "r"(a), "r"(b) : "memory"); }
 __device__ __forceinline__ void stg_b32(void* p, uint32_t a) { asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(a) : "memory"); }
 __device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, %0;" ::"n"(NCT) : "memory"); }
+// the cluster kernel's chain CTA: the compute warps and the sync warp
+__device__ __forceinline__ void bar_chain() { asm volatile("bar.sync 2, %0;" ::"n"(NCT + 32) : "memory"); }
 using wn::pack_h2;
 using wn::unpack_h2;
 __device__ __forceinline__ uint32_t u32(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
@@ -944,6 +946,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
 //                   Zs and Za, softmax, sampling
 //   rank 2 "prep":  (Bh + Lh) + Wprev . x[t-d] of the steps to come, up to NAP ahead;  ring pieces Wprev_l (16 KB)
 //                   output columns 128-255 of Zs and Za, between two of its steps
+// In the chain CTA a sync warp does every mbarrier wait and hand-back of the layer loop and enters the compute warps' named barriers
+// behind what it saw land, so that a compute warp's layer step is its loads, HMMAs, gate, residual and the two barriers.
 // The output weights stay resident: every compute thread of the tail and prep CTAs loads the B fragments of its two n-tiles once, at
 // kernel start, Wzs into registers (S / 4) and Wza into its CTA's shared memory (64 KB per CTA).
 // Distributed shared memory carries six flows, all as st.async with complete_tx on a transaction barrier that the receiver arms
@@ -1019,6 +1023,7 @@ struct CfgC {
     static_assert(O_BAR + B_END <= SMEM, "the mbarriers outgrow their reservation");
 };
 constexpr int NCL = 3;                       // CTAs per cluster
+constexpr int NTC = NT + 32;                 // threads of a cluster CTA: + the chain CTA's sync warp (idle in the tail and prep CTAs)
 
 __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank)
 {
@@ -1088,7 +1093,7 @@ struct ClusterCta {
 // Their B fragments (lat_pack_kernel: piece q of a matrix = k-step pairs [q OJP, (q+1) OJP) of all 32 n-tiles, fragment
 // (n-tile OJP + jp) x 512 + lane x 16) are loaded once, at kernel start: Wzs into registers (S / 4 per thread), Wza into this
 // CTA's ZA region, where every thread reads back only the 16 B it stored itself (fragment (2w + i) x A/32 + jp).  Wza resident
-// in registers as well would not fit: nine warps leave 168 registers per thread (three warps share a sub-partition's 64 KB),
+// in registers as well would not fit: ten warps leave 168 registers per thread (three warps share a sub-partition's 64 KB),
 // and the tail's skip loop and the prep's step loop would spill ~300 B at S = 256.
 template <int S, int TR>
 __device__ __forceinline__ void load_out_w(const ClusterCta& c, uint4 (&zsw)[2][S / 32], const uint32_t half)
@@ -1247,10 +1252,41 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
                     tma_load_1d(sm + M::C_RING + sl * M::PIECE0 + 16384, img + (size_t)l * im.layer_bytes + C::W_RES, 8192, s_full + 8 * sl);
                 }
         }
-    } else {
+    } else if (w == NCW + 1) {
+        // Sync warp: every mbarrier of the layer loop, so that the compute warps pass only their two named barriers per step.  Its
+        // lane 0 enters a barrier once what the compute warps will read behind it has landed, and answers for what they have read
+        // before it:
+        //   before the x barrier of step n: ring piece n (Wcur, Wres) is full; the tail's h buffer n % NHB is free (it has read tile
+        //     n - NHB), so that every compute thread sends its words of h tile n with st.async behind that barrier;
+        //   after it: pre-activation tile n has been read (behind the h barrier of step n - 1): re-armed, handed back to the prep CTA;
+        //   before the h barrier of step n: pre-activation tile n + 1 is full (the compute warps read it behind that barrier);
+        //   after it: ring piece n has been read (empty).
+        const int nsteps = (t_end - t_begin) * L;
+        const uint32_t r_apfree = mapa_u32(s_apfree, 2);
+        if (lane == 0 && nsteps > 0) mbar_wait(s_apfull, 0);
+        bar_chain();
+        for (int n = 0; n < nsteps; n++) {
+            const uint32_t b = (uint32_t)n % M::NAP, hb = (uint32_t)n % M::NHB;
+            if (lane == 0) {
+                mbar_wait(s_full + 8 * (n & 1), ((uint32_t)n >> 1) & 1);
+                mbar_wait(s_hfree + 8 * hb, (((uint32_t)n / M::NHB) & 1) ^ 1);
+            }
+            __syncwarp();
+            bar_chain();                                   // x barrier of step n
+            if (lane == 0) {
+                mbar_arrive_expect_tx(s_apfull + 8 * b, M::AP);    // armed for the tile NAP steps on, before the buffer goes back
+                mbar_arrive_remote(r_apfree + 8 * b);
+                if (n + 1 < nsteps) mbar_wait(s_apfull + 8 * ((uint32_t)(n + 1) % M::NAP), ((uint32_t)(n + 1) / M::NAP) & 1);
+            }
+            __syncwarp();
+            bar_chain();                                   // h barrier of step n
+            if (lane == 0) mbar_arrive(s_empty + 8 * (n & 1));
+        }
+    } else if (w < NCW) {
         const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u;
         unsigned char* gring = static_cast<unsigned char*>(p.ring) + (size_t)tile * 2048 + hw4;
         const int cw = 8 * w + 2 * t4;
+        const int nsteps = (t_end - t_begin) * L;
         const uint32_t o_t0 = (uint32_t)(w * 2) * 512 + lane16, o_g0 = (uint32_t)((8 + w) * 2) * 512 + lane16, o_res = 16384u + (uint32_t)(w * 2) * 512 + lane16;
         const uint32_t r_hbuf = mapa_u32(sm + M::T_HBUF + xchg, 1);            // this thread's slot of the tail CTA's h tiles
         const uint32_t r_hfull = mapa_u32(s_hfull, 1);
@@ -1260,42 +1296,30 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
         float accp[2][4];
         float2 brn = make_float2(0.f, 0.f);
         float xres[4] = {0.f, 0.f, 0.f, 0.f};
-        int t1 = t_begin, l1 = 0;                          // the coming step (number pn)
-        uint32_t pn = 0;
-        // accp <- (Bh + Lh) + Wprev . x[t-d] of the coming step: computed by the prep CTA, read from this CTA's shared memory
-        auto prep = [&](const bool ap_ok) {
-            if (t1 < t_end) {
-                const uint2 b2 = lds64(s_bias + l1 * 1024 + 16);
-                if (!ap_ok) mbar_wait(s_apfull + 8 * (pn % M::NAP), (pn / M::NAP) & 1);
-                const uint4 a0 = lds128(s_ap + (pn % M::NAP) * M::AP);
-                brn = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
-                if (TR == TU) {
-                    const uint4 a1 = lds128(s_ap + (pn % M::NAP) * M::AP + 16);
-                    accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
-                    accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
-                } else {                                   // row g only: tanh pair, sigmoid pair
-                    accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[1][0] = __uint_as_float(a0.z); accp[1][1] = __uint_as_float(a0.w);
-                    accp[0][2] = accp[0][3] = accp[1][2] = accp[1][3] = 0.f;
-                }
-                // the tile has been read: arm its barrier for the tile NAP steps on (one thread, ordered before this warp's "free"
-                // signal), then hand the buffer back to the prep CTA
-                if (tid == 0) mbar_arrive_expect_tx(s_apfull + 8 * (pn % M::NAP), M::AP);
-                release_remote(s_apfree + 8 * (pn % M::NAP), 2, lane);
+        // accp <- (Bh + Lh) + Wprev . x[t-d] of step n (layer l), computed by the prep CTA; brn <- Bres of layer l
+        auto load_ap = [&](const uint32_t n, const int l) {
+            const uint2 b2 = lds64(s_bias + l * 1024 + 16);
+            const uint4 a0 = lds128(s_ap + (n % M::NAP) * M::AP);
+            brn = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
+            if (TR == TU) {
+                const uint4 a1 = lds128(s_ap + (n % M::NAP) * M::AP + 16);
+                accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[0][2] = __uint_as_float(a0.z); accp[0][3] = __uint_as_float(a0.w);
+                accp[1][0] = __uint_as_float(a1.x); accp[1][1] = __uint_as_float(a1.y); accp[1][2] = __uint_as_float(a1.z); accp[1][3] = __uint_as_float(a1.w);
+            } else {                                       // row g only: tanh pair, sigmoid pair
+                accp[0][0] = __uint_as_float(a0.x); accp[0][1] = __uint_as_float(a0.y); accp[1][0] = __uint_as_float(a0.z); accp[1][1] = __uint_as_float(a0.w);
+                accp[0][2] = accp[0][3] = accp[1][2] = accp[1][3] = 0.f;
             }
-            pn++;
-            if (++l1 == L) { l1 = 0; t1++; }
         };
-        {   // prologue: previous-index rows of the first sample; staging of steps 0, 1, 2; pre-activation of step 0
+        {   // prologue: previous-index rows of the first sample
             const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
             sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TR + g] * 32 + 4 * w + t4]);
             if (TR == TU) sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
         }
         StepIt it0{t_begin, 0, p.ring_slot};
-        prep(false);                                       // step 0
-        bar_compute();
+        bar_chain();                                       // pre-activation tile 0 has landed
+        if (nsteps > 0) load_ap(0, 0);
 
-        uint32_t pc = 0, epar = 0, hcnt = 0;               // ring piece counter, sample parity, h tiles handed over
-        bool ok_f = false, ok_ap = false, ok_hf = false;
+        uint32_t n = 0, epar = 0;                          // step, sample parity
         for (int t = t_begin; t < t_end; t++) {
             TRACE2(0, 1);
             if (t > t_begin) {                             // the tail CTA has written this sample's indices into ys
@@ -1324,15 +1348,14 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
                 if (TR == TU) cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
                 cp_async_commit();                         // landed long before the next sample starts (waited for at the end of this one)
             }
-            bar_compute();
+            bar_chain();
 #pragma unroll
             for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
             TRACE2(0, 2);
 
-            for (int l = 0; l < L; l++, pc++) {
-                const uint32_t sl = pc & 1, p1 = sm + M::C_RING + sl * M::PIECE0, fph = (pc >> 1) & 1;
+            for (int l = 0; l < L; l++, n++) {
+                const uint32_t p1 = sm + M::C_RING + (n & 1) * M::PIECE0;
                 const float2 br = brn;
-                if (!ok_f) mbar_wait(s_full + 8 * sl, fph);
                 {
                     const uint4 bt0 = lds128(p1 + o_t0), bg0 = lds128(p1 + o_g0), bt1 = lds128(p1 + o_t0 + 512), bg1 = lds128(p1 + o_g0 + 512);
                     float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
@@ -1347,34 +1370,24 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
                 {
                     uint32_t h01, h23;
                     gate<TR>(accp, sm + M::C_HBUF + xchg, h01, h23);
-                    // the tail CTA's copy: buffer hcnt % NHB, free once the tail has read the tile of two steps ago
-                    if (!ok_hf) mbar_wait(s_hfree + 8 * (hcnt % M::NHB), ((hcnt / M::NHB) & 1) ^ 1);
-                    if (TR == TU) st_async_v2(r_hbuf + (hcnt % M::NHB) * M::XT, h01, h23, r_hfull + 8 * (hcnt % M::NHB));
-                    else st_async_b32(r_hbuf + (hcnt % M::NHB) * M::XT, h01, r_hfull + 8 * (hcnt % M::NHB));
-                    hcnt++;
+                    // the tail CTA's copy: buffer n % NHB, free since the x barrier (the sync warp)
+                    if (TR == TU) st_async_v2(r_hbuf + (n % M::NHB) * M::XT, h01, h23, r_hfull + 8 * (n % M::NHB));
+                    else st_async_b32(r_hbuf + (n % M::NHB) * M::XT, h01, r_hfull + 8 * (n % M::NHB));
                 }
                 TRACE2(0, 12);
-                prep(ok_ap);
-                bar_compute();
+                bar_chain();
                 uint32_t ha[4][4];
 #pragma unroll
                 for (int j = 0; j < 4; j++) load_a_rows<TR>(ha[j], sm + M::C_HBUF, j, lane);
                 TRACE2(0, 10);
+                if (n + 1 < (uint32_t)nsteps) load_ap(n + 1, l + 1 < L ? l + 1 : 0);
                 float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
                 hmma_res(ra, rb, ha, bw0, bw1);
-                release(s_empty + 8 * sl, lane);
                 residual<TR>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
                 TRACE2(0, 14);
                 dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
-                {   // look at the coming step's barriers
-                    const uint32_t npc = pc + 1;
-                    ok_f = mbar_test_wait(s_full + 8 * (npc & 1), (npc >> 1) & 1);
-                    ok_ap = mbar_test_wait(s_apfull + 8 * (pn % M::NAP), (pn / M::NAP) & 1);
-                    ok_hf = mbar_test_wait(s_hfree + 8 * (hcnt % M::NHB), ((hcnt / M::NHB) & 1) ^ 1);
-                }
-                TRACE2(0, 13);
                 if (l + 1 < L) {
-                    bar_compute();
+                    bar_chain();
 #pragma unroll
                     for (int j = 0; j < 4; j++) load_a_rows<TR>(xa[j], sm + M::C_XBUF, j, lane);
                 }
@@ -1421,7 +1434,7 @@ __device__ __forceinline__ void tail_cta(const ClusterCta& c, int& trn)
             for (int t = t_begin; t < t_end; t++)
                 for (int l = 0; l < L; l++) put(img + (size_t)l * im.layer_bytes + C::W_SKIP, S * 128);
         }
-    } else {
+    } else if (w < NCW) {
         const float* s_bout = reinterpret_cast<const float*>(smem_raw + M::T_BOUT);
         const uint32_t o_skip = (uint32_t)(w * C::NSK * 2) * 512 + lane16;
         uint4 zsw[2][S / 32];
@@ -1637,7 +1650,7 @@ __device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
                 if (++l == L) l = 0;
             }
         }
-    } else {
+    } else if (w < NCW) {
         int* dil = reinterpret_cast<int*>(smem_raw + M::P_DIL);
         const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u, cstride = (uint32_t)ntiles_alloc * 4096u;
         const unsigned char* gring = static_cast<const unsigned char*>(p.ring) + (size_t)tile * 2048;
@@ -1742,7 +1755,7 @@ __device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
 }
 
 template <int S, int TR, bool DUMP, bool TRC>
-__global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
+__global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
 {
     // debug timeline (tools/lat_trace.py, TRACE2): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
     unsigned long long* trc = (TRC && p.trace && blockIdx.x < NCL) ? p.trace : nullptr;
@@ -1780,10 +1793,10 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     int* ys = reinterpret_cast<int*>(smem_raw + M::O_YS);
 
     if (tid == 0) {
-        for (int i = 0; i < M::NRING; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, NCW); }
+        for (int i = 0; i < M::NRING; i++) { mbar_init(s_full + 8 * i, 1); mbar_init(s_empty + 8 * i, is_chain ? 1 : NCW); }
         for (int i = 0; i < M::NPS; i++) mbar_init(s_pfull + 8 * i, 128);
         for (int i = 0; i < M::NHB; i++) { mbar_init(s_hfull + 8 * i, 1); mbar_init(s_hfree + 8 * i, NCW); }
-        for (int i = 0; i < M::NAP; i++) { mbar_init(s_apfull + 8 * i, 1); mbar_init(s_apfree + 8 * i, NCW); }
+        for (int i = 0; i < M::NAP; i++) { mbar_init(s_apfull + 8 * i, 1); mbar_init(s_apfree + 8 * i, 1); }
         mbar_init(s_yfull, 1);
         mbar_init(s_ob0full, 1); mbar_init(s_ob0free, NCW); mbar_init(s_ob1full, 1); mbar_init(s_ob1free, 2 * NCW);
         mbar_init(s_lfull, 1); mbar_init(s_lfree, NCW);
@@ -1805,18 +1818,18 @@ __global__ void __launch_bounds__(NT, 1) wn_lat2_kernel(const WnParams p, const 
     }
     if (is_chain) {
         const uint32_t* ec = static_cast<const uint32_t*>(p.embCur);
-        for (int i = tid; i < A * 32; i += NT) sts32(sm + M::C_EMB + ((i >> 5) * EROW + (i & 31)) * 4, ec[i]);
-        for (int i = tid; i < L * 256; i += NT) sts32(sm + M::C_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + i]));
+        for (int i = tid; i < A * 32; i += NTC) sts32(sm + M::C_EMB + ((i >> 5) * EROW + (i & 31)) * 4, ec[i]);
+        for (int i = tid; i < L * 256; i += NTC) sts32(sm + M::C_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + i]));
     } else if (is_tail) {
         float* s_bout = reinterpret_cast<float*>(smem_raw + M::T_BOUT);
-        for (int i = tid; i < S; i += NT) s_bout[i] = gbias[im.b_skpre + (size_t)(L - 1) * S + i];
-        for (int i = tid; i < A; i += NT) { s_bout[S + i] = gbias[im.b_bzs + i]; s_bout[S + A + i] = gbias[im.b_bza + i]; }
+        for (int i = tid; i < S; i += NTC) s_bout[i] = gbias[im.b_skpre + (size_t)(L - 1) * S + i];
+        for (int i = tid; i < A; i += NTC) { s_bout[S + i] = gbias[im.b_bzs + i]; s_bout[S + A + i] = gbias[im.b_bza + i]; }
     } else {
         int* dil = reinterpret_cast<int*>(smem_raw + M::P_DIL);
         if (tid == 0) { int d = 1; for (int l = 0; l < L; l++) { dil[l] = d; d <<= 1; if (d > p.maxDil) d = 1; } }   // nv_wavenet.cuh:99-111
-        for (int i = tid; i < L * 128; i += NT) sts32(sm + M::P_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + (i >> 2) * 8 + (i & 3)]));
+        for (int i = tid; i < L * 128; i += NTC) sts32(sm + M::P_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + (i >> 2) * 8 + (i & 3)]));
         float* s_bout = reinterpret_cast<float*>(smem_raw + M::P_BOUT);
-        for (int i = tid; i < A; i += NT) { s_bout[i] = gbias[im.b_bzs + i]; s_bout[A + i] = gbias[im.b_bza + i]; }
+        for (int i = tid; i < A; i += NTC) { s_bout[i] = gbias[im.b_bzs + i]; s_bout[A + i] = gbias[im.b_bza + i]; }
     }
     __syncthreads();
     cluster_sync_all();                                    // every CTA's barriers are initialised before anybody signals a peer
@@ -1881,7 +1894,7 @@ static cudaLaunchConfig_t lat2_config(int clusters, cudaStream_t stream, cudaLau
 {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(NCL * clusters, 1, 1);
-    cfg.blockDim = dim3(NT, 1, 1);
+    cfg.blockDim = dim3(NTC, 1, 1);
     cfg.dynamicSmemBytes = CfgC<S, TR>::SMEM;
     cfg.stream = stream;
     at.id = cudaLaunchAttributeClusterDimension;
@@ -1966,7 +1979,7 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
         else if (tr == TU) e = p.S == 256 ? lat2_launch_S<256, TU>(p, im8, clusters, ntiles_alloc, stream, &smem) : lat2_launch_S<128, TU>(p, im8, clusters, ntiles_alloc, stream, &smem);
         if (tr) {
             if (e != cudaSuccess) return e;
-            if (info) { info->kernel = NVWN_KERNEL_LATENCY; info->grid = NCL * clusters; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = tr; info->cluster = NCL; }
+            if (info) { info->kernel = NVWN_KERNEL_LATENCY; info->grid = NCL * clusters; info->block = NTC; info->smem_bytes = (int)smem; info->batch_per_cta = tr; info->cluster = NCL; }
             return cudaGetLastError();
         }
     }

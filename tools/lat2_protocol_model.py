@@ -1,5 +1,6 @@
 """Discrete-event model of the synchronisation protocol of the three-CTA cluster kernel (csrc/wn_lat_kernel.cu, wn_lat2_kernel):
-chain / tail / prep CTAs, each with eight compute warps and a weight-ring producer lane, exchange mbarrier phases, transaction
+chain / tail / prep CTAs, each with eight compute warps and a weight-ring producer lane (and the chain CTA's sync warp, which waits
+on its mbarriers for the compute warps and joins their named barrier), exchange mbarrier phases, transaction
 bytes (st.async ... complete_tx), ring slots and tile buffers in the order the kernel does, with randomised latencies.  It checks
 what a passing GPU run cannot show:
 
@@ -92,7 +93,7 @@ class Sim:
         B = lambda n, c: Barrier(self, n, c)
         # chain CTA
         self.c_full = [B(f"chain.full{i}", 1) for i in range(2)]
-        self.c_empty = [B(f"chain.empty{i}", NCW) for i in range(2)]
+        self.c_empty = [B(f"chain.empty{i}", 1) for i in range(2)]           # arrived by the sync warp
         self.hfree = [B(f"chain.hfree{i}", NCW) for i in range(2)]
         self.yfull = B("chain.yfull", 1)
         self.apfull = [B(f"chain.apfull{i}", 1) for i in range(NAP)]
@@ -111,7 +112,7 @@ class Sim:
         self.p_full = [B(f"prep.full{i}", 1) for i in range(4)]
         self.p_empty = [B(f"prep.empty{i}", NCW) for i in range(4)]
         self.pfull = [B(f"prep.pfull{i}", 4) for i in range(NPS)]          # warps 0-3 stage the history tile (128 thread arrivals)
-        self.apfree = [B(f"prep.apfree{i}", NCW) for i in range(NAP)]
+        self.apfree = [B(f"prep.apfree{i}", 1) for i in range(NAP)]          # arrived by the chain's sync warp
         # armed by their owners one phase ahead (kernel prologue)
         self.yfull.expect_tx(self.nb(128))
         for b in self.apfull:
@@ -213,26 +214,13 @@ class Sim:
             yield ("delay", self.lat(20, 60, who))
 
     def chain_warp(self, w):
+        """A compute warp of the chain CTA: its layer step waits only on the CTA barrier it shares with the sync warp."""
         who = f"chain.w{w}"
         L, T = self.L, self.T
-        pn = 0
-
-        def prep():
-            nonlocal pn
-            if pn < self.nsteps:
-                b = pn % NAP
-                yield ("wait", self.apfull[b], pn // NAP)
-                self.read(who, f"ap{b}", pn)
-                yield ("delay", self.lat(20, 40, who))
-                if w == 0:
-                    self.apfull[b].expect_tx(self.nb(8192))  # armed for the tile NAP steps on, before this warp's "free" signal
-                if self.bug != "no_apfree":
-                    self.after(self.lat(150, 400), self.apfree[b].arrive)
-            pn += 1
-
-        yield from prep()
         yield from self.cta_bar("chain", who)
-        k = hc = 0
+        if self.nsteps:
+            self.read(who, "ap0", 0)                         # pre-activation tile 0 (the sync warp saw it land)
+        k = 0
         for t in range(T):
             if t > 0:
                 yield ("wait", self.yfull, t - 1)
@@ -240,33 +228,54 @@ class Sim:
                     self.yfull.expect_tx(self.nb(128))
             yield ("delay", self.lat(150, 300, who))         # embedding, history write of (t, layer 0)
             self.emb_done[t] = self.emb_done.get(t, 0) + 1
-            yield from self.cta_bar("chain", who)
+            yield from self.cta_bar("chain", who)            # x barrier
             for l in range(L):
-                yield ("wait", self.c_full[k & 1], k >> 1)
                 self.read(who, f"cring{k & 1}", k)
                 yield ("delay", self.lat(200, 400, who))     # cur GEMM + gate
-                if self.bug != "no_hfree":
-                    yield ("wait", self.hfree[hc & 1], (hc >> 1) - 1)
 
-
-                def land_h(hc=hc):                           # this warp's 256 (8 rows: 128) bytes of the h tile + their complete_tx
-                    self.touch(f"h{hc & 1}", hc, NCW)
-                    self.hfull[hc & 1].complete_tx(self.nb(256))
+                def land_h(k=k):                             # this warp's 256 (8 rows: 128) bytes of the h tile + their complete_tx
+                    self.touch(f"h{k & 1}", k, NCW)          # (the tail's buffer is free: the sync warp waited before the x barrier)
+                    self.hfull[k & 1].complete_tx(self.nb(256))
                 self.after(self.lat(200, 700), land_h)
-                hc += 1
-                yield from prep()
-                yield from self.cta_bar("chain", who)
+                yield from self.cta_bar("chain", who)        # h barrier
+                if k + 1 < self.nsteps:
+                    self.read(who, f"ap{(k + 1) % NAP}", k + 1)
                 yield ("delay", self.lat(150, 300, who))     # res GEMM (weights of the same piece)
-                self.c_empty[k & 1].arrive()
                 yield ("delay", self.lat(30, 80, who))       # x tile + history ring write of (t, l + 1)
                 self.chain_step_warps[k] = self.chain_step_warps.get(k, 0) + 1
                 while self.chain_step_warps.get(self.chain_steps_done, 0) == NCW:
                     self.chain_steps_done += 1
-                yield from self.cta_bar("chain", who)
+                if l + 1 < L:
+                    yield from self.cta_bar("chain", who)    # x barrier
                 k += 1
 
-    def cta_bar(self, cta, who):                             # bar.sync among the eight compute warps of one CTA
-        bar = self.__dict__.setdefault("_barobj", {}).setdefault(cta, Barrier(self, f"{cta}.bar.sync", NCW))
+    def chain_sync(self):
+        """The chain CTA's sync warp (lane 0): every mbarrier wait and hand-back of the layer loop."""
+        who = "chain.sync"
+        if self.nsteps:
+            yield ("wait", self.apfull[0], 0)
+        yield from self.cta_bar("chain", who)
+        for n in range(self.nsteps):
+            b, hb = n % NAP, n & 1
+            if self.bug != "no_full_wait":
+                yield ("wait", self.c_full[n & 1], n >> 1)
+            if self.bug not in ("no_hfree", "hfree_late"):   # the tail has read h tile n - 2: the compute warps may send tile n
+                yield ("wait", self.hfree[hb], (n >> 1) - 1)
+            yield from self.cta_bar("chain", who)            # x barrier of step n: pre-activation tile n has been read
+            if self.bug == "hfree_late":
+                yield ("wait", self.hfree[hb], (n >> 1) - 1)
+            self.apfull[b].expect_tx(self.nb(8192))          # armed for the tile NAP steps on, before the "free" signal
+            if self.bug != "no_apfree":
+                self.after(self.lat(150, 400), self.apfree[b].arrive)
+            if n + 1 < self.nsteps and self.bug != "no_apfull_wait":
+                yield ("wait", self.apfull[(n + 1) % NAP], (n + 1) // NAP)
+            yield from self.cta_bar("chain", who)            # h barrier of step n: ring piece n has been read
+            if self.bug != "no_empty":
+                self.c_empty[n & 1].arrive()
+            yield ("delay", self.lat(10, 40, who))
+
+    def cta_bar(self, cta, who):                             # bar.sync among the compute warps of one CTA (+ the chain's sync warp)
+        bar = self.__dict__.setdefault("_barobj", {}).setdefault(cta, Barrier(self, f"{cta}.bar.sync", NCW + (cta == "chain")))
         mine = bar.completed
         bar.arrive()
         if bar.completed == mine:
@@ -417,6 +426,7 @@ class Sim:
         self.spawn("chain.producer", self.producer("chain.producer", self.c_full, self.c_empty, 2, [24576] * (T * L), "cring"))
         self.spawn("tail.producer", self.producer("tail.producer", self.t_full, self.t_empty, TSLOTS, [32768] * (T * L), "tring"))
         self.spawn("prep.producer", self.producer("prep.producer", self.p_full, self.p_empty, 4, [16384] * (T * L), "pring"))
+        self.spawn("chain.sync", self.chain_sync())
         for w in range(NCW):
             self.spawn(f"chain.w{w}", self.chain_warp(w))
             self.spawn(f"tail.w{w}", self.tail_warp(w))
