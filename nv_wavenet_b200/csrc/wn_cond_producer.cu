@@ -1,6 +1,6 @@
 // wn_cond_producer.cu -- conditioning producer (SURVEY.md 8f next-2): local-conditioning features (mel frames) ->
 // Lh[n][l][b][2R] on the device, in chunks of whole samples that go straight into the engine's conditioning store
-// (nvwn_set_conditioning), so the [N][L][B][2R] fp32 tensor of the reference (10.5 GB for C3) never exists.
+// (the kernel family's convert / convert_rows), so the [N][L][B][2R] fp32 tensor of the reference (10.5 GB for C3) never exists.
 //
 // Replaces, for inference, WaveNet.get_cond_input (pytorch/wavenet.py:190-202) and the permutes that follow it
 // (pytorch/nv_wavenet.py:48-49,181):
@@ -13,8 +13,9 @@
 // fp32 FMA, every output element accumulated in the order of the shared element functions (so host reference, simple kernels
 // and the tiled kernel below agree bit for bit).  The projection is 94 % of the flops (C3: 0.42 TFLOP per 16000 samples x 64
 // utterances): a register-tiled kernel (128 x 128 outputs per CTA, 8 x 8 per thread, operands through shared memory).
-// The per-slot producer (wn_cond_produce_slots, continuous batching) differs only in the upsampling: each row of a chunk reads its
-// own utterance's frames at its own sample offset; the projection is the same kernel with B = the number of slots.
+// One producer serves the whole-batch and the per-slot calls: each of the k rows of a chunk reads its own utterance's frames at its
+// own sample offset through a small table (for a whole batch, row b's frames are features[b] and its start is 0); the projection
+// is one kernel with B = k.
 #include "wn_common.h"
 
 namespace {
@@ -56,20 +57,9 @@ __global__ void transpose_wu_kernel(float* __restrict__ dst, const float* __rest
     }
 }
 
-// U[b][j][co] for samples n0 + j, j < m
-__global__ void upsample_kernel(float* __restrict__ U, const float* __restrict__ feat, const float* __restrict__ WuT, const float* __restrict__ bu,
-                                int B, int C, int T, int K, int stride, int n0, int m)
-{
-    const size_t total = (size_t)B * m * C;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int co = (int)(i % C), j = (int)((i / C) % m), b = (int)(i / ((size_t)C * m));
-        U[i] = upsample_element<true>(feat, WuT, bu, C, T, K, stride, b, co, n0 + j);
-    }
-}
-
-// Per-slot twin of upsample_kernel: U[i][j][co] for the k rows of a chunk, row i = absolute sample n0 + j of the utterance in
-// tab[i], i.e. sample n0 + j - start of its own frames [C][T] at frames + foff.  Samples at or past its end (T * stride) are left
-// at 0: mask_slots_kernel zeroes their projected rows.
+// U[i][j][co] for the k rows of a chunk, row i = absolute sample n0 + j of the utterance in tab[i], i.e. sample n0 + j - start of
+// its own frames [C][T] at frames + foff.  Samples at or past its end (T * stride) are left at 0: mask_slots_kernel zeroes their
+// projected rows.
 __global__ void upsample_slots_kernel(float* __restrict__ U, const float* __restrict__ frames, const WnCondSlot* __restrict__ tab,
                                       const float* __restrict__ WuT, const float* __restrict__ bu, int k, int C, int K, int stride, long long n0, int m)
 {
@@ -83,7 +73,7 @@ __global__ void upsample_slots_kernel(float* __restrict__ U, const float* __rest
 }
 
 // zeroes out[j][l][r][c] for every (j, r) whose sample n0 + j is at or past the end of row r's utterance (the projection of a zero
-// U row is the bias, not 0).  One thread per (j, r): only an utterance's last window has such rows, so almost every thread returns.
+// U row is the bias, not 0).  One thread per (j, r); launched only for a chunk in which some row's utterance ends.
 __global__ void mask_slots_kernel(float* __restrict__ out, const WnCondSlot* __restrict__ tab, int k, int L, int R2, int stride, long long n0, int m)
 {
     const size_t total = (size_t)m * k;
@@ -201,24 +191,14 @@ cudaError_t wn_cond_transpose_wu(float* WuT, const float* Wu, int C, int K, cuda
     return cudaGetLastError();
 }
 
-cudaError_t wn_cond_produce(float* out, float* U, const float* feat, const float* WuT, const float* bu, const float* Wc, const float* bc,
-                            int B, int C, int T, int K, int stride, int L, int R, int n0, int m, cudaStream_t stream)
-{
-    if (m <= 0) return cudaSuccess;
-    upsample_kernel<<<grid_for((size_t)B * m * C), 256, 0, stream>>>(U, feat, WuT, bu, B, C, T, K, stride, n0, m);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    return project(out, U, Wc, bc, B, C, L, R, m, stream);
-}
-
 cudaError_t wn_cond_produce_slots(float* out, float* U, const float* frames, const WnCondSlot* tab, const float* WuT, const float* bu, const float* Wc,
-                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, cudaStream_t stream)
+                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, bool mask, cudaStream_t stream)
 {
     if (m <= 0) return cudaSuccess;
     upsample_slots_kernel<<<grid_for((size_t)k * m * C), 256, 0, stream>>>(U, frames, tab, WuT, bu, k, C, K, stride, n0, m);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = project(out, U, Wc, bc, k, C, L, R, m, stream);     // rows b * m + j -> out[j][l][b][2R]: the chunk's layout
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess || !mask) return e;
     mask_slots_kernel<<<grid_for((size_t)m * k), 256, 0, stream>>>(out, tab, k, L, 2 * R, stride, n0, m);
     return cudaGetLastError();
 }

@@ -61,6 +61,21 @@ bool is_device_ptr(const void* p)
     return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
 }
 
+// A conditioning producer (DESIGN.md §6): a network of C channels, upsampling window K and stride; `scratch` of cond_scratch()'s
+// layout, chunks of up to `rows` (row, sample) rows; row b's frames [C][T[b]] at frames + b * cap * C; the row list and WnCondSlot
+// table of the last production (device); per row on the host, the frames of its utterance (0: none) and its absolute start.
+struct CondProducer {
+    int C = 0, K = 0, stride = 0, rows = 0;
+    float* scratch = nullptr;
+    size_t scratch_floats = 0;
+    float* frames = nullptr;
+    size_t frames_floats = 0;
+    int cap = 0;
+    char* tables = nullptr;                  // int [B] rows, then WnCondSlot [B] at cond_table_offset
+    std::vector<int> T;
+    std::vector<long long> start;
+};
+
 }  // namespace
 
 struct nvwn_engine : WnConfig {
@@ -109,22 +124,10 @@ struct nvwn_engine : WnConfig {
     void* image = nullptr;                   // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
 
-    // conditioning producer (nvwn_cond_producer_load / _run): features | Wu | WuT | bu | Wc | bc | U chunk | Lh chunk in one allocation
-    float* cp_scratch = nullptr;
-    size_t cp_floats = 0;
-    int cp_C = 0, cp_T = 0, cp_K = 0, cp_stride = 0, cp_chunk = 0;
-
-    // per-slot conditioning producer (nvwn_cond_producer_set_weights / _set_slots / _run_slots), apart from the one above:
-    // Wu | WuT | bu | Wc | bc | U chunk | Lh chunk in one allocation, chunks of up to cs_rows (slot, sample) rows; the frames of
-    // slot b's utterance at cs_frames + b * cs_cap * C; the slot list and WnCondSlot table of the last _run_slots (device); per slot
-    // on the host, the attached utterance's frames (0: none) and absolute start
-    float* cs_scratch = nullptr;
-    int cs_C = 0, cs_K = 0, cs_stride = 0, cs_rows = 0;
-    float* cs_frames = nullptr;
-    int cs_cap = 0;
-    char* cs_tables = nullptr;               // int [B] slots, then WnCondSlot [B]
-    std::vector<int> cs_T;
-    std::vector<long long> cs_start;
+    // the conditioning producers of the whole-batch calls (nvwn_cond_producer_load / _run / _run_stream) and of the per-slot calls
+    // (nvwn_cond_producer_set_weights / _set_slots / _run_slots): each has its own weights, frames and scratch, so the two sets of
+    // calls may be interleaved
+    CondProducer cond_whole, cond_slots;
 
     // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
     void* score_image = nullptr;
@@ -184,24 +187,80 @@ int copy_snapshot(T* dst_dev, const T* src, size_t n, cudaStream_t stream)
     return 0;
 }
 
-// Floats of the conditioning network in engine memory: Wu [C][C][K] | its [K][C][C] transpose WuT | bu [C] | Wc [L*2R][C] | bc [L*2R]
-size_t cond_weight_floats(const nvwn_engine* e, int C, int K)
+// Where a producer's scratch holds each part, in floats from its start: Wu [C][C][K] | its [K][C][C] transpose WuT | bu [C] |
+// Wc [L*2R][C] | bc [L*2R] | U chunk [rows][C] | output chunk [rows][L*2R], the last 16-byte aligned for the tiled projection's
+// float4 stores
+struct CondScratch {
+    size_t wu, wut, bu, wc, bc, u, out, floats;
+};
+CondScratch cond_scratch(const nvwn_engine* e, int C, int K, int rows)
 {
-    return 2 * (size_t)C * C * K + C + (size_t)e->L * 2 * e->R * (C + 1);
+    const size_t lrow = (size_t)e->L * 2 * e->R, n_wu = (size_t)C * C * K;
+    CondScratch o;
+    o.wu = 0; o.wut = n_wu; o.bu = 2 * n_wu; o.wc = o.bu + C; o.bc = o.wc + lrow * C; o.u = o.bc + lrow;
+    o.out = align_up(o.u + (size_t)rows * C, 4);
+    o.floats = o.out + (size_t)rows * lrow;
+    return o;
 }
 
-// The conditioning network into that layout at `w`, from host or device sources, and the transpose the kernels read.  Stream-ordered
-// on `st`: the caller synchronises before the sources may be released.  Both producers load their weights through it.
-cudaError_t put_cond_weights(const nvwn_engine* e, float* w, const float* Wu, const float* bu, const float* Wc, const float* bc, int C, int K,
-                             cudaStream_t st)
+// bytes before the WnCondSlot table in a producer's `tables`
+size_t cond_table_offset(const nvwn_engine* e) { return align_up((size_t)e->B * sizeof(int), 16); }
+
+// Gives P the conditioning network, from host or device sources, and the transpose the kernels read; sizes its chunks to about
+// 64 MB of fp32 and at least one sample of every row, and grows its scratch when that is too small.  Stream-ordered on `st`: the
+// caller synchronises before the sources may be released.
+int put_cond_network(nvwn_engine* e, CondProducer& P, const std::string& who, int C, int K, int stride, const float* Wu, const float* bu,
+                     const float* Wc, const float* bc, cudaStream_t st)
 {
-    const size_t n_wu = (size_t)C * C * K, n_wc = (size_t)e->L * 2 * e->R * C, n_bc = (size_t)e->L * 2 * e->R;
-    float* d_wu = w; float* d_wut = d_wu + n_wu; float* d_bu = d_wut + n_wu; float* d_wc = d_bu + C; float* d_bc = d_wc + n_wc;
+    const size_t lrow = (size_t)e->L * 2 * e->R;                             // floats of one (row, sample) of conditioning
+    const size_t rows = ((size_t)16 << 20) / lrow > (size_t)e->B ? ((size_t)16 << 20) / lrow : (size_t)e->B;
+    const CondScratch o = cond_scratch(e, C, K, (int)rows);
+    if (o.floats > P.scratch_floats) {
+        if (P.scratch) { CK(cudaDeviceSynchronize()); cudaFree(P.scratch); P.scratch = nullptr; P.scratch_floats = 0; }
+        CK(cudaMalloc((void**)&P.scratch, o.floats * sizeof(float)));
+        P.scratch_floats = o.floats;
+    }
+    if (!P.tables) CK(cudaMalloc((void**)&P.tables, cond_table_offset(e) + (size_t)e->B * sizeof(WnCondSlot)));
+    P.C = C; P.K = K; P.stride = stride; P.rows = (int)rows;
+    float* w = P.scratch;
     cudaError_t ce = cudaSuccess;
-    auto put = [&](float* dst, const float* src, size_t n) { if (ce == cudaSuccess) ce = cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDefault, st); };
-    put(d_wu, Wu, n_wu); put(d_bu, bu, C); put(d_wc, Wc, n_wc); put(d_bc, bc, n_bc);
-    if (ce == cudaSuccess) ce = wn_cond_transpose_wu(d_wut, d_wu, C, K, st);
-    return ce;
+    auto put = [&](size_t dst, const float* src, size_t n) { if (ce == cudaSuccess) ce = cudaMemcpyAsync(w + dst, src, n * sizeof(float), cudaMemcpyDefault, st); };
+    put(o.wu, Wu, o.wut - o.wu); put(o.bu, bu, C); put(o.wc, Wc, o.bc - o.wc); put(o.bc, bc, lrow);
+    if (ce == cudaSuccess) ce = wn_cond_transpose_wu(w + o.wut, w + o.wu, C, K, st);
+    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
+    return 0;
+}
+
+// Conditioning of absolute samples t_first .. t_first + count - 1 for rows rows[0..n) of P (host list; NULL: rows 0 .. B - 1 of
+// the whole-batch producer, n = B), each read from its own utterance, into store positions pos .. pos + count - 1: the caller has
+// checked the ranges, split them at the ring's wrap and put the rows' WnCondSlot table (and list) into P.tables.  Chunks of
+// P.rows / n whole samples, stored by convert_rows, or for a whole batch by the family's convert: the latency family's convert
+// writes 16-byte stores and zeroes the padding rows of the last tile, which convert_rows does not.
+int produce(nvwn_engine* e, const CondProducer& P, const std::string& who, const int* rows, int n, long long t_first, int pos, int count,
+            cudaStream_t st)
+{
+    const CondScratch o = cond_scratch(e, P.C, P.K, P.rows);
+    float* w = P.scratch;
+    const int* rows_dev = rows ? reinterpret_cast<const int*>(P.tables) : nullptr;
+    const WnCondSlot* tab = reinterpret_cast<const WnCondSlot*>(P.tables + cond_table_offset(e));
+    long long end = LLONG_MAX;                                                // the earliest end of a listed utterance
+    for (int i = 0; i < n; i++) {
+        const int r = rows ? rows[i] : i;
+        const long long end_r = P.start[r] + (long long)P.T[r] * P.stride;
+        if (end_r < end) end = end_r;
+    }
+    const int chunk = P.rows / n;                                             // >= 1 as P.rows >= B
+    cudaError_t ce = cudaSuccess;
+    for (int done = 0; done < count && ce == cudaSuccess; done += chunk) {
+        const int m = count - done < chunk ? count - done : chunk;
+        const long long t0 = t_first + done;
+        ce = wn_cond_produce_slots(w + o.out, w + o.u, P.frames, tab, w + o.wut, w + o.bu, w + o.wc, w + o.bc, n, P.C, P.K, P.stride, e->L, e->R,
+                                   t0, m, end < t0 + m, st);
+        if (ce == cudaSuccess)
+            ce = rows ? e->family->convert_rows(*e, e->Lh, w + o.out, rows_dev, n, pos + done, m, st) : e->family->convert(*e, e->Lh, w + o.out, pos + done, m, st);
+    }
+    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
+    return 0;
 }
 
 // Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.
@@ -454,8 +513,10 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     cudaMemsetAsync(e->ring, 0, ring_bytes, 0);
     cudaMemsetAsync(e->origin, 0, Bz * sizeof(long long), 0);
     cudaMemsetAsync(e->seed, 0, Bz * sizeof(unsigned long long), 0);
-    e->cs_T.assign(Bz, 0);
-    e->cs_start.assign(Bz, 0);
+    for (CondProducer* P : {&e->cond_whole, &e->cond_slots}) {
+        P->T.assign(Bz, 0);
+        P->start.assign(Bz, 0);
+    }
     wn_fill_int(e->yPrev, 128, Bz, 0);
     wn_fill_int(e->yCur, 128, Bz, 0);
     cudaError_t se = cudaDeviceSynchronize();
@@ -468,8 +529,9 @@ int nvwn_destroy(nvwn_engine* e)
 {
     if (!e) return 0;
     void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
-                    e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->cp_scratch, e->score_image, e->score_scratch,
-                    e->origin, e->seed, e->slot_rows, e->slot_seeds, e->row_stage, e->cs_scratch, e->cs_frames, e->cs_tables, e->prime_rows};
+                    e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->score_image, e->score_scratch, e->origin, e->seed,
+                    e->slot_rows, e->slot_seeds, e->row_stage, e->prime_rows, e->cond_whole.scratch, e->cond_whole.frames, e->cond_whole.tables,
+                    e->cond_slots.scratch, e->cond_slots.frames, e->cond_slots.tables};
     for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
@@ -538,75 +600,49 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
     const int C = n_cond_channels, T = num_frames, K = window;
     if (C < 1 || T < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, "nvwn_cond_producer_load: bad sizes (need window >= stride >= 1)");
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t per = (size_t)e->L * e->B * 2 * e->R;                       // floats of conditioning per sample
-    int chunk = (int)(((size_t)16 << 20) / per);                             // chunk of whole samples: ~64 MB of fp32 at a time
-    if (chunk < 1) chunk = 1;
+    CondProducer& P = e->cond_whole;
+    P.T.assign(e->B, 0);                                                      // loaded once every copy has been made
+    int rc = put_cond_network(e, P, "nvwn_cond_producer_load", C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
+    if (rc != 0) return rc;
+    // features [B][C][T] are the frame arena with cap = T, in one copy; row b's utterance starts at sample 0
     const size_t n_feat = (size_t)e->B * C * T;
-    const size_t floats = n_feat + cond_weight_floats(e, C, K) + (size_t)e->B * chunk * C + (size_t)chunk * per + 16;
-    if (floats > e->cp_floats) {
-        if (e->cp_scratch) { CK(cudaDeviceSynchronize()); cudaFree(e->cp_scratch); e->cp_scratch = nullptr; e->cp_floats = 0; }
-        CK(cudaMalloc((void**)&e->cp_scratch, floats * sizeof(float)));
-        e->cp_floats = floats;
+    if (n_feat > P.frames_floats) {
+        if (P.frames) { CK(cudaDeviceSynchronize()); cudaFree(P.frames); P.frames = nullptr; P.frames_floats = 0; }
+        CK(cudaMalloc((void**)&P.frames, n_feat * sizeof(float)));
+        P.frames_floats = n_feat;
     }
-    e->cp_C = C; e->cp_T = T; e->cp_K = K; e->cp_stride = stride; e->cp_chunk = chunk;
-    float* d_feat = e->cp_scratch;
-    cudaError_t ce = cudaMemcpyAsync(d_feat, features, n_feat * sizeof(float), cudaMemcpyDefault, st);
-    if (ce == cudaSuccess) ce = put_cond_weights(e, d_feat + n_feat, upsample_weight, upsample_bias, cond_weight, cond_bias, C, K, st);
+    P.cap = T;
+    std::vector<WnCondSlot> tab(e->B);
+    for (int b = 0; b < e->B; b++) tab[b] = {(long long)b * C * T, 0, T, 0};
+    cudaError_t ce = cudaMemcpyAsync(P.frames, features, n_feat * sizeof(float), cudaMemcpyDefault, st);
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(P.tables + cond_table_offset(e), tab.data(), tab.size() * sizeof(WnCondSlot), cudaMemcpyHostToDevice, st);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);                   // host sources may be released by the caller now
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_cond_producer_load: ") + cudaGetErrorString(ce));
+    P.T.assign(e->B, T);
     return 0;
 }
-
-}  // extern "C"
-
-namespace {
-
-// conditioning of samples [sample_begin, sample_begin + sample_count) of the loaded sequence into store positions from `pos`; the
-// caller has checked both ranges
-int cond_produce(nvwn_engine* e, int pos, int sample_begin, int sample_count, void* stream)
-{
-    const int C = e->cp_C, T = e->cp_T, K = e->cp_K, stride = e->cp_stride, chunk = e->cp_chunk;
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t n_feat = (size_t)e->B * C * T, n_wu = (size_t)C * C * K, n_wc = (size_t)e->L * 2 * e->R * C, n_bc = (size_t)e->L * 2 * e->R;
-    float* d_feat = e->cp_scratch; float* d_wut = d_feat + n_feat + n_wu; float* d_bu = d_wut + n_wu;
-    float* d_wc = d_bu + C; float* d_bc = d_wc + n_wc; float* d_u = d_bc + n_bc;
-    float* d_out = d_u + (size_t)e->B * chunk * C;
-    d_out += (4 - ((size_t)(d_out - e->cp_scratch) & 3)) & 3;                 // 16-byte aligned rows for the tiled projection's float4 stores
-    cudaError_t ce = cudaSuccess;
-    int rc = 0;
-    for (long long done = sample_begin; done < sample_begin + (long long)sample_count && ce == cudaSuccess && rc == 0; done += chunk) {
-        const long long left = sample_begin + (long long)sample_count - done;
-        const int m = (int)(left < chunk ? left : chunk);
-        ce = wn_cond_produce(d_out, d_u, d_feat, d_wut, d_bu, d_wc, d_bc, e->B, C, T, K, stride, e->L, e->R, (int)done, m, st);
-        if (ce == cudaSuccess) rc = nvwn_set_conditioning(e, d_out, pos + (int)(done - sample_begin), m, stream);      // device source: converted in place, stream-ordered
-    }
-    if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_cond_producer: ") + cudaGetErrorString(ce));
-    return rc;
-}
-
-}  // namespace
-
-extern "C" {
 
 int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, int sample_count, void* stream)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: NULL engine");
-    if (!e->cp_scratch || e->cp_T < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: nvwn_cond_producer_load has not been called");
-    const long long Nn = (long long)e->cp_T * e->cp_stride;
+    const CondProducer& P = e->cond_whole;
+    if (P.T[0] < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: nvwn_cond_producer_load has not been called");
+    const long long Nn = (long long)P.T[0] * P.stride;
     if (sample_begin < 0 || sample_count < 0 || sample_begin + (long long)sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: sample range outside num_frames * stride");
     if (first_sample < 0 || first_sample + (long long)sample_begin + sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: samples do not fit the engine");
-    return cond_produce(e, first_sample + sample_begin, sample_begin, sample_count, stream);
+    return produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin, first_sample + sample_begin, sample_count, (cudaStream_t)stream);
 }
 
 int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sample_count, void* stream)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: NULL engine");
-    if (!e->cp_scratch || e->cp_T < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: nvwn_cond_producer_load has not been called");
-    const long long Nn = (long long)e->cp_T * e->cp_stride;
+    const CondProducer& P = e->cond_whole;
+    if (P.T[0] < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: nvwn_cond_producer_load has not been called");
+    const long long Nn = (long long)P.T[0] * P.stride;
     if (sample_begin < 0 || sample_count < 0 || sample_begin + sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: sample range outside num_frames * stride");
     if (sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: more samples than the engine's num_samples (" + std::to_string(e->N) + ")");
     for (const WrapPiece& w : split_at_wrap(sample_begin, sample_count, e->N)) {
-        const int rc = cond_produce(e, w.pos, (int)sample_begin + w.off, w.len, stream);
+        const int rc = produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin + w.off, w.pos, w.len, (cudaStream_t)stream);
         if (rc != 0) return rc;
     }
     return 0;
@@ -635,20 +671,15 @@ int nvwn_cond_producer_set_weights(nvwn_engine* e, int n_cond_channels, const fl
     const int C = n_cond_channels, K = window;
     if (C < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, who + ": bad sizes (need n_cond_channels >= 1 and window >= stride >= 1)");
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t lrow = (size_t)e->L * 2 * e->R;                             // floats of one (slot, sample) row of conditioning
-    size_t rows = ((size_t)16 << 20) / lrow;                                  // chunks of ~64 MB of fp32, and of at least one sample
-    if (rows < (size_t)e->B) rows = e->B;                                     // of every slot
-    if (!e->cs_scratch || C != e->cs_C || K != e->cs_K) {
-        if (e->cs_scratch || e->cs_frames) CK(cudaDeviceSynchronize());
-        if (e->cs_scratch) { cudaFree(e->cs_scratch); e->cs_scratch = nullptr; }
-        if (e->cs_frames) { cudaFree(e->cs_frames); e->cs_frames = nullptr; e->cs_cap = 0; }      // sized for the old channel count
-        if (!e->cs_tables) CK(cudaMalloc((void**)&e->cs_tables, align_up((size_t)e->B * sizeof(int), 16) + (size_t)e->B * sizeof(WnCondSlot)));
-        CK(cudaMalloc((void**)&e->cs_scratch, (cond_weight_floats(e, C, K) + rows * (C + lrow) + 16) * sizeof(float)));
+    CondProducer& P = e->cond_slots;
+    if (P.frames && C != P.C) {                                               // the arena is laid out for the old channel count
+        CK(cudaDeviceSynchronize());
+        cudaFree(P.frames); P.frames = nullptr; P.frames_floats = 0; P.cap = 0;
     }
-    e->cs_C = C; e->cs_K = K; e->cs_stride = stride; e->cs_rows = (int)rows;
-    e->cs_T.assign(e->B, 0);                                                  // frames attached under the old network are forgotten
-    cudaError_t ce = put_cond_weights(e, e->cs_scratch, upsample_weight, upsample_bias, cond_weight, cond_bias, C, K, st);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);                   // host sources may be released by the caller now
+    P.T.assign(e->B, 0);                                                      // frames attached under the old network are forgotten
+    const int rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
+    if (rc != 0) return rc;
+    const cudaError_t ce = cudaStreamSynchronize(st);                        // host sources may be released by the caller now
     if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
     return 0;
 }
@@ -658,45 +689,47 @@ int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const 
 {
     const std::string who = "nvwn_cond_producer_set_slots";
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    if (!e->cs_scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
+    CondProducer& P = e->cond_slots;
+    if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
     int rc = check_slots(e, who.c_str(), slots, n);
     if (rc != 0) return rc;
     if (!features || !num_frames || !starts) return fail(NVWN_EINVAL, who + ": features, num_frames or starts is NULL");
-    const int C = e->cs_C;
+    const int C = P.C;
     int most = 0;
     for (int i = 0; i < n; i++) {
         const std::string u = "utterance " + std::to_string(i) + " (slot " + std::to_string(slots[i]) + ")";
         if (!features[i]) return fail(NVWN_EINVAL, who + ": the frames of " + u + " are NULL");
         if (num_frames[i] < 1) return fail(NVWN_EINVAL, who + ": " + u + " has num_frames = " + std::to_string(num_frames[i]) + "; need >= 1");
-        if ((long long)num_frames[i] * e->cs_stride > INT_MAX) return fail(NVWN_EINVAL, who + ": " + u + " has more than INT_MAX samples");
+        if ((long long)num_frames[i] * P.stride > INT_MAX) return fail(NVWN_EINVAL, who + ": " + u + " has more than INT_MAX samples");
         if (starts[i] < 0) return fail(NVWN_EINVAL, who + ": " + u + " starts at " + std::to_string(starts[i]) + " < 0");
         if (num_frames[i] > most) most = num_frames[i];
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if (most > e->cs_cap) {
+    if (most > P.cap) {
         // a larger arena; the frames of the other slots move with it
-        const int cap = most > 2 * e->cs_cap ? most : 2 * e->cs_cap;
+        const int cap = most > 2 * P.cap ? most : 2 * P.cap;
         float* grown = nullptr;
         CK(cudaMalloc((void**)&grown, (size_t)e->B * cap * C * sizeof(float)));
-        if (e->cs_frames) {
-            const size_t old_pitch = (size_t)e->cs_cap * C * sizeof(float);
-            cudaError_t ce = cudaMemcpy2DAsync(grown, (size_t)cap * C * sizeof(float), e->cs_frames, old_pitch, old_pitch, e->B, cudaMemcpyDeviceToDevice, st);
+        if (P.frames) {
+            const size_t old_pitch = (size_t)P.cap * C * sizeof(float);
+            cudaError_t ce = cudaMemcpy2DAsync(grown, (size_t)cap * C * sizeof(float), P.frames, old_pitch, old_pitch, e->B, cudaMemcpyDeviceToDevice, st);
             if (ce == cudaSuccess) ce = cudaDeviceSynchronize();             // no launch reads the old arena any more
             if (ce != cudaSuccess) { cudaFree(grown); return fail((int)ce, who + ": " + cudaGetErrorString(ce)); }
-            cudaFree(e->cs_frames);
+            cudaFree(P.frames);
         }
-        e->cs_frames = grown;
-        e->cs_cap = cap;
+        P.frames = grown;
+        P.frames_floats = (size_t)e->B * cap * C;
+        P.cap = cap;
     }
     for (int i = 0; i < n; i++) {
-        float* dst = e->cs_frames + (size_t)slots[i] * e->cs_cap * C;
+        float* dst = P.frames + (size_t)slots[i] * P.cap * C;
         const size_t count = (size_t)C * num_frames[i];
         if (is_device_ptr(features[i])) CK(cudaMemcpyAsync(dst, features[i], count * sizeof(float), cudaMemcpyDeviceToDevice, st));
         else if ((rc = copy_snapshot(dst, features[i], count, st))) return rc;     // staged: the caller may reuse its memory on return
     }
     for (int i = 0; i < n; i++) {
-        e->cs_T[slots[i]] = num_frames[i];
-        e->cs_start[slots[i]] = starts[i];
+        P.T[slots[i]] = num_frames[i];
+        P.start[slots[i]] = starts[i];
     }
     e->slot_rows_used = true;
     return 0;
@@ -706,50 +739,34 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
 {
     const std::string who = "nvwn_cond_producer_run_slots";
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    if (!e->cs_scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
+    const CondProducer& P = e->cond_slots;
+    if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
     int rc = check_slots(e, who.c_str(), slots, n);
     if (rc != 0) return rc;
     if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
         return fail(NVWN_EINVAL, who + ": need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) + ") of the engine");
-    const int C = e->cs_C, L = e->L, R = e->R;
     std::vector<WnCondSlot> tab(n);
     for (int i = 0; i < n; i++) {
         const int s = slots[i];
-        if (e->cs_T[s] < 1)
+        if (P.T[s] < 1)
             return fail(NVWN_EINVAL, who + ": slot " + std::to_string(s) + " has no frames attached (nvwn_cond_producer_set_slots; nvwn_reset_history "
                                            "and nvwn_cond_producer_set_weights forget them)");
-        if (first_sample < e->cs_start[s])
-            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " is before the start " + std::to_string(e->cs_start[s]) +
+        if (first_sample < P.start[s])
+            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " is before the start " + std::to_string(P.start[s]) +
                                          " of slot " + std::to_string(s) + "'s utterance");
-        tab[i] = {(long long)s * e->cs_cap * C, e->cs_start[s], e->cs_T[s], 0};
+        tab[i] = {(long long)s * P.cap * P.C, P.start[s], P.T[s], 0};
     }
     e->slot_rows_used = true;
     if (num_samples == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     // the slot list and the table in one copy, staged from pageable memory: the caller's arrays are free again on return
-    const size_t tab_off = align_up((size_t)e->B * sizeof(int), 16);
+    const size_t tab_off = cond_table_offset(e);
     std::vector<char> host(tab_off + (size_t)n * sizeof(WnCondSlot));
     memcpy(host.data(), slots, (size_t)n * sizeof(int));
     memcpy(host.data() + tab_off, tab.data(), (size_t)n * sizeof(WnCondSlot));
-    CK(cudaMemcpyAsync(e->cs_tables, host.data(), host.size(), cudaMemcpyHostToDevice, st));
-    const int* d_slots = reinterpret_cast<const int*>(e->cs_tables);
-    const WnCondSlot* d_tab = reinterpret_cast<const WnCondSlot*>(e->cs_tables + tab_off);
-
-    const size_t n_wu = (size_t)C * C * e->cs_K, n_wc = (size_t)L * 2 * R * C, n_bc = (size_t)L * 2 * R;
-    const float* d_wut = e->cs_scratch + n_wu; const float* d_bu = d_wut + n_wu; const float* d_wc = d_bu + C; const float* d_bc = d_wc + n_wc;
-    float* d_u = e->cs_scratch + 2 * n_wu + C + n_wc + n_bc;
-    float* d_out = d_u + (size_t)e->cs_rows * C;
-    d_out += (4 - ((size_t)(d_out - e->cs_scratch) & 3)) & 3;                 // 16-byte aligned rows for the tiled projection's float4 stores
-    const int chunk = e->cs_rows / n;                                         // whole samples of every listed slot; >= 1 as cs_rows >= B
-    cudaError_t ce = cudaSuccess;
+    CK(cudaMemcpyAsync(P.tables, host.data(), host.size(), cudaMemcpyHostToDevice, st));
     for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
-        for (int done = 0; done < w.len && ce == cudaSuccess; done += chunk) {
-            const int m = w.len - done < chunk ? w.len - done : chunk;
-            ce = wn_cond_produce_slots(d_out, d_u, e->cs_frames, d_tab, d_wut, d_bu, d_wc, d_bc, n, C, e->cs_K, e->cs_stride, L, R,
-                                       first_sample + w.off + done, m, st);
-            if (ce == cudaSuccess) ce = e->family->convert_rows(*e, e->Lh, d_out, d_slots, n, w.pos + done, m, st);
-        }
-    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
+        if ((rc = produce(e, P, who, slots, n, first_sample + w.off, w.pos, w.len, st))) return rc;
     return 0;
 }
 
@@ -764,7 +781,7 @@ int nvwn_reset_history(nvwn_engine* e)
     e->slot_rows_used = false;
     e->prime_bs = 0;
     e->early_prime = false;
-    e->cs_T.assign(e->B, 0);                      // attached frames: their starts are absolute samples of the old timeline
+    e->cond_slots.T.assign(e->B, 0);              // attached frames: their starts are absolute samples of the old timeline
     return 0;
 }
 

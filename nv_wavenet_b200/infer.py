@@ -116,32 +116,31 @@ class NVWavenetInfer:
         check(self._l.nvwn_set_conditioning(self._h, a, first_sample, num_samples, _stream(stream)), "setConditioning")
         return k
 
+    def _call_with_features(self, fn, name, features, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, *tail):
+        """fn(engine, features, C, T, upsample_weight, upsample_bias, window, stride, cond_weight, cond_bias, *tail) of the
+        whole-batch producer calls, with the arrays' shapes checked; returns T * stride."""
+        shp = lambda a: tuple(a.shape)
+        B, Cc, T = shp(features)
+        assert B == self.B and shp(upsample_weight)[:2] == (Cc, Cc) and shp(cond_weight)[:2] == (self.L * 2 * self.R, Cc)
+        window = shp(upsample_weight)[2]
+        f, k1 = _ptr(features, np.float32); wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
+        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
+        check(fn(self._h, f, Cc, T, wu, bu, window, stride, wc, bc, *tail), name)
+        return T * stride
+
     def set_conditioning_from_features(self, features, upsample_weight, upsample_bias, cond_weight, cond_bias, stride,
                                        first_sample=0, stream=None):
         """Device-side WaveNet.get_cond_input (pytorch/wavenet.py:190-202) + the permutes of pytorch/nv_wavenet.py:48-49,181:
         features [B][C][T], upsample_weight [C][C][window] (ConvTranspose1d), cond_weight [L*2R][C] (or [L*2R][C][1]),
         numpy arrays or torch tensors (host or CUDA).  Fills conditioning for T*stride samples from `first_sample`."""
-        shp = lambda a: tuple(a.shape)
-        B, Cc, T = shp(features)
-        assert B == self.B and shp(upsample_weight)[:2] == (Cc, Cc) and shp(cond_weight)[:2] == (self.L * 2 * self.R, Cc)
-        window = shp(upsample_weight)[2]
-        f, k1 = _ptr(features, np.float32); wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
-        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
-        check(self._l.nvwn_set_conditioning_from_features(self._h, f, Cc, T, wu, bu, window, stride, wc, bc, first_sample,
-                                                          _stream(stream)), "setConditioningFromFeatures")
-        return T * stride
+        return self._call_with_features(self._l.nvwn_set_conditioning_from_features, "setConditioningFromFeatures", features, upsample_weight,
+                                        upsample_bias, cond_weight, cond_bias, stride, first_sample, _stream(stream))
 
     def cond_producer_load(self, features, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, stream=None):
         """First half of set_conditioning_from_features: copies the features and both layers' weights into engine-owned device
         memory.  Returns the number of samples the sequence covers (T * stride)."""
-        shp = lambda a: tuple(a.shape)
-        B, Cc, T = shp(features)
-        assert B == self.B and shp(upsample_weight)[:2] == (Cc, Cc) and shp(cond_weight)[:2] == (self.L * 2 * self.R, Cc)
-        window = shp(upsample_weight)[2]
-        f, k1 = _ptr(features, np.float32); wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
-        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
-        check(self._l.nvwn_cond_producer_load(self._h, f, Cc, T, wu, bu, window, stride, wc, bc, _stream(stream)), "condProducerLoad")
-        return T * stride
+        return self._call_with_features(self._l.nvwn_cond_producer_load, "condProducerLoad", features, upsample_weight, upsample_bias,
+                                        cond_weight, cond_bias, stride, _stream(stream))
 
     def cond_producer_run(self, sample_begin, sample_count, first_sample=0, stream=None):
         """Second half: conditioning of samples [sample_begin, sample_begin + sample_count) of the loaded sequence, asynchronously on
