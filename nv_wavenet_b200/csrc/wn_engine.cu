@@ -4,7 +4,7 @@
 // Re-design of the reference host class nvWavenetInfer<T_weight,T_data,R,S,A> (nv_wavenet.cuh:220-640):
 //   * all weights live in ONE packed device blob (so a multi-GPU job broadcasts it with a single NCCL call);
 //   * fp32 -> fp16 conversion runs on the device from a pinned/device staging area, asynchronously;
-//   * every buffer is freed; pointer kinds are detected with cudaPointerGetAttributes().type
+//   * every buffer frees itself (DevBuf); pointer kinds are detected with cudaPointerGetAttributes().type
 //     (the reference's attributes.memoryType no longer compiles, nv_wavenet_conversions.cuh:41);
 //   * yOut copies use cudaMemcpyDefault, so `samples` may be host or device memory.
 #include "../../include/nvwn_b200.h"
@@ -14,7 +14,9 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace {
@@ -61,17 +63,34 @@ bool is_device_ptr(const void* p)
     return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
 }
 
+// A device allocation that frees itself, and reads as the pointer it holds.  alloc() replaces the buffer only once the new
+// allocation has succeeded: a failed grow leaves the old one in place.
+struct CudaFree {
+    void operator()(void* p) const { cudaFree(p); }
+};
+template <typename T>
+struct DevBuf : std::unique_ptr<T, CudaFree> {
+    operator T*() const { return this->get(); }
+    cudaError_t alloc(size_t bytes)
+    {
+        void* p = nullptr;
+        const cudaError_t ce = cudaMalloc(&p, bytes);
+        if (ce == cudaSuccess) this->reset(static_cast<T*>(p));
+        return ce;
+    }
+};
+
 // A conditioning producer (DESIGN.md §6): a network of C channels, upsampling window K and stride; `scratch` of cond_scratch()'s
 // layout, chunks of up to `rows` (row, sample) rows; row b's frames [C][T[b]] at frames + b * cap * C; the row list and WnCondSlot
 // table of the last production (device); per row on the host, the frames of its utterance (0: none) and its absolute start.
 struct CondProducer {
     int C = 0, K = 0, stride = 0, rows = 0;
-    float* scratch = nullptr;
+    DevBuf<float> scratch;
     size_t scratch_floats = 0;
-    float* frames = nullptr;
+    DevBuf<float> frames;
     size_t frames_floats = 0;
     int cap = 0;
-    char* tables = nullptr;                  // int [B] rows, then WnCondSlot [B] at cond_table_offset
+    DevBuf<char> tables;                     // int [B] rows, then WnCondSlot [B] at cond_table_offset
     std::vector<int> T;
     std::vector<long long> start;
 };
@@ -84,30 +103,28 @@ struct nvwn_engine : WnConfig {
     const WnFamily* family;                  // the kernel family of `kernel`: the layouts of Lh, ring and image, and the launch
 
     // packed weight blob (TD elements), offsets in bytes
-    char* blob = nullptr;
+    DevBuf<char> blob;
     size_t blob_bytes = 0;
     size_t o_embPrev, o_embCur, o_Wprev, o_Wcur, o_Wres, o_Wskip, o_Wzs, o_Wza, o_Bh, o_Bres, o_Bskip, o_Bzs, o_Bza;
 
-    void* Lh = nullptr;                      // TD [N][L][B][2R]
-    float* sel = nullptr;                    // [N][B]
-    int* forced = nullptr;                   // [B][N]
+    DevBuf<void> Lh;                         // TD [N][L][B][2R]
+    DevBuf<float> sel;                       // [N][B]
+    DevBuf<int> forced;                      // [B][N]
     bool use_forced = false;
-    int *yPrev = nullptr, *yCur = nullptr, *yOut = nullptr;
-    void* ring = nullptr;
+    DevBuf<int> yPrev, yCur, yOut;
+    DevBuf<void> ring;
     long long next_t = 0;                    // absolute time of the next sample to generate: where nvwn_run_stream must continue
-    float *xtOut = nullptr, *skipOut = nullptr, *Zs = nullptr, *Za = nullptr, *P = nullptr;
+    DevBuf<float> xtOut, skipOut, Zs, Za, P;
 
-    float* stage_dev = nullptr;              // device fp32 staging for host->fp16 uploads (fp16 engines only)
+    DevBuf<float> stage;                     // device fp32 staging of host sources (feed); fp16 engines allocate it at creation
     size_t stage_elems = 0;
 
     // continuous batching (nvwn_restart_slots): per slot, the absolute sample its utterance started at and its selector key; the
-    // slot indices and seeds of the last per-slot call; fp32 staging of host conditioning for slot rows on engines without stage_dev
-    long long* origin = nullptr;             // [B]
-    unsigned long long* seed = nullptr;      // [B]
-    int* slot_rows = nullptr;                // [B]
-    unsigned long long* slot_seeds = nullptr;    // [B]
-    float* row_stage = nullptr;
-    size_t row_stage_elems = 0;
+    // slot indices and seeds of the last per-slot call
+    DevBuf<long long> origin;                // [B]
+    DevBuf<unsigned long long> seed;         // [B]
+    DevBuf<int> slot_rows;                   // [B]
+    DevBuf<unsigned long long> slot_seeds;   // [B]
     // a per-slot call since the last nvwn_reset_history: its rows (history, conditioning, selectors) sit at the engine's batch
     // stride, which the kernels read at the run's, so until the next reset a run must take the whole batch
     bool slot_rows_used = false;
@@ -118,10 +135,10 @@ struct nvwn_engine : WnConfig {
     // before sample maxDil since the last nvwn_reset_history.  Such a slot's history holds real values at times the kernels would
     // skip as "before the start" (t < d_l), so while this is set every launch reads the ring at every step (fill_params), and the
     // entries of the negative times were zeroed in every row.
-    int* prime_rows = nullptr;
+    DevBuf<int> prime_rows;
     bool early_prime = false;
 
-    void* image = nullptr;                   // the family's weight image, packed from the blob before the first launch after a change
+    DevBuf<void> image;                      // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
 
     // the conditioning producers of the whole-batch calls (nvwn_cond_producer_load / _run / _run_stream) and of the per-slot calls
@@ -130,17 +147,17 @@ struct nvwn_engine : WnConfig {
     CondProducer cond_whole, cond_slots;
 
     // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
-    void* score_image = nullptr;
+    DevBuf<void> score_image;
     bool score_dirty = true;                 // set with image_dirty (weights_changed): the image is repacked on the next scoring call
-    char* score_scratch = nullptr;
+    DevBuf<char> score_scratch;
     int score_T = 0;                         // time steps per chunk: SCORE_ROWS / B
     // the open scoring stream (nvwn_score_stream): the absolute sample its next call starts at, -1 if none is open, and its
     // batch_size; its state is the layer fronts and the codes in score_scratch
     long long score_next = -1;
     int score_bs = 0;
 
-    float* lut_f = nullptr;                  // mu-law decode tables (nvwn_get_audio): A floats, then 2 x A int16 (wrap / saturate)
-    unsigned long long* trace = nullptr;     // debug timeline (nvwn_debug_trace)
+    DevBuf<float> lut_f;                     // mu-law decode tables (nvwn_get_audio): A floats, then 2 x A int16 (wrap / saturate)
+    DevBuf<unsigned long long> trace;        // debug timeline (nvwn_debug_trace)
     int trace_t = -1;
 
     WnLaunchInfo last{};
@@ -151,36 +168,33 @@ struct nvwn_engine : WnConfig {
 
 namespace {
 
-// Hands n units of `unit` fp32 values at `src` (host or device) to convert(src_dev, first_unit, num_units).  fp16 engines bounce a
-// host source through the device staging buffer, whole units at a time, and wait for those copies: the buffer and the source are
-// free again on return.  fp32 engines have no staging buffer: their conversions are copies that also read host memory.
+// Hands n units of `unit` fp32 values at `src` (host or device) to convert(src_dev, first_unit, num_units).  A host source goes
+// through the engine's device staging buffer, whole units at a time, and the call waits for those copies: the buffer and the
+// source are free again on return.  On fp32 engines only the row conversions (`rows`) need that, and allocate the buffer on first
+// need: the other conversions are copies that also read host memory.
 template <typename Convert>
-int feed_via(float* stage, size_t stage_elems, const float* src, size_t n, size_t unit, cudaStream_t stream, Convert convert)
+int feed(nvwn_engine* e, const float* src, size_t n, size_t unit, bool rows, cudaStream_t stream, Convert convert)
 {
     if (n == 0) return 0;
-    if (!stage || is_device_ptr(src)) {
+    if ((e->dtype != NVWN_FP16 && !rows) || is_device_ptr(src)) {
         CK(convert(src, 0, n));
         return 0;
     }
-    const size_t chunk = stage_elems / unit;                                 // >= 1: the callers size the buffer for it
+    if (!e->stage) CK(e->stage.alloc(e->stage_elems * sizeof(float)));
+    const size_t chunk = e->stage_elems / unit;                              // >= 1: stage_elems holds a sample of the whole batch
     for (size_t done = 0; done < n; done += chunk) {
         const size_t m = n - done < chunk ? n - done : chunk;
-        CK(cudaMemcpyAsync(stage, src + done * unit, m * unit * sizeof(float), cudaMemcpyHostToDevice, stream));
-        CK(convert(stage, done, m));
+        CK(cudaMemcpyAsync(e->stage, src + done * unit, m * unit * sizeof(float), cudaMemcpyHostToDevice, stream));
+        CK(convert(e->stage, done, m));
     }
     CK(cudaStreamSynchronize(stream));
     return 0;
-}
-template <typename Convert>
-int feed(nvwn_engine* e, const float* src, size_t n, size_t unit, cudaStream_t stream, Convert convert)
-{
-    return feed_via(e->stage_dev, e->stage_elems, src, n, unit, stream, convert);
 }
 
 // Host array -> device scratch, stream-ordered, through a snapshot in pageable memory: a pageable source is staged before
 // cudaMemcpyAsync returns, so the caller's array (pinned or not) is free again on return.
 template <typename T>
-int copy_snapshot(T* dst_dev, const T* src, size_t n, cudaStream_t stream)
+int copy_snapshot(void* dst_dev, const T* src, size_t n, cudaStream_t stream)
 {
     const std::vector<T> snap(src, src + n);
     CK(cudaMemcpyAsync(dst_dev, snap.data(), n * sizeof(T), cudaMemcpyHostToDevice, stream));
@@ -216,11 +230,11 @@ int put_cond_network(nvwn_engine* e, CondProducer& P, const std::string& who, in
     const size_t rows = ((size_t)16 << 20) / lrow > (size_t)e->B ? ((size_t)16 << 20) / lrow : (size_t)e->B;
     const CondScratch o = cond_scratch(e, C, K, (int)rows);
     if (o.floats > P.scratch_floats) {
-        if (P.scratch) { CK(cudaDeviceSynchronize()); cudaFree(P.scratch); P.scratch = nullptr; P.scratch_floats = 0; }
-        CK(cudaMalloc((void**)&P.scratch, o.floats * sizeof(float)));
+        if (P.scratch) CK(cudaDeviceSynchronize());                         // no launch reads the old scratch any more
+        CK(P.scratch.alloc(o.floats * sizeof(float)));
         P.scratch_floats = o.floats;
     }
-    if (!P.tables) CK(cudaMalloc((void**)&P.tables, cond_table_offset(e) + (size_t)e->B * sizeof(WnCondSlot)));
+    if (!P.tables) CK(P.tables.alloc(cond_table_offset(e) + (size_t)e->B * sizeof(WnCondSlot)));
     P.C = C; P.K = K; P.stride = stride; P.rows = (int)rows;
     float* w = P.scratch;
     cudaError_t ce = cudaSuccess;
@@ -241,7 +255,7 @@ int produce(nvwn_engine* e, const CondProducer& P, const std::string& who, const
 {
     const CondScratch o = cond_scratch(e, P.C, P.K, P.rows);
     float* w = P.scratch;
-    const int* rows_dev = rows ? reinterpret_cast<const int*>(P.tables) : nullptr;
+    const int* rows_dev = rows ? reinterpret_cast<const int*>(P.tables.get()) : nullptr;
     const WnCondSlot* tab = reinterpret_cast<const WnCondSlot*>(P.tables + cond_table_offset(e));
     long long end = LLONG_MAX;                                                // the earliest end of a listed utterance
     for (int i = 0; i < n; i++) {
@@ -263,29 +277,57 @@ int produce(nvwn_engine* e, const CondProducer& P, const std::string& who, const
     return 0;
 }
 
-// Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.
-int check_slots(nvwn_engine* e, const char* who, const int* slots, int n)
+// The window of a call on absolute samples [first_sample, first_sample + count) of the engine's N-sample buffers used as rings:
+// first_sample >= 0 and least <= count <= N.
+int check_window(const nvwn_engine* e, const std::string& who, long long first_sample, int count, const char* count_name, int least)
 {
-    if (!slots) return fail(NVWN_EINVAL, std::string(who) + ": slots is NULL");
-    if (n < 1 || n > e->B) return fail(NVWN_EINVAL, std::string(who) + ": need 1 <= n <= B (" + std::to_string(e->B) + "); got n = " + std::to_string(n));
+    if (first_sample >= 0 && count >= least && count <= e->N) return 0;
+    const std::string got = first_sample < 0 ? "first_sample " + std::to_string(first_sample) + " < 0" : std::string(count_name) + " = " + std::to_string(count);
+    return fail(NVWN_EINVAL, who + ": need first_sample >= 0 and " + std::to_string(least) + " <= " + count_name + " <= num_samples (" +
+                                 std::to_string(e->N) + ") of the engine; got " + got);
+}
+
+// The batch a run, or a prime, may take: the tensor-core kernels take whole batches only, and so does every run after a per-slot
+// call until nvwn_reset_history (slot_rows_used).
+int check_run_batch(const nvwn_engine* e, const std::string& who, int batch)
+{
+    if (e->family->whole_batch && batch != e->B)
+        return fail(NVWN_EINVAL, who + ": the tensor-core path needs batch_size equal to the engine's batch size (" + std::to_string(e->B) + "); got " +
+                                     std::to_string(batch));
+    if (e->slot_rows_used && batch != e->B)
+        return fail(NVWN_EINVAL, who + ": after a per-slot call (nvwn_restart_slots, nvwn_set_conditioning_slots and the other *_slots calls) runs need "
+                                     "batch_size equal to the engine's batch size (" + std::to_string(e->B) + ") until nvwn_reset_history; got " +
+                                     std::to_string(batch));
+    return 0;
+}
+
+// Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.
+int check_slots(const nvwn_engine* e, const std::string& who, const int* slots, int n)
+{
+    if (!slots) return fail(NVWN_EINVAL, who + ": slots is NULL");
+    if (n < 1 || n > e->B) return fail(NVWN_EINVAL, who + ": need 1 <= n <= B (" + std::to_string(e->B) + "); got n = " + std::to_string(n));
     std::vector<char> seen(e->B, 0);
     for (int i = 0; i < n; i++) {
         if (slots[i] < 0 || slots[i] >= e->B)
-            return fail(NVWN_EINVAL, std::string(who) + ": slot " + std::to_string(slots[i]) + " is outside [0, " + std::to_string(e->B) + ")");
-        if (seen[slots[i]]) return fail(NVWN_EINVAL, std::string(who) + ": slot " + std::to_string(slots[i]) + " is given twice");
+            return fail(NVWN_EINVAL, who + ": slot " + std::to_string(slots[i]) + " is outside [0, " + std::to_string(e->B) + ")");
+        if (seen[slots[i]]) return fail(NVWN_EINVAL, who + ": slot " + std::to_string(slots[i]) + " is given twice");
         seen[slots[i]] = 1;
     }
     return 0;
 }
 
-// check_slots, then copies the list to the device scratch slot_rows, stream-ordered, and marks the engine's rows as laid out for
-// runs of the whole batch.
-int take_slots(nvwn_engine* e, const char* who, const int* slots, int n, cudaStream_t stream)
+// check_slots, then copies the list to slot_rows and the seeds, if any, to slot_seeds (device, stream-ordered), and marks the
+// engine's rows as laid out for runs of the whole batch.  *seeds_dev: slot_seeds, or NULL without seeds (every seed 0).
+int take_slots(nvwn_engine* e, const std::string& who, const int* slots, int n, const unsigned long long* seeds,
+               const unsigned long long** seeds_dev, cudaStream_t stream)
 {
-    const int rc = check_slots(e, who, slots, n);
+    int rc = check_slots(e, who, slots, n);
     if (rc != 0) return rc;
     e->slot_rows_used = true;
-    return copy_snapshot(e->slot_rows, slots, n, stream);
+    if ((rc = copy_snapshot(e->slot_rows, slots, n, stream))) return rc;
+    if (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, stream))) return rc;
+    if (seeds_dev) *seeds_dev = seeds ? e->slot_seeds.get() : nullptr;
+    return 0;
 }
 
 // The weights changed: both images are repacked before their next use, and an open scoring stream ends (its carried layer inputs
@@ -299,7 +341,7 @@ void weights_changed(nvwn_engine* e)
 // dst (TD, device) <- src (fp32, host or device), n elements
 int upload(nvwn_engine* e, void* dst, const float* src, size_t n)
 {
-    return feed(e, src, n, 1, 0, [&](const float* s, size_t first, size_t m) {
+    return feed(e, src, n, 1, false, 0, [&](const float* s, size_t first, size_t m) {
         return e->dtype == NVWN_FP16 ? wn_f32_to_f16(static_cast<__half*>(dst) + first, s, m, 0)
                                      : cudaMemcpyAsync(static_cast<float*>(dst) + first, s, m * sizeof(float), cudaMemcpyDefault, 0);
     });
@@ -361,7 +403,7 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, long long t
     p.Wprev = e->blob + e->o_Wprev; p.Wcur = e->blob + e->o_Wcur; p.Wres = e->blob + e->o_Wres; p.Wskip = e->blob + e->o_Wskip;
     p.Wzs = e->blob + e->o_Wzs; p.Wza = e->blob + e->o_Wza;
     p.Bh = e->blob + e->o_Bh; p.Bres = e->blob + e->o_Bres; p.Bskip = e->blob + e->o_Bskip; p.Bzs = e->blob + e->o_Bzs; p.Bza = e->blob + e->o_Bza;
-    p.Lh = e->Lh; p.sel = e->sel; p.forced = e->use_forced ? e->forced : nullptr;
+    p.Lh = e->Lh; p.sel = e->sel; p.forced = e->use_forced ? e->forced.get() : nullptr;
     p.yPrev = e->yPrev; p.yCur = e->yCur; p.ring = e->ring; p.yOut = e->yOut;
     p.xtOut = e->xtOut; p.skipOut = e->skipOut; p.Zs = e->Zs; p.Za = e->Za; p.P = e->P;
     p.trace = e->trace; p.trace_t = e->trace_t;
@@ -374,12 +416,8 @@ int launch_steps(nvwn_engine* e, const char* who, int pos, long long t_abs, int 
     WnParams p;
     fill_params(e, p, pos, t_abs, count, num_samples, batch, dump);
     if (count > 0) {
-        if (e->family->whole_batch && batch != e->B)
-            return fail(NVWN_EINVAL, std::string(who) + ": the tensor-core path needs batch_size equal to the engine's batch size");
-        if (e->slot_rows_used && batch != e->B)
-            return fail(NVWN_EINVAL, std::string(who) + ": after a per-slot call (nvwn_restart_slots, nvwn_set_conditioning_slots, "
-                                     "nvwn_set_selectors_random_slots) runs need batch_size equal to the engine's batch size (" +
-                                     std::to_string(e->B) + ") until nvwn_reset_history");
+        const int rc = check_run_batch(e, who, batch);
+        if (rc != 0) return rc;
         if (e->prime_bs && batch != e->prime_bs)
             return fail(NVWN_EINVAL, std::string(who) + ": after nvwn_prime_from_score runs need batch_size equal to the primed batch_size (" +
                                      std::to_string(e->prime_bs) + ") until nvwn_reset_history; got " + std::to_string(batch));
@@ -420,6 +458,34 @@ ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
     return o;
 }
 
+// The preamble both primes share: an fp16 engine with an open scoring stream of P >= 1 samples.
+int check_prime(const nvwn_engine* e, const std::string& who)
+{
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score, so only they can be primed");
+    if (e->score_next < 1)
+        return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompt with nvwn_score_stream "
+                                       "from first_sample = 0 first");
+    return 0;
+}
+
+// Hands every layer's front of the open scoring stream of P samples to write(layer, src, tau, n): x_l of stream times [tau, P),
+// tau = max(0, P - d_l), as fp16 [n][Bs][R] in the scoring scratch.  These are the entries a generation from stream time P reads
+// (x_l[t - d_l] with t >= P); earlier times are never read (hist_t).
+template <typename Write>
+int put_fronts(const nvwn_engine* e, Write write)
+{
+    const long long P = e->score_next;
+    const __half* xh = reinterpret_cast<const __half*>(e->score_scratch + score_scratch_layout(e, e->score_T).xh);
+    for (int l = 0; l < e->L; l++) {
+        const int d = wn_score_dilation(l, e->maxDil);
+        const long long tau = P - d > 0 ? P - d : 0;
+        CK(write(l, xh + wn_score_xh_offset(l, e->L, e->maxDil, e->score_T, e->B, e->R) + (size_t)(tau - (P - d)) * e->score_bs * e->R, tau,
+                 (int)(P - tau)));
+    }
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -453,7 +519,7 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
         cudaGetLastError();
         return fail(NVWN_EUNSUPPORTED, "nvwn_create: no CUDA device (this engine has no CPU fallback)");
     }
-    nvwn_engine* e = new nvwn_engine();
+    std::unique_ptr<nvwn_engine> e(new nvwn_engine());                 // freed with its buffers on every refusal below
     e->dtype = dtype; e->R = R; e->S = S; e->A = A; e->L = num_layers; e->maxDil = max_dilation;
     e->B = batch_size; e->N = num_samples; e->impl = impl; e->tanhEmbed = tanh_embed ? 1 : 0;
     e->td = dtype == NVWN_FP16 ? 2 : 4;
@@ -473,41 +539,29 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     e->blob_bytes = off;
 
     const size_t Bz = batch_size, Nz = num_samples;
-    if (dtype == NVWN_FP16) {                                          // 64 MB of fp32 staging, or one sample of conditioning if larger
-        const size_t per = L * Bz * 2 * R;
-        e->stage_elems = per > ((size_t)16 << 20) ? per : ((size_t)16 << 20);
-    }
-#define ALLOC(ptr, bytes)                                                                     \
-    do {                                                                                      \
-        cudaError_t _e = cudaMalloc((void**)&(ptr), (bytes));                                 \
-        if (_e != cudaSuccess) {                                                              \
-            int rc = fail((int)_e, std::string("cudaMalloc(" #ptr "): ") + cudaGetErrorString(_e)); \
-            nvwn_destroy(e);                                                                  \
-            return rc;                                                                        \
-        }                                                                                     \
-    } while (0)
-    ALLOC(e->blob, e->blob_bytes);
-    ALLOC(e->Lh, e->family->store_bytes(*e));
-    ALLOC(e->sel, Nz * Bz * sizeof(float));
-    ALLOC(e->forced, Nz * Bz * sizeof(int));
-    ALLOC(e->yPrev, Bz * sizeof(int));
-    ALLOC(e->yCur, Bz * sizeof(int));
-    ALLOC(e->yOut, Nz * Bz * sizeof(int));
+    const size_t per = L * Bz * 2 * R;                                 // 64 MB of fp32 staging, or one sample of conditioning if larger
+    e->stage_elems = per > ((size_t)16 << 20) ? per : ((size_t)16 << 20);
+    CK(e->blob.alloc(e->blob_bytes));
+    CK(e->Lh.alloc(e->family->store_bytes(*e)));
+    CK(e->sel.alloc(Nz * Bz * sizeof(float)));
+    CK(e->forced.alloc(Nz * Bz * sizeof(int)));
+    CK(e->yPrev.alloc(Bz * sizeof(int)));
+    CK(e->yCur.alloc(Bz * sizeof(int)));
+    CK(e->yOut.alloc(Nz * Bz * sizeof(int)));
     const size_t ring_bytes = e->family->ring_bytes(*e);
-    ALLOC(e->ring, ring_bytes);
-    ALLOC(e->xtOut, L * Bz * R * sizeof(float));
-    ALLOC(e->skipOut, L * Bz * S * sizeof(float));
-    ALLOC(e->Zs, Bz * A * sizeof(float));
-    ALLOC(e->Za, Bz * A * sizeof(float));
-    ALLOC(e->P, Bz * A * sizeof(float));
-    ALLOC(e->origin, Bz * sizeof(long long));
-    ALLOC(e->seed, Bz * sizeof(unsigned long long));
-    ALLOC(e->slot_rows, Bz * sizeof(int));
-    ALLOC(e->slot_seeds, Bz * sizeof(unsigned long long));
-    ALLOC(e->prime_rows, Bz * sizeof(int));
-    if (e->stage_elems) ALLOC(e->stage_dev, e->stage_elems * sizeof(float));
-    if (e->family->pack) ALLOC(e->image, e->family->image_bytes(*e));
-#undef ALLOC
+    CK(e->ring.alloc(ring_bytes));
+    CK(e->xtOut.alloc(L * Bz * R * sizeof(float)));
+    CK(e->skipOut.alloc(L * Bz * S * sizeof(float)));
+    CK(e->Zs.alloc(Bz * A * sizeof(float)));
+    CK(e->Za.alloc(Bz * A * sizeof(float)));
+    CK(e->P.alloc(Bz * A * sizeof(float)));
+    CK(e->origin.alloc(Bz * sizeof(long long)));
+    CK(e->seed.alloc(Bz * sizeof(unsigned long long)));
+    CK(e->slot_rows.alloc(Bz * sizeof(int)));
+    CK(e->slot_seeds.alloc(Bz * sizeof(unsigned long long)));
+    CK(e->prime_rows.alloc(Bz * sizeof(int)));
+    if (dtype == NVWN_FP16) CK(e->stage.alloc(e->stage_elems * sizeof(float)));
+    if (e->family->pack) CK(e->image.alloc(e->family->image_bytes(*e)));
     cudaMemsetAsync(e->blob, 0, e->blob_bytes, 0);
     cudaMemsetAsync(e->yOut, 0, Nz * Bz * sizeof(int), 0);
     cudaMemsetAsync(e->ring, 0, ring_bytes, 0);
@@ -520,19 +574,13 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     wn_fill_int(e->yPrev, 128, Bz, 0);
     wn_fill_int(e->yCur, 128, Bz, 0);
     cudaError_t se = cudaDeviceSynchronize();
-    if (se != cudaSuccess) { int rc = fail((int)se, cudaGetErrorString(se)); nvwn_destroy(e); return rc; }
-    *out = e;
+    if (se != cudaSuccess) return fail((int)se, cudaGetErrorString(se));
+    *out = e.release();
     return 0;
 }
 
 int nvwn_destroy(nvwn_engine* e)
 {
-    if (!e) return 0;
-    void* ptrs[] = {e->blob, e->Lh, e->sel, e->forced, e->yPrev, e->yCur, e->yOut, e->ring, e->xtOut, e->skipOut,
-                    e->Zs, e->Za, e->P, e->stage_dev, e->image, e->trace, e->lut_f, e->score_image, e->score_scratch, e->origin, e->seed,
-                    e->slot_rows, e->slot_seeds, e->row_stage, e->prime_rows, e->cond_whole.scratch, e->cond_whole.frames, e->cond_whole.tables,
-                    e->cond_slots.scratch, e->cond_slots.frames, e->cond_slots.tables};
-    for (void* p : ptrs) if (p) cudaFree(p);
     delete e;
     return 0;
 }
@@ -607,8 +655,8 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
     // features [B][C][T] are the frame arena with cap = T, in one copy; row b's utterance starts at sample 0
     const size_t n_feat = (size_t)e->B * C * T;
     if (n_feat > P.frames_floats) {
-        if (P.frames) { CK(cudaDeviceSynchronize()); cudaFree(P.frames); P.frames = nullptr; P.frames_floats = 0; }
-        CK(cudaMalloc((void**)&P.frames, n_feat * sizeof(float)));
+        if (P.frames) CK(cudaDeviceSynchronize());                          // no launch reads the old frames any more
+        CK(P.frames.alloc(n_feat * sizeof(float)));
         P.frames_floats = n_feat;
     }
     P.cap = T;
@@ -640,9 +688,10 @@ int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sa
     if (P.T[0] < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: nvwn_cond_producer_load has not been called");
     const long long Nn = (long long)P.T[0] * P.stride;
     if (sample_begin < 0 || sample_count < 0 || sample_begin + sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: sample range outside num_frames * stride");
-    if (sample_count > e->N) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: more samples than the engine's num_samples (" + std::to_string(e->N) + ")");
+    int rc = check_window(e, "nvwn_cond_producer_run_stream", sample_begin, sample_count, "sample_count", 0);
+    if (rc != 0) return rc;
     for (const WrapPiece& w : split_at_wrap(sample_begin, sample_count, e->N)) {
-        const int rc = produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin + w.off, w.pos, w.len, (cudaStream_t)stream);
+        rc = produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin + w.off, w.pos, w.len, (cudaStream_t)stream);
         if (rc != 0) return rc;
     }
     return 0;
@@ -674,7 +723,7 @@ int nvwn_cond_producer_set_weights(nvwn_engine* e, int n_cond_channels, const fl
     CondProducer& P = e->cond_slots;
     if (P.frames && C != P.C) {                                               // the arena is laid out for the old channel count
         CK(cudaDeviceSynchronize());
-        cudaFree(P.frames); P.frames = nullptr; P.frames_floats = 0; P.cap = 0;
+        P.frames.reset(); P.frames_floats = 0; P.cap = 0;
     }
     P.T.assign(e->B, 0);                                                      // frames attached under the old network are forgotten
     const int rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
@@ -691,7 +740,7 @@ int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const 
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
     CondProducer& P = e->cond_slots;
     if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
-    int rc = check_slots(e, who.c_str(), slots, n);
+    int rc = check_slots(e, who, slots, n);
     if (rc != 0) return rc;
     if (!features || !num_frames || !starts) return fail(NVWN_EINVAL, who + ": features, num_frames or starts is NULL");
     const int C = P.C;
@@ -708,16 +757,15 @@ int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const 
     if (most > P.cap) {
         // a larger arena; the frames of the other slots move with it
         const int cap = most > 2 * P.cap ? most : 2 * P.cap;
-        float* grown = nullptr;
-        CK(cudaMalloc((void**)&grown, (size_t)e->B * cap * C * sizeof(float)));
+        DevBuf<float> grown;
+        CK(grown.alloc((size_t)e->B * cap * C * sizeof(float)));
         if (P.frames) {
             const size_t old_pitch = (size_t)P.cap * C * sizeof(float);
             cudaError_t ce = cudaMemcpy2DAsync(grown, (size_t)cap * C * sizeof(float), P.frames, old_pitch, old_pitch, e->B, cudaMemcpyDeviceToDevice, st);
             if (ce == cudaSuccess) ce = cudaDeviceSynchronize();             // no launch reads the old arena any more
-            if (ce != cudaSuccess) { cudaFree(grown); return fail((int)ce, who + ": " + cudaGetErrorString(ce)); }
-            cudaFree(P.frames);
+            if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
         }
-        P.frames = grown;
+        P.frames = std::move(grown);
         P.frames_floats = (size_t)e->B * cap * C;
         P.cap = cap;
     }
@@ -741,10 +789,9 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
     const CondProducer& P = e->cond_slots;
     if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
-    int rc = check_slots(e, who.c_str(), slots, n);
+    int rc = check_slots(e, who, slots, n);
+    if (rc == 0) rc = check_window(e, who, first_sample, num_samples, "num_samples", 0);
     if (rc != 0) return rc;
-    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
-        return fail(NVWN_EINVAL, who + ": need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) + ") of the engine");
     std::vector<WnCondSlot> tab(n);
     for (int i = 0; i < n; i++) {
         const int s = slots[i];
@@ -789,42 +836,27 @@ int nvwn_restart_slots(nvwn_engine* e, const int* slots, int n, const unsigned l
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_restart_slots: NULL engine");
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = take_slots(e, "nvwn_restart_slots", slots, n, st);
+    const unsigned long long* seeds_dev;
+    const int rc = take_slots(e, "nvwn_restart_slots", slots, n, seeds, &seeds_dev, st);
     if (rc != 0) return rc;
-    if (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st))) return rc;
     // a zero history row and silence fed back are exactly the state of a fresh start (DESIGN.md §6)
     CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
-    CK(wn_restart_rows(e->slot_rows, n, seeds ? e->slot_seeds : nullptr, e->next_t, e->yPrev, e->yCur, e->origin, e->seed, st));
+    CK(wn_restart_rows(e->slot_rows, n, seeds_dev, e->next_t, e->yPrev, e->yCur, e->origin, e->seed, st));
     return 0;
 }
 
 int nvwn_set_conditioning_slots(nvwn_engine* e, const float* Lh, const int* slots, int n, long long first_sample, int num_samples, void* stream)
 {
-    if (!e) return fail(NVWN_EINVAL, "nvwn_set_conditioning_slots: NULL engine");
-    if (!Lh) return fail(NVWN_EINVAL, "nvwn_set_conditioning_slots: Lh is NULL");
-    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
-        return fail(NVWN_EINVAL, "nvwn_set_conditioning_slots: need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) +
-                                     ") of the engine");
+    const std::string who = "nvwn_set_conditioning_slots";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (!Lh) return fail(NVWN_EINVAL, who + ": Lh is NULL");
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = take_slots(e, "nvwn_set_conditioning_slots", slots, n, st);
+    int rc = check_window(e, who, first_sample, num_samples, "num_samples", 0);
+    if (rc == 0) rc = take_slots(e, who, slots, n, nullptr, nullptr, st);
     if (rc != 0) return rc;
     const size_t unit = (size_t)e->L * n * 2 * e->R;                        // floats per sample
-    float* stage = e->stage_dev;
-    size_t stage_elems = e->stage_elems;
-    if (!stage && num_samples > 0 && !is_device_ptr(Lh)) {
-        // the row conversions are kernels: a host source goes through device memory on fp32 engines too
-        size_t want = (size_t)num_samples * unit;
-        if (want > ((size_t)16 << 20)) want = unit > ((size_t)16 << 20) ? unit : ((size_t)16 << 20);
-        if (want > e->row_stage_elems) {
-            if (e->row_stage) { CK(cudaStreamSynchronize(st)); cudaFree(e->row_stage); e->row_stage = nullptr; e->row_stage_elems = 0; }
-            CK(cudaMalloc((void**)&e->row_stage, want * sizeof(float)));
-            e->row_stage_elems = want;
-        }
-        stage = e->row_stage;
-        stage_elems = e->row_stage_elems;
-    }
     for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N)) {
-        rc = feed_via(stage, stage_elems, Lh + (size_t)w.off * unit, (size_t)w.len, unit, st, [&](const float* s, size_t first, size_t m) {
+        rc = feed(e, Lh + (size_t)w.off * unit, (size_t)w.len, unit, true, st, [&](const float* s, size_t first, size_t m) {
             return e->family->convert_rows(*e, e->Lh, s, e->slot_rows, n, w.pos + (int)first, (int)m, st);
         });
         if (rc != 0) return rc;
@@ -835,9 +867,8 @@ int nvwn_set_conditioning_slots(nvwn_engine* e, const float* Lh, const int* slot
 int nvwn_set_selectors_random_slots(nvwn_engine* e, long long first_sample, int num_samples, void* stream)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_set_selectors_random_slots: NULL engine");
-    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
-        return fail(NVWN_EINVAL, "nvwn_set_selectors_random_slots: need first_sample >= 0 and 0 <= num_samples <= num_samples (" +
-                                     std::to_string(e->N) + ") of the engine");
+    const int rc = check_window(e, "nvwn_set_selectors_random_slots", first_sample, num_samples, "num_samples", 0);
+    if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t B = e->B;
     e->slot_rows_used = true;
@@ -880,8 +911,8 @@ int nvwn_set_selectors_random(nvwn_engine* e, unsigned long long seed, void* str
 int nvwn_set_selectors_random_stream(nvwn_engine* e, unsigned long long seed, long long first_sample, int num_samples, void* stream)
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_set_selectors_random_stream: NULL engine");
-    if (first_sample < 0 || num_samples < 0 || num_samples > e->N)
-        return fail(NVWN_EINVAL, "nvwn_set_selectors_random_stream: need first_sample >= 0 and 0 <= num_samples <= num_samples (" + std::to_string(e->N) + ") of the engine");
+    const int rc = check_window(e, "nvwn_set_selectors_random_stream", first_sample, num_samples, "num_samples", 0);
+    if (rc != 0) return rc;
     const size_t B = e->B;
     for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
         CK(wn_fill_selectors(e->sel + (size_t)w.pos * B, (size_t)w.len * B, seed, (unsigned long long)(first_sample + w.off) * B, (cudaStream_t)stream));
@@ -893,7 +924,7 @@ int nvwn_set_conditioning(nvwn_engine* e, const float* Lh, int first_sample, int
     if (!e || !Lh) return fail(NVWN_EINVAL, "nvwn_set_conditioning: NULL argument");
     if (first_sample < 0 || num_samples < 0 || first_sample + num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_set_conditioning: sample range out of bounds");
     cudaStream_t st = (cudaStream_t)stream;
-    return feed(e, Lh, num_samples, (size_t)e->L * e->B * 2 * e->R, st, [&](const float* src, size_t first, size_t m) {
+    return feed(e, Lh, num_samples, (size_t)e->L * e->B * 2 * e->R, false, st, [&](const float* src, size_t first, size_t m) {
         return e->family->convert(*e, e->Lh, src, first_sample + (int)first, (int)m, st);
     });
 }
@@ -951,17 +982,16 @@ int nvwn_run_stream(nvwn_engine* e, long long first_sample, int count, int batch
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_run_stream: NULL engine");
     if (batch_size < 1 || batch_size > e->B) return fail(NVWN_EINVAL, "nvwn_run_stream: batch_size outside [1, B] of the engine");
-    if (first_sample < 0 || count < 0 || count > e->N)
-        return fail(NVWN_EINVAL, "nvwn_run_stream: need first_sample >= 0 and 0 <= count <= num_samples (" + std::to_string(e->N) + ") of the engine");
+    int rc = check_window(e, "nvwn_run_stream", first_sample, count, "count", 0);
+    if (rc != 0) return rc;
     if (first_sample != e->next_t)
         return fail(NVWN_EINVAL, "nvwn_run_stream: first_sample " + std::to_string(first_sample) + " does not continue the utterance batch: the next sample is " +
                                      std::to_string(e->next_t) + " (nvwn_reset_history starts over at 0)");
     cudaStream_t stream = (cudaStream_t)stream_;
     const int dump = dump_activations ? 1 : 0;
-    for (const WrapPiece& w : split_at_wrap(first_sample, count, e->N)) {
-        const int rc = launch_steps(e, "nvwn_run_stream", w.pos, first_sample + w.off, w.len, e->N, batch_size, w.off + w.len == count ? dump : 0, stream);
-        if (rc != 0) return rc;
-    }
+    for (const WrapPiece& w : split_at_wrap(first_sample, count, e->N))
+        if ((rc = launch_steps(e, "nvwn_run_stream", w.pos, first_sample + w.off, w.len, e->N, batch_size, w.off + w.len == count ? dump : 0, stream)))
+            return rc;
     return 0;
 }
 
@@ -1031,7 +1061,7 @@ int nvwn_get_audio(nvwn_engine* e, float* audio_f32, short* audio_i16, int offse
         float* hf = reinterpret_cast<float*>(host.data());
         short* hw = reinterpret_cast<short*>(host.data() + (size_t)A * sizeof(float));
         nvwn_mulaw_table(A, hf, hw, hw + A);
-        CK(cudaMalloc((void**)&e->lut_f, host.size()));
+        CK(e->lut_f.alloc(host.size()));
         CK(cudaMemcpy(e->lut_f, host.data(), host.size(), cudaMemcpyHostToDevice));
     }
     const short* lut_s = reinterpret_cast<const short*>(e->lut_f + A) + (saturate ? A : 0);
@@ -1039,19 +1069,16 @@ int nvwn_get_audio(nvwn_engine* e, float* audio_f32, short* audio_i16, int offse
     const bool f_dev = !audio_f32 || is_device_ptr(audio_f32), s_dev = !audio_i16 || is_device_ptr(audio_i16);
     float* df = audio_f32;
     short* ds = audio_i16;
-    void* tmp = nullptr;
+    DevBuf<char> tmp;
     if (!f_dev || !s_dev) {                                                   // host destination(s): decode into a device scratch, copy out
-        CK(cudaMalloc(&tmp, total * (sizeof(float) + sizeof(short))));
-        if (!f_dev) df = static_cast<float*>(tmp);
-        if (!s_dev) ds = reinterpret_cast<short*>(static_cast<char*>(tmp) + total * sizeof(float));
+        CK(tmp.alloc(total * (sizeof(float) + sizeof(short))));
+        if (!f_dev) df = reinterpret_cast<float*>(tmp.get());
+        if (!s_dev) ds = reinterpret_cast<short*>(tmp + total * sizeof(float));
     }
     cudaError_t ce = wn_mulaw_decode(e->yOut, e->N, offset, size, e->B, A, e->lut_f, lut_s, df, ds, st);
     if (ce == cudaSuccess && !f_dev) ce = cudaMemcpyAsync(audio_f32, df, total * sizeof(float), cudaMemcpyDeviceToHost, st);
     if (ce == cudaSuccess && !s_dev) ce = cudaMemcpyAsync(audio_i16, ds, total * sizeof(short), cudaMemcpyDeviceToHost, st);
-    if (tmp) {
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-        cudaFree(tmp);
-    }
+    if (tmp && ce == cudaSuccess) ce = cudaStreamSynchronize(st);            // before tmp is freed on return
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_get_audio: ") + cudaGetErrorString(ce));
     return 0;
 }
@@ -1084,9 +1111,10 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, long long fir
         if (T < 1) T = 1;
         if (T > e->N) T = e->N;
         const ScoreScratch o = score_scratch_layout(e, T);
-        CK(cudaMalloc((void**)&e->score_scratch, o.bytes));
-        cudaError_t ce = cudaMalloc(&e->score_image, wn_score_image_bytes(R, e->S, A, L));
-        if (ce != cudaSuccess) { cudaFree(e->score_scratch); e->score_scratch = nullptr; CK(ce); }
+        DevBuf<char> scratch;                // kept only with the image: a scratch means both are there
+        CK(scratch.alloc(o.bytes));
+        CK(e->score_image.alloc(wn_score_image_bytes(R, e->S, A, L)));
+        e->score_scratch = std::move(scratch);
         e->score_T = T;
         e->score_dirty = true;
     }
@@ -1192,10 +1220,8 @@ int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, 
 {
     const std::string who = "nvwn_score_stream";
     int rc = score_args(e, who.c_str(), audio, batch_size, logp);
+    if (rc == 0) rc = check_window(e, who, first_sample, count, "count", 1);
     if (rc != 0) return rc;
-    if (count < 1 || count > e->N)
-        return fail(NVWN_EINVAL, who + ": count " + std::to_string(count) + " is outside [1, " + std::to_string(e->N) + "] (num_samples of the engine)");
-    if (first_sample < 0) return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " < 0");
     if (first_sample != 0) {
         if (e->score_next < 0)
             return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " continues no scoring stream (nvwn_score and weight "
@@ -1213,33 +1239,17 @@ int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, 
 int nvwn_prime_from_score(nvwn_engine* e, void* stream)
 {
     const std::string who = "nvwn_prime_from_score";
-    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score, so only they can be primed");
-    if (e->score_next < 1)
-        return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompt with nvwn_score_stream "
-                                       "from first_sample = 0 first");
-    const int Bs = e->score_bs;
-    if (e->family->whole_batch && Bs != e->B)
-        return fail(NVWN_EINVAL, who + ": the tensor-core path needs the scoring stream's batch_size (" + std::to_string(Bs) +
-                                     ") equal to the engine's batch size (" + std::to_string(e->B) + ")");
-    if (e->slot_rows_used && Bs != e->B)
-        return fail(NVWN_EINVAL, who + ": after a per-slot call the scoring stream's batch_size (" + std::to_string(Bs) +
-                                     ") must equal the engine's batch size (" + std::to_string(e->B) + ") until nvwn_reset_history");
+    int rc = check_prime(e, who);
+    if (rc == 0) rc = check_run_batch(e, who, e->score_bs);
+    if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const long long P = e->score_next;
-    const int T = e->score_T, R = e->R, L = e->L;
-    const ScoreScratch o = score_scratch_layout(e, T);
-    const __half* xh = reinterpret_cast<const __half*>(e->score_scratch + o.xh);
-    // layer l's front holds x_l of times [P - d_l, P), d_l rows of Bs utterances: the entries with t >= 0 are the ring entries a
-    // generation from sample P reads (x_l[t - d_l] with t >= P); earlier times are never read (hist_t)
-    for (int l = 0; l < L; l++) {
-        const int d = wn_score_dilation(l, e->maxDil);
-        const long long t_first = P - d > 0 ? P - d : 0;
-        const __half* src = xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R) + (size_t)(t_first - (P - d)) * Bs * R;
-        CK(e->family->put_history(*e, e->ring, src, l, t_first, (int)(P - t_first), Bs, st));
-    }
-    CK(wn_feedback_from_codes(reinterpret_cast<const int*>(e->score_scratch + o.codes), Bs, e->yPrev, e->yCur, st));
-    e->next_t = P;
+    const int Bs = e->score_bs;
+    rc = put_fronts(e, [&](int l, const __half* src, long long t_first, int n_t) {
+        return e->family->put_history(*e, e->ring, src, l, t_first, n_t, Bs, st);
+    });
+    if (rc != 0) return rc;
+    CK(wn_feedback_from_codes(reinterpret_cast<const int*>(e->score_scratch + score_scratch_layout(e, e->score_T).codes), Bs, e->yPrev, e->yCur, st));
+    e->next_t = e->score_next;
     e->prime_bs = Bs;
     return 0;
 }
@@ -1247,14 +1257,10 @@ int nvwn_prime_from_score(nvwn_engine* e, void* stream)
 int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slots, int n, const unsigned long long* seeds, void* stream)
 {
     const std::string who = "nvwn_prime_slots_from_score";
-    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score, so only they can be primed");
-    if (!rows) return fail(NVWN_EINVAL, who + ": rows is NULL");
-    if (e->score_next < 1)
-        return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompts with nvwn_score_stream "
-                                       "from first_sample = 0 first");
-    int rc = check_slots(e, who.c_str(), slots, n);
+    int rc = check_prime(e, who);
     if (rc != 0) return rc;
+    if (!rows) return fail(NVWN_EINVAL, who + ": rows is NULL");
+    if ((rc = check_slots(e, who, slots, n))) return rc;
     const int Bs = e->score_bs;
     std::vector<char> seen(Bs, 0);
     for (int i = 0; i < n; i++) {
@@ -1264,10 +1270,10 @@ int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slot
         seen[rows[i]] = 1;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = take_slots(e, who.c_str(), slots, n, st)) || (rc = copy_snapshot(e->prime_rows, rows, n, st))) return rc;
-    if (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st))) return rc;
+    const unsigned long long* seeds_dev;
+    if ((rc = take_slots(e, who, slots, n, seeds, &seeds_dev, st)) || (rc = copy_snapshot(e->prime_rows, rows, n, st))) return rc;
     const long long P = e->score_next, t0 = e->next_t, origin = t0 - P;
-    const int M = e->maxDil + 1, T = e->score_T, R = e->R, L = e->L;
+    const int M = e->maxDil + 1;
     if (t0 < e->maxDil && !e->early_prime) {
         // from now on every launch reads the ring at every step: the entries of the negative times, which no row has written since
         // the reset, must read as the zeros the kernels stage for "before the start"
@@ -1275,18 +1281,14 @@ int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slot
         e->early_prime = true;
     }
     // what nvwn_restart_slots at t0 - P does to these slots, then nvwn_prime_from_score of their rows with local time tau at engine
-    // time t0 - P + tau: layer l's front of times tau in [max(0, P - d_l), P)
+    // time t0 - P + tau
     CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
-    const ScoreScratch o = score_scratch_layout(e, T);
-    const __half* xh = reinterpret_cast<const __half*>(e->score_scratch + o.xh);
-    for (int l = 0; l < L; l++) {
-        const int d = wn_score_dilation(l, e->maxDil);
-        const long long tau = P - d > 0 ? P - d : 0;
-        const __half* src = xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R) + (size_t)(tau - (P - d)) * Bs * R;
-        CK(e->family->put_history_rows(*e, e->ring, src, Bs, e->prime_rows, e->slot_rows, n, l, origin + tau, (int)(P - tau), st));
-    }
-    CK(wn_prime_rows(reinterpret_cast<const int*>(e->score_scratch + o.codes), e->prime_rows, e->slot_rows, n, seeds ? e->slot_seeds : nullptr, origin,
-                     e->yPrev, e->yCur, e->origin, e->seed, st));
+    rc = put_fronts(e, [&](int l, const __half* src, long long tau, int n_t) {
+        return e->family->put_history_rows(*e, e->ring, src, Bs, e->prime_rows, e->slot_rows, n, l, origin + tau, n_t, st);
+    });
+    if (rc != 0) return rc;
+    CK(wn_prime_rows(reinterpret_cast<const int*>(e->score_scratch + score_scratch_layout(e, e->score_T).codes), e->prime_rows, e->slot_rows, n, seeds_dev,
+                     origin, e->yPrev, e->yCur, e->origin, e->seed, st));
     return 0;
 }
 
@@ -1298,11 +1300,10 @@ int nvwn_debug_get_conditioning(nvwn_engine* e, float* out, int first_sample, in
     if (first_sample < 0 || num_samples < 0 || first_sample + num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_debug_get_conditioning: range out of bounds");
     const size_t per = (size_t)e->L * e->B * 2 * e->R, n = per * num_samples;
     if (n == 0) return 0;
-    float* tmp = nullptr;
-    CK(cudaMalloc((void**)&tmp, n * sizeof(float)));
+    DevBuf<float> tmp;
+    CK(tmp.alloc(n * sizeof(float)));
     cudaError_t ce = e->family->readback(*e, tmp, e->Lh, first_sample, num_samples, 0);
     if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
-    cudaFree(tmp);
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_conditioning: ") + cudaGetErrorString(ce));
     return 0;
 }
@@ -1314,11 +1315,10 @@ int nvwn_debug_get_history(nvwn_engine* e, float* out, int batch)
     if (!e || !out) return fail(NVWN_EINVAL, "nvwn_debug_get_history: NULL argument");
     if (batch < 1 || batch > e->B) return fail(NVWN_EINVAL, "nvwn_debug_get_history: batch outside [1, B]");
     const size_t n = (size_t)(e->maxDil + 1) * e->L * batch * e->R;
-    float* tmp = nullptr;
-    CK(cudaMalloc((void**)&tmp, n * sizeof(float)));
+    DevBuf<float> tmp;
+    CK(tmp.alloc(n * sizeof(float)));
     cudaError_t ce = e->family->get_history(*e, tmp, e->ring, batch, 0);
     if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
-    cudaFree(tmp);
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_history: ") + cudaGetErrorString(ce));
     return 0;
 }
@@ -1328,7 +1328,7 @@ int nvwn_debug_trace(nvwn_engine* e, int t, unsigned long long* out_host, int fe
 {
     if (!e) return NVWN_EINVAL;
     if (!fetch) {
-        if (!e->trace) CK(cudaMalloc((void**)&e->trace, 3 * 1024 * sizeof(unsigned long long)));
+        if (!e->trace) CK(e->trace.alloc(3 * 1024 * sizeof(unsigned long long)));
         CK(cudaMemset(e->trace, 0, 3 * 1024 * sizeof(unsigned long long)));
         e->trace_t = t;
         return 0;

@@ -116,13 +116,25 @@ class NVWavenetInfer:
         check(self._l.nvwn_set_conditioning(self._h, a, first_sample, num_samples, _stream(stream)), "setConditioning")
         return k
 
+    def _check_network(self, what, upsample_weight, upsample_bias, cond_weight, cond_bias):
+        """(C, window) of a conditioning network, upsample_weight [C][C][window], upsample_bias [C], cond_weight [L*2R][C] (or
+        [L*2R][C][1]), cond_bias [L*2R]; ValueError naming `what` for other shapes."""
+        shp = lambda a: tuple(int(v) for v in a.shape)
+        lr, Cc = self.L * 2 * self.R, shp(upsample_weight)[0]
+        if (len(shp(upsample_weight)) != 3 or shp(upsample_weight)[1] != Cc or shp(upsample_bias) != (Cc,)
+                or shp(cond_weight)[:2] != (lr, Cc) or shp(cond_bias) != (lr,)):
+            raise ValueError(f"{what}: need upsample_weight [C][C][window], upsample_bias [C], cond_weight [{lr}][C], cond_bias [{lr}]; "
+                             f"got {shp(upsample_weight)}, {shp(upsample_bias)}, {shp(cond_weight)}, {shp(cond_bias)}")
+        return Cc, shp(upsample_weight)[2]
+
     def _call_with_features(self, fn, name, features, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, *tail):
         """fn(engine, features, C, T, upsample_weight, upsample_bias, window, stride, cond_weight, cond_bias, *tail) of the
         whole-batch producer calls, with the arrays' shapes checked; returns T * stride."""
-        shp = lambda a: tuple(a.shape)
-        B, Cc, T = shp(features)
-        assert B == self.B and shp(upsample_weight)[:2] == (Cc, Cc) and shp(cond_weight)[:2] == (self.L * 2 * self.R, Cc)
-        window = shp(upsample_weight)[2]
+        Cc, window = self._check_network(name, upsample_weight, upsample_bias, cond_weight, cond_bias)
+        shape = tuple(int(v) for v in features.shape)
+        if len(shape) != 3 or shape[:2] != (self.B, Cc):
+            raise ValueError(f"{name}: features must be [{self.B}][{Cc}][T] for this engine and network; got {shape}")
+        T = shape[2]
         f, k1 = _ptr(features, np.float32); wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
         wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
         check(fn(self._h, f, Cc, T, wu, bu, window, stride, wc, bc, *tail), name)
@@ -201,18 +213,23 @@ class NVWavenetInfer:
         s = np.ascontiguousarray(np.asarray(slots, dtype=np.int64).reshape(-1)).astype(np.int32)
         return C.c_void_p(s.ctypes.data), s
 
+    @staticmethod
+    def _seeds(what, seeds, n):
+        """(void* or None, keepalive) of one uint64 seed per slot of n slots; None: no seeds (every seed 0)."""
+        if seeds is None:
+            return None, None
+        k = np.ascontiguousarray([int(v) & (2 ** 64 - 1) for v in seeds], dtype=np.uint64)
+        if k.size != n:
+            raise ValueError(f"{what}: {n} slots but {k.size} seeds")
+        return C.c_void_p(k.ctypes.data), k
+
     def restart_slots(self, slots, seeds=None, stream=None):
         """Starts a new utterance in each of `slots` at the engine's next sample: their history is cleared and silence fed back,
         the other slots are not touched.  seeds (one per slot, None = 0) key the slots' selectors for
         set_selectors_random_slots.  Asynchronous on `stream`."""
         p, s = self._slots(slots)
-        k = None
-        if seeds is not None:
-            k = np.ascontiguousarray([int(v) & (2 ** 64 - 1) for v in seeds], dtype=np.uint64)
-            if k.size != s.size:
-                raise ValueError(f"restart_slots: {s.size} slots but {k.size} seeds")
-        check(self._l.nvwn_restart_slots(self._h, p, s.size, None if k is None else C.c_void_p(k.ctypes.data), _stream(stream)),
-              "restartSlots")
+        k, keep = self._seeds("restart_slots", seeds, s.size)
+        check(self._l.nvwn_restart_slots(self._h, p, s.size, k, _stream(stream)), "restartSlots")
 
     def set_conditioning_slots(self, Lh, slots, first_sample, stream=None):
         """Lh [n][L][k][2R] (numpy array or CUDA tensor): the conditioning of absolute samples [first_sample, first_sample + n)
@@ -236,14 +253,7 @@ class NVWavenetInfer:
     def cond_producer_set_weights(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, stream=None):
         """The conditioning network of set_conditioning_from_features (upsample_weight [C][C][window], upsample_bias [C],
         cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]), for cond_producer_run_slots.  Forgets every attached utterance."""
-        shp = lambda a: tuple(int(v) for v in a.shape)
-        Cc = shp(upsample_weight)[0]
-        if (len(shp(upsample_weight)) != 3 or shp(upsample_weight)[1] != Cc or shp(upsample_bias) != (Cc,)
-                or shp(cond_weight)[:2] != (self.L * 2 * self.R, Cc) or shp(cond_bias) != (self.L * 2 * self.R,)):
-            raise ValueError(f"cond_producer_set_weights: need upsample_weight [C][C][window], upsample_bias [C], cond_weight "
-                             f"[{self.L * 2 * self.R}][C], cond_bias [{self.L * 2 * self.R}]; got {shp(upsample_weight)}, {shp(upsample_bias)}, "
-                             f"{shp(cond_weight)}, {shp(cond_bias)}")
-        window = shp(upsample_weight)[2]
+        Cc, window = self._check_network("cond_producer_set_weights", upsample_weight, upsample_bias, cond_weight, cond_bias)
         wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
         wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
         check(self._l.nvwn_cond_producer_set_weights(self._h, Cc, wu, bu, window, stride, wc, bc, _stream(stream)), "condProducerSetWeights")
@@ -320,12 +330,15 @@ class NVWavenetInfer:
         if out is None:
             out = np.empty((self.B, size), np.int16 if int16 else np.float32)
         if isinstance(out, np.ndarray):
-            assert out.flags["C_CONTIGUOUS"] and out.dtype == (np.int16 if int16 else np.float32) and out.size == self.B * size
+            ok = out.flags["C_CONTIGUOUS"] and out.dtype == (np.int16 if int16 else np.float32) and out.size == self.B * size
             p = C.c_void_p(out.ctypes.data)
         else:                               # torch tensor
             import torch
-            assert out.is_contiguous() and out.dtype == (torch.int16 if int16 else torch.float32) and out.numel() == self.B * size
+            ok = out.is_contiguous() and out.dtype == (torch.int16 if int16 else torch.float32) and out.numel() == self.B * size
             p = C.c_void_p(out.data_ptr())
+        if not ok:                          # the library writes B * size values into it
+            raise ValueError(f"get_audio: out must be contiguous {'int16' if int16 else 'float32'} [{self.B}][{size}]; got "
+                             f"{out.dtype} {tuple(out.shape)}")
         check(self._l.nvwn_get_audio(self._h, None if int16 else p, p if int16 else None, offset, size, int(saturate),
                                      _stream(stream)), "getAudio")
         return out
@@ -360,13 +373,8 @@ class NVWavenetInfer:
         r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1)).astype(np.int32)
         if r.size != s.size:
             raise ValueError(f"prime_slots_from_score: {s.size} slots but {r.size} rows")
-        k = None
-        if seeds is not None:
-            k = np.ascontiguousarray([int(v) & (2 ** 64 - 1) for v in seeds], dtype=np.uint64)
-            if k.size != s.size:
-                raise ValueError(f"prime_slots_from_score: {s.size} slots but {k.size} seeds")
-        check(self._l.nvwn_prime_slots_from_score(self._h, C.c_void_p(r.ctypes.data), p, s.size, None if k is None else C.c_void_p(k.ctypes.data),
-                                                  _stream(stream)), "primeSlotsFromScore")
+        k, keep = self._seeds("prime_slots_from_score", seeds, s.size)
+        check(self._l.nvwn_prime_slots_from_score(self._h, C.c_void_p(r.ctypes.data), p, s.size, k, _stream(stream)), "primeSlotsFromScore")
 
     def _score(self, audio, num_samples, batch_size, logits, what, call):
         """audio[:batch_size, :num_samples] as int32 and the outputs of score() in matching memory; call(audio, n, bs, logp, logits)

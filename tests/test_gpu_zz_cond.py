@@ -85,6 +85,9 @@ def test_out_of_range_is_rejected():
     with pytest.raises(Exception):
         e.set_conditioning_from_features(z, np.zeros((3, 3, 8), np.float32), np.zeros(3, np.float32), np.zeros((2 * 2 * 64, 3), np.float32),
                                          np.zeros(2 * 2 * 64, np.float32), 4)        # 5 * 4 = 20 samples > 16
+    with pytest.raises(ValueError):
+        e.set_conditioning_from_features(np.zeros((3, 3, 4), np.float32), np.zeros((3, 3, 8), np.float32), np.zeros(3, np.float32),
+                                         np.zeros((2 * 2 * 64, 3), np.float32), np.zeros(2 * 2 * 64, np.float32), 4)   # 3 utterances, B = 2
 
 
 def test_producer_ranges_on_a_side_stream_equal_the_one_shot_call_and_the_host_arithmetic():

@@ -160,6 +160,25 @@ def test_conditioning_slots_write_only_their_rows(kind, monkeypatch):
     assert bits_equal(got, want), np.argwhere(got.view(np.uint32) != want.view(np.uint32))[:5]
 
 
+def test_conditioning_slots_fp32_host_source_over_several_staging_chunks(monkeypatch):
+    """On an fp32 engine a host source reaches the row conversion through the 64 MB staging buffer: a source of more samples than
+    one chunk holds, across the wrap, leaves the same store as the same values from device memory, and the values themselves."""
+    import torch
+    B, N, shift = 8, 1500, 100
+    slots = [7, 0, 3, 5, 1, 6, 2, 4]
+    new = np.random.default_rng(43).standard_normal((N, L, B, 2 * R)).astype(np.float32)
+    assert new[:N - shift].nbytes > 64 << 20                              # the piece before the wrap takes two chunks
+    want = np.empty_like(new)
+    want[:, :, slots] = new
+    want = np.roll(want, shift, axis=0)                                   # sample N + shift + i sits at position (shift + i) mod N
+    for src in (new, torch.from_numpy(new).cuda()):
+        e = _eng("fp32", B, N, monkeypatch)
+        e.set_conditioning_slots(src, slots, N + shift)
+        torch.cuda.synchronize()
+        assert bits_equal(_store(e), want), "host" if src is new else "device"
+        e.close()
+
+
 def test_selectors_per_slot(monkeypatch):
     """Per-slot selectors equal the host restatement (counter t - origin, key seed) and a one-utterance engine's stream draw."""
     B, W, Tn = 5, 16, 40
