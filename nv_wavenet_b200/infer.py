@@ -42,6 +42,21 @@ def _stream(stream):
     return C.c_void_p(int(stream))
 
 
+def check_cond_network(num_layers, R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, error, what):
+    """(C, window) of a conditioning network for num_layers layers of R residual channels: upsample_weight [C][C][window],
+    upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R], and window >= stride >= 1.  Raises error(message
+    naming `what`) for anything else."""
+    shp = lambda a: tuple(int(v) for v in a.shape)
+    lr, wu = num_layers * 2 * R, shp(upsample_weight)
+    Cc = wu[0] if len(wu) == 3 and wu[0] == wu[1] else None
+    if Cc is None or shp(upsample_bias) != (Cc,) or shp(cond_weight) not in ((lr, Cc), (lr, Cc, 1)) or shp(cond_bias) != (lr,):
+        raise error(f"{what}: need upsample_weight [C][C][window], upsample_bias [C], cond_weight [{lr}][C] or [{lr}][C][1] and "
+                    f"cond_bias [{lr}]; got {wu}, {shp(upsample_bias)}, {shp(cond_weight)}, {shp(cond_bias)}")
+    if not 1 <= stride <= wu[2]:
+        raise error(f"{what}: need upsampling window >= stride >= 1; got {wu[2]}, {stride}")
+    return Cc, wu[2]
+
+
 def split_at_wrap(first_sample, count, num_samples):
     """Absolute samples [first_sample, first_sample + count) of buffers of `num_samples` used as rings, as at most two pieces
     (position, offset, n): samples first_sample + offset .. + n - 1 sit at positions position .. position + n - 1."""
@@ -116,21 +131,10 @@ class NVWavenetInfer:
         check(self._l.nvwn_set_conditioning(self._h, a, first_sample, num_samples, _stream(stream)), "setConditioning")
         return k
 
-    def _check_network(self, what, upsample_weight, upsample_bias, cond_weight, cond_bias):
-        """(C, window) of a conditioning network, upsample_weight [C][C][window], upsample_bias [C], cond_weight [L*2R][C] (or
-        [L*2R][C][1]), cond_bias [L*2R]; ValueError naming `what` for other shapes."""
-        shp = lambda a: tuple(int(v) for v in a.shape)
-        lr, Cc = self.L * 2 * self.R, shp(upsample_weight)[0]
-        if (len(shp(upsample_weight)) != 3 or shp(upsample_weight)[1] != Cc or shp(upsample_bias) != (Cc,)
-                or shp(cond_weight)[:2] != (lr, Cc) or shp(cond_bias) != (lr,)):
-            raise ValueError(f"{what}: need upsample_weight [C][C][window], upsample_bias [C], cond_weight [{lr}][C], cond_bias [{lr}]; "
-                             f"got {shp(upsample_weight)}, {shp(upsample_bias)}, {shp(cond_weight)}, {shp(cond_bias)}")
-        return Cc, shp(upsample_weight)[2]
-
     def _call_with_features(self, fn, name, features, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, *tail):
         """fn(engine, features, C, T, upsample_weight, upsample_bias, window, stride, cond_weight, cond_bias, *tail) of the
         whole-batch producer calls, with the arrays' shapes checked; returns T * stride."""
-        Cc, window = self._check_network(name, upsample_weight, upsample_bias, cond_weight, cond_bias)
+        Cc, window = check_cond_network(self.L, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, ValueError, name)
         shape = tuple(int(v) for v in features.shape)
         if len(shape) != 3 or shape[:2] != (self.B, Cc):
             raise ValueError(f"{name}: features must be [{self.B}][{Cc}][T] for this engine and network; got {shape}")
@@ -253,7 +257,8 @@ class NVWavenetInfer:
     def cond_producer_set_weights(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, stream=None):
         """The conditioning network of set_conditioning_from_features (upsample_weight [C][C][window], upsample_bias [C],
         cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]), for cond_producer_run_slots.  Forgets every attached utterance."""
-        Cc, window = self._check_network("cond_producer_set_weights", upsample_weight, upsample_bias, cond_weight, cond_bias)
+        Cc, window = check_cond_network(self.L, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, ValueError,
+                                        "cond_producer_set_weights")
         wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
         wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
         check(self._l.nvwn_cond_producer_set_weights(self._h, Cc, wu, bu, window, stride, wc, bc, _stream(stream)), "condProducerSetWeights")

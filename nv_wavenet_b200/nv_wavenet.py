@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .infer import check_cond_network
 
 
 class Impl:
@@ -93,6 +94,11 @@ def _expect(name, tensor, shape):
         raise AssertionError(f"{name}: shape {got} does not match the compiled kernel's {tuple(shape)}")
 
 
+def _check_window(window):
+    if window is not None and window < 1:
+        raise AssertionError(f"window must be at least 1; got {window}")
+
+
 class NVWaveNet:
     def __init__(self, embedding_prev, embedding_curr, conv_out_weight, conv_end_weight, dilate_weights, dilate_biases,
                  max_dilation, res_weights, res_biases, skip_weights, skip_biases, use_embed_tanh):
@@ -157,31 +163,44 @@ class NVWaveNet:
             self.engines_created += 1
         return eng
 
+    def _cond_size(self, cond_input):
+        """(batch, samples) of conditioning channels x batch x num_layers x samples."""
+        if cond_input.dim() != 4 or (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
+            raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
+        return cond_input.size(1), cond_input.size(3)
+
+    def _check_prompt(self, what, prompt, rows, n, fp16):
+        """Checks a prompt: int mu-law codes [P] (rows None) or [rows][P], 1 <= P < n, each in [0, A), with fp16 set, since prompts
+        are scored by the fp16 scorer.  Returns it as a tensor."""
+        p = torch.as_tensor(prompt)
+        lead = () if rows is None else (rows,)
+        shape = tuple(p.shape)
+        if len(shape) != len(lead) + 1 or shape[:-1] != lead or not 1 <= shape[-1] < n:
+            raise AssertionError(f"{what} must be {''.join(f'[{r}]' for r in lead)}[P] with 1 <= P < {n}; got {shape}")
+        if p.dtype.is_floating_point or p.dtype.is_complex or p.dtype == torch.bool:
+            raise AssertionError(f"{what} must hold integer mu-law codes; got {p.dtype}")
+        if int(p.min()) < 0 or int(p.max()) >= self.A:
+            raise AssertionError(f"{what} holds codes outside [0, {self.A})")
+        if not fp16:
+            raise AssertionError(f"{what} needs fp16=True: prompts are scored by the fp16 scorer")
+        return p
+
     def infer(self, cond_input, implementation, seed=None, fp16=False, window=None, prompt=None):
         """cond_input: channels x batch x num_layers x samples (pytorch/nv_wavenet.py:172-196); returns int32 [batch][samples].
         `implementation` (Impl.*) is accepted for compatibility: one kernel family serves all of them.
-        window=W generates through one engine of W samples per (batch, W, precision), whatever the length, in windows of W
-        samples (nvwn_run_stream); the result is the same as without a window, bit for bit.
-        prompt: int mu-law codes [batch][P], 1 <= P < samples (host or CUDA tensor), fp16 only.  The prompt is scored all steps at
-        once (nvwn_score_stream, a window at a time with a window), generation is primed from the scoring state
+        Generation runs in windows of W samples (nvwn_run_stream) through one engine of W samples per (batch, W, precision):
+        W = samples without a window, so one window of the whole length; with window=W any length fits, and the result is the
+        same as without a window, bit for bit.
+        prompt: int mu-law codes [batch][P], 1 <= P < samples, each in [0, A) (host or CUDA tensor), fp16 only.  The prompt is
+        scored all steps at once, a window at a time (nvwn_score_stream), generation is primed from the scoring state
         (nvwn_prime_from_score) and continues with samples [P, samples), drawn with the selectors infer() uses at those samples.
         The first P columns of the result are the prompt.  The continuation is not bit-identical to forced generation of the
         prompt (the history holds the scorer's fp16 values, DESIGN.md §5.4); with a window it is bit-identical to without one."""
-        if (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
-            raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
-        batch_size, sample_count = cond_input.size(1), cond_input.size(3)
+        batch_size, sample_count = self._cond_size(cond_input)
+        _check_window(window)
         if prompt is not None:
-            prompt = torch.as_tensor(prompt)
-            shape = tuple(prompt.shape)
-            if len(shape) != 2 or shape[0] != batch_size or not 1 <= shape[1] < sample_count:
-                raise AssertionError(f"prompt must be [batch][P] with batch {batch_size} and 1 <= P < {sample_count}; got {shape}")
-            if prompt.dtype.is_floating_point or prompt.dtype.is_complex or prompt.dtype == torch.bool:
-                raise AssertionError(f"prompt must hold integer mu-law codes; got {prompt.dtype}")
-            if not fp16:
-                raise AssertionError("a prompt needs fp16=True: it is scored by the fp16 scorer")
-            if window is not None and window < 1:
-                raise AssertionError(f"window must be at least 1; got {window}")
-        eng = self._engine(batch_size, sample_count if window is None else window, fp16)
+            prompt = self._check_prompt("prompt", prompt, batch_size, sample_count, fp16).to(device="cuda", dtype=torch.int32)
+        eng = self._engine(batch_size, window or sample_count, fp16)
         lh = column_major(cond_input).float()                       # [samples][layers][batch][2R]
         eng.reset_history()
         sel = None
@@ -189,40 +208,20 @@ class NVWaveNet:
             sel = np.empty(sample_count * batch_size, np.float32)
             _lib.check(self._lib.nvwn_libc_selectors(C.c_void_p(sel.ctypes.data), batch_size, sample_count), "selectors")
         samples = torch.empty((batch_size, sample_count), dtype=torch.int32, device="cuda")
-        if prompt is not None:
-            self._continue(eng, lh, prompt.to(device="cuda", dtype=torch.int32), seed, sel, sample_count if window is None else window,
-                           samples)
-        elif window is None:
-            eng.set_conditioning(lh, 0, sample_count)
-            if sel is None:
-                eng.set_selectors_random(seed)
-            else:
-                eng.set_selectors(sel)
-            eng.run(sample_count, batch_size, samples, dump_activations=False)
-        else:
-            # windows start at multiples of W, so each one fills the buffers from position 0
-            for first in range(0, sample_count, window):
-                n = min(window, sample_count - first)
-                eng.set_conditioning(lh[first:first + n], 0, n)
-                if sel is None:
-                    eng.set_selectors_random_stream(seed, first, n)
-                else:
-                    chunk = np.zeros(window * batch_size, np.float32)
-                    chunk[:n * batch_size] = sel[first * batch_size:(first + n) * batch_size]
-                    eng.set_selectors(chunk)
-                eng.run_stream(first, n, batch_size)
-                eng.get_yout_stream(samples[:, first:first + n], first, n)
+        self._generate(eng, lh, prompt, seed, sel, samples)
         torch.cuda.synchronize()
         return samples
 
     @staticmethod
-    def _continue(eng, lh, prompt, seed, sel, window, samples):
-        """The prompted path of infer() on a reset engine of `window` samples: windows at multiples of W, each one's conditioning
-        set once; the prompt's part of a window is scored, the engine primed at the prompt's end and the rest of the window
-        generated with the selectors of those samples (Philox under `seed`, or the host draw `sel`)."""
+    def _generate(eng, lh, prompt, seed, sel, samples):
+        """The window loop of infer() on a reset engine of W samples: windows at multiples of W, each one's conditioning set once.
+        With a prompt [batch][P], the prompt's part of a window is scored, the engine primed at the prompt's end and the rest of the
+        window generated; without one (P = 0) every window is generated whole.  Selectors of the generated samples: Philox under
+        `seed`, or the host draw `sel` placed at their positions."""
         batch_size, sample_count = samples.shape
-        P = prompt.shape[1]
-        samples[:, :P] = prompt
+        window, P = eng.N, 0 if prompt is None else prompt.shape[1]
+        if P:
+            samples[:, :P] = prompt
         for first in range(0, sample_count, window):
             n = min(window, sample_count - first)
             eng.set_conditioning(lh[first:first + n], 0, n)
@@ -327,21 +326,7 @@ class NVWaveNet:
             return [None] * len(lengths)
         if len(prompts) != len(lengths):
             raise AssertionError(f"{len(lengths)} utterances but {len(prompts)} prompts")
-        out = []
-        for u, p in enumerate(prompts):
-            if p is None:
-                out.append(None)
-                continue
-            p = torch.as_tensor(p)
-            if p.dim() != 1 or not 1 <= p.numel() < lengths[u]:
-                raise AssertionError(f"prompt {u} must be [P] with 1 <= P < {lengths[u]} (its utterance's samples); got {tuple(p.shape)}")
-            if p.dtype.is_floating_point or p.dtype.is_complex or p.dtype == torch.bool:
-                raise AssertionError(f"prompt {u} must hold integer mu-law codes; got {p.dtype}")
-            if int(p.min()) < 0 or int(p.max()) >= self.A:
-                raise AssertionError(f"prompt {u} holds codes outside [0, {self.A})")
-            out.append(p)
-        if any(p is not None for p in out) and not fp16:
-            raise AssertionError("prompts need fp16=True: they are scored by the fp16 scorer")
+        out = [None if p is None else self._check_prompt(f"prompt {u}", p, None, lengths[u], fp16) for u, p in enumerate(prompts)]
         return [None if p is None else p.to(device="cuda", dtype=torch.int32) for p in out]
 
     def infer_many_from_features(self, features, seeds, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots=64,
@@ -359,7 +344,9 @@ class NVWaveNet:
         shp = lambda a: tuple(int(v) for v in a.shape)
         if len(features) != len(seeds):
             raise AssertionError(f"{len(features)} utterances but {len(seeds)} seeds")
-        Cc, lr = self._cond_network(upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
+        Cc, _ = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
+                                   "infer_many_from_features")
+        lr = self.num_layers * 2 * self.R
         for f in features:
             if len(shp(f)) != 2 or shp(f)[0] != Cc or shp(f)[1] < 1:
                 raise AssertionError(f"each utterance's frames are [{Cc}][T] with T >= 1; got {shp(f)}")
@@ -415,21 +402,6 @@ class NVWaveNet:
             timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
         return outs
 
-    def _cond_network(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride):
-        """Checks the shapes of a conditioning network (upsample_weight [C][C][window], upsample_bias [C], cond_weight [L*2R][C] or
-        [L*2R][C][1], cond_bias [L*2R]) and its stride (window >= stride >= 1).  Returns (C, L*2R)."""
-        shp = lambda a: tuple(int(v) for v in a.shape)
-        lr = self.num_layers * 2 * self.R
-        if len(shp(upsample_weight)) != 3 or shp(upsample_weight)[0] != shp(upsample_weight)[1]:
-            raise AssertionError(f"upsample_weight must be [C][C][window]; got {shp(upsample_weight)}")
-        Cc, window_u = shp(upsample_weight)[0], shp(upsample_weight)[2]
-        if shp(upsample_bias) != (Cc,) or shp(cond_weight) not in ((lr, Cc), (lr, Cc, 1)) or shp(cond_bias) != (lr,):
-            raise AssertionError(f"need upsample_bias [{Cc}], cond_weight [{lr}][{Cc}] and cond_bias [{lr}]; got {shp(upsample_bias)}, "
-                                 f"{shp(cond_weight)}, {shp(cond_bias)}")
-        if stride < 1 or window_u < stride:
-            raise AssertionError(f"need upsampling window >= stride >= 1; got {window_u}, {stride}")
-        return Cc, lr
-
     def _serve(self, eng, plan, windows, lengths, seeds, timed, condition, after=None, before=None, prompts=None):
         """The window loop of infer_many and infer_many_from_features on the current stream.  Per window k: before(k), which
         primes the prompted slots that start there; condition(k), which leaves the conditioning of the window's live slots in the
@@ -476,33 +448,20 @@ class NVWaveNet:
 
     def log_likelihood(self, cond_input, audio, window=None):
         """Per-sample log-likelihood of `audio` (int mu-law codes [batch][samples]) given `cond_input` (channels x batch x
-        num_layers x samples, as for infer()): log p(audio[b][t] | audio[b][0..t), conditioning) under the fp16 engine of that
-        size, all steps at once.  Returns a float32 CUDA tensor [batch][samples].
-        window=W scores through one fp16 engine of W samples per batch size, whatever the length, a window at a time
-        (nvwn_score_stream): the engine holds W samples of conditioning instead of all of them, and the result is the same as
-        without a window, bit for bit."""
-        if (cond_input.size(0), cond_input.size(2)) != (2 * self.R, self.num_layers):
-            raise AssertionError(f"Inputs are channels x batch x num_layers x samples; got {tuple(cond_input.size())}")
-        batch_size, sample_count = cond_input.size(1), cond_input.size(3)
+        num_layers x samples, as for infer()): log p(audio[b][t] | audio[b][0..t), conditioning) under the fp16 model, all steps
+        of a window at once.  Returns a float32 CUDA tensor [batch][samples].
+        Scoring runs in windows of W samples (nvwn_score_stream) through one fp16 engine of W samples per (batch, W): W = samples
+        without a window, so one window of the whole length; with window=W the engine holds W samples of conditioning instead of
+        all of them, and the result is the same as without a window, bit for bit.  Either way the engine's scoring stream is left
+        open, so the last window also carries every layer's front for a call that would continue it."""
+        batch_size, sample_count = self._cond_size(cond_input)
         if tuple(audio.size()) != (batch_size, sample_count):
             raise AssertionError(f"audio must be [batch][samples] = {(batch_size, sample_count)}; got {tuple(audio.size())}")
-        if window is not None and window < 1:
-            raise AssertionError(f"window must be at least 1; got {window}")
-        audio = audio.to(device="cuda", dtype=torch.int32)
-        if window is None:
-            eng = self._engine(batch_size, sample_count, True)
-            eng.set_conditioning(column_major(cond_input).float(), 0, sample_count)
-            logp = eng.score(audio)
-        else:
-            eng = self._engine(batch_size, window, True)
-            logp = torch.empty((batch_size, sample_count), dtype=torch.float32, device="cuda")
-            # windows start at multiples of W, so each one fills the store from position 0
-            for first in range(0, sample_count, window):
-                n = min(window, sample_count - first)
-                eng.set_conditioning(column_major(cond_input[..., first:first + n]).float(), 0, n)
-                logp[:, first:first + n] = eng.score_stream(audio[:, first:first + n], first)
-        torch.cuda.synchronize()
-        return logp
+        _check_window(window)
+        eng = self._engine(batch_size, window or sample_count, True)
+        # converted a window at a time, so a windowed call never holds an fp32 copy of the whole length
+        fill = lambda first, n: eng.set_conditioning(column_major(cond_input[..., first:first + n]).float(), 0, n)
+        return self._score(eng, audio.to(device="cuda", dtype=torch.int32), fill)
 
     def log_likelihood_from_features(self, features, audio, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, window=None,
                                      timing=None):
@@ -511,21 +470,34 @@ class NVWaveNet:
         upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]); numpy arrays or torch tensors.  Returns a
         float32 CUDA tensor [batch][T * stride], equal bit for bit to log_likelihood of the conditioning the producer's arithmetic
         gives (nvwn_cond_from_features_host).
-        window=None fills one engine of the whole length; window=W uses one engine of W samples, producing each window's
-        conditioning from the frames just before scoring it, so neither the expanded conditioning nor a store of the whole length
-        ever exists.  timing: a dict, or None; if given, receives the GPU seconds of production ("produce_s") and of scoring
-        ("score_s")."""
+        The frames are loaded into the engine once (nvwn_cond_producer_load); each window's conditioning is then produced from
+        them just before it is scored (nvwn_cond_producer_run_stream).  window=None uses one engine of the whole length; window=W
+        one engine of W samples, so neither the expanded conditioning nor a store of the whole length ever exists.  timing: a dict,
+        or None; if given, receives the GPU seconds of production over the windows ("produce_s", the load not included) and of
+        scoring ("score_s")."""
         shp = lambda a: tuple(int(v) for v in a.shape)
-        Cc, lr = self._cond_network(upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
+        Cc, _ = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
+                                   "log_likelihood_from_features")
         if len(shp(features)) != 3 or shp(features)[1] != Cc or shp(features)[2] < 1:
             raise AssertionError(f"features must be [batch][{Cc}][T] with T >= 1; got {shp(features)}")
         batch_size, sample_count = shp(features)[0], shp(features)[2] * stride
         if shp(audio) != (batch_size, sample_count):
             raise AssertionError(f"audio must be [batch][T * stride] = {(batch_size, sample_count)}; got {shp(audio)}")
-        if window is not None and window < 1:
-            raise AssertionError(f"window must be at least 1; got {window}")
+        _check_window(window)
         audio = torch.as_tensor(audio).to(device="cuda", dtype=torch.int32)
-        net = (upsample_weight, upsample_bias, cond_weight.reshape(lr, Cc), cond_bias, stride)
+        eng = self._engine(batch_size, window or sample_count, True)
+        eng.cond_producer_load(features, upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias,
+                               stride)
+        return self._score(eng, audio, eng.cond_producer_run_stream, timing)
+
+    @staticmethod
+    def _score(eng, audio, fill, timing=None):
+        """The window loop of log_likelihood and log_likelihood_from_features: audio int32 CUDA [batch][samples] scored through the
+        fp16 engine `eng` of W samples in windows at multiples of W, each after fill(first, n) has put the conditioning of samples
+        [first, first + n) into the store.  timing: None, or a dict for the GPU seconds of fill ("produce_s") and of scoring
+        ("score_s")."""
+        batch_size, sample_count = audio.shape
+        logp = torch.empty((batch_size, sample_count), dtype=torch.float32, device="cuda")
         events = []
 
         def mark():
@@ -533,24 +505,13 @@ class NVWaveNet:
                 events.append(torch.cuda.Event(enable_timing=True))
                 events[-1].record()
 
-        if window is None:
-            eng = self._engine(batch_size, sample_count, True)
+        for first in range(0, sample_count, eng.N):
+            n = min(eng.N, sample_count - first)
             mark()
-            eng.set_conditioning_from_features(features, *net)
+            fill(first, n)
             mark()
-            logp = eng.score(audio)
+            logp[:, first:first + n] = eng.score_stream(audio[:, first:first + n], first)
             mark()
-        else:
-            eng = self._engine(batch_size, window, True)
-            eng.cond_producer_load(features, *net)
-            logp = torch.empty((batch_size, sample_count), dtype=torch.float32, device="cuda")
-            for first in range(0, sample_count, window):
-                n = min(window, sample_count - first)
-                mark()
-                eng.cond_producer_run_stream(first, n)
-                mark()
-                logp[:, first:first + n] = eng.score_stream(audio[:, first:first + n], first)
-                mark()
         torch.cuda.synchronize()
         if timing is not None:
             timing["produce_s"] = sum(events[i].elapsed_time(events[i + 1]) for i in range(0, len(events), 3)) / 1e3

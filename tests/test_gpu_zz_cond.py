@@ -88,6 +88,13 @@ def test_out_of_range_is_rejected():
     with pytest.raises(ValueError):
         e.set_conditioning_from_features(np.zeros((3, 3, 4), np.float32), np.zeros((3, 3, 8), np.float32), np.zeros(3, np.float32),
                                          np.zeros((2 * 2 * 64, 3), np.float32), np.zeros(2 * 2 * 64, np.float32), 4)   # 3 utterances, B = 2
+    z = np.zeros((2, 3, 2), np.float32)
+    with pytest.raises(ValueError):
+        e.set_conditioning_from_features(z, np.zeros((3, 3, 8), np.float32), np.zeros(3, np.float32), np.zeros((2 * 2 * 64, 3), np.float32),
+                                         np.zeros(2 * 2 * 64, np.float32), 9)        # upsampling window 8 < stride
+    with pytest.raises(ValueError):
+        e.cond_producer_set_weights(np.zeros((3, 3, 8), np.float32), np.zeros(3, np.float32), np.zeros((2 * 2 * 64, 3, 2), np.float32),
+                                    np.zeros(2 * 2 * 64, np.float32), 4)             # cond_weight [L*2R][C][2]
 
 
 def test_producer_ranges_on_a_side_stream_equal_the_one_shot_call_and_the_host_arithmetic():

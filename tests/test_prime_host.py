@@ -1,6 +1,6 @@
 """Prompted generation at the C-ABI boundary and in NVWaveNet, without a GPU: the C++ facade's prime_from_score() compiles (and runs
-where a GPU is present), nvwn_prime_from_score refuses a NULL engine before it needs a device, and infer(prompt=...) refuses a bad
-prompt before it creates an engine."""
+where a GPU is present), nvwn_prime_from_score refuses a NULL engine before it needs a device, and infer() refuses a bad prompt or
+window before it creates an engine."""
 import os
 import subprocess
 import tempfile
@@ -66,8 +66,12 @@ def test_infer_prompt_rejects_bad_prompts_before_any_engine():
            dict(prompt=torch.zeros(B, 4)),                                # float codes
            dict(prompt=np.zeros((B, 4), np.float64)),
            dict(prompt=torch.zeros(B, 4, dtype=torch.bool)),
+           dict(prompt=torch.full((B, 4), 256, dtype=torch.int32)),       # codes outside [0, A)
+           dict(prompt=torch.full((B, 4), -1, dtype=torch.int32)),
            dict(prompt=good, fp16=False),                                 # the scorer is fp16
-           dict(prompt=good, window=0)]
+           dict(prompt=good, window=0),
+           dict(prompt=None, window=0),                                   # the window rule holds without a prompt too
+           dict(prompt=None, window=0, fp16=False)]
     for kw in bad:
         kw = dict(fp16=True, seed=1, **kw) if "fp16" not in kw else dict(seed=1, **kw)
         with pytest.raises(AssertionError):
