@@ -186,3 +186,22 @@ def lively_inputs(seed, R, S, A, L, B, N):
         "Lh": n((N, L, B, 2 * R), 0.5),
     }
     return w
+
+
+def export_inputs(seed, R, S, A, L, B, N, peak=5.0):
+    """The configuration a PyTorch model's export_weights() hands NVWaveNet, on lively_inputs weights: run it with
+    tanh_embed=False.  embPrev is zero and embCur ~ N(0, 1) (an nn.Embedding, not bounded by the tanh), there are no output
+    biases (Bzs = Bza = 0), and the last layer's residual weights and bias are zero (the layer NVWaveNet appends).
+    Wza is lively_inputs' times `peak`, so the sampled distribution is peaked as a trained model's is: at L16 R64 S256 A256,
+    peak 5 gives a mean max-probability of about 0.46 and a logit spread of about 20 (peak 2.5: 0.16 and 10).  That a trained
+    model looks like this is an assumption: no trained checkpoint is part of the project."""
+    w = lively_inputs(seed, R, S, A, L, B, N)
+    g = np.random.Generator(np.random.PCG64(seed + 0x5EED))
+    w["embPrev"] = np.zeros((A, R), np.float32)
+    w["embCur"] = g.standard_normal((A, R), dtype=np.float32)
+    w["Bzs"] = np.zeros(A, np.float32)
+    w["Bza"] = np.zeros(A, np.float32)
+    w["Wres"][L - 1] = 0
+    w["Bres"][L - 1] = 0
+    w["Wza"] = (w["Wza"] * np.float32(peak)).astype(np.float32)
+    return w

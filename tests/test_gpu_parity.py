@@ -272,25 +272,26 @@ def _check_sampled_index(p, sel, y):
     (64, 256, 256, 20, 130, 6, 2),        # several batch tiles, the last one nearly empty
     (64, 256, 256, 5, 100, 10, 16),       # odd layer count, partially filled tile
     (64, 256, 256, 12, 20, 30, 4),        # the shortest stack the cluster kernel takes
+    (64, 256, 256, 16, 20, 24, 128, False),   # the exported model's configuration (refgen.export_inputs): no embedding tanh
 ])
 def test_fp16_logits_teacher_forced(shape, kernel, monkeypatch):
-    R, S, A, L, B, N, md = shape
+    R, S, A, L, B, N, md, tanh_embed = shape + (True,) * (8 - len(shape))
     _select_fp16_kernel(kernel, monkeypatch)
-    w = refgen.lively_inputs(21 + B, R, S, A, L, B, N)
-    o32 = cpu_oracle(w, L, B, N, R, S, A, md)
+    w = (refgen.lively_inputs if tanh_embed else refgen.export_inputs)(21 + B, R, S, A, L, B, N)
+    o32 = cpu_oracle(w, L, B, N, R, S, A, md, tanh_embed=tanh_embed)
     forced = o32.run(N, B)                                     # the fp32 model's own trajectory as history
     for n_run in (1, N):                                       # step 0 (identical history) and the last step
         wn_ = dict(w); wn_["Lh"] = np.ascontiguousarray(w["Lh"][:n_run]); wn_["selectors"] = np.ascontiguousarray(w["selectors"][:n_run])
         f = np.ascontiguousarray(forced[:, :n_run])
-        e = gpu_engine(wn_, L, B, n_run, R, S, A, md, dtype=nw.FP16)
+        e = gpu_engine(wn_, L, B, n_run, R, S, A, md, dtype=nw.FP16, tanh_embed=tanh_embed)
         e.set_forced(f)
         y = np.zeros((B, n_run), np.int32)
         e.run(n_run, B, y, dump_activations=True); e.synchronize()
         assert e.launch_info()["kernel"] == {"stream": 16, "lat": 18, "lat_single": 18}.get(kernel, 17)
         if kernel.startswith("lat"):
             assert e.launch_info()["cluster"] == (3 if kernel == "lat" and L >= 12 else 1)     # shorter stacks: single-CTA kernel
-        o16 = cpu_oracle(wn_, L, B, n_run, R, S, A, md, prec=po.PREC_FP16); o16.set_forced(f); o16.run(n_run, B)
-        o = cpu_oracle(wn_, L, B, n_run, R, S, A, md); o.set_forced(f); o.run(n_run, B)
+        o16 = cpu_oracle(wn_, L, B, n_run, R, S, A, md, prec=po.PREC_FP16, tanh_embed=tanh_embed); o16.set_forced(f); o16.run(n_run, B)
+        o = cpu_oracle(wn_, L, B, n_run, R, S, A, md, tanh_embed=tanh_embed); o.set_forced(f); o.run(n_run, B)
         ag = e.activations()
         _logit_check(o16.get_za(), ag["za"], 1e-2, mean_rel=3e-4)   # vs the fp16-contract oracle (catches layout slips)
         _logit_check(o.get_za(), ag["za"], 1e-2)                    # vs the fp32 oracle: the north-star tolerance

@@ -11,7 +11,7 @@ import torch
 import nv_wavenet_b200 as nw
 from nv_wavenet_b200 import _lib
 from oracle import pyoracle as po
-from tests import common, refgen
+from tests import common, refgen, replay
 
 pytestmark = pytest.mark.gpu
 
@@ -41,25 +41,6 @@ def _engine(w, L, B, N, R, S, A, md, impl=nw.AUTO, tanh_embed=True):
     return e
 
 
-def _oracle_trace(w, L, B, N, R, S, A, md, prec, forced, tanh_embed=True):
-    o = po.Oracle(L, B, N, R, S, A, md, math=po.MATH_PORTABLE, prec=prec, tanh_embed=tanh_embed)
-    o.load(w)
-    o.set_inputs(w["Lh"], w["selectors"])
-    if forced is not None:
-        o.set_forced(forced)
-    trace = np.zeros((N, B, A), np.float32)
-    o.set_logit_trace(trace)
-    y = o.run(N, B)
-    return y, np.ascontiguousarray(trace.transpose(1, 0, 2))          # [B][N][A]
-
-
-def _sub(w, b):
-    """The inputs of the first b utterances."""
-    v = dict(w)
-    v["Lh"] = np.ascontiguousarray(w["Lh"][:, :, :b]); v["selectors"] = np.ascontiguousarray(w["selectors"][:, :b])
-    return v
-
-
 @pytest.mark.parametrize("shape", [
     (32, 128, 256, 20, 4, 24, 8, True),
     (64, 128, 256, 20, 4, 24, 8, True),
@@ -67,21 +48,28 @@ def _sub(w, b):
     (128, 256, 256, 30, 3, 16, 8, True),
     (64, 256, 256, 4, 64, 800, 512, True),        # 256-step chunks at B = 64: the second chunk boundary is 544 steps in
     (64, 256, 256, 20, 4, 24, 8, False),          # the export path: no embedding tanh, zero embPrev
+    (64, 256, 256, 16, 72, 160, 128, "export"),   # the exported model's configuration (refgen.export_inputs) at L16 maxDil 128
 ])
 def test_oracle_parity_at_every_step(shape):
     R, S, A, L, B, N, md, tanh_embed = shape
-    w = refgen.lively_inputs(70 + L + R, R, S, A, L, B, N)
+    if tanh_embed == "export":
+        tanh_embed = False
+        w = refgen.export_inputs(70 + L + R, R, S, A, L, B, N)
+    else:
+        w = refgen.lively_inputs(70 + L + R, R, S, A, L, B, N)
     if not tanh_embed:
         w["embPrev"] = np.zeros_like(w["embPrev"])
-    Bo = min(B, 8)                                                    # utterances the CPU oracle follows (rows are independent)
-    wo = _sub(w, Bo)
-    audio, z32 = _oracle_trace(wo, L, Bo, N, R, S, A, md, po.PREC_FP32, None, tanh_embed)   # the fp32 model's own trajectory
-    _, z16 = _oracle_trace(wo, L, Bo, N, R, S, A, md, po.PREC_FP16, audio, tanh_embed)
+    # utterances the CPU oracle follows (rows are independent): the scorer's rows t * B + b run in 64-row tiles, so at B >= 64
+    # rows sit at both edges of a tile's 8- and 16-row groups, at the tile's middle and end, and in the ragged last tile
+    rows = [b for b in (0, 7, 8, 31, 32, 56, 63, 64, 71) if b < B] if B >= 64 else list(range(min(B, 8)))
+    Bo = len(rows)
+    audio, z32 = replay.oracle_trace(w, rows, (R, S, A, L, md), N, tanh_embed=tanh_embed)      # the fp32 model's own trajectory
+    _, z16 = replay.oracle_trace(w, rows, (R, S, A, L, md), N, forced=audio, tanh_embed=tanh_embed, prec=po.PREC_FP16)
     full_audio = np.random.default_rng(1).integers(0, A, (B, N)).astype(np.int32)
-    full_audio[:Bo] = audio
+    full_audio[rows] = audio
     e = _engine(w, L, B, N, R, S, A, md, tanh_embed=tanh_embed)
     logp, logits = e.score(full_audio, logits=True)
-    logp, logits = logp[:Bo], logits[:Bo]
+    logp, logits = logp[rows], logits[rows]
     assert logits.shape == (Bo, N, A) and np.isfinite(logits).all()
     _fp16_rule(z16, logits, mean_rel=3e-4)                            # the fp16 contract
     _fp16_rule(z32, logits)                                           # the fp32 model
