@@ -196,6 +196,15 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Not in the reference class: score_stream of a queue of utterances packed end to end in the rows; starts[b * count + i] != 0
+     * begins a new utterance in row b at sample first_sample + i.  See nvwn_score_stream_packed. */
+    bool score_stream_packed(const int* audio, const unsigned char* starts, long long first_sample, int count, int batch_size, float* logp,
+                             float* logits = NULL, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_score_stream_packed(m_engine, audio, starts, first_sample, count, batch_size, logp, logits, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
     /* Not in the reference class: after score_stream over a prompt [0, P), generation continues it from sample P (run_stream of
      * the scoring stream's batch_size).  See nvwn_prime_from_score. */
     bool prime_from_score(cudaStream_t stream = 0)

@@ -190,6 +190,18 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
  * calls share scratch with nvwn_score: issue them on one stream, or order them. */
 int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, int count, int batch_size,
                       float* logp, float* logits, void* stream);
+/* Packed scoring: a queue of utterances scored end to end in the rows of one scoring stream (sequence packing).  Arguments and
+ * results are those of nvwn_score_stream, plus starts [batch_size][count] (host or device memory): a nonzero starts[b][i] begins a
+ * new utterance in row b at absolute sample first_sample + i.  Its codes of steps -1 and -2 are 128 and every layer's x_l[t - d]
+ * reads 0 for t - d before that sample, so its results from that sample on are the bits nvwn_score gives that utterance alone, on
+ * conditioning put at the same store positions.  first_sample = 0 opens a packed stream, and every row starts at sample 0 whatever
+ * starts[b][0] says.  Between calls the engine keeps, besides the fronts and codes, each row's local time (samples since its
+ * utterance began).  A stream is packed or not from its first call: continuing a packed stream with nvwn_score_stream, or one that
+ * is not with this call, is NVWN_EINVAL; nvwn_prime_from_score and nvwn_prime_slots_from_score refuse a packed stream with
+ * NVWN_EUNSUPPORTED (a row's fronts may hold an earlier utterance's inputs).  starts NULL is NVWN_EINVAL.  Every other rule --
+ * continuation, ending, refused calls leaving the stream as it was, memory kinds, completion, engine kinds -- is nvwn_score_stream's. */
+int nvwn_score_stream_packed(nvwn_engine* e, const int* audio, const unsigned char* starts, long long first_sample, int count,
+                             int batch_size, float* logp, float* logits, void* stream);
 /* Prompted generation: continue given audio.  Score the prompt, samples [0, P), with nvwn_score_stream (any windows), then this call
  * moves the open scoring stream's state into generation: for its batch_size Bs utterances, each layer's last d_l inputs go into the
  * history ring and the last two codes become the fed-back indices, and the engine's next sample becomes P.  Then

@@ -57,6 +57,7 @@ SYMBOLS = {
     "nvwn_cond_from_features_host": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int]),
     "nvwn_score": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_score_stream": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_int, _vp, _vp, _vp]),
+    "nvwn_score_stream_packed": (C.c_int, [_vp, _vp, _vp, C.c_longlong, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_prime_from_score": (C.c_int, [_vp, _vp]),
     "nvwn_prime_slots_from_score": (C.c_int, [_vp, _vp, _vp, C.c_int, _vp, _vp]),
     "nvwn_get_xt_out": (C.c_int, [_vp, C.c_int, _vp]),

@@ -129,6 +129,11 @@ struct WnScoreChunk {
     float* logits;                  // row (t, b) -> logits + b * logits_ld + (t - logits_t0) * A, or NULL
     long long logits_ld;
     int logits_t0;
+    // packed scoring (nvwn_score_stream_packed), or starts NULL: the call's start flags, device [Bs][N]; the chunk's local times
+    // [T][Bs] are made in tau from the per-row carry tau_carry [Bs], which moves on to the sample after the chunk
+    const unsigned char* starts;
+    int* tau;
+    int* tau_carry;
 };
 int wn_score_dilation(int layer, int maxDil);
 size_t wn_score_xh_offset(int layer, int L, int maxDil, int Tcap, int Be, int R);   // in elements; layer = L gives the total

@@ -151,10 +151,12 @@ struct nvwn_engine : WnConfig {
     bool score_dirty = true;                 // set with image_dirty (weights_changed): the image is repacked on the next scoring call
     DevBuf<char> score_scratch;
     int score_T = 0;                         // time steps per chunk: SCORE_ROWS / B
-    // the open scoring stream (nvwn_score_stream): the absolute sample its next call starts at, -1 if none is open, and its
-    // batch_size; its state is the layer fronts and the codes in score_scratch
+    // the open scoring stream (nvwn_score_stream): the absolute sample its next call starts at, -1 if none is open, its batch_size,
+    // and whether it is packed (nvwn_score_stream_packed); its state is the layer fronts, the codes and, packed, the local-time
+    // carry in score_scratch
     long long score_next = -1;
     int score_bs = 0;
+    bool score_packed = false;
 
     DevBuf<float> lut_f;                     // mu-law decode tables (nvwn_get_audio): A floats, then 2 x A int16 (wrap / saturate)
     DevBuf<unsigned long long> trace;        // debug timeline (nvwn_debug_trace)
@@ -437,7 +439,7 @@ constexpr int SCORE_ROWS = 16384;
 
 // byte offsets of the scoring scratch, for the engine's B and N and a chunk of T steps
 struct ScoreScratch {
-    size_t audio, logp, bad, codes, lh, xh, xf, H, lgt, bytes;
+    size_t audio, logp, bad, codes, starts, tau, carry, lh, xh, xf, H, lgt, bytes;
 };
 ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
 {
@@ -449,6 +451,9 @@ ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
     o.logp = take(B * N * sizeof(float));
     o.bad = take(sizeof(unsigned long long));
     o.codes = take(B * 2 * sizeof(int));
+    o.starts = take(B * N);                  // packed scoring: the call's start flags, its chunk's local times and their carry
+    o.tau = take(Tz * B * sizeof(int));
+    o.carry = take(B * sizeof(int));
     o.lh = take(Tz * L * B * 2 * R * sizeof(float));
     o.xh = take(wn_score_xh_offset(e->L, e->L, e->maxDil, T, e->B, e->R) * sizeof(__half));
     o.xf = take(Tz * B * R * sizeof(float));
@@ -466,6 +471,9 @@ int check_prime(const nvwn_engine* e, const std::string& who)
     if (e->score_next < 1)
         return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompt with nvwn_score_stream "
                                        "from first_sample = 0 first");
+    if (e->score_packed)
+        return fail(NVWN_EUNSUPPORTED, who + ": the scoring stream is packed (nvwn_score_stream_packed): a row's layer fronts may hold an earlier "
+                                             "utterance's inputs, so they are no history to generate from");
     return 0;
 }
 
@@ -1087,7 +1095,7 @@ int nvwn_get_audio(nvwn_engine* e, float* audio_f32, short* audio_i16, int offse
 
 namespace {
 
-// The checks nvwn_score and nvwn_score_stream share, in their order: arguments, engine kind, batch_size.
+// The checks every scoring call shares, in their order: arguments, engine kind, batch_size.
 int score_args(const nvwn_engine* e, const char* who, const int* audio, int batch_size, const float* logp)
 {
     if (!e || !audio || !logp) return fail(NVWN_EINVAL, std::string(who) + ": NULL engine, audio or logp");
@@ -1097,13 +1105,40 @@ int score_args(const nvwn_engine* e, const char* who, const int* audio, int batc
     return 0;
 }
 
-// The chunk loop of both scoring calls: absolute samples [first, first + count) of the first Bs utterances, 1 <= count <= N, sample t
+// The checks of nvwn_score_stream (packed false) and nvwn_score_stream_packed, in their order: score_args, the starts flags, the window,
+// and for a call that continues the open stream (first_sample != 0) its next sample, batch_size and kind.
+int score_stream_args(const nvwn_engine* e, const std::string& who, const int* audio, const unsigned char* starts, bool packed, long long first_sample,
+                      int count, int batch_size, const float* logp)
+{
+    int rc = score_args(e, who.c_str(), audio, batch_size, logp);
+    if (rc == 0 && packed && !starts) rc = fail(NVWN_EINVAL, who + ": starts is NULL");
+    if (rc == 0) rc = check_window(e, who, first_sample, count, "count", 1);
+    if (rc != 0 || first_sample == 0) return rc;
+    if (e->score_next < 0)
+        return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " continues no scoring stream (nvwn_score and weight "
+                                       "changes end one): start one at first_sample = 0");
+    if (first_sample != e->score_next)
+        return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " does not continue the scoring stream: the next sample is " +
+                                     std::to_string(e->score_next) + " (first_sample = 0 starts over)");
+    if (batch_size != e->score_bs)
+        return fail(NVWN_EINVAL, who + ": batch_size " + std::to_string(batch_size) + " differs from the scoring stream's batch_size " +
+                                     std::to_string(e->score_bs) + " (first_sample = 0 starts over)");
+    if (packed != e->score_packed)
+        return fail(NVWN_EINVAL, who + ": the scoring stream is " + (e->score_packed ? "packed: continue it with nvwn_score_stream_packed"
+                                                                                    : "not packed: continue it with nvwn_score_stream") +
+                                     " (first_sample = 0 starts over)");
+    return 0;
+}
+
+// The chunk loop of every scoring call: absolute samples [first, first + count) of the first Bs utterances, 1 <= count <= N, sample t
 // with the conditioning at store position t mod N; audio, logp and logits hold [Bs][count] (host or device).  first == 0 starts
 // afresh (x_l[t - d] = 0 for t < d, codes 128 / 128); any other first continues from the layer fronts and codes the last call left.
-// keep leaves the call's own fronts and codes there and opens the stream at first + count; otherwise the stream ends.  The caller has
-// checked the arguments; the audio is checked here, before any state changes.
-int score_range(nvwn_engine* e, const char* who, const int* audio, long long first, int count, int Bs, float* logp, float* logits, bool keep,
-                cudaStream_t st)
+// keep leaves the call's own fronts and codes there and opens the stream at first + count; otherwise the stream ends.  starts (host or
+// device [Bs][count], or NULL) packs the call: each row's local time, carried from the last call and 0 at a flag and at first == 0,
+// selects the packed kernels' masks, and the stream it keeps open is packed.  The caller has checked the arguments; the audio is
+// checked here, before any state changes.
+int score_range(nvwn_engine* e, const char* who, const int* audio, const unsigned char* starts, long long first, int count, int Bs, float* logp,
+                float* logits, bool keep, cudaStream_t st)
 {
     const int N = count, L = e->L, R = e->R, A = e->A;
     if (!e->score_scratch) {
@@ -1153,6 +1188,7 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, long long fir
             CK(cudaMemsetAsync(xh + wn_score_xh_offset(l, L, e->maxDil, T, e->B, R), 0,
                                (size_t)wn_score_dilation(l, e->maxDil) * Bs * R * sizeof(__half), st));
         CK(wn_fill_int(d_codes, 128, (size_t)Bs * 2, st));
+        if (starts) CK(cudaMemsetAsync(sc + o.carry, 0, (size_t)Bs * sizeof(int), st));
     }
     WnScoreChunk c;
     c.L = L; c.R = R; c.S = e->S; c.A = A; c.maxDil = e->maxDil; c.tanhEmbed = e->tanhEmbed;
@@ -1166,6 +1202,13 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, long long fir
     c.xf = reinterpret_cast<float*>(sc + o.xf);
     c.H = reinterpret_cast<__half*>(sc + o.H);
     c.logp = logp_dev ? logp : reinterpret_cast<float*>(sc + o.logp);
+    c.starts = nullptr;
+    if (starts) {
+        CK(cudaMemcpyAsync(sc + o.starts, starts, n_audio, cudaMemcpyDefault, st));
+        c.starts = reinterpret_cast<const unsigned char*>(sc + o.starts);
+        c.tau = reinterpret_cast<int*>(sc + o.tau);
+        c.tau_carry = reinterpret_cast<int*>(sc + o.carry);
+    }
     float* lgt = reinterpret_cast<float*>(sc + o.lgt);
     for (int t0 = 0; t0 < N; t0 += T) {
         const int Tc = N - t0 < T ? N - t0 : T;
@@ -1198,6 +1241,7 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, long long fir
         CK(wn_score_carry_codes(d_codes, d_audio, N, N, Bs, st));
         e->score_next = first + N;
         e->score_bs = Bs;
+        e->score_packed = starts != nullptr;
     }
     if (!logp_dev) CK(cudaMemcpyAsync(logp, c.logp, n_audio * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (!logp_dev || (logits && !logits_dev)) CK(cudaStreamSynchronize(st));
@@ -1213,27 +1257,24 @@ int nvwn_score(nvwn_engine* e, const int* audio, int num_samples, int batch_size
     int rc = score_args(e, "nvwn_score", audio, batch_size, logp);
     if (rc != 0) return rc;
     if (num_samples < 1 || num_samples > e->N) return fail(NVWN_EINVAL, "nvwn_score: num_samples outside [1, N]");
-    return score_range(e, "nvwn_score", audio, 0, num_samples, batch_size, logp, logits, false, (cudaStream_t)stream);
+    return score_range(e, "nvwn_score", audio, nullptr, 0, num_samples, batch_size, logp, logits, false, (cudaStream_t)stream);
 }
 
 int nvwn_score_stream(nvwn_engine* e, const int* audio, long long first_sample, int count, int batch_size, float* logp, float* logits, void* stream)
 {
     const std::string who = "nvwn_score_stream";
-    int rc = score_args(e, who.c_str(), audio, batch_size, logp);
-    if (rc == 0) rc = check_window(e, who, first_sample, count, "count", 1);
+    const int rc = score_stream_args(e, who, audio, nullptr, false, first_sample, count, batch_size, logp);
     if (rc != 0) return rc;
-    if (first_sample != 0) {
-        if (e->score_next < 0)
-            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " continues no scoring stream (nvwn_score and weight "
-                                           "changes end one): start one at first_sample = 0");
-        if (first_sample != e->score_next)
-            return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " does not continue the scoring stream: the next sample is " +
-                                         std::to_string(e->score_next) + " (first_sample = 0 starts over)");
-        if (batch_size != e->score_bs)
-            return fail(NVWN_EINVAL, who + ": batch_size " + std::to_string(batch_size) + " differs from the scoring stream's batch_size " +
-                                         std::to_string(e->score_bs) + " (first_sample = 0 starts over)");
-    }
-    return score_range(e, who.c_str(), audio, first_sample, count, batch_size, logp, logits, true, (cudaStream_t)stream);
+    return score_range(e, who.c_str(), audio, nullptr, first_sample, count, batch_size, logp, logits, true, (cudaStream_t)stream);
+}
+
+int nvwn_score_stream_packed(nvwn_engine* e, const int* audio, const unsigned char* starts, long long first_sample, int count, int batch_size,
+                             float* logp, float* logits, void* stream)
+{
+    const std::string who = "nvwn_score_stream_packed";
+    const int rc = score_stream_args(e, who, audio, starts, true, first_sample, count, batch_size, logp);
+    if (rc != 0) return rc;
+    return score_range(e, who.c_str(), audio, starts, first_sample, count, batch_size, logp, logits, true, (cudaStream_t)stream);
 }
 
 int nvwn_prime_from_score(nvwn_engine* e, void* stream)

@@ -15,6 +15,8 @@
 // calls, so the first chunk of a call continues the previous call's last one.  Tensor cores through mma.sync.m16n8k16 (fp16 in,
 // fp32 accumulate) from XOR-swizzled shared-memory tiles loaded with cp.async; every output element accumulates its K in one
 // fixed order in one CTA (no split-K, no atomics), so a row's result does not depend on which tile, chunk or batch it is computed in.
+// Packed scoring (nvwn_score_stream_packed) starts utterances inside a row: the PACKED instantiations of the embedding and layer
+// kernels read codes 128 and zero x[t-d] by each row's local time, where a fresh start reads the 128s and the zeroed fronts.
 #include "wn_common.h"
 #include "wn_math.cuh"
 
@@ -143,19 +145,50 @@ __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile(
 __device__ __forceinline__ uint32_t u32(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 
 // ---- embedding: x_0 of every row of the chunk; the codes of call steps -2 and -1 come from codes[b][0..1] ----
+// PACKED (nvwn_score_stream_packed): tau[m] is row m's local time, the samples its utterance has run before this one; the codes of
+// its steps -1 and -2 are 128 where tau < 1 and tau < 2
+template <bool PACKED>
 __global__ void score_embed_kernel(const __half* __restrict__ embPrev, const __half* __restrict__ embCur, const int* __restrict__ audio,
                                    const int* __restrict__ codes, int N, int t0, int M, int Bs, int R, int tanhEmbed, float* __restrict__ xf,
-                                   __half* __restrict__ x0)
+                                   __half* __restrict__ x0, const int* __restrict__ tau)
 {
     const size_t n_all = (size_t)M * R;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (size_t)gridDim.x * blockDim.x) {
         const int m = (int)(i / R), r = (int)(i % R), b = m % Bs, t = t0 + m / Bs;
-        const int yp = t >= 2 ? audio[(size_t)b * N + t - 2] : codes[2 * b + t], yc = t >= 1 ? audio[(size_t)b * N + t - 1] : codes[2 * b + 1];
+        int yp = t >= 2 ? audio[(size_t)b * N + t - 2] : codes[2 * b + t], yc = t >= 1 ? audio[(size_t)b * N + t - 1] : codes[2 * b + 1];
+        if (PACKED) {
+            const int tm = tau[m];
+            if (tm < 2) yp = 128;
+            if (tm < 1) yc = 128;
+        }
         float v = __half2float(embPrev[(size_t)yp * R + r]) + __half2float(embCur[(size_t)yc * R + r]);
         if (tanhEmbed) v = wn::tanhf_fast(v);         // as the latency kernel (wn_lat_kernel.cu)
         xf[i] = v;
         x0[i] = __float2half_rn(v);
     }
+}
+
+// ---- packed scoring: tau [T][Bs] of the chunk's rows from the call's start flags [Bs][N]; carry[b] is the tau row b's next sample
+// has without a flag (0 when a stream opens), and leaves as that of the sample after the chunk.  Clamped at cap = max(maxDil, 2):
+// the kernels only compare tau with 1, 2 and d_l <= maxDil.  One warp per row, 32 steps at a time: a lane's tau counts from the
+// last flag at or before it, or on from the carry ----
+__global__ void score_tau_kernel(int* __restrict__ tau, int* __restrict__ carry, const unsigned char* __restrict__ starts, int N, int t0, int T,
+                                 int Bs, int cap)
+{
+    const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (b >= Bs) return;                              // whole warps
+    int c = carry[b];
+    for (int i0 = 0; i0 < T; i0 += 32) {
+        const int i = i0 + lane;
+        const bool f = i < T && starts[(size_t)b * N + t0 + i];
+        const unsigned m = __ballot_sync(0xffffffffu, f) & (0xffffffffu >> (31 - lane));     // flags at lanes <= lane
+        int v = m ? lane - (31 - __clz(m)) : c + lane;
+        v = v < cap ? v : cap;
+        if (i < T) tau[(size_t)i * Bs + b] = v;
+        const int last = __shfl_sync(0xffffffffu, v, T - 1 - i0 < 31 ? T - 1 - i0 : 31);
+        c = last + 1 < cap ? last + 1 : cap;
+    }
+    if (lane == 0) carry[b] = c;
 }
 
 // ---- one residual layer over all rows of the chunk; weights resident in shared memory, persistent over row tiles ----
@@ -171,12 +204,14 @@ struct LayerArgs {
     const float* lh;                // conditioning of this layer: row (tl, b) at lh + tl * lh_t + b * 2R
     size_t lh_t;
     int M, Bs;
+    int d;                          // the layer's dilation
+    const int* tau;                 // PACKED: local time of row m (score_tau_kernel); x[t-d] reads 0 where tau[m] < d
 };
 
 template <int R>
 constexpr int layer_smem() { return (4 * R * R + R * R + BM * 2 * R + BM * R) * 2; }
 
-template <int R>
+template <int R, bool PACKED>
 __global__ void __launch_bounds__(NTHREADS) score_layer_kernel(const LayerArgs a)
 {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -195,7 +230,8 @@ __global__ void __launch_bounds__(NTHREADS) score_layer_kernel(const LayerArgs a
             const int r = i / N1, c = i % N1, m = m0 + r;
             const bool v = m < a.M;
             const size_t row = v ? (size_t)m + (c < NR ? a.hist : 0) : 0;
-            cp16(sXA + swz(r, c, N1), a.xin + row * R + (c % NR) * 8, v);
+            // packed: x[t-d] of a row whose utterance began less than d samples ago is the zero a fresh start reads from its front
+            cp16(sXA + swz(r, c, N1), a.xin + row * R + (c % NR) * 8, PACKED ? v && (c < NR || a.tau[m] >= a.d) : v);
         }
         cp_commit();
         cp_wait<0>();
@@ -470,7 +506,7 @@ template <int R>
 cudaError_t launch_layer(const LayerArgs& a, cudaStream_t st)
 {
     static_assert(layer_smem<R>() <= 227 * 1024, "layer kernel shared memory");
-    return launch_persistent(score_layer_kernel<R>, layer_smem<R>(), (a.M + BM - 1) / BM, st, a);
+    return launch_persistent(a.tau ? score_layer_kernel<R, true> : score_layer_kernel<R, false>, layer_smem<R>(), (a.M + BM - 1) / BM, st, a);
 }
 
 template <int S>
@@ -543,13 +579,19 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
     const char* im = static_cast<const char*>(c.image);
     const int M = c.T * c.Bs, R = c.R;
     cudaError_t e;
+    if (c.starts) {
+        score_tau_kernel<<<(c.Bs + 3) / 4, 128, 0, st>>>(c.tau, c.tau_carry, c.starts, c.N, c.t0, c.T, c.Bs, c.maxDil > 2 ? c.maxDil : 2);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    const int* tau = c.starts ? c.tau : nullptr;
     {
         const size_t n = (size_t)M * R;
         size_t blocks = (n + 255) / 256;
         if (blocks > 132 * 16) blocks = 132 * 16;
         __half* x0 = c.xh + (size_t)wn_score_dilation(0, c.maxDil) * c.Bs * R;
-        score_embed_kernel<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const __half*>(c.embPrev), static_cast<const __half*>(c.embCur), c.audio,
-                                                            c.codes, c.N, c.t0, M, c.Bs, R, c.tanhEmbed, c.xf, x0);
+        (tau ? score_embed_kernel<true> : score_embed_kernel<false>)<<<(unsigned)blocks, 256, 0, st>>>(
+            static_cast<const __half*>(c.embPrev), static_cast<const __half*>(c.embCur), c.audio, c.codes, c.N, c.t0, M, c.Bs, R, c.tanhEmbed, c.xf,
+            x0, tau);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     for (int l = 0; l < c.L; l++) {
@@ -558,7 +600,9 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
         a.Wr = reinterpret_cast<const __half*>(im + o.Wr) + (size_t)l * R * R;
         a.Bh = reinterpret_cast<const float*>(im + o.Bh) + (size_t)l * 2 * R;
         a.Br = reinterpret_cast<const float*>(im + o.Br) + (size_t)l * R;
-        a.hist = wn_score_dilation(l, c.maxDil) * c.Bs;
+        a.d = wn_score_dilation(l, c.maxDil);
+        a.hist = a.d * c.Bs;
+        a.tau = tau;
         a.xin = c.xh + wn_score_xh_offset(l, c.L, c.maxDil, c.Tcap, c.Be, R);
         a.xf = c.xf;
         a.xout = l + 1 < c.L ? c.xh + wn_score_xh_offset(l + 1, c.L, c.maxDil, c.Tcap, c.Be, R) + (size_t)wn_score_dilation(l + 1, c.maxDil) * c.Bs * R

@@ -365,6 +365,27 @@ class NVWavenetInfer:
         return self._score(audio, num_samples, batch_size, logits, "score_stream",
                            lambda a, n, bs, lp, lg: self._l.nvwn_score_stream(self._h, a, first_sample, n, bs, lp, lg, _stream(stream)))
 
+    def score_stream_packed(self, audio, starts, first_sample, num_samples=None, batch_size=None, logits=False, stream=None):
+        """score_stream of a queue of utterances packed end to end in the rows: starts [batch][num_samples] (numpy array or CUDA
+        tensor), nonzero where a new utterance begins in that row at that sample.  From its start each utterance's results are the
+        bits score() gives it alone on the same conditioning.  first_sample 0 opens a packed stream (every row starts there); a
+        packed stream is continued only by this call.  Arrays and results as for score(); see nvwn_score_stream_packed."""
+        n = audio.shape[1] if num_samples is None else num_samples
+        bs = audio.shape[0] if batch_size is None else batch_size
+        shape = tuple(int(v) for v in starts.shape)
+        if len(shape) != 2 or shape[0] < bs or shape[1] < n:
+            raise ValueError(f"score_stream_packed: starts must be [batch][samples] covering [{bs}][{n}]; got {shape}")
+        if hasattr(starts, "is_cuda") and starts.is_cuda:
+            import torch
+            flags = (starts[:bs, :n] != 0).to(torch.uint8).contiguous()
+            p = flags.data_ptr()
+        else:
+            flags = np.ascontiguousarray(np.asarray(starts)[:bs, :n] != 0, dtype=np.uint8)
+            p = flags.ctypes.data
+        return self._score(audio, n, bs, logits, "score_stream_packed",
+                           lambda a, n, bs, lp, lg: self._l.nvwn_score_stream_packed(self._h, a, C.c_void_p(p), first_sample, n, bs, lp, lg,
+                                                                                     _stream(stream)))
+
     def prime_from_score(self, stream=None):
         """After score_stream over a prompt, samples [0, P): generation continues the prompt from sample P, run_stream(P, count, bs)
         with the scoring stream's batch_size bs.  The scoring stream stays open.  Asynchronous on `stream`; see nvwn_prime_from_score."""

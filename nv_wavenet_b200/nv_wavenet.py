@@ -88,6 +88,64 @@ def _windows(plan, lengths, window):
     return out
 
 
+def plan_packed(lengths, slots):
+    """Packed scoring schedule of log_likelihood_many: utterances of `lengths` samples, in arrival order, each to the row whose
+    current end is earliest (the lowest row on ties), starting at that end.  Returns [(slot, start)] per utterance."""
+    if slots < 1:
+        raise ValueError(f"need slots >= 1; got {slots}")
+    if any(n < 1 for n in lengths):
+        raise ValueError("every utterance needs at least one sample")
+    ends, plan = [0] * slots, []
+    for n in lengths:
+        s = ends.index(min(ends))
+        plan.append((s, ends[s]))
+        ends[s] += n
+    return plan
+
+
+def _packed_windows(plan, lengths, window):
+    """The windows of a plan_packed schedule at multiples of `window`: per window (first sample, samples, segments), a segment
+    (slot, utterance, its first sample in the utterance, its first sample in the window, samples) for every utterance that has
+    samples in the window, ordered by slot and, within a slot, by time."""
+    rows = {}
+    for u, (s, _) in enumerate(plan):
+        rows.setdefault(s, []).append(u)                          # in arrival order, which is time order within a row
+    end = max((start + n for (_, start), n in zip(plan, lengths)), default=0)
+    done = {s: 0 for s in rows}                                   # per row, its utterances that ended before the window
+    out = []
+    for first in range(0, end, window):
+        last = min(first + window, end)
+        segs = []
+        for s in sorted(rows):
+            us, i = rows[s], done[s]
+            while i < len(us) and plan[us[i]][1] + lengths[us[i]] <= first:
+                i += 1
+            done[s] = i
+            while i < len(us) and plan[us[i]][1] < last:
+                u, start = us[i], plan[us[i]][1]
+                b, e = max(start, first), min(start + lengths[u], last)
+                segs.append((s, u, b - start, b - first, e - b))
+                i += 1
+        out.append((first, last - first, segs))
+    return out
+
+
+def _pack_window(count, segs, audios, slots):
+    """The audio [slots][count] (int32, code 128 where a row has no utterance) and start flags [slots][count] (uint8, 1 at each
+    utterance's first sample) of one window's segments (_packed_windows), on the device of `audios`, per utterance int32 [n_u]."""
+    dev = audios[0].device if audios else "cpu"
+    audio = torch.full((slots, count), 128, dtype=torch.int32, device=dev)
+    rows, cols = [], []
+    for s, u, a, o, m in segs:
+        audio[s, o:o + m] = audios[u][a:a + m]
+        if a == 0:
+            rows.append(s)
+            cols.append(o)
+    starts = torch.zeros((slots, count), dtype=torch.uint8, device=dev)
+    starts[torch.tensor(rows, dtype=torch.long, device=dev), torch.tensor(cols, dtype=torch.long, device=dev)] = 1
+    return audio, starts
+
+
 def _expect(name, tensor, shape):
     got = tuple(tensor.size())[:len(shape)]
     if got != tuple(shape):
@@ -489,6 +547,108 @@ class NVWaveNet:
         eng.cond_producer_load(features, upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias,
                                stride)
         return self._score(eng, audio, eng.cond_producer_run_stream, timing)
+
+    def _check_queue(self, what, lengths, audios, slots, window):
+        """The audios of a scoring queue as int32 CUDA codes [n_u], checked against `lengths` (each >= 1), and slots and window
+        checked, before any engine exists."""
+        if len(audios) != len(lengths):
+            raise AssertionError(f"{what}: {len(lengths)} utterances but {len(audios)} audios")
+        if any(n < 1 for n in lengths):
+            raise AssertionError(f"{what}: every utterance needs at least one sample")
+        for u, (a, n) in enumerate(zip(audios, lengths)):
+            if tuple(a.shape) != (n,):
+                raise AssertionError(f"{what}: audio {u} must be [{n}] codes; got {tuple(a.shape)}")
+        if slots < 1 or window is None or window < 1:
+            raise AssertionError(f"{what}: need slots >= 1 and window >= 1; got {slots}, {window}")
+        return [torch.as_tensor(a).to(device="cuda", dtype=torch.int32) for a in audios]
+
+    def log_likelihood_many(self, cond_inputs, audios, slots=64, window=4096, timing=None):
+        """Packed scoring of a queue: log_likelihood of utterances of different lengths through one fp16 engine of `slots` rows and
+        `window` samples, with no padding between utterances.  cond_inputs: per utterance, conditioning [2R][L][n_u] (channels x
+        num_layers x samples); audios: per utterance, int mu-law codes [n_u] (host or CUDA).  Returns float32 CUDA tensors [n_u],
+        each bit-identical to log_likelihood(c_u[:, None], a_u[None])[0] of that utterance alone.  Each utterance goes to the row
+        that frees first (plan_packed) and starts there at the very next sample; the rows are scored in windows at multiples of
+        `window` (nvwn_score_stream_packed), each window's conditioning set once, zero where a row has nothing.  timing: a dict, or
+        None; if given, receives the GPU seconds of filling the conditioning ("produce_s") and of scoring ("score_s")."""
+        for c in cond_inputs:
+            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * self.R, self.num_layers):
+                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
+        lengths = [int(c.size(2)) for c in cond_inputs]
+        audios = self._check_queue("log_likelihood_many", lengths, audios, slots, window)
+        plan = plan_packed(lengths, slots)
+        eng = self._engine(slots, window, True)
+
+        def fill(first, count, segs):
+            lh = torch.zeros((count, self.num_layers, slots, 2 * self.R), dtype=torch.float32, device="cuda")
+            for s, u, a, o, m in segs:
+                lh[o:o + m, :, s].copy_(cond_inputs[u][:, :, a:a + m].permute(2, 1, 0))
+            eng.set_conditioning(lh, 0, count)
+
+        return self._score_packed(eng, plan, lengths, audios, fill, timing)
+
+    def log_likelihood_many_from_features(self, features, audios, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots=64,
+                                          window=4096, timing=None):
+        """log_likelihood_many with each utterance given as its mel frames [C][T_u] instead of expanded conditioning; utterance u has
+        T_u * stride samples and audios[u] is [T_u * stride] codes.  The conditioning network is that of set_conditioning_from_features
+        (upsample_weight [C][C][w], upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]).  Returns float32
+        CUDA tensors, each bit-identical to log_likelihood of that utterance alone on the conditioning the producer's arithmetic gives
+        it (nvwn_cond_from_features_host).  Each window's conditioning comes from the per-slot producer: an utterance's frames are
+        attached to its row at its start, and the producer runs once per distinct segment range of the window, in time order.
+        timing as for log_likelihood_many."""
+        shp = lambda a: tuple(int(v) for v in a.shape)
+        Cc, _ = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
+                                   "log_likelihood_many_from_features")
+        for f in features:
+            if len(shp(f)) != 2 or shp(f)[0] != Cc or shp(f)[1] < 1:
+                raise AssertionError(f"each utterance's frames are [{Cc}][T] with T >= 1; got {shp(f)}")
+        lengths = [shp(f)[1] * stride for f in features]
+        audios = self._check_queue("log_likelihood_many_from_features", lengths, audios, slots, window)
+        plan = plan_packed(lengths, slots)
+        eng = self._engine(slots, window, True)
+        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride)
+        keep = []
+
+        def fill(first, count, segs):
+            ranges = {}
+            for s, u, a, o, m in segs:
+                ranges.setdefault((o, m), []).append((s, u, a))
+            # by first sample: a row's earlier segment is produced before the row's next utterance is attached
+            for (o, m), group in sorted(ranges.items()):
+                new = [(s, u) for s, u, a in group if a == 0]
+                if new:
+                    keep.append(eng.cond_producer_set_slots([s for s, _ in new], [features[u] for _, u in new], [plan[u][1] for _, u in new]))
+                eng.cond_producer_run_slots([s for s, _, _ in group], first + o, m)
+
+        return self._score_packed(eng, plan, lengths, audios, fill, timing)
+
+    @staticmethod
+    def _score_packed(eng, plan, lengths, audios, fill, timing):
+        """The window loop of log_likelihood_many and log_likelihood_many_from_features: the plan_packed schedule `plan` of `lengths`
+        over the fp16 engine `eng` of as many rows and W samples, in windows at multiples of W.  Per window: fill(first, count, segments)
+        puts the conditioning of the window's segments into the store, then the window's audio and start flags are scored
+        (nvwn_score_stream_packed) and each segment's logp copied out.  timing as for _score."""
+        outs = [torch.empty(n, dtype=torch.float32, device="cuda") for n in lengths]
+        events = []
+
+        def mark():
+            if timing is not None:
+                events.append(torch.cuda.Event(enable_timing=True))
+                events[-1].record()
+
+        for first, count, segs in _packed_windows(plan, lengths, eng.N):
+            mark()
+            fill(first, count, segs)
+            mark()
+            audio, starts = _pack_window(count, segs, audios, eng.B)
+            logp = eng.score_stream_packed(audio, starts, first)
+            for s, u, a, o, m in segs:
+                outs[u][a:a + m].copy_(logp[s, o:o + m])
+            mark()
+        torch.cuda.synchronize()
+        if timing is not None:
+            timing["produce_s"] = sum(events[i].elapsed_time(events[i + 1]) for i in range(0, len(events), 3)) / 1e3
+            timing["score_s"] = sum(events[i + 1].elapsed_time(events[i + 2]) for i in range(0, len(events), 3)) / 1e3
+        return outs
 
     @staticmethod
     def _score(eng, audio, fill, timing=None):
