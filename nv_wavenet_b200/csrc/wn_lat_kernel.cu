@@ -964,21 +964,32 @@ struct CfgC {
     using C = Cfg<S>;
     static_assert(TR == 16 || TR == 8, "a cluster serves 16 or 8 utterances");
     static constexpr uint32_t PIECE0 = 24576;                              // chain: [Wcur | Wres]
+    // The chain's compute warps read the Wcur fragments of step n + 1 behind the h barrier of step n (8-row clusters), or those of
+    // step n behind the x barrier of step n (16-row clusters, which measured 2 % slower reading them ahead: DESIGN §5.1b).
+    static constexpr bool WCUR_AHEAD = TR == 8;
+    // chain ring slots: piece n (step n) sits in slot n % NSLOT0.  Read ahead, piece n + 1 must have landed before the h barrier of
+    // step n, and its slot is handed back behind the h barrier of step n + 1 - NSLOT0: the producer has NSLOT0 - 1 steps to refill
+    // it.  With two slots (one step) the chain waits for the ring.
+    static constexpr int NSLOT0 = WCUR_AHEAD ? 3 : 2;
+    static_assert(NSLOT0 == 2 || NSLOT0 == 3, "the chain ring has two or three slots");
+    __device__ static __forceinline__ uint32_t slot0(uint32_t n) { return n % NSLOT0; }
+    __device__ static __forceinline__ uint32_t par0(uint32_t n) { return (n / NSLOT0) & 1; }   // phase parity of piece n's fill
     static constexpr uint32_t SLOT1 = S * 128;                             // tail: Wskip_l
     static constexpr int NSLOT1 = 3;
     static constexpr int NAP = 4;                                          // pre-activation tiles in flight from the prep CTA to the chain CTA
     static constexpr int NPS = 8;                                          // staged history / conditioning tiles of the prep CTA
     static constexpr int NPRING = 4;                                       // Wprev ring slots of the prep CTA
     static constexpr int NHB = 2;                                          // h tiles in flight from the chain CTA to the tail CTA
-    static constexpr int NRING = NSLOT1 > NPRING ? NSLOT1 : NPRING;        // weight-ring barrier pairs (the chain uses two)
+    static constexpr int NRING = NSLOT1 > NPRING ? NSLOT1 : NPRING;        // weight-ring barrier pairs (the chain uses NSLOT0)
+    static_assert(NSLOT0 <= NRING, "the chain ring's barriers fit the reserved pairs");
     static_assert((NAP & (NAP - 1)) == 0 && (NPS & (NPS - 1)) == 0 && (NPRING & (NPRING - 1)) == 0 && (NHB & (NHB - 1)) == 0,
                   "slot counts are powers of two, so that slot and parity arithmetic stays a mask and a shift");
     static constexpr int RPW = TR / NCW;                                   // rows sampled per tail warp
     static constexpr uint32_t XT = TR * 128;                               // activation tile (x, h, x[t-d]): TR rows x 64 channels fp16
     static constexpr uint32_t AP = TR * 512;                               // pre-activation tile: TR rows x 128 channels fp32
     // chain CTA
-    static constexpr uint32_t C_RING = 0;                                  // 2 x PIECE0
-    static constexpr uint32_t C_EMB = 2 * PIECE0;
+    static constexpr uint32_t C_RING = 0;                                  // NSLOT0 x PIECE0
+    static constexpr uint32_t C_EMB = NSLOT0 * PIECE0;
     static constexpr uint32_t C_EPBUF = C_EMB + A * EROW * 4;
     static constexpr uint32_t C_XBUF = C_EPBUF + 2 * TR * EROW * 4;
     static constexpr uint32_t C_HBUF = C_XBUF + XT;
@@ -1010,6 +1021,7 @@ struct CfgC {
     static constexpr uint32_t P_ZA = P_OB1 + OB1_BYTES;
     static constexpr uint32_t P_END = P_ZA + ZA_BYTES;
     // common tail of the maps (same offsets in every CTA, so that remote addresses are computed with mapa on local ones)
+    static_assert(C_END <= P_END, "the chain's map (its ring included) stays below the prep CTA's, so the ring depth does not grow SMEM");
     static constexpr uint32_t O_YS = (C_END > T_END ? (C_END > P_END ? C_END : P_END) : (T_END > P_END ? T_END : P_END));
     static constexpr uint32_t O_BAR = O_YS + 2 * TR * 4;
     static constexpr uint32_t SMEM = O_BAR + 40 * 8;
@@ -1245,8 +1257,8 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
             uint32_t pc = 0;
             for (int t = t_begin; t < t_end; t++)
                 for (int l = 0; l < L; l++, pc++) {
-                    const uint32_t sl = pc & 1;
-                    mbar_wait(s_empty + 8 * sl, ((pc >> 1) & 1) ^ 1);
+                    const uint32_t sl = M::slot0(pc);
+                    mbar_wait(s_empty + 8 * sl, M::par0(pc) ^ 1);
                     mbar_arrive_expect_tx(s_full + 8 * sl, M::PIECE0);
                     tma_load_1d(sm + M::C_RING + sl * M::PIECE0, img + (size_t)l * im.layer_bytes + C::W_CUR, 16384, s_full + 8 * sl);
                     tma_load_1d(sm + M::C_RING + sl * M::PIECE0 + 16384, img + (size_t)l * im.layer_bytes + C::W_RES, 8192, s_full + 8 * sl);
@@ -1256,19 +1268,25 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
         // Sync warp: every mbarrier of the layer loop, so that the compute warps pass only their two named barriers per step.  Its
         // lane 0 enters a barrier once what the compute warps will read behind it has landed, and answers for what they have read
         // before it:
-        //   before the x barrier of step n: ring piece n (Wcur, Wres) is full; the tail's h buffer n % NHB is free (it has read tile
-        //     n - NHB), so that every compute thread sends its words of h tile n with st.async behind that barrier;
+        //   before the first barrier: pre-activation tile 0 is full (WCUR_AHEAD: and ring piece 0);
+        //   before the x barrier of step n: the tail's h buffer n % NHB is free (it has read tile n - NHB), so that every compute
+        //     thread sends its words of h tile n with st.async behind that barrier (!WCUR_AHEAD: and ring piece n is full);
         //   after it: pre-activation tile n has been read (behind the h barrier of step n - 1): re-armed, handed back to the prep CTA;
-        //   before the h barrier of step n: pre-activation tile n + 1 is full (the compute warps read it behind that barrier);
-        //   after it: ring piece n has been read (empty).
+        //   before the h barrier of step n: pre-activation tile n + 1 is full (WCUR_AHEAD: and ring piece n + 1); the compute warps
+        //     read the tile (and piece n + 1's Wcur fragments) behind that barrier;
+        //   after it: ring piece n has been read (its Wcur behind the h barrier of step n - 1 or the x barrier of step n, its Wres
+        //     before this one): empty.
         const int nsteps = (t_end - t_begin) * L;
         const uint32_t r_apfree = mapa_u32(s_apfree, 2);
-        if (lane == 0 && nsteps > 0) mbar_wait(s_apfull, 0);
+        if (lane == 0 && nsteps > 0) {
+            mbar_wait(s_apfull, 0);
+            if (M::WCUR_AHEAD) mbar_wait(s_full, 0);
+        }
         bar_chain();
         for (int n = 0; n < nsteps; n++) {
             const uint32_t b = (uint32_t)n % M::NAP, hb = (uint32_t)n % M::NHB;
             if (lane == 0) {
-                mbar_wait(s_full + 8 * (n & 1), ((uint32_t)n >> 1) & 1);
+                if (!M::WCUR_AHEAD) mbar_wait(s_full + 8 * M::slot0(n), M::par0(n));
                 mbar_wait(s_hfree + 8 * hb, (((uint32_t)n / M::NHB) & 1) ^ 1);
             }
             __syncwarp();
@@ -1276,11 +1294,14 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
             if (lane == 0) {
                 mbar_arrive_expect_tx(s_apfull + 8 * b, M::AP);    // armed for the tile NAP steps on, before the buffer goes back
                 mbar_arrive_remote(r_apfree + 8 * b);
-                if (n + 1 < nsteps) mbar_wait(s_apfull + 8 * ((uint32_t)(n + 1) % M::NAP), ((uint32_t)(n + 1) / M::NAP) & 1);
+                if (n + 1 < nsteps) {
+                    mbar_wait(s_apfull + 8 * ((uint32_t)(n + 1) % M::NAP), ((uint32_t)(n + 1) / M::NAP) & 1);
+                    if (M::WCUR_AHEAD) mbar_wait(s_full + 8 * M::slot0(n + 1), M::par0(n + 1));
+                }
             }
             __syncwarp();
             bar_chain();                                   // h barrier of step n
-            if (lane == 0) mbar_arrive(s_empty + 8 * (n & 1));
+            if (lane == 0) mbar_arrive(s_empty + 8 * M::slot0(n));
         }
     } else if (w < NCW) {
         const uint32_t rstride = (uint32_t)ntiles_alloc * 2048u;
@@ -1316,8 +1337,17 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
             if (TR == TU) sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
         }
         StepIt it0{t_begin, 0, p.ring_slot};
-        bar_chain();                                       // pre-activation tile 0 has landed
-        if (nsteps > 0) load_ap(0, 0);
+        bar_chain();                                       // pre-activation tile 0 (and ring piece 0) have landed
+        // wc (WCUR_AHEAD): the Wcur fragments of the next step, read behind the h barrier of the step before (they are in a ring
+        // piece the sync warp saw land), so that after the x barrier only the x tile is read before the cur HMMAs
+        GateW wc{};
+        if (nsteps > 0) {
+            load_ap(0, 0);
+            if (M::WCUR_AHEAD) wc = lds_gate_w(sm + M::C_RING, o_t0, o_g0);
+        }
+        auto load_wcur = [&](const uint32_t n1) {
+            if (n1 < (uint32_t)nsteps) wc = lds_gate_w(sm + M::C_RING + M::slot0(n1) * M::PIECE0, o_t0, o_g0);
+        };
 
         uint32_t n = 0, epar = 0;                          // step, sample parity
         for (int t = t_begin; t < t_end; t++) {
@@ -1354,10 +1384,11 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
             TRACE2(0, 2);
 
             for (int l = 0; l < L; l++, n++) {
-                const uint32_t p1 = sm + M::C_RING + (n & 1) * M::PIECE0;
+                const uint32_t p1 = sm + M::C_RING + M::slot0(n) * M::PIECE0;
                 const float2 br = brn;
                 {
-                    const uint4 bt0 = lds128(p1 + o_t0), bg0 = lds128(p1 + o_g0), bt1 = lds128(p1 + o_t0 + 512), bg1 = lds128(p1 + o_g0 + 512);
+                    if (!M::WCUR_AHEAD) wc = lds_gate_w(p1, o_t0, o_g0);
+                    const uint4 bt0 = wc.t0, bg0 = wc.g0, bt1 = wc.t1, bg1 = wc.g1;
                     float u0[4] = {0.f, 0.f, 0.f, 0.f}, u1[4] = {0.f, 0.f, 0.f, 0.f};
                     hmma(accp[0], xa[0], bt0.x, bt0.y); hmma(accp[1], xa[0], bg0.x, bg0.y); hmma(u0, xa[2], bt1.x, bt1.y); hmma(u1, xa[2], bg1.x, bg1.y);
                     hmma(accp[0], xa[1], bt0.z, bt0.w); hmma(accp[1], xa[1], bg0.z, bg0.w); hmma(u0, xa[3], bt1.z, bt1.w); hmma(u1, xa[3], bg1.z, bg1.w);
@@ -1384,6 +1415,9 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
                 float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
                 hmma_res(ra, rb, ha, bw0, bw1);
                 residual<TR>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
+                // after the x store, which the x barrier waits for, so that the store is not queued behind these loads (placed right
+                // after the res HMMAs, the layer step measured slower: DESIGN §5.1b)
+                if (M::WCUR_AHEAD) load_wcur(n + 1);
                 TRACE2(0, 14);
                 dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
                 if (l + 1 < L) {
@@ -1779,7 +1813,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
 
-    // barriers (same offsets in every CTA): ring full[NRING] / empty[NRING] (the chain uses two of each, the tail NSLOT1, the prep NPRING);
+    // barriers (same offsets in every CTA): ring full[NRING] / empty[NRING] (the chain uses NSLOT0 of each, the tail NSLOT1, the prep NPRING);
     // pfull[NPS] (prep: staged history tiles); hfull[NHB] (tail: h tiles, bytes from the chain); hfree[NHB], yfull, apfull[NAP] (chain: bytes from the tail / the prep CTA);
     // apfree[NAP] (prep: arrived by the chain's warps).  Output layers, once per sample: ob0full (prep: relu(skip) bytes from the
     // tail); ob0free (tail: arrived by the prep's warps); ob1full (tail and prep: the peer's relu(Zs) half); ob1free (tail and prep:

@@ -13,6 +13,11 @@ what a passing GPU run cannot show:
   * history visibility: the prep CTA stages x_l[t-d] from global memory with plain loads -- the chain CTA must have finished the step
     that wrote it; the model reports the smallest distance (in chain steps) it saw, which is what `L >= 12` in wn_launch_lat buys.
 
+The chain CTA's weight ring has `nslot0` slots (2 or 3; the kernel's CfgC::NSLOT0).  With `wcur_ahead` (CfgC::WCUR_AHEAD) the
+compute warps read the Wcur fragments of step n + 1 behind the h barrier of step n, and the sync warp waits for ring piece n + 1
+before that barrier; without it they read them behind the x barrier of step n, and the sync warp waits for piece n before the
+x barrier.  By default both follow the kernel: read ahead with three slots for 8 rows, behind the x barrier with two for 16.
+
 Byte counts are those of a cluster of `rows` utterances (16, or 8 when all 8-row clusters are resident): every flow moves
 rows / 16 of its 16-row bytes, with the same arrival counts.
 
@@ -78,9 +83,12 @@ class Proc:
 
 
 class Sim:
-    def __init__(self, L=12, T=3, seed=0, slow=None, bug=None, max_dil=4, rows=16):
-        assert rows in (8, 16)
+    def __init__(self, L=12, T=3, seed=0, slow=None, bug=None, max_dil=4, rows=16, nslot0=None, wcur_ahead=None):
+        wcur_ahead = rows == 8 if wcur_ahead is None else wcur_ahead
+        nslot0 = nslot0 or (3 if wcur_ahead else 2)
+        assert rows in (8, 16) and nslot0 in (2, 3)
         self.L, self.T, self.rows = L, T, rows
+        self.nslot0, self.wcur_ahead = nslot0, wcur_ahead
         self.rng = random.Random(seed)
         self.slow = slow or {}
         self.bug = bug
@@ -92,8 +100,8 @@ class Sim:
             d = d * 2 if d * 2 <= max_dil else 1
         B = lambda n, c: Barrier(self, n, c)
         # chain CTA
-        self.c_full = [B(f"chain.full{i}", 1) for i in range(2)]
-        self.c_empty = [B(f"chain.empty{i}", 1) for i in range(2)]           # arrived by the sync warp
+        self.c_full = [B(f"chain.full{i}", 1) for i in range(nslot0)]
+        self.c_empty = [B(f"chain.empty{i}", 1) for i in range(nslot0)]      # arrived by the sync warp
         self.hfree = [B(f"chain.hfree{i}", NCW) for i in range(2)]
         self.yfull = B("chain.yfull", 1)
         self.apfull = [B(f"chain.apfull{i}", 1) for i in range(NAP)]
@@ -201,14 +209,14 @@ class Sim:
         cur[1] += 1
 
     # ------------------------------------------------------------------ roles
-    def producer(self, who, full, empty, nslots, pieces, slotname):
+    def producer(self, who, full, empty, nslots, pieces, slotname, readers=NCW):
         for n, nbytes in enumerate(pieces):
             sl = n % nslots
             yield ("wait", empty[sl], n // nslots - 1)
             full[sl].expect_tx(nbytes)
 
             def land(n=n, sl=sl, nbytes=nbytes):
-                self.write(f"{slotname}{sl}", n, NCW)
+                self.write(f"{slotname}{sl}", n, readers)
                 full[sl].complete_tx(nbytes)
             self.after(self.lat(300, 900, who), land)
             yield ("delay", self.lat(20, 60, who))
@@ -216,10 +224,12 @@ class Sim:
     def chain_warp(self, w):
         """A compute warp of the chain CTA: its layer step waits only on the CTA barrier it shares with the sync warp."""
         who = f"chain.w{w}"
-        L, T = self.L, self.T
+        L, T, ns = self.L, self.T, self.nslot0
         yield from self.cta_bar("chain", who)
         if self.nsteps:
             self.read(who, "ap0", 0)                         # pre-activation tile 0 (the sync warp saw it land)
+            if self.wcur_ahead:
+                self.read(who, "cring0", 0)                  # Wcur of step 0 (so did ring piece 0)
         k = 0
         for t in range(T):
             if t > 0:
@@ -230,8 +240,11 @@ class Sim:
             self.emb_done[t] = self.emb_done.get(t, 0) + 1
             yield from self.cta_bar("chain", who)            # x barrier
             for l in range(L):
-                self.read(who, f"cring{k & 1}", k)
-                yield ("delay", self.lat(200, 400, who))     # cur GEMM + gate
+                if not self.wcur_ahead:
+                    self.read(who, f"cring{k % ns}", k)      # Wcur of this step
+                yield ("delay", self.lat(100, 200, who))     # cur GEMM
+                self.read(who, f"cring{k % ns}", k)          # Wres of this step, under the gate
+                yield ("delay", self.lat(100, 200, who))     # gate
 
                 def land_h(k=k):                             # this warp's 256 (8 rows: 128) bytes of the h tile + their complete_tx
                     self.touch(f"h{k & 1}", k, NCW)          # (the tail's buffer is free: the sync warp waited before the x barrier)
@@ -241,6 +254,8 @@ class Sim:
                 if k + 1 < self.nsteps:
                     self.read(who, f"ap{(k + 1) % NAP}", k + 1)
                 yield ("delay", self.lat(150, 300, who))     # res GEMM (weights of the same piece)
+                if self.wcur_ahead and k + 1 < self.nsteps:
+                    self.read(who, f"cring{(k + 1) % ns}", k + 1)   # Wcur of the next step (the sync warp saw its piece land)
                 yield ("delay", self.lat(30, 80, who))       # x tile + history ring write of (t, l + 1)
                 self.chain_step_warps[k] = self.chain_step_warps.get(k, 0) + 1
                 while self.chain_step_warps.get(self.chain_steps_done, 0) == NCW:
@@ -252,13 +267,16 @@ class Sim:
     def chain_sync(self):
         """The chain CTA's sync warp (lane 0): every mbarrier wait and hand-back of the layer loop."""
         who = "chain.sync"
+        ns, ahead = self.nslot0, self.wcur_ahead
         if self.nsteps:
             yield ("wait", self.apfull[0], 0)
+            if ahead and self.bug != "no_full_wait":
+                yield ("wait", self.c_full[0], 0)
         yield from self.cta_bar("chain", who)
         for n in range(self.nsteps):
             b, hb = n % NAP, n & 1
-            if self.bug != "no_full_wait":
-                yield ("wait", self.c_full[n & 1], n >> 1)
+            if not ahead and self.bug != "no_full_wait":
+                yield ("wait", self.c_full[n % ns], n // ns)
             if self.bug not in ("no_hfree", "hfree_late"):   # the tail has read h tile n - 2: the compute warps may send tile n
                 yield ("wait", self.hfree[hb], (n >> 1) - 1)
             yield from self.cta_bar("chain", who)            # x barrier of step n: pre-activation tile n has been read
@@ -267,11 +285,15 @@ class Sim:
             self.apfull[b].expect_tx(self.nb(8192))          # armed for the tile NAP steps on, before the "free" signal
             if self.bug != "no_apfree":
                 self.after(self.lat(150, 400), self.apfree[b].arrive)
+            if self.bug == "empty_early":                    # (Wres of piece n is still to be read)
+                self.c_empty[n % ns].arrive()
             if n + 1 < self.nsteps and self.bug != "no_apfull_wait":
                 yield ("wait", self.apfull[(n + 1) % NAP], (n + 1) // NAP)
+            if ahead and n + 1 < self.nsteps and self.bug not in ("no_full_wait", "no_early_full_wait"):
+                yield ("wait", self.c_full[(n + 1) % ns], (n + 1) // ns)
             yield from self.cta_bar("chain", who)            # h barrier of step n: ring piece n has been read
-            if self.bug != "no_empty":
-                self.c_empty[n & 1].arrive()
+            if self.bug not in ("no_empty", "empty_early"):
+                self.c_empty[n % ns].arrive()
             yield ("delay", self.lat(10, 40, who))
 
     def cta_bar(self, cta, who):                             # bar.sync among the compute warps of one CTA (+ the chain's sync warp)
@@ -423,7 +445,7 @@ class Sim:
 
     def build(self):
         L, T = self.L, self.T
-        self.spawn("chain.producer", self.producer("chain.producer", self.c_full, self.c_empty, 2, [24576] * (T * L), "cring"))
+        self.spawn("chain.producer", self.producer("chain.producer", self.c_full, self.c_empty, self.nslot0, [24576] * (T * L), "cring", 2 * NCW))
         self.spawn("tail.producer", self.producer("tail.producer", self.t_full, self.t_empty, TSLOTS, [32768] * (T * L), "tring"))
         self.spawn("prep.producer", self.producer("prep.producer", self.p_full, self.p_empty, 4, [16384] * (T * L), "pring"))
         self.spawn("chain.sync", self.chain_sync())
