@@ -180,6 +180,30 @@ public:
         return rc == 0;
     }
 
+    /* Not in the reference class: live vocoding, mel frames pushed as they arrive into a ring of ring_frames frames per utterance and
+     * each sample's conditioning produced once its frames are in; see nvwn_cond_producer_open_live, nvwn_cond_producer_push and
+     * nvwn_cond_producer_run_stream. */
+    bool cond_producer_open_live(int n_cond_channels, const float* upsample_weight, const float* upsample_bias, int window, int stride,
+                                 const float* cond_weight, const float* cond_bias, int ring_frames, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_open_live(m_engine, n_cond_channels, upsample_weight, upsample_bias, window, stride, cond_weight,
+                                                    cond_bias, ring_frames, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool cond_producer_push(const float* features, int num_frames, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_push(m_engine, features, num_frames, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool cond_producer_run_stream(long long sample_begin, int sample_count, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_run_stream(m_engine, sample_begin, sample_count, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
     /* Not in the reference class: teacher-forced scoring, logp[b * num_samples + t] = log p(audio[b][t] | audio[b][0..t),
      * conditioning) for every step at once, and optionally the fp32 logits; see nvwn_score.  fp16 engines only. */
     bool score(const int* audio, int num_samples, int batch_size, float* logp, float* logits = NULL, cudaStream_t stream = 0)

@@ -82,6 +82,24 @@ int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, i
 /* Streaming (see nvwn_run_stream): samples [sample_begin, sample_begin + sample_count) of the loaded sequence, sample s stored at
  * position s mod num_samples; sample_count <= num_samples.  Asynchronous on `stream` like nvwn_cond_producer_run. */
 int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sample_count, void* stream);
+/* Live vocoding: mel frames that arrive over time, a few at a time, into a bounded ring on the device, and conditioning produced
+ * for each sample as soon as its frames are in.  Sample n reads frames ceil((n - window + 1) / stride) .. floor(n / stride) only,
+ * so its conditioning is final, bit for bit, once frame floor(n / stride) has been pushed: the same bits nvwn_cond_producer_load
+ * of the finished frames gives it.
+ *
+ * _open_live starts a live sequence of 0 frames for the B rows on the whole-batch producer, with a ring of ring_frames frames per
+ * row; ring_frames < ceil(window / stride) + 1 is NVWN_EINVAL.  The network as for nvwn_cond_producer_load; returns when the
+ * sources may be released.  It replaces a loaded sequence, and nvwn_cond_producer_load ends a live one.
+ * _push appends features [B][n_cond_channels][num_frames] (host or device memory) as frames [T, T + num_frames) of the sequence,
+ * T the frames pushed so far.  A host array may be reused on return; device frames are copied in order on `stream`.  A push that
+ * would overwrite a frame a sample not produced yet reads (one at or past the end of the furthest nvwn_cond_producer_run_stream of
+ * this sequence) is NVWN_EINVAL and changes nothing; num_frames = 0 does nothing.  A sequence holds at most INT_MAX samples.
+ * nvwn_cond_producer_run_stream on a live sequence takes samples below T * stride whose frames are all still in the ring (else
+ * NVWN_EINVAL, naming the first missing frame); nvwn_cond_producer_run refuses a live sequence.  Issue pushes and productions on
+ * one stream, or order them: a push writes ring columns that earlier productions read. */
+int nvwn_cond_producer_open_live(nvwn_engine* e, int n_cond_channels, const float* upsample_weight, const float* upsample_bias, int window,
+                                 int stride, const float* cond_weight, const float* cond_bias, int ring_frames, void* stream);
+int nvwn_cond_producer_push(nvwn_engine* e, const float* features, int num_frames, void* stream);
 /* The same arithmetic on the host (needs no GPU; test / reference use): Lh [T*stride][L][B][2R], host pointers. */
 int nvwn_cond_from_features_host(float* Lh, const float* features, int batch_size, int n_cond_channels, int num_frames,
                                  const float* upsample_weight, const float* upsample_bias, int window, int stride,

@@ -54,6 +54,8 @@ SYMBOLS = {
     "nvwn_cond_producer_load": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_cond_producer_run": (C.c_int, [_vp, C.c_int, C.c_int, C.c_int, _vp]),
     "nvwn_cond_producer_run_stream": (C.c_int, [_vp, C.c_longlong, C.c_int, _vp]),
+    "nvwn_cond_producer_open_live": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, _vp]),
+    "nvwn_cond_producer_push": (C.c_int, [_vp, _vp, C.c_int, _vp]),
     "nvwn_cond_from_features_host": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, C.c_int, C.c_int]),
     "nvwn_score": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_score_stream": (C.c_int, [_vp, _vp, C.c_longlong, C.c_int, C.c_int, _vp, _vp, _vp]),

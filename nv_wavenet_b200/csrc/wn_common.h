@@ -169,12 +169,15 @@ cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B,
 cudaError_t wn_cond_transpose_wu(float* WuT, const float* Wu, int C, int K, cudaStream_t stream);
 void wn_cond_host(float* Lh, const float* feat, const float* Wu, const float* bu, const float* Wc, const float* bc,
                   int B, int C, int T, int K, int stride, int L, int R);
-// row i of a chunk is the utterance with frames [C][T] at frames + foff whose sample 0 is absolute sample start
+// row i of a chunk is the utterance with frames [C][T] at frames + foff whose sample 0 is absolute sample start; in a live sequence
+// (DESIGN.md §6) its frames are a ring [C][ring] there instead, frame m at column m mod ring, and T counts the frames pushed so far
 struct WnCondSlot {
     long long foff, start;
-    int T, pad;
+    int T, ring;
 };
 // out [m][L][k][2R] for absolute samples [n0, n0 + m) of the k utterances in tab (device); with `mask`, zero at or past each one's
-// end (without it the caller knows no utterance ends before n0 + m); U scratch holds k * m * C floats
+// end (without it the caller knows no utterance ends before n0 + m); with `ring`, the rows' frames are rings and the caller has
+// checked that every frame the samples read is still in them; U scratch holds k * m * C floats
 cudaError_t wn_cond_produce_slots(float* out, float* U, const float* frames, const WnCondSlot* tab, const float* WuT, const float* bu, const float* Wc,
-                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, bool mask, cudaStream_t stream);
+                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, bool mask, bool ring,
+                                  cudaStream_t stream);

@@ -22,18 +22,22 @@ namespace {
 
 // u[b][co][n] of the trimmed transposed convolution.  features [B][C][T], Wu [C_in][C_out][K] (torch ConvTranspose1d
 // layout) or, with WU_T, its [K][C_in][C_out] transpose (coalesced across co).  out[n] += in[m] * W[k] for m*stride + k = n.
-template <bool WU_T>
+// With RING the frames are a ring [B][C][F] (F = ring): frame m at column m mod F.  Either way sample n reads frames
+// ceil((n - K + 1) / stride) .. floor(n / stride), in that order from the last, so its value is fixed once frame floor(n / stride) is in.
+template <bool WU_T, bool RING = false>
 __host__ __device__ inline float upsample_element(const float* __restrict__ feat, const float* __restrict__ Wu, const float* __restrict__ bu,
-                                                  int C, int T, int K, int stride, int b, int co, int n)
+                                                  int C, int T, int K, int stride, int b, int co, int n, int ring = 0)
 {
+    const int pitch = RING ? ring : T;
     float acc = bu[co];
     for (int m = n / stride; m >= 0; m--) {
         const int k = n - m * stride;
         if (k >= K) break;
         if (m >= T) continue;
+        const int col = RING ? m % ring : m;
         for (int ci = 0; ci < C; ci++) {
             const float w = WU_T ? Wu[((size_t)k * C + ci) * C + co] : Wu[((size_t)ci * C + co) * K + k];
-            acc = fmaf(feat[((size_t)b * C + ci) * T + m], w, acc);
+            acc = fmaf(feat[((size_t)b * C + ci) * pitch + col], w, acc);
         }
     }
     return acc;
@@ -58,8 +62,9 @@ __global__ void transpose_wu_kernel(float* __restrict__ dst, const float* __rest
 }
 
 // U[i][j][co] for the k rows of a chunk, row i = absolute sample n0 + j of the utterance in tab[i], i.e. sample n0 + j - start of
-// its own frames [C][T] at frames + foff.  Samples at or past its end (T * stride) are left at 0: mask_slots_kernel zeroes their
-// projected rows.
+// its own frames [C][T] at frames + foff, or with RING its ring [C][ring] there.  Samples at or past its end (T * stride) are left
+// at 0: mask_slots_kernel zeroes their projected rows.
+template <bool RING>
 __global__ void upsample_slots_kernel(float* __restrict__ U, const float* __restrict__ frames, const WnCondSlot* __restrict__ tab,
                                       const float* __restrict__ WuT, const float* __restrict__ bu, int k, int C, int K, int stride, long long n0, int m)
 {
@@ -68,7 +73,7 @@ __global__ void upsample_slots_kernel(float* __restrict__ U, const float* __rest
         const int co = (int)(i % C), j = (int)((i / C) % m), r = (int)(i / ((size_t)C * m));
         const WnCondSlot s = tab[r];
         const long long n = n0 + j - s.start;
-        U[i] = n < (long long)s.T * stride ? upsample_element<true>(frames + s.foff, WuT, bu, C, s.T, K, stride, 0, co, (int)n) : 0.f;
+        U[i] = n < (long long)s.T * stride ? upsample_element<true, RING>(frames + s.foff, WuT, bu, C, s.T, K, stride, 0, co, (int)n, s.ring) : 0.f;
     }
 }
 
@@ -192,10 +197,12 @@ cudaError_t wn_cond_transpose_wu(float* WuT, const float* Wu, int C, int K, cuda
 }
 
 cudaError_t wn_cond_produce_slots(float* out, float* U, const float* frames, const WnCondSlot* tab, const float* WuT, const float* bu, const float* Wc,
-                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, bool mask, cudaStream_t stream)
+                                  const float* bc, int k, int C, int K, int stride, int L, int R, long long n0, int m, bool mask, bool ring,
+                                  cudaStream_t stream)
 {
     if (m <= 0) return cudaSuccess;
-    upsample_slots_kernel<<<grid_for((size_t)k * m * C), 256, 0, stream>>>(U, frames, tab, WuT, bu, k, C, K, stride, n0, m);
+    if (ring) upsample_slots_kernel<true><<<grid_for((size_t)k * m * C), 256, 0, stream>>>(U, frames, tab, WuT, bu, k, C, K, stride, n0, m);
+    else upsample_slots_kernel<false><<<grid_for((size_t)k * m * C), 256, 0, stream>>>(U, frames, tab, WuT, bu, k, C, K, stride, n0, m);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = project(out, U, Wc, bc, k, C, L, R, m, stream);     // rows b * m + j -> out[j][l][b][2R]: the chunk's layout
     if (e != cudaSuccess || !mask) return e;

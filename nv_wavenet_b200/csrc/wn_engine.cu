@@ -83,8 +83,13 @@ struct DevBuf : std::unique_ptr<T, CudaFree> {
 // A conditioning producer (DESIGN.md §6): a network of C channels, upsampling window K and stride; `scratch` of cond_scratch()'s
 // layout, chunks of up to `rows` (row, sample) rows; row b's frames [C][T[b]] at frames + b * cap * C; the row list and WnCondSlot
 // table of the last production (device); per row on the host, the frames of its utterance (0: none) and its absolute start.
+// A live sequence of the whole-batch producer (nvwn_cond_producer_open_live) keeps row b's frames in a ring [C][ring] at
+// frames + b * ring * C, T[b] counting the frames pushed so far, and `produced` is the end of its furthest production: the
+// frames the samples from there on read may not be overwritten.
 struct CondProducer {
     int C = 0, K = 0, stride = 0, rows = 0;
+    int ring = 0;                            // frames per row of a live sequence's ring; 0: frames loaded whole
+    long long produced = 0;
     DevBuf<float> scratch;
     size_t scratch_floats = 0;
     DevBuf<float> frames;
@@ -271,7 +276,7 @@ int produce(nvwn_engine* e, const CondProducer& P, const std::string& who, const
         const int m = count - done < chunk ? count - done : chunk;
         const long long t0 = t_first + done;
         ce = wn_cond_produce_slots(w + o.out, w + o.u, P.frames, tab, w + o.wut, w + o.bu, w + o.wc, w + o.bc, n, P.C, P.K, P.stride, e->L, e->R,
-                                   t0, m, end < t0 + m, st);
+                                   t0, m, end < t0 + m, P.ring > 0, st);
         if (ce == cudaSuccess)
             ce = rows ? e->family->convert_rows(*e, e->Lh, w + o.out, rows_dev, n, pos + done, m, st) : e->family->convert(*e, e->Lh, w + o.out, pos + done, m, st);
     }
@@ -287,6 +292,13 @@ int check_window(const nvwn_engine* e, const std::string& who, long long first_s
     const std::string got = first_sample < 0 ? "first_sample " + std::to_string(first_sample) + " < 0" : std::string(count_name) + " = " + std::to_string(count);
     return fail(NVWN_EINVAL, who + ": need first_sample >= 0 and " + std::to_string(least) + " <= " + count_name + " <= num_samples (" +
                                  std::to_string(e->N) + ") of the engine; got " + got);
+}
+
+// The first frame that sample n of a sequence reads: frames ceil((n - K + 1) / stride) .. floor(n / stride), none below 0
+long long first_frame(long long n, int K, int stride)
+{
+    const long long lo = n - K + 1;
+    return lo <= 0 ? 0 : (lo + stride - 1) / stride;
 }
 
 // The batch a run, or a prime, may take: the tensor-core kernels take whole batches only, and so does every run after a per-slot
@@ -658,6 +670,7 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
     cudaStream_t st = (cudaStream_t)stream;
     CondProducer& P = e->cond_whole;
     P.T.assign(e->B, 0);                                                      // loaded once every copy has been made
+    P.ring = 0;                                                               // ends a live sequence
     int rc = put_cond_network(e, P, "nvwn_cond_producer_load", C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
     if (rc != 0) return rc;
     // features [B][C][T] are the frame arena with cap = T, in one copy; row b's utterance starts at sample 0
@@ -682,6 +695,7 @@ int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, i
 {
     if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: NULL engine");
     const CondProducer& P = e->cond_whole;
+    if (P.ring) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: a live sequence is produced with nvwn_cond_producer_run_stream");
     if (P.T[0] < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: nvwn_cond_producer_load has not been called");
     const long long Nn = (long long)P.T[0] * P.stride;
     if (sample_begin < 0 || sample_count < 0 || sample_begin + (long long)sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run: sample range outside num_frames * stride");
@@ -691,17 +705,102 @@ int nvwn_cond_producer_run(nvwn_engine* e, int first_sample, int sample_begin, i
 
 int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sample_count, void* stream)
 {
-    if (!e) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: NULL engine");
-    const CondProducer& P = e->cond_whole;
-    if (P.T[0] < 1) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: nvwn_cond_producer_load has not been called");
+    const std::string who = "nvwn_cond_producer_run_stream";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    CondProducer& P = e->cond_whole;
+    if (P.T[0] < 1 && !P.ring) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_load has not been called");
     const long long Nn = (long long)P.T[0] * P.stride;
-    if (sample_begin < 0 || sample_count < 0 || sample_begin + sample_count > Nn) return fail(NVWN_EINVAL, "nvwn_cond_producer_run_stream: sample range outside num_frames * stride");
-    int rc = check_window(e, "nvwn_cond_producer_run_stream", sample_begin, sample_count, "sample_count", 0);
+    if (sample_begin < 0 || sample_count < 0 || sample_begin + sample_count > Nn)
+        return fail(NVWN_EINVAL, P.ring ? who + ": samples [" + std::to_string(sample_begin) + ", " + std::to_string(sample_begin + sample_count) +
+                                             ") of the live sequence are not all below the " + std::to_string(Nn) + " its " + std::to_string(P.T[0]) +
+                                             " pushed frames give"
+                                        : who + ": sample range outside num_frames * stride");
+    int rc = check_window(e, who, sample_begin, sample_count, "sample_count", 0);
     if (rc != 0) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (P.ring && sample_count > 0) {
+        // the ring holds frames [T - ring, T): the first frame the range reads must still be there
+        const long long need = first_frame(sample_begin, P.K, P.stride);
+        if (need < (long long)P.T[0] - P.ring)
+            return fail(NVWN_EINVAL, who + ": frame " + std::to_string(need) + ", which sample " + std::to_string(sample_begin) +
+                                         " reads, has left the ring (it holds frames " + std::to_string(P.T[0] - P.ring) + " .. " +
+                                         std::to_string(P.T[0] - 1) + ")");
+        // the table with the frame count of now, staged from pageable memory in stream order
+        std::vector<WnCondSlot> tab(e->B);
+        for (int b = 0; b < e->B; b++) tab[b] = {(long long)b * P.C * P.ring, 0, P.T[0], P.ring};
+        CK(cudaMemcpyAsync(P.tables + cond_table_offset(e), tab.data(), tab.size() * sizeof(WnCondSlot), cudaMemcpyHostToDevice, st));
+        if (sample_begin + sample_count > P.produced) P.produced = sample_begin + sample_count;
+    }
     for (const WrapPiece& w : split_at_wrap(sample_begin, sample_count, e->N)) {
-        rc = produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin + w.off, w.pos, w.len, (cudaStream_t)stream);
+        rc = produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin + w.off, w.pos, w.len, st);
         if (rc != 0) return rc;
     }
+    return 0;
+}
+
+int nvwn_cond_producer_open_live(nvwn_engine* e, int n_cond_channels, const float* upsample_weight, const float* upsample_bias, int window, int stride,
+                                 const float* cond_weight, const float* cond_bias, int ring_frames, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_open_live";
+    if (!e || !upsample_weight || !upsample_bias || !cond_weight || !cond_bias) return fail(NVWN_EINVAL, who + ": NULL argument");
+    const int C = n_cond_channels, K = window;
+    if (C < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, who + ": bad sizes (need n_cond_channels >= 1 and window >= stride >= 1)");
+    const int least = (K + stride - 1) / stride + 1;
+    if (ring_frames < least)
+        return fail(NVWN_EINVAL, who + ": ring_frames = " + std::to_string(ring_frames) + "; need at least ceil(window / stride) + 1 = " +
+                                     std::to_string(least));
+    cudaStream_t st = (cudaStream_t)stream;
+    CondProducer& P = e->cond_whole;
+    P.T.assign(e->B, 0);                                                      // replaces a loaded sequence
+    P.ring = 0;
+    int rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
+    if (rc != 0) return rc;
+    const size_t n_ring = (size_t)e->B * C * ring_frames;
+    if (n_ring > P.frames_floats) {
+        if (P.frames) CK(cudaDeviceSynchronize());                          // no launch reads the old frames any more
+        CK(P.frames.alloc(n_ring * sizeof(float)));
+        P.frames_floats = n_ring;
+    }
+    const cudaError_t ce = cudaStreamSynchronize(st);                        // host sources may be released by the caller now
+    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
+    P.ring = ring_frames;
+    P.produced = 0;
+    return 0;
+}
+
+int nvwn_cond_producer_push(nvwn_engine* e, const float* features, int num_frames, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_push";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    CondProducer& P = e->cond_whole;
+    if (!P.ring) return fail(NVWN_EINVAL, who + ": no live sequence is open (nvwn_cond_producer_open_live; nvwn_cond_producer_load ends one)");
+    if (num_frames < 0) return fail(NVWN_EINVAL, who + ": num_frames = " + std::to_string(num_frames) + " < 0");
+    if (num_frames == 0) return 0;
+    if (!features) return fail(NVWN_EINVAL, who + ": features is NULL");
+    const long long T = P.T[0], T1 = T + num_frames;
+    if (T1 * P.stride > INT_MAX)
+        return fail(NVWN_EINVAL, who + ": a live sequence holds at most INT_MAX samples; " + std::to_string(T1) + " frames would give " +
+                                     std::to_string(T1 * P.stride));
+    // frames [T, T1) go where frames [T - ring, T1 - ring) were; the samples from `produced` on read frames from first_frame(produced)
+    const long long keep = first_frame(P.produced, P.K, P.stride);
+    if (T1 - P.ring > keep)
+        return fail(NVWN_EINVAL, who + ": " + std::to_string(num_frames) + " frames would overwrite frame " + std::to_string(keep) +
+                                     ", which sample " + std::to_string(P.produced) + " (not produced yet) reads; at most " +
+                                     std::to_string(keep + P.ring - T) + " frames fit before production moves on");
+    cudaStream_t st = (cudaStream_t)stream;
+    // [B][C][num_frames] -> columns T mod ring ... of the B * C ring rows, split at the wrap.  A host source is snapshotted into
+    // pageable memory, which the copies stage before they return: the caller's array (pinned or not) is free again on return.
+    std::vector<float> snap;
+    const float* src = features;
+    if (!is_device_ptr(features)) {
+        snap.assign(features, features + (size_t)e->B * P.C * num_frames);
+        src = snap.data();
+    }
+    const size_t f = sizeof(float);
+    for (const WrapPiece& w : split_at_wrap(T, num_frames, P.ring))
+        CK(cudaMemcpy2DAsync(P.frames + w.pos, (size_t)P.ring * f, src + w.off, (size_t)num_frames * f, (size_t)w.len * f, (size_t)e->B * P.C,
+                             cudaMemcpyDefault, st));
+    P.T.assign(e->B, (int)T1);
     return 0;
 }
 

@@ -70,6 +70,25 @@ def split_at_wrap(first_sample, count, num_samples):
     return pieces
 
 
+def live_frames(first_sample, count, window, stride):
+    """Frames [lo, hi) that samples [first_sample, first_sample + count), count >= 1, of a sequence read through an upsampling
+    window of `window` samples and `stride`: sample n reads frames ceil((n - window + 1) / stride) .. floor(n / stride), none below 0."""
+    lo = max(0, -(-(first_sample - window + 1) // stride))
+    return lo, (first_sample + count - 1) // stride + 1
+
+
+def live_push_limit(frames, produced, ring_frames, window, stride):
+    """The most frames a push may append to a live sequence of `frames` frames whose productions reach sample `produced`: the ring of
+    `ring_frames` frames per row must keep every frame the samples from `produced` on read (nvwn_cond_producer_push)."""
+    return live_frames(produced, 1, window, stride)[0] + ring_frames - frames
+
+
+def live_ring_frames(samples, window, stride):
+    """A ring size for live pieces of up to `samples` samples: the most frames such a piece can read, plus one for the next push,
+    so every push of one frame fits once everything before it has been produced; never below ceil(window / stride) + 1."""
+    return (samples + window - 2) // stride + 2
+
+
 class NVWavenetInfer:
     """nvWavenetInfer(numLayers, maxDilation, batchSize, numSamples, impl=0, tanhEmbed=True)
     with the template parameters (precision, R, S, A) as keyword arguments."""
@@ -162,6 +181,28 @@ class NVWavenetInfer:
         """Second half: conditioning of samples [sample_begin, sample_begin + sample_count) of the loaded sequence, asynchronously on
         `stream` (record an event after it and make the generating stream wait for it)."""
         check(self._l.nvwn_cond_producer_run(self._h, first_sample, sample_begin, sample_count, _stream(stream)), "condProducerRun")
+
+    def cond_producer_open_live(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, ring_frames, stream=None):
+        """Starts a live sequence of 0 frames on the whole-batch producer with the conditioning network of
+        set_conditioning_from_features and a ring of `ring_frames` frames per utterance; frames then arrive with cond_producer_push
+        and cond_producer_run_stream produces the samples they complete.  Replaces a loaded sequence; see nvwn_cond_producer_open_live."""
+        Cc, window = check_cond_network(self.L, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, ValueError,
+                                        "condProducerOpenLive")
+        wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
+        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
+        check(self._l.nvwn_cond_producer_open_live(self._h, Cc, wu, bu, window, stride, wc, bc, ring_frames, _stream(stream)),
+              "condProducerOpenLive")
+        self._cond_channels = Cc
+
+    def cond_producer_push(self, features, stream=None):
+        """Appends features [B][C][n] (numpy array or torch tensor) to the live sequence.  Host frames may be reused on return; CUDA
+        frames are copied in order on `stream`: keep what this returns alive until then."""
+        shape = tuple(int(v) for v in features.shape)
+        if len(shape) != 3 or shape[0] != self.B or shape[1] != getattr(self, "_cond_channels", shape[1]):
+            raise ValueError(f"condProducerPush: features must be [{self.B}][C][n] with the C of cond_producer_open_live; got {shape}")
+        f, keep = _ptr(features, np.float32)
+        check(self._l.nvwn_cond_producer_push(self._h, f, shape[2], _stream(stream)), "condProducerPush")
+        return keep
 
     # ---- streaming: the N-sample buffers used as rings (nvwn_run_stream); ranges are in absolute samples ----
     def set_selectors_random_stream(self, seed, first_sample, num_samples, stream=None):

@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .infer import check_cond_network
+from .infer import check_cond_network, live_push_limit, live_ring_frames
 
 
 class Impl:
@@ -157,6 +157,64 @@ def _check_window(window):
         raise AssertionError(f"window must be at least 1; got {window}")
 
 
+class LiveSession:
+    """Live vocoding of one batch of utterances whose mel frames arrive over time (NVWaveNet.open_live): each push appends frames
+    and generates every sample they complete, so audio starts with the first frames and an open-ended stream can be vocoded.
+    The session owns its engine of `window` samples; close() releases it."""
+
+    device = "cuda"                 # where push() puts its samples
+
+    def __init__(self, eng, channels, upsample_window, stride, seed, window):
+        self._eng = eng
+        self.channels, self.upsample_window, self.stride, self.seed, self.window = channels, upsample_window, stride, seed, window
+        self.ring_frames = live_ring_frames(window, upsample_window, stride)
+        self.frames = 0             # frames pushed so far
+        self.samples = 0            # samples generated so far: every sample the frames complete, [0, frames * stride)
+
+    def push(self, frames, audio=None, saturate=False):
+        """Appends frames [batch][C][n] (numpy array or torch tensor, n >= 0) and generates samples [samples, (frames + n) * stride),
+        in pieces of at most `window` samples, each one's conditioning produced from the ring just before it is generated.  Frames
+        the ring cannot take at once are fed in pieces, each generated before the next is pushed.  Returns those samples as an
+        int32 CUDA tensor [batch][k]; with audio="float" or "int16" returns (samples, audio), audio the mu-law decoded samples
+        [batch][k] as a numpy array (get_audio_stream; saturate as for get_audio).  Together the pushes give infer() of the finished
+        utterance with the same seed and window, bit for bit."""
+        if audio not in (None, "float", "int16"):
+            raise AssertionError(f"push: audio is None, 'float' or 'int16'; got {audio!r}")
+        shape = tuple(int(v) for v in frames.shape)
+        if len(shape) != 3 or shape[:2] != (self._eng.B, self.channels):
+            raise AssertionError(f"push: frames must be [{self._eng.B}][{self.channels}][n]; got {shape}")
+        frames = frames.to(torch.float32) if isinstance(frames, torch.Tensor) else np.asarray(frames, np.float32)
+        eng, n, done = self._eng, shape[2], 0
+        ys, auds = [], []
+        while True:
+            k = min(n - done, live_push_limit(self.frames, self.samples, self.ring_frames, self.upsample_window, self.stride))
+            if k > 0:
+                eng.cond_producer_push(frames[:, :, done:done + k])
+                self.frames += k
+                done += k
+            end = self.frames * self.stride
+            while self.samples < end:
+                first, m = self.samples, min(self.window, end - self.samples)
+                eng.cond_producer_run_stream(first, m)
+                eng.set_selectors_random_stream(self.seed, first, m)
+                eng.run_stream(first, m, eng.B)
+                ys.append(eng.get_yout_stream(torch.empty((eng.B, m), dtype=torch.int32, device=self.device), first, m))
+                if audio is not None:
+                    auds.append(eng.get_audio_stream(first, m, int16=audio == "int16", saturate=saturate))
+                self.samples += m
+            if done == n:
+                break
+        y = torch.cat(ys, dim=1) if ys else torch.empty((eng.B, 0), dtype=torch.int32, device=self.device)
+        if audio is None:
+            return y
+        return y, np.concatenate(auds, axis=1) if auds else np.empty((eng.B, 0), np.int16 if audio == "int16" else np.float32)
+
+    def close(self):
+        if self._eng is not None:
+            self._eng.close()
+            self._eng = None
+
+
 class NVWaveNet:
     def __init__(self, embedding_prev, embedding_curr, conv_out_weight, conv_end_weight, dilate_weights, dilate_biases,
                  max_dilation, res_weights, res_biases, skip_weights, skip_biases, use_embed_tanh):
@@ -205,21 +263,43 @@ class NVWaveNet:
 
     def _engine(self, batch_size, sample_count, fp16):
         """The persistent engine for this problem size (created and loaded on first use)."""
-        from .infer import NVWavenetInfer
         key = (batch_size, sample_count, bool(fp16))
         eng = self._engines.get(key)
         if eng is None:
-            eng = NVWavenetInfer(self.num_layers, self.max_dilation, batch_size, sample_count, 0, bool(self.use_embed_tanh),
-                                 R=self.R, S=self.S, A=self.A, dtype=_lib.FP16 if fp16 else _lib.FP32)
-            f32 = lambda t: t.float().contiguous()
-            eng.set_embeddings(f32(self.embedding_prev), f32(self.embedding_curr))
-            for l, layer in enumerate(self.layers):
-                eng.set_layer_weights(l, *[f32(t) for t in layer])
-            zero = torch.zeros(self.A, dtype=torch.float32)                 # "We didn't use biases on our outputs" (wavenet_infer.cu:75-82)
-            eng.set_out_weights(f32(self.conv_out), zero, f32(self.conv_end), zero)
+            eng = self._new_engine(batch_size, sample_count, fp16)
             self._engines[key] = eng
             self.engines_created += 1
         return eng
+
+    def _new_engine(self, batch_size, sample_count, fp16):
+        """A new engine of this problem size with the model's weights."""
+        from .infer import NVWavenetInfer
+        eng = NVWavenetInfer(self.num_layers, self.max_dilation, batch_size, sample_count, 0, bool(self.use_embed_tanh),
+                             R=self.R, S=self.S, A=self.A, dtype=_lib.FP16 if fp16 else _lib.FP32)
+        f32 = lambda t: t.float().contiguous()
+        eng.set_embeddings(f32(self.embedding_prev), f32(self.embedding_curr))
+        for l, layer in enumerate(self.layers):
+            eng.set_layer_weights(l, *[f32(t) for t in layer])
+        zero = torch.zeros(self.A, dtype=torch.float32)                     # "We didn't use biases on our outputs" (wavenet_infer.cu:75-82)
+        eng.set_out_weights(f32(self.conv_out), zero, f32(self.conv_end), zero)
+        return eng
+
+    def open_live(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, batch_size, seed, window=4096, fp16=False):
+        """Live vocoding: a LiveSession that generates `batch_size` utterances while their mel frames [batch][C][n] are still
+        arriving (LiveSession.push).  The conditioning network is that of set_conditioning_from_features (upsample_weight [C][C][w],
+        upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]; numpy arrays or torch tensors); the frames go
+        into a ring on the device of live_ring_frames(window, w, stride) frames per utterance.  Selectors are Philox under `seed`,
+        drawn by absolute sample, so the pushes together give infer(cond, seed=seed, fp16=fp16, window=window) of the finished
+        frames' conditioning (nvwn_cond_from_features_host), bit for bit.  The session has an engine of its own, apart from the
+        engines infer() and the other calls share."""
+        Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
+                                    "open_live")
+        if batch_size < 1 or window is None or window < 1:
+            raise AssertionError(f"open_live: need batch_size >= 1 and window >= 1; got {batch_size}, {window}")
+        eng = self._new_engine(batch_size, window, fp16)
+        eng.cond_producer_open_live(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride,
+                                    live_ring_frames(window, up, stride))
+        return LiveSession(eng, Cc, up, stride, seed, window)
 
     def _cond_size(self, cond_input):
         """(batch, samples) of conditioning channels x batch x num_layers x samples."""
