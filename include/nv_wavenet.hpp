@@ -180,6 +180,28 @@ public:
         return rc == 0;
     }
 
+    /* Not in the reference class: live frames for single slots, each slot's utterance fed from a ring of its own; see
+     * nvwn_cond_producer_open_live_slots, nvwn_cond_producer_attach_live and nvwn_cond_producer_push_slots. */
+    bool cond_producer_open_live_slots(int ring_frames, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_open_live_slots(m_engine, ring_frames, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool cond_producer_attach_live(const int* slots, int n, const long long* starts, const int* first_frames, const float* const* features,
+                                   const int* num_frames, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_attach_live(m_engine, slots, n, starts, first_frames, features, num_frames, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool cond_producer_push_slots(const int* slots, int n, const float* const* features, const int* num_frames, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_cond_producer_push_slots(m_engine, slots, n, features, num_frames, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
     /* Not in the reference class: live vocoding, mel frames pushed as they arrive into a ring of ring_frames frames per utterance and
      * each sample's conditioning produced once its frames are in; see nvwn_cond_producer_open_live, nvwn_cond_producer_push and
      * nvwn_cond_producer_run_stream. */
@@ -242,6 +264,27 @@ public:
     bool prime_slots_from_score(const int* rows, const int* slots, int n, const unsigned long long* seeds = NULL, cudaStream_t stream = 0)
     {
         const int rc = nvwn_prime_slots_from_score(m_engine, rows, slots, n, seeds, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+
+    /* Not in the reference class: park slots and resume them in any slot of any engine of the same dtype, R, L and maxDil.
+     * slot_state_bytes is the size of one state (0 on failure); see nvwn_save_slots and nvwn_load_slots. */
+    unsigned long long slot_state_bytes()
+    {
+        unsigned long long bytes = 0;
+        if (nvwn_slot_state_bytes(m_engine, &bytes) != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return bytes;
+    }
+    bool save_slots(const int* slots, int n, void* states, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_save_slots(m_engine, slots, n, states, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    bool load_slots(const int* slots, int n, const void* states, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_load_slots(m_engine, slots, n, states, stream);
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }

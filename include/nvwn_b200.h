@@ -170,6 +170,26 @@ int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const 
  * at position t mod N: slot s gets sample t - start of its utterance, and 0 at or past that utterance's end.  Every listed slot needs
  * an attached utterance with start <= first_sample.  Asynchronous on `stream`; other rows are not touched. */
 int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long long first_sample, int num_samples, void* stream);
+/* Live frames for single slots: each slot's utterance gets its mel frames as they arrive, into a ring of its own, as the whole-batch
+ * live sequence of nvwn_cond_producer_open_live does for a batch that moves in lockstep.
+ *
+ * _open_live_slots switches the per-slot producer (after nvwn_cond_producer_set_weights) to rings of ring_frames >= ceil(window /
+ * stride) + 1 frames per slot and forgets every attached utterance.  Until nvwn_cond_producer_set_weights or nvwn_reset_history
+ * leaves this live mode, _set_slots is NVWN_EINVAL. */
+int nvwn_cond_producer_open_live_slots(nvwn_engine* e, int ring_frames, void* stream);
+/* Slot slots[i] takes a live utterance whose sample 0 is absolute sample starts[i] (negative for a resumed utterance further along than
+ * the engine), with its frames [first_frames[i], first_frames[i] + num_frames[i]) given as features[i] [n_cond_channels][num_frames[i]],
+ * num_frames[i] <= ring_frames; the frames before first_frames[i] count as pushed but have left the ring.  A fresh utterance passes
+ * first_frames 0 and num_frames 0, and may pass NULL features.  Host frames may be reused on return; device frames are copied in
+ * order on `stream`. */
+int nvwn_cond_producer_attach_live(nvwn_engine* e, const int* slots, int n, const long long* starts, const int* first_frames,
+                                   const float* const* features, const int* num_frames, void* stream);
+/* Appends features[i] [n_cond_channels][num_frames[i]] to slot slots[i]'s live utterance.  Refused with NVWN_EINVAL, changing nothing,
+ * when a push would overwrite a frame that a sample of that slot not produced yet reads (as nvwn_cond_producer_push), or a slot has no
+ * live utterance.  Host frames may be reused on return.
+ * nvwn_cond_producer_run_slots produces a live slot from its ring: its end is T * stride for the T frames pushed so far, samples past
+ * it are 0, and a range whose first sample reads a frame no longer in the ring is NVWN_EINVAL. */
+int nvwn_cond_producer_push_slots(nvwn_engine* e, const int* slots, int n, const float* const* features, const int* num_frames, void* stream);
 /* nv_wavenet.cuh:439-444: 2-D copy of yOut[b][offset .. offset+size) for every b */
 int nvwn_get_yout(nvwn_engine* e, int* yOut, int offset, int size, void* stream);
 /* Output side (SURVEY.md 8f next-3): replaces the host post-processing of pytorch/nv_wavenet_inference.py:55-60 --
@@ -249,6 +269,41 @@ int nvwn_prime_from_score(nvwn_engine* e, void* stream);
  * slot list (1 <= n <= B, distinct slots in [0, B)).  NVWN_FP16 engines only (else NVWN_EUNSUPPORTED).  Numerics as
  * nvwn_prime_from_score. */
 int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slots, int n, const unsigned long long* seeds, void* stream);
+/* Slot states: park a slot's utterance and resume it later, in any slot of any engine of the same dtype, R, L and maxDil.  Between
+ * launches a slot's whole state is its history row, its two fed-back indices and its selector origin and seed, and an utterance's
+ * samples do not depend on its slot, its start or its neighbours; so a saved and loaded utterance goes on with the bits it would
+ * have had without the pause (DESIGN.md §6).  A state is a blob of nvwn_slot_state_bytes bytes, the same for every kernel family
+ * and any B or N:
+ *   - this 64-byte header, with position = the samples the utterance has generated or been primed with;
+ *   - then for each layer l in order the layer inputs x_l of its times [position - d_l, position) as [d_l][R], in the ring's
+ *     element type (fp16 on NVWN_FP16 engines, fp32 otherwise, so fp32 engines resume bit-exact); d_l = 1, 2, 4, ... doubling
+ *     per layer and back to 1 past maxDil.  Times before 0 hold zeros. */
+typedef struct {
+    unsigned int tag;                   /* NVWN_SLOT_STATE_TAG */
+    int dtype, R, L, max_dilation;
+    int y_prev, y_cur;                  /* the fed-back indices: the codes of the two samples before `position` */
+    int reserved0;
+    long long position;
+    unsigned long long seed;            /* the selector key (nvwn_restart_slots) */
+    unsigned long long reserved[2];     /* zero */
+} nvwn_slot_state_header;
+enum { NVWN_SLOT_STATE_TAG = 0x3153564E };     /* "NVS1" */
+int nvwn_slot_state_bytes(nvwn_engine* e, unsigned long long* bytes);
+/* Writes the states of slots slots[0..n) at the engine's next sample to states + i * nvwn_slot_state_bytes, host or device memory
+ * (16-byte aligned).  The engine does not change.  Device states are written asynchronously on `stream`; host states are complete
+ * on return.  The slots' history rows are read at the engine's batch stride, where the per-slot calls and every run of the whole
+ * batch keep them.  A bad slot list is NVWN_EINVAL. */
+int nvwn_save_slots(nvwn_engine* e, const int* slots, int n, void* states, void* stream);
+/* Slot slots[i] continues state i (states + i * nvwn_slot_state_bytes, host or device memory, 16-byte aligned) from the engine's
+ * next sample t0: its history row is cleared and the state's inputs written at engine times t0 - d_l .. t0 - 1 (negative times
+ * included), its fed-back indices set, its selector origin set to t0 - position and its key to the state's seed, so
+ * nvwn_set_selectors_random_slots draws what the utterance would have drawn.  A per-slot call, as nvwn_restart_slots.  The first
+ * such call at t0 < maxDil since nvwn_reset_history also zeroes the negative times of every slot and makes every launch read the
+ * history at every step, as nvwn_prime_slots_from_score does.  Host states may be reused on return; device states are read in
+ * order on `stream` (their headers are read before return).  Refused with NVWN_EINVAL, changing nothing: NULL arguments, a bad
+ * slot list, a header whose tag, dtype, R, L or max_dilation differs from the engine's, or whose position or indices are out of
+ * range.  That the state was made with the same weights is the caller's responsibility: nothing in it records them. */
+int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states, void* stream);
 
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);

@@ -47,6 +47,9 @@ SYMBOLS = {
     "nvwn_cond_producer_set_weights": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_cond_producer_set_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp]),
     "nvwn_cond_producer_run_slots": (C.c_int, [_vp, _vp, C.c_int, C.c_longlong, C.c_int, _vp]),
+    "nvwn_cond_producer_open_live_slots": (C.c_int, [_vp, C.c_int, _vp]),
+    "nvwn_cond_producer_attach_live": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]),
+    "nvwn_cond_producer_push_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp]),
     "nvwn_get_yout": (C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp]),
     "nvwn_get_audio": (C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int, _vp]),
     "nvwn_mulaw_table": (C.c_int, [C.c_int, _vp, _vp, _vp]),
@@ -62,6 +65,9 @@ SYMBOLS = {
     "nvwn_score_stream_packed": (C.c_int, [_vp, _vp, _vp, C.c_longlong, C.c_int, C.c_int, _vp, _vp, _vp]),
     "nvwn_prime_from_score": (C.c_int, [_vp, _vp]),
     "nvwn_prime_slots_from_score": (C.c_int, [_vp, _vp, _vp, C.c_int, _vp, _vp]),
+    "nvwn_slot_state_bytes": (C.c_int, [_vp, _vp]),
+    "nvwn_save_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
+    "nvwn_load_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "nvwn_get_xt_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_skip_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_zs": (C.c_int, [_vp, _vp]),

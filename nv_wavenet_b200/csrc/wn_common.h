@@ -87,13 +87,18 @@ struct WnFamily {
     // as fp32 [(maxDil+1)][L][batch][R] (device), slot by slot, at that stride.
     cudaError_t (*put_history)(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream);
     cudaError_t (*get_history)(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream);
-    // Per-slot history writers (priming single slots, DESIGN.md §6), at the engine's batch stride, for absolute times t that may be
-    // negative, in ring slot ((t mod M) + M) mod M, M = maxDil + 1.  put_history_rows writes rows src_rows_dev[i] of fp16 src
-    // [n_t][src_batch][R] (device), the values x_layer[t] of times [t_first, t_first + n_t), n_t <= M, into ring rows rows_dev[i]
-    // (n distinct rows in [0, c.B)), and no other byte; clear_times zeroes rows 0..c.B-1 of every layer's entries of times
-    // [t_first, t_first + n_t), n_t <= M, and no other byte.
-    cudaError_t (*put_history_rows)(const WnConfig& c, void* ring, const __half* src, int src_batch, const int* src_rows_dev, const int* rows_dev,
-                                    int n, int layer, long long t_first, int n_t, cudaStream_t stream);
+    // Per-slot history writers and reader (priming single slots, parking and resuming them, DESIGN.md §6), at the engine's batch
+    // stride, for absolute times t that may be negative, in ring slot ((t mod M) + M) mod M, M = maxDil + 1.  A row's values are
+    // in the ring's element type (fp16 on NVWN_FP16 engines, else fp32) in device memory: the value of time t_first + j of source
+    // row i at element src_row(i) * row_pitch + j * time_pitch, src_row(i) = src_rows_dev[i] (src_rows_dev NULL: i); both pitches
+    // are multiples of 8 elements, and the base 16-byte aligned.  put_history_rows writes the values x_layer[t] of times [t_first,
+    // t_first + n_t), n_t <= M, into ring rows rows_dev[i] (n distinct rows in [0, c.B)), and no other byte; get_history_rows
+    // reads them back into dst at the same addresses, src_row(i) = i, writing zeros for the times before origin_dev[rows_dev[i]];
+    // clear_times zeroes rows 0..c.B-1 of every layer's entries of times [t_first, t_first + n_t), n_t <= M, and no other byte.
+    cudaError_t (*put_history_rows)(const WnConfig& c, void* ring, const void* src, const int* src_rows_dev, size_t row_pitch, size_t time_pitch,
+                                    const int* rows_dev, int n, int layer, long long t_first, int n_t, cudaStream_t stream);
+    cudaError_t (*get_history_rows)(const WnConfig& c, const void* ring, void* dst, size_t row_pitch, size_t time_pitch, const int* rows_dev, int n,
+                                    int layer, long long t_first, int n_t, const long long* origin_dev, cudaStream_t stream);
     cudaError_t (*clear_times)(const WnConfig& c, void* ring, long long t_first, int n_t, cudaStream_t stream);
     cudaError_t (*pack)(void* image, const WnParams& p, cudaStream_t stream);      // weight blob -> image; NULL: the kernels read the blob
     cudaError_t (*launch)(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info);
@@ -162,6 +167,16 @@ cudaError_t wn_feedback_from_codes(const int* codes, int n, int* yPrev, int* yCu
 // seed = seeds[i] (seeds NULL: 0)
 cudaError_t wn_prime_rows(const int* codes, const int* rows, const int* slots, int n, const unsigned long long* seeds, long long t_origin, int* yPrev,
                           int* yCur, long long* origin, unsigned long long* seed, cudaStream_t stream);
+// A saved slot state (nvwn_save_slots) starts with this header; wn_slot_state_bytes gives the whole blob
+static_assert(sizeof(nvwn_slot_state_header) == 64, "the slot state header is 64 bytes");
+size_t wn_slot_state_bytes(const WnConfig& c);
+// headers of the states at states + i * bytes for slots rows[i]: the engine's sizes, position next_t - origin[rows[i]], seed and
+// fed-back indices of the slot
+cudaError_t wn_save_slot_scalars(void* states, size_t bytes, const int* rows, int n, const WnConfig& c, long long next_t, const int* yPrev,
+                                 const int* yCur, const long long* origin, const unsigned long long* seed, cudaStream_t stream);
+// the reverse for a load at engine time t0: slot rows[i] takes state i's fed-back indices and seed, and origin t0 - position
+cudaError_t wn_load_slot_scalars(const void* states, size_t bytes, const int* rows, int n, long long t0, int* yPrev, int* yCur, long long* origin,
+                                 unsigned long long* seed, cudaStream_t stream);
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream);
 

@@ -193,6 +193,60 @@ cudaError_t wn_prime_rows(const int* codes, const int* rows, const int* slots, i
     return cudaGetLastError();
 }
 
+// the header, then per layer its d_l history rows of R elements of the ring's type
+size_t wn_slot_state_bytes(const WnConfig& c)
+{
+    size_t rows = 0;
+    for (int l = 0; l < c.L; l++) rows += (size_t)wn_score_dilation(l, c.maxDil);
+    return sizeof(nvwn_slot_state_header) + rows * c.R * (c.dtype == NVWN_FP16 ? sizeof(__half) : sizeof(float));
+}
+
+// Slot states (DESIGN.md §6): the scalar fields, next to the history rows the layout kernels move.  The position is computed here
+// from the slot's origin, so a save needs no host synchronisation.
+__global__ void save_slot_scalars_kernel(char* states, size_t bytes, const int* __restrict__ rows, int n, nvwn_slot_state_header h, long long next_t,
+                                         const int* __restrict__ yPrev, const int* __restrict__ yCur, const long long* __restrict__ origin,
+                                         const unsigned long long* __restrict__ seed)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int b = rows[i];
+        h.y_prev = yPrev[b];
+        h.y_cur = yCur[b];
+        h.position = next_t - origin[b];
+        h.seed = seed[b];
+        *reinterpret_cast<nvwn_slot_state_header*>(states + (size_t)i * bytes) = h;
+    }
+}
+cudaError_t wn_save_slot_scalars(void* states, size_t bytes, const int* rows, int n, const WnConfig& c, long long next_t, const int* yPrev,
+                                 const int* yCur, const long long* origin, const unsigned long long* seed, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    nvwn_slot_state_header h = {};
+    h.tag = NVWN_SLOT_STATE_TAG;
+    h.dtype = c.dtype; h.R = c.R; h.L = c.L; h.max_dilation = c.maxDil;
+    save_slot_scalars_kernel<<<(n + 255) / 256, 256, 0, stream>>>(static_cast<char*>(states), bytes, rows, n, h, next_t, yPrev, yCur, origin, seed);
+    return cudaGetLastError();
+}
+
+__global__ void load_slot_scalars_kernel(const char* states, size_t bytes, const int* __restrict__ rows, int n, long long t0, int* yPrev, int* yCur,
+                                         long long* origin, unsigned long long* seed)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int b = rows[i];
+        const nvwn_slot_state_header h = *reinterpret_cast<const nvwn_slot_state_header*>(states + (size_t)i * bytes);
+        yPrev[b] = h.y_prev;
+        yCur[b] = h.y_cur;
+        origin[b] = t0 - h.position;
+        seed[b] = h.seed;
+    }
+}
+cudaError_t wn_load_slot_scalars(const void* states, size_t bytes, const int* rows, int n, long long t0, int* yPrev, int* yCur, long long* origin,
+                                 unsigned long long* seed, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    load_slot_scalars_kernel<<<(n + 255) / 256, 256, 0, stream>>>(static_cast<const char*>(states), bytes, rows, n, t0, yPrev, yCur, origin, seed);
+    return cudaGetLastError();
+}
+
 cudaError_t wn_mulaw_decode(const int* yOut, int N, int offset, int size, int B, int A, const float* lut_f, const short* lut_s, float* out_f,
                             short* out_s, cudaStream_t stream)
 {

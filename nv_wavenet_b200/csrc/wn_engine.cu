@@ -86,6 +86,9 @@ struct DevBuf : std::unique_ptr<T, CudaFree> {
 // A live sequence of the whole-batch producer (nvwn_cond_producer_open_live) keeps row b's frames in a ring [C][ring] at
 // frames + b * ring * C, T[b] counting the frames pushed so far, and `produced` is the end of its furthest production: the
 // frames the samples from there on read may not be overwritten.
+// In live mode the per-slot producer (nvwn_cond_producer_open_live_slots) keeps slot s's frames in a ring [C][ring] at
+// frames + s * ring * C (cap = ring), and per slot whether a live utterance is attached, the first frame it was attached with
+// (the frames before it left the ring elsewhere) and the end of its furthest production, in its own samples.
 struct CondProducer {
     int C = 0, K = 0, stride = 0, rows = 0;
     int ring = 0;                            // frames per row of a live sequence's ring; 0: frames loaded whole
@@ -98,6 +101,9 @@ struct CondProducer {
     DevBuf<char> tables;                     // int [B] rows, then WnCondSlot [B] at cond_table_offset
     std::vector<int> T;
     std::vector<long long> start;
+    std::vector<char> live;
+    std::vector<int> first;
+    std::vector<long long> done;
 };
 
 }  // namespace
@@ -142,6 +148,9 @@ struct nvwn_engine : WnConfig {
     // entries of the negative times were zeroed in every row.
     DevBuf<int> prime_rows;
     bool early_prime = false;
+    // device staging of slot states in host memory (nvwn_save_slots, nvwn_load_slots), grown on demand
+    DevBuf<char> state_stage;
+    size_t state_stage_bytes = 0;
 
     DevBuf<void> image;                      // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
@@ -506,6 +515,53 @@ int put_fronts(const nvwn_engine* e, Write write)
     return 0;
 }
 
+// The earliest frame a live slot of the per-slot producer still holds: frames before `first` left the ring before the attach,
+// and a ring of P.ring frames holds [T - ring, T)
+long long live_held(const CondProducer& P, int s)
+{
+    const long long wrap = (long long)P.T[s] - P.ring;
+    return wrap > P.first[s] ? wrap : P.first[s];
+}
+
+// Frames [C][num] at src (host or device) -> frames T .. T + num - 1 of slot s's live ring, split at the wrap.  A host source is
+// snapshotted into pageable memory, which the copies stage before they return: the caller's array is free again on return.
+int put_live_frames(CondProducer& P, int s, long long T, const float* src, int num, cudaStream_t st)
+{
+    std::vector<float> snap;
+    if (!is_device_ptr(src)) {
+        snap.assign(src, src + (size_t)P.C * num);
+        src = snap.data();
+    }
+    const size_t f = sizeof(float);
+    for (const WrapPiece& w : split_at_wrap(T, num, P.ring))
+        CK(cudaMemcpy2DAsync(P.frames + (size_t)s * P.ring * P.C + w.pos, (size_t)P.ring * f, src + w.off, (size_t)num * f, (size_t)w.len * f, P.C,
+                             cudaMemcpyDefault, st));
+    return 0;
+}
+
+// Hands each layer's part of a slot state to part(layer, its byte offset in the state, d_l): [d_l][R] elements of the ring's type
+template <typename Part>
+int state_layers(const nvwn_engine* e, Part part)
+{
+    size_t off = sizeof(nvwn_slot_state_header);
+    for (int l = 0; l < e->L; l++) {
+        const int d = wn_score_dilation(l, e->maxDil);
+        CK(part(l, off, d));
+        off += (size_t)d * e->R * e->td;
+    }
+    return 0;
+}
+
+// The engine's staging buffer for slot states, at least `bytes` long
+int state_stage(nvwn_engine* e, size_t bytes)
+{
+    if (bytes <= e->state_stage_bytes) return 0;
+    if (e->state_stage) CK(cudaDeviceSynchronize());                        // no launch reads the old buffer any more
+    CK(e->state_stage.alloc(bytes));
+    e->state_stage_bytes = bytes;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -590,6 +646,9 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     for (CondProducer* P : {&e->cond_whole, &e->cond_slots}) {
         P->T.assign(Bz, 0);
         P->start.assign(Bz, 0);
+        P->live.assign(Bz, 0);
+        P->first.assign(Bz, 0);
+        P->done.assign(Bz, 0);
     }
     wn_fill_int(e->yPrev, 128, Bz, 0);
     wn_fill_int(e->yCur, 128, Bz, 0);
@@ -833,6 +892,8 @@ int nvwn_cond_producer_set_weights(nvwn_engine* e, int n_cond_channels, const fl
         P.frames.reset(); P.frames_floats = 0; P.cap = 0;
     }
     P.T.assign(e->B, 0);                                                      // frames attached under the old network are forgotten
+    P.live.assign(e->B, 0);                                                   // and live mode ends
+    P.ring = 0;
     const int rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
     if (rc != 0) return rc;
     const cudaError_t ce = cudaStreamSynchronize(st);                        // host sources may be released by the caller now
@@ -847,6 +908,9 @@ int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const 
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
     CondProducer& P = e->cond_slots;
     if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
+    if (P.ring)
+        return fail(NVWN_EINVAL, who + ": the per-slot producer is in live mode (nvwn_cond_producer_open_live_slots; nvwn_cond_producer_set_weights and "
+                                       "nvwn_reset_history end it)");
     int rc = check_slots(e, who, slots, n);
     if (rc != 0) return rc;
     if (!features || !num_frames || !starts) return fail(NVWN_EINVAL, who + ": features, num_frames or starts is NULL");
@@ -894,7 +958,7 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
 {
     const std::string who = "nvwn_cond_producer_run_slots";
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    const CondProducer& P = e->cond_slots;
+    CondProducer& P = e->cond_slots;
     if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
     int rc = check_slots(e, who, slots, n);
     if (rc == 0) rc = check_window(e, who, first_sample, num_samples, "num_samples", 0);
@@ -902,15 +966,31 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
     std::vector<WnCondSlot> tab(n);
     for (int i = 0; i < n; i++) {
         const int s = slots[i];
-        if (P.T[s] < 1)
-            return fail(NVWN_EINVAL, who + ": slot " + std::to_string(s) + " has no frames attached (nvwn_cond_producer_set_slots; nvwn_reset_history "
-                                           "and nvwn_cond_producer_set_weights forget them)");
+        if (P.ring ? !P.live[s] : P.T[s] < 1)
+            return fail(NVWN_EINVAL, who + ": slot " + std::to_string(s) +
+                                         (P.ring ? " has no live utterance attached (nvwn_cond_producer_attach_live)"
+                                                 : " has no frames attached (nvwn_cond_producer_set_slots; nvwn_reset_history and nvwn_cond_producer_set_weights "
+                                                   "forget them)"));
         if (first_sample < P.start[s])
             return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " is before the start " + std::to_string(P.start[s]) +
                                          " of slot " + std::to_string(s) + "'s utterance");
-        tab[i] = {(long long)s * P.cap * P.C, P.start[s], P.T[s], 0};
+        const long long n0 = first_sample - P.start[s];
+        if (P.ring && num_samples > 0 && n0 < (long long)P.T[s] * P.stride) {
+            // the range's first sample reads the earliest frames of the range: they must still be in the ring
+            const long long need = first_frame(n0, P.K, P.stride), held = live_held(P, s);
+            if (need < held)
+                return fail(NVWN_EINVAL, who + ": frame " + std::to_string(need) + ", which sample " + std::to_string(n0) + " of slot " + std::to_string(s) +
+                                             "'s utterance reads, has left the ring (it holds frames " + std::to_string(held) + " .. " +
+                                             std::to_string(P.T[s] - 1) + ")");
+        }
+        tab[i] = {(long long)s * P.cap * P.C, P.start[s], P.T[s], P.ring};
     }
     e->slot_rows_used = true;
+    if (P.ring && num_samples > 0)
+        for (int i = 0; i < n; i++) {
+            const long long end = first_sample + num_samples - P.start[slots[i]];
+            if (end > P.done[slots[i]]) P.done[slots[i]] = end;
+        }
     if (num_samples == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     // the slot list and the table in one copy, staged from pageable memory: the caller's arrays are free again on return
@@ -921,6 +1001,97 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
     CK(cudaMemcpyAsync(P.tables, host.data(), host.size(), cudaMemcpyHostToDevice, st));
     for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
         if ((rc = produce(e, P, who, slots, n, first_sample + w.off, w.pos, w.len, st))) return rc;
+    return 0;
+}
+
+int nvwn_cond_producer_open_live_slots(nvwn_engine* e, int ring_frames, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_open_live_slots";
+    (void)stream;                                                             // nothing is enqueued: the rings fill with the pushes
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    CondProducer& P = e->cond_slots;
+    if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
+    const int least = (P.K + P.stride - 1) / P.stride + 1;
+    if (ring_frames < least)
+        return fail(NVWN_EINVAL, who + ": ring_frames = " + std::to_string(ring_frames) + "; need at least ceil(window / stride) + 1 = " +
+                                     std::to_string(least));
+    const size_t n_ring = (size_t)e->B * P.C * ring_frames;
+    if (n_ring > P.frames_floats) {
+        if (P.frames) CK(cudaDeviceSynchronize());                          // no launch reads the old frames any more
+        CK(P.frames.alloc(n_ring * sizeof(float)));
+        P.frames_floats = n_ring;
+    }
+    P.cap = P.ring = ring_frames;
+    P.T.assign(e->B, 0);
+    P.live.assign(e->B, 0);
+    return 0;
+}
+
+int nvwn_cond_producer_attach_live(nvwn_engine* e, const int* slots, int n, const long long* starts, const int* first_frames,
+                                   const float* const* features, const int* num_frames, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_attach_live";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    CondProducer& P = e->cond_slots;
+    if (!P.ring) return fail(NVWN_EINVAL, who + ": the per-slot producer is not in live mode (nvwn_cond_producer_open_live_slots)");
+    int rc = check_slots(e, who, slots, n);
+    if (rc != 0) return rc;
+    if (!starts || !first_frames || !num_frames) return fail(NVWN_EINVAL, who + ": starts, first_frames or num_frames is NULL");
+    for (int i = 0; i < n; i++) {
+        const std::string u = "utterance " + std::to_string(i) + " (slot " + std::to_string(slots[i]) + ")";
+        if (first_frames[i] < 0 || num_frames[i] < 0 || num_frames[i] > P.ring)
+            return fail(NVWN_EINVAL, who + ": " + u + " has first_frames = " + std::to_string(first_frames[i]) + " and num_frames = " +
+                                         std::to_string(num_frames[i]) + "; need first_frames >= 0 and 0 <= num_frames <= ring_frames (" +
+                                         std::to_string(P.ring) + ")");
+        if (num_frames[i] > 0 && (!features || !features[i])) return fail(NVWN_EINVAL, who + ": the frames of " + u + " are NULL");
+        if (((long long)first_frames[i] + num_frames[i]) * P.stride > INT_MAX) return fail(NVWN_EINVAL, who + ": " + u + " has more than INT_MAX samples");
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int i = 0; i < n; i++)
+        if (num_frames[i] > 0 && (rc = put_live_frames(P, slots[i], first_frames[i], features[i], num_frames[i], st))) return rc;
+    for (int i = 0; i < n; i++) {
+        const int s = slots[i];
+        P.live[s] = 1;
+        P.first[s] = first_frames[i];
+        P.T[s] = first_frames[i] + num_frames[i];
+        P.start[s] = starts[i];
+        P.done[s] = 0;
+    }
+    e->slot_rows_used = true;
+    return 0;
+}
+
+int nvwn_cond_producer_push_slots(nvwn_engine* e, const int* slots, int n, const float* const* features, const int* num_frames, void* stream)
+{
+    const std::string who = "nvwn_cond_producer_push_slots";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    CondProducer& P = e->cond_slots;
+    if (!P.ring) return fail(NVWN_EINVAL, who + ": the per-slot producer is not in live mode (nvwn_cond_producer_open_live_slots)");
+    int rc = check_slots(e, who, slots, n);
+    if (rc != 0) return rc;
+    if (!features || !num_frames) return fail(NVWN_EINVAL, who + ": features or num_frames is NULL");
+    for (int i = 0; i < n; i++) {
+        const int s = slots[i];
+        const std::string u = "slot " + std::to_string(s);
+        if (!P.live[s]) return fail(NVWN_EINVAL, who + ": " + u + " has no live utterance attached (nvwn_cond_producer_attach_live)");
+        if (num_frames[i] < 0) return fail(NVWN_EINVAL, who + ": num_frames = " + std::to_string(num_frames[i]) + " < 0 for " + u);
+        if (num_frames[i] > 0 && !features[i]) return fail(NVWN_EINVAL, who + ": the frames of " + u + " are NULL");
+        const long long T1 = (long long)P.T[s] + num_frames[i];
+        if (T1 * P.stride > INT_MAX) return fail(NVWN_EINVAL, who + ": " + u + "'s utterance would hold more than INT_MAX samples");
+        // frames [T, T1) go where frames [T - ring, T1 - ring) were; the samples from `done` on read frames from first_frame(done),
+        // and the frames before `first` are gone already
+        const long long ff = first_frame(P.done[s], P.K, P.stride), keep = ff > P.first[s] ? ff : P.first[s];
+        if (T1 - P.ring > keep)
+            return fail(NVWN_EINVAL, who + ": " + std::to_string(num_frames[i]) + " frames would overwrite frame " + std::to_string(keep) + " of " + u +
+                                         ", which sample " + std::to_string(P.done[s]) + " (not produced yet) reads; at most " +
+                                         std::to_string(keep + P.ring - P.T[s]) + " frames fit before production moves on");
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int i = 0; i < n; i++) {
+        if (num_frames[i] == 0) continue;
+        if ((rc = put_live_frames(P, slots[i], P.T[slots[i]], features[i], num_frames[i], st))) return rc;
+        P.T[slots[i]] += num_frames[i];
+    }
     return 0;
 }
 
@@ -936,6 +1107,8 @@ int nvwn_reset_history(nvwn_engine* e)
     e->prime_bs = 0;
     e->early_prime = false;
     e->cond_slots.T.assign(e->B, 0);              // attached frames: their starts are absolute samples of the old timeline
+    e->cond_slots.live.assign(e->B, 0);           // and the per-slot producer's live mode ends
+    e->cond_slots.ring = 0;
     return 0;
 }
 
@@ -1424,11 +1597,96 @@ int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slot
     // time t0 - P + tau
     CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
     rc = put_fronts(e, [&](int l, const __half* src, long long tau, int n_t) {
-        return e->family->put_history_rows(*e, e->ring, src, Bs, e->prime_rows, e->slot_rows, n, l, origin + tau, n_t, st);
+        return e->family->put_history_rows(*e, e->ring, src, e->prime_rows, e->R, (size_t)Bs * e->R, e->slot_rows, n, l, origin + tau, n_t, st);
     });
     if (rc != 0) return rc;
     CK(wn_prime_rows(reinterpret_cast<const int*>(e->score_scratch + score_scratch_layout(e, e->score_T).codes), e->prime_rows, e->slot_rows, n, seeds_dev,
                      origin, e->yPrev, e->yCur, e->origin, e->seed, st));
+    return 0;
+}
+
+int nvwn_slot_state_bytes(nvwn_engine* e, unsigned long long* bytes)
+{
+    if (!e || !bytes) return fail(NVWN_EINVAL, "nvwn_slot_state_bytes: NULL argument");
+    *bytes = wn_slot_state_bytes(*e);
+    return 0;
+}
+
+int nvwn_save_slots(nvwn_engine* e, const int* slots, int n, void* states, void* stream)
+{
+    const std::string who = "nvwn_save_slots";
+    if (!e || !states) return fail(NVWN_EINVAL, who + ": NULL argument");
+    int rc = check_slots(e, who, slots, n);
+    if (rc != 0) return rc;
+    const bool host = !is_device_ptr(states);
+    if (!host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
+    const size_t bytes = wn_slot_state_bytes(*e);
+    if (host && (rc = state_stage(e, (size_t)n * bytes))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    char* dst = host ? e->state_stage.get() : static_cast<char*>(states);
+    // the slot list goes through the slot scratch, but this is no per-slot call: the engine does not change
+    if ((rc = copy_snapshot(e->slot_rows, slots, n, st))) return rc;
+    CK(wn_save_slot_scalars(dst, bytes, e->slot_rows, n, *e, e->next_t, e->yPrev, e->yCur, e->origin, e->seed, st));
+    rc = state_layers(e, [&](int l, size_t off, int d) {
+        return e->family->get_history_rows(*e, e->ring, dst + off, bytes / e->td, e->R, e->slot_rows, n, l, e->next_t - d, d, e->origin, st);
+    });
+    if (rc != 0) return rc;
+    if (host) {
+        CK(cudaMemcpyAsync(states, dst, (size_t)n * bytes, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    return 0;
+}
+
+int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states, void* stream)
+{
+    const std::string who = "nvwn_load_slots";
+    if (!e || !states) return fail(NVWN_EINVAL, who + ": NULL argument");
+    int rc = check_slots(e, who, slots, n);
+    if (rc != 0) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool host = !is_device_ptr(states);
+    if (!host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
+    const size_t bytes = wn_slot_state_bytes(*e), hb = sizeof(nvwn_slot_state_header);
+    // every header is checked before anything changes; device headers are read in stream order (the call runs at a window boundary)
+    std::vector<nvwn_slot_state_header> h(n);
+    if (host) {
+        for (int i = 0; i < n; i++) memcpy(&h[i], static_cast<const char*>(states) + (size_t)i * bytes, hb);
+    } else {
+        CK(cudaMemcpy2DAsync(h.data(), hb, states, bytes, hb, n, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    for (int i = 0; i < n; i++) {
+        const nvwn_slot_state_header& x = h[i];
+        const std::string s = "state " + std::to_string(i);
+        if (x.tag != NVWN_SLOT_STATE_TAG) return fail(NVWN_EINVAL, who + ": " + s + " is not a slot state (nvwn_save_slots)");
+        if (x.dtype != e->dtype || x.R != e->R || x.L != e->L || x.max_dilation != e->maxDil)
+            return fail(NVWN_EINVAL, who + ": " + s + " has dtype " + std::to_string(x.dtype) + ", R " + std::to_string(x.R) + ", L " + std::to_string(x.L) +
+                                         " and max_dilation " + std::to_string(x.max_dilation) + "; the engine has " + std::to_string(e->dtype) + ", " +
+                                         std::to_string(e->R) + ", " + std::to_string(e->L) + " and " + std::to_string(e->maxDil));
+        if (x.position < 0 || x.y_prev < 0 || x.y_prev >= e->A || x.y_cur < 0 || x.y_cur >= e->A)
+            return fail(NVWN_EINVAL, who + ": " + s + " has position " + std::to_string(x.position) + " and fed-back indices " + std::to_string(x.y_prev) +
+                                         ", " + std::to_string(x.y_cur) + "; need position >= 0 and indices in [0, " + std::to_string(e->A) + ")");
+    }
+    const char* src = static_cast<const char*>(states);
+    if (host) {
+        if ((rc = state_stage(e, (size_t)n * bytes)) || (rc = copy_snapshot(e->state_stage, src, (size_t)n * bytes, st))) return rc;
+        src = e->state_stage;
+    }
+    if ((rc = take_slots(e, who, slots, n, nullptr, nullptr, st))) return rc;
+    const long long t0 = e->next_t;
+    const int M = e->maxDil + 1;
+    if (t0 < e->maxDil && !e->early_prime) {
+        // as nvwn_prime_slots_from_score: the loaded rows hold real values at times the kernels would skip as "before the start"
+        CK(e->family->clear_times(*e, e->ring, t0 - M, (int)(M - t0), st));
+        e->early_prime = true;
+    }
+    CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
+    rc = state_layers(e, [&](int l, size_t off, int d) {
+        return e->family->put_history_rows(*e, e->ring, src + off, nullptr, bytes / e->td, e->R, e->slot_rows, n, l, t0 - d, d, st);
+    });
+    if (rc != 0) return rc;
+    CK(wn_load_slot_scalars(src, bytes, e->slot_rows, n, t0, e->yPrev, e->yCur, e->origin, e->seed, st));
     return 0;
 }
 

@@ -2027,5 +2027,5 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
 
 const WnFamily wn_lat_family = {LatLayout::store_bytes, LatLayout::ring_bytes, image_bytes, cond_convert, wn_readback<LatLayout>,
                                 wn_clear_rows<LatLayout>, wn_convert_rows<LatLayout>, wn_put_history<LatLayout>, wn_get_history<LatLayout>,
-                                wn_put_history_rows<LatLayout>, wn_clear_times<LatLayout>,
+                                wn_put_history_rows<LatLayout>, wn_get_history_rows<LatLayout>, wn_clear_times<LatLayout>,
                                 wn_lat_pack, wn_launch_lat, false};

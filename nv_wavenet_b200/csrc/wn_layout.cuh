@@ -124,20 +124,44 @@ __global__ void wn_put_history_kernel(size_t total, WnConfig c, void* ring, cons
 // ((t mod M) + M) mod M, M = maxDil + 1.  wn_put_history_kernel's t % M is only right for t >= 0.
 __device__ __forceinline__ int wn_ring_slot(long long t, int M) { return (int)((t % M + M) % M); }
 
-// fp16 rows src_rows[r] of a front src [n_t][src_batch][R] -> ring rows rows[r] of entries slot(t) * L + layer, t = t_first + j, at
-// the engine's batch stride
+// rows src_row(r) of src (the ring's type; src_rows NULL: row r) -> ring rows rows[r] of entries slot(t) * L + layer, t = t_first + j,
+// at the engine's batch stride; time j of source row q at element q * row_pitch + j * time_pitch
 template <class Lay>
-__global__ void wn_put_history_rows_kernel(size_t total, WnConfig c, void* ring, const __half* __restrict__ src, int src_batch,
-                                           const int* __restrict__ src_rows, const int* __restrict__ rows, int n, int layer, long long t_first)
+__global__ void wn_put_history_rows_kernel(size_t total, WnConfig c, void* ring, const void* __restrict__ src, const int* __restrict__ src_rows,
+                                           size_t row_pitch, size_t time_pitch, const int* __restrict__ rows, int n, int layer, long long t_first)
 {
     constexpr int U = Lay::RING_UNIT;
+    using TD = typename Lay::TD;
     const int units = c.R / U, lg = wn_log2(units);
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const size_t row = i >> lg;                                   // j * n + r
         const int r = (int)(row % n), k = (int)i & (units - 1);
         const size_t j = row / n;
+        const size_t q = src_rows ? (size_t)src_rows[r] : (size_t)r;
         *Lay::ring_unit(c, ring, (size_t)wn_ring_slot(t_first + (long long)j, c.maxDil + 1) * c.L + layer, c.B, rows[r], k) =
-            wn_vec_cast<typename Lay::TD>(wn_load(reinterpret_cast<const WnVec<__half, U>*>(src) + ((j * src_batch + src_rows[r]) << lg) + k));
+            wn_load(reinterpret_cast<const WnVec<TD, U>*>(static_cast<const TD*>(src) + q * row_pitch + j * time_pitch) + k);
+    }
+}
+
+// ring rows rows[r] of entries slot(t) * L + layer, t = t_first + j, at the engine's batch stride -> dst row r (the ring's type),
+// time j at element r * row_pitch + j * time_pitch; zeros for the times before origin[rows[r]], whose ring bytes may be stale
+template <class Lay>
+__global__ void wn_get_history_rows_kernel(size_t total, WnConfig c, const void* ring, void* __restrict__ dst, size_t row_pitch, size_t time_pitch,
+                                           const int* __restrict__ rows, int n, int layer, long long t_first, const long long* __restrict__ origin)
+{
+    constexpr int U = Lay::RING_UNIT;
+    using V = WnVec<typename Lay::TD, U>;
+    const int units = c.R / U, lg = wn_log2(units);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t row = i >> lg;                                   // j * n + r
+        const int r = (int)(row % n), k = (int)i & (units - 1);
+        const size_t j = row / n;
+        const long long t = t_first + (long long)j;
+        const int b = rows[r];
+        V v{};
+        if (t >= origin[b])
+            v = wn_load(Lay::ring_unit(c, const_cast<void*>(ring), (size_t)wn_ring_slot(t, c.maxDil + 1) * c.L + layer, c.B, b, k));
+        reinterpret_cast<V*>(static_cast<typename Lay::TD*>(dst) + r * row_pitch + j * time_pitch)[k] = v;
     }
 }
 
@@ -198,11 +222,18 @@ cudaError_t wn_put_history(const WnConfig& c, void* ring, const __half* src, int
     return wn_layout_launch(wn_put_history_kernel<Lay>, (size_t)n * batch * (c.R / Lay::RING_UNIT), stream, c, ring, src, layer, t_first, batch);
 }
 template <class Lay>
-cudaError_t wn_put_history_rows(const WnConfig& c, void* ring, const __half* src, int src_batch, const int* src_rows_dev, const int* rows_dev, int n,
-                                int layer, long long t_first, int n_t, cudaStream_t stream)
+cudaError_t wn_put_history_rows(const WnConfig& c, void* ring, const void* src, const int* src_rows_dev, size_t row_pitch, size_t time_pitch,
+                                const int* rows_dev, int n, int layer, long long t_first, int n_t, cudaStream_t stream)
 {
-    return wn_layout_launch(wn_put_history_rows_kernel<Lay>, (size_t)n_t * n * (c.R / Lay::RING_UNIT), stream, c, ring, src, src_batch, src_rows_dev,
-                            rows_dev, n, layer, t_first);
+    return wn_layout_launch(wn_put_history_rows_kernel<Lay>, (size_t)n_t * n * (c.R / Lay::RING_UNIT), stream, c, ring, src, src_rows_dev, row_pitch,
+                            time_pitch, rows_dev, n, layer, t_first);
+}
+template <class Lay>
+cudaError_t wn_get_history_rows(const WnConfig& c, const void* ring, void* dst, size_t row_pitch, size_t time_pitch, const int* rows_dev, int n,
+                                int layer, long long t_first, int n_t, const long long* origin_dev, cudaStream_t stream)
+{
+    return wn_layout_launch(wn_get_history_rows_kernel<Lay>, (size_t)n_t * n * (c.R / Lay::RING_UNIT), stream, c, ring, dst, row_pitch, time_pitch,
+                            rows_dev, n, layer, t_first, origin_dev);
 }
 template <class Lay>
 cudaError_t wn_clear_times(const WnConfig& c, void* ring, long long t_first, int n_t, cudaStream_t stream)

@@ -717,6 +717,22 @@ cudaError_t plain_get_history(const WnConfig& c, float* dst, const void* ring, i
 {
     return c.dtype == NVWN_FP16 ? wn_get_history<PlainH>(c, dst, ring, batch, stream) : wn_get_history<PlainF>(c, dst, ring, batch, stream);
 }
+cudaError_t plain_put_history_rows(const WnConfig& c, void* ring, const void* src, const int* src_rows_dev, size_t row_pitch, size_t time_pitch,
+                                   const int* rows_dev, int n, int layer, long long t_first, int n_t, cudaStream_t stream)
+{
+    return c.dtype == NVWN_FP16 ? wn_put_history_rows<PlainH>(c, ring, src, src_rows_dev, row_pitch, time_pitch, rows_dev, n, layer, t_first, n_t, stream)
+                                : wn_put_history_rows<PlainF>(c, ring, src, src_rows_dev, row_pitch, time_pitch, rows_dev, n, layer, t_first, n_t, stream);
+}
+cudaError_t plain_get_history_rows(const WnConfig& c, const void* ring, void* dst, size_t row_pitch, size_t time_pitch, const int* rows_dev, int n,
+                                   int layer, long long t_first, int n_t, const long long* origin_dev, cudaStream_t stream)
+{
+    return c.dtype == NVWN_FP16 ? wn_get_history_rows<PlainH>(c, ring, dst, row_pitch, time_pitch, rows_dev, n, layer, t_first, n_t, origin_dev, stream)
+                                : wn_get_history_rows<PlainF>(c, ring, dst, row_pitch, time_pitch, rows_dev, n, layer, t_first, n_t, origin_dev, stream);
+}
+cudaError_t plain_clear_times(const WnConfig& c, void* ring, long long t_first, int n_t, cudaStream_t stream)
+{
+    return c.dtype == NVWN_FP16 ? wn_clear_times<PlainH>(c, ring, t_first, n_t, stream) : wn_clear_times<PlainF>(c, ring, t_first, n_t, stream);
+}
 
 }  // namespace
 
@@ -728,7 +744,8 @@ bool wn_stream_supported(int R, int S, int A, bool)
 
 // The kernels read the weight blob and the plain conditioning store; any batch up to the engine's.  convert and readback are
 // contiguous conversions (wn_convert.cu): the plain store already is the source layout, and an fp32 convert also copies from host
-// memory, which no kernel can read.  put_history, put_history_rows and clear_times are fp16 only: the engine primes no other precision.
+// memory, which no kernel can read.  put_history is fp16 only: the engine primes no other precision.  The per-slot history
+// operations follow the engine's precision: fp32 engines park and resume slots too.
 const WnFamily wn_stream_family = {plain_store_bytes, plain_ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, plain_clear_rows,
-                                   plain_convert_rows, wn_put_history<PlainH>, plain_get_history, wn_put_history_rows<PlainH>, wn_clear_times<PlainH>,
-                                   nullptr, wn_launch_stream, false};
+                                   plain_convert_rows, wn_put_history<PlainH>, plain_get_history, plain_put_history_rows, plain_get_history_rows,
+                                   plain_clear_times, nullptr, wn_launch_stream, false};

@@ -683,5 +683,5 @@ bool wn_tc_supported(int R_, int S, int A_, int, int)
 // convert is convert_rows with every row: the whole-store and the per-row paths are one kernel
 const WnFamily wn_tc_family = {TcLayout::store_bytes, TcLayout::ring_bytes, image_bytes, wn_convert<TcLayout>, wn_readback<TcLayout>,
                                wn_clear_rows<TcLayout>, wn_convert_rows<TcLayout>, wn_put_history<TcLayout>, wn_get_history<TcLayout>,
-                               wn_put_history_rows<TcLayout>, wn_clear_times<TcLayout>, wn_tc_pack,
+                               wn_put_history_rows<TcLayout>, wn_get_history_rows<TcLayout>, wn_clear_times<TcLayout>, wn_tc_pack,
                                wn_launch_tc, true};

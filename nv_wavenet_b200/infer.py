@@ -312,8 +312,17 @@ class NVWavenetInfer:
         p, s = self._slots(slots)
         if len(features) != s.size or len(starts) != s.size:
             raise ValueError(f"cond_producer_set_slots: {s.size} slots, {len(features)} frame arrays and {len(starts)} starts")
-        keep, ptrs = [], (C.c_void_p * s.size)()
-        counts = np.empty(s.size, np.int32)
+        ptrs, counts, keep = self._frames("cond_producer_set_slots", features, stream)
+        st = np.ascontiguousarray([int(v) for v in starts], dtype=np.int64)
+        check(self._l.nvwn_cond_producer_set_slots(self._h, p, s.size, ptrs, C.c_void_p(counts.ctypes.data), C.c_void_p(st.ctypes.data),
+                                                   _stream(stream)), "condProducerSetSlots")
+        return keep
+
+    def _frames(self, what, features, stream):
+        """(float*[n], int32 counts [n], keepalive) of per-slot frames [C][T_i] (numpy arrays or torch tensors; None: no frames), C
+        that of cond_producer_set_weights."""
+        keep, ptrs = [], (C.c_void_p * max(1, len(features)))()
+        counts = np.zeros(len(features), np.int32)
         import contextlib
         on_stream = contextlib.nullcontext()
         if hasattr(stream, "cuda_stream"):                 # CUDA frames that need a contiguous fp32 copy get it on `stream`
@@ -321,16 +330,87 @@ class NVWavenetInfer:
             on_stream = torch.cuda.stream(stream)
         with on_stream:
             for i, f in enumerate(features):
+                if f is None:
+                    continue
                 shape = tuple(int(v) for v in f.shape)
                 if len(shape) != 2 or shape[0] != getattr(self, "_cond_channels", shape[0]):
-                    raise ValueError(f"cond_producer_set_slots: frames must be [C][T] with the C of cond_producer_set_weights; got {shape}")
+                    raise ValueError(f"{what}: frames must be [C][T] with the C of cond_producer_set_weights; got {shape}")
                 a, k = _ptr(f, np.float32)
                 ptrs[i], counts[i] = a, shape[1]
                 keep.append(k)
+        return ptrs, counts, keep
+
+    def cond_producer_open_live_slots(self, ring_frames, stream=None):
+        """Switches the per-slot producer to live mode: each slot's frames arrive over time into a ring of `ring_frames` frames
+        (cond_producer_attach_live, cond_producer_push_slots), and cond_producer_run_slots produces the samples they complete.
+        Forgets every attached utterance; cond_producer_set_weights and reset_history end live mode."""
+        check(self._l.nvwn_cond_producer_open_live_slots(self._h, int(ring_frames), _stream(stream)), "condProducerOpenLiveSlots")
+
+    def cond_producer_attach_live(self, slots, starts, first_frames=None, features=None, stream=None):
+        """Slot slots[i] takes a live utterance whose sample 0 is absolute sample starts[i] (negative for a resumed one), holding frames
+        features[i] [C][n_i] (None: none) as its frames first_frames[i] .. (None: all 0); frames before first_frames[i] count as
+        pushed.  Host frames may be reused on return; CUDA frames are copied in order on `stream`: keep what this returns alive."""
+        p, s = self._slots(slots)
+        features = [None] * s.size if features is None else list(features)
+        first = np.zeros(s.size, np.int32) if first_frames is None else np.ascontiguousarray([int(v) for v in first_frames], dtype=np.int32)
+        if len(features) != s.size or len(starts) != s.size or first.size != s.size:
+            raise ValueError(f"cond_producer_attach_live: {s.size} slots, {len(starts)} starts, {first.size} first frames and {len(features)} frame arrays")
+        ptrs, counts, keep = self._frames("cond_producer_attach_live", features, stream)
         st = np.ascontiguousarray([int(v) for v in starts], dtype=np.int64)
-        check(self._l.nvwn_cond_producer_set_slots(self._h, p, s.size, ptrs, C.c_void_p(counts.ctypes.data), C.c_void_p(st.ctypes.data),
-                                                   _stream(stream)), "condProducerSetSlots")
+        check(self._l.nvwn_cond_producer_attach_live(self._h, p, s.size, C.c_void_p(st.ctypes.data), C.c_void_p(first.ctypes.data), ptrs,
+                                                     C.c_void_p(counts.ctypes.data), _stream(stream)), "condProducerAttachLive")
         return keep
+
+    def cond_producer_push_slots(self, slots, features, stream=None):
+        """Appends features[i] [C][n_i] (numpy array or torch tensor) to slot slots[i]'s live utterance.  Host frames may be reused on
+        return; CUDA frames are copied in order on `stream`: keep what this returns alive until then."""
+        p, s = self._slots(slots)
+        if len(features) != s.size:
+            raise ValueError(f"cond_producer_push_slots: {s.size} slots but {len(features)} frame arrays")
+        ptrs, counts, keep = self._frames("cond_producer_push_slots", features, stream)
+        check(self._l.nvwn_cond_producer_push_slots(self._h, p, s.size, ptrs, C.c_void_p(counts.ctypes.data), _stream(stream)),
+              "condProducerPushSlots")
+        return keep
+
+    # ---- slot states: park a slot's utterance and resume it in any slot of a compatible engine (nvwn_save_slots) ----
+    def slot_state_bytes(self):
+        """Bytes of one slot state of this engine (nvwn_slot_state_bytes)."""
+        n = C.c_ulonglong()
+        check(self._l.nvwn_slot_state_bytes(self._h, C.byref(n)), "slotStateBytes")
+        return n.value
+
+    def save_slots(self, slots, out=None, stream=None):
+        """The states of `slots` at the engine's next sample, as a uint8 CUDA tensor [n][slot_state_bytes] written asynchronously on
+        `stream`, or into `out` (a uint8 CUDA tensor or numpy array of that size; a numpy array is complete on return).  The engine
+        does not change."""
+        p, s = self._slots(slots)
+        bytes_ = self.slot_state_bytes()
+        if out is None:
+            import torch
+            out = torch.empty((s.size, bytes_), dtype=torch.uint8, device="cuda")
+        size = out.size if isinstance(out, np.ndarray) else out.numel()
+        contiguous = out.flags["C_CONTIGUOUS"] if isinstance(out, np.ndarray) else out.is_contiguous()
+        if str(out.dtype) not in ("uint8", "torch.uint8") or size != s.size * bytes_ or not contiguous:
+            raise ValueError(f"save_slots: out must be contiguous uint8 [{s.size}][{bytes_}]; got {out.dtype} {tuple(out.shape)}")
+        ptr = out.ctypes.data if isinstance(out, np.ndarray) else out.data_ptr()
+        check(self._l.nvwn_save_slots(self._h, p, s.size, C.c_void_p(ptr), _stream(stream)), "saveSlots")
+        return out
+
+    def load_slots(self, slots, states, stream=None):
+        """Slot slots[i] continues state i of `states` (uint8 [n][slot_state_bytes], numpy array or CUDA tensor, as save_slots gives
+        them) from the engine's next sample.  A per-slot call; see nvwn_load_slots."""
+        p, s = self._slots(slots)
+        bytes_ = self.slot_state_bytes()
+        if isinstance(states, np.ndarray):
+            a = np.ascontiguousarray(states, dtype=np.uint8)
+            ptr, size = a.ctypes.data, a.size
+        else:
+            a = states.contiguous()
+            ptr, size = a.data_ptr(), a.numel() * a.element_size()
+        if size != s.size * bytes_:
+            raise ValueError(f"load_slots: {s.size} slots need {s.size} states of {bytes_} bytes; got {size} bytes")
+        check(self._l.nvwn_load_slots(self._h, p, s.size, C.c_void_p(ptr), _stream(stream)), "loadSlots")
+        return a
 
     def cond_producer_run_slots(self, slots, first_sample, num_samples, stream=None):
         """Conditioning of absolute samples [first_sample, first_sample + num_samples), num_samples <= N, for `slots` only, from

@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .infer import check_cond_network, live_push_limit, live_ring_frames
+from .infer import check_cond_network, live_frames, live_push_limit, live_ring_frames
 
 
 class Impl:
@@ -215,6 +215,206 @@ class LiveSession:
             self._eng = None
 
 
+def live_ready(position, frames, finished, window, stride):
+    """Whether a live stream can take a launch of `window` samples: its `frames` frames complete at least `window` samples past the
+    `position` it has generated, or it is finished and has samples left."""
+    return frames * stride - position >= window or (finished and frames * stride > position)
+
+
+def plan_live_step(resident, waiting, slots, window, stride):
+    """The slot decision of one LivePool.step, from the streams' counters alone.  resident: {id: (slot, position, frames, finished)}
+    of the streams in slots; waiting: [(id, position, frames, finished)] of the others, in the order they began to wait.  Resident
+    streams that are not ready (live_ready) are parked; ready waiting streams take the free slots (lowest first) in FIFO order.
+    Returns (parked ids, [(id, slot)] of the streams that take a slot)."""
+    park = [i for i, (_, p, f, fin) in resident.items() if not live_ready(p, f, fin, window, stride)]
+    held = {s for i, (s, _, _, _) in resident.items() if i not in park}
+    free = [s for s in range(slots) if s not in held]
+    place = []
+    for i, p, f, fin in waiting:
+        if free and live_ready(p, f, fin, window, stride):
+            place.append((i, free.pop(0)))
+    return park, place
+
+
+class _LiveStream:
+    """A LivePool stream's counters and its frames on the host: frames [base, base + held) of the `frames` given so far, `pushed` of
+    them in its slot's ring while it is resident, the samples it has generated (`position`), and its state while parked."""
+
+    def __init__(self, seed, channels):
+        self.seed, self.finished = seed, False
+        self.buf, self.base, self.frames = np.empty((channels, 64), np.float32), 0, 0
+        self.position, self.slot, self.pushed, self.state, self.started = 0, None, 0, None, False
+
+    def append(self, frames):
+        n = frames.shape[1]
+        held = self.frames - self.base
+        if held + n > self.buf.shape[1]:
+            grown = np.empty((self.buf.shape[0], max(2 * self.buf.shape[1], held + n)), np.float32)
+            grown[:, :held] = self.buf[:, :held]
+            self.buf = grown
+        self.buf[:, held:held + n] = frames
+        self.frames += n
+
+    def span(self, lo, hi):
+        """frames [lo, hi) as [C][hi - lo]"""
+        return self.buf[:, lo - self.base:hi - self.base]
+
+    def drop_before(self, lo):
+        """forgets the frames before lo"""
+        if lo > self.base:
+            held = self.frames - lo
+            self.buf[:, :held] = self.buf[:, lo - self.base:self.frames - self.base].copy()
+            self.base = lo
+
+
+class LivePool:
+    """Live serving: many live streams, each with its own mel frames arriving at its own pace, share one engine of `slots` rows and
+    `window` samples (NVWaveNet.open_live_pool).  push() only stores frames; each step() generates one window for the streams whose
+    frames complete it.  A stream whose frames are late is parked: its slot state is saved (nvwn_save_slots) and its slot given to a
+    stream that is ready; once its frames arrive it is loaded into any free slot (nvwn_load_slots) and goes on with the bits it
+    would have had without the pause.  So stream s's outputs, concatenated, equal infer() of its finished frames' conditioning with
+    its seed, bit for bit, however its frames were paced.  The pool owns its engine; close() releases it."""
+
+    device = "cuda"                 # where step() puts its samples
+
+    def __init__(self, eng, channels, upsample_window, stride, timed=False):
+        """eng: an engine whose per-slot producer has the conditioning network (cond_producer_set_weights); the pool opens its live
+        mode, with rings of live_ring_frames(N, upsample_window, stride) frames.  timed: record the GPU time of saves and loads."""
+        self._eng = eng
+        self.channels, self.upsample_window, self.stride, self.window = channels, upsample_window, stride, eng.N
+        self.ring_frames = live_ring_frames(self.window, upsample_window, stride)
+        eng.cond_producer_open_live_slots(self.ring_frames)
+        self.t = 0                                      # the engine's next sample
+        self.launches = self.parks = self.resumes = 0
+        self._streams, self._waiting, self._next_id = {}, [], 0
+        self._stage = None                              # yOut staging [B][N], allocated on the first launch
+        self._timed, self._save_ev, self._load_ev = timed, [], []
+
+    def open(self, seed):
+        """A new stream with selector key `seed`; returns its id.  It waits for frames."""
+        i = self._next_id
+        self._next_id += 1
+        self._streams[i] = _LiveStream(seed, self.channels)
+        self._waiting.append(i)
+        return i
+
+    def _stream(self, i):
+        if i not in self._streams:
+            raise AssertionError(f"no open stream {i}")
+        return self._streams[i]
+
+    def push(self, i, frames):
+        """Appends frames [C][n] (numpy array or torch tensor) to stream i.  Nothing is generated until step()."""
+        s = self._stream(i)
+        if s.finished:
+            raise AssertionError(f"push: stream {i} is finished")
+        shape = tuple(int(v) for v in frames.shape)
+        if len(shape) != 2 or shape[0] != self.channels:
+            raise AssertionError(f"push: frames must be [{self.channels}][n]; got {shape}")
+        s.append(frames.detach().to("cpu", torch.float32).numpy() if isinstance(frames, torch.Tensor) else np.asarray(frames, np.float32))
+
+    def finish(self, i):
+        """Stream i gets no more frames: step() generates the rest of its samples and then closes it."""
+        s = self._stream(i)
+        s.finished = True
+        if s.frames * self.stride == s.position:                              # nothing left to generate: its slot, if any, is free
+            if i in self._waiting:
+                self._waiting.remove(i)
+            del self._streams[i]
+
+    def _timed_call(self, events, fn, *args):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if self._timed else None
+        if ev:
+            ev[0].record()
+        out = fn(*args)
+        if ev:
+            ev[1].record()
+            events.append(ev)
+        return out
+
+    def state_seconds(self):
+        """GPU seconds spent saving and loading slot states so far (timed pools; synchronises)."""
+        torch.cuda.synchronize()
+        return tuple(sum(a.elapsed_time(b) for a, b in evs) / 1e3 for evs in (self._save_ev, self._load_ev))
+
+    def step(self, audio=None, saturate=False):
+        """One window at the engine's next sample: pushes each resident stream's pending frames (as many as its ring takes), parks the
+        resident streams that are not ready and gives the free slots to ready waiting streams (plan_live_step), and if any slot is
+        occupied generates `window` samples.  Returns {id: int32 CUDA tensor [k]} of the streams that advanced; with audio="float" or
+        "int16" returns (samples, audio), audio {id: numpy [k]} decoded as LiveSession.push decodes.  A finished stream that has all
+        its samples leaves the pool."""
+        if audio not in (None, "float", "int16"):
+            raise AssertionError(f"step: audio is None, 'float' or 'int16'; got {audio!r}")
+        eng, K, st = self._eng, self.upsample_window, self.stride
+        resident = {i: s for i, s in self._streams.items() if s.slot is not None}
+        push = [(i, s, min(s.frames - s.pushed, live_push_limit(s.pushed, s.position, self.ring_frames, K, st))) for i, s in resident.items()]
+        push = [(i, s, k) for i, s, k in push if k > 0]
+        if push:
+            eng.cond_producer_push_slots([s.slot for _, s, _ in push], [s.span(s.pushed, s.pushed + k) for _, s, k in push])
+            for _, s, k in push:
+                s.pushed += k
+        park, place = plan_live_step({i: (s.slot, s.position, s.frames, s.finished) for i, s in resident.items()},
+                                     [(i, self._streams[i].position, self._streams[i].frames, self._streams[i].finished) for i in self._waiting],
+                                     eng.B, self.window, st)
+        if park:
+            states = self._timed_call(self._save_ev, eng.save_slots, [resident[i].slot for i in park])
+            for j, i in enumerate(park):
+                s = resident.pop(i)
+                s.state, s.slot = states[j], None
+                self._waiting.append(i)
+            self.parks += len(park)
+        if place:
+            placed = {i for i, _ in place}
+            self._waiting = [i for i in self._waiting if i not in placed]
+            new = [(i, b) for i, b in place if not self._streams[i].started]
+            old = [(i, b) for i, b in place if self._streams[i].started]
+            if new:
+                eng.restart_slots([b for _, b in new], [self._streams[i].seed for i, _ in new])
+            if old:
+                self._timed_call(self._load_ev, eng.load_slots, [b for _, b in old], torch.stack([self._streams[i].state for i, _ in old]))
+                self.resumes += len(old)
+            spans = []
+            for i, b in place:
+                s = self._streams[i]
+                first = live_frames(s.position, 1, K, st)[0]
+                s.drop_before(first)
+                s.pushed = min(s.frames, first + self.ring_frames)
+                s.slot, s.state, s.started = b, None, True
+                spans.append(s.span(first, s.pushed))
+                resident[i] = s
+            eng.cond_producer_attach_live([b for _, b in place], [self.t - self._streams[i].position for i, _ in place],
+                                          [live_frames(self._streams[i].position, 1, K, st)[0] for i, _ in place], spans)
+        out, auds = {}, {}
+        if not resident:
+            return out if audio is None else (out, auds)
+        t, n = self.t, self.window
+        eng.cond_producer_run_slots([s.slot for s in resident.values()], t, n)
+        eng.set_selectors_random_slots(t, n)
+        eng.run_stream(t, n, eng.B)
+        self.launches += 1
+        self.t += n
+        pos = t % eng.N                                           # windows start at multiples of the window: no wrap inside
+        if self._stage is None:
+            self._stage = torch.empty((eng.B, eng.N), dtype=torch.int32, device=self.device)
+        eng.get_yout(self._stage, pos, n)
+        decoded = eng.get_audio(pos, n, int16=audio == "int16", saturate=saturate) if audio is not None else None
+        for i, s in resident.items():
+            k = min(n, s.frames * st - s.position)
+            out[i] = self._stage[s.slot, pos:pos + k].clone()
+            if decoded is not None:
+                auds[i] = decoded[s.slot, :k].copy()
+            s.position += k
+            s.drop_before(live_frames(s.position, 1, K, st)[0])   # a resume reads from the first frame its next sample reads
+            if s.finished and s.position == s.frames * st:        # all its samples delivered: the slot is free
+                del self._streams[i]
+        return out if audio is None else (out, auds)
+
+    def close(self):
+        if self._eng is not None:
+            self._eng.close()
+            self._eng = None
+
+
 class NVWaveNet:
     def __init__(self, embedding_prev, embedding_curr, conv_out_weight, conv_end_weight, dilate_weights, dilate_biases,
                  max_dilation, res_weights, res_biases, skip_weights, skip_biases, use_embed_tanh):
@@ -300,6 +500,21 @@ class NVWaveNet:
         eng.cond_producer_open_live(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride,
                                     live_ring_frames(window, up, stride))
         return LiveSession(eng, Cc, up, stride, seed, window)
+
+    def open_live_pool(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots, window, fp16=False, timed=False):
+        """Live serving: a LivePool whose streams, each with its own mel frames [C][n] arriving at its own pace, share one engine of
+        `slots` rows and `window` samples; `window` is also the samples per launch, so it trades latency against launches.  The
+        conditioning network is that of set_conditioning_from_features (upsample_weight [C][C][w], upsample_bias [C], cond_weight
+        [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]; numpy arrays or torch tensors).  Each stream's outputs, concatenated, equal
+        infer(cond, seed=seed, fp16=fp16) of its finished frames' conditioning (nvwn_cond_from_features_host), bit for bit.  The
+        pool has an engine of its own, apart from the engines infer() and the other calls share.  timed: see LivePool."""
+        Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
+                                    "open_live_pool")
+        if slots < 1 or window is None or window < 1:
+            raise AssertionError(f"open_live_pool: need slots >= 1 and window >= 1; got {slots}, {window}")
+        eng = self._new_engine(slots, window, fp16)
+        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride)
+        return LivePool(eng, Cc, up, stride, timed)
 
     def _cond_size(self, cond_input):
         """(batch, samples) of conditioning channels x batch x num_layers x samples."""
