@@ -288,6 +288,14 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Not in the reference class: the slot states of scoring rows rows[0..n) of the open scoring stream at its next sample P, for
+     * load_slots on any compatible engine.  See nvwn_score_save_states. */
+    bool score_save_states(const int* rows, int n, const unsigned long long* seeds, void* states, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_score_save_states(m_engine, rows, n, seeds, states, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
 
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)

@@ -304,6 +304,17 @@ int nvwn_save_slots(nvwn_engine* e, const int* slots, int n, void* states, void*
  * slot list, a header whose tag, dtype, R, L or max_dilation differs from the engine's, or whose position or indices are out of
  * range.  That the state was made with the same weights is the caller's responsibility: nothing in it records them. */
 int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states, void* stream);
+/* Prompted streams: the slot states of scored prompts.  With an open scoring stream of batch_size Bs and next sample P >= 1, writes
+ * state i for scoring row rows[i] to states + i * nvwn_slot_state_bytes (host or device memory, 16-byte aligned), in the format of
+ * nvwn_save_slots: dtype NVWN_FP16, position P, the row's codes of samples P - 2 and P - 1 as the fed-back indices, seed seeds[i]
+ * (seeds NULL: 0), zero reserved fields, then each layer's inputs x_l of times [P - d_l, P) from the scorer's fronts, zeros before
+ * time 0.  It is byte for byte the state nvwn_save_slots writes of a slot primed from that row by nvwn_prime_slots_from_score, so
+ * nvwn_load_slots resumes the prompt in any slot of any fp16 engine of the same R, L and maxDil, and no engine has to keep rows or
+ * store positions free for the scoring.  The scoring stream stays open and unchanged; nothing else changes.  Device states are
+ * written asynchronously on `stream`; host states are complete on return.  Refused, changing nothing: no open scoring stream,
+ * NULL arguments, n outside [1, Bs], rows outside [0, Bs) or given twice (NVWN_EINVAL); a packed stream (a row's fronts may hold
+ * an earlier utterance's inputs) or an engine that is not NVWN_FP16 (NVWN_EUNSUPPORTED). */
+int nvwn_score_save_states(nvwn_engine* e, const int* rows, int n, const unsigned long long* seeds, void* states, void* stream);
 
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);

@@ -68,6 +68,7 @@ SYMBOLS = {
     "nvwn_slot_state_bytes": (C.c_int, [_vp, _vp]),
     "nvwn_save_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "nvwn_load_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
+    "nvwn_score_save_states": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp]),
     "nvwn_get_xt_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_skip_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_zs": (C.c_int, [_vp, _vp]),

@@ -174,6 +174,11 @@ size_t wn_slot_state_bytes(const WnConfig& c);
 // fed-back indices of the slot
 cudaError_t wn_save_slot_scalars(void* states, size_t bytes, const int* rows, int n, const WnConfig& c, long long next_t, const int* yPrev,
                                  const int* yCur, const long long* origin, const unsigned long long* seed, cudaStream_t stream);
+// the states of scoring rows rows[0..n) of an open stream of next sample P, at states + i * bytes (nvwn_score_save_states): the
+// fp16 header of the engine's sizes with position P, codes[rows[i]] as the fed-back indices and seeds[i] (NULL: 0), then each
+// layer's front rows of rows[i], read from the scoring scratch's xh (chunk capacity Tcap, engine batch Be, stream batch Bs)
+cudaError_t wn_score_save_states(void* states, size_t bytes, const __half* xh, const int* codes, const int* rows, int n, const unsigned long long* seeds,
+                                 const WnConfig& c, long long P, int Tcap, int Be, int Bs, cudaStream_t stream);
 // the reverse for a load at engine time t0: slot rows[i] takes state i's fed-back indices and seed, and origin t0 - position
 cudaError_t wn_load_slot_scalars(const void* states, size_t bytes, const int* rows, int n, long long t0, int* yPrev, int* yCur, long long* origin,
                                  unsigned long long* seed, cudaStream_t stream);

@@ -227,6 +227,52 @@ cudaError_t wn_save_slot_scalars(void* states, size_t bytes, const int* rows, in
     return cudaGetLastError();
 }
 
+// Slot states of scoring rows (nvwn_score_save_states): block (x, i) writes parts of state i.  Its body is the concatenation over
+// layers of the fronts' rows of scoring row rows[i], [d_l][R] fp16 each, moved as 16-byte vectors; row g of the body is layer l's
+// front row g - (d_0 + .. + d_{l-1}), which sits at xh + wn_score_xh_offset(l) time-major [d_l][Bs][R] (the layers' buffers are
+// [d_l + Tcap][Be][R] apart, the rows inside at the scoring stream's batch Bs).  Block (0, i) also writes the
+// header: position P, the row's codes of steps P - 2 and P - 1, seeds[i] (seeds NULL: 0).
+__global__ void score_save_states_kernel(char* states, size_t bytes, const __half* __restrict__ xh, const int* __restrict__ codes,
+                                         const int* __restrict__ rows, const unsigned long long* __restrict__ seeds, nvwn_slot_state_header h,
+                                         int L, int R, int maxDil, int Tcap, int Be, int Bs, size_t vecs)
+{
+    const int i = blockIdx.y, row = rows[i];
+    char* st = states + (size_t)i * bytes;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        h.y_prev = codes[2 * row];
+        h.y_cur = codes[2 * row + 1];
+        h.seed = seeds ? seeds[i] : 0ull;
+        *reinterpret_cast<nvwn_slot_state_header*>(st) = h;
+    }
+    const int vpr = R * (int)sizeof(__half) / 16;                       // vectors per [R] row
+    uint4* body = reinterpret_cast<uint4*>(st + sizeof(nvwn_slot_state_header));
+    for (size_t v = (size_t)blockIdx.x * blockDim.x + threadIdx.x; v < vecs; v += (size_t)gridDim.x * blockDim.x) {
+        const int g = (int)(v / vpr), c = (int)(v % vpr);
+        int first = 0, d = 1;                                           // layer l's first body row and d_l
+        size_t off = 0;                                                 // wn_score_xh_offset(l)
+        for (int l = 0; l < L && g >= first + d; l++) {
+            off += ((size_t)d + Tcap) * Be * R;
+            first += d;
+            d = 2 * d > maxDil ? 1 : 2 * d;
+        }
+        body[v] = reinterpret_cast<const uint4*>(xh + off + ((size_t)(g - first) * Bs + row) * R)[c];
+    }
+}
+cudaError_t wn_score_save_states(void* states, size_t bytes, const __half* xh, const int* codes, const int* rows, int n, const unsigned long long* seeds,
+                                 const WnConfig& c, long long P, int Tcap, int Be, int Bs, cudaStream_t stream)
+{
+    if (n <= 0) return cudaSuccess;
+    nvwn_slot_state_header h = {};
+    h.tag = NVWN_SLOT_STATE_TAG;
+    h.dtype = NVWN_FP16; h.R = c.R; h.L = c.L; h.max_dilation = c.maxDil;
+    h.position = P;
+    const size_t vecs = (bytes - sizeof(nvwn_slot_state_header)) / 16;
+    const unsigned blocks = (unsigned)((vecs + 255) / 256 < 64 ? (vecs + 255) / 256 : 64);
+    score_save_states_kernel<<<dim3(blocks, (unsigned)n), 256, 0, stream>>>(static_cast<char*>(states), bytes, xh, codes, rows, seeds, h, c.L, c.R,
+                                                                            c.maxDil, Tcap, Be, Bs, vecs);
+    return cudaGetLastError();
+}
+
 __global__ void load_slot_scalars_kernel(const char* states, size_t bytes, const int* __restrict__ rows, int n, long long t0, int* yPrev, int* yCur,
                                          long long* origin, unsigned long long* seed)
 {

@@ -1638,6 +1638,44 @@ int nvwn_save_slots(nvwn_engine* e, const int* slots, int n, void* states, void*
     return 0;
 }
 
+int nvwn_score_save_states(nvwn_engine* e, const int* rows, int n, const unsigned long long* seeds, void* states, void* stream)
+{
+    const std::string who = "nvwn_score_save_states";
+    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score");
+    if (e->score_next < 1) return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one)");
+    if (e->score_packed)
+        return fail(NVWN_EUNSUPPORTED, who + ": the scoring stream is packed (nvwn_score_stream_packed): a row's layer fronts may hold an earlier "
+                                             "utterance's inputs, so they are no utterance's state");
+    if (!rows || !states) return fail(NVWN_EINVAL, who + ": NULL argument");
+    const int Bs = e->score_bs;
+    if (n < 1 || n > Bs) return fail(NVWN_EINVAL, who + ": n " + std::to_string(n) + " is outside [1, " + std::to_string(Bs) + "] (the scoring stream's batch_size)");
+    std::vector<char> seen(Bs, 0);
+    for (int i = 0; i < n; i++) {
+        if (rows[i] < 0 || rows[i] >= Bs)
+            return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is outside [0, " + std::to_string(Bs) + ") (the scoring stream's batch_size)");
+        if (seen[rows[i]]) return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is given twice");
+        seen[rows[i]] = 1;
+    }
+    const bool host = !is_device_ptr(states);
+    if (!host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
+    const size_t bytes = wn_slot_state_bytes(*e);
+    int rc;
+    if (host && (rc = state_stage(e, (size_t)n * bytes))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    char* dst = host ? e->state_stage.get() : static_cast<char*>(states);
+    // rows and seeds go through the per-call scratch of the primes; nothing else of the engine is touched
+    if ((rc = copy_snapshot(e->prime_rows, rows, n, st)) || (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st)))) return rc;
+    const ScoreScratch o = score_scratch_layout(e, e->score_T);
+    CK(wn_score_save_states(dst, bytes, reinterpret_cast<const __half*>(e->score_scratch + o.xh), reinterpret_cast<const int*>(e->score_scratch + o.codes),
+                            e->prime_rows, n, seeds ? e->slot_seeds.get() : nullptr, *e, e->score_next, e->score_T, e->B, Bs, st));
+    if (host) {
+        CK(cudaMemcpyAsync(states, dst, (size_t)n * bytes, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    return 0;
+}
+
 int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states, void* stream)
 {
     const std::string who = "nvwn_load_slots";

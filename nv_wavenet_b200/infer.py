@@ -384,17 +384,21 @@ class NVWavenetInfer:
         `stream`, or into `out` (a uint8 CUDA tensor or numpy array of that size; a numpy array is complete on return).  The engine
         does not change."""
         p, s = self._slots(slots)
+        out, ptr = self._states_out("save_slots", s.size, out)
+        check(self._l.nvwn_save_slots(self._h, p, s.size, C.c_void_p(ptr), _stream(stream)), "saveSlots")
+        return out
+
+    def _states_out(self, what, n, out):
+        """(out, its address) for n slot states: `out` checked as contiguous uint8 [n][slot_state_bytes], or a new CUDA tensor."""
         bytes_ = self.slot_state_bytes()
         if out is None:
             import torch
-            out = torch.empty((s.size, bytes_), dtype=torch.uint8, device="cuda")
+            out = torch.empty((n, bytes_), dtype=torch.uint8, device="cuda")
         size = out.size if isinstance(out, np.ndarray) else out.numel()
         contiguous = out.flags["C_CONTIGUOUS"] if isinstance(out, np.ndarray) else out.is_contiguous()
-        if str(out.dtype) not in ("uint8", "torch.uint8") or size != s.size * bytes_ or not contiguous:
-            raise ValueError(f"save_slots: out must be contiguous uint8 [{s.size}][{bytes_}]; got {out.dtype} {tuple(out.shape)}")
-        ptr = out.ctypes.data if isinstance(out, np.ndarray) else out.data_ptr()
-        check(self._l.nvwn_save_slots(self._h, p, s.size, C.c_void_p(ptr), _stream(stream)), "saveSlots")
-        return out
+        if str(out.dtype) not in ("uint8", "torch.uint8") or size != n * bytes_ or not contiguous:
+            raise ValueError(f"{what}: out must be contiguous uint8 [{n}][{bytes_}]; got {out.dtype} {tuple(out.shape)}")
+        return out, out.ctypes.data if isinstance(out, np.ndarray) else out.data_ptr()
 
     def load_slots(self, slots, states, stream=None):
         """Slot slots[i] continues state i of `states` (uint8 [n][slot_state_bytes], numpy array or CUDA tensor, as save_slots gives
@@ -522,6 +526,18 @@ class NVWavenetInfer:
             raise ValueError(f"prime_slots_from_score: {s.size} slots but {r.size} rows")
         k, keep = self._seeds("prime_slots_from_score", seeds, s.size)
         check(self._l.nvwn_prime_slots_from_score(self._h, C.c_void_p(r.ctypes.data), p, s.size, k, _stream(stream)), "primeSlotsFromScore")
+
+    def score_save_states(self, rows, seeds=None, out=None, stream=None):
+        """After score_stream over prompts [0, P): the slot states of scoring rows `rows` at P, as a uint8 CUDA tensor
+        [n][slot_state_bytes] written asynchronously on `stream`, or into `out` as for save_slots; seeds (one per row, None = 0) are
+        the states' selector keys.  load_slots resumes them in any slot of a compatible engine.  The scoring stream stays open; see
+        nvwn_score_save_states."""
+        r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1)).astype(np.int32)
+        k, keep = self._seeds("score_save_states", seeds, r.size)
+        out, ptr = self._states_out("score_save_states", r.size, out)
+        check(self._l.nvwn_score_save_states(self._h, C.c_void_p(r.ctypes.data), r.size, k, C.c_void_p(ptr), _stream(stream)),
+              "scoreSaveStates")
+        return out
 
     def _score(self, audio, num_samples, batch_size, logits, what, call):
         """audio[:batch_size, :num_samples] as int32 and the outputs of score() in matching memory; call(audio, n, bs, logp, logits)

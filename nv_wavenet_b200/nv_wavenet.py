@@ -157,19 +157,51 @@ def _check_window(window):
         raise AssertionError(f"window must be at least 1; got {window}")
 
 
+def check_prompt(what, prompt, rows, n, fp16, A):
+    """Checks a prompt: int mu-law codes [P] (rows None) or [rows][P], 1 <= P < n (n None: no upper bound), each in [0, A), with
+    fp16 set, since prompts are scored by the fp16 scorer.  Returns it as a tensor."""
+    p = torch.as_tensor(prompt)
+    lead = () if rows is None else (rows,)
+    shape = tuple(p.shape)
+    if len(shape) != len(lead) + 1 or shape[:-1] != lead or not 1 <= shape[-1] or (n is not None and shape[-1] >= n):
+        bound = "1 <= P" if n is None else f"1 <= P < {n}"
+        raise AssertionError(f"{what} must be {''.join(f'[{r}]' for r in lead)}[P] with {bound}; got {shape}")
+    if p.dtype.is_floating_point or p.dtype.is_complex or p.dtype == torch.bool:
+        raise AssertionError(f"{what} must hold integer mu-law codes; got {p.dtype}")
+    if int(p.min()) < 0 or int(p.max()) >= A:
+        raise AssertionError(f"{what} holds codes outside [0, {A})")
+    if not fp16:
+        raise AssertionError(f"{what} needs fp16=True: prompts are scored by the fp16 scorer")
+    return p
+
+
+def prompt_frames(P, stride):
+    """The frames a prompt of P samples needs before it can be scored: samples [0, P) read frames up to floor((P - 1) / stride)."""
+    return (P - 1) // stride + 1
+
+
+def plan_prompt_groups(prompted, rows):
+    """The scoring streams of one LivePool.step: the streams in `prompted` [(id, P)], in order, in groups of at most `rows` (the
+    scoring engine's rows), each group's rows by prompt length.  Returns [[(id, P)] per group]; row j of a group is its j-th entry."""
+    return [sorted(prompted[k:k + rows], key=lambda x: x[1]) for k in range(0, len(prompted), rows)]
+
+
 class LiveSession:
     """Live vocoding of one batch of utterances whose mel frames arrive over time (NVWaveNet.open_live): each push appends frames
     and generates every sample they complete, so audio starts with the first frames and an open-ended stream can be vocoded.
-    The session owns its engine of `window` samples; close() releases it."""
+    The session owns its engine of `window` samples; close() releases it.
+    With a prompt [batch][P] (int32 CUDA codes), the frames' first P samples are not generated: as the pushes complete them they
+    are scored on the session's engine (nvwn_score_stream), which then continues the prompt from sample P (nvwn_prime_from_score)."""
 
     device = "cuda"                 # where push() puts its samples
 
-    def __init__(self, eng, channels, upsample_window, stride, seed, window):
+    def __init__(self, eng, channels, upsample_window, stride, seed, window, prompt=None):
         self._eng = eng
         self.channels, self.upsample_window, self.stride, self.seed, self.window = channels, upsample_window, stride, seed, window
         self.ring_frames = live_ring_frames(window, upsample_window, stride)
+        self.prompt = prompt
         self.frames = 0             # frames pushed so far
-        self.samples = 0            # samples generated so far: every sample the frames complete, [0, frames * stride)
+        self.samples = 0            # samples scored or generated so far: every sample the frames complete, [0, frames * stride)
 
     def push(self, frames, audio=None, saturate=False):
         """Appends frames [batch][C][n] (numpy array or torch tensor, n >= 0) and generates samples [samples, (frames + n) * stride),
@@ -177,7 +209,8 @@ class LiveSession:
         the ring cannot take at once are fed in pieces, each generated before the next is pushed.  Returns those samples as an
         int32 CUDA tensor [batch][k]; with audio="float" or "int16" returns (samples, audio), audio the mu-law decoded samples
         [batch][k] as a numpy array (get_audio_stream; saturate as for get_audio).  Together the pushes give infer() of the finished
-        utterance with the same seed and window, bit for bit."""
+        utterance with the same seed and window, bit for bit.  With a prompt of P samples, samples before P are scored instead and
+        not returned: the pushes give infer(prompt=prompt)[:, P:]."""
         if audio not in (None, "float", "int16"):
             raise AssertionError(f"push: audio is None, 'float' or 'int16'; got {audio!r}")
         shape = tuple(int(v) for v in frames.shape)
@@ -193,8 +226,17 @@ class LiveSession:
                 self.frames += k
                 done += k
             end = self.frames * self.stride
+            P = 0 if self.prompt is None else self.prompt.shape[1]
             while self.samples < end:
                 first, m = self.samples, min(self.window, end - self.samples)
+                if first < P:
+                    m = min(m, P - first)
+                    eng.cond_producer_run_stream(first, m)
+                    eng.score_stream(self.prompt[:, first:first + m], first)
+                    self.samples += m
+                    if self.samples == P:
+                        eng.prime_from_score()
+                    continue
                 eng.cond_producer_run_stream(first, m)
                 eng.set_selectors_random_stream(self.seed, first, m)
                 eng.run_stream(first, m, eng.B)
@@ -240,8 +282,8 @@ class _LiveStream:
     """A LivePool stream's counters and its frames on the host: frames [base, base + held) of the `frames` given so far, `pushed` of
     them in its slot's ring while it is resident, the samples it has generated (`position`), and its state while parked."""
 
-    def __init__(self, seed, channels):
-        self.seed, self.finished = seed, False
+    def __init__(self, seed, channels, prompt=None):
+        self.seed, self.finished, self.prompt = seed, False, prompt          # prompt: int32 CUDA [P] until it is scored, then None
         self.buf, self.base, self.frames = np.empty((channels, 64), np.float32), 0, 0
         self.position, self.slot, self.pushed, self.state, self.started = 0, None, 0, None, False
 
@@ -273,14 +315,21 @@ class LivePool:
     frames complete it.  A stream whose frames are late is parked: its slot state is saved (nvwn_save_slots) and its slot given to a
     stream that is ready; once its frames arrive it is loaded into any free slot (nvwn_load_slots) and goes on with the bits it
     would have had without the pause.  So stream s's outputs, concatenated, equal infer() of its finished frames' conditioning with
-    its seed, bit for bit, however its frames were paced.  The pool owns its engine; close() releases it."""
+    its seed, bit for bit, however its frames were paced.  The pool owns its engine; close() releases it.
+    A stream opened with a prompt continues given audio: once its frames cover the prompt, the prompt is scored on a scoring engine
+    the pool owns and its state saved there (nvwn_score_save_states); the stream then waits as a parked stream at position P and is
+    resumed like one.  Its outputs are infer(cond, seed=seed, fp16=True, prompt=prompt)[0, P:], bit for bit."""
 
     device = "cuda"                 # where step() puts its samples
 
-    def __init__(self, eng, channels, upsample_window, stride, timed=False):
+    def __init__(self, eng, channels, upsample_window, stride, timed=False, scorer=None, network=None):
         """eng: an engine whose per-slot producer has the conditioning network (cond_producer_set_weights); the pool opens its live
-        mode, with rings of live_ring_frames(N, upsample_window, stride) frames.  timed: record the GPU time of saves and loads."""
+        mode, with rings of live_ring_frames(N, upsample_window, stride) frames.  timed: record the GPU time of saves, loads and
+        prompt scoring.  scorer: None (no prompts), or a callable that makes the pool's scoring engine, an fp16 engine with eng's
+        weights, called when the first prompt is scored; network: the conditioning network (upsample_weight, upsample_bias,
+        cond_weight [L*2R][C], cond_bias) for its whole-batch producer."""
         self._eng = eng
+        self._scorer, self._scorer_eng, self._network = scorer, None, network
         self.channels, self.upsample_window, self.stride, self.window = channels, upsample_window, stride, eng.N
         self.ring_frames = live_ring_frames(self.window, upsample_window, stride)
         eng.cond_producer_open_live_slots(self.ring_frames)
@@ -288,13 +337,20 @@ class LivePool:
         self.launches = self.parks = self.resumes = 0
         self._streams, self._waiting, self._next_id = {}, [], 0
         self._stage = None                              # yOut staging [B][N], allocated on the first launch
-        self._timed, self._save_ev, self._load_ev = timed, [], []
+        self._timed, self._save_ev, self._load_ev, self._prompt_ev = timed, [], [], []
 
-    def open(self, seed):
-        """A new stream with selector key `seed`; returns its id.  It waits for frames."""
+    def open(self, seed, prompt=None):
+        """A new stream with selector key `seed`; returns its id.  It waits for frames.  prompt: None, or int mu-law codes [P], P >= 1
+        (host or CUDA tensor), on fp16 pools only: the stream continues given audio, its first output being sample P.  It is scored
+        in the step() after its frames cover samples [0, P), and generates from there."""
+        if prompt is not None:
+            prompt = check_prompt("prompt", prompt, None, None, self._eng.dtype == _lib.FP16, self._eng.A)
+            if self._scorer is None:
+                raise AssertionError("open: this pool has no scoring engine for prompts (NVWaveNet.open_live_pool makes one)")
+            prompt = prompt.to(device=self.device, dtype=torch.int32)
         i = self._next_id
         self._next_id += 1
-        self._streams[i] = _LiveStream(seed, self.channels)
+        self._streams[i] = _LiveStream(seed, self.channels, prompt)
         self._waiting.append(i)
         return i
 
@@ -317,7 +373,8 @@ class LivePool:
         """Stream i gets no more frames: step() generates the rest of its samples and then closes it."""
         s = self._stream(i)
         s.finished = True
-        if s.frames * self.stride == s.position:                              # nothing left to generate: its slot, if any, is free
+        if s.prompt is None and s.frames * self.stride == s.position or s.prompt is not None and s.frames * self.stride < s.prompt.numel():
+            # nothing left to generate, or a prompt its frames never cover: its slot, if any, is free
             if i in self._waiting:
                 self._waiting.remove(i)
             del self._streams[i]
@@ -337,9 +394,64 @@ class LivePool:
         torch.cuda.synchronize()
         return tuple(sum(a.elapsed_time(b) for a, b in evs) / 1e3 for evs in (self._save_ev, self._load_ev))
 
+    def prompt_seconds(self):
+        """GPU seconds spent producing, scoring and saving prompts so far (timed pools; synchronises)."""
+        torch.cuda.synchronize()
+        return sum(a.elapsed_time(b) for a, b in self._prompt_ev) / 1e3
+
+    def _score_prompts(self):
+        """Scores the waiting streams whose frames now cover their prompts, in groups of the scoring engine's rows
+        (plan_prompt_groups); each becomes a parked stream at position P with the state its scoring row left."""
+        st = self.stride
+        ready = [(i, self._streams[i].prompt.numel()) for i in self._waiting
+                 if self._streams[i].prompt is not None and self._streams[i].frames >= prompt_frames(self._streams[i].prompt.numel(), st)]
+        if not ready:
+            return
+        if self._scorer_eng is None:
+            self._scorer_eng = self._scorer()
+            # on the device once, so a group's producer load copies no weights from the host
+            self._network = tuple(torch.as_tensor(a).to(device=self.device, dtype=torch.float32).contiguous() for a in self._network)
+        for group in plan_prompt_groups(ready, self._scorer_eng.B):
+            states = self._timed_call(self._prompt_ev, self._score_group, group)
+            for (i, P), state in zip(group, states):
+                s = self._streams[i]
+                s.state, s.position, s.started, s.prompt = state, P, True, None
+                if s.finished and s.frames * st == P:                        # a prompt and nothing after it
+                    self._waiting.remove(i)
+                    del self._streams[i]
+
+    def _score_group(self, group):
+        """One scoring stream on the scoring engine: row j is group[j] = (id, P_j), rows by P.  Its conditioning comes from the
+        rows' frames through the whole-batch producer; it is scored in pieces that end at each distinct P_j and at multiples of
+        the window, rows past their prompt's end on code 128 (their results unused), and each row's state is saved where its prompt
+        ends (nvwn_score_save_states, with the stream's seed).  Returns the states in group order."""
+        eng, W = self._scorer_eng, self._scorer_eng.N
+        P_max = group[-1][1]
+        F = prompt_frames(P_max, self.stride)
+        feats = np.zeros((eng.B, self.channels, F), np.float32)
+        codes = torch.full((len(group), P_max), 128, dtype=torch.int32, device=self.device)
+        for j, (i, P) in enumerate(group):
+            s = self._streams[i]
+            n = min(s.frames, F)
+            feats[j, :, :n] = s.span(0, n)
+            codes[j, :P] = s.prompt
+        eng.cond_producer_load(feats, *self._network, self.stride)
+        states, a = [None] * len(group), 0
+        for end in sorted({P for _, P in group}):
+            while a < end:
+                m = min(end - a, W - a % W)
+                eng.cond_producer_run_stream(a, m)
+                eng.score_stream(codes[:, a:a + m], a)
+                a += m
+            done = [j for j, (_, P) in enumerate(group) if P == end]
+            saved = eng.score_save_states(done, [self._streams[group[j][0]].seed for j in done])
+            for k, j in enumerate(done):
+                states[j] = saved[k]
+        return states
+
     def step(self, audio=None, saturate=False):
-        """One window at the engine's next sample: pushes each resident stream's pending frames (as many as its ring takes), parks the
-        resident streams that are not ready and gives the free slots to ready waiting streams (plan_live_step), and if any slot is
+        """One window at the engine's next sample: pushes each resident stream's pending frames (as many as its ring takes), scores the
+        prompts whose frames are in (_score_prompts), parks the resident streams that are not ready and gives the free slots to ready waiting streams (plan_live_step), and if any slot is
         occupied generates `window` samples.  Returns {id: int32 CUDA tensor [k]} of the streams that advanced; with audio="float" or
         "int16" returns (samples, audio), audio {id: numpy [k]} decoded as LiveSession.push decodes.  A finished stream that has all
         its samples leaves the pool."""
@@ -353,8 +465,10 @@ class LivePool:
             eng.cond_producer_push_slots([s.slot for _, s, _ in push], [s.span(s.pushed, s.pushed + k) for _, s, k in push])
             for _, s, k in push:
                 s.pushed += k
+        self._score_prompts()
         park, place = plan_live_step({i: (s.slot, s.position, s.frames, s.finished) for i, s in resident.items()},
-                                     [(i, self._streams[i].position, self._streams[i].frames, self._streams[i].finished) for i in self._waiting],
+                                     [(i, self._streams[i].position, self._streams[i].frames, self._streams[i].finished) for i in self._waiting
+                                      if self._streams[i].prompt is None],
                                      eng.B, self.window, st)
         if park:
             states = self._timed_call(self._save_ev, eng.save_slots, [resident[i].slot for i in park])
@@ -410,9 +524,10 @@ class LivePool:
         return out if audio is None else (out, auds)
 
     def close(self):
-        if self._eng is not None:
-            self._eng.close()
-            self._eng = None
+        for e in (self._eng, self._scorer_eng):
+            if e is not None:
+                e.close()
+        self._eng = self._scorer_eng = None
 
 
 class NVWaveNet:
@@ -484,22 +599,27 @@ class NVWaveNet:
         eng.set_out_weights(f32(self.conv_out), zero, f32(self.conv_end), zero)
         return eng
 
-    def open_live(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, batch_size, seed, window=4096, fp16=False):
+    def open_live(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, batch_size, seed, window=4096, fp16=False, prompt=None):
         """Live vocoding: a LiveSession that generates `batch_size` utterances while their mel frames [batch][C][n] are still
         arriving (LiveSession.push).  The conditioning network is that of set_conditioning_from_features (upsample_weight [C][C][w],
         upsample_bias [C], cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]; numpy arrays or torch tensors); the frames go
         into a ring on the device of live_ring_frames(window, w, stride) frames per utterance.  Selectors are Philox under `seed`,
         drawn by absolute sample, so the pushes together give infer(cond, seed=seed, fp16=fp16, window=window) of the finished
         frames' conditioning (nvwn_cond_from_features_host), bit for bit.  The session has an engine of its own, apart from the
-        engines infer() and the other calls share."""
+        engines infer() and the other calls share.
+        prompt: None, or int mu-law codes [batch_size][P], P >= 1 (host or CUDA tensor), fp16 only: the utterances continue given
+        audio.  The pushes then give infer(cond, seed=seed, fp16=True, window=window, prompt=prompt)[:, P:], bit for bit: the
+        frames' first P samples are scored as they arrive, and generation starts at sample P once they all are."""
         Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
                                     "open_live")
         if batch_size < 1 or window is None or window < 1:
             raise AssertionError(f"open_live: need batch_size >= 1 and window >= 1; got {batch_size}, {window}")
+        if prompt is not None:
+            prompt = self._check_prompt("prompt", prompt, batch_size, None, fp16).to(device="cuda", dtype=torch.int32)
         eng = self._new_engine(batch_size, window, fp16)
         eng.cond_producer_open_live(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride,
                                     live_ring_frames(window, up, stride))
-        return LiveSession(eng, Cc, up, stride, seed, window)
+        return LiveSession(eng, Cc, up, stride, seed, window, prompt)
 
     def open_live_pool(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots, window, fp16=False, timed=False):
         """Live serving: a LivePool whose streams, each with its own mel frames [C][n] arriving at its own pace, share one engine of
@@ -507,14 +627,18 @@ class NVWaveNet:
         conditioning network is that of set_conditioning_from_features (upsample_weight [C][C][w], upsample_bias [C], cond_weight
         [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]; numpy arrays or torch tensors).  Each stream's outputs, concatenated, equal
         infer(cond, seed=seed, fp16=fp16) of its finished frames' conditioning (nvwn_cond_from_features_host), bit for bit.  The
-        pool has an engine of its own, apart from the engines infer() and the other calls share.  timed: see LivePool."""
+        pool has an engine of its own, apart from the engines infer() and the other calls share.  timed: see LivePool.
+        On fp16 pools LivePool.open takes a prompt; the pool then makes, on the first prompt, a scoring engine of `slots` rows and
+        `window` samples with the same weights."""
         Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
                                     "open_live_pool")
         if slots < 1 or window is None or window < 1:
             raise AssertionError(f"open_live_pool: need slots >= 1 and window >= 1; got {slots}, {window}")
         eng = self._new_engine(slots, window, fp16)
-        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride)
-        return LivePool(eng, Cc, up, stride, timed)
+        cw = cond_weight.reshape(self.num_layers * 2 * self.R, Cc)
+        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cw, cond_bias, stride)
+        scorer = (lambda: self._new_engine(slots, window, True)) if fp16 else None
+        return LivePool(eng, Cc, up, stride, timed, scorer, (upsample_weight, upsample_bias, cw, cond_bias))
 
     def _cond_size(self, cond_input):
         """(batch, samples) of conditioning channels x batch x num_layers x samples."""
@@ -523,20 +647,7 @@ class NVWaveNet:
         return cond_input.size(1), cond_input.size(3)
 
     def _check_prompt(self, what, prompt, rows, n, fp16):
-        """Checks a prompt: int mu-law codes [P] (rows None) or [rows][P], 1 <= P < n, each in [0, A), with fp16 set, since prompts
-        are scored by the fp16 scorer.  Returns it as a tensor."""
-        p = torch.as_tensor(prompt)
-        lead = () if rows is None else (rows,)
-        shape = tuple(p.shape)
-        if len(shape) != len(lead) + 1 or shape[:-1] != lead or not 1 <= shape[-1] < n:
-            raise AssertionError(f"{what} must be {''.join(f'[{r}]' for r in lead)}[P] with 1 <= P < {n}; got {shape}")
-        if p.dtype.is_floating_point or p.dtype.is_complex or p.dtype == torch.bool:
-            raise AssertionError(f"{what} must hold integer mu-law codes; got {p.dtype}")
-        if int(p.min()) < 0 or int(p.max()) >= self.A:
-            raise AssertionError(f"{what} holds codes outside [0, {self.A})")
-        if not fp16:
-            raise AssertionError(f"{what} needs fp16=True: prompts are scored by the fp16 scorer")
-        return p
+        return check_prompt(what, prompt, rows, n, fp16, self.A)
 
     def infer(self, cond_input, implementation, seed=None, fp16=False, window=None, prompt=None):
         """cond_input: channels x batch x num_layers x samples (pytorch/nv_wavenet.py:172-196); returns int32 [batch][samples].
