@@ -296,6 +296,27 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Not in the reference class: multi-model serving.  set_model copies src's weights into model `model` (1 <= model <
+     * NVWN_MAX_MODELS) of this engine; model_group is the rows G per model group (0 on failure); set_group_models gives each of the
+     * ceil(B / G) groups its model from the next launch on `stream`.  See nvwn_set_model, nvwn_model_group and nvwn_set_group_models. */
+    bool set_model(int model, const nvWavenetInfer& src)
+    {
+        const int rc = nvwn_set_model(m_engine, model, src.m_engine);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
+    int model_group()
+    {
+        int rows = 0;
+        if (nvwn_model_group(m_engine, &rows) != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rows;
+    }
+    bool set_group_models(const int* models, int n_groups, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_set_group_models(m_engine, models, n_groups, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
 
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)

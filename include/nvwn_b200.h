@@ -316,6 +316,29 @@ int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states,
  * an earlier utterance's inputs) or an engine that is not NVWN_FP16 (NVWN_EUNSUPPORTED). */
 int nvwn_score_save_states(nvwn_engine* e, const int* rows, int n, const unsigned long long* seeds, void* states, void* stream);
 
+/* Multi-model serving: several models of one shape in one engine, each group of rows generating with its own weights.  Model 0 is
+ * the engine's own weights (the setters, nvwn_weight_blob and nvwn_weights_updated); every generation kernel reads the weights of
+ * a row's model, and nothing else about a row changes.  Scope:
+ *   - scoring (nvwn_score*, nvwn_score_save_states) uses model 0 only;
+ *   - nvwn_prime_from_score and nvwn_prime_slots_from_score refuse (NVWN_EINVAL) rows or slots whose group runs another model: a
+ *     prompt for model m is scored on an engine holding m as model 0, and its state goes in through nvwn_score_save_states and
+ *     nvwn_load_slots;
+ *   - slot states record no model, as they record no weights: loading one into a group that runs the right model is the caller's job. */
+enum { NVWN_MAX_MODELS = 64 };
+/* Copies src's weights (its blob, as uploaded) into model `model` (1 <= model < NVWN_MAX_MODELS) of e.  src is any engine on the
+ * same device with the same dtype, R, S, A, L, max_dilation and tanh_embed (any B, N or kernel).  Later changes to src do not
+ * reach e; calling again replaces the model.  Returns when src may be changed or destroyed.  Refused with NVWN_EINVAL, changing
+ * nothing: NULL arguments, model 0 or an index out of range, a source of another shape, dtype, tanh_embed or device. */
+int nvwn_set_model(nvwn_engine* e, int model, const nvwn_engine* src);
+/* Rows per model group: rows [g*G, (g+1)*G) always run one model.  Fixed at creation by the kernel family: the latency kernels 8
+ * when a full-batch run takes 8-utterance clusters, else 16; the tensor-core kernel its tile; the CUDA-core kernel 4. */
+int nvwn_model_group(nvwn_engine* e, int* rows);
+/* models[g] for each of the ceil(B / G) groups; every entry must be 0 or a model already set.  Stream-ordered on `stream`; takes
+ * effect from the next launch.  Host array, copied before return.  Default: every group runs model 0, also after
+ * nvwn_reset_history, which leaves the models and the table alone.  Refused with NVWN_EINVAL, changing nothing: NULL arguments,
+ * n_groups != ceil(B / G), an entry naming a model that was never set. */
+int nvwn_set_group_models(nvwn_engine* e, const int* models, int n_groups, void* stream);
+
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);
 int nvwn_get_skip_out(nvwn_engine* e, int layer, float* out);

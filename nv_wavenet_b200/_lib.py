@@ -9,6 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NVWN_LIB_PATH") or os.path.join(HERE, "lib", "libwavenet_infer.so")      # (override: experimental builds)
 
 FP32, FP16, FP32_FAST = 0, 1, 2
+MAX_MODELS = 64                 # NVWN_MAX_MODELS: models per engine, model 0 its own weights
 KERNEL_AUTO, KERNEL_STREAM, KERNEL_TENSORCORE, KERNEL_LATENCY = 0, 16, 17, 18
 
 _vp = C.c_void_p
@@ -69,6 +70,9 @@ SYMBOLS = {
     "nvwn_save_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "nvwn_load_slots": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp]),
     "nvwn_score_save_states": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp]),
+    "nvwn_set_model": (C.c_int, [_vp, C.c_int, _vp]),
+    "nvwn_model_group": (C.c_int, [_vp, _vp]),
+    "nvwn_set_group_models": (C.c_int, [_vp, _vp, C.c_int, _vp]),
     "nvwn_get_xt_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_skip_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_zs": (C.c_int, [_vp, _vp]),

@@ -19,6 +19,12 @@ struct WnConfig {
     bool stream_ring;                       // stream, fp32: the weights may go through the shared-memory ring
 };
 
+// One model's weights on the device: its blob, laid out as the engine's, and its family's image (NULL: the family reads the blob)
+struct WnModel {
+    const char* blob;
+    const void* image;
+};
+
 // Everything a kernel launch needs.  Device pointers only.
 // Replaces nv_wavenet_params<T_weight,T_data> (nv_wavenet.cuh:40-85) of the reference.
 struct WnParams {
@@ -48,7 +54,31 @@ struct WnParams {
     // Absolute time of step init_sample, for the history only (the buffers are rings in streaming use, DESIGN.md §6):
     int ring_slot;      // its history-ring slot, t mod (maxDil+1)
     int hist_t;         // t clamped to maxDil: x_l[t-d] exists iff hist_t + (step - init_sample) >= d, and d <= maxDil
+    // Model groups (nvwn_set_group_models, DESIGN.md §6): rows [g * group_rows, (g + 1) * group_rows) run model group_model[g]
+    // (device [ceil(B / group_rows)]), whose blob and image are models[group_model[g]] (device [NVWN_MAX_MODELS]).  The model
+    // pointers above and the launch's image are model 0's.  group_model NULL: every row runs them, and no kernel looks anything up.
+    int group_rows;
+    const int* group_model;
+    const WnModel* models;
 };
+
+#ifdef __CUDACC__
+// The weights a CTA or cluster whose first row is `row` runs with p.group_model set: every blob pointer of p moved by `shift`
+// bytes, from model 0's blob to its group's model's, and that model's image.  Read once, at kernel entry.
+struct WnGroupWeights {
+    long long shift;
+    const unsigned char* image;
+    template <typename T> __device__ __forceinline__ const T* at(const void* q) const
+    {
+        return reinterpret_cast<const T*>(static_cast<const char*>(q) + shift);
+    }
+};
+__device__ __forceinline__ WnGroupWeights wn_group_weights(const WnParams& p, int row)
+{
+    const WnModel m = p.models[p.group_model[row / p.group_rows]];
+    return {(long long)(m.blob - p.models[0].blob), static_cast<const unsigned char*>(m.image)};
+}
+#endif
 
 // p with its first k steps dropped (a launch split into pieces)
 inline WnParams wn_params_skip(WnParams p, int k)
@@ -103,6 +133,8 @@ struct WnFamily {
     cudaError_t (*pack)(void* image, const WnParams& p, cudaStream_t stream);      // weight blob -> image; NULL: the kernels read the blob
     cudaError_t (*launch)(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info);
     bool whole_batch;                               // a run must take all c.B utterances
+    // rows per model group (WnParams::group_rows): a multiple of the rows every CTA or cluster of any run of the engine serves
+    int (*group_rows)(const WnConfig& c);
 };
 extern const WnFamily wn_stream_family;             // wn_stream_kernel.cu: CUDA-core, one CTA per batch tile, weights streamed from L2
 extern const WnFamily wn_tc_family;                 // wn_tc_kernel.cu: fp16 tensor-core (wgmma) kernel

@@ -155,6 +155,22 @@ struct nvwn_engine : WnConfig {
     DevBuf<void> image;                      // the family's weight image, packed from the blob before the first launch after a change
     bool image_dirty = true;
 
+    // Multi-model serving (nvwn_set_model, DESIGN.md §6).  Models 1 .. NVWN_MAX_MODELS - 1, each with a blob copied from its source
+    // and the family's image, packed before the first launch after a change; model 0 is blob and image above.  model_tab holds
+    // every model's bases for the kernels (device [NVWN_MAX_MODELS]); entry m is written when model m is first set, and its buffers
+    // never move after that.  group_tab is the model of each group of group_rows rows (device [ceil(B / group_rows)]), and
+    // group_host its host copy, empty until nvwn_set_group_models: then launches look the models up.
+    struct Model {
+        DevBuf<char> blob;
+        DevBuf<void> image;
+        bool dirty = true;
+    };
+    std::vector<Model> models;
+    DevBuf<WnModel> model_tab;
+    DevBuf<int> group_tab;
+    std::vector<int> group_host;
+    int group_rows = 0;
+
     // the conditioning producers of the whole-batch calls (nvwn_cond_producer_load / _run / _run_stream) and of the per-slot calls
     // (nvwn_cond_producer_set_weights / _set_slots / _run_slots): each has its own weights, frames and scratch, so the two sets of
     // calls may be interleaved
@@ -413,6 +429,15 @@ void resolve_config(WnConfig& c, int impl)
     c.stream_ring = num("NVWN_STREAM_RING", 1) != 0;
 }
 
+// p's model pointers: the model whose blob starts at `blob`
+void point_weights(const nvwn_engine* e, WnParams& p, const char* blob)
+{
+    p.embPrev = blob + e->o_embPrev; p.embCur = blob + e->o_embCur;
+    p.Wprev = blob + e->o_Wprev; p.Wcur = blob + e->o_Wcur; p.Wres = blob + e->o_Wres; p.Wskip = blob + e->o_Wskip;
+    p.Wzs = blob + e->o_Wzs; p.Wza = blob + e->o_Wza;
+    p.Bh = blob + e->o_Bh; p.Bres = blob + e->o_Bres; p.Bskip = blob + e->o_Bskip; p.Bzs = blob + e->o_Bzs; p.Bza = blob + e->o_Bza;
+}
+
 // init_sample: buffer position of the first step; t_abs: its absolute time in the utterance batch (equal outside streaming use)
 void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, long long t_abs, int count, int num_samples, int batch, int dump)
 {
@@ -422,14 +447,13 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, long long t
     p.ring_slot = (int)(t_abs % (e->maxDil + 1));
     p.hist_t = (int)(t_abs < e->maxDil && !e->early_prime ? t_abs : e->maxDil);
     p.tanhEmbed = e->tanhEmbed; p.dump = dump;
-    p.embPrev = e->blob + e->o_embPrev; p.embCur = e->blob + e->o_embCur;
-    p.Wprev = e->blob + e->o_Wprev; p.Wcur = e->blob + e->o_Wcur; p.Wres = e->blob + e->o_Wres; p.Wskip = e->blob + e->o_Wskip;
-    p.Wzs = e->blob + e->o_Wzs; p.Wza = e->blob + e->o_Wza;
-    p.Bh = e->blob + e->o_Bh; p.Bres = e->blob + e->o_Bres; p.Bskip = e->blob + e->o_Bskip; p.Bzs = e->blob + e->o_Bzs; p.Bza = e->blob + e->o_Bza;
+    point_weights(e, p, e->blob);
     p.Lh = e->Lh; p.sel = e->sel; p.forced = e->use_forced ? e->forced.get() : nullptr;
     p.yPrev = e->yPrev; p.yCur = e->yCur; p.ring = e->ring; p.yOut = e->yOut;
     p.xtOut = e->xtOut; p.skipOut = e->skipOut; p.Zs = e->Zs; p.Za = e->Za; p.P = e->P;
     p.trace = e->trace; p.trace_t = e->trace_t;
+    p.group_rows = e->group_rows;
+    if (!e->group_host.empty()) { p.group_model = e->group_tab; p.models = e->model_tab; }
 }
 
 // One generation launch: `count` steps from buffer position `pos` (pos + count <= num_samples, the yOut row stride), the first at
@@ -447,6 +471,13 @@ int launch_steps(nvwn_engine* e, const char* who, int pos, long long t_abs, int 
         if (e->family->pack && e->image_dirty) {
             CK(e->family->pack(e->image, p, stream));
             e->image_dirty = false;
+        }
+        for (nvwn_engine::Model& m : e->models) {
+            if (!e->family->pack || !m.blob || !m.dirty) continue;
+            WnParams q = p;
+            point_weights(e, q, m.blob);
+            CK(e->family->pack(m.image, q, stream));
+            m.dirty = false;
         }
         CK(e->family->launch(*e, p, e->image, stream, &e->last));
         e->launches++;
@@ -495,6 +526,19 @@ int check_prime(const nvwn_engine* e, const std::string& who)
     if (e->score_packed)
         return fail(NVWN_EUNSUPPORTED, who + ": the scoring stream is packed (nvwn_score_stream_packed): a row's layer fronts may hold an earlier "
                                              "utterance's inputs, so they are no history to generate from");
+    return 0;
+}
+
+// Scoring runs model 0, so a prime may only write rows whose group runs it: rows[0..n) (NULL: rows 0 .. n - 1)
+int check_prime_model(const nvwn_engine* e, const std::string& who, const int* rows, int n)
+{
+    if (e->group_host.empty()) return 0;
+    for (int i = 0; i < n; i++) {
+        const int r = rows ? rows[i] : i, m = e->group_host[r / e->group_rows];
+        if (m != 0)
+            return fail(NVWN_EINVAL, who + ": row " + std::to_string(r) + " is in a group that runs model " + std::to_string(m) + ", and scoring runs model 0: "
+                                           "score the prompt on an engine holding that model and load its state (nvwn_score_save_states, nvwn_load_slots)");
+    }
     return 0;
 }
 
@@ -638,6 +682,12 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     CK(e->prime_rows.alloc(Bz * sizeof(int)));
     if (dtype == NVWN_FP16) CK(e->stage.alloc(e->stage_elems * sizeof(float)));
     if (e->family->pack) CK(e->image.alloc(e->family->image_bytes(*e)));
+    e->models.resize(NVWN_MAX_MODELS);
+    e->group_rows = e->family->group_rows(*e);
+    CK(e->model_tab.alloc(NVWN_MAX_MODELS * sizeof(WnModel)));
+    CK(e->group_tab.alloc((Bz + e->group_rows - 1) / e->group_rows * sizeof(int)));
+    const WnModel model0{e->blob, e->image};
+    CK(cudaMemcpy(e->model_tab, &model0, sizeof model0, cudaMemcpyHostToDevice));
     cudaMemsetAsync(e->blob, 0, e->blob_bytes, 0);
     cudaMemsetAsync(e->yOut, 0, Nz * Bz * sizeof(int), 0);
     cudaMemsetAsync(e->ring, 0, ring_bytes, 0);
@@ -1244,6 +1294,56 @@ int nvwn_weights_updated(nvwn_engine* e)
     return 0;
 }
 
+int nvwn_set_model(nvwn_engine* e, int model, const nvwn_engine* src)
+{
+    const std::string who = "nvwn_set_model";
+    if (!e || !src) return fail(NVWN_EINVAL, who + ": NULL engine");
+    if (model < 1 || model >= NVWN_MAX_MODELS)
+        return fail(NVWN_EINVAL, who + ": model " + std::to_string(model) + " is outside [1, " + std::to_string(NVWN_MAX_MODELS) +
+                                       ") (model 0 is the engine's own weights: use the setters)");
+    if (src->dtype != e->dtype || src->R != e->R || src->S != e->S || src->A != e->A || src->L != e->L || src->maxDil != e->maxDil ||
+        src->tanhEmbed != e->tanhEmbed || src->device != e->device)
+        return fail(NVWN_EINVAL, who + ": the source engine differs in dtype, R, S, A, L, max_dilation, tanh_embed or device");
+    nvwn_engine::Model& m = e->models[model];
+    if (!m.blob) {
+        // first set: the buffers, and the model's entry of the base table, which no launch reads before a group names the model
+        nvwn_engine::Model fresh;
+        CK(fresh.blob.alloc(e->blob_bytes));
+        if (e->family->pack) CK(fresh.image.alloc(e->family->image_bytes(*e)));
+        const WnModel bases{fresh.blob, fresh.image};
+        CK(cudaMemcpy(e->model_tab + model, &bases, sizeof bases, cudaMemcpyHostToDevice));
+        m = std::move(fresh);
+    }
+    CK(cudaMemcpyAsync(m.blob, src->blob, e->blob_bytes, cudaMemcpyDeviceToDevice, 0));
+    m.dirty = true;
+    CK(cudaStreamSynchronize(0));       // src may be changed or destroyed on return
+    return 0;
+}
+
+int nvwn_model_group(nvwn_engine* e, int* rows)
+{
+    if (!e || !rows) return fail(NVWN_EINVAL, "nvwn_model_group: NULL argument");
+    *rows = e->group_rows;
+    return 0;
+}
+
+int nvwn_set_group_models(nvwn_engine* e, const int* models, int n_groups, void* stream)
+{
+    const std::string who = "nvwn_set_group_models";
+    if (!e || !models) return fail(NVWN_EINVAL, who + ": NULL argument");
+    const int groups = (e->B + e->group_rows - 1) / e->group_rows;
+    if (n_groups != groups)
+        return fail(NVWN_EINVAL, who + ": need n_groups = ceil(B / G) = " + std::to_string(groups) + " (G = " + std::to_string(e->group_rows) + "); got " +
+                                       std::to_string(n_groups));
+    for (int g = 0; g < n_groups; g++)
+        if (models[g] != 0 && (models[g] < 0 || models[g] >= NVWN_MAX_MODELS || !e->models[models[g]].blob))
+            return fail(NVWN_EINVAL, who + ": group " + std::to_string(g) + " names model " + std::to_string(models[g]) + ", which was never set");
+    const int rc = copy_snapshot(e->group_tab, models, n_groups, (cudaStream_t)stream);
+    if (rc != 0) return rc;
+    e->group_host.assign(models, models + n_groups);
+    return 0;
+}
+
 int nvwn_run_partial(nvwn_engine* e, int init_sample, int count, int num_samples, int batch_size,
                      int* yOut, int dump_activations, void* stream_)
 {
@@ -1554,6 +1654,7 @@ int nvwn_prime_from_score(nvwn_engine* e, void* stream)
     const std::string who = "nvwn_prime_from_score";
     int rc = check_prime(e, who);
     if (rc == 0) rc = check_run_batch(e, who, e->score_bs);
+    if (rc == 0) rc = check_prime_model(e, who, nullptr, e->score_bs);
     if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int Bs = e->score_bs;
@@ -1573,7 +1674,7 @@ int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slot
     int rc = check_prime(e, who);
     if (rc != 0) return rc;
     if (!rows) return fail(NVWN_EINVAL, who + ": rows is NULL");
-    if ((rc = check_slots(e, who, slots, n))) return rc;
+    if ((rc = check_slots(e, who, slots, n)) || (rc = check_prime_model(e, who, slots, n))) return rc;
     const int Bs = e->score_bs;
     std::vector<char> seen(Bs, 0);
     for (int i = 0; i < n; i++) {

@@ -439,7 +439,8 @@ __device__ __forceinline__ void relu_skip(float (&sk)[4], const float* bskip, in
 // What both roles of wn_lat_kernel (the TMA producer lane and the compute warps) use; set once, by the kernel's prologue.
 struct LatCta {
     const WnParams& p;
-    const unsigned char* img;
+    const unsigned char* img;                   // the tile's weight image and previous-index embedding table (its model's)
+    const void* embPrev;
     LatImage im;
     uint32_t sm;                                // shared-memory base
     int L, B, tid, w, lane, tile, slots, t_begin, t_end;
@@ -608,7 +609,7 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
 
     // ---------------- prologue: previous-index rows of the first sample, prefetch pipeline
     {
-        const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
+        const uint32_t* ep = static_cast<const uint32_t*>(c.embPrev);
         sts32(sm + C::O_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TU + g] * 32 + 4 * w + t4]);
         sts32(sm + C::O_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
     }
@@ -721,7 +722,7 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
             sts64(sm + C::O_XBUF + xchg, x01, x23);
             stg_v2(gring + (size_t)((uint32_t)(it0.slot * L) * rstride) + jw * 512 + hw * 8, x01, x23);
             // previous-index rows of the NEXT sample (= this sample's current index): global -> shared, asynchronously
-            const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
+            const unsigned char* ep = static_cast<const unsigned char*>(c.embPrev);
             const uint32_t en = sm + C::O_EPBUF + (epar ^ 1) * (TU * EROW * 4);
             cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
             cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
@@ -886,8 +887,9 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
 
 // DUMP: write the last-sample activations (the host runs the final sample of a dumping launch with this variant).
 // TRC:  record the clock64 timeline (debug; tools/lat_trace.py).
-template <int S, bool DUMP, bool TRC>
-__global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
+// MODELS: p.group_model is set, and the tile's weights are its group's model's (DESIGN.md §6).
+template <int S, bool DUMP, bool TRC, bool MODELS>
+__global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const unsigned char* __restrict__ img0, const int ntiles_alloc)
 {
     using C = Cfg<S>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -896,6 +898,8 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
     const LatImage im = lat_image(S, L);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tile = blockIdx.x;
+    const WnGroupWeights gw = MODELS ? wn_group_weights(p, tile * TU) : WnGroupWeights{0, img0};
+    const unsigned char* __restrict__ img = gw.image;
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
@@ -916,7 +920,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
     }
     {   // current-index embedding table -> shared memory (rows padded to 33 words: gathers of different rows fall into
         // different banks); output-layer biases; feedback state
-        const uint32_t* ec = static_cast<const uint32_t*>(p.embCur);
+        const uint32_t* ec = gw.at<uint32_t>(p.embCur);
         for (int i = tid; i < A * 32; i += NT) sts32(sm + C::O_EMB + ((i >> 5) * EROW + (i & 31)) * 4, ec[i]);
         for (int i = tid; i < S; i += NT) s_bout[i] = gbias[im.b_skpre + (size_t)(L - 1) * S + i];
         for (int i = tid; i < A; i += NT) { s_bout[S + i] = gbias[im.b_bzs + i]; s_bout[S + A + i] = gbias[im.b_bza + i]; }
@@ -928,7 +932,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
     }
     __syncthreads();
 
-    const LatCta c{p, img, im, sm, L, B, tid, warp, lane, tile, slots, t_begin, t_end, gbias, s_full, s_empty, s_pfull, dil, ys, s_bout, trc, tr_t};
+    const LatCta c{p, img, gw.at<void>(p.embPrev), im, sm, L, B, tid, warp, lane, tile, slots, t_begin, t_end, gbias, s_full, s_empty, s_pfull, dil, ys, s_bout, trc, tr_t};
     if (warp == NCW) {
         if (lane == 0) lat_producer<S, TRC>(c, trn);
     } else {
@@ -1079,7 +1083,8 @@ __device__ __forceinline__ void release_remote(uint32_t local_bar, uint32_t rank
 // What more than one role of wn_lat2_kernel uses; set once, by the kernel's prologue.
 struct ClusterCta {
     const WnParams& p;
-    const unsigned char* img;
+    const unsigned char* img;                   // the cluster's weight image and previous-index embedding table (its model's)
+    const void* embPrev;
     LatImage im;
     unsigned char* smem;                        // shared memory, and its shared-window address
     uint32_t sm;
@@ -1332,7 +1337,7 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
             }
         };
         {   // prologue: previous-index rows of the first sample
-            const uint32_t* ep = static_cast<const uint32_t*>(p.embPrev);
+            const uint32_t* ep = static_cast<const uint32_t*>(c.embPrev);
             sts32(sm + M::C_EPBUF + (g * EROW + 4 * w + t4) * 4, ep[ys[TR + g] * 32 + 4 * w + t4]);
             if (TR == TU) sts32(sm + M::C_EPBUF + ((g + 8) * EROW + 4 * w + t4) * 4, ep[ys[TU + g + 8] * 32 + 4 * w + t4]);
         }
@@ -1359,7 +1364,7 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
             {   // embedding (reference.cpp:42-57), this warp's 8 channels
                 const int yc0 = ys[g], yc1 = TR == TU ? ys[g + 8] : 0;
                 const uint32_t eo = sm + M::C_EPBUF + epar * (TR * EROW * 4);
-                const unsigned char* ep = static_cast<const unsigned char*>(p.embPrev);
+                const unsigned char* ep = static_cast<const unsigned char*>(c.embPrev);
                 const uint32_t en = sm + M::C_EPBUF + (epar ^ 1) * (TR * EROW * 4);
                 const float2 a0 = unpack_h2(lds32(eo + (g * EROW + 4 * w + t4) * 4));
                 const float2 c0 = unpack_h2(lds32(sm + M::C_EMB + (yc0 * EROW + 4 * w + t4) * 4));
@@ -1788,8 +1793,9 @@ __device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
     }
 }
 
-template <int S, int TR, bool DUMP, bool TRC>
-__global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img, const int ntiles_alloc)
+// MODELS: p.group_model is set, and the cluster's weights are its group's model's (DESIGN.md §6).
+template <int S, int TR, bool DUMP, bool TRC, bool MODELS>
+__global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img0, const int ntiles_alloc)
 {
     // debug timeline (tools/lat_trace.py, TRACE2): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
     unsigned long long* trc = (TRC && p.trace && blockIdx.x < NCL) ? p.trace : nullptr;
@@ -1808,6 +1814,8 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     // this cluster serves utterances ub .. ub + TR - 1: all of 16-row tile `tile` of the conditioning store and the history ring, or
     // (TR = 8) its half ub & 8, whose words sit `hw4` bytes into every 16-byte group of the tile's accumulator / A-fragment order
     const int ub = blockIdx.x / NCL * TR, tile = ub / TU;
+    const WnGroupWeights gw = MODELS ? wn_group_weights(p, ub) : WnGroupWeights{0, img0};
+    const unsigned char* __restrict__ img = gw.image;
     const uint32_t hw4 = (uint32_t)(ub & 8) >> 1;
     const int slots = p.maxDil + 1;
     const int t_begin = p.init_sample, t_end = p.init_sample + p.count;
@@ -1851,7 +1859,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
         ys[TR + tid] = b < B ? p.yPrev[b] : 128;
     }
     if (is_chain) {
-        const uint32_t* ec = static_cast<const uint32_t*>(p.embCur);
+        const uint32_t* ec = gw.at<uint32_t>(p.embCur);
         for (int i = tid; i < A * 32; i += NTC) sts32(sm + M::C_EMB + ((i >> 5) * EROW + (i & 31)) * 4, ec[i]);
         for (int i = tid; i < L * 256; i += NTC) sts32(sm + M::C_BIAS + i * 4, __float_as_uint(gbias[im.b_layer + i]));
     } else if (is_tail) {
@@ -1873,7 +1881,7 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     const bool v0 = b0 < B, v1 = b1 < B;
     const uint32_t lane16 = (uint32_t)lane * 16;
     const uint32_t xchg = xslot<TR>(w, lane);                // this thread's slot of an activation tile
-    const ClusterCta c{p, img, im, smem_raw, sm, L, B, tid, crank, ub, tile, hw4, slots, t_begin, t_end, ntiles_alloc, gbias,
+    const ClusterCta c{p, img, gw.at<void>(p.embPrev), im, smem_raw, sm, L, B, tid, crank, ub, tile, hw4, slots, t_begin, t_end, ntiles_alloc, gbias,
                        s_full, s_empty, s_pfull, s_hfull, s_hfree, s_yfull, s_apfull, s_apfree, s_ob0full, s_ob0free, s_ob1full, s_ob1free, s_lfull, s_lfree,
                        ys, w, lane, g, t4, b0, b1, v0, v1, lane16, xchg, trc, tr_t};
     if (is_chain) chain_cta<S, TR, DUMP, TRC>(c, trn);
@@ -1912,13 +1920,13 @@ static cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stre
 // store / history ring were laid out for
 using LatGo = cudaError_t (*)(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream);
 
-template <int S, bool DUMP, bool TRC>
+template <int S, bool DUMP, bool TRC, bool MODELS>
 static cudaError_t lat_go(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
 {
     const size_t smem = Cfg<S>::SMEM;
-    const cudaError_t e = cudaFuncSetAttribute(wn_lat_kernel<S, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t e = cudaFuncSetAttribute(wn_lat_kernel<S, DUMP, TRC, MODELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    wn_lat_kernel<S, DUMP, TRC><<<tiles, NT, smem, stream>>>(p, im8, ntiles_alloc);
+    wn_lat_kernel<S, DUMP, TRC, MODELS><<<tiles, NT, smem, stream>>>(p, im8, ntiles_alloc);
     return cudaGetLastError();
 }
 
@@ -1937,14 +1945,14 @@ static cudaLaunchConfig_t lat2_config(int clusters, cudaStream_t stream, cudaLau
     cfg.numAttrs = 1;
     return cfg;
 }
-template <int S, int TR, bool DUMP, bool TRC>
+template <int S, int TR, bool DUMP, bool TRC, bool MODELS>
 static cudaError_t lat2_go(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream)
 {
-    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, TR, DUMP, TRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, TR, DUMP, TRC, MODELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM);
     if (e != cudaSuccess) return e;
     cudaLaunchAttribute at;
     const cudaLaunchConfig_t cfg = lat2_config<S, TR>(clusters, stream, at);
-    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, TR, DUMP, TRC>, p, im8, ntiles_alloc);
+    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, TR, DUMP, TRC, MODELS>, p, im8, ntiles_alloc);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 // how many clusters the device runs at once (a cluster needs NCL SMs of one GPC: fewer than 132 / NCL fit on an H100); 0 if the query fails
@@ -1953,11 +1961,11 @@ static int lat2_max_clusters()
 {
     static int cached = -1;
     if (cached >= 0) return cached;
-    if (cudaFuncSetAttribute(wn_lat2_kernel<S, TR, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
+    if (cudaFuncSetAttribute(wn_lat2_kernel<S, TR, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
     cudaLaunchAttribute at;
     const cudaLaunchConfig_t cfg = lat2_config<S, TR>(48, 0, at);
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, TR, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+    if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, TR, false, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
     return cached = n;
 }
 
@@ -1977,13 +1985,19 @@ template <int S>
 static cudaError_t lat_launch_S(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
 {
     *smem_out = Cfg<S>::SMEM;
-    return lat_launch_split(p, lat_go<S, false, false>, lat_go<S, false, true>, lat_go<S, true, false>, im8, tiles, ntiles_alloc, stream);
+    if (p.group_model)
+        return lat_launch_split(p, lat_go<S, false, false, true>, lat_go<S, false, true, true>, lat_go<S, true, false, true>, im8, tiles, ntiles_alloc, stream);
+    return lat_launch_split(p, lat_go<S, false, false, false>, lat_go<S, false, true, false>, lat_go<S, true, false, false>, im8, tiles, ntiles_alloc, stream);
 }
 template <int S, int TR>
 static cudaError_t lat2_launch_S(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
 {
     *smem_out = CfgC<S, TR>::SMEM;
-    return lat_launch_split(p, lat2_go<S, TR, false, false>, lat2_go<S, TR, false, true>, lat2_go<S, TR, true, false>, im8, clusters, ntiles_alloc, stream);
+    if (p.group_model)
+        return lat_launch_split(p, lat2_go<S, TR, false, false, true>, lat2_go<S, TR, false, true, true>, lat2_go<S, TR, true, false, true>, im8, clusters,
+                                ntiles_alloc, stream);
+    return lat_launch_split(p, lat2_go<S, TR, false, false, false>, lat2_go<S, TR, false, true, false>, lat2_go<S, TR, true, false, false>, im8, clusters,
+                            ntiles_alloc, stream);
 }
 
 template <int TR>
@@ -1996,19 +2010,27 @@ int wn_lat_max_clusters(int S, int rows) { return rows == 8 ? lat2_fit<8>(S) : r
 // weight reads, so it is faster per utterance as long as there are SMs for twice the clusters.  A run of fewer utterances than the
 // engine holds takes the first p.B of them: the conditioning store and the history ring stay laid out per 16-utterance tile of the
 // engine's batch, whichever tile height runs.
+// The utterances per cluster of a run of `batch` utterances: 8, 16 (TU), or 0 when the single-CTA kernel runs.
+// The cluster kernel's prep CTA reads history tiles the chain CTA wrote at least L - 9 steps earlier: it wants a few steps of margin.
+static int lat_cluster_rows(const WnConfig& c, int batch)
+{
+    if (!c.lat_cluster || c.L < 12 || (c.S != 256 && c.S != 128)) return 0;
+    if ((batch + 7) / 8 <= lat2_fit<8>(c.S)) return 8;
+    if (lat_tiles(batch) <= lat2_fit<TU>(c.S)) return TU;
+    return 0;
+}
+// A model group is what a full-batch run serves per cluster when that is 8 rows, else a 16-row tile.  A smaller run's clusters lie
+// inside these groups: fewer utterances never take a taller tile.
+static int lat_group_rows(const WnConfig& c) { return lat_cluster_rows(c, c.B) == 8 ? 8 : TU; }
+
 static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const void* image, cudaStream_t stream, WnLaunchInfo* info)
 {
-    const bool cluster = c.lat_cluster;
     const int grid = lat_tiles(p.B), ntiles_alloc = lat_tiles(c.B);
     const unsigned char* im8 = static_cast<const unsigned char*>(image);
     size_t smem = 0;
     cudaError_t e;
-    // the cluster kernel's prep CTA reads history tiles the chain CTA wrote at least L - 9 steps earlier: it wants a few steps of margin
-    if (cluster && p.L >= 12 && (p.S == 256 || p.S == 128)) {
-        const int c8 = (p.B + 7) / 8;
-        int tr = 0, clusters = 0;
-        if (c8 <= lat2_fit<8>(p.S)) { tr = 8; clusters = c8; }
-        else if (grid <= lat2_fit<TU>(p.S)) { tr = TU; clusters = grid; }
+    {
+        const int tr = lat_cluster_rows(c, p.B), clusters = tr == 8 ? (p.B + 7) / 8 : grid;
         if (tr == 8) e = p.S == 256 ? lat2_launch_S<256, 8>(p, im8, clusters, ntiles_alloc, stream, &smem) : lat2_launch_S<128, 8>(p, im8, clusters, ntiles_alloc, stream, &smem);
         else if (tr == TU) e = p.S == 256 ? lat2_launch_S<256, TU>(p, im8, clusters, ntiles_alloc, stream, &smem) : lat2_launch_S<128, TU>(p, im8, clusters, ntiles_alloc, stream, &smem);
         if (tr) {
@@ -2028,4 +2050,4 @@ static cudaError_t wn_launch_lat(const WnConfig& c, const WnParams& p, const voi
 const WnFamily wn_lat_family = {LatLayout::store_bytes, LatLayout::ring_bytes, image_bytes, cond_convert, wn_readback<LatLayout>,
                                 wn_clear_rows<LatLayout>, wn_convert_rows<LatLayout>, wn_put_history<LatLayout>, wn_get_history<LatLayout>,
                                 wn_put_history_rows<LatLayout>, wn_get_history_rows<LatLayout>, wn_clear_times<LatLayout>,
-                                wn_lat_pack, wn_launch_lat, false};
+                                wn_lat_pack, wn_launch_lat, false, lat_group_rows};

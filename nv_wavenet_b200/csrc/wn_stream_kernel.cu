@@ -172,7 +172,8 @@ __host__ __device__ constexpr size_t stream_smem_floats(int A, int L)
     return (size_t)BT * (3 * R + 4 * R + R + 2 * S + 3 * A) + BT * 4 + BT * 2 + L + 4;
 }
 
-template <typename TD, int R, int S, int BT, bool FAST, bool RING>
+// MODELS: p.group_model is set, and the CTA's weights are its group's model's (DESIGN.md §6)
+template <typename TD, int R, int S, int BT, bool FAST, bool RING, bool MODELS>
 __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_stream_kernel(const WnParams p)
 {
     using N = typename NumSel<TD, FAST>::type;
@@ -211,19 +212,20 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
     // all compute threads (the producer warp of the RING kernels is not among them)
     auto SYNC = [&]() { if (RING) asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); else __syncthreads(); };
 
-    const TD* embPrev = static_cast<const TD*>(p.embPrev);
-    const TD* embCur = static_cast<const TD*>(p.embCur);
-    const TD* Wprev = static_cast<const TD*>(p.Wprev);
-    const TD* Wcur = static_cast<const TD*>(p.Wcur);
-    const TD* Wres = static_cast<const TD*>(p.Wres);
-    const TD* Wskip = static_cast<const TD*>(p.Wskip);
-    const TD* Wzs = static_cast<const TD*>(p.Wzs);
-    const TD* Wza = static_cast<const TD*>(p.Wza);
-    const TD* Bh = static_cast<const TD*>(p.Bh);
-    const TD* Bres = static_cast<const TD*>(p.Bres);
-    const TD* Bskip = static_cast<const TD*>(p.Bskip);
-    const TD* Bzs = static_cast<const TD*>(p.Bzs);
-    const TD* Bza = static_cast<const TD*>(p.Bza);
+    const WnGroupWeights gw = MODELS ? wn_group_weights(p, b0) : WnGroupWeights{0, nullptr};
+    const TD* embPrev = gw.at<TD>(p.embPrev);
+    const TD* embCur = gw.at<TD>(p.embCur);
+    const TD* Wprev = gw.at<TD>(p.Wprev);
+    const TD* Wcur = gw.at<TD>(p.Wcur);
+    const TD* Wres = gw.at<TD>(p.Wres);
+    const TD* Wskip = gw.at<TD>(p.Wskip);
+    const TD* Wzs = gw.at<TD>(p.Wzs);
+    const TD* Wza = gw.at<TD>(p.Wza);
+    const TD* Bh = gw.at<TD>(p.Bh);
+    const TD* Bres = gw.at<TD>(p.Bres);
+    const TD* Bskip = gw.at<TD>(p.Bskip);
+    const TD* Bzs = gw.at<TD>(p.Bzs);
+    const TD* Bza = gw.at<TD>(p.Bza);
     const TD* Lh = static_cast<const TD*>(p.Lh);
     TD* ring = static_cast<TD*>(p.ring);
 
@@ -243,9 +245,9 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
     if (RING && tid >= NT) {
         // ---- producer warp: one lane streams the pieces in consumption order ----
         if (tid == NT) {
-            const float* fWprev = reinterpret_cast<const float*>(p.Wprev); const float* fWcur = reinterpret_cast<const float*>(p.Wcur);
-            const float* fWres = reinterpret_cast<const float*>(p.Wres); const float* fWskip = reinterpret_cast<const float*>(p.Wskip);
-            const float* fWzs = reinterpret_cast<const float*>(p.Wzs); const float* fWza = reinterpret_cast<const float*>(p.Wza);
+            const float* fWprev = gw.at<float>(p.Wprev); const float* fWcur = gw.at<float>(p.Wcur);
+            const float* fWres = gw.at<float>(p.Wres); const float* fWskip = gw.at<float>(p.Wskip);
+            const float* fWzs = gw.at<float>(p.Wzs); const float* fWza = gw.at<float>(p.Wza);
             uint32_t n = 0;
             auto put = [&](const float* s0, uint32_t f0, const float* s1, uint32_t f1) {       // floats of the one or two parts of a piece
                 const uint32_t sl = n % RC::SLOTS;
@@ -607,20 +609,26 @@ __global__ void __launch_bounds__(Shape<R, S>::NT + (RING ? 32 : 0), 1) wn_strea
     if (tid < BT) { p.yPrev[b0 + tid] = ysm[tid * 2]; p.yCur[b0 + tid] = ysm[tid * 2 + 1]; }
 }
 
-template <typename TD, int R, int S, int BT, bool FAST, bool RING>
-cudaError_t launch_kernel(const WnParams& p, cudaStream_t stream, WnLaunchInfo* info)
+template <typename TD, int R, int S, int BT, bool FAST, bool RING, bool MODELS>
+cudaError_t launch_variant(const WnParams& p, cudaStream_t stream, WnLaunchInfo* info)
 {
     constexpr int NT = Shape<R, S>::NT;
     using RC = RingCfg<R, S>;
     size_t smem = stream_smem_floats<R, S, BT>(p.A, p.L) * sizeof(float);
     if (RING) smem += 128 + (size_t)RC::SLOTS * RC::PIECE + 2 * RC::SLOTS * sizeof(uint64_t);
-    auto kfn = wn_stream_kernel<TD, R, S, BT, FAST, RING>;
+    auto kfn = wn_stream_kernel<TD, R, S, BT, FAST, RING, MODELS>;
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     const int grid = p.B / BT, block = NT + (RING ? 32 : 0);
     kfn<<<grid, block, smem, stream>>>(p);
     if (info) { info->grid = grid; info->block = block; info->smem_bytes = (int)smem; info->batch_per_cta = BT; info->cluster = 1; }
     return cudaGetLastError();
+}
+template <typename TD, int R, int S, int BT, bool FAST, bool RING>
+cudaError_t launch_kernel(const WnParams& p, cudaStream_t stream, WnLaunchInfo* info)
+{
+    if (p.group_model) return launch_variant<TD, R, S, BT, FAST, RING, true>(p, stream, info);
+    return launch_variant<TD, R, S, BT, FAST, RING, false>(p, stream, info);
 }
 
 // fp32: weights through the shared-memory ring when the engine allows it (WnConfig::stream_ring), the output layers fit one row
@@ -745,7 +753,9 @@ bool wn_stream_supported(int R, int S, int A, bool)
 // The kernels read the weight blob and the plain conditioning store; any batch up to the engine's.  convert and readback are
 // contiguous conversions (wn_convert.cu): the plain store already is the source layout, and an fp32 convert also copies from host
 // memory, which no kernel can read.  put_history is fp16 only: the engine primes no other precision.  The per-slot history
-// operations follow the engine's precision: fp32 engines park and resume slots too.
+// operations follow the engine's precision: fp32 engines park and resume slots too.  A CTA serves BT = 1, 2 or 4 rows from a
+// multiple of BT, so a model group of 4 rows holds whole CTAs whichever BT runs.
+static int plain_group_rows(const WnConfig&) { return 4; }
 const WnFamily wn_stream_family = {plain_store_bytes, plain_ring_bytes, nullptr, wn_plain_convert, wn_plain_readback, plain_clear_rows,
                                    plain_convert_rows, wn_put_history<PlainH>, plain_get_history, plain_put_history_rows, plain_get_history_rows,
-                                   plain_clear_times, nullptr, wn_launch_stream, false};
+                                   plain_clear_times, nullptr, wn_launch_stream, false, plain_group_rows};

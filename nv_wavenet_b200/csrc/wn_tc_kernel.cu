@@ -186,8 +186,9 @@ __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;
 // Accumulator fragment of a warpgroup (wn_sm90.cuh): thread i holds rows r0 = 16 (i / 32) + (i % 32) / 4 and r0 + 8, and in
 // every 8-column group j the columns 8 j + 2 (i % 4) + {0, 1}.  Index 4 j + 2 r + e of a fragment array = row r0 + 8 r,
 // column 8 j + 2 (i % 4) + e.  x, the gate inputs and Dx of one thread are the same 16 (row, channel) pairs.
-template <int S, bool FUSED>
-__global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const unsigned char* __restrict__ img, const int nstage, const int tu)
+// MODELS: p.group_model is set, and the CTA's weights are its tile's model's (a model group is one tile, DESIGN.md §6)
+template <int S, bool FUSED, bool MODELS>
+__global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const unsigned char* __restrict__ img0, const int nstage, const int tu)
 {
     constexpr int SKN = S / 2;                     // skip columns per warpgroup
     constexpr int SKC = S / 128;                   // skip weight chunks per layer
@@ -210,6 +211,8 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
     const int tid = threadIdx.x;
     const int sub = tu > TU ? tu / TU : 1;                         // CTAs per tile
     const int tile = blockIdx.x / sub, ntiles = gridDim.x / sub;
+    const WnGroupWeights gw = MODELS ? wn_group_weights(p, tile * tu) : WnGroupWeights{0, img0};
+    const unsigned char* __restrict__ img = gw.image;
     const int row0 = (blockIdx.x % sub) * TU;                      // first row of this CTA inside its tile
     const int live = tu < TU ? tu : TU;                            // MMA rows that hold utterances
     const int slots = p.maxDil + 1;
@@ -300,8 +303,8 @@ __global__ void __launch_bounds__(NT, 1) wn_tc_kernel(const WnParams p, const un
         yp[r] = valid[r] ? p.yPrev[bb[r]] : 0;
         yc[r] = valid[r] ? p.yCur[bb[r]] : 0;
     }
-    const __half* embPrev = static_cast<const __half*>(p.embPrev);
-    const __half* embCur = static_cast<const __half*>(p.embCur);
+    const __half* embPrev = gw.at<__half>(p.embPrev);
+    const __half* embCur = gw.at<__half>(p.embCur);
     const float* gbias = reinterpret_cast<const float*>(img + im.off_bias);
 
     int stage = 0;
@@ -660,14 +663,16 @@ cudaError_t wn_launch_tc(const WnConfig& c, const WnParams& p, const void* tc_im
     const int grid = (p.B + tu - 1) / tu * (tu > TU ? tu / TU : 1);
     const unsigned char* im8 = static_cast<const unsigned char*>(tc_image_);
     cudaError_t e = cudaErrorInvalidValue;
-#define WN_TC_LAUNCH(SV, FV)                                                                                     \
-    do {                                                                                                         \
-        e = cudaFuncSetAttribute(wn_tc_kernel<SV, FV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
-        if (e != cudaSuccess) return e;                                                                          \
-        wn_tc_kernel<SV, FV><<<grid, NT, smem, stream>>>(p, im8, nstage, tu);                                   \
+#define WN_TC_LAUNCH(SV, FV, MV)                                                                                     \
+    do {                                                                                                             \
+        e = cudaFuncSetAttribute(wn_tc_kernel<SV, FV, MV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
+        if (e != cudaSuccess) return e;                                                                              \
+        wn_tc_kernel<SV, FV, MV><<<grid, NT, smem, stream>>>(p, im8, nstage, tu);                                   \
     } while (0)
-    if (p.S == 256) { if (fused) WN_TC_LAUNCH(256, true); else WN_TC_LAUNCH(256, false); }
-    else { if (fused) WN_TC_LAUNCH(128, true); else WN_TC_LAUNCH(128, false); }
+#define WN_TC_LAUNCH_M(SV, FV) do { if (p.group_model) WN_TC_LAUNCH(SV, FV, true); else WN_TC_LAUNCH(SV, FV, false); } while (0)
+    if (p.S == 256) { if (fused) WN_TC_LAUNCH_M(256, true); else WN_TC_LAUNCH_M(256, false); }
+    else { if (fused) WN_TC_LAUNCH_M(128, true); else WN_TC_LAUNCH_M(128, false); }
+#undef WN_TC_LAUNCH_M
 #undef WN_TC_LAUNCH
     if (info) { info->kernel = NVWN_KERNEL_TENSORCORE; info->grid = grid; info->block = NT; info->smem_bytes = (int)smem; info->batch_per_cta = tu < TU ? tu : TU; info->cluster = 1; }
     return cudaGetLastError();
@@ -680,8 +685,11 @@ bool wn_tc_supported(int R_, int S, int A_, int, int)
     return R_ == R && A_ == A && (S == 128 || S == 256);
 }
 
+// a model group is one tile: every CTA of a tile of 128 runs its model
+static int tc_group_rows(const WnConfig& c) { return c.tc_tile; }
+
 // convert is convert_rows with every row: the whole-store and the per-row paths are one kernel
 const WnFamily wn_tc_family = {TcLayout::store_bytes, TcLayout::ring_bytes, image_bytes, wn_convert<TcLayout>, wn_readback<TcLayout>,
                                wn_clear_rows<TcLayout>, wn_convert_rows<TcLayout>, wn_put_history<TcLayout>, wn_get_history<TcLayout>,
                                wn_put_history_rows<TcLayout>, wn_get_history_rows<TcLayout>, wn_clear_times<TcLayout>, wn_tc_pack,
-                               wn_launch_tc, true};
+                               wn_launch_tc, true, tc_group_rows};

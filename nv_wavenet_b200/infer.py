@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import FP16, FP32, FP32_FAST, KERNEL_AUTO, KERNEL_STREAM, KERNEL_TENSORCORE, check  # noqa: F401
+from ._lib import FP16, FP32, FP32_FAST, KERNEL_AUTO, KERNEL_STREAM, KERNEL_TENSORCORE, MAX_MODELS, check  # noqa: F401
 
 # Implementation enum of the reference (nv_wavenet.cuh:223-229); accepted, all map to the sm_90a kernels
 AUTO, SINGLE_BLOCK, DUAL_BLOCK, PERSISTENT, MANYBLOCK_NONPERSISTENT = 0, 1, 2, 3, 4
@@ -415,6 +415,28 @@ class NVWavenetInfer:
             raise ValueError(f"load_slots: {s.size} slots need {s.size} states of {bytes_} bytes; got {size} bytes")
         check(self._l.nvwn_load_slots(self._h, p, s.size, C.c_void_p(ptr), _stream(stream)), "loadSlots")
         return a
+
+    # ---- multi-model serving (DESIGN.md §6) ----
+    def set_model(self, model, src):
+        """Copies the weights of engine `src` (same dtype, R, S, A, L, max_dilation and tanh_embed) into model `model`,
+        1 <= model < MAX_MODELS, of this engine.  Later changes to src do not reach it; see nvwn_set_model."""
+        check(self._l.nvwn_set_model(self._h, model, src._h), "setModel")
+
+    @property
+    def model_group(self):
+        """Rows per model group G: rows [g*G, (g+1)*G) always run one model (nvwn_model_group)."""
+        g = C.c_int()
+        check(self._l.nvwn_model_group(self._h, C.byref(g)), "modelGroup")
+        return g.value
+
+    def set_group_models(self, models, stream=None):
+        """The model of each of the ceil(B / model_group) groups: 0 or a model given to set_model.  Takes effect from the next
+        launch on `stream`; see nvwn_set_group_models."""
+        m = np.asarray(models, dtype=np.int64).ravel()
+        if m.size and (m.min() < np.iinfo(np.int32).min or m.max() > np.iinfo(np.int32).max):
+            raise ValueError(f"setGroupModels: model indices must fit a C int; got {m.min()} .. {m.max()}")
+        m = np.ascontiguousarray(m.astype(np.int32))
+        check(self._l.nvwn_set_group_models(self._h, C.c_void_p(m.ctypes.data), m.size, _stream(stream)), "setGroupModels")
 
     def cond_producer_run_slots(self, slots, first_sample, num_samples, stream=None):
         """Conditioning of absolute samples [first_sample, first_sample + num_samples), num_samples <= N, for `slots` only, from

@@ -14,6 +14,7 @@ Constructor arguments, accepted shapes, the appended unused residual layer and t
 kernel are those of pytorch/nv_wavenet.py:55-196; the code is organised around one table of expected shapes.
 """
 import ctypes as C
+from collections import deque
 
 import numpy as np
 import torch
@@ -47,26 +48,52 @@ def column_major(x):
     raise AssertionError(f"column_major: unsupported rank {nd}")
 
 
-def plan_slots(lengths, slots, window):
+def plan_slots(lengths, slots, window, models=None, group=1):
     """Continuous batching schedule of infer_many: utterances of `lengths` samples, in arrival order, through `slots` slots
     restarted only at multiples of `window`.  At each window boundary the free slots (lowest first) take the next queued
-    utterances; a slot is free once its utterance has ended.  Returns [(slot, start)] per utterance, start a multiple of window."""
-    if slots < 1 or window < 1:
-        raise ValueError(f"need slots >= 1 and window >= 1; got {slots}, {window}")
+    utterances; a slot is free once its utterance has ended.  Returns [(slot, start)] per utterance, start a multiple of window.
+    models: None, or the model of each utterance (ModelSet.infer_many), slots in groups of `group` that run one model at a time
+    (slots [g*group, (g+1)*group)): a free slot takes the earliest queued utterance whose model its group runs, and a group with
+    no live utterance first takes the model of the earliest queued one.  A group so runs one model for every utterance's whole
+    span.  models=None is the one-model schedule."""
+    if slots < 1 or window < 1 or group < 1:
+        raise ValueError(f"need slots >= 1, window >= 1 and group >= 1; got {slots}, {window}, {group}")
     if any(n < 1 for n in lengths):
         raise ValueError("every utterance needs at least one sample")
+    if models is None:
+        models = [0] * len(lengths)
+    elif len(models) != len(lengths) or any(int(m) != m or m < 0 for m in models):
+        raise ValueError(f"need one model index >= 0 per utterance; got {len(models)} for {len(lengths)} utterances")
     ends = [0] * slots                              # sample at which each slot's current utterance ends
-    plan, t = [], 0
-    for n in lengths:
-        while True:
-            free = [s for s in range(slots) if ends[s] <= t]
-            if free:
-                break
-            t = (min(ends) + window - 1) // window * window       # the first boundary at which a slot is free
-        s = free[0]
-        plan.append((s, t))
-        ends[s] = t + n
+    runs = [None] * ((slots + group - 1) // group)  # the model each group runs while it has a live utterance
+    waiting = {}                                    # model -> its queued utterances, in arrival order
+    for u, m in enumerate(models):
+        waiting.setdefault(m, deque()).append(u)
+    plan, left, t = [None] * len(lengths), len(lengths), 0
+    while left:
+        for s in range(slots):
+            if ends[s] > t or not left:
+                continue
+            g = s // group
+            if all(ends[x] <= t for x in range(g * group, min(slots, (g + 1) * group))):
+                runs[g] = models[min(q[0] for q in waiting.values())]
+            q = waiting.get(runs[g])
+            if q:
+                u = q.popleft()
+                if not q:
+                    del waiting[runs[g]]
+                plan[u] = (s, t)
+                ends[s] = t + lengths[u]
+                left -= 1
+        if left:
+            t = (min(e for e in ends if e > t) + window - 1) // window * window   # the next boundary at which a slot is free
     return plan
+
+
+def _reset(eng):
+    """eng.reset_history(), which writes on the default stream, with the current stream ordered after it"""
+    eng.reset_history()
+    torch.cuda.current_stream().wait_stream(torch.cuda.default_stream())
 
 
 def _windows(plan, lengths, window):
@@ -732,7 +759,8 @@ class NVWaveNet:
         plan = plan_slots([n - P for n, P in zip(lengths, skip)], slots, window)
         windows = _windows(plan, [n - P for n, P in zip(lengths, skip)], window)
         eng = self._engine(slots, window, fp16)
-        eng.reset_history()
+        _reset(eng)
+        st = torch.cuda.current_stream()
         primes = []
 
         def prime(k):
@@ -757,14 +785,28 @@ class NVWaveNet:
                         if e > a:
                             lh[:e - a, :, j].copy_(cond_inputs[u][:, :, a:e].permute(2, 1, 0))
                             codes[j, :e - a] = prompts[u][a:e]
-                    eng.set_conditioning_slots(lh, list(range(g)), a)
-                    eng.score_stream(codes, a)
+                    eng.set_conditioning_slots(lh, list(range(g)), a, stream=st)
+                    eng.score_stream(codes, a, stream=st)
                     a += m
                 done = [j for j, u in enumerate(group) if skip[u] == end]
-                eng.prime_slots_from_score(done, [plan[group[j]][0] for j in done], [seeds[group[j]] for j in done])
+                eng.prime_slots_from_score(done, [plan[group[j]][0] for j in done], [seeds[group[j]] for j in done], stream=st)
             if ev:
                 ev[1].record()
                 primes.append(ev)
+
+        condition = self._condition_slots(eng, windows, cond_inputs, skip)
+        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, before=prime, prompts=prompts)
+        torch.cuda.synchronize()
+        if timing is not None:
+            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
+            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
+            timing["prime_s"] = sum(a.elapsed_time(b) for a, b in primes) / 1e3
+        return outs
+
+    def _condition_slots(self, eng, windows, cond_inputs, skip):
+        """The condition(k) of _serve for expanded conditioning: window k's conditioning of its live slots goes into the engine.
+        Utterance u's generated samples read its conditioning from sample skip[u] on.  On the current stream."""
+        st = torch.cuda.current_stream()
 
         def condition(k):
             first, count, _, live = windows[k]
@@ -773,15 +815,8 @@ class NVWaveNet:
                 lh = torch.zeros((count, self.num_layers, len(live), 2 * self.R), dtype=torch.float32, device="cuda")
                 for j, (_, u, a, m) in enumerate(live):
                     lh[:m, :, j].copy_(cond_inputs[u][:, :, skip[u] + a:skip[u] + a + m].permute(2, 1, 0))
-                eng.set_conditioning_slots(lh, [s for s, _, _, _ in live], first)
-
-        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, before=prime, prompts=prompts)
-        torch.cuda.synchronize()
-        if timing is not None:
-            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
-            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
-            timing["prime_s"] = sum(a.elapsed_time(b) for a, b in primes) / 1e3
-        return outs
+                eng.set_conditioning_slots(lh, [s for s, _, _, _ in live], first, stream=st)
+        return condition
 
     def _slot_prompts(self, prompts, lengths, fp16):
         """infer_many's prompts checked: per utterance None or int32 CUDA codes [P_u], 1 <= P_u < n_u, each in [0, A), and fp16 if any
@@ -820,7 +855,7 @@ class NVWaveNet:
         plan = plan_slots(lengths, slots, window)
         windows = _windows(plan, lengths, window)
         eng = self._engine(slots, 2 * window, fp16)
-        eng.reset_history()
+        _reset(eng)
         eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(lr, Cc), cond_bias, stride)
 
         cur, side = torch.cuda.current_stream(), torch.cuda.Stream()
@@ -882,6 +917,7 @@ class NVWaveNet:
             if p is not None:
                 o[:p.numel()].copy_(p)
         stage = torch.empty((eng.B, eng.N), dtype=torch.int32, device="cuda")
+        st = torch.cuda.current_stream()
         events = []
         for k, (first, count, starting, live) in enumerate(windows):
             if before is not None:
@@ -894,13 +930,13 @@ class NVWaveNet:
                 ev[1].record()
             restart = [u for u in starting if prompts[u] is None]
             if restart:
-                eng.restart_slots([plan[u][0] for u in restart], [seeds[u] for u in restart])
-            eng.set_selectors_random_slots(first, count)
+                eng.restart_slots([plan[u][0] for u in restart], [seeds[u] for u in restart], stream=st)
+            eng.set_selectors_random_slots(first, count, stream=st)
             if ev:
                 ev[2].record()
-            eng.run_stream(first, count, eng.B)
+            eng.run_stream(first, count, eng.B, stream=st)
             pos = first % eng.N                                       # windows start at multiples of the window: no wrap inside
-            eng.get_yout(stage, pos, count)
+            eng.get_yout(stage, pos, count, stream=st)
             for s, u, a, m in live:
                 outs[u][skip[u] + a:skip[u] + a + m].copy_(stage[s, pos:pos + m])
             if ev:
@@ -1083,3 +1119,88 @@ class NVWaveNet:
             timing["produce_s"] = sum(events[i].elapsed_time(events[i + 1]) for i in range(0, len(events), 3)) / 1e3
             timing["score_s"] = sum(events[i + 1].elapsed_time(events[i + 2]) for i in range(0, len(events), 3)) / 1e3
         return logp
+
+
+def group_models(plan, lengths, models, first, count, group, slots):
+    """The model of each of the ceil(slots / group) slot groups in the window [first, first + count) of a plan_slots schedule
+    with `models`: that of the group's utterances live in the window, 0 for a group with none."""
+    table = [0] * ((slots + group - 1) // group)
+    for u, (s, start) in enumerate(plan):
+        if start < first + count and start + lengths[u] > first:
+            table[s // group] = models[u]
+    return table
+
+
+class ModelSet:
+    """Multi-model serving: several NVWaveNets of one shape (one voice each, say) served by one engine, each group of its slots
+    generating with the weights of the utterance it holds (nvwn_set_model, DESIGN.md §6).  The set owns its engines, one per
+    (slots, window, precision), each holding every net as a model (net m is model m); close() frees them."""
+
+    def __init__(self, nets):
+        nets = list(nets)
+        if not nets:
+            raise AssertionError("ModelSet needs at least one NVWaveNet")
+        shape = lambda n: (n.R, n.S, n.A, n.num_layers, n.max_dilation, bool(n.use_embed_tanh))
+        if any(shape(n) != shape(nets[0]) for n in nets):
+            raise AssertionError(f"the nets of a ModelSet share R, S, A, layers, max_dilation and use_embed_tanh; got {[shape(n) for n in nets]}")
+        from .infer import MAX_MODELS
+        if len(nets) > MAX_MODELS:
+            raise AssertionError(f"a ModelSet holds at most {MAX_MODELS} nets; got {len(nets)}")
+        self.nets = nets
+        self._engines = {}
+
+    def _engine(self, slots, window, fp16):
+        """The engine of (slots, window, precision), holding net m as model m (made on first use)."""
+        key = (slots, window, bool(fp16))
+        eng = self._engines.get(key)
+        if eng is None:
+            eng = self.nets[0]._new_engine(slots, window, fp16)
+            for m, net in enumerate(self.nets[1:], 1):
+                donor = net._new_engine(1, 1, fp16)
+                try:
+                    eng.set_model(m, donor)
+                finally:
+                    donor.close()
+            self._engines[key] = eng
+        return eng
+
+    def infer_many(self, models, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None):
+        """NVWaveNet.infer_many over several models: utterance u runs net models[u].  One engine of `slots` slots and `window`
+        samples serves the whole queue; its slots are in groups of eng.model_group that run one model at a time, scheduled by
+        plan_slots(..., models, group), and before each window's restarts the engine's group table is set to the models of the
+        window's live utterances.  Returns int32 CUDA tensors [n_u], each bit-identical to
+        nets[models[u]].infer(cond_u[:, None], Impl.AUTO, seed=seeds[u], fp16=fp16)[0].  timing: a dict, or None; if given,
+        receives the GPU seconds spent in restarts and per-slot uploads ("restart_upload_s") and in generation ("generate_s")."""
+        net = self.nets[0]
+        if not (len(models) == len(cond_inputs) == len(seeds)):
+            raise AssertionError(f"{len(models)} models, {len(cond_inputs)} utterances and {len(seeds)} seeds")
+        if any(int(m) != m or not 0 <= m < len(self.nets) for m in models):
+            raise AssertionError(f"every model index is in [0, {len(self.nets)})")
+        for c in cond_inputs:
+            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * net.R, net.num_layers):
+                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
+        lengths = [int(c.size(2)) for c in cond_inputs]
+        models = [int(m) for m in models]
+        eng = self._engine(slots, window, fp16)
+        group = eng.model_group
+        plan = plan_slots(lengths, slots, window, models, group)
+        windows = _windows(plan, lengths, window)
+        _reset(eng)
+        st = torch.cuda.current_stream()
+
+        def tables(k):
+            first, count, _, _ = windows[k]
+            eng.set_group_models(group_models(plan, lengths, models, first, count, group, slots), stream=st)
+
+        condition = net._condition_slots(eng, windows, cond_inputs, [0] * len(lengths))
+        outs, events = net._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, before=tables)
+        torch.cuda.synchronize()
+        if timing is not None:
+            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
+            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
+        return outs
+
+    def close(self):
+        for eng in self._engines.values():
+            eng.close()
+        self._engines = {}
