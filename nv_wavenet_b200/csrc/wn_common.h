@@ -114,9 +114,10 @@ struct WnFamily {
     // History writers (priming from a scoring stream, DESIGN.md §5.4).  put_history writes fp16 src [n][batch][R] (device), the
     // values x_layer[t] of absolute times [t_first, t_first + n), n <= maxDil + 1, rows 0..batch-1, into ring slot t mod (maxDil+1)
     // of that layer, where a run of batch_size = batch reads them, and no other byte; get_history (debug) reads the whole ring back
-    // as fp32 [(maxDil+1)][L][batch][R] (device), slot by slot, at that stride.
+    // as fp32 [(maxDil+1)][L][batch][R] (device), slot by slot, at that stride, or with rows_dev (device, batch rows in [0, c.B))
+    // those rows at the engine's batch stride.
     cudaError_t (*put_history)(const WnConfig& c, void* ring, const __half* src, int layer, long long t_first, int n, int batch, cudaStream_t stream);
-    cudaError_t (*get_history)(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream);
+    cudaError_t (*get_history)(const WnConfig& c, float* dst, const void* ring, int batch, const int* rows_dev, cudaStream_t stream);
     // Per-slot history writers and reader (priming single slots, parking and resuming them, DESIGN.md §6), at the engine's batch
     // stride, for absolute times t that may be negative, in ring slot ((t mod M) + M) mod M, M = maxDil + 1.  A row's values are
     // in the ring's element type (fp16 on NVWN_FP16 engines, else fp32) in device memory: the value of time t_first + j of source

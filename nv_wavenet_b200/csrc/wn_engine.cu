@@ -1854,9 +1854,28 @@ int nvwn_debug_get_history(nvwn_engine* e, float* out, int batch)
     const size_t n = (size_t)(e->maxDil + 1) * e->L * batch * e->R;
     DevBuf<float> tmp;
     CK(tmp.alloc(n * sizeof(float)));
-    cudaError_t ce = e->family->get_history(*e, tmp, e->ring, batch, 0);
+    cudaError_t ce = e->family->get_history(*e, tmp, e->ring, batch, nullptr, 0);
     if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, n * sizeof(float), cudaMemcpyDefault);
     if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_history: ") + cudaGetErrorString(ce));
+    return 0;
+}
+
+// debug only (not part of the public ABI): rows rows[0..n) (host memory; distinct, in [0, B)) of every history-ring entry, as fp32
+// [(maxDil+1)][L][n][R] in slot order: what nvwn_debug_get_history reads for those rows, without reading back a whole large ring
+int nvwn_debug_get_history_rows(nvwn_engine* e, float* out, const int* rows, int n)
+{
+    if (!e || !out) return fail(NVWN_EINVAL, "nvwn_debug_get_history_rows: NULL argument");
+    int rc = check_slots(e, "nvwn_debug_get_history_rows", rows, n);
+    if (rc != 0) return rc;
+    const size_t count = (size_t)(e->maxDil + 1) * e->L * n * e->R;
+    DevBuf<int> rows_dev;
+    DevBuf<float> tmp;
+    CK(rows_dev.alloc(n * sizeof(int)));
+    CK(tmp.alloc(count * sizeof(float)));
+    cudaError_t ce = cudaMemcpy(rows_dev, rows, n * sizeof(int), cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess) ce = e->family->get_history(*e, tmp, e->ring, n, rows_dev, 0);
+    if (ce == cudaSuccess) ce = cudaMemcpy(out, tmp, count * sizeof(float), cudaMemcpyDefault);
+    if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_debug_get_history_rows: ") + cudaGetErrorString(ce));
     return 0;
 }
 

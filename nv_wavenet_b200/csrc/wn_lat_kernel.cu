@@ -341,6 +341,17 @@ template <int TR> __device__ __forceinline__ uint4 own_rows(uint4 v, bool hi)
     return make_uint4(hi ? v.y : v.x, 0u, hi ? v.w : v.z, 0u);
 }
 
+// byte offset of history-ring row `row` (= slot x L + layer) of `rstride` bytes.  A ring of at most 4 GiB runs the kernels' WIDE = false
+// instantiations: every row starts below 2^32 bytes, so the 32-bit product is exact, and it is the form the step loop is fastest
+// with (the 64-bit forms tried measured 0.5-6 % slower at C3, B = 64, H100 80GB HBM3 at 700 W).  A larger ring (C3 from 3 265
+// utterances, L64 maxDil 2048 from 256) runs WIDE = true, whose offsets are 64-bit.
+template <bool WIDE> __device__ __forceinline__ size_t ring_off(uint32_t row, uint32_t rstride)
+{
+    return WIDE ? (size_t)row * rstride : (size_t)(row * rstride);
+}
+// WIDE for a ring of `ntiles` tiles per entry (LatLayout::ring_bytes) past 4 GiB
+static bool lat_ring_wide(int maxDil, int L, int ntiles) { return (size_t)(maxDil + 1) * L * ntiles * 2048 > ((size_t)1 << 32); }
+
 // feedback state of the tile ([TR] current index, [TR] previous index) of utterances ub .. ub + TR - 1 -> yCur / yPrev
 template <int TR = TU>
 __device__ __forceinline__ void store_ys(const WnParams& p, int B, const int* ys, int ub, int tid)
@@ -349,10 +360,10 @@ __device__ __forceinline__ void store_ys(const WnParams& p, int B, const int* ys
 }
 // this thread's values of x (fp16) -> the x exchange tile and row `row` (= history slot x L + layer) of the history ring.  The
 // ring keeps the 16-row A-fragment order; an 8-row tile writes only its rows' words (`gring` points at them).
-template <int TR = TU>
+template <int TR = TU, bool WIDE = false>
 __device__ __forceinline__ void store_x(const float (&x)[4], uint32_t xtile, unsigned char* gring, uint32_t row, uint32_t rstride, int w)
 {
-    unsigned char* gp = gring + (size_t)(row * rstride) + (w >> 1) * 512 + (w & 1) * 8;
+    unsigned char* gp = gring + ring_off<WIDE>(row, rstride) + (w >> 1) * 512 + (w & 1) * 8;
     const uint32_t x01 = pack_h2(x[0], x[1]);
     if (TR == TU) {
         const uint32_t x23 = pack_h2(x[2], x[3]);
@@ -408,13 +419,13 @@ __device__ __forceinline__ void hmma_res(float (&ra)[4], float (&rb)[4], const u
     hmma(ra, ha[1], bw0.z, bw0.w); hmma(rb, ha[3], bw1.z, bw1.w);
 }
 // x' = ((ra + rb) + Bres) + x; below the last layer x' goes to the x tile and history ring row `row` (8-row tiles: row g only)
-template <int TR = TU>
+template <int TR = TU, bool WIDE = false>
 __device__ __forceinline__ void residual(float (&x)[4], const float (&ra)[4], const float (&rb)[4], float2 br, bool store, uint32_t xtile,
                                          unsigned char* gring, uint32_t row, uint32_t rstride, int w)
 {
     x[0] = ((ra[0] + rb[0]) + br.x) + x[0]; x[1] = ((ra[1] + rb[1]) + br.y) + x[1];
     if (TR == TU) { x[2] = ((ra[2] + rb[2]) + br.x) + x[2]; x[3] = ((ra[3] + rb[3]) + br.y) + x[3]; }
-    if (store) store_x<TR>(x, xtile, gring, row, rstride, w);
+    if (store) store_x<TR, WIDE>(x, xtile, gring, row, rstride, w);
 }
 template <bool DUMP>
 __device__ __forceinline__ void dump_xt(const WnParams& p, int B, int l, int b0, int b1, int cw, const float (&x)[4])
@@ -492,7 +503,7 @@ __device__ __forceinline__ void lat_producer(const LatCta& c, int& trn)
 }
 
 // the eight compute warps
-template <int S, bool DUMP, bool TRC>
+template <int S, bool DUMP, bool TRC, bool WIDE>
 __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int ntiles_alloc)
 {
     using C = Cfg<S>;
@@ -547,7 +558,7 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
                 mbar_arrive(s_pfull + 8 * slot3);
             } else {
                 int sl = itp.slot - d; if (sl < 0) sl += slots;
-                cp_async16(dst, gring - lane16 + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
+                cp_async16(dst, gring - lane16 + ring_off<WIDE>(sl * L + itp.l, rstride) + (size_t)(w * 32 + lane) * 16);
                 cp_async_arrive_noinc(s_pfull + 8 * slot3);
             }
         }
@@ -661,7 +672,7 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
             const uint4 bw0 = lds128(p2 + o_res), bw1 = lds128(p2 + o_res + 512);
             hmma_res(ra, rb, ha, bw0, bw1);
         }
-        residual(xres, ra, rb, br, l + 1 < L, sm + C::O_XBUF + xchg, gring, (uint32_t)(it0.slot * L + l + 1), rstride, w);
+        residual<TU, WIDE>(xres, ra, rb, br, l + 1 < L, sm + C::O_XBUF + xchg, gring, (uint32_t)(it0.slot * L + l + 1), rstride, w);
         if (tid == 0) TRACE(0, 14);
         dump_xt<DUMP>(p, B, l, b0, b1, cw, xres);
         // ---- while the other warps finish their part of x': skip += Wskip.h   (biases are added once, after the last layer)
@@ -720,7 +731,7 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
             }
             const uint32_t x01 = pack_h2(xres[0], xres[1]), x23 = pack_h2(xres[2], xres[3]);
             sts64(sm + C::O_XBUF + xchg, x01, x23);
-            stg_v2(gring + (size_t)((uint32_t)(it0.slot * L) * rstride) + jw * 512 + hw * 8, x01, x23);
+            stg_v2(gring + ring_off<WIDE>(it0.slot * L, rstride) + jw * 512 + hw * 8, x01, x23);
             // previous-index rows of the NEXT sample (= this sample's current index): global -> shared, asynchronously
             const unsigned char* ep = static_cast<const unsigned char*>(c.embPrev);
             const uint32_t en = sm + C::O_EPBUF + (epar ^ 1) * (TU * EROW * 4);
@@ -888,7 +899,8 @@ __device__ __forceinline__ void lat_compute(const LatCta& c, int& trn, const int
 // DUMP: write the last-sample activations (the host runs the final sample of a dumping launch with this variant).
 // TRC:  record the clock64 timeline (debug; tools/lat_trace.py).
 // MODELS: p.group_model is set, and the tile's weights are its group's model's (DESIGN.md §6).
-template <int S, bool DUMP, bool TRC, bool MODELS>
+// WIDE: the history ring passes 4 GiB, and its offsets are formed in 64 bits (ring_off).
+template <int S, bool DUMP, bool TRC, bool MODELS, bool WIDE>
 __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const unsigned char* __restrict__ img0, const int ntiles_alloc)
 {
     using C = Cfg<S>;
@@ -936,7 +948,7 @@ __global__ void __launch_bounds__(NT, 1) wn_lat_kernel(const WnParams p, const u
     if (warp == NCW) {
         if (lane == 0) lat_producer<S, TRC>(c, trn);
     } else {
-        lat_compute<S, DUMP, TRC>(c, trn, ntiles_alloc);
+        lat_compute<S, DUMP, TRC, WIDE>(c, trn, ntiles_alloc);
     }
 }
 #undef TRACE
@@ -1241,7 +1253,7 @@ __device__ __forceinline__ void out_half(const ClusterCta& c, int& trn, const in
 }
 
 // ===================================================================================== chain CTA
-template <int S, int TR, bool DUMP, bool TRC>
+template <int S, int TR, bool DUMP, bool TRC, bool WIDE>
 __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
 {
     using C = Cfg<S>;
@@ -1378,7 +1390,7 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
 #pragma unroll
                     for (int i = 0; i < (TR == TU ? 4 : 2); i++) xres[i] = wn::tanhf_fast(xres[i]);
                 }
-                store_x<TR>(xres, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L), rstride, w);
+                store_x<TR, WIDE>(xres, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L), rstride, w);
                 cp_async4(en + (g * EROW + 4 * w + t4) * 4, ep + (size_t)yc0 * 128 + (4 * w + t4) * 4);
                 if (TR == TU) cp_async4(en + ((g + 8) * EROW + 4 * w + t4) * 4, ep + (size_t)yc1 * 128 + (4 * w + t4) * 4);
                 cp_async_commit();                         // landed long before the next sample starts (waited for at the end of this one)
@@ -1419,7 +1431,7 @@ __device__ __forceinline__ void chain_cta(const ClusterCta& c, int& trn)
                 if (n + 1 < (uint32_t)nsteps) load_ap(n + 1, l + 1 < L ? l + 1 : 0);
                 float ra[4] = {0.f, 0.f, 0.f, 0.f}, rb[4] = {0.f, 0.f, 0.f, 0.f};
                 hmma_res(ra, rb, ha, bw0, bw1);
-                residual<TR>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
+                residual<TR, WIDE>(xres, ra, rb, br, l + 1 < L, sm + M::C_XBUF + xchg, gring + lane16, (uint32_t)(it0.slot * L + l + 1), rstride, w);
                 // after the x store, which the x barrier waits for, so that the store is not queued behind these loads (placed right
                 // after the res HMMAs, the layer step measured slower: DESIGN §5.1b)
                 if (M::WCUR_AHEAD) load_wcur(n + 1);
@@ -1660,7 +1672,7 @@ __device__ __forceinline__ void tail_cta(const ClusterCta& c, int& trn)
 // ===================================================================================== prep CTA
 // (Bh + Lh) + Wprev . x[t-d] of every step, as far ahead of the chain CTA as its NAP tile buffers allow.  Nothing here depends on
 // the current sample: the history it reads was written by the chain CTA at least L - 9 steps earlier (wn_launch_lat asks for L >= 12).
-template <int S, int TR, bool DUMP, bool TRC>
+template <int S, int TR, bool DUMP, bool TRC, bool WIDE>
 __device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
 {
     using C = Cfg<S>;
@@ -1725,7 +1737,7 @@ __device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
                     mbar_arrive(s_pfull + 8 * slot);
                 } else {
                     int sl = itp.slot - d; if (sl < 0) sl += slots;
-                    cp_async16(dst, gring + (size_t)((uint32_t)(sl * L + itp.l) * rstride) + (size_t)(w * 32 + lane) * 16);
+                    cp_async16(dst, gring + ring_off<WIDE>(sl * L + itp.l, rstride) + (size_t)(w * 32 + lane) * 16);
                     cp_async_arrive_noinc(s_pfull + 8 * slot);
                 }
             }
@@ -1794,7 +1806,8 @@ __device__ __forceinline__ void prep_cta(const ClusterCta& c, int& trn)
 }
 
 // MODELS: p.group_model is set, and the cluster's weights are its group's model's (DESIGN.md §6).
-template <int S, int TR, bool DUMP, bool TRC, bool MODELS>
+// WIDE: the history ring passes 4 GiB, and its offsets are formed in 64 bits (ring_off).
+template <int S, int TR, bool DUMP, bool TRC, bool MODELS, bool WIDE>
 __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const unsigned char* __restrict__ img0, const int ntiles_alloc)
 {
     // debug timeline (tools/lat_trace.py, TRACE2): role = cluster rank (0 chain, 1 tail, 2 prep), thread 0 of each CTA of the first cluster
@@ -1884,9 +1897,9 @@ __global__ void __launch_bounds__(NTC, 1) wn_lat2_kernel(const WnParams p, const
     const ClusterCta c{p, img, gw.at<void>(p.embPrev), im, smem_raw, sm, L, B, tid, crank, ub, tile, hw4, slots, t_begin, t_end, ntiles_alloc, gbias,
                        s_full, s_empty, s_pfull, s_hfull, s_hfree, s_yfull, s_apfull, s_apfree, s_ob0full, s_ob0free, s_ob1full, s_ob1free, s_lfull, s_lfree,
                        ys, w, lane, g, t4, b0, b1, v0, v1, lane16, xchg, trc, tr_t};
-    if (is_chain) chain_cta<S, TR, DUMP, TRC>(c, trn);
+    if (is_chain) chain_cta<S, TR, DUMP, TRC, WIDE>(c, trn);
     else if (is_tail) tail_cta<S, TR, DUMP, TRC>(c, trn);
-    else prep_cta<S, TR, DUMP, TRC>(c, trn);
+    else prep_cta<S, TR, DUMP, TRC, WIDE>(c, trn);
     // nobody leaves while the peer may still write into this CTA's shared memory or arrive on its barriers
     cluster_sync_all();
 }
@@ -1920,13 +1933,13 @@ static cudaError_t wn_lat_pack(void* image, const WnParams& p, cudaStream_t stre
 // store / history ring were laid out for
 using LatGo = cudaError_t (*)(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream);
 
-template <int S, bool DUMP, bool TRC, bool MODELS>
+template <int S, bool DUMP, bool TRC, bool MODELS, bool WIDE>
 static cudaError_t lat_go(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
 {
     const size_t smem = Cfg<S>::SMEM;
-    const cudaError_t e = cudaFuncSetAttribute(wn_lat_kernel<S, DUMP, TRC, MODELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t e = cudaFuncSetAttribute(wn_lat_kernel<S, DUMP, TRC, MODELS, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    wn_lat_kernel<S, DUMP, TRC, MODELS><<<tiles, NT, smem, stream>>>(p, im8, ntiles_alloc);
+    wn_lat_kernel<S, DUMP, TRC, MODELS, WIDE><<<tiles, NT, smem, stream>>>(p, im8, ntiles_alloc);
     return cudaGetLastError();
 }
 
@@ -1945,14 +1958,14 @@ static cudaLaunchConfig_t lat2_config(int clusters, cudaStream_t stream, cudaLau
     cfg.numAttrs = 1;
     return cfg;
 }
-template <int S, int TR, bool DUMP, bool TRC, bool MODELS>
+template <int S, int TR, bool DUMP, bool TRC, bool MODELS, bool WIDE>
 static cudaError_t lat2_go(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream)
 {
-    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, TR, DUMP, TRC, MODELS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(wn_lat2_kernel<S, TR, DUMP, TRC, MODELS, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM);
     if (e != cudaSuccess) return e;
     cudaLaunchAttribute at;
     const cudaLaunchConfig_t cfg = lat2_config<S, TR>(clusters, stream, at);
-    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, TR, DUMP, TRC, MODELS>, p, im8, ntiles_alloc);
+    e = cudaLaunchKernelEx(&cfg, wn_lat2_kernel<S, TR, DUMP, TRC, MODELS, WIDE>, p, im8, ntiles_alloc);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 // how many clusters the device runs at once (a cluster needs NCL SMs of one GPC: fewer than 132 / NCL fit on an H100); 0 if the query fails
@@ -1961,11 +1974,11 @@ static int lat2_max_clusters()
 {
     static int cached = -1;
     if (cached >= 0) return cached;
-    if (cudaFuncSetAttribute(wn_lat2_kernel<S, TR, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
+    if (cudaFuncSetAttribute(wn_lat2_kernel<S, TR, false, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CfgC<S, TR>::SMEM) != cudaSuccess) { cudaGetLastError(); return cached = 0; }
     cudaLaunchAttribute at;
     const cudaLaunchConfig_t cfg = lat2_config<S, TR>(48, 0, at);
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, TR, false, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
+    if (cudaOccupancyMaxActiveClusters(&n, wn_lat2_kernel<S, TR, false, false, false, false>, &cfg) != cudaSuccess) { cudaGetLastError(); n = 0; }
     return cached = n;
 }
 
@@ -1981,23 +1994,37 @@ static cudaError_t lat_launch_split(const WnParams& p, LatGo plain, LatGo trace,
     if (e == cudaSuccess && p.dump) e = dump(tail, im8, tiles, ntiles_alloc, stream);
     return e;
 }
+template <int S, bool WIDE>
+static cudaError_t lat_launch_W(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream)
+{
+    if (p.group_model)
+        return lat_launch_split(p, lat_go<S, false, false, true, WIDE>, lat_go<S, false, true, true, WIDE>, lat_go<S, true, false, true, WIDE>, im8, tiles,
+                                ntiles_alloc, stream);
+    return lat_launch_split(p, lat_go<S, false, false, false, WIDE>, lat_go<S, false, true, false, WIDE>, lat_go<S, true, false, false, WIDE>, im8, tiles,
+                            ntiles_alloc, stream);
+}
 template <int S>
 static cudaError_t lat_launch_S(const WnParams& p, const unsigned char* im8, int tiles, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
 {
     *smem_out = Cfg<S>::SMEM;
+    return lat_ring_wide(p.maxDil, p.L, ntiles_alloc) ? lat_launch_W<S, true>(p, im8, tiles, ntiles_alloc, stream)
+                                                      : lat_launch_W<S, false>(p, im8, tiles, ntiles_alloc, stream);
+}
+template <int S, int TR, bool WIDE>
+static cudaError_t lat2_launch_W(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream)
+{
     if (p.group_model)
-        return lat_launch_split(p, lat_go<S, false, false, true>, lat_go<S, false, true, true>, lat_go<S, true, false, true>, im8, tiles, ntiles_alloc, stream);
-    return lat_launch_split(p, lat_go<S, false, false, false>, lat_go<S, false, true, false>, lat_go<S, true, false, false>, im8, tiles, ntiles_alloc, stream);
+        return lat_launch_split(p, lat2_go<S, TR, false, false, true, WIDE>, lat2_go<S, TR, false, true, true, WIDE>, lat2_go<S, TR, true, false, true, WIDE>, im8,
+                                clusters, ntiles_alloc, stream);
+    return lat_launch_split(p, lat2_go<S, TR, false, false, false, WIDE>, lat2_go<S, TR, false, true, false, WIDE>, lat2_go<S, TR, true, false, false, WIDE>,
+                            im8, clusters, ntiles_alloc, stream);
 }
 template <int S, int TR>
 static cudaError_t lat2_launch_S(const WnParams& p, const unsigned char* im8, int clusters, int ntiles_alloc, cudaStream_t stream, size_t* smem_out)
 {
     *smem_out = CfgC<S, TR>::SMEM;
-    if (p.group_model)
-        return lat_launch_split(p, lat2_go<S, TR, false, false, true>, lat2_go<S, TR, false, true, true>, lat2_go<S, TR, true, false, true>, im8, clusters,
-                                ntiles_alloc, stream);
-    return lat_launch_split(p, lat2_go<S, TR, false, false, false>, lat2_go<S, TR, false, true, false>, lat2_go<S, TR, true, false, false>, im8, clusters,
-                            ntiles_alloc, stream);
+    return lat_ring_wide(p.maxDil, p.L, ntiles_alloc) ? lat2_launch_W<S, TR, true>(p, im8, clusters, ntiles_alloc, stream)
+                                                      : lat2_launch_W<S, TR, false>(p, im8, clusters, ntiles_alloc, stream);
 }
 
 template <int TR>

@@ -180,16 +180,18 @@ __global__ void wn_clear_times_kernel(size_t total, WnConfig c, void* ring, long
     }
 }
 
-// every ring entry -> fp32 [entries][batch][R], at the batch stride `batch`
+// every ring entry -> fp32 [entries][batch][R]: rows 0..batch-1 at the batch stride `batch`, or (rows not NULL) rows rows[r] at the
+// engine's batch stride
 template <class Lay>
-__global__ void wn_get_history_kernel(size_t total, WnConfig c, float* __restrict__ dst, const void* ring, int batch)
+__global__ void wn_get_history_kernel(size_t total, WnConfig c, float* __restrict__ dst, const void* ring, int batch, const int* __restrict__ rows)
 {
     constexpr int U = Lay::RING_UNIT;
     const int units = c.R / U, lg = wn_log2(units);
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const size_t row = i >> lg;                                   // e * batch + b
-        reinterpret_cast<WnVec<float, U>*>(dst)[i] =
-            wn_vec_cast<float>(wn_load(Lay::ring_unit(c, const_cast<void*>(ring), row / batch, batch, (int)(row % batch), (int)i & (units - 1))));
+        const size_t row = i >> lg;                                   // e * batch + r
+        const int r = (int)(row % batch);
+        reinterpret_cast<WnVec<float, U>*>(dst)[i] = wn_vec_cast<float>(
+            wn_load(Lay::ring_unit(c, const_cast<void*>(ring), row / batch, rows ? c.B : batch, rows ? rows[r] : r, (int)i & (units - 1))));
     }
 }
 
@@ -241,7 +243,8 @@ cudaError_t wn_clear_times(const WnConfig& c, void* ring, long long t_first, int
     return wn_layout_launch(wn_clear_times_kernel<Lay>, (size_t)n_t * c.L * c.B * (c.R / Lay::RING_UNIT), stream, c, ring, t_first);
 }
 template <class Lay>
-cudaError_t wn_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
+cudaError_t wn_get_history(const WnConfig& c, float* dst, const void* ring, int batch, const int* rows_dev, cudaStream_t stream)
 {
-    return wn_layout_launch(wn_get_history_kernel<Lay>, (size_t)(c.maxDil + 1) * c.L * batch * (c.R / Lay::RING_UNIT), stream, c, dst, ring, batch);
+    return wn_layout_launch(wn_get_history_kernel<Lay>, (size_t)(c.maxDil + 1) * c.L * batch * (c.R / Lay::RING_UNIT), stream, c, dst, ring, batch,
+                            rows_dev);
 }

@@ -721,9 +721,9 @@ cudaError_t plain_convert_rows(const WnConfig& c, void* store, const float* src,
     return c.dtype == NVWN_FP16 ? wn_convert_rows<PlainH>(c, store, src, rows_dev, n, first_pos, num_pos, stream)
                                 : wn_convert_rows<PlainF>(c, store, src, rows_dev, n, first_pos, num_pos, stream);
 }
-cudaError_t plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, cudaStream_t stream)
+cudaError_t plain_get_history(const WnConfig& c, float* dst, const void* ring, int batch, const int* rows_dev, cudaStream_t stream)
 {
-    return c.dtype == NVWN_FP16 ? wn_get_history<PlainH>(c, dst, ring, batch, stream) : wn_get_history<PlainF>(c, dst, ring, batch, stream);
+    return c.dtype == NVWN_FP16 ? wn_get_history<PlainH>(c, dst, ring, batch, rows_dev, stream) : wn_get_history<PlainF>(c, dst, ring, batch, rows_dev, stream);
 }
 cudaError_t plain_put_history_rows(const WnConfig& c, void* ring, const void* src, const int* src_rows_dev, size_t row_pitch, size_t time_pitch,
                                    const int* rows_dev, int n, int layer, long long t_first, int n_t, cudaStream_t stream)
