@@ -184,6 +184,94 @@ def _check_window(window):
         raise AssertionError(f"window must be at least 1; got {window}")
 
 
+def _check_rows(what, name, rows, window):
+    """The rows (`name`: slots or batch_size) and window of an engine a call makes: both at least 1."""
+    if rows < 1 or window is None or window < 1:
+        raise AssertionError(f"{what}: need {name} >= 1 and window >= 1; got {rows}, {window}")
+
+
+def _check_frames(features, C):
+    """The frame counts T_u of per-utterance mel frames [C][T_u], each T_u >= 1."""
+    shapes = [tuple(int(v) for v in f.shape) for f in features]
+    for s in shapes:
+        if len(s) != 2 or s[0] != C or s[1] < 1:
+            raise AssertionError(f"each utterance's frames are [{C}][T] with T >= 1; got {s}")
+    return [s[1] for s in shapes]
+
+
+class _Timer:
+    """GPU time between named points of the work on a stream, for a `timing` dict (None: timing is off).  mark(name, stream)
+    records an event there when timing is on and does nothing (no event) when it is off; seconds(start, end) sums, over the marks
+    in order, the time from the i-th `start` mark to the i-th `end` mark; report(key=(start, end), ...) puts those sums into the
+    dict.  Read it after a synchronise."""
+
+    def __init__(self, timing):
+        self.on, self.timing, self._marks = timing is not None, timing, {}
+
+    def mark(self, name, stream=None):
+        if self.on:
+            ev = torch.cuda.Event(enable_timing=True)
+            ev.record(stream)
+            self._marks.setdefault(name, []).append(ev)
+
+    def seconds(self, start, end):
+        return sum(a.elapsed_time(b) for a, b in zip(self._marks.get(start, ()), self._marks.get(end, ()))) / 1e3
+
+    def report(self, **spans):
+        if self.on:
+            self.timing.update({key: self.seconds(start, end) for key, (start, end) in spans.items()})
+
+
+def _score_prompt_group(eng, prompts, fill, at_end, **stream):
+    """One scoring stream on `eng` (W = eng.N samples) whose row j is prompts[j], int32 codes [P_j] on the device, rows by length.
+    It is scored in pieces that end at each distinct P_j and at multiples of W, each after fill(a, m) has put the conditioning of
+    samples [a, a + m) into the store; a row past its prompt's end is scored on code 128 and its results are unused.  At each
+    distinct P, at_end(rows) acts on the rows whose prompt ends there.  stream: stream=s to score on s, or nothing."""
+    ends = [int(p.numel()) for p in prompts]
+    codes = torch.full((len(prompts), ends[-1]), 128, dtype=torch.int32, device=prompts[0].device)
+    for j, p in enumerate(prompts):
+        codes[j, :ends[j]] = p
+    a, W = 0, eng.N
+    for end in sorted(set(ends)):
+        while a < end:
+            m = min(end - a, W - a % W)
+            fill(a, m)
+            eng.score_stream(codes[:, a:a + m], a, **stream)
+            a += m
+        at_end([j for j, P in enumerate(ends) if P == end])
+
+
+def _score_windows(windows, fill, score, timing):
+    """The window loop of the log_likelihood family: per window w, fill(*w) puts its conditioning into the store and score(*w)
+    scores it; then a synchronise.  timing: None, or a dict for the GPU seconds of fill ("produce_s") and of scoring ("score_s")."""
+    timer = _Timer(timing)
+    for w in windows:
+        timer.mark("fill")
+        fill(*w)
+        timer.mark("score")
+        score(*w)
+        timer.mark("done")
+    torch.cuda.synchronize()
+    timer.report(produce_s=("fill", "score"), score_s=("score", "done"))
+
+
+def _score_then_generate(eng, prompt, first, m, select, read):
+    """Samples [first, first + m) of a batch on `eng`, their conditioning already in the store: with a prompt [batch][P], the part
+    before P is scored and the engine primed at P; the rest, [g0, g0 + k), gets its selectors from select(g0, k), is generated
+    and read out by read(g0, k)."""
+    P, g0 = 0 if prompt is None else prompt.shape[1], first
+    if first < P:
+        g0 = min(first + m, P)
+        eng.score_stream(prompt[:, first:g0], first)
+        if g0 == P:
+            eng.prime_from_score()
+    k = first + m - g0
+    if k:
+        select(g0, k)
+        eng.run_stream(g0, k, eng.B)
+        read(g0, k)
+
+
 def check_prompt(what, prompt, rows, n, fp16, A):
     """Checks a prompt: int mu-law codes [P] (rows None) or [rows][P], 1 <= P < n (n None: no upper bound), each in [0, A), with
     fp16 set, since prompts are scored by the fp16 scorer.  Returns it as a tensor."""
@@ -246,6 +334,12 @@ class LiveSession:
         frames = frames.to(torch.float32) if isinstance(frames, torch.Tensor) else np.asarray(frames, np.float32)
         eng, n, done = self._eng, shape[2], 0
         ys, auds = [], []
+
+        def read(first, m):
+            ys.append(eng.get_yout_stream(torch.empty((eng.B, m), dtype=torch.int32, device=self.device), first, m))
+            if audio is not None:
+                auds.append(eng.get_audio_stream(first, m, int16=audio == "int16", saturate=saturate))
+
         while True:
             k = min(n - done, live_push_limit(self.frames, self.samples, self.ring_frames, self.upsample_window, self.stride))
             if k > 0:
@@ -257,19 +351,9 @@ class LiveSession:
             while self.samples < end:
                 first, m = self.samples, min(self.window, end - self.samples)
                 if first < P:
-                    m = min(m, P - first)
-                    eng.cond_producer_run_stream(first, m)
-                    eng.score_stream(self.prompt[:, first:first + m], first)
-                    self.samples += m
-                    if self.samples == P:
-                        eng.prime_from_score()
-                    continue
+                    m = min(m, P - first)                         # a piece is all prompt or all generated
                 eng.cond_producer_run_stream(first, m)
-                eng.set_selectors_random_stream(self.seed, first, m)
-                eng.run_stream(first, m, eng.B)
-                ys.append(eng.get_yout_stream(torch.empty((eng.B, m), dtype=torch.int32, device=self.device), first, m))
-                if audio is not None:
-                    auds.append(eng.get_audio_stream(first, m, int16=audio == "int16", saturate=saturate))
+                _score_then_generate(eng, self.prompt, first, m, lambda g0, k: eng.set_selectors_random_stream(self.seed, g0, k), read)
                 self.samples += m
             if done == n:
                 break
@@ -364,7 +448,7 @@ class LivePool:
         self.launches = self.parks = self.resumes = 0
         self._streams, self._waiting, self._next_id = {}, [], 0
         self._stage = None                              # yOut staging [B][N], allocated on the first launch
-        self._timed, self._save_ev, self._load_ev, self._prompt_ev = timed, [], [], []
+        self._timer = _Timer({} if timed else None)         # read by state_seconds and prompt_seconds
 
     def open(self, seed, prompt=None):
         """A new stream with selector key `seed`; returns its id.  It waits for frames.  prompt: None, or int mu-law codes [P], P >= 1
@@ -406,25 +490,15 @@ class LivePool:
                 self._waiting.remove(i)
             del self._streams[i]
 
-    def _timed_call(self, events, fn, *args):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if self._timed else None
-        if ev:
-            ev[0].record()
-        out = fn(*args)
-        if ev:
-            ev[1].record()
-            events.append(ev)
-        return out
-
     def state_seconds(self):
         """GPU seconds spent saving and loading slot states so far (timed pools; synchronises)."""
         torch.cuda.synchronize()
-        return tuple(sum(a.elapsed_time(b) for a, b in evs) / 1e3 for evs in (self._save_ev, self._load_ev))
+        return self._timer.seconds("save", "saved"), self._timer.seconds("load", "loaded")
 
     def prompt_seconds(self):
         """GPU seconds spent producing, scoring and saving prompts so far (timed pools; synchronises)."""
         torch.cuda.synchronize()
-        return sum(a.elapsed_time(b) for a, b in self._prompt_ev) / 1e3
+        return self._timer.seconds("prompt", "prompted")
 
     def _score_prompts(self):
         """Scores the waiting streams whose frames now cover their prompts, in groups of the scoring engine's rows
@@ -439,7 +513,9 @@ class LivePool:
             # on the device once, so a group's producer load copies no weights from the host
             self._network = tuple(torch.as_tensor(a).to(device=self.device, dtype=torch.float32).contiguous() for a in self._network)
         for group in plan_prompt_groups(ready, self._scorer_eng.B):
-            states = self._timed_call(self._prompt_ev, self._score_group, group)
+            self._timer.mark("prompt")
+            states = self._score_group(group)
+            self._timer.mark("prompted")
             for (i, P), state in zip(group, states):
                 s = self._streams[i]
                 s.state, s.position, s.started, s.prompt = state, P, True, None
@@ -452,28 +528,26 @@ class LivePool:
         rows' frames through the whole-batch producer; it is scored in pieces that end at each distinct P_j and at multiples of
         the window, rows past their prompt's end on code 128 (their results unused), and each row's state is saved where its prompt
         ends (nvwn_score_save_states, with the stream's seed).  Returns the states in group order."""
-        eng, W = self._scorer_eng, self._scorer_eng.N
+        eng = self._scorer_eng
         P_max = group[-1][1]
         F = prompt_frames(P_max, self.stride)
         feats = np.zeros((eng.B, self.channels, F), np.float32)
-        codes = torch.full((len(group), P_max), 128, dtype=torch.int32, device=self.device)
-        for j, (i, P) in enumerate(group):
+        for j, (i, _) in enumerate(group):
             s = self._streams[i]
             n = min(s.frames, F)
             feats[j, :, :n] = s.span(0, n)
-            codes[j, :P] = s.prompt
-        eng.cond_producer_load(feats, *self._network, self.stride)
-        states, a = [None] * len(group), 0
-        for end in sorted({P for _, P in group}):
-            while a < end:
-                m = min(end - a, W - a % W)
-                eng.cond_producer_run_stream(a, m)
-                eng.score_stream(codes[:, a:a + m], a)
-                a += m
-            done = [j for j, (_, P) in enumerate(group) if P == end]
-            saved = eng.score_save_states(done, [self._streams[group[j][0]].seed for j in done])
-            for k, j in enumerate(done):
-                states[j] = saved[k]
+        states = [None] * len(group)
+
+        def fill(a, m):
+            if a == 0:                          # the frames go in once, after the scorer has made its code rows
+                eng.cond_producer_load(feats, *self._network, self.stride)
+            eng.cond_producer_run_stream(a, m)
+
+        def save(rows):
+            for j, state in zip(rows, eng.score_save_states(rows, [self._streams[group[j][0]].seed for j in rows])):
+                states[j] = state
+
+        _score_prompt_group(eng, [self._streams[i].prompt for i, _ in group], fill, save)
         return states
 
     def step(self, audio=None, saturate=False):
@@ -498,7 +572,9 @@ class LivePool:
                                       if self._streams[i].prompt is None],
                                      eng.B, self.window, st)
         if park:
-            states = self._timed_call(self._save_ev, eng.save_slots, [resident[i].slot for i in park])
+            self._timer.mark("save")
+            states = eng.save_slots([resident[i].slot for i in park])
+            self._timer.mark("saved")
             for j, i in enumerate(park):
                 s = resident.pop(i)
                 s.state, s.slot = states[j], None
@@ -512,7 +588,10 @@ class LivePool:
             if new:
                 eng.restart_slots([b for _, b in new], [self._streams[i].seed for i, _ in new])
             if old:
-                self._timed_call(self._load_ev, eng.load_slots, [b for _, b in old], torch.stack([self._streams[i].state for i, _ in old]))
+                states = torch.stack([self._streams[i].state for i, _ in old])         # before the span: it times the load alone
+                self._timer.mark("load")
+                eng.load_slots([b for _, b in old], states)
+                self._timer.mark("loaded")
                 self.resumes += len(old)
             spans = []
             for i, b in place:
@@ -637,15 +716,12 @@ class NVWaveNet:
         prompt: None, or int mu-law codes [batch_size][P], P >= 1 (host or CUDA tensor), fp16 only: the utterances continue given
         audio.  The pushes then give infer(cond, seed=seed, fp16=True, window=window, prompt=prompt)[:, P:], bit for bit: the
         frames' first P samples are scored as they arrive, and generation starts at sample P once they all are."""
-        Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
-                                    "open_live")
-        if batch_size < 1 or window is None or window < 1:
-            raise AssertionError(f"open_live: need batch_size >= 1 and window >= 1; got {batch_size}, {window}")
+        Cc, up, network = self._cond_network("open_live", upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
+        _check_rows("open_live", "batch_size", batch_size, window)
         if prompt is not None:
             prompt = self._check_prompt("prompt", prompt, batch_size, None, fp16).to(device="cuda", dtype=torch.int32)
         eng = self._new_engine(batch_size, window, fp16)
-        eng.cond_producer_open_live(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride,
-                                    live_ring_frames(window, up, stride))
+        eng.cond_producer_open_live(*network, stride, live_ring_frames(window, up, stride))
         return LiveSession(eng, Cc, up, stride, seed, window, prompt)
 
     def open_live_pool(self, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, slots, window, fp16=False, timed=False):
@@ -657,15 +733,34 @@ class NVWaveNet:
         pool has an engine of its own, apart from the engines infer() and the other calls share.  timed: see LivePool.
         On fp16 pools LivePool.open takes a prompt; the pool then makes, on the first prompt, a scoring engine of `slots` rows and
         `window` samples with the same weights."""
-        Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
-                                    "open_live_pool")
-        if slots < 1 or window is None or window < 1:
-            raise AssertionError(f"open_live_pool: need slots >= 1 and window >= 1; got {slots}, {window}")
+        Cc, up, network = self._cond_network("open_live_pool", upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
+        _check_rows("open_live_pool", "slots", slots, window)
         eng = self._new_engine(slots, window, fp16)
-        cw = cond_weight.reshape(self.num_layers * 2 * self.R, Cc)
-        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cw, cond_bias, stride)
+        eng.cond_producer_set_weights(*network, stride)
         scorer = (lambda: self._new_engine(slots, window, True)) if fp16 else None
-        return LivePool(eng, Cc, up, stride, timed, scorer, (upsample_weight, upsample_bias, cw, cond_bias))
+        return LivePool(eng, Cc, up, stride, timed, scorer, network)
+
+    def _cond_network(self, what, upsample_weight, upsample_bias, cond_weight, cond_bias, stride):
+        """(C, window, network) of a conditioning network checked for this model (check_cond_network, its errors naming `what`),
+        network being (upsample_weight, upsample_bias, cond_weight [L*2R][C], cond_bias) as the producer calls take them."""
+        Cc, up = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
+                                    what)
+        return Cc, up, (upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias)
+
+    def _check_utterances(self, cond_inputs):
+        """The sample counts n_u of per-utterance conditioning [2R][L][n_u] (channels x num_layers x samples)."""
+        for c in cond_inputs:
+            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * self.R, self.num_layers):
+                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
+        return [int(c.size(2)) for c in cond_inputs]
+
+    def _gather(self, cond_inputs, count, rows, pieces):
+        """A store slab [count][L][rows][2R] of per-utterance conditioning [2R][L][n_u]: piece (row, u, a, o, m) puts samples
+        [a, a + m) of utterance u at positions [o, o + m) of its row; everything else is zero."""
+        lh = torch.zeros((count, self.num_layers, rows, 2 * self.R), dtype=torch.float32, device="cuda")
+        for j, u, a, o, m in pieces:
+            lh[o:o + m, :, j].copy_(cond_inputs[u][:, :, a:a + m].permute(2, 1, 0))
+        return lh
 
     def _cond_size(self, cond_input):
         """(batch, samples) of conditioning channels x batch x num_layers x samples."""
@@ -710,29 +805,22 @@ class NVWaveNet:
         window generated; without one (P = 0) every window is generated whole.  Selectors of the generated samples: Philox under
         `seed`, or the host draw `sel` placed at their positions."""
         batch_size, sample_count = samples.shape
-        window, P = eng.N, 0 if prompt is None else prompt.shape[1]
-        if P:
-            samples[:, :P] = prompt
-        for first in range(0, sample_count, window):
-            n = min(window, sample_count - first)
-            eng.set_conditioning(lh[first:first + n], 0, n)
-            g0 = first
-            if first < P:
-                g0 = min(first + n, P)
-                eng.score_stream(prompt[:, first:g0], first)
-                if g0 == P:
-                    eng.prime_from_score()
-            k = first + n - g0
-            if k == 0:
-                continue
+        window = eng.N
+        if prompt is not None:
+            samples[:, :prompt.shape[1]] = prompt
+
+        def select(g0, k):
             if sel is None:
                 eng.set_selectors_random_stream(seed, g0, k)
             else:
-                chunk = np.zeros(window * batch_size, np.float32)
-                chunk[(g0 - first) * batch_size:n * batch_size] = sel[g0 * batch_size:(first + n) * batch_size]
+                chunk, o = np.zeros(window * batch_size, np.float32), g0 % window
+                chunk[o * batch_size:(o + k) * batch_size] = sel[g0 * batch_size:(g0 + k) * batch_size]
                 eng.set_selectors(chunk)
-            eng.run_stream(g0, k, batch_size)
-            eng.get_yout_stream(samples[:, g0:g0 + k], g0, k)
+
+        for first in range(0, sample_count, window):
+            n = min(window, sample_count - first)
+            eng.set_conditioning(lh[first:first + n], 0, n)
+            _score_then_generate(eng, prompt, first, n, select, lambda g0, k: eng.get_yout_stream(samples[:, g0:g0 + k], g0, k))
 
     def infer_many(self, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None, prompts=None):
         """Continuous batching: generates a queue of utterances of different lengths through one engine of `slots` utterances and
@@ -750,73 +838,54 @@ class NVWaveNet:
         ("restart_upload_s"), in generation ("generate_s") and in scoring and priming prompts ("prime_s")."""
         if len(cond_inputs) != len(seeds):
             raise AssertionError(f"{len(cond_inputs)} utterances but {len(seeds)} seeds")
-        for c in cond_inputs:
-            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * self.R, self.num_layers):
-                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
-        lengths = [int(c.size(2)) for c in cond_inputs]
+        lengths = self._check_utterances(cond_inputs)
         prompts = self._slot_prompts(prompts, lengths, fp16)
         skip = [0 if p is None else int(p.numel()) for p in prompts]                  # samples before the generated ones
         plan = plan_slots([n - P for n, P in zip(lengths, skip)], slots, window)
         windows = _windows(plan, [n - P for n, P in zip(lengths, skip)], window)
         eng = self._engine(slots, window, fp16)
-        _reset(eng)
         st = torch.cuda.current_stream()
-        primes = []
+        timer = _Timer(timing)
 
         def prime(k):
-            # the prompted utterances starting at this boundary, by prompt length: scoring rows 0..g-1, in pieces that end at each
-            # distinct P_u and at multiples of the window (the store holds one window, free now that the last one was generated)
-            first, _, starting, _ = windows[k]
-            group = sorted((u for u in starting if prompts[u] is not None), key=lambda u: skip[u])
+            # the prompted utterances starting at this boundary, by prompt length, are the rows of one scoring stream through the
+            # engine's own conditioning store (free now that the last window was generated); each slot is primed from its row
+            group = sorted((u for u in windows[k][2] if prompts[u] is not None), key=lambda u: skip[u])
             if not group:
                 return
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if timing is not None else None
-            if ev:
-                ev[0].record()
-            g, a = len(group), 0
-            for end in sorted({skip[u] for u in group}):
-                while a < end:
-                    m = min(end - a, window - a % window)
-                    # rows whose prompt has ended are scored on padding (codes 128, zero conditioning); their results are unused
-                    lh = torch.zeros((m, self.num_layers, g, 2 * self.R), dtype=torch.float32, device="cuda")
-                    codes = torch.full((g, m), 128, dtype=torch.int32, device="cuda")
-                    for j, u in enumerate(group):
-                        e = min(skip[u], a + m)
-                        if e > a:
-                            lh[:e - a, :, j].copy_(cond_inputs[u][:, :, a:e].permute(2, 1, 0))
-                            codes[j, :e - a] = prompts[u][a:e]
-                    eng.set_conditioning_slots(lh, list(range(g)), a, stream=st)
-                    eng.score_stream(codes, a, stream=st)
-                    a += m
-                done = [j for j, u in enumerate(group) if skip[u] == end]
-                eng.prime_slots_from_score(done, [plan[group[j]][0] for j in done], [seeds[group[j]] for j in done], stream=st)
-            if ev:
-                ev[1].record()
-                primes.append(ev)
+            timer.mark("prime")
 
-        condition = self._condition_slots(eng, windows, cond_inputs, skip)
-        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, before=prime, prompts=prompts)
-        torch.cuda.synchronize()
-        if timing is not None:
-            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
-            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
-            timing["prime_s"] = sum(a.elapsed_time(b) for a, b in primes) / 1e3
+            def fill(a, m):
+                lh = self._gather(cond_inputs, m, len(group), [(j, u, a, 0, min(skip[u], a + m) - a) for j, u in enumerate(group) if skip[u] > a])
+                eng.set_conditioning_slots(lh, list(range(len(group))), a, stream=st)
+
+            def at_end(rows):
+                eng.prime_slots_from_score(rows, [plan[group[j]][0] for j in rows], [seeds[group[j]] for j in rows], stream=st)
+
+            _score_prompt_group(eng, [prompts[u] for u in group], fill, at_end, stream=st)
+            timer.mark("primed")
+
+        outs = self._serve_queue(eng, plan, windows, lengths, skip, cond_inputs, seeds, timer, prime, prompts)
+        timer.report(prime_s=("prime", "primed"))
         return outs
 
-    def _condition_slots(self, eng, windows, cond_inputs, skip):
-        """The condition(k) of _serve for expanded conditioning: window k's conditioning of its live slots goes into the engine.
-        Utterance u's generated samples read its conditioning from sample skip[u] on.  On the current stream."""
+    def _serve_queue(self, eng, plan, windows, lengths, skip, cond_inputs, seeds, timer, before, prompts=None):
+        """The queue of infer_many and ModelSet.infer_many once it is planned: the engine reset, then _serve with before(k) and
+        each window's conditioning of its live slots gathered from cond_inputs (utterance u's generated samples reading it from
+        sample skip[u] on).  timer: a _Timer that receives the GPU seconds of restarts and per-slot uploads ("restart_upload_s")
+        and of generation ("generate_s")."""
+        _reset(eng)
         st = torch.cuda.current_stream()
 
         def condition(k):
             first, count, _, live = windows[k]
             if live:
-                # this window's conditioning of the live slots, [count][L][slots][2R], zero past an utterance's end
-                lh = torch.zeros((count, self.num_layers, len(live), 2 * self.R), dtype=torch.float32, device="cuda")
-                for j, (_, u, a, m) in enumerate(live):
-                    lh[:m, :, j].copy_(cond_inputs[u][:, :, skip[u] + a:skip[u] + a + m].permute(2, 1, 0))
+                lh = self._gather(cond_inputs, count, len(live), [(j, u, skip[u] + a, 0, m) for j, (_, u, a, m) in enumerate(live)])
                 eng.set_conditioning_slots(lh, [s for s, _, _, _ in live], first, stream=st)
-        return condition
+
+        outs = self._serve(eng, plan, windows, lengths, skip, seeds, timer, condition, before=before, prompts=prompts)
+        timer.report(restart_upload_s=("condition", "launch"), generate_s=("launch", "done"))
+        return outs
 
     def _slot_prompts(self, prompts, lengths, fp16):
         """infer_many's prompts checked: per utterance None or int32 CUDA codes [P_u], 1 <= P_u < n_u, each in [0, A), and fp16 if any
@@ -840,27 +909,22 @@ class NVWaveNet:
         or torch tensors (CUDA ones are read in stream order).  timing: a dict, or None; if given, receives the GPU seconds of
         production on the side stream ("produce_s"), the time generation waited for it ("produce_wait_s"), of restarts and
         selectors ("restart_select_s") and of generation ("generate_s")."""
-        shp = lambda a: tuple(int(v) for v in a.shape)
         if len(features) != len(seeds):
             raise AssertionError(f"{len(features)} utterances but {len(seeds)} seeds")
-        Cc, _ = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
-                                   "infer_many_from_features")
-        lr = self.num_layers * 2 * self.R
-        for f in features:
-            if len(shp(f)) != 2 or shp(f)[0] != Cc or shp(f)[1] < 1:
-                raise AssertionError(f"each utterance's frames are [{Cc}][T] with T >= 1; got {shp(f)}")
-        lengths = [shp(f)[1] * stride for f in features]
+        Cc, _, network = self._cond_network("infer_many_from_features", upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
+        lengths = [T * stride for T in _check_frames(features, Cc)]
         # contiguous fp32 frames, made on the current stream before the side stream is ordered after it
         features = [f.to(torch.float32).contiguous() if isinstance(f, torch.Tensor) else np.ascontiguousarray(f, np.float32) for f in features]
         plan = plan_slots(lengths, slots, window)
         windows = _windows(plan, lengths, window)
         eng = self._engine(slots, 2 * window, fp16)
         _reset(eng)
-        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(lr, Cc), cond_bias, stride)
+        eng.cond_producer_set_weights(*network, stride)
 
         cur, side = torch.cuda.current_stream(), torch.cuda.Stream()
         side.wait_stream(cur)                                         # frames made on the current stream
-        ready, read, produced, keep = {}, {}, [], []
+        timer = _Timer(timing)
+        ready, read, keep = {}, {}, []
 
         def produce(k):
             # window k on the side stream, into the positions of window k - 2: after that window has been generated and read
@@ -869,17 +933,13 @@ class NVWaveNet:
             first, count, starting, live = windows[k]
             if k - 2 in read:
                 side.wait_event(read.pop(k - 2))
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)] if timing is not None else None
-            if ev:
-                ev[0].record(side)
+            timer.mark("produce", side)
             if starting:
                 keep.append(eng.cond_producer_set_slots([plan[u][0] for u in starting], [features[u] for u in starting],
                                                         [first] * len(starting), stream=side))
             if live:
                 eng.cond_producer_run_slots([s for s, _, _, _ in live], first, count, stream=side)
-            if ev:
-                ev[1].record(side)
-                produced.append(ev)
+            timer.mark("produced", side)
             ready[k] = torch.cuda.Event()
             ready[k].record(side)
 
@@ -892,59 +952,46 @@ class NVWaveNet:
             produce(k + 1)                                            # enqueued after window k's generation, which it overlaps
 
         produce(0)
-        outs, events = self._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, after)
-        torch.cuda.synchronize()
-        if timing is not None:
-            timing["produce_s"] = sum(a.elapsed_time(b) for a, b in produced) / 1e3
-            timing["produce_wait_s"] = sum(e[0].elapsed_time(e[1]) for e in events) / 1e3
-            timing["restart_select_s"] = sum(e[1].elapsed_time(e[2]) for e in events) / 1e3
-            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
+        outs = self._serve(eng, plan, windows, lengths, [0] * len(lengths), seeds, timer, condition, after)
+        timer.report(produce_s=("produce", "produced"), produce_wait_s=("condition", "restart"), restart_select_s=("restart", "launch"),
+                     generate_s=("launch", "done"))
         return outs
 
-    def _serve(self, eng, plan, windows, lengths, seeds, timed, condition, after=None, before=None, prompts=None):
+    def _serve(self, eng, plan, windows, lengths, skip, seeds, timer, condition, after=None, before=None, prompts=None):
         """The window loop of infer_many and infer_many_from_features on the current stream.  Per window k: before(k), which
         primes the prompted slots that start there; condition(k), which leaves the conditioning of the window's live slots in the
         engine or makes the stream wait for it; the restarts of the other slots whose utterance starts there; their selectors;
-        the launch; the outputs; then after(k).  prompts: None, or per utterance its prompt [P_u] (CUDA) or None: the output's
-        first P_u samples, generated ones after them (windows and lengths count generated samples; outputs have `lengths`).
-        Returns the outputs and, if timed, per window four events around those steps (before condition, restarts, launch, and
-        after the outputs)."""
-        prompts = prompts or [None] * len(lengths)
+        the launch; the outputs; then after(k); a synchronise at the end.  skip: per utterance the length P_u of its prompt, 0 for
+        none; prompts: None, or per utterance its prompt [P_u] (CUDA) or None: the output's first P_u samples, generated ones after
+        them (windows count generated samples; outputs have `lengths`).  Returns the outputs; `timer` (a _Timer) is marked per window before condition ("condition"), the restarts ("restart"), the
+        launch ("launch") and after the outputs ("done")."""
         outs = [torch.empty(n, dtype=torch.int32, device="cuda") for n in lengths]
-        skip = []
-        for o, p in zip(outs, prompts):
-            skip.append(0 if p is None else p.numel())
+        for o, p in zip(outs, prompts or ()):
             if p is not None:
                 o[:p.numel()].copy_(p)
         stage = torch.empty((eng.B, eng.N), dtype=torch.int32, device="cuda")
         st = torch.cuda.current_stream()
-        events = []
         for k, (first, count, starting, live) in enumerate(windows):
             if before is not None:
                 before(k)
-            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timed else None
-            if ev:
-                ev[0].record()
+            timer.mark("condition")
             condition(k)
-            if ev:
-                ev[1].record()
-            restart = [u for u in starting if prompts[u] is None]
+            timer.mark("restart")
+            restart = [u for u in starting if not skip[u]]
             if restart:
                 eng.restart_slots([plan[u][0] for u in restart], [seeds[u] for u in restart], stream=st)
             eng.set_selectors_random_slots(first, count, stream=st)
-            if ev:
-                ev[2].record()
+            timer.mark("launch")
             eng.run_stream(first, count, eng.B, stream=st)
             pos = first % eng.N                                       # windows start at multiples of the window: no wrap inside
             eng.get_yout(stage, pos, count, stream=st)
             for s, u, a, m in live:
                 outs[u][skip[u] + a:skip[u] + a + m].copy_(stage[s, pos:pos + m])
-            if ev:
-                ev[3].record()
-                events.append(ev)
+            timer.mark("done")
             if after is not None:
                 after(k)
-        return outs, events
+        torch.cuda.synchronize()
+        return outs
 
     def log_likelihood(self, cond_input, audio, window=None):
         """Per-sample log-likelihood of `audio` (int mu-law codes [batch][samples]) given `cond_input` (channels x batch x
@@ -976,8 +1023,7 @@ class NVWaveNet:
         or None; if given, receives the GPU seconds of production over the windows ("produce_s", the load not included) and of
         scoring ("score_s")."""
         shp = lambda a: tuple(int(v) for v in a.shape)
-        Cc, _ = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
-                                   "log_likelihood_from_features")
+        Cc, _, network = self._cond_network("log_likelihood_from_features", upsample_weight, upsample_bias, cond_weight, cond_bias, stride)
         if len(shp(features)) != 3 or shp(features)[1] != Cc or shp(features)[2] < 1:
             raise AssertionError(f"features must be [batch][{Cc}][T] with T >= 1; got {shp(features)}")
         batch_size, sample_count = shp(features)[0], shp(features)[2] * stride
@@ -986,8 +1032,7 @@ class NVWaveNet:
         _check_window(window)
         audio = torch.as_tensor(audio).to(device="cuda", dtype=torch.int32)
         eng = self._engine(batch_size, window or sample_count, True)
-        eng.cond_producer_load(features, upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias,
-                               stride)
+        eng.cond_producer_load(features, *network, stride)
         return self._score(eng, audio, eng.cond_producer_run_stream, timing)
 
     def _check_queue(self, what, lengths, audios, slots, window):
@@ -1000,8 +1045,7 @@ class NVWaveNet:
         for u, (a, n) in enumerate(zip(audios, lengths)):
             if tuple(a.shape) != (n,):
                 raise AssertionError(f"{what}: audio {u} must be [{n}] codes; got {tuple(a.shape)}")
-        if slots < 1 or window is None or window < 1:
-            raise AssertionError(f"{what}: need slots >= 1 and window >= 1; got {slots}, {window}")
+        _check_rows(what, "slots", slots, window)
         return [torch.as_tensor(a).to(device="cuda", dtype=torch.int32) for a in audios]
 
     def log_likelihood_many(self, cond_inputs, audios, slots=64, window=4096, timing=None):
@@ -1012,19 +1056,13 @@ class NVWaveNet:
         that frees first (plan_packed) and starts there at the very next sample; the rows are scored in windows at multiples of
         `window` (nvwn_score_stream_packed), each window's conditioning set once, zero where a row has nothing.  timing: a dict, or
         None; if given, receives the GPU seconds of filling the conditioning ("produce_s") and of scoring ("score_s")."""
-        for c in cond_inputs:
-            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * self.R, self.num_layers):
-                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
-        lengths = [int(c.size(2)) for c in cond_inputs]
+        lengths = self._check_utterances(cond_inputs)
         audios = self._check_queue("log_likelihood_many", lengths, audios, slots, window)
         plan = plan_packed(lengths, slots)
         eng = self._engine(slots, window, True)
 
         def fill(first, count, segs):
-            lh = torch.zeros((count, self.num_layers, slots, 2 * self.R), dtype=torch.float32, device="cuda")
-            for s, u, a, o, m in segs:
-                lh[o:o + m, :, s].copy_(cond_inputs[u][:, :, a:a + m].permute(2, 1, 0))
-            eng.set_conditioning(lh, 0, count)
+            eng.set_conditioning(self._gather(cond_inputs, count, slots, segs), 0, count)
 
         return self._score_packed(eng, plan, lengths, audios, fill, timing)
 
@@ -1037,17 +1075,13 @@ class NVWaveNet:
         it (nvwn_cond_from_features_host).  Each window's conditioning comes from the per-slot producer: an utterance's frames are
         attached to its row at its start, and the producer runs once per distinct segment range of the window, in time order.
         timing as for log_likelihood_many."""
-        shp = lambda a: tuple(int(v) for v in a.shape)
-        Cc, _ = check_cond_network(self.num_layers, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, AssertionError,
-                                   "log_likelihood_many_from_features")
-        for f in features:
-            if len(shp(f)) != 2 or shp(f)[0] != Cc or shp(f)[1] < 1:
-                raise AssertionError(f"each utterance's frames are [{Cc}][T] with T >= 1; got {shp(f)}")
-        lengths = [shp(f)[1] * stride for f in features]
+        Cc, _, network = self._cond_network("log_likelihood_many_from_features", upsample_weight, upsample_bias, cond_weight, cond_bias,
+                                            stride)
+        lengths = [T * stride for T in _check_frames(features, Cc)]
         audios = self._check_queue("log_likelihood_many_from_features", lengths, audios, slots, window)
         plan = plan_packed(lengths, slots)
         eng = self._engine(slots, window, True)
-        eng.cond_producer_set_weights(upsample_weight, upsample_bias, cond_weight.reshape(self.num_layers * 2 * self.R, Cc), cond_bias, stride)
+        eng.cond_producer_set_weights(*network, stride)
         keep = []
 
         def fill(first, count, segs):
@@ -1070,26 +1104,14 @@ class NVWaveNet:
         puts the conditioning of the window's segments into the store, then the window's audio and start flags are scored
         (nvwn_score_stream_packed) and each segment's logp copied out.  timing as for _score."""
         outs = [torch.empty(n, dtype=torch.float32, device="cuda") for n in lengths]
-        events = []
 
-        def mark():
-            if timing is not None:
-                events.append(torch.cuda.Event(enable_timing=True))
-                events[-1].record()
-
-        for first, count, segs in _packed_windows(plan, lengths, eng.N):
-            mark()
-            fill(first, count, segs)
-            mark()
+        def score(first, count, segs):
             audio, starts = _pack_window(count, segs, audios, eng.B)
             logp = eng.score_stream_packed(audio, starts, first)
             for s, u, a, o, m in segs:
                 outs[u][a:a + m].copy_(logp[s, o:o + m])
-            mark()
-        torch.cuda.synchronize()
-        if timing is not None:
-            timing["produce_s"] = sum(events[i].elapsed_time(events[i + 1]) for i in range(0, len(events), 3)) / 1e3
-            timing["score_s"] = sum(events[i + 1].elapsed_time(events[i + 2]) for i in range(0, len(events), 3)) / 1e3
+
+        _score_windows(_packed_windows(plan, lengths, eng.N), fill, score, timing)
         return outs
 
     @staticmethod
@@ -1100,24 +1122,8 @@ class NVWaveNet:
         ("score_s")."""
         batch_size, sample_count = audio.shape
         logp = torch.empty((batch_size, sample_count), dtype=torch.float32, device="cuda")
-        events = []
-
-        def mark():
-            if timing is not None:
-                events.append(torch.cuda.Event(enable_timing=True))
-                events[-1].record()
-
-        for first in range(0, sample_count, eng.N):
-            n = min(eng.N, sample_count - first)
-            mark()
-            fill(first, n)
-            mark()
-            logp[:, first:first + n] = eng.score_stream(audio[:, first:first + n], first)
-            mark()
-        torch.cuda.synchronize()
-        if timing is not None:
-            timing["produce_s"] = sum(events[i].elapsed_time(events[i + 1]) for i in range(0, len(events), 3)) / 1e3
-            timing["score_s"] = sum(events[i + 1].elapsed_time(events[i + 2]) for i in range(0, len(events), 3)) / 1e3
+        _score_windows([(first, min(eng.N, sample_count - first)) for first in range(0, sample_count, eng.N)], fill,
+                       lambda first, n: logp[:, first:first + n].copy_(eng.score_stream(audio[:, first:first + n], first)), timing)
         return logp
 
 
@@ -1176,29 +1182,19 @@ class ModelSet:
             raise AssertionError(f"{len(models)} models, {len(cond_inputs)} utterances and {len(seeds)} seeds")
         if any(int(m) != m or not 0 <= m < len(self.nets) for m in models):
             raise AssertionError(f"every model index is in [0, {len(self.nets)})")
-        for c in cond_inputs:
-            if c.dim() != 3 or (c.size(0), c.size(1)) != (2 * net.R, net.num_layers):
-                raise AssertionError(f"each input is channels x num_layers x samples; got {tuple(c.size())}")
-        lengths = [int(c.size(2)) for c in cond_inputs]
+        lengths = net._check_utterances(cond_inputs)
         models = [int(m) for m in models]
         eng = self._engine(slots, window, fp16)
         group = eng.model_group
         plan = plan_slots(lengths, slots, window, models, group)
         windows = _windows(plan, lengths, window)
-        _reset(eng)
         st = torch.cuda.current_stream()
 
         def tables(k):
             first, count, _, _ = windows[k]
             eng.set_group_models(group_models(plan, lengths, models, first, count, group, slots), stream=st)
 
-        condition = net._condition_slots(eng, windows, cond_inputs, [0] * len(lengths))
-        outs, events = net._serve(eng, plan, windows, lengths, seeds, timing is not None, condition, before=tables)
-        torch.cuda.synchronize()
-        if timing is not None:
-            timing["restart_upload_s"] = sum(e[0].elapsed_time(e[2]) for e in events) / 1e3
-            timing["generate_s"] = sum(e[2].elapsed_time(e[3]) for e in events) / 1e3
-        return outs
+        return net._serve_queue(eng, plan, windows, lengths, [0] * len(lengths), cond_inputs, seeds, _Timer(timing), tables)
 
     def close(self):
         for eng in self._engines.values():
