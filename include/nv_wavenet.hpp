@@ -317,6 +317,13 @@ public:
         if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
         return rc == 0;
     }
+    /* Scoring by model: models[b] is the model scoring row b runs, for each of the B rows (n_rows = B).  See nvwn_set_score_models. */
+    bool set_score_models(const int* models, int n_rows, cudaStream_t stream = 0)
+    {
+        const int rc = nvwn_set_score_models(m_engine, models, n_rows, stream);
+        if (rc != 0) fprintf(stderr, "GPUassert: %s %s %d\n", nvwn_last_error(), __FILE__, __LINE__);
+        return rc == 0;
+    }
 
     bool run(int num_samples, int batch_size, int* yOut = NULL, int batch_size_per_block = 1, bool dumpActivations = false,
              cudaStream_t stream = 0)

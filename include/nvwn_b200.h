@@ -316,13 +316,12 @@ int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states,
  * an earlier utterance's inputs) or an engine that is not NVWN_FP16 (NVWN_EUNSUPPORTED). */
 int nvwn_score_save_states(nvwn_engine* e, const int* rows, int n, const unsigned long long* seeds, void* states, void* stream);
 
-/* Multi-model serving: several models of one shape in one engine, each group of rows generating with its own weights.  Model 0 is
- * the engine's own weights (the setters, nvwn_weight_blob and nvwn_weights_updated); every generation kernel reads the weights of
- * a row's model, and nothing else about a row changes.  Scope:
- *   - scoring (nvwn_score*, nvwn_score_save_states) uses model 0 only;
- *   - nvwn_prime_from_score and nvwn_prime_slots_from_score refuse (NVWN_EINVAL) rows or slots whose group runs another model: a
- *     prompt for model m is scored on an engine holding m as model 0, and its state goes in through nvwn_score_save_states and
- *     nvwn_load_slots;
+/* Multi-model serving: several models of one shape in one engine, each group of rows generating with its own weights, and each
+ * scoring row scoring with its own.  Model 0 is the engine's own weights (the setters, nvwn_weight_blob and nvwn_weights_updated);
+ * every generation kernel reads the weights of a row's group's model, and the scorer those of a scoring row's model
+ * (nvwn_set_score_models); nothing else about a row changes.  Scope:
+ *   - nvwn_prime_from_score and nvwn_prime_slots_from_score refuse (NVWN_EINVAL) a row or slot whose group runs another model than
+ *     the one its scoring row was scored with;
  *   - slot states record no model, as they record no weights: loading one into a group that runs the right model is the caller's job. */
 enum { NVWN_MAX_MODELS = 64 };
 /* Copies src's weights (its blob, as uploaded) into model `model` (1 <= model < NVWN_MAX_MODELS) of e.  src is any engine on the
@@ -338,6 +337,19 @@ int nvwn_model_group(nvwn_engine* e, int* rows);
  * nvwn_reset_history, which leaves the models and the table alone.  Refused with NVWN_EINVAL, changing nothing: NULL arguments,
  * n_groups != ceil(B / G), an entry naming a model that was never set. */
 int nvwn_set_group_models(nvwn_engine* e, const int* models, int n_groups, void* stream);
+/* Scoring by model: models[b] is the model scoring row b runs, for every b in [0, B) (n_rows = B); each entry 0 or a model already
+ * set.  It applies to nvwn_score, nvwn_score_stream, nvwn_score_stream_packed and nvwn_score_save_states; a call of batch_size
+ * Bs < B uses entries [0, Bs).  A row's logp, logits and state are, bit for bit, those an engine holding its model as model 0
+ * gives the same utterance.  Rows are independent of the generation groups.  Host array, copied before return; the device copy
+ * is made on `stream`, which the scoring calls must follow (one stream, or ordered).
+ *   - Default: all 0, which runs the one-model scorer: every call gives the bits of an engine that never had a table.
+ *   - Setting a table ends an open scoring stream (its fronts were computed with the old models), as nvwn_set_model of a model
+ *     that one of the stream's rows runs does; nvwn_reset_history, generation calls and nvwn_set_group_models leave it alone.
+ *   - Each model in use gets its own scorer image, packed on the first scoring call that runs it after a change, freed by
+ *     nvwn_destroy (the size of model 0's: about 1.75 MB at R64 L20 S256, 7 MB at R128 L30).
+ * Refused, changing nothing: NULL arguments, n_rows != B, an entry negative, >= NVWN_MAX_MODELS or never set (NVWN_EINVAL); an
+ * engine that is not NVWN_FP16 (NVWN_EUNSUPPORTED). */
+int nvwn_set_score_models(nvwn_engine* e, const int* models, int n_rows, void* stream);
 
 /* last-sample activations [B][dim] as fp32 (nv_wavenet.cuh:424-438); valid after a run with dump=1 */
 int nvwn_get_xt_out(nvwn_engine* e, int layer, float* out);

@@ -73,6 +73,7 @@ SYMBOLS = {
     "nvwn_set_model": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_model_group": (C.c_int, [_vp, _vp]),
     "nvwn_set_group_models": (C.c_int, [_vp, _vp, C.c_int, _vp]),
+    "nvwn_set_score_models": (C.c_int, [_vp, _vp, C.c_int, _vp]),
     "nvwn_get_xt_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_skip_out": (C.c_int, [_vp, C.c_int, _vp]),
     "nvwn_get_zs": (C.c_int, [_vp, _vp]),

@@ -150,6 +150,19 @@ int wn_lat_max_clusters(int S, int rows);          // three-CTA clusters of `row
 cudaError_t wn_plain_convert(const WnConfig& c, void* store, const float* src, int first_sample, int num_samples, cudaStream_t stream);
 cudaError_t wn_plain_readback(const WnConfig& c, float* dst_dev, const void* store, int first_sample, int num_samples, cudaStream_t stream);
 
+// Scoring by model (nvwn_set_score_models, DESIGN.md §5.5): the rows b < Bs of a call grouped by model.  Segment k holds the n[k]
+// rows order[first[k] .. first[k] + n[k]) (ascending) of model model[k], segments by model.  In a chunk of T steps its T * n[k] local
+// rows q go to the chunk's row m = (q / n[k]) * Bs + order[first[k] + q % n[k]], and they make ceil(T * n[k] / 64) tiles of one
+// model, the segments' tiles in order.  image[v], embPrev[v] and embCur[v] are model v's score image and embeddings.
+struct WnScoreSegs {
+    int count;
+    int model[NVWN_MAX_MODELS], n[NVWN_MAX_MODELS], first[NVWN_MAX_MODELS];
+    const void* image[NVWN_MAX_MODELS];
+    const void *embPrev[NVWN_MAX_MODELS], *embCur[NVWN_MAX_MODELS];
+    const int* order;               // device: every row of the table by model, then by row; a call's rows of a model are a prefix
+    const int* row_model;           // device [Be]: the model of row b
+};
+
 // teacher-forced scoring (wn_score_kernel.cu, DESIGN.md §5.4): one time chunk of T steps x Bs utterances, rows m = (t - t0) * Bs + b
 struct WnScoreChunk {
     int L, R, S, A, maxDil, tanhEmbed;
@@ -172,6 +185,10 @@ struct WnScoreChunk {
     const unsigned char* starts;
     int* tau;
     int* tau_carry;
+    // scoring by model, or NULL: every row runs `image` and the blob's embeddings.  segs is the host copy, segs_dev the same bytes
+    // on the device, which the kernels read
+    const WnScoreSegs* segs;
+    const WnScoreSegs* segs_dev;
 };
 int wn_score_dilation(int layer, int maxDil);
 size_t wn_score_xh_offset(int layer, int L, int maxDil, int Tcap, int Be, int R);   // in elements; layer = L gives the total

@@ -14,6 +14,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <memory>
 #include <string>
 #include <utility>
@@ -164,6 +165,8 @@ struct nvwn_engine : WnConfig {
         DevBuf<char> blob;
         DevBuf<void> image;
         bool dirty = true;
+        DevBuf<void> score_image;            // the scorer's image of the model, allocated and packed on the first scoring call that
+        bool score_dirty = true;             // runs the model after a change
     };
     std::vector<Model> models;
     DevBuf<WnModel> model_tab;
@@ -187,6 +190,12 @@ struct nvwn_engine : WnConfig {
     long long score_next = -1;
     int score_bs = 0;
     bool score_packed = false;
+    // scoring by model (nvwn_set_score_models): the model of every row (host, empty until the first table: all 0); score_tab its
+    // device form, the rows by model then row (WnScoreSegs::order) followed by the table itself; score_segs the device copy of a
+    // call's segments
+    std::vector<int> score_models;
+    DevBuf<int> score_tab;
+    DevBuf<WnScoreSegs> score_segs;
 
     DevBuf<float> lut_f;                     // mu-law decode tables (nvwn_get_audio): A floats, then 2 x A int16 (wrap / saturate)
     DevBuf<unsigned long long> trace;        // debug timeline (nvwn_debug_trace)
@@ -529,15 +538,21 @@ int check_prime(const nvwn_engine* e, const std::string& who)
     return 0;
 }
 
-// Scoring runs model 0, so a prime may only write rows whose group runs it: rows[0..n) (NULL: rows 0 .. n - 1)
-int check_prime_model(const nvwn_engine* e, const std::string& who, const int* rows, int n)
+// The model scoring row b runs (nvwn_set_score_models)
+int score_model(const nvwn_engine* e, int b) { return e->score_models.empty() ? 0 : e->score_models[b]; }
+
+// A prime may only write a row or slot whose group generates with the model its scoring row was scored with: scoring rows
+// rows[0..n) into slots slots[0..n) (NULL: 0 .. n - 1 for either)
+int check_prime_model(const nvwn_engine* e, const std::string& who, const int* rows, const int* slots, int n)
 {
-    if (e->group_host.empty()) return 0;
     for (int i = 0; i < n; i++) {
-        const int r = rows ? rows[i] : i, m = e->group_host[r / e->group_rows];
-        if (m != 0)
-            return fail(NVWN_EINVAL, who + ": row " + std::to_string(r) + " is in a group that runs model " + std::to_string(m) + ", and scoring runs model 0: "
-                                           "score the prompt on an engine holding that model and load its state (nvwn_score_save_states, nvwn_load_slots)");
+        const int r = rows ? rows[i] : i, s = slots ? slots[i] : i;
+        const int sm = score_model(e, r), gm = e->group_host.empty() ? 0 : e->group_host[s / e->group_rows];
+        if (sm != gm)
+            return fail(NVWN_EINVAL, who + ": row " + std::to_string(s) + " is in a group that runs model " + std::to_string(gm) + ", and its scoring row " +
+                                           std::to_string(r) + " was scored with model " + std::to_string(sm) + ": set the scoring table (nvwn_set_score_models) "
+                                           "to the group's model, or score the prompt on an engine holding that model and load its state (nvwn_score_save_states, "
+                                           "nvwn_load_slots)");
     }
     return 0;
 }
@@ -1315,7 +1330,10 @@ int nvwn_set_model(nvwn_engine* e, int model, const nvwn_engine* src)
         m = std::move(fresh);
     }
     CK(cudaMemcpyAsync(m.blob, src->blob, e->blob_bytes, cudaMemcpyDeviceToDevice, 0));
-    m.dirty = true;
+    m.dirty = m.score_dirty = true;
+    if (e->score_next >= 0)                  // an open scoring stream whose rows run the model ends, as at a weight change
+        for (int b = 0; b < e->score_bs; b++)
+            if (score_model(e, b) == model) { e->score_next = -1; break; }
     CK(cudaStreamSynchronize(0));       // src may be changed or destroyed on return
     return 0;
 }
@@ -1341,6 +1359,30 @@ int nvwn_set_group_models(nvwn_engine* e, const int* models, int n_groups, void*
     const int rc = copy_snapshot(e->group_tab, models, n_groups, (cudaStream_t)stream);
     if (rc != 0) return rc;
     e->group_host.assign(models, models + n_groups);
+    return 0;
+}
+
+int nvwn_set_score_models(nvwn_engine* e, const int* models, int n_rows, void* stream)
+{
+    const std::string who = "nvwn_set_score_models";
+    if (!e || !models) return fail(NVWN_EINVAL, who + ": NULL argument");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score");
+    if (n_rows != e->B) return fail(NVWN_EINVAL, who + ": need n_rows = B = " + std::to_string(e->B) + "; got " + std::to_string(n_rows));
+    for (int b = 0; b < n_rows; b++)
+        if (models[b] != 0 && (models[b] < 0 || models[b] >= NVWN_MAX_MODELS || !e->models[models[b]].blob))
+            return fail(NVWN_EINVAL, who + ": row " + std::to_string(b) + " names model " + std::to_string(models[b]) + ", which was never set");
+    // the rows by model, then by row, and the table: a call of Bs rows takes of each model's rows the prefix below Bs
+    std::vector<int> tab(2 * (size_t)n_rows);
+    size_t k = 0;
+    for (int v = 0; v < NVWN_MAX_MODELS; v++)
+        for (int b = 0; b < n_rows; b++)
+            if (models[b] == v) tab[k++] = b;
+    std::copy(models, models + n_rows, tab.begin() + n_rows);
+    if (!e->score_tab) CK(e->score_tab.alloc(tab.size() * sizeof(int)));
+    const int rc = copy_snapshot(e->score_tab, tab.data(), tab.size(), (cudaStream_t)stream);
+    if (rc != 0) return rc;
+    e->score_models.assign(models, models + n_rows);
+    e->score_next = -1;                      // the open stream's fronts were computed with the old models
     return 0;
 }
 
@@ -1548,11 +1590,47 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, const unsigne
                                      std::to_string(v) + " is outside [0, " + std::to_string(A) + ")");
     }
     e->score_next = -1;                      // reopened below once this call's state is complete
+    WnParams p;
+    fill_params(e, p, 0, 0, 0, N, Bs, 0);
     if (e->score_dirty) {
-        WnParams p;
-        fill_params(e, p, 0, 0, 0, N, Bs, 0);
         CK(wn_score_pack(e->score_image, p, st));
         e->score_dirty = false;
+    }
+    // scoring by model, when a row of the call runs another model than 0: its segments, each model's image packed if it changed
+    WnScoreSegs segs{};
+    bool by_model = false;
+    for (int b = 0; b < Bs && !by_model; b++) by_model = score_model(e, b) != 0;
+    if (by_model) {
+        std::vector<int> n_of(NVWN_MAX_MODELS, 0), all_of(NVWN_MAX_MODELS, 0);
+        for (int b = 0; b < e->B; b++) {
+            all_of[score_model(e, b)]++;
+            if (b < Bs) n_of[score_model(e, b)]++;
+        }
+        for (int v = 0, first = 0; v < NVWN_MAX_MODELS; first += all_of[v++]) {
+            if (!n_of[v]) continue;
+            const char* blob = e->blob;
+            const void* image = e->score_image;
+            if (v) {
+                nvwn_engine::Model& m = e->models[v];
+                if (!m.score_image) CK(m.score_image.alloc(wn_score_image_bytes(R, e->S, A, L)));
+                if (m.score_dirty) {
+                    WnParams q = p;
+                    point_weights(e, q, m.blob);
+                    CK(wn_score_pack(m.score_image, q, st));
+                    m.score_dirty = false;
+                }
+                blob = m.blob;
+                image = m.score_image;
+            }
+            const int k = segs.count++;
+            segs.model[k] = v; segs.n[k] = n_of[v]; segs.first[k] = first;
+            segs.image[v] = image; segs.embPrev[v] = blob + e->o_embPrev; segs.embCur[v] = blob + e->o_embCur;
+        }
+        segs.order = e->score_tab;
+        segs.row_model = e->score_tab + e->B;
+        if (!e->score_segs) CK(e->score_segs.alloc(sizeof(WnScoreSegs)));
+        const int rc = copy_snapshot(e->score_segs, &segs, 1, st);
+        if (rc != 0) return rc;
     }
     const bool logp_dev = is_device_ptr(logp), logits_dev = logits && is_device_ptr(logits);
     if (first == 0) {
@@ -1575,6 +1653,8 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, const unsigne
     c.H = reinterpret_cast<__half*>(sc + o.H);
     c.logp = logp_dev ? logp : reinterpret_cast<float*>(sc + o.logp);
     c.starts = nullptr;
+    c.segs = by_model ? &segs : nullptr;
+    c.segs_dev = by_model ? e->score_segs.get() : nullptr;
     if (starts) {
         CK(cudaMemcpyAsync(sc + o.starts, starts, n_audio, cudaMemcpyDefault, st));
         c.starts = reinterpret_cast<const unsigned char*>(sc + o.starts);
@@ -1654,7 +1734,7 @@ int nvwn_prime_from_score(nvwn_engine* e, void* stream)
     const std::string who = "nvwn_prime_from_score";
     int rc = check_prime(e, who);
     if (rc == 0) rc = check_run_batch(e, who, e->score_bs);
-    if (rc == 0) rc = check_prime_model(e, who, nullptr, e->score_bs);
+    if (rc == 0) rc = check_prime_model(e, who, nullptr, nullptr, e->score_bs);
     if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int Bs = e->score_bs;
@@ -1674,7 +1754,7 @@ int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slot
     int rc = check_prime(e, who);
     if (rc != 0) return rc;
     if (!rows) return fail(NVWN_EINVAL, who + ": rows is NULL");
-    if ((rc = check_slots(e, who, slots, n)) || (rc = check_prime_model(e, who, slots, n))) return rc;
+    if ((rc = check_slots(e, who, slots, n))) return rc;
     const int Bs = e->score_bs;
     std::vector<char> seen(Bs, 0);
     for (int i = 0; i < n; i++) {
@@ -1683,6 +1763,7 @@ int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slot
         if (seen[rows[i]]) return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is given twice");
         seen[rows[i]] = 1;
     }
+    if ((rc = check_prime_model(e, who, rows, slots, n))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned long long* seeds_dev;
     if ((rc = take_slots(e, who, slots, n, seeds, &seeds_dev, st)) || (rc = copy_snapshot(e->prime_rows, rows, n, st))) return rc;

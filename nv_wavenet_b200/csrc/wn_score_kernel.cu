@@ -17,6 +17,9 @@
 // fixed order in one CTA (no split-K, no atomics), so a row's result does not depend on which tile, chunk or batch it is computed in.
 // Packed scoring (nvwn_score_stream_packed) starts utterances inside a row: the PACKED instantiations of the embedding and layer
 // kernels read codes 128 and zero x[t-d] by each row's local time, where a fresh start reads the 128s and the zeroed fronts.
+// Scoring by model (nvwn_set_score_models): the MODELS instantiations take the chunk's rows model by model (WnScoreSegs), in tiles
+// of one model each, and read each tile's weights from its model's image; a row's arithmetic is the one-model kernels', so its
+// results are the bits an engine holding its model as model 0 gives.
 #include "wn_common.h"
 #include "wn_math.cuh"
 
@@ -147,10 +150,11 @@ __device__ __forceinline__ uint32_t u32(__half2 h) { return *reinterpret_cast<ui
 // ---- embedding: x_0 of every row of the chunk; the codes of call steps -2 and -1 come from codes[b][0..1] ----
 // PACKED (nvwn_score_stream_packed): tau[m] is row m's local time, the samples its utterance has run before this one; the codes of
 // its steps -1 and -2 are 128 where tau < 1 and tau < 2
-template <bool PACKED>
+// MODELS: row b reads the embeddings of its model segs->row_model[b]
+template <bool PACKED, bool MODELS>
 __global__ void score_embed_kernel(const __half* __restrict__ embPrev, const __half* __restrict__ embCur, const int* __restrict__ audio,
                                    const int* __restrict__ codes, int N, int t0, int M, int Bs, int R, int tanhEmbed, float* __restrict__ xf,
-                                   __half* __restrict__ x0, const int* __restrict__ tau)
+                                   __half* __restrict__ x0, const int* __restrict__ tau, const WnScoreSegs* __restrict__ segs)
 {
     const size_t n_all = (size_t)M * R;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_all; i += (size_t)gridDim.x * blockDim.x) {
@@ -161,7 +165,13 @@ __global__ void score_embed_kernel(const __half* __restrict__ embPrev, const __h
             if (tm < 2) yp = 128;
             if (tm < 1) yc = 128;
         }
-        float v = __half2float(embPrev[(size_t)yp * R + r]) + __half2float(embCur[(size_t)yc * R + r]);
+        const __half *eP = embPrev, *eC = embCur;
+        if (MODELS) {
+            const int v = segs->row_model[b];
+            eP = static_cast<const __half*>(segs->embPrev[v]);
+            eC = static_cast<const __half*>(segs->embCur[v]);
+        }
+        float v = __half2float(eP[(size_t)yp * R + r]) + __half2float(eC[(size_t)yc * R + r]);
         if (tanhEmbed) v = wn::tanhf_fast(v);         // as the latency kernel (wn_lat_kernel.cu)
         xf[i] = v;
         x0[i] = __float2half_rn(v);
@@ -208,27 +218,82 @@ struct LayerArgs {
     const int* tau;                 // PACKED: local time of row m (score_tau_kernel); x[t-d] reads 0 where tau[m] < d
 };
 
-template <int R>
-constexpr int layer_smem() { return (4 * R * R + R * R + BM * 2 * R + BM * R) * 2; }
+// The second argument of the layer and output kernels, read by their MODELS instantiations only: the chunk's segments (device),
+// their tiles, and the byte offsets in every image of the weights the launch reads (the layer's W1, Wr, Bh, Br; the output's)
+struct ModelArgs {
+    const WnScoreSegs* segs;
+    int tiles;
+    size_t oW1, oWr, oBh, oBr, oWs, oWzs, oWza, oBsk, oBzs, oBza;
+};
 
-template <int R, bool PACKED>
-__global__ void __launch_bounds__(NTHREADS) score_layer_kernel(const LayerArgs a)
+template <int R>
+__host__ __device__ constexpr int layer_smem() { return (4 * R * R + R * R + BM * 2 * R + BM * R) * 2; }
+
+// MODELS: the segment of tile `tile` of a chunk of T steps, and in `start` the chunk tile its segment begins at
+__device__ __forceinline__ int score_seg(const WnScoreSegs* __restrict__ s, int T, int tile, int& start)
+{
+    int k = 0, base = 0;
+    for (; k + 1 < s->count; k++) {
+        const int nt = (T * s->n[k] + BM - 1) / BM;
+        if (tile < base + nt) break;
+        base += nt;
+    }
+    start = base;
+    return k;
+}
+// MODELS: the chunk row of local row q of segment k (T steps, Bs rows per step), -1 past the segment's rows
+__device__ __forceinline__ int score_row(const WnScoreSegs* __restrict__ s, int k, int q, int T, int Bs)
+{
+    const int n = s->n[k];
+    return q < T * n ? (q / n) * Bs + s->order[s->first[k] + q % n] : -1;
+}
+
+// MODELS: a CTA takes a contiguous range of the chunk's tiles (segment by segment) and loads a tile's model's weights only where
+// they differ from the last tile's, so it reloads them at most once per segment boundary in its range; srow holds the chunk row of
+// each of the tile's rows (-1 past its segment's rows), through which every row access goes
+template <int R, bool PACKED, bool MODELS>
+__global__ void __launch_bounds__(NTHREADS) score_layer_kernel(const LayerArgs a, const ModelArgs x)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     constexpr int N1 = 2 * R / 8, NR = R / 8, NJ = R / 16;       // chunks per row of W1 / XA, of Wr / HT; n-tiles per warp and half
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp & 3, wn = warp >> 2, g = lane >> 2, q = lane & 3;
     const uint32_t sW1 = smem_u32(smem), sWr = sW1 + 4 * R * R * 2, sXA = sWr + R * R * 2, sHT = sXA + BM * 2 * R * 2;
+    int* srow = reinterpret_cast<int*>(smem + layer_smem<R>());
+    const float *Bh = nullptr, *Br = nullptr;         // MODELS: the resident model's biases
 
-    for (int i = tid; i < 2 * R * N1; i += NTHREADS) cp16(sW1 + swz(i / N1, i % N1, N1), a.W1 + (size_t)i * 8, true);
-    for (int i = tid; i < R * NR; i += NTHREADS) cp16(sWr + swz(i / NR, i % NR, NR), a.Wr + (size_t)i * 8, true);
-    cp_commit();
+    if (!MODELS) {
+        for (int i = tid; i < 2 * R * N1; i += NTHREADS) cp16(sW1 + swz(i / N1, i % N1, N1), a.W1 + (size_t)i * 8, true);
+        for (int i = tid; i < R * NR; i += NTHREADS) cp16(sWr + swz(i / NR, i % NR, NR), a.Wr + (size_t)i * 8, true);
+        cp_commit();
+    }
 
-    const int tiles = (a.M + BM - 1) / BM;
-    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int tiles = MODELS ? x.tiles : (a.M + BM - 1) / BM;
+    const int lo = MODELS ? (int)((long long)blockIdx.x * tiles / gridDim.x) : (int)blockIdx.x;
+    const int hi = MODELS ? (int)((long long)(blockIdx.x + 1) * tiles / gridDim.x) : tiles;
+    int resident = -1;
+    for (int tile = lo; tile < hi; tile += MODELS ? 1 : gridDim.x) {
         const int m0 = tile * BM;
+        if (MODELS) {
+            const int T = a.M / a.Bs;
+            int start;
+            const int k = score_seg(x.segs, T, tile, start);
+            __syncthreads();                            // the last tile's reads of srow and of the weights are done
+            if (k != resident) {
+                const char* im = static_cast<const char*>(x.segs->image[x.segs->model[k]]);
+                const __half* W1 = reinterpret_cast<const __half*>(im + x.oW1);
+                const __half* Wr = reinterpret_cast<const __half*>(im + x.oWr);
+                Bh = reinterpret_cast<const float*>(im + x.oBh);
+                Br = reinterpret_cast<const float*>(im + x.oBr);
+                for (int i = tid; i < 2 * R * N1; i += NTHREADS) cp16(sW1 + swz(i / N1, i % N1, N1), W1 + (size_t)i * 8, true);
+                for (int i = tid; i < R * NR; i += NTHREADS) cp16(sWr + swz(i / NR, i % NR, NR), Wr + (size_t)i * 8, true);
+                resident = k;
+            }
+            if (tid < BM) srow[tid] = score_row(x.segs, k, (tile - start) * BM + tid, T, a.Bs);
+            __syncthreads();
+        }
         for (int i = tid; i < BM * N1; i += NTHREADS) {
-            const int r = i / N1, c = i % N1, m = m0 + r;
-            const bool v = m < a.M;
+            const int r = i / N1, c = i % N1, m = MODELS ? srow[r] : m0 + r;
+            const bool v = MODELS ? m >= 0 : m < a.M;
             const size_t row = v ? (size_t)m + (c < NR ? a.hist : 0) : 0;
             // packed: x[t-d] of a row whose utterance began less than d samples ago is the zero a fresh start reads from its front
             cp16(sXA + swz(r, c, N1), a.xin + row * R + (c % NR) * 8, PACKED ? v && (c < NR || a.tau[m] >= a.d) : v);
@@ -263,13 +328,13 @@ __global__ void __launch_bounds__(NTHREADS) score_layer_kernel(const LayerArgs a
         const __half2 half = __floats2half2_rn(0.5f, 0.5f);
 #pragma unroll
         for (int hr = 0; hr < 2; hr++) {
-            const int r = wm * 16 + g + 8 * hr, m = m0 + r;
-            const bool v = m < a.M;
+            const int r = wm * 16 + g + 8 * hr, m = MODELS ? srow[r] : m0 + r;
+            const bool v = MODELS ? m >= 0 : m < a.M;
             const float* lh = a.lh + (v ? (size_t)(m / a.Bs) * a.lh_t + (size_t)(m % a.Bs) * 2 * R : 0);
 #pragma unroll
             for (int j = 0; j < NJ; j++) {
                 const int c = wn * (R / 2) + 8 * j + 2 * q;
-                const float2 bt = *reinterpret_cast<const float2*>(a.Bh + c), bs = *reinterpret_cast<const float2*>(a.Bh + R + c);
+                const float2 bt = *reinterpret_cast<const float2*>(MODELS ? Bh + c : a.Bh + c), bs = *reinterpret_cast<const float2*>(MODELS ? Bh + R + c : a.Bh + R + c);
                 float2 lt = make_float2(0.f, 0.f), ls = lt;
                 if (v) { lt = *reinterpret_cast<const float2*>(lh + c); ls = *reinterpret_cast<const float2*>(lh + R + c); }
                 const float t0 = (at[j][2 * hr] + bt.x) + lt.x, t1 = (at[j][2 * hr + 1] + bt.y) + lt.y;
@@ -303,12 +368,12 @@ __global__ void __launch_bounds__(NTHREADS) score_layer_kernel(const LayerArgs a
             }
 #pragma unroll
             for (int hr = 0; hr < 2; hr++) {
-                const int m = m0 + wm * 16 + g + 8 * hr;
-                if (m >= a.M) continue;
+                const int m = MODELS ? srow[wm * 16 + g + 8 * hr] : m0 + wm * 16 + g + 8 * hr;
+                if (MODELS ? m < 0 : m >= a.M) continue;
 #pragma unroll
                 for (int j = 0; j < NJ; j++) {
                     const int c = wn * (R / 2) + 8 * j + 2 * q;
-                    const float2 br = *reinterpret_cast<const float2*>(a.Br + c);
+                    const float2 br = *reinterpret_cast<const float2*>(MODELS ? Br + c : a.Br + c);
                     float2* xp = reinterpret_cast<float2*>(a.xf + (size_t)m * R + c);
                     const float2 x = *xp;
                     const float2 y = make_float2((ar[j][2 * hr] + br.x) + x.x, (ar[j][2 * hr + 1] + br.y) + x.y);
@@ -339,9 +404,10 @@ constexpr int LG_LD = A_OUT + 8;                         // padded fp32 logit ro
 constexpr int OUT_SMEM = 2 * STAGE + BM * A_OUT * 2 * 2 + BM * LG_LD * 4;
 
 // acc (16 rows x NT * 8 columns of this warp) = A[rows][0..K) . B[N][0..K)^T with B (and A when A_GLOBAL) streamed through a
-// two-stage cp.async ring in k-slices of 64; otherwise A is a resident row-major tile of a_nch chunks per row
-template <int NT, bool A_GLOBAL>
-__device__ __forceinline__ void gemm_stream(float (&acc)[NT][4], const __half* __restrict__ Ag, int lda, int m0, int M, uint32_t sAres, int a_nch,
+// two-stage cp.async ring in k-slices of 64; otherwise A is a resident row-major tile of a_nch chunks per row.  A's rows are
+// m0 + r below M, or with MAPPED rows[r] where that is not negative
+template <int NT, bool A_GLOBAL, bool MAPPED = false>
+__device__ __forceinline__ void gemm_stream(float (&acc)[NT][4], const __half* __restrict__ Ag, int lda, int m0, int M, const int* rows, uint32_t sAres, int a_nch,
                                             const __half* __restrict__ Bg, int K, uint32_t ring, int tid, int lane, int wm, int wn)
 {
     constexpr int N = NT * 16;
@@ -354,8 +420,8 @@ __device__ __forceinline__ void gemm_stream(float (&acc)[NT][4], const __half* _
         const uint32_t sa = ring + (s & 1) * STAGE, sb = sa + BM * KS * 2;
         if (A_GLOBAL) {
             for (int i = tid; i < BM * 8; i += NTHREADS) {
-                const int r = i / 8, c = i % 8, m = m0 + r, k = s * KS + c * 8;
-                const bool v = m < M && k < K;
+                const int r = i / 8, c = i % 8, m = MAPPED ? rows[r] : m0 + r, k = s * KS + c * 8;
+                const bool v = (MAPPED ? m >= 0 : m < M) && k < K;
                 cp16(sa + swz(r, c, 8), Ag + (v ? (size_t)m * lda + k : 0), v);
             }
         }
@@ -405,49 +471,61 @@ __device__ __forceinline__ void relu_to_tile(const float (&acc)[NT][4], const fl
     }
 }
 
-template <int S>
-__global__ void __launch_bounds__(NTHREADS) score_out_kernel(const OutArgs a)
+// MODELS: each tile reads its model's weights, and its rows through srow as the layer kernel's
+template <int S, bool MODELS>
+__global__ void __launch_bounds__(NTHREADS) score_out_kernel(const OutArgs a, const ModelArgs x)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     constexpr int A = A_OUT;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, wm = warp & 3, wn = warp >> 2;
     const uint32_t ring = smem_u32(smem), sZ1 = ring + 2 * STAGE, sZ2 = sZ1 + BM * A * 2;
     float* lg = reinterpret_cast<float*>(smem + 2 * STAGE + 2 * BM * A * 2);
+    int* srow = reinterpret_cast<int*>(smem + OUT_SMEM);
 
-    const int tiles = (a.M + BM - 1) / BM;
+    const int tiles = MODELS ? x.tiles : (a.M + BM - 1) / BM;
     for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const int m0 = tile * BM;
+        const char* im = nullptr;                     // MODELS: the tile's model's image
+        if (MODELS) {
+            const int T = a.M / a.Bs;
+            int start;
+            const int k = score_seg(x.segs, T, tile, start);
+            im = static_cast<const char*>(x.segs->image[x.segs->model[k]]);
+            if (tid < BM) srow[tid] = score_row(x.segs, k, (tile - start) * BM + tid, T, a.Bs);
+            __syncthreads();                            // the last tile ended with a barrier: its reads of srow are done
+        }
         {
             float acc[S / 16][4];
-            gemm_stream<S / 16, true>(acc, a.H, a.K1, m0, a.M, 0, 0, a.Ws, a.K1, ring, tid, lane, wm, wn);
-            relu_to_tile<S / 16>(acc, a.Bsk, sZ1, S / 8, wm, wn, lane);
+            gemm_stream<S / 16, true, MODELS>(acc, a.H, a.K1, m0, a.M, srow, 0, 0, MODELS ? reinterpret_cast<const __half*>(im + x.oWs) : a.Ws, a.K1, ring, tid, lane, wm, wn);
+            relu_to_tile<S / 16>(acc, MODELS ? reinterpret_cast<const float*>(im + x.oBsk) : a.Bsk, sZ1, S / 8, wm, wn, lane);
         }
         __syncthreads();
         {
             float acc[A / 16][4];
-            gemm_stream<A / 16, false>(acc, nullptr, 0, m0, a.M, sZ1, S / 8, a.Wzs, S, ring, tid, lane, wm, wn);
-            relu_to_tile<A / 16>(acc, a.Bzs, sZ2, A / 8, wm, wn, lane);
+            gemm_stream<A / 16, false>(acc, nullptr, 0, m0, a.M, nullptr, sZ1, S / 8, MODELS ? reinterpret_cast<const __half*>(im + x.oWzs) : a.Wzs, S, ring, tid, lane, wm, wn);
+            relu_to_tile<A / 16>(acc, MODELS ? reinterpret_cast<const float*>(im + x.oBzs) : a.Bzs, sZ2, A / 8, wm, wn, lane);
         }
         __syncthreads();
         {
             float acc[A / 16][4];
-            gemm_stream<A / 16, false>(acc, nullptr, 0, m0, a.M, sZ2, A / 8, a.Wza, A, ring, tid, lane, wm, wn);
+            gemm_stream<A / 16, false>(acc, nullptr, 0, m0, a.M, nullptr, sZ2, A / 8, MODELS ? reinterpret_cast<const __half*>(im + x.oWza) : a.Wza, A, ring, tid, lane, wm, wn);
             const int g = lane >> 2, q = lane & 3;
+            const float* Bza = MODELS ? reinterpret_cast<const float*>(im + x.oBza) : a.Bza;
 #pragma unroll
             for (int hr = 0; hr < 2; hr++) {
                 const int r = wm * 16 + g + 8 * hr;
 #pragma unroll
                 for (int j = 0; j < A / 16; j++) {
                     const int c = wn * (A / 2) + 8 * j + 2 * q;
-                    *reinterpret_cast<float2*>(lg + r * LG_LD + c) = make_float2(acc[j][2 * hr] + a.Bza[c], acc[j][2 * hr + 1] + a.Bza[c + 1]);
+                    *reinterpret_cast<float2*>(lg + r * LG_LD + c) = make_float2(acc[j][2 * hr] + Bza[c], acc[j][2 * hr + 1] + Bza[c + 1]);
                 }
             }
         }
         __syncthreads();
         // log-softmax in fp32 with accurate expf / logf, one warp per row, fixed reduction trees
         for (int r = warp; r < BM; r += NTHREADS / 32) {
-            const int m = m0 + r;
-            if (m >= a.M) break;
+            const int m = MODELS ? srow[r] : m0 + r;
+            if (MODELS ? m < 0 : m >= a.M) break;
             const int b = m % a.Bs, t = a.t0 + m / a.Bs;
             float z[A / 32], mx = -INFINITY;
 #pragma unroll
@@ -488,7 +566,7 @@ int num_sms()
 
 // one wave of CTAs, each looping over row tiles (the weights a CTA stages are loaded once per launch)
 template <typename Args>
-cudaError_t launch_persistent(void (*kernel)(Args), int smem, int tiles, cudaStream_t st, const Args& args)
+cudaError_t launch_persistent(void (*kernel)(Args, ModelArgs), int smem, int tiles, cudaStream_t st, const Args& args, const ModelArgs& x)
 {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
@@ -498,22 +576,25 @@ cudaError_t launch_persistent(void (*kernel)(Args), int smem, int tiles, cudaStr
     if (per_sm < 1) return cudaErrorInvalidConfiguration;
     int grid = num_sms() * per_sm;
     if (grid > tiles) grid = tiles;
-    kernel<<<grid, NTHREADS, smem, st>>>(args);
+    kernel<<<grid, NTHREADS, smem, st>>>(args, x);
     return cudaGetLastError();
 }
 
 template <int R>
-cudaError_t launch_layer(const LayerArgs& a, cudaStream_t st)
+cudaError_t launch_layer(const LayerArgs& a, const ModelArgs& x, cudaStream_t st)
 {
-    static_assert(layer_smem<R>() <= 227 * 1024, "layer kernel shared memory");
-    return launch_persistent(a.tau ? score_layer_kernel<R, true> : score_layer_kernel<R, false>, layer_smem<R>(), (a.M + BM - 1) / BM, st, a);
+    static_assert(layer_smem<R>() + BM * 4 <= 227 * 1024, "layer kernel shared memory");
+    if (x.segs)
+        return launch_persistent(a.tau ? score_layer_kernel<R, true, true> : score_layer_kernel<R, false, true>, layer_smem<R>() + BM * 4, x.tiles, st, a, x);
+    return launch_persistent(a.tau ? score_layer_kernel<R, true, false> : score_layer_kernel<R, false, false>, layer_smem<R>(), (a.M + BM - 1) / BM, st, a, x);
 }
 
 template <int S>
-cudaError_t launch_out(const OutArgs& a, cudaStream_t st)
+cudaError_t launch_out(const OutArgs& a, const ModelArgs& x, cudaStream_t st)
 {
-    static_assert(OUT_SMEM <= 227 * 1024, "output kernel shared memory");
-    return launch_persistent(score_out_kernel<S>, OUT_SMEM, (a.M + BM - 1) / BM, st, a);
+    static_assert(OUT_SMEM + BM * 4 <= 227 * 1024, "output kernel shared memory");
+    if (x.segs) return launch_persistent(score_out_kernel<S, true>, OUT_SMEM + BM * 4, x.tiles, st, a, x);
+    return launch_persistent(score_out_kernel<S, false>, OUT_SMEM, (a.M + BM - 1) / BM, st, a, x);
 }
 
 }  // namespace
@@ -584,14 +665,21 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     const int* tau = c.starts ? c.tau : nullptr;
+    ModelArgs x = {};
+    if (c.segs) {                                     // scoring by model: the chunk's tiles, segment by segment
+        x.segs = c.segs_dev;
+        for (int k = 0; k < c.segs->count; k++) x.tiles += (c.T * c.segs->n[k] + BM - 1) / BM;
+        x.oWs = o.Ws; x.oWzs = o.Wzs; x.oWza = o.Wza; x.oBsk = o.Bsk; x.oBzs = o.Bzs; x.oBza = o.Bza;
+    }
     {
         const size_t n = (size_t)M * R;
         size_t blocks = (n + 255) / 256;
         if (blocks > 132 * 16) blocks = 132 * 16;
         __half* x0 = c.xh + (size_t)wn_score_dilation(0, c.maxDil) * c.Bs * R;
-        (tau ? score_embed_kernel<true> : score_embed_kernel<false>)<<<(unsigned)blocks, 256, 0, st>>>(
-            static_cast<const __half*>(c.embPrev), static_cast<const __half*>(c.embCur), c.audio, c.codes, c.N, c.t0, M, c.Bs, R, c.tanhEmbed, c.xf,
-            x0, tau);
+        auto embed = c.segs ? (tau ? score_embed_kernel<true, true> : score_embed_kernel<false, true>)
+                            : (tau ? score_embed_kernel<true, false> : score_embed_kernel<false, false>);
+        embed<<<(unsigned)blocks, 256, 0, st>>>(static_cast<const __half*>(c.embPrev), static_cast<const __half*>(c.embCur), c.audio, c.codes, c.N, c.t0,
+                                                M, c.Bs, R, c.tanhEmbed, c.xf, x0, tau, c.segs_dev);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
     for (int l = 0; l < c.L; l++) {
@@ -612,7 +700,9 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
         a.lh = c.lh + (size_t)l * c.Be * 2 * R;
         a.lh_t = (size_t)c.L * c.Be * 2 * R;
         a.M = M; a.Bs = c.Bs;
-        e = R == 32 ? launch_layer<32>(a, st) : R == 64 ? launch_layer<64>(a, st) : launch_layer<128>(a, st);
+        x.oW1 = o.W1 + (size_t)l * 4 * R * R * 2; x.oWr = o.Wr + (size_t)l * R * R * 2;
+        x.oBh = o.Bh + (size_t)l * 2 * R * 4; x.oBr = o.Br + (size_t)l * R * 4;
+        e = R == 32 ? launch_layer<32>(a, x, st) : R == 64 ? launch_layer<64>(a, x, st) : launch_layer<128>(a, x, st);
         if (e != cudaSuccess) return e;
     }
     OutArgs a;
@@ -621,5 +711,5 @@ cudaError_t wn_score_chunk(const WnScoreChunk& c, cudaStream_t st)
     a.Bsk = reinterpret_cast<const float*>(im + o.Bsk); a.Bzs = reinterpret_cast<const float*>(im + o.Bzs); a.Bza = reinterpret_cast<const float*>(im + o.Bza);
     a.audio = c.audio; a.N = c.N; a.t0 = c.t0; a.M = M; a.Bs = c.Bs;
     a.logp = c.logp; a.logits = c.logits; a.logits_ld = c.logits_ld; a.logits_t0 = c.logits_t0;
-    return c.S == 128 ? launch_out<128>(a, st) : launch_out<256>(a, st);
+    return c.S == 128 ? launch_out<128>(a, x, st) : launch_out<256>(a, x, st);
 }

@@ -438,6 +438,15 @@ class NVWavenetInfer:
         m = np.ascontiguousarray(m.astype(np.int32))
         check(self._l.nvwn_set_group_models(self._h, C.c_void_p(m.ctypes.data), m.size, _stream(stream)), "setGroupModels")
 
+    def set_score_models(self, models, stream=None):
+        """The model of each of the B scoring rows: 0 or a model given to set_model.  Applies to the scoring calls from the next one;
+        ends an open scoring stream; see nvwn_set_score_models."""
+        m = np.asarray(models, dtype=np.int64).ravel()
+        if m.size and (m.min() < np.iinfo(np.int32).min or m.max() > np.iinfo(np.int32).max):
+            raise ValueError(f"setScoreModels: model indices must fit a C int; got {m.min()} .. {m.max()}")
+        m = np.ascontiguousarray(m.astype(np.int32))
+        check(self._l.nvwn_set_score_models(self._h, C.c_void_p(m.ctypes.data), m.size, _stream(stream)), "setScoreModels")
+
     def cond_producer_run_slots(self, slots, first_sample, num_samples, stream=None):
         """Conditioning of absolute samples [first_sample, first_sample + num_samples), num_samples <= N, for `slots` only, from
         their attached utterances (0 past an utterance's end).  Asynchronous on `stream`."""

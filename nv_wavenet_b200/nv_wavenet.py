@@ -130,6 +130,35 @@ def plan_packed(lengths, slots):
     return plan
 
 
+def plan_packed_models(lengths, models, slots):
+    """Packed scoring schedule of ModelSet.log_likelihood_many: utterances of `lengths` samples, utterance u scored with model
+    models[u], through `slots` rows that each keep one model.  The rows are split among the distinct models, in model order, in
+    proportion to their total samples: each gets 1 + floor((slots - V) * share) rows, V distinct models, and the rows left over
+    go to the model of most samples (the lowest on ties).  Within a model's rows its utterances, in arrival order, follow
+    plan_packed.  Returns (plan, table): [(row, start)] per utterance, and the model of each row."""
+    if len(models) != len(lengths) or any(int(m) != m or m < 0 for m in models):
+        raise ValueError(f"need one model index >= 0 per utterance; got {len(models)} for {len(lengths)} utterances")
+    if any(n < 1 for n in lengths):
+        raise ValueError("every utterance needs at least one sample")
+    totals = {}
+    for n, m in zip(lengths, models):
+        totals[int(m)] = totals.get(int(m), 0) + n
+    used = sorted(totals)
+    if slots < len(used):
+        raise ValueError(f"{len(used)} distinct models need at least as many slots; got {slots}")
+    whole = sum(totals.values())
+    rows = {m: 1 + (slots - len(used)) * totals[m] // whole for m in used}
+    rows[max(used, key=lambda m: (totals[m], -m))] += slots - sum(rows.values())
+    plan, table, base = [None] * len(lengths), [], 0
+    for m in used:
+        mine = [u for u in range(len(lengths)) if models[u] == m]
+        for u, (s, start) in zip(mine, plan_packed([lengths[u] for u in mine], rows[m])):
+            plan[u] = (base + s, start)
+        table += [m] * rows[m]
+        base += rows[m]
+    return plan, table
+
+
 def _packed_windows(plan, lengths, window):
     """The windows of a plan_packed schedule at multiples of `window`: per window (first sample, samples, segments), a segment
     (slot, utterance, its first sample in the utterance, its first sample in the window, samples) for every utterance that has
@@ -846,28 +875,33 @@ class NVWaveNet:
         eng = self._engine(slots, window, fp16)
         st = torch.cuda.current_stream()
         timer = _Timer(timing)
-
-        def prime(k):
-            # the prompted utterances starting at this boundary, by prompt length, are the rows of one scoring stream through the
-            # engine's own conditioning store (free now that the last window was generated); each slot is primed from its row
-            group = sorted((u for u in windows[k][2] if prompts[u] is not None), key=lambda u: skip[u])
-            if not group:
-                return
-            timer.mark("prime")
-
-            def fill(a, m):
-                lh = self._gather(cond_inputs, m, len(group), [(j, u, a, 0, min(skip[u], a + m) - a) for j, u in enumerate(group) if skip[u] > a])
-                eng.set_conditioning_slots(lh, list(range(len(group))), a, stream=st)
-
-            def at_end(rows):
-                eng.prime_slots_from_score(rows, [plan[group[j]][0] for j in rows], [seeds[group[j]] for j in rows], stream=st)
-
-            _score_prompt_group(eng, [prompts[u] for u in group], fill, at_end, stream=st)
-            timer.mark("primed")
-
+        prime = lambda k: self._prime(eng, windows[k], plan, prompts, skip, cond_inputs, seeds, timer)
         outs = self._serve_queue(eng, plan, windows, lengths, skip, cond_inputs, seeds, timer, prime, prompts)
         timer.report(prime_s=("prime", "primed"))
         return outs
+
+    def _prime(self, eng, window, plan, prompts, skip, cond_inputs, seeds, timer, score_models=None):
+        """The prompts of a prompted queue that start at one window boundary (window: its _windows entry): the prompted utterances
+        starting there, by prompt length, are the rows of one scoring stream through the engine's own conditioning store (free now
+        that the last window was generated), and each slot is primed from its row.  score_models: None, or called with those
+        utterances before they are scored.  timer: marked "prime" before and "primed" after, when there are any."""
+        st = torch.cuda.current_stream()
+        group = sorted((u for u in window[2] if prompts[u] is not None), key=lambda u: skip[u])
+        if not group:
+            return
+        timer.mark("prime")
+        if score_models is not None:
+            score_models(group)
+
+        def fill(a, m):
+            lh = self._gather(cond_inputs, m, len(group), [(j, u, a, 0, min(skip[u], a + m) - a) for j, u in enumerate(group) if skip[u] > a])
+            eng.set_conditioning_slots(lh, list(range(len(group))), a, stream=st)
+
+        def at_end(rows):
+            eng.prime_slots_from_score(rows, [plan[group[j]][0] for j in rows], [seeds[group[j]] for j in rows], stream=st)
+
+        _score_prompt_group(eng, [prompts[u] for u in group], fill, at_end, stream=st)
+        timer.mark("primed")
 
     def _serve_queue(self, eng, plan, windows, lengths, skip, cond_inputs, seeds, timer, before, prompts=None):
         """The queue of infer_many and ModelSet.infer_many once it is planned: the engine reset, then _serve with before(k) and
@@ -1001,11 +1035,19 @@ class NVWaveNet:
         without a window, so one window of the whole length; with window=W the engine holds W samples of conditioning instead of
         all of them, and the result is the same as without a window, bit for bit.  Either way the engine's scoring stream is left
         open, so the last window also carries every layer's front for a call that would continue it."""
+        batch_size, sample_count = self._check_scoring(cond_input, audio, window)
+        return self._score_cond(self._engine(batch_size, window or sample_count, True), cond_input, audio)
+
+    def _check_scoring(self, cond_input, audio, window):
+        """(batch, samples) of log_likelihood's arguments, checked"""
         batch_size, sample_count = self._cond_size(cond_input)
         if tuple(audio.size()) != (batch_size, sample_count):
             raise AssertionError(f"audio must be [batch][samples] = {(batch_size, sample_count)}; got {tuple(audio.size())}")
         _check_window(window)
-        eng = self._engine(batch_size, window or sample_count, True)
+        return batch_size, sample_count
+
+    def _score_cond(self, eng, cond_input, audio):
+        """log_likelihood on the fp16 engine `eng`, its arguments checked"""
         # converted a window at a time, so a windowed call never holds an fp32 copy of the whole length
         fill = lambda first, n: eng.set_conditioning(column_major(cond_input[..., first:first + n]).float(), 0, n)
         return self._score(eng, audio.to(device="cuda", dtype=torch.int32), fill)
@@ -1170,31 +1212,81 @@ class ModelSet:
             self._engines[key] = eng
         return eng
 
-    def infer_many(self, models, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None):
+    def _check_models(self, models, n, what="utterances"):
+        """models as ints, checked: one per utterance (or row), each in [0, len(nets))"""
+        if len(models) != n:
+            raise AssertionError(f"{len(models)} models for {n} {what}")
+        if any(int(m) != m or not 0 <= m < len(self.nets) for m in models):
+            raise AssertionError(f"every model index is in [0, {len(self.nets)})")
+        return [int(m) for m in models]
+
+    def infer_many(self, models, cond_inputs, seeds, slots=64, window=4096, fp16=False, timing=None, prompts=None):
         """NVWaveNet.infer_many over several models: utterance u runs net models[u].  One engine of `slots` slots and `window`
         samples serves the whole queue; its slots are in groups of eng.model_group that run one model at a time, scheduled by
         plan_slots(..., models, group), and before each window's restarts the engine's group table is set to the models of the
         window's live utterances.  Returns int32 CUDA tensors [n_u], each bit-identical to
-        nets[models[u]].infer(cond_u[:, None], Impl.AUTO, seed=seeds[u], fp16=fp16)[0].  timing: a dict, or None; if given,
-        receives the GPU seconds spent in restarts and per-slot uploads ("restart_upload_s") and in generation ("generate_s")."""
+        nets[models[u]].infer(cond_u[:, None], Impl.AUTO, seed=seeds[u], fp16=fp16)[0].
+        prompts: None, or per utterance None or int mu-law codes [P_u], as NVWaveNet.infer_many takes them (fp16 only).  At a
+        boundary where prompted utterances start, the group table is set first, then the scoring table gives each of their
+        scoring rows its utterance's model (nvwn_set_score_models), and they are scored and primed as NVWaveNet.infer_many does;
+        each is bit-identical to nets[models[u]].infer(cond_u[:, None], Impl.AUTO, seed=seeds[u], fp16=True, prompt=p_u)[0].
+        timing: a dict, or None; if given, receives the GPU seconds spent in restarts and per-slot uploads ("restart_upload_s"), in
+        generation ("generate_s") and, with prompts, in scoring and priming them ("prime_s")."""
         net = self.nets[0]
         if not (len(models) == len(cond_inputs) == len(seeds)):
             raise AssertionError(f"{len(models)} models, {len(cond_inputs)} utterances and {len(seeds)} seeds")
-        if any(int(m) != m or not 0 <= m < len(self.nets) for m in models):
-            raise AssertionError(f"every model index is in [0, {len(self.nets)})")
+        models = self._check_models(models, len(cond_inputs))
         lengths = net._check_utterances(cond_inputs)
-        models = [int(m) for m in models]
+        prompts = net._slot_prompts(prompts, lengths, fp16)
+        skip = [0 if p is None else int(p.numel()) for p in prompts]
+        made = [n - P for n, P in zip(lengths, skip)]                      # the generated samples
         eng = self._engine(slots, window, fp16)
         group = eng.model_group
-        plan = plan_slots(lengths, slots, window, models, group)
-        windows = _windows(plan, lengths, window)
+        plan = plan_slots(made, slots, window, models, group)
+        windows = _windows(plan, made, window)
         st = torch.cuda.current_stream()
+        timer = _Timer(timing)
 
-        def tables(k):
+        def before(k):
             first, count, _, _ = windows[k]
-            eng.set_group_models(group_models(plan, lengths, models, first, count, group, slots), stream=st)
+            eng.set_group_models(group_models(plan, made, models, first, count, group, slots), stream=st)
+            net._prime(eng, windows[k], plan, prompts, skip, cond_inputs, seeds, timer,
+                       lambda us: eng.set_score_models([models[u] for u in us] + [0] * (slots - len(us)), stream=st))
 
-        return net._serve_queue(eng, plan, windows, lengths, [0] * len(lengths), cond_inputs, seeds, _Timer(timing), tables)
+        outs = net._serve_queue(eng, plan, windows, lengths, skip, cond_inputs, seeds, timer, before, prompts)
+        if any(p is not None for p in prompts):
+            timer.report(prime_s=("prime", "primed"))
+        return outs
+
+    def log_likelihood(self, models, cond_input, audio, window=None):
+        """NVWaveNet.log_likelihood over several models: batch row b is scored with net models[b] (nvwn_set_score_models), all rows
+        in one fp16 engine of the batch and W samples.  Returns a float32 CUDA tensor [batch][samples] whose row b is, bit for bit,
+        nets[models[b]].log_likelihood of that row, windowed or not."""
+        net = self.nets[0]
+        batch_size, sample_count = net._check_scoring(cond_input, audio, window)
+        models = self._check_models(models, batch_size, "batch rows")
+        eng = self._engine(batch_size, window or sample_count, True)
+        eng.set_score_models(models)
+        return net._score_cond(eng, cond_input, audio)
+
+    def log_likelihood_many(self, models, cond_inputs, audios, slots=64, window=4096, timing=None):
+        """NVWaveNet.log_likelihood_many over several models: utterance u is scored with net models[u].  The rows of one fp16 engine
+        of `slots` rows and `window` samples are split among the queue's models (plan_packed_models), each row keeping its model for
+        the whole stream, and packed within each model as plan_packed does.  Returns float32 CUDA tensors [n_u], each bit-identical
+        to nets[models[u]].log_likelihood_many([c_u], [a_u])[0].  timing as for NVWaveNet.log_likelihood_many."""
+        net = self.nets[0]
+        lengths = net._check_utterances(cond_inputs)
+        models = self._check_models(models, len(lengths))
+        _check_rows("log_likelihood_many", "slots", slots, window)
+        plan, table = plan_packed_models(lengths, models, slots)
+        audios = net._check_queue("log_likelihood_many", lengths, audios, slots, window)
+        eng = self._engine(slots, window, True)
+        eng.set_score_models(table)
+
+        def fill(first, count, segs):
+            eng.set_conditioning(net._gather(cond_inputs, count, slots, segs), 0, count)
+
+        return net._score_packed(eng, plan, lengths, audios, fill, timing)
 
     def close(self):
         for eng in self._engines.values():
