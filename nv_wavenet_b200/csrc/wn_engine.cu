@@ -71,33 +71,39 @@ struct CudaFree {
 };
 template <typename T>
 struct DevBuf : std::unique_ptr<T, CudaFree> {
+    size_t bytes = 0;                        // of the allocation held
     operator T*() const { return this->get(); }
-    cudaError_t alloc(size_t bytes)
+    cudaError_t alloc(size_t n)
     {
         void* p = nullptr;
-        const cudaError_t ce = cudaMalloc(&p, bytes);
-        if (ce == cudaSuccess) this->reset(static_cast<T*>(p));
+        const cudaError_t ce = cudaMalloc(&p, n);
+        if (ce == cudaSuccess) {
+            this->reset(static_cast<T*>(p));
+            bytes = n;
+        }
         return ce;
+    }
+    // At least n bytes.  A larger buffer replaces a smaller one after a device synchronise, so that no launch reads the old one any
+    // more; the contents do not carry over.
+    cudaError_t reserve(size_t n)
+    {
+        if (n <= bytes) return cudaSuccess;
+        const cudaError_t ce = this->get() ? cudaDeviceSynchronize() : cudaSuccess;
+        return ce != cudaSuccess ? ce : alloc(n);
     }
 };
 
 // A conditioning producer (DESIGN.md §6): a network of C channels, upsampling window K and stride; `scratch` of cond_scratch()'s
 // layout, chunks of up to `rows` (row, sample) rows; row b's frames [C][T[b]] at frames + b * cap * C; the row list and WnCondSlot
 // table of the last production (device); per row on the host, the frames of its utterance (0: none) and its absolute start.
-// A live sequence of the whole-batch producer (nvwn_cond_producer_open_live) keeps row b's frames in a ring [C][ring] at
-// frames + b * ring * C, T[b] counting the frames pushed so far, and `produced` is the end of its furthest production: the
-// frames the samples from there on read may not be overwritten.
-// In live mode the per-slot producer (nvwn_cond_producer_open_live_slots) keeps slot s's frames in a ring [C][ring] at
-// frames + s * ring * C (cap = ring), and per slot whether a live utterance is attached, the first frame it was attached with
-// (the frames before it left the ring elsewhere) and the end of its furthest production, in its own samples.
+// Live, both producers (nvwn_cond_producer_open_live, _open_live_slots) keep row b's frames in a ring [C][ring] at frames + b * ring * C
+// (cap = ring), T[b] counting the frames pushed; per row whether a live utterance is attached (per-slot only), the first frame it was
+// attached with (0 for the whole batch) and the end `done` of its furthest production, in its own samples.
 struct CondProducer {
     int C = 0, K = 0, stride = 0, rows = 0;
     int ring = 0;                            // frames per row of a live sequence's ring; 0: frames loaded whole
-    long long produced = 0;
     DevBuf<float> scratch;
-    size_t scratch_floats = 0;
     DevBuf<float> frames;
-    size_t frames_floats = 0;
     int cap = 0;
     DevBuf<char> tables;                     // int [B] rows, then WnCondSlot [B] at cond_table_offset
     std::vector<int> T;
@@ -114,8 +120,7 @@ struct nvwn_engine : WnConfig {
     size_t td;                               // sizeof(TD)
     const WnFamily* family;                  // the kernel family of `kernel`: the layouts of Lh, ring and image, and the launch
 
-    // packed weight blob (TD elements), offsets in bytes
-    DevBuf<char> blob;
+    // bytes of a packed weight blob (TD elements, models[m].blob), and the offsets in it
     size_t blob_bytes = 0;
     size_t o_embPrev, o_embCur, o_Wprev, o_Wcur, o_Wres, o_Wskip, o_Wzs, o_Wza, o_Bh, o_Bres, o_Bskip, o_Bzs, o_Bza;
 
@@ -151,22 +156,18 @@ struct nvwn_engine : WnConfig {
     bool early_prime = false;
     // device staging of slot states in host memory (nvwn_save_slots, nvwn_load_slots), grown on demand
     DevBuf<char> state_stage;
-    size_t state_stage_bytes = 0;
 
-    DevBuf<void> image;                      // the family's weight image, packed from the blob before the first launch after a change
-    bool image_dirty = true;
-
-    // Multi-model serving (nvwn_set_model, DESIGN.md §6).  Models 1 .. NVWN_MAX_MODELS - 1, each with a blob copied from its source
-    // and the family's image, packed before the first launch after a change; model 0 is blob and image above.  model_tab holds
-    // every model's bases for the kernels (device [NVWN_MAX_MODELS]); entry m is written when model m is first set, and its buffers
-    // never move after that.  group_tab is the model of each group of group_rows rows (device [ceil(B / group_rows)]), and
-    // group_host its host copy, empty until nvwn_set_group_models: then launches look the models up.
+    // The models (DESIGN.md §6): model 0 is the engine's own weights (the setters), models 1 .. NVWN_MAX_MODELS - 1 copies of source
+    // engines' (nvwn_set_model).  A model's blob and the family's image, packed from it before the first launch after a change, are
+    // allocated by nvwn_create for model 0 and when first set for the others, and never move: model_tab holds their bases for the
+    // kernels (device [NVWN_MAX_MODELS]).  group_tab is the model of each group of group_rows rows (device [ceil(B / group_rows)]),
+    // and group_host its host copy, empty until nvwn_set_group_models: then launches look the models up.
     struct Model {
         DevBuf<char> blob;
         DevBuf<void> image;
-        bool dirty = true;
+        bool repack = true;
         DevBuf<void> score_image;            // the scorer's image of the model, allocated and packed on the first scoring call that
-        bool score_dirty = true;             // runs the model after a change
+        bool score_repack = true;            // runs the model after a change
     };
     std::vector<Model> models;
     DevBuf<WnModel> model_tab;
@@ -179,9 +180,7 @@ struct nvwn_engine : WnConfig {
     // calls may be interleaved
     CondProducer cond_whole, cond_slots;
 
-    // teacher-forced scoring (nvwn_score): pre-tiled fp16 weight image + chunk scratch, allocated on the first call
-    DevBuf<void> score_image;
-    bool score_dirty = true;                 // set with image_dirty (weights_changed): the image is repacked on the next scoring call
+    // teacher-forced scoring (nvwn_score): chunk scratch, allocated on the first call (each model's image is in models)
     DevBuf<char> score_scratch;
     int score_T = 0;                         // time steps per chunk: SCORE_ROWS / B
     // the open scoring stream (nvwn_score_stream): the absolute sample its next call starts at, -1 if none is open, its batch_size,
@@ -203,8 +202,6 @@ struct nvwn_engine : WnConfig {
 
     WnLaunchInfo last{};
     unsigned long long launches = 0;
-
-    template <typename T> T* at(size_t off) const { return reinterpret_cast<T*>(blob + off); }
 };
 
 namespace {
@@ -270,11 +267,7 @@ int put_cond_network(nvwn_engine* e, CondProducer& P, const std::string& who, in
     const size_t lrow = (size_t)e->L * 2 * e->R;                             // floats of one (row, sample) of conditioning
     const size_t rows = ((size_t)16 << 20) / lrow > (size_t)e->B ? ((size_t)16 << 20) / lrow : (size_t)e->B;
     const CondScratch o = cond_scratch(e, C, K, (int)rows);
-    if (o.floats > P.scratch_floats) {
-        if (P.scratch) CK(cudaDeviceSynchronize());                         // no launch reads the old scratch any more
-        CK(P.scratch.alloc(o.floats * sizeof(float)));
-        P.scratch_floats = o.floats;
-    }
+    CK(P.scratch.reserve(o.floats * sizeof(float)));
     if (!P.tables) CK(P.tables.alloc(cond_table_offset(e) + (size_t)e->B * sizeof(WnCondSlot)));
     P.C = C; P.K = K; P.stride = stride; P.rows = (int)rows;
     float* w = P.scratch;
@@ -349,18 +342,40 @@ int check_run_batch(const nvwn_engine* e, const std::string& who, int batch)
     return 0;
 }
 
+// Checks a list of n indices (host memory): every one in [0, bound), none twice.  A refusal names an index as `noun` and follows the
+// bound with `note`.
+int check_list(const std::string& who, const int* list, int n, int bound, const char* noun, const char* note)
+{
+    std::vector<char> seen(bound, 0);
+    for (int i = 0; i < n; i++) {
+        const std::string x = std::string(noun) + " " + std::to_string(list[i]);
+        if (list[i] < 0 || list[i] >= bound) return fail(NVWN_EINVAL, who + ": " + x + " is outside [0, " + std::to_string(bound) + ")" + note);
+        if (seen[list[i]]) return fail(NVWN_EINVAL, who + ": " + x + " is given twice");
+        seen[list[i]] = 1;
+    }
+    return 0;
+}
+
 // Checks the slot list of a per-slot call (host memory): 1 <= n <= B, every slot in [0, B), none twice.
 int check_slots(const nvwn_engine* e, const std::string& who, const int* slots, int n)
 {
     if (!slots) return fail(NVWN_EINVAL, who + ": slots is NULL");
     if (n < 1 || n > e->B) return fail(NVWN_EINVAL, who + ": need 1 <= n <= B (" + std::to_string(e->B) + "); got n = " + std::to_string(n));
-    std::vector<char> seen(e->B, 0);
-    for (int i = 0; i < n; i++) {
-        if (slots[i] < 0 || slots[i] >= e->B)
-            return fail(NVWN_EINVAL, who + ": slot " + std::to_string(slots[i]) + " is outside [0, " + std::to_string(e->B) + ")");
-        if (seen[slots[i]]) return fail(NVWN_EINVAL, who + ": slot " + std::to_string(slots[i]) + " is given twice");
-        seen[slots[i]] = 1;
-    }
+    return check_list(who, slots, n, e->B, "slot", "");
+}
+
+// Checks a list of n scoring rows of the open scoring stream (host memory): every row in [0, Bs), none twice.
+int check_rows(const nvwn_engine* e, const std::string& who, const int* rows, int n)
+{
+    return check_list(who, rows, n, e->score_bs, "row", " (the scoring stream's batch_size)");
+}
+
+// Checks that a model table names only model 0 and models given to nvwn_set_model: entry i of `what` ("group", "row") is models[i].
+int check_models(const nvwn_engine* e, const std::string& who, const char* what, const int* models, int n)
+{
+    for (int i = 0; i < n; i++)
+        if (models[i] < 0 || models[i] >= NVWN_MAX_MODELS || !e->models[models[i]].blob)
+            return fail(NVWN_EINVAL, who + ": " + what + " " + std::to_string(i) + " names model " + std::to_string(models[i]) + ", which was never set");
     return 0;
 }
 
@@ -378,17 +393,32 @@ int take_slots(nvwn_engine* e, const std::string& who, const int* slots, int n, 
     return 0;
 }
 
-// The weights changed: both images are repacked before their next use, and an open scoring stream ends (its carried layer inputs
-// were computed with the old weights).
+// Model m's weights changed: both its images are repacked before their next use.
+void model_changed(nvwn_engine* e, int m) { e->models[m].repack = e->models[m].score_repack = true; }
+
+// Model 0's weights changed: model_changed, and an open scoring stream ends (its carried layer inputs used the old weights).
 void weights_changed(nvwn_engine* e)
 {
-    e->image_dirty = e->score_dirty = true;
+    model_changed(e, 0);
     e->score_next = -1;
 }
 
-// dst (TD, device) <- src (fp32, host or device), n elements
-int upload(nvwn_engine* e, void* dst, const float* src, size_t n)
+// Gives model m a blob and the family's image, and writes their bases into entry m of model_tab
+int add_model(nvwn_engine* e, int m)
 {
+    nvwn_engine::Model fresh;
+    CK(fresh.blob.alloc(e->blob_bytes));
+    if (e->family->pack) CK(fresh.image.alloc(e->family->image_bytes(*e)));
+    const WnModel bases{fresh.blob, fresh.image};
+    CK(cudaMemcpy(e->model_tab + m, &bases, sizeof bases, cudaMemcpyHostToDevice));
+    e->models[m] = std::move(fresh);
+    return 0;
+}
+
+// Model 0's blob at byte offset off (TD, device) <- src (fp32, host or device), n elements
+int upload(nvwn_engine* e, size_t off, const float* src, size_t n)
+{
+    void* dst = e->models[0].blob + off;
     return feed(e, src, n, 1, false, 0, [&](const float* s, size_t first, size_t m) {
         return e->dtype == NVWN_FP16 ? wn_f32_to_f16(static_cast<__half*>(dst) + first, s, m, 0)
                                      : cudaMemcpyAsync(static_cast<float*>(dst) + first, s, m * sizeof(float), cudaMemcpyDefault, 0);
@@ -456,7 +486,7 @@ void fill_params(const nvwn_engine* e, WnParams& p, int init_sample, long long t
     p.ring_slot = (int)(t_abs % (e->maxDil + 1));
     p.hist_t = (int)(t_abs < e->maxDil && !e->early_prime ? t_abs : e->maxDil);
     p.tanhEmbed = e->tanhEmbed; p.dump = dump;
-    point_weights(e, p, e->blob);
+    point_weights(e, p, e->models[0].blob);
     p.Lh = e->Lh; p.sel = e->sel; p.forced = e->use_forced ? e->forced.get() : nullptr;
     p.yPrev = e->yPrev; p.yCur = e->yCur; p.ring = e->ring; p.yOut = e->yOut;
     p.xtOut = e->xtOut; p.skipOut = e->skipOut; p.Zs = e->Zs; p.Za = e->Za; p.P = e->P;
@@ -477,18 +507,14 @@ int launch_steps(nvwn_engine* e, const char* who, int pos, long long t_abs, int 
         if (e->prime_bs && batch != e->prime_bs)
             return fail(NVWN_EINVAL, std::string(who) + ": after nvwn_prime_from_score runs need batch_size equal to the primed batch_size (" +
                                      std::to_string(e->prime_bs) + ") until nvwn_reset_history; got " + std::to_string(batch));
-        if (e->family->pack && e->image_dirty) {
-            CK(e->family->pack(e->image, p, stream));
-            e->image_dirty = false;
-        }
         for (nvwn_engine::Model& m : e->models) {
-            if (!e->family->pack || !m.blob || !m.dirty) continue;
+            if (!e->family->pack || !m.blob || !m.repack) continue;
             WnParams q = p;
             point_weights(e, q, m.blob);
             CK(e->family->pack(m.image, q, stream));
-            m.dirty = false;
+            m.repack = false;
         }
-        CK(e->family->launch(*e, p, e->image, stream, &e->last));
+        CK(e->family->launch(*e, p, e->models[0].image, stream, &e->last));
         e->launches++;
     }
     e->next_t = t_abs + count;
@@ -524,17 +550,18 @@ ScoreScratch score_scratch_layout(const nvwn_engine* e, int T)
     return o;
 }
 
-// The preamble both primes share: an fp16 engine with an open scoring stream of P >= 1 samples.
-int check_prime(const nvwn_engine* e, const std::string& who)
+// The preamble of the calls that take the layer fronts of the open scoring stream (the primes, nvwn_score_save_states): an fp16
+// engine with an open scoring stream of P >= 1 samples, not packed.  `fronts` says what the caller takes the fronts for.
+int check_open_stream(const nvwn_engine* e, const std::string& who, const char* fronts)
 {
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score, so only they can be primed");
+    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score");
     if (e->score_next < 1)
         return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one): score the prompt with nvwn_score_stream "
                                        "from first_sample = 0 first");
     if (e->score_packed)
         return fail(NVWN_EUNSUPPORTED, who + ": the scoring stream is packed (nvwn_score_stream_packed): a row's layer fronts may hold an earlier "
-                                             "utterance's inputs, so they are no history to generate from");
+                                             "utterance's inputs, so they are no " + fronts);
     return 0;
 }
 
@@ -574,27 +601,81 @@ int put_fronts(const nvwn_engine* e, Write write)
     return 0;
 }
 
-// The earliest frame a live slot of the per-slot producer still holds: frames before `first` left the ring before the attach,
-// and a ring of P.ring frames holds [T - ring, T)
-long long live_held(const CondProducer& P, int s)
+// The sizes of a conditioning network: C >= 1 channels, window K >= stride >= 1
+int check_cond_sizes(const std::string& who, int C, int K, int stride)
 {
-    const long long wrap = (long long)P.T[s] - P.ring;
-    return wrap > P.first[s] ? wrap : P.first[s];
+    if (C >= 1 && stride >= 1 && K >= stride) return 0;
+    return fail(NVWN_EINVAL, who + ": bad sizes (need n_cond_channels >= 1 and window >= stride >= 1)");
 }
 
-// Frames [C][num] at src (host or device) -> frames T .. T + num - 1 of slot s's live ring, split at the wrap.  A host source is
-// snapshotted into pageable memory, which the copies stage before they return: the caller's array is free again on return.
-int put_live_frames(CondProducer& P, int s, long long T, const float* src, int num, cudaStream_t st)
+// A live ring holds at least the frames one sample reads, and one frame more
+int check_ring_frames(const std::string& who, int ring_frames, int K, int stride)
+{
+    const int least = (K + stride - 1) / stride + 1;
+    if (ring_frames >= least) return 0;
+    return fail(NVWN_EINVAL, who + ": ring_frames = " + std::to_string(ring_frames) + "; need at least ceil(window / stride) + 1 = " +
+                                 std::to_string(least));
+}
+
+// Row r's entry of P's WnCondSlot table, with T frames
+WnCondSlot cond_row(const CondProducer& P, int r, int T) { return {(long long)r * P.cap * P.C, P.start[r], T, P.ring}; }
+
+// The WnCondSlot table of rows rows[0..n) (NULL: 0 .. n - 1) with their frames of now, and the row list if given, into P.tables in
+// one copy staged from pageable memory in stream order: the caller's arrays are free again on return
+int put_cond_table(const nvwn_engine* e, const CondProducer& P, const int* rows, int n, cudaStream_t st)
+{
+    const size_t off = cond_table_offset(e), skip = rows ? 0 : off;
+    std::vector<char> host(off + (size_t)n * sizeof(WnCondSlot));
+    if (rows) memcpy(host.data(), rows, (size_t)n * sizeof(int));
+    WnCondSlot* tab = reinterpret_cast<WnCondSlot*>(host.data() + off);
+    for (int i = 0; i < n; i++) tab[i] = cond_row(P, rows ? rows[i] : i, P.T[rows ? rows[i] : i]);
+    CK(cudaMemcpyAsync(P.tables + skip, host.data() + skip, host.size() - skip, cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+// A production of row r of a live sequence from sample n of its utterance reads frames from first_frame(n) on: they must still be in
+// the ring, which holds [T - ring, T) and none before the frame the row was attached with.  `of` names the row's utterance in a refusal.
+int check_held(const CondProducer& P, const std::string& who, int r, long long n, const std::string& of)
+{
+    const long long need = first_frame(n, P.K, P.stride), wrap = (long long)P.T[r] - P.ring, held = wrap > P.first[r] ? wrap : P.first[r];
+    if (need >= held) return 0;
+    return fail(NVWN_EINVAL, who + ": frame " + std::to_string(need) + ", which sample " + std::to_string(n) + of + " reads, has left the ring (it holds frames " +
+                                 std::to_string(held) + " .. " + std::to_string(P.T[r] - 1) + ")");
+}
+
+// A push of num frames to row r of a live sequence overwrites frames [T - ring, T + num - ring): the samples from done[r] on read
+// frames from first_frame(done[r]), and the frames before first[r] are gone already.  `of` names the row in a refusal.
+int check_push(const CondProducer& P, const std::string& who, int r, int num, const std::string& of)
+{
+    const long long ff = first_frame(P.done[r], P.K, P.stride), keep = ff > P.first[r] ? ff : P.first[r];
+    if ((long long)P.T[r] + num - P.ring <= keep) return 0;
+    return fail(NVWN_EINVAL, who + ": " + std::to_string(num) + " frames would overwrite frame " + std::to_string(keep) + of + ", which sample " +
+                                 std::to_string(P.done[r]) + " (not produced yet) reads; at most " + std::to_string(keep + P.ring - P.T[r]) +
+                                 " frames fit before production moves on");
+}
+
+// Rows rows[0..n) of P (NULL: 0 .. n - 1) have been produced up to absolute sample `end`
+void mark_produced(CondProducer& P, const int* rows, int n, long long end)
+{
+    for (int i = 0; i < n; i++) {
+        const int r = rows ? rows[i] : i;
+        if (end - P.start[r] > P.done[r]) P.done[r] = end - P.start[r];
+    }
+}
+
+// Frames [rows][C][num] at src (host or device) -> frames T .. T + num - 1 of the rings of rows row .. row + rows - 1, split at the
+// wrap.  A host source is snapshotted into pageable memory, which the copies stage before they return: the caller's array is free.
+int put_live_frames(CondProducer& P, int row, int rows, long long T, const float* src, int num, cudaStream_t st)
 {
     std::vector<float> snap;
     if (!is_device_ptr(src)) {
-        snap.assign(src, src + (size_t)P.C * num);
+        snap.assign(src, src + (size_t)rows * P.C * num);
         src = snap.data();
     }
     const size_t f = sizeof(float);
     for (const WrapPiece& w : split_at_wrap(T, num, P.ring))
-        CK(cudaMemcpy2DAsync(P.frames + (size_t)s * P.ring * P.C + w.pos, (size_t)P.ring * f, src + w.off, (size_t)num * f, (size_t)w.len * f, P.C,
-                             cudaMemcpyDefault, st));
+        CK(cudaMemcpy2DAsync(P.frames + (size_t)row * P.ring * P.C + w.pos, (size_t)P.ring * f, src + w.off, (size_t)num * f, (size_t)w.len * f,
+                             (size_t)rows * P.C, cudaMemcpyDefault, st));
     return 0;
 }
 
@@ -611,14 +692,81 @@ int state_layers(const nvwn_engine* e, Part part)
     return 0;
 }
 
-// The engine's staging buffer for slot states, at least `bytes` long
-int state_stage(nvwn_engine* e, size_t bytes)
+// Slot states at `states`, host or device memory (*host); device states need a 16-byte alignment
+int check_states(const std::string& who, const void* states, bool* host)
 {
-    if (bytes <= e->state_stage_bytes) return 0;
-    if (e->state_stage) CK(cudaDeviceSynchronize());                        // no launch reads the old buffer any more
-    CK(e->state_stage.alloc(bytes));
-    e->state_stage_bytes = bytes;
+    *host = !is_device_ptr(states);
+    if (!*host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
     return 0;
+}
+
+// Writes n slot states to `states` (host or device memory) through write(dst): device states in place, host states into the
+// engine's staging buffer and from there to `states` before return.
+template <typename Write>
+int write_states(nvwn_engine* e, const std::string& who, void* states, int n, cudaStream_t st, Write write)
+{
+    bool host;
+    int rc = check_states(who, states, &host);
+    if (rc != 0) return rc;
+    const size_t bytes = (size_t)n * wn_slot_state_bytes(*e);
+    if (host) CK(e->state_stage.reserve(bytes));
+    char* dst = host ? e->state_stage.get() : static_cast<char*>(states);
+    if ((rc = write(dst))) return rc;
+    if (host) {
+        CK(cudaMemcpyAsync(states, dst, bytes, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    return 0;
+}
+
+// Before a call writes real history into rows at next_t < maxDil: from then on every launch reads the ring at every step, so the
+// entries of the negative times, which no row has written since the reset, must read as the zeros of "before the start".
+int clear_early_times(nvwn_engine* e, cudaStream_t st)
+{
+    const long long t0 = e->next_t;
+    const int M = e->maxDil + 1;
+    if (t0 < e->maxDil && !e->early_prime) {
+        CK(e->family->clear_times(*e, e->ring, t0 - M, (int)(M - t0), st));
+        e->early_prime = true;
+    }
+    return 0;
+}
+
+// Model v's scorer image for a scoring call of parameters p: allocated on first use, packed from the model's blob after a change
+int put_score_image(nvwn_engine* e, int v, const WnParams& p, cudaStream_t st)
+{
+    nvwn_engine::Model& m = e->models[v];
+    if (!m.score_image) CK(m.score_image.alloc(wn_score_image_bytes(e->R, e->S, e->A, e->L)));
+    if (m.score_repack) {
+        WnParams q = p;
+        point_weights(e, q, m.blob);
+        CK(wn_score_pack(m.score_image, q, st));
+        m.score_repack = false;
+    }
+    return 0;
+}
+
+// Scoring by model: the segments of a call of Bs rows, each model it runs with its image packed, also copied to score_segs (device)
+int score_segments(nvwn_engine* e, const WnParams& p, int Bs, WnScoreSegs& segs, cudaStream_t st)
+{
+    std::vector<int> n_of(NVWN_MAX_MODELS, 0), all_of(NVWN_MAX_MODELS, 0);
+    for (int b = 0; b < e->B; b++) {
+        all_of[score_model(e, b)]++;
+        if (b < Bs) n_of[score_model(e, b)]++;
+    }
+    for (int v = 0, first = 0; v < NVWN_MAX_MODELS; first += all_of[v++]) {
+        if (!n_of[v]) continue;
+        const int rc = put_score_image(e, v, p, st);
+        if (rc != 0) return rc;
+        const nvwn_engine::Model& m = e->models[v];
+        const int k = segs.count++;
+        segs.model[k] = v; segs.n[k] = n_of[v]; segs.first[k] = first;
+        segs.image[v] = m.score_image; segs.embPrev[v] = m.blob + e->o_embPrev; segs.embCur[v] = m.blob + e->o_embCur;
+    }
+    segs.order = e->score_tab;
+    segs.row_model = e->score_tab + e->B;
+    if (!e->score_segs) CK(e->score_segs.alloc(sizeof(WnScoreSegs)));
+    return copy_snapshot(e->score_segs, &segs, 1, st);
 }
 
 }  // namespace
@@ -676,7 +824,6 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     const size_t Bz = batch_size, Nz = num_samples;
     const size_t per = L * Bz * 2 * R;                                 // 64 MB of fp32 staging, or one sample of conditioning if larger
     e->stage_elems = per > ((size_t)16 << 20) ? per : ((size_t)16 << 20);
-    CK(e->blob.alloc(e->blob_bytes));
     CK(e->Lh.alloc(e->family->store_bytes(*e)));
     CK(e->sel.alloc(Nz * Bz * sizeof(float)));
     CK(e->forced.alloc(Nz * Bz * sizeof(int)));
@@ -696,14 +843,13 @@ int nvwn_create(nvwn_engine** out, int dtype, int R, int S, int A, int num_layer
     CK(e->slot_seeds.alloc(Bz * sizeof(unsigned long long)));
     CK(e->prime_rows.alloc(Bz * sizeof(int)));
     if (dtype == NVWN_FP16) CK(e->stage.alloc(e->stage_elems * sizeof(float)));
-    if (e->family->pack) CK(e->image.alloc(e->family->image_bytes(*e)));
     e->models.resize(NVWN_MAX_MODELS);
     e->group_rows = e->family->group_rows(*e);
     CK(e->model_tab.alloc(NVWN_MAX_MODELS * sizeof(WnModel)));
     CK(e->group_tab.alloc((Bz + e->group_rows - 1) / e->group_rows * sizeof(int)));
-    const WnModel model0{e->blob, e->image};
-    CK(cudaMemcpy(e->model_tab, &model0, sizeof model0, cudaMemcpyHostToDevice));
-    cudaMemsetAsync(e->blob, 0, e->blob_bytes, 0);
+    const int rc = add_model(e.get(), 0);
+    if (rc != 0) return rc;
+    cudaMemsetAsync(e->models[0].blob, 0, e->blob_bytes, 0);
     cudaMemsetAsync(e->yOut, 0, Nz * Bz * sizeof(int), 0);
     cudaMemsetAsync(e->ring, 0, ring_bytes, 0);
     cudaMemsetAsync(e->origin, 0, Bz * sizeof(long long), 0);
@@ -733,8 +879,8 @@ int nvwn_set_embeddings(nvwn_engine* e, const float* embedPrev, const float* emb
 {
     if (!e || !embedPrev || !embedCur) return fail(NVWN_EINVAL, "nvwn_set_embeddings: NULL argument");
     int rc;
-    if ((rc = upload(e, e->blob + e->o_embPrev, embedPrev, (size_t)e->A * e->R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_embCur, embedCur, (size_t)e->A * e->R))) return rc;
+    if ((rc = upload(e, e->o_embPrev, embedPrev, (size_t)e->A * e->R))) return rc;
+    if ((rc = upload(e, e->o_embCur, embedCur, (size_t)e->A * e->R))) return rc;
     weights_changed(e);
     CK(cudaStreamSynchronize(0));
     return 0;
@@ -747,13 +893,13 @@ int nvwn_set_layer_weights(nvwn_engine* e, int layer, const float* Wprev, const 
     if (layer < 0 || layer >= e->L) return fail(NVWN_EINVAL, "nvwn_set_layer_weights: layer out of range");
     const size_t R = e->R, S = e->S, l = layer, td = e->td;
     int rc;
-    if ((rc = upload(e, e->blob + e->o_Wprev + l * 2 * R * R * td, Wprev, 2 * R * R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Wcur + l * 2 * R * R * td, Wcur, 2 * R * R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Bh + l * 2 * R * td, Bh, 2 * R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Wres + l * R * R * td, Wres, R * R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Bres + l * R * td, Bres, R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Wskip + l * S * R * td, Wskip, S * R))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Bskip + l * S * td, Bskip, S))) return rc;
+    if ((rc = upload(e, e->o_Wprev + l * 2 * R * R * td, Wprev, 2 * R * R))) return rc;
+    if ((rc = upload(e, e->o_Wcur + l * 2 * R * R * td, Wcur, 2 * R * R))) return rc;
+    if ((rc = upload(e, e->o_Bh + l * 2 * R * td, Bh, 2 * R))) return rc;
+    if ((rc = upload(e, e->o_Wres + l * R * R * td, Wres, R * R))) return rc;
+    if ((rc = upload(e, e->o_Bres + l * R * td, Bres, R))) return rc;
+    if ((rc = upload(e, e->o_Wskip + l * S * R * td, Wskip, S * R))) return rc;
+    if ((rc = upload(e, e->o_Bskip + l * S * td, Bskip, S))) return rc;
     weights_changed(e);
     CK(cudaStreamSynchronize(0));       // sources may be freed by the caller right after return
     return 0;
@@ -764,10 +910,10 @@ int nvwn_set_out_weights(nvwn_engine* e, const float* Wzs, const float* Bzs, con
     if (!e || !Wzs || !Bzs || !Wza || !Bza) return fail(NVWN_EINVAL, "nvwn_set_out_weights: NULL argument");
     const size_t A = e->A, S = e->S;
     int rc;
-    if ((rc = upload(e, e->blob + e->o_Wzs, Wzs, A * S))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Bzs, Bzs, A))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Wza, Wza, A * A))) return rc;
-    if ((rc = upload(e, e->blob + e->o_Bza, Bza, A))) return rc;
+    if ((rc = upload(e, e->o_Wzs, Wzs, A * S))) return rc;
+    if ((rc = upload(e, e->o_Bzs, Bzs, A))) return rc;
+    if ((rc = upload(e, e->o_Wza, Wza, A * A))) return rc;
+    if ((rc = upload(e, e->o_Bza, Bza, A))) return rc;
     weights_changed(e);
     CK(cudaStreamSynchronize(0));
     return 0;
@@ -788,29 +934,27 @@ int nvwn_cond_producer_load(nvwn_engine* e, const float* features, int n_cond_ch
                             const float* upsample_weight, const float* upsample_bias, int window, int stride,
                             const float* cond_weight, const float* cond_bias, void* stream)
 {
-    if (!e || !features || !upsample_weight || !upsample_bias || !cond_weight || !cond_bias) return fail(NVWN_EINVAL, "nvwn_cond_producer_load: NULL argument");
+    const std::string who = "nvwn_cond_producer_load";
+    if (!e || !features || !upsample_weight || !upsample_bias || !cond_weight || !cond_bias) return fail(NVWN_EINVAL, who + ": NULL argument");
     const int C = n_cond_channels, T = num_frames, K = window;
-    if (C < 1 || T < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, "nvwn_cond_producer_load: bad sizes (need window >= stride >= 1)");
+    int rc = check_cond_sizes(who, C, K, stride);
+    if (rc != 0) return rc;
+    if (T < 1) return fail(NVWN_EINVAL, who + ": num_frames = " + std::to_string(T) + "; need >= 1");
     cudaStream_t st = (cudaStream_t)stream;
     CondProducer& P = e->cond_whole;
     P.T.assign(e->B, 0);                                                      // loaded once every copy has been made
     P.ring = 0;                                                               // ends a live sequence
-    int rc = put_cond_network(e, P, "nvwn_cond_producer_load", C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
-    if (rc != 0) return rc;
+    if ((rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st))) return rc;
     // features [B][C][T] are the frame arena with cap = T, in one copy; row b's utterance starts at sample 0
     const size_t n_feat = (size_t)e->B * C * T;
-    if (n_feat > P.frames_floats) {
-        if (P.frames) CK(cudaDeviceSynchronize());                          // no launch reads the old frames any more
-        CK(P.frames.alloc(n_feat * sizeof(float)));
-        P.frames_floats = n_feat;
-    }
+    CK(P.frames.reserve(n_feat * sizeof(float)));
     P.cap = T;
     std::vector<WnCondSlot> tab(e->B);
-    for (int b = 0; b < e->B; b++) tab[b] = {(long long)b * C * T, 0, T, 0};
+    for (int b = 0; b < e->B; b++) tab[b] = cond_row(P, b, T);
     cudaError_t ce = cudaMemcpyAsync(P.frames, features, n_feat * sizeof(float), cudaMemcpyDefault, st);
     if (ce == cudaSuccess) ce = cudaMemcpyAsync(P.tables + cond_table_offset(e), tab.data(), tab.size() * sizeof(WnCondSlot), cudaMemcpyHostToDevice, st);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);                   // host sources may be released by the caller now
-    if (ce != cudaSuccess) return fail((int)ce, std::string("nvwn_cond_producer_load: ") + cudaGetErrorString(ce));
+    if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
     P.T.assign(e->B, T);
     return 0;
 }
@@ -843,17 +987,11 @@ int nvwn_cond_producer_run_stream(nvwn_engine* e, long long sample_begin, int sa
     if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (P.ring && sample_count > 0) {
-        // the ring holds frames [T - ring, T): the first frame the range reads must still be there
-        const long long need = first_frame(sample_begin, P.K, P.stride);
-        if (need < (long long)P.T[0] - P.ring)
-            return fail(NVWN_EINVAL, who + ": frame " + std::to_string(need) + ", which sample " + std::to_string(sample_begin) +
-                                         " reads, has left the ring (it holds frames " + std::to_string(P.T[0] - P.ring) + " .. " +
-                                         std::to_string(P.T[0] - 1) + ")");
-        // the table with the frame count of now, staged from pageable memory in stream order
-        std::vector<WnCondSlot> tab(e->B);
-        for (int b = 0; b < e->B; b++) tab[b] = {(long long)b * P.C * P.ring, 0, P.T[0], P.ring};
-        CK(cudaMemcpyAsync(P.tables + cond_table_offset(e), tab.data(), tab.size() * sizeof(WnCondSlot), cudaMemcpyHostToDevice, st));
-        if (sample_begin + sample_count > P.produced) P.produced = sample_begin + sample_count;
+        // the first frame the range reads must still be in the ring; every row holds the same frames
+        rc = check_held(P, who, 0, sample_begin, "");
+        if (rc != 0) return rc;
+        if ((rc = put_cond_table(e, P, nullptr, e->B, st))) return rc;
+        mark_produced(P, nullptr, e->B, sample_begin + sample_count);
     }
     for (const WrapPiece& w : split_at_wrap(sample_begin, sample_count, e->N)) {
         rc = produce(e, P, "nvwn_cond_producer", nullptr, e->B, sample_begin + w.off, w.pos, w.len, st);
@@ -867,28 +1005,19 @@ int nvwn_cond_producer_open_live(nvwn_engine* e, int n_cond_channels, const floa
 {
     const std::string who = "nvwn_cond_producer_open_live";
     if (!e || !upsample_weight || !upsample_bias || !cond_weight || !cond_bias) return fail(NVWN_EINVAL, who + ": NULL argument");
-    const int C = n_cond_channels, K = window;
-    if (C < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, who + ": bad sizes (need n_cond_channels >= 1 and window >= stride >= 1)");
-    const int least = (K + stride - 1) / stride + 1;
-    if (ring_frames < least)
-        return fail(NVWN_EINVAL, who + ": ring_frames = " + std::to_string(ring_frames) + "; need at least ceil(window / stride) + 1 = " +
-                                     std::to_string(least));
+    int rc = check_cond_sizes(who, n_cond_channels, window, stride);
+    if (rc == 0) rc = check_ring_frames(who, ring_frames, window, stride);
+    if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CondProducer& P = e->cond_whole;
     P.T.assign(e->B, 0);                                                      // replaces a loaded sequence
     P.ring = 0;
-    int rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
-    if (rc != 0) return rc;
-    const size_t n_ring = (size_t)e->B * C * ring_frames;
-    if (n_ring > P.frames_floats) {
-        if (P.frames) CK(cudaDeviceSynchronize());                          // no launch reads the old frames any more
-        CK(P.frames.alloc(n_ring * sizeof(float)));
-        P.frames_floats = n_ring;
-    }
+    if ((rc = put_cond_network(e, P, who, n_cond_channels, window, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st))) return rc;
+    CK(P.frames.reserve((size_t)e->B * n_cond_channels * ring_frames * sizeof(float)));
     const cudaError_t ce = cudaStreamSynchronize(st);                        // host sources may be released by the caller now
     if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
-    P.ring = ring_frames;
-    P.produced = 0;
+    P.cap = P.ring = ring_frames;
+    P.done.assign(e->B, 0);
     return 0;
 }
 
@@ -905,25 +1034,9 @@ int nvwn_cond_producer_push(nvwn_engine* e, const float* features, int num_frame
     if (T1 * P.stride > INT_MAX)
         return fail(NVWN_EINVAL, who + ": a live sequence holds at most INT_MAX samples; " + std::to_string(T1) + " frames would give " +
                                      std::to_string(T1 * P.stride));
-    // frames [T, T1) go where frames [T - ring, T1 - ring) were; the samples from `produced` on read frames from first_frame(produced)
-    const long long keep = first_frame(P.produced, P.K, P.stride);
-    if (T1 - P.ring > keep)
-        return fail(NVWN_EINVAL, who + ": " + std::to_string(num_frames) + " frames would overwrite frame " + std::to_string(keep) +
-                                     ", which sample " + std::to_string(P.produced) + " (not produced yet) reads; at most " +
-                                     std::to_string(keep + P.ring - T) + " frames fit before production moves on");
-    cudaStream_t st = (cudaStream_t)stream;
-    // [B][C][num_frames] -> columns T mod ring ... of the B * C ring rows, split at the wrap.  A host source is snapshotted into
-    // pageable memory, which the copies stage before they return: the caller's array (pinned or not) is free again on return.
-    std::vector<float> snap;
-    const float* src = features;
-    if (!is_device_ptr(features)) {
-        snap.assign(features, features + (size_t)e->B * P.C * num_frames);
-        src = snap.data();
-    }
-    const size_t f = sizeof(float);
-    for (const WrapPiece& w : split_at_wrap(T, num_frames, P.ring))
-        CK(cudaMemcpy2DAsync(P.frames + w.pos, (size_t)P.ring * f, src + w.off, (size_t)num_frames * f, (size_t)w.len * f, (size_t)e->B * P.C,
-                             cudaMemcpyDefault, st));
+    int rc = check_push(P, who, 0, num_frames, "");                          // every row holds the same frames
+    if (rc == 0) rc = put_live_frames(P, 0, e->B, T, features, num_frames, (cudaStream_t)stream);
+    if (rc != 0) return rc;
     P.T.assign(e->B, (int)T1);
     return 0;
 }
@@ -948,19 +1061,20 @@ int nvwn_cond_producer_set_weights(nvwn_engine* e, int n_cond_channels, const fl
 {
     const std::string who = "nvwn_cond_producer_set_weights";
     if (!e || !upsample_weight || !upsample_bias || !cond_weight || !cond_bias) return fail(NVWN_EINVAL, who + ": NULL argument");
-    const int C = n_cond_channels, K = window;
-    if (C < 1 || stride < 1 || K < stride) return fail(NVWN_EINVAL, who + ": bad sizes (need n_cond_channels >= 1 and window >= stride >= 1)");
+    const int C = n_cond_channels;
+    int rc = check_cond_sizes(who, C, window, stride);
+    if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CondProducer& P = e->cond_slots;
     if (P.frames && C != P.C) {                                               // the arena is laid out for the old channel count
         CK(cudaDeviceSynchronize());
-        P.frames.reset(); P.frames_floats = 0; P.cap = 0;
+        P.frames = DevBuf<float>();
+        P.cap = 0;
     }
     P.T.assign(e->B, 0);                                                      // frames attached under the old network are forgotten
     P.live.assign(e->B, 0);                                                   // and live mode ends
     P.ring = 0;
-    const int rc = put_cond_network(e, P, who, C, K, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st);
-    if (rc != 0) return rc;
+    if ((rc = put_cond_network(e, P, who, C, window, stride, upsample_weight, upsample_bias, cond_weight, cond_bias, st))) return rc;
     const cudaError_t ce = cudaStreamSynchronize(st);                        // host sources may be released by the caller now
     if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
     return 0;
@@ -1002,7 +1116,6 @@ int nvwn_cond_producer_set_slots(nvwn_engine* e, const int* slots, int n, const 
             if (ce != cudaSuccess) return fail((int)ce, who + ": " + cudaGetErrorString(ce));
         }
         P.frames = std::move(grown);
-        P.frames_floats = (size_t)e->B * cap * C;
         P.cap = cap;
     }
     for (int i = 0; i < n; i++) {
@@ -1028,7 +1141,6 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
     int rc = check_slots(e, who, slots, n);
     if (rc == 0) rc = check_window(e, who, first_sample, num_samples, "num_samples", 0);
     if (rc != 0) return rc;
-    std::vector<WnCondSlot> tab(n);
     for (int i = 0; i < n; i++) {
         const int s = slots[i];
         if (P.ring ? !P.live[s] : P.T[s] < 1)
@@ -1039,31 +1151,17 @@ int nvwn_cond_producer_run_slots(nvwn_engine* e, const int* slots, int n, long l
         if (first_sample < P.start[s])
             return fail(NVWN_EINVAL, who + ": first_sample " + std::to_string(first_sample) + " is before the start " + std::to_string(P.start[s]) +
                                          " of slot " + std::to_string(s) + "'s utterance");
+        // the range's first sample reads the earliest frames of the range
         const long long n0 = first_sample - P.start[s];
-        if (P.ring && num_samples > 0 && n0 < (long long)P.T[s] * P.stride) {
-            // the range's first sample reads the earliest frames of the range: they must still be in the ring
-            const long long need = first_frame(n0, P.K, P.stride), held = live_held(P, s);
-            if (need < held)
-                return fail(NVWN_EINVAL, who + ": frame " + std::to_string(need) + ", which sample " + std::to_string(n0) + " of slot " + std::to_string(s) +
-                                             "'s utterance reads, has left the ring (it holds frames " + std::to_string(held) + " .. " +
-                                             std::to_string(P.T[s] - 1) + ")");
-        }
-        tab[i] = {(long long)s * P.cap * P.C, P.start[s], P.T[s], P.ring};
+        if (P.ring && num_samples > 0 && n0 < (long long)P.T[s] * P.stride &&
+            (rc = check_held(P, who, s, n0, " of slot " + std::to_string(s) + "'s utterance")))
+            return rc;
     }
     e->slot_rows_used = true;
-    if (P.ring && num_samples > 0)
-        for (int i = 0; i < n; i++) {
-            const long long end = first_sample + num_samples - P.start[slots[i]];
-            if (end > P.done[slots[i]]) P.done[slots[i]] = end;
-        }
+    if (P.ring && num_samples > 0) mark_produced(P, slots, n, first_sample + num_samples);
     if (num_samples == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    // the slot list and the table in one copy, staged from pageable memory: the caller's arrays are free again on return
-    const size_t tab_off = cond_table_offset(e);
-    std::vector<char> host(tab_off + (size_t)n * sizeof(WnCondSlot));
-    memcpy(host.data(), slots, (size_t)n * sizeof(int));
-    memcpy(host.data() + tab_off, tab.data(), (size_t)n * sizeof(WnCondSlot));
-    CK(cudaMemcpyAsync(P.tables, host.data(), host.size(), cudaMemcpyHostToDevice, st));
+    if ((rc = put_cond_table(e, P, slots, n, st))) return rc;
     for (const WrapPiece& w : split_at_wrap(first_sample, num_samples, e->N))
         if ((rc = produce(e, P, who, slots, n, first_sample + w.off, w.pos, w.len, st))) return rc;
     return 0;
@@ -1076,16 +1174,9 @@ int nvwn_cond_producer_open_live_slots(nvwn_engine* e, int ring_frames, void* st
     if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
     CondProducer& P = e->cond_slots;
     if (!P.scratch) return fail(NVWN_EINVAL, who + ": nvwn_cond_producer_set_weights has not been called");
-    const int least = (P.K + P.stride - 1) / P.stride + 1;
-    if (ring_frames < least)
-        return fail(NVWN_EINVAL, who + ": ring_frames = " + std::to_string(ring_frames) + "; need at least ceil(window / stride) + 1 = " +
-                                     std::to_string(least));
-    const size_t n_ring = (size_t)e->B * P.C * ring_frames;
-    if (n_ring > P.frames_floats) {
-        if (P.frames) CK(cudaDeviceSynchronize());                          // no launch reads the old frames any more
-        CK(P.frames.alloc(n_ring * sizeof(float)));
-        P.frames_floats = n_ring;
-    }
+    const int rc = check_ring_frames(who, ring_frames, P.K, P.stride);
+    if (rc != 0) return rc;
+    CK(P.frames.reserve((size_t)e->B * P.C * ring_frames * sizeof(float)));
     P.cap = P.ring = ring_frames;
     P.T.assign(e->B, 0);
     P.live.assign(e->B, 0);
@@ -1113,7 +1204,7 @@ int nvwn_cond_producer_attach_live(nvwn_engine* e, const int* slots, int n, cons
     }
     cudaStream_t st = (cudaStream_t)stream;
     for (int i = 0; i < n; i++)
-        if (num_frames[i] > 0 && (rc = put_live_frames(P, slots[i], first_frames[i], features[i], num_frames[i], st))) return rc;
+        if (num_frames[i] > 0 && (rc = put_live_frames(P, slots[i], 1, first_frames[i], features[i], num_frames[i], st))) return rc;
     for (int i = 0; i < n; i++) {
         const int s = slots[i];
         P.live[s] = 1;
@@ -1143,18 +1234,13 @@ int nvwn_cond_producer_push_slots(nvwn_engine* e, const int* slots, int n, const
         if (num_frames[i] > 0 && !features[i]) return fail(NVWN_EINVAL, who + ": the frames of " + u + " are NULL");
         const long long T1 = (long long)P.T[s] + num_frames[i];
         if (T1 * P.stride > INT_MAX) return fail(NVWN_EINVAL, who + ": " + u + "'s utterance would hold more than INT_MAX samples");
-        // frames [T, T1) go where frames [T - ring, T1 - ring) were; the samples from `done` on read frames from first_frame(done),
-        // and the frames before `first` are gone already
-        const long long ff = first_frame(P.done[s], P.K, P.stride), keep = ff > P.first[s] ? ff : P.first[s];
-        if (T1 - P.ring > keep)
-            return fail(NVWN_EINVAL, who + ": " + std::to_string(num_frames[i]) + " frames would overwrite frame " + std::to_string(keep) + " of " + u +
-                                         ", which sample " + std::to_string(P.done[s]) + " (not produced yet) reads; at most " +
-                                         std::to_string(keep + P.ring - P.T[s]) + " frames fit before production moves on");
+        rc = check_push(P, who, s, num_frames[i], " of " + u);
+        if (rc != 0) return rc;
     }
     cudaStream_t st = (cudaStream_t)stream;
     for (int i = 0; i < n; i++) {
         if (num_frames[i] == 0) continue;
-        if ((rc = put_live_frames(P, slots[i], P.T[slots[i]], features[i], num_frames[i], st))) return rc;
+        if ((rc = put_live_frames(P, slots[i], 1, P.T[slots[i]], features[i], num_frames[i], st))) return rc;
         P.T[slots[i]] += num_frames[i];
     }
     return 0;
@@ -1297,7 +1383,7 @@ int nvwn_set_forced(nvwn_engine* e, const int* forced)
 int nvwn_weight_blob(nvwn_engine* e, void** dev_ptr, unsigned long long* bytes)
 {
     if (!e || !dev_ptr || !bytes) return fail(NVWN_EINVAL, "nvwn_weight_blob: NULL argument");
-    *dev_ptr = e->blob;
+    *dev_ptr = e->models[0].blob;
     *bytes = e->blob_bytes;
     return 0;
 }
@@ -1319,18 +1405,11 @@ int nvwn_set_model(nvwn_engine* e, int model, const nvwn_engine* src)
     if (src->dtype != e->dtype || src->R != e->R || src->S != e->S || src->A != e->A || src->L != e->L || src->maxDil != e->maxDil ||
         src->tanhEmbed != e->tanhEmbed || src->device != e->device)
         return fail(NVWN_EINVAL, who + ": the source engine differs in dtype, R, S, A, L, max_dilation, tanh_embed or device");
-    nvwn_engine::Model& m = e->models[model];
-    if (!m.blob) {
-        // first set: the buffers, and the model's entry of the base table, which no launch reads before a group names the model
-        nvwn_engine::Model fresh;
-        CK(fresh.blob.alloc(e->blob_bytes));
-        if (e->family->pack) CK(fresh.image.alloc(e->family->image_bytes(*e)));
-        const WnModel bases{fresh.blob, fresh.image};
-        CK(cudaMemcpy(e->model_tab + model, &bases, sizeof bases, cudaMemcpyHostToDevice));
-        m = std::move(fresh);
-    }
-    CK(cudaMemcpyAsync(m.blob, src->blob, e->blob_bytes, cudaMemcpyDeviceToDevice, 0));
-    m.dirty = m.score_dirty = true;
+    // first set: the buffers, and the model's entry of the base table, which no launch reads before a group names the model
+    int rc;
+    if (!e->models[model].blob && (rc = add_model(e, model))) return rc;
+    CK(cudaMemcpyAsync(e->models[model].blob, src->models[0].blob, e->blob_bytes, cudaMemcpyDeviceToDevice, 0));
+    model_changed(e, model);
     if (e->score_next >= 0)                  // an open scoring stream whose rows run the model ends, as at a weight change
         for (int b = 0; b < e->score_bs; b++)
             if (score_model(e, b) == model) { e->score_next = -1; break; }
@@ -1353,10 +1432,8 @@ int nvwn_set_group_models(nvwn_engine* e, const int* models, int n_groups, void*
     if (n_groups != groups)
         return fail(NVWN_EINVAL, who + ": need n_groups = ceil(B / G) = " + std::to_string(groups) + " (G = " + std::to_string(e->group_rows) + "); got " +
                                        std::to_string(n_groups));
-    for (int g = 0; g < n_groups; g++)
-        if (models[g] != 0 && (models[g] < 0 || models[g] >= NVWN_MAX_MODELS || !e->models[models[g]].blob))
-            return fail(NVWN_EINVAL, who + ": group " + std::to_string(g) + " names model " + std::to_string(models[g]) + ", which was never set");
-    const int rc = copy_snapshot(e->group_tab, models, n_groups, (cudaStream_t)stream);
+    int rc = check_models(e, who, "group", models, n_groups);
+    if (rc == 0) rc = copy_snapshot(e->group_tab, models, n_groups, (cudaStream_t)stream);
     if (rc != 0) return rc;
     e->group_host.assign(models, models + n_groups);
     return 0;
@@ -1368,9 +1445,8 @@ int nvwn_set_score_models(nvwn_engine* e, const int* models, int n_rows, void* s
     if (!e || !models) return fail(NVWN_EINVAL, who + ": NULL argument");
     if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score");
     if (n_rows != e->B) return fail(NVWN_EINVAL, who + ": need n_rows = B = " + std::to_string(e->B) + "; got " + std::to_string(n_rows));
-    for (int b = 0; b < n_rows; b++)
-        if (models[b] != 0 && (models[b] < 0 || models[b] >= NVWN_MAX_MODELS || !e->models[models[b]].blob))
-            return fail(NVWN_EINVAL, who + ": row " + std::to_string(b) + " names model " + std::to_string(models[b]) + ", which was never set");
+    int rc = check_models(e, who, "row", models, n_rows);
+    if (rc != 0) return rc;
     // the rows by model, then by row, and the table: a call of Bs rows takes of each model's rows the prefix below Bs
     std::vector<int> tab(2 * (size_t)n_rows);
     size_t k = 0;
@@ -1379,7 +1455,7 @@ int nvwn_set_score_models(nvwn_engine* e, const int* models, int n_rows, void* s
             if (models[b] == v) tab[k++] = b;
     std::copy(models, models + n_rows, tab.begin() + n_rows);
     if (!e->score_tab) CK(e->score_tab.alloc(tab.size() * sizeof(int)));
-    const int rc = copy_snapshot(e->score_tab, tab.data(), tab.size(), (cudaStream_t)stream);
+    rc = copy_snapshot(e->score_tab, tab.data(), tab.size(), (cudaStream_t)stream);
     if (rc != 0) return rc;
     e->score_models.assign(models, models + n_rows);
     e->score_next = -1;                      // the open stream's fronts were computed with the old models
@@ -1559,13 +1635,8 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, const unsigne
         int T = SCORE_ROWS / e->B;
         if (T < 1) T = 1;
         if (T > e->N) T = e->N;
-        const ScoreScratch o = score_scratch_layout(e, T);
-        DevBuf<char> scratch;                // kept only with the image: a scratch means both are there
-        CK(scratch.alloc(o.bytes));
-        CK(e->score_image.alloc(wn_score_image_bytes(R, e->S, A, L)));
-        e->score_scratch = std::move(scratch);
+        CK(e->score_scratch.alloc(score_scratch_layout(e, T).bytes));
         e->score_T = T;
-        e->score_dirty = true;
     }
     const int T = e->score_T;
     const ScoreScratch o = score_scratch_layout(e, T);
@@ -1592,46 +1663,13 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, const unsigne
     e->score_next = -1;                      // reopened below once this call's state is complete
     WnParams p;
     fill_params(e, p, 0, 0, 0, N, Bs, 0);
-    if (e->score_dirty) {
-        CK(wn_score_pack(e->score_image, p, st));
-        e->score_dirty = false;
-    }
-    // scoring by model, when a row of the call runs another model than 0: its segments, each model's image packed if it changed
+    // model 0's image, which a call reads unless a row runs another model; then, if one does, the call's segments
     WnScoreSegs segs{};
     bool by_model = false;
     for (int b = 0; b < Bs && !by_model; b++) by_model = score_model(e, b) != 0;
-    if (by_model) {
-        std::vector<int> n_of(NVWN_MAX_MODELS, 0), all_of(NVWN_MAX_MODELS, 0);
-        for (int b = 0; b < e->B; b++) {
-            all_of[score_model(e, b)]++;
-            if (b < Bs) n_of[score_model(e, b)]++;
-        }
-        for (int v = 0, first = 0; v < NVWN_MAX_MODELS; first += all_of[v++]) {
-            if (!n_of[v]) continue;
-            const char* blob = e->blob;
-            const void* image = e->score_image;
-            if (v) {
-                nvwn_engine::Model& m = e->models[v];
-                if (!m.score_image) CK(m.score_image.alloc(wn_score_image_bytes(R, e->S, A, L)));
-                if (m.score_dirty) {
-                    WnParams q = p;
-                    point_weights(e, q, m.blob);
-                    CK(wn_score_pack(m.score_image, q, st));
-                    m.score_dirty = false;
-                }
-                blob = m.blob;
-                image = m.score_image;
-            }
-            const int k = segs.count++;
-            segs.model[k] = v; segs.n[k] = n_of[v]; segs.first[k] = first;
-            segs.image[v] = image; segs.embPrev[v] = blob + e->o_embPrev; segs.embCur[v] = blob + e->o_embCur;
-        }
-        segs.order = e->score_tab;
-        segs.row_model = e->score_tab + e->B;
-        if (!e->score_segs) CK(e->score_segs.alloc(sizeof(WnScoreSegs)));
-        const int rc = copy_snapshot(e->score_segs, &segs, 1, st);
-        if (rc != 0) return rc;
-    }
+    int rc = put_score_image(e, 0, p, st);
+    if (rc == 0 && by_model) rc = score_segments(e, p, Bs, segs, st);
+    if (rc != 0) return rc;
     const bool logp_dev = is_device_ptr(logp), logits_dev = logits && is_device_ptr(logits);
     if (first == 0) {
         for (int l = 0; l < L; l++)          // x_l[t - d] = 0 for t < d
@@ -1643,7 +1681,7 @@ int score_range(nvwn_engine* e, const char* who, const int* audio, const unsigne
     WnScoreChunk c;
     c.L = L; c.R = R; c.S = e->S; c.A = A; c.maxDil = e->maxDil; c.tanhEmbed = e->tanhEmbed;
     c.Bs = Bs; c.Be = e->B; c.N = N; c.Tcap = T;
-    c.image = e->score_image; c.embPrev = e->blob + e->o_embPrev; c.embCur = e->blob + e->o_embCur;
+    c.image = e->models[0].score_image; c.embPrev = e->models[0].blob + e->o_embPrev; c.embCur = e->models[0].blob + e->o_embCur;
     c.audio = d_audio;
     c.codes = d_codes;
     float* lh = reinterpret_cast<float*>(sc + o.lh);
@@ -1732,7 +1770,7 @@ int nvwn_score_stream_packed(nvwn_engine* e, const int* audio, const unsigned ch
 int nvwn_prime_from_score(nvwn_engine* e, void* stream)
 {
     const std::string who = "nvwn_prime_from_score";
-    int rc = check_prime(e, who);
+    int rc = check_open_stream(e, who, "history to generate from");
     if (rc == 0) rc = check_run_batch(e, who, e->score_bs);
     if (rc == 0) rc = check_prime_model(e, who, nullptr, nullptr, e->score_bs);
     if (rc != 0) return rc;
@@ -1751,32 +1789,18 @@ int nvwn_prime_from_score(nvwn_engine* e, void* stream)
 int nvwn_prime_slots_from_score(nvwn_engine* e, const int* rows, const int* slots, int n, const unsigned long long* seeds, void* stream)
 {
     const std::string who = "nvwn_prime_slots_from_score";
-    int rc = check_prime(e, who);
+    int rc = check_open_stream(e, who, "history to generate from");
     if (rc != 0) return rc;
     if (!rows) return fail(NVWN_EINVAL, who + ": rows is NULL");
-    if ((rc = check_slots(e, who, slots, n))) return rc;
-    const int Bs = e->score_bs;
-    std::vector<char> seen(Bs, 0);
-    for (int i = 0; i < n; i++) {
-        if (rows[i] < 0 || rows[i] >= Bs)
-            return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is outside [0, " + std::to_string(Bs) + ") (the scoring stream's batch_size)");
-        if (seen[rows[i]]) return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is given twice");
-        seen[rows[i]] = 1;
-    }
-    if ((rc = check_prime_model(e, who, rows, slots, n))) return rc;
+    if ((rc = check_slots(e, who, slots, n)) || (rc = check_rows(e, who, rows, n)) || (rc = check_prime_model(e, who, rows, slots, n))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned long long* seeds_dev;
-    if ((rc = take_slots(e, who, slots, n, seeds, &seeds_dev, st)) || (rc = copy_snapshot(e->prime_rows, rows, n, st))) return rc;
-    const long long P = e->score_next, t0 = e->next_t, origin = t0 - P;
-    const int M = e->maxDil + 1;
-    if (t0 < e->maxDil && !e->early_prime) {
-        // from now on every launch reads the ring at every step: the entries of the negative times, which no row has written since
-        // the reset, must read as the zeros the kernels stage for "before the start"
-        CK(e->family->clear_times(*e, e->ring, t0 - M, (int)(M - t0), st));
-        e->early_prime = true;
-    }
-    // what nvwn_restart_slots at t0 - P does to these slots, then nvwn_prime_from_score of their rows with local time tau at engine
-    // time t0 - P + tau
+    if ((rc = take_slots(e, who, slots, n, seeds, &seeds_dev, st)) || (rc = copy_snapshot(e->prime_rows, rows, n, st)) || (rc = clear_early_times(e, st)))
+        return rc;
+    const int Bs = e->score_bs;
+    const long long P = e->score_next, origin = e->next_t - P;
+    // what nvwn_restart_slots at origin = next_t - P does to these slots, then nvwn_prime_from_score of their rows with local time tau
+    // at engine time origin + tau
     CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
     rc = put_fronts(e, [&](int l, const __half* src, long long tau, int n_t) {
         return e->family->put_history_rows(*e, e->ring, src, e->prime_rows, e->R, (size_t)Bs * e->R, e->slot_rows, n, l, origin + tau, n_t, st);
@@ -1798,64 +1822,41 @@ int nvwn_save_slots(nvwn_engine* e, const int* slots, int n, void* states, void*
 {
     const std::string who = "nvwn_save_slots";
     if (!e || !states) return fail(NVWN_EINVAL, who + ": NULL argument");
-    int rc = check_slots(e, who, slots, n);
+    const int rc = check_slots(e, who, slots, n);
     if (rc != 0) return rc;
-    const bool host = !is_device_ptr(states);
-    if (!host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
     const size_t bytes = wn_slot_state_bytes(*e);
-    if (host && (rc = state_stage(e, (size_t)n * bytes))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    char* dst = host ? e->state_stage.get() : static_cast<char*>(states);
-    // the slot list goes through the slot scratch, but this is no per-slot call: the engine does not change
-    if ((rc = copy_snapshot(e->slot_rows, slots, n, st))) return rc;
-    CK(wn_save_slot_scalars(dst, bytes, e->slot_rows, n, *e, e->next_t, e->yPrev, e->yCur, e->origin, e->seed, st));
-    rc = state_layers(e, [&](int l, size_t off, int d) {
-        return e->family->get_history_rows(*e, e->ring, dst + off, bytes / e->td, e->R, e->slot_rows, n, l, e->next_t - d, d, e->origin, st);
+    return write_states(e, who, states, n, st, [&](char* dst) {
+        // the slot list goes through the slot scratch, but this is no per-slot call: the engine does not change
+        const int rc = copy_snapshot(e->slot_rows, slots, n, st);
+        if (rc != 0) return rc;
+        CK(wn_save_slot_scalars(dst, bytes, e->slot_rows, n, *e, e->next_t, e->yPrev, e->yCur, e->origin, e->seed, st));
+        return state_layers(e, [&](int l, size_t off, int d) {
+            return e->family->get_history_rows(*e, e->ring, dst + off, bytes / e->td, e->R, e->slot_rows, n, l, e->next_t - d, d, e->origin, st);
+        });
     });
-    if (rc != 0) return rc;
-    if (host) {
-        CK(cudaMemcpyAsync(states, dst, (size_t)n * bytes, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    return 0;
 }
 
 int nvwn_score_save_states(nvwn_engine* e, const int* rows, int n, const unsigned long long* seeds, void* states, void* stream)
 {
     const std::string who = "nvwn_score_save_states";
-    if (!e) return fail(NVWN_EINVAL, who + ": NULL engine");
-    if (e->dtype != NVWN_FP16) return fail(NVWN_EUNSUPPORTED, who + ": only NVWN_FP16 engines can score");
-    if (e->score_next < 1) return fail(NVWN_EINVAL, who + ": no open scoring stream (nvwn_score and weight changes end one)");
-    if (e->score_packed)
-        return fail(NVWN_EUNSUPPORTED, who + ": the scoring stream is packed (nvwn_score_stream_packed): a row's layer fronts may hold an earlier "
-                                             "utterance's inputs, so they are no utterance's state");
+    int rc = check_open_stream(e, who, "utterance's state");
+    if (rc != 0) return rc;
     if (!rows || !states) return fail(NVWN_EINVAL, who + ": NULL argument");
     const int Bs = e->score_bs;
     if (n < 1 || n > Bs) return fail(NVWN_EINVAL, who + ": n " + std::to_string(n) + " is outside [1, " + std::to_string(Bs) + "] (the scoring stream's batch_size)");
-    std::vector<char> seen(Bs, 0);
-    for (int i = 0; i < n; i++) {
-        if (rows[i] < 0 || rows[i] >= Bs)
-            return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is outside [0, " + std::to_string(Bs) + ") (the scoring stream's batch_size)");
-        if (seen[rows[i]]) return fail(NVWN_EINVAL, who + ": row " + std::to_string(rows[i]) + " is given twice");
-        seen[rows[i]] = 1;
-    }
-    const bool host = !is_device_ptr(states);
-    if (!host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
+    if ((rc = check_rows(e, who, rows, n))) return rc;
     const size_t bytes = wn_slot_state_bytes(*e);
-    int rc;
-    if (host && (rc = state_stage(e, (size_t)n * bytes))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    char* dst = host ? e->state_stage.get() : static_cast<char*>(states);
-    // rows and seeds go through the per-call scratch of the primes; nothing else of the engine is touched
-    if ((rc = copy_snapshot(e->prime_rows, rows, n, st)) || (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st)))) return rc;
-    const ScoreScratch o = score_scratch_layout(e, e->score_T);
-    CK(wn_score_save_states(dst, bytes, reinterpret_cast<const __half*>(e->score_scratch + o.xh), reinterpret_cast<const int*>(e->score_scratch + o.codes),
-                            e->prime_rows, n, seeds ? e->slot_seeds.get() : nullptr, *e, e->score_next, e->score_T, e->B, Bs, st));
-    if (host) {
-        CK(cudaMemcpyAsync(states, dst, (size_t)n * bytes, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    return 0;
+    return write_states(e, who, states, n, st, [&](char* dst) {
+        // rows and seeds go through the per-call scratch of the primes; nothing else of the engine is touched
+        int rc;
+        if ((rc = copy_snapshot(e->prime_rows, rows, n, st)) || (seeds && (rc = copy_snapshot(e->slot_seeds, seeds, n, st)))) return rc;
+        const ScoreScratch o = score_scratch_layout(e, e->score_T);
+        CK(wn_score_save_states(dst, bytes, reinterpret_cast<const __half*>(e->score_scratch + o.xh), reinterpret_cast<const int*>(e->score_scratch + o.codes),
+                                e->prime_rows, n, seeds ? e->slot_seeds.get() : nullptr, *e, e->score_next, e->score_T, e->B, Bs, st));
+        return 0;
+    });
 }
 
 int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states, void* stream)
@@ -1865,8 +1866,8 @@ int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states,
     int rc = check_slots(e, who, slots, n);
     if (rc != 0) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const bool host = !is_device_ptr(states);
-    if (!host && reinterpret_cast<uintptr_t>(states) % 16) return fail(NVWN_EINVAL, who + ": device states must be 16-byte aligned");
+    bool host;
+    if ((rc = check_states(who, states, &host))) return rc;
     const size_t bytes = wn_slot_state_bytes(*e), hb = sizeof(nvwn_slot_state_header);
     // every header is checked before anything changes; device headers are read in stream order (the call runs at a window boundary)
     std::vector<nvwn_slot_state_header> h(n);
@@ -1890,17 +1891,12 @@ int nvwn_load_slots(nvwn_engine* e, const int* slots, int n, const void* states,
     }
     const char* src = static_cast<const char*>(states);
     if (host) {
-        if ((rc = state_stage(e, (size_t)n * bytes)) || (rc = copy_snapshot(e->state_stage, src, (size_t)n * bytes, st))) return rc;
+        CK(e->state_stage.reserve((size_t)n * bytes));
+        if ((rc = copy_snapshot(e->state_stage, src, (size_t)n * bytes, st))) return rc;
         src = e->state_stage;
     }
-    if ((rc = take_slots(e, who, slots, n, nullptr, nullptr, st))) return rc;
+    if ((rc = take_slots(e, who, slots, n, nullptr, nullptr, st)) || (rc = clear_early_times(e, st))) return rc;
     const long long t0 = e->next_t;
-    const int M = e->maxDil + 1;
-    if (t0 < e->maxDil && !e->early_prime) {
-        // as nvwn_prime_slots_from_score: the loaded rows hold real values at times the kernels would skip as "before the start"
-        CK(e->family->clear_times(*e, e->ring, t0 - M, (int)(M - t0), st));
-        e->early_prime = true;
-    }
     CK(e->family->clear_rows(*e, e->ring, e->slot_rows, n, st));
     rc = state_layers(e, [&](int l, size_t off, int d) {
         return e->family->put_history_rows(*e, e->ring, src + off, nullptr, bytes / e->td, e->R, e->slot_rows, n, l, t0 - d, d, st);

@@ -16,6 +16,15 @@ from ._lib import FP16, FP32, FP32_FAST, KERNEL_AUTO, KERNEL_STREAM, KERNEL_TENS
 AUTO, SINGLE_BLOCK, DUAL_BLOCK, PERSISTENT, MANYBLOCK_NONPERSISTENT = 0, 1, 2, 3, 4
 
 
+def _model_table(what, models):
+    """(void*, int32 array) of a model table, every index checked to fit a C int."""
+    m = np.asarray(models, dtype=np.int64).ravel()
+    if m.size and (m.min() < np.iinfo(np.int32).min or m.max() > np.iinfo(np.int32).max):
+        raise ValueError(f"{what}: model indices must fit a C int; got {m.min()} .. {m.max()}")
+    m = np.ascontiguousarray(m.astype(np.int32))
+    return C.c_void_p(m.ctypes.data), m
+
+
 def _ptr(a, dtype):
     """(void*, keepalive) of a numpy array or torch tensor holding `dtype`, C-contiguous."""
     if a is None:
@@ -150,6 +159,12 @@ class NVWavenetInfer:
         check(self._l.nvwn_set_conditioning(self._h, a, first_sample, num_samples, _stream(stream)), "setConditioning")
         return k
 
+    @staticmethod
+    def _network(upsample_weight, upsample_bias, cond_weight, cond_bias):
+        """((wu, bu, wc, bc) pointers, keepalive) of the four arrays of a conditioning network, as fp32."""
+        pairs = [_ptr(a, np.float32) for a in (upsample_weight, upsample_bias, cond_weight, cond_bias)]
+        return tuple(p for p, _ in pairs), [k for _, k in pairs]
+
     def _call_with_features(self, fn, name, features, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, *tail):
         """fn(engine, features, C, T, upsample_weight, upsample_bias, window, stride, cond_weight, cond_bias, *tail) of the
         whole-batch producer calls, with the arrays' shapes checked; returns T * stride."""
@@ -158,8 +173,8 @@ class NVWavenetInfer:
         if len(shape) != 3 or shape[:2] != (self.B, Cc):
             raise ValueError(f"{name}: features must be [{self.B}][{Cc}][T] for this engine and network; got {shape}")
         T = shape[2]
-        f, k1 = _ptr(features, np.float32); wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
-        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
+        f, k1 = _ptr(features, np.float32)
+        (wu, bu, wc, bc), keep = self._network(upsample_weight, upsample_bias, cond_weight, cond_bias)
         check(fn(self._h, f, Cc, T, wu, bu, window, stride, wc, bc, *tail), name)
         return T * stride
 
@@ -188,8 +203,7 @@ class NVWavenetInfer:
         and cond_producer_run_stream produces the samples they complete.  Replaces a loaded sequence; see nvwn_cond_producer_open_live."""
         Cc, window = check_cond_network(self.L, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, ValueError,
                                         "condProducerOpenLive")
-        wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
-        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
+        (wu, bu, wc, bc), keep = self._network(upsample_weight, upsample_bias, cond_weight, cond_bias)
         check(self._l.nvwn_cond_producer_open_live(self._h, Cc, wu, bu, window, stride, wc, bc, ring_frames, _stream(stream)),
               "condProducerOpenLive")
         self._cond_channels = Cc
@@ -255,6 +269,7 @@ class NVWavenetInfer:
 
     # ---- continuous batching: the B rows are slots, each restarted with a new utterance at a launch boundary ----
     def _slots(self, slots):
+        """(void*, int32 array) of a list of slot or scoring-row indices."""
         s = np.ascontiguousarray(np.asarray(slots, dtype=np.int64).reshape(-1)).astype(np.int32)
         return C.c_void_p(s.ctypes.data), s
 
@@ -300,8 +315,7 @@ class NVWavenetInfer:
         cond_weight [L*2R][C] or [L*2R][C][1], cond_bias [L*2R]), for cond_producer_run_slots.  Forgets every attached utterance."""
         Cc, window = check_cond_network(self.L, self.R, upsample_weight, upsample_bias, cond_weight, cond_bias, stride, ValueError,
                                         "cond_producer_set_weights")
-        wu, k2 = _ptr(upsample_weight, np.float32); bu, k3 = _ptr(upsample_bias, np.float32)
-        wc, k4 = _ptr(cond_weight, np.float32); bc, k5 = _ptr(cond_bias, np.float32)
+        (wu, bu, wc, bc), keep = self._network(upsample_weight, upsample_bias, cond_weight, cond_bias)
         check(self._l.nvwn_cond_producer_set_weights(self._h, Cc, wu, bu, window, stride, wc, bc, _stream(stream)), "condProducerSetWeights")
         self._cond_channels = Cc
 
@@ -432,20 +446,14 @@ class NVWavenetInfer:
     def set_group_models(self, models, stream=None):
         """The model of each of the ceil(B / model_group) groups: 0 or a model given to set_model.  Takes effect from the next
         launch on `stream`; see nvwn_set_group_models."""
-        m = np.asarray(models, dtype=np.int64).ravel()
-        if m.size and (m.min() < np.iinfo(np.int32).min or m.max() > np.iinfo(np.int32).max):
-            raise ValueError(f"setGroupModels: model indices must fit a C int; got {m.min()} .. {m.max()}")
-        m = np.ascontiguousarray(m.astype(np.int32))
-        check(self._l.nvwn_set_group_models(self._h, C.c_void_p(m.ctypes.data), m.size, _stream(stream)), "setGroupModels")
+        p, m = _model_table("setGroupModels", models)
+        check(self._l.nvwn_set_group_models(self._h, p, m.size, _stream(stream)), "setGroupModels")
 
     def set_score_models(self, models, stream=None):
         """The model of each of the B scoring rows: 0 or a model given to set_model.  Applies to the scoring calls from the next one;
         ends an open scoring stream; see nvwn_set_score_models."""
-        m = np.asarray(models, dtype=np.int64).ravel()
-        if m.size and (m.min() < np.iinfo(np.int32).min or m.max() > np.iinfo(np.int32).max):
-            raise ValueError(f"setScoreModels: model indices must fit a C int; got {m.min()} .. {m.max()}")
-        m = np.ascontiguousarray(m.astype(np.int32))
-        check(self._l.nvwn_set_score_models(self._h, C.c_void_p(m.ctypes.data), m.size, _stream(stream)), "setScoreModels")
+        p, m = _model_table("setScoreModels", models)
+        check(self._l.nvwn_set_score_models(self._h, p, m.size, _stream(stream)), "setScoreModels")
 
     def cond_producer_run_slots(self, slots, first_sample, num_samples, stream=None):
         """Conditioning of absolute samples [first_sample, first_sample + num_samples), num_samples <= N, for `slots` only, from
@@ -552,21 +560,21 @@ class NVWavenetInfer:
         continued by generation from the engine's next sample t0 (its sample P at t0).  seeds (one per slot, None = 0) key the slots'
         selectors as restart_slots does.  The scoring stream stays open.  Asynchronous on `stream`; see nvwn_prime_slots_from_score."""
         p, s = self._slots(slots)
-        r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1)).astype(np.int32)
+        pr, r = self._slots(rows)
         if r.size != s.size:
             raise ValueError(f"prime_slots_from_score: {s.size} slots but {r.size} rows")
         k, keep = self._seeds("prime_slots_from_score", seeds, s.size)
-        check(self._l.nvwn_prime_slots_from_score(self._h, C.c_void_p(r.ctypes.data), p, s.size, k, _stream(stream)), "primeSlotsFromScore")
+        check(self._l.nvwn_prime_slots_from_score(self._h, pr, p, s.size, k, _stream(stream)), "primeSlotsFromScore")
 
     def score_save_states(self, rows, seeds=None, out=None, stream=None):
         """After score_stream over prompts [0, P): the slot states of scoring rows `rows` at P, as a uint8 CUDA tensor
         [n][slot_state_bytes] written asynchronously on `stream`, or into `out` as for save_slots; seeds (one per row, None = 0) are
         the states' selector keys.  load_slots resumes them in any slot of a compatible engine.  The scoring stream stays open; see
         nvwn_score_save_states."""
-        r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1)).astype(np.int32)
+        pr, r = self._slots(rows)
         k, keep = self._seeds("score_save_states", seeds, r.size)
         out, ptr = self._states_out("score_save_states", r.size, out)
-        check(self._l.nvwn_score_save_states(self._h, C.c_void_p(r.ctypes.data), r.size, k, C.c_void_p(ptr), _stream(stream)),
+        check(self._l.nvwn_score_save_states(self._h, pr, r.size, k, C.c_void_p(ptr), _stream(stream)),
               "scoreSaveStates")
         return out
 

@@ -184,9 +184,16 @@ def test_refused_loads_change_nothing(monkeypatch):
         o.close()
     bad = good.copy()
     bad[0, :4] = 0                                                      # not a slot state
+    import torch
+    shifted = torch.zeros(good.size + 16, dtype=torch.uint8, device="cuda")
+    misaligned = shifted[1:1 + good.size].view(1, -1)                   # device states off their 16-byte alignment
+    misaligned.copy_(torch.from_numpy(good))
+    with pytest.raises(nw.NvwnError, match="device states must be 16-byte aligned"):
+        r.e.save_slots([0], out=misaligned)
     for states, slots, match in [(foreign[0], [1], "has dtype 1"), (foreign[1], [1], "R 32"), (foreign[2], [1], "L 13"),
                                  (foreign[3], [1], "max_dilation 16"), (bad, [1], "is not a slot state"), (good, [B], "outside"),
-                                 (np.concatenate([good, good]), [1, 1], "given twice")]:
+                                 (np.concatenate([good, good]), [1, 1], "given twice"),
+                                 (misaligned, [1], "device states must be 16-byte aligned")]:
         if states.shape[1] != good.shape[1]:
             states = np.resize(states, (len(slots), good.shape[1]))             # same size, so the header check decides
         with pytest.raises(nw.NvwnError, match=match):

@@ -118,6 +118,9 @@ def test_refusals_change_nothing(monkeypatch):
     _refused(-1, e.score_save_states, [BS])
     _refused(-1, e.score_save_states, [-1])
     _refused(-1, e.score_save_states, [1, 1])
+    import torch
+    shifted = torch.zeros(e.slot_state_bytes() + 16, dtype=torch.uint8, device="cuda")
+    _refused(-1, e.score_save_states, [0], None, shifted[1:1 + e.slot_state_bytes()].view(1, -1))     # device states off 16 bytes
     out = np.empty((1, e.slot_state_bytes()), np.uint8)
     lib = _lib.lib()
     row = np.zeros(1, np.int32)
